@@ -3,7 +3,7 @@
 calibration tokens (configs[1]; YAML = configs/gptq_w_only.yml, the schema of the reference's
 configs/quantization/methods/GPTQ/gptq_w_only.yml).
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl reference]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl reference] [--dump-outputs DIR]
 
 A STEP = GPTQ calibration of ONE decoder block (7 linears: RTN seed qparams, Hessians over the
 full calibration set, Cholesky, column sweep, fake-quant forward that feeds the next block).
@@ -25,6 +25,11 @@ does it per batch); total work fixed => "scaling": "strong".
 the GPU box) on the host cores: every step is the same workload — one decoder block through the
 reference's schedule at the real shapes — on a bounded sample (see REF_SAMPLE), and the reported
 value is extrapolated to the full calibration set with stated rules.
+
+--dump-outputs DIR: after the timed steps, what the last timed step handed its caller is written
+as DIR/<name>.npy (float32 / float64): a fixed, seeded sample of the block output and of every
+linear's calibrated weight and group scales / zeros, and every linear's per-row losses.  Inputs
+are seeded, so two builds run with the same arguments can be compared output for output.
 """
 import argparse
 import json
@@ -56,9 +61,9 @@ DATA = 'synthetic (random-init N(0,0.02^2) weights, uniform random token ids)'
 
 
 def bench_config(args, world):
-    """`config` of the JSON line — the SAME dict in both arms (the driver compares them)."""
+    """`config` of the JSON line — the SAME dict in both arms, so their results are comparable."""
     return {'workload': workload_name(args), 'yaml': 'configs/gptq_w_only.yml',
-            'l2': 'inputs (>=2 GiB activations per step) exceed the 126 MB L2',
+            'l2': 'inputs (>=2 GiB activations per step) exceed the 50 MB L2',
             'parallelism': (f'dp{world} over calibration samples, 1 NCCL all-reduce of H per distinct input'
                             if world > 1 else 'single GPU')}
 
@@ -73,11 +78,12 @@ def peaks():
     try:
         return json.load(open(os.path.join(ROOT, 'MEASURED_PEAKS.json'))), 'measured'
     except Exception:
-        return {'hbm_gbs': 6650.0, 'bf16_tflops': 1590.0, 'bf16_tflops_sustained': 1400.0}, 'fallback'
+        # NVIDIA H100 SXM data sheet (700 W): HBM3 3.35 TB/s, dense BF16 989 TFLOP/s
+        return {'hbm_gbs': 3350.0, 'bf16_tflops': 989.0, 'bf16_tflops_sustained': None}, 'H100 SXM data sheet'
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons sampled DURING the timed region (B200_PROFILING.md)."""
+    """nvidia-smi clocks / throttle reasons sampled DURING the timed region."""
     Q = ('clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,'
          'clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,'
          'clocks_event_reasons.sw_power_cap')
@@ -275,6 +281,8 @@ def run_ours(args):
     TIMER.enabled = False
     clocks = sampler.stop()
     loss_probe = algo.layer_loss(f'{W}.self_attn.q_proj') if K > 0 else None
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, algo, blocks[W + K - 1], W + K - 1)
     del algo, model, blocks
     torch.cuda.empty_cache()
 
@@ -342,34 +350,25 @@ def run_ours(args):
     dom = max(kern, key=lambda k: kern[k]['ms'])
     # the roofline object describes the dominant TENSOR kernel by time among our kernels
     # Spans are grouped by the device kernel behind them: 'gemm' (fake-quant forward) and 'syrk'
-    # (Hessian) are the two instantiations of csrc/gemm.cu:umma_gemm_kernel.
+    # (Hessian) are the two instantiations of csrc/gemm.cu:wgmma_gemm_kernel.
     own = {k: v for k, v in kern.items() if 'cusolver' not in k}
-    umma = {'ms': 0.0, 'calls': 0, 'flops': 0.0, 'bytes': 0.0}
+    mma = {'ms': 0.0, 'calls': 0, 'flops': 0.0, 'bytes': 0.0}
     for k in ('gemm', 'syrk'):
         if k in own:
-            for f in umma:
-                umma[f] += own[k][f]
+            for f in mma:
+                mma[f] += own[k][f]
     dom_own = max(own, key=lambda k: own[k]['ms'])
     d = own[dom_own]
-    ncu = {}
-    try:
-        with open(os.path.join(os.path.dirname(os.path.abspath(__file__)), 'profiles', 'roofline_traffic.json')) as f:
-            ncu = json.load(f)
-    except (OSError, ValueError):
-        pass
-    if umma['ms'] >= d['ms'] and umma['flops'] > 0:
+    if mma['ms'] >= d['ms'] and mma['flops'] > 0:
         # one launch = one 16-sample chunk GEMM or one SYRK; algorithmic flops = 2MNK (GEMM),
         # T*C*(C+1) (SYRK, unique entries only); DESIGN.md section 4
-        ach = umma['flops'] / umma['ms'] / 1e9
+        ach = mma['flops'] / mma['ms'] / 1e9
         peak_tf = pk['bf16_tflops']
-        roof = {'kernel': 'umma_gemm_kernel (spans gemm+syrk)', 'bound': 'tensor', 'achieved': round(ach, 1),
-                'peak': peak_tf, 'unit': 'TFLOP/s', 'frac': round(ach / peak_tf, 4),
-                'traffic': ncu.get('umma_gemm_kernel', {}).get('dram_bytes_per_launch'),
-                'traffic_note': ncu.get('umma_gemm_kernel', {}).get('note'),
-                'peak_source': f'{pk_src} bf16_tflops (cuBLAS burst); sustained figure: '
-                               f'{pk.get("bf16_tflops_sustained")}',
-                'avg_launch_ms': round(umma['ms'] / umma['calls'], 4), 'launches': umma['calls'],
-                'algorithmic_flops_per_launch': round(umma['flops'] / umma['calls'], 1)}
+        roof = {'kernel': 'wgmma_gemm_kernel (spans gemm+syrk)', 'bound': 'tensor', 'achieved': round(ach, 1),
+                'peak': peak_tf, 'unit': 'TFLOP/s', 'frac': round(ach / peak_tf, 4), 'traffic': None,
+                'peak_source': f'{pk_src} bf16_tflops',
+                'avg_launch_ms': round(mma['ms'] / mma['calls'], 4), 'launches': mma['calls'],
+                'algorithmic_flops_per_launch': round(mma['flops'] / mma['calls'], 1)}
     else:
         ach = d['bytes'] / d['ms'] / 1e6
         roof = {'kernel': dom_own, 'bound': 'hbm', 'achieved': round(ach, 1), 'peak': pk['hbm_gbs'],
@@ -402,6 +401,39 @@ def run_ours(args):
         'check': {'q_proj_loss_first_timed_block': loss_probe, 'dominant_span': dom},
     }
     emit(line)
+
+
+# ---------------------------------------------------------------------------------- output dump
+DUMP_SAMPLE = dict(block_out=1 << 20, weight=1 << 18, qparams=1 << 16)
+
+
+def _sample(t, n, seed):
+    """float32 copy of a fixed, seeded sample of n elements of t (all of t when it is smaller);
+    the indices depend only on (numel, n, seed), so equal shapes give equal positions."""
+    flat = t.detach().reshape(-1)
+    if flat.numel() <= n:
+        return flat.float().cpu().numpy()
+    g = torch.Generator().manual_seed(seed)
+    idx = torch.randint(0, flat.numel(), (n,), generator=g).sort().values
+    return flat[idx.to(flat.device)].float().cpu().numpy()
+
+
+def dump_outputs(out_dir, algo, block, idx):
+    """What the step of block `idx` returned to its caller: the block output that feeds the next
+    block, and per linear the calibrated weight, group scales / zeros and per-row losses."""
+    import numpy as np
+    os.makedirs(out_dir, exist_ok=True)
+    torch.cuda.synchronize()
+    np.save(os.path.join(out_dir, 'block_out.npy'), _sample(algo.input['stacked'], DUMP_SAMPLE['block_out'], 0))
+    mods = dict(block.named_modules())
+    for name in ('self_attn.q_proj', 'self_attn.k_proj', 'self_attn.v_proj', 'self_attn.o_proj',
+                 'mlp.gate_proj', 'mlp.up_proj', 'mlp.down_proj'):
+        m = mods[name]
+        np.save(os.path.join(out_dir, f'{name}.weight.npy'), _sample(m.weight, DUMP_SAMPLE['weight'], 1))
+        np.save(os.path.join(out_dir, f'{name}.scales.npy'), _sample(m.buf_scales, DUMP_SAMPLE['qparams'], 2))
+        np.save(os.path.join(out_dir, f'{name}.zeros.npy'), _sample(m.buf_zeros, DUMP_SAMPLE['qparams'], 3))
+        np.save(os.path.join(out_dir, f'{name}.loss.npy'),
+                algo.losses[f'{idx}.{name}'].detach().double().cpu().numpy())
 
 
 # ---------------------------------------------------------------------------------- CPU baseline
@@ -578,7 +610,13 @@ def main():
     ap.add_argument('--model', default=MODEL)
     ap.add_argument('--samples', type=int, default=N_SAMPLES)
     ap.add_argument('--seq-len', dest='seq_len', type=int, default=SEQ_LEN)
+    ap.add_argument('--dump-outputs', dest='dump_outputs', default=None, metavar='DIR',
+                    help='write what the last timed step of the GPU path computed as DIR/<name>.npy')
     args = ap.parse_args()
+    if args.steps < 1:
+        ap.error('--steps must be at least 1')
+    if args.dump_outputs and args.impl == 'reference':
+        ap.error('--dump-outputs writes what the GPU path computed; --impl reference has none')
     if args.impl == 'reference':
         return run_reference(args)
     if not torch.cuda.is_available():

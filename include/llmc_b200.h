@@ -1,5 +1,5 @@
 /*
- * llmc_b200.h — C ABI of libllmc_b200.so: the B200 (sm_100a) kernels behind llmc's
+ * llmc_b200.h — C ABI of libllmc_b200.so: the H100 (sm_90a) kernels behind llmc's
  * weight-quantization hot path (SURVEY.md §8).
  *
  * The reference (ModelTC/llmc) has no FFI: its plug-in boundary is the Python object
@@ -164,8 +164,8 @@ int llmc_pack_awq(const void* w, int64_t R, int64_t C, int dtype, const void* sc
  * K3  llmc_syrk_accum — replaces GPTQ.add_batch's Hessian update (gptq.py:283-290):
  *       H <- H * n/(n+b) + (2/(n+b)) * X^T X          (fp32 H, bf16/fp16 X)
  *   x   [T, C] row-major activations (tokens x in_features), dtype bf16 or fp16
- *   H   [C, C] fp32, full symmetric matrix on return (upper computed on tcgen05 tensor
- *       cores with fp32 TMEM accumulation, mirrored into the lower triangle)
+ *   H   [C, C] fp32, full symmetric matrix on return (upper computed on wgmma tensor
+ *       cores with fp32 register accumulation, mirrored into the lower triangle)
  *   n   samples accumulated so far, b = samples in this call (inp.shape[0], :258)
  *   workspace: split-K partials, >= llmc_syrk_workspace_bytes(T, C) bytes
  * ------------------------------------------------------------------------------------ */
@@ -221,7 +221,7 @@ int llmc_chol_inv_upper(float* A, int64_t C, void* workspace, int64_t workspace_
  *   llmc_gemm_f32x3:  C[M,N] = (mode 1) or C -= (mode 0)  A * B  with
  *       A(i,k) = a[i*lda + k] (a_mn = 0, K-major)  or  a[k*lda + i] (a_mn = 1, MN-major)
  *       B(j,k) = b[j*ldb + k] (b_mn = 0)           or  b[k*ldb + j] (b_mn = 1)
- *     evaluated as A_hi*B_hi + A_lo*B_hi + A_hi*B_lo on tcgen05 kind::tf32 with fp32 TMEM
+ *     evaluated as A_hi*B_hi + A_lo*B_hi + A_hi*B_lo on mma.sync tf32 with fp32 register
  *     accumulation; lower_only != 0 restricts the update to tiles touching col <= row.
  *   These replace the fp32 cuBLAS SGEMMs of gptq.py:244 and the potrf/potri updates of :172-174.
  * ------------------------------------------------------------------------------------ */
@@ -289,7 +289,7 @@ int llmc_spqr_colblock(float* W, const float* Hinv, int64_t R, int64_t C, int64_
 
 /* ------------------------------------------------------------------------------------
  * K6  llmc_gemm_bf16 — Y[M,N] = X[M,K] · W[N,K]^T (+ bias[N]); X, W, Y bf16 or fp16,
- *   fp32 accumulation in TMEM (tcgen05.mma kind::f16), TMA-fed.  This is F.linear of
+ *   fp32 accumulation in registers (wgmma.mma_async), TMA-fed.  This is F.linear of
  *   FakeQuantLinear / EffcientFakeQuantLinear.forward (module_utils.py:643, 719).
  * ------------------------------------------------------------------------------------ */
 int llmc_gemm_bf16(const void* x, const void* w, const void* bias, void* y, int64_t M,
@@ -299,7 +299,7 @@ int llmc_gemm_bf16(const void* x, const void* w, const void* bias, void* y, int6
  * K6  llmc_gemm_w4a16 — fake-quant forward on PACKED weights:
  *   Y[M,N] = X[M,K] · dequant(Wq)[N,K]^T (+ bias), dequant(Wq)[n,k] =
  *   rT((code - zero) * scale) rounded to `dtype` exactly like the materialised weight of
- *   FakeQuantLinear (module_utils.py:626-643); group-wise dequant runs inside the tcgen05
+ *   FakeQuantLinear (module_utils.py:626-643); group-wise dequant runs inside the wgmma
  *   operand pipeline.
  *   wq      [N, K/8] int32, LLMC_OUT_PACK_VLLM layout of UNSIGNED codes (code+2^(bit-1) for
  *           symmetric, code for asymmetric)
@@ -357,7 +357,7 @@ int llmc_fp8_quant(const void* w, int64_t rows, int64_t cols, int dtype, int64_t
  *       out_mode 0 scales only | 1 QDQ (`dtype`) | 2 fp8 bytes.
  *   llmc_fp8_block_dequant  weight_cast_to_bf16 (quant.py:18-29): bf16(fp8.float() * scale_inv).
  *   (The reference's Triton act_quant / fp8_gemm pair, kernel.py:31-53, 141-242, is not built: the
- *   forward of LlmcFp8Linear dequantises once and runs the bf16 tcgen05 GEMM, the reference's own
+ *   forward of LlmcFp8Linear dequantises once and runs the bf16 wgmma GEMM, the reference's own
  *   non-Triton branch, module_utils.py:171-178.)
  * ------------------------------------------------------------------------------------ */
 int llmc_fp8_block_quant(const void* w, int64_t M, int64_t N, int dtype, int block, int e5m2,

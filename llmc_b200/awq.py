@@ -1,5 +1,5 @@
 """AWQ — mirror of llmc/compression/quantization/awq.py (class Awq :28-372) and
-auto_clip.py (class AutoClipper :22-281) on the B200 kernels, plus the scale-migration helpers of
+auto_clip.py (class AutoClipper :22-281) on the CUDA kernels, plus the scale-migration helpers of
 base_blockwise_quantization.py (:596-778, :876-897).
 
 Same YAML knobs (`special: trans, trans_version, weight_clip, clip_sym, clip_version, save_scale,
@@ -11,7 +11,7 @@ inside the batch loop, awq.py:245-248).  What changes is how the numbers are pro
   * x / s, |x| column means and the MSE are single kernels; losses and the running best stay on
     the device (the reference synchronises with `.item()` every grid step);
   * the per-input |x| mean is computed once per subset (the reference recomputes it 20 times);
-  * module forwards run on the tcgen05 GEMM through the swapped weights;
+  * module forwards run on the wgmma GEMM through the swapped weights;
   * auto-clip evaluates its 10 shrink levels in one kernel without the [256, 512, ng, g]
     broadcast temporaries (auto_clip.py:127-179).
 """

@@ -14,7 +14,7 @@ Schedule, one process per GPU (N ranks, block i owned by rank i mod N):
      (L x n/N x S x hidden, e.g. 8.6 GB for Llama-3-8B at N = 8);
   2. per round of N blocks, one NCCL all-gather per block hands its owner the full [n, S, hidden]
      input of the block in the original sample order — the "activation broadcast" of the
-     north_star, 2-4 GiB per block over NVLink / NVSwitch (ring collective, > 200 GB/s);
+     north_star, 2-4 GiB per block over NVLink / NVSwitch (ring collective);
   3. every owner runs the unchanged `block_opt` on its block: no collective inside;
   4. the calibrated block (weights + buf_* qparams) is broadcast from its owner (or only sent to
      rank 0, which saves) — metadata first, because GPTQ changes dtypes and adds buffers.
@@ -132,9 +132,8 @@ class BlockParallelRunner:
                 full = None
                 # The activation "broadcast": one NCCL all-gather per block of the round; the owner
                 # keeps the result, the other ranks reuse one scratch buffer.  (A single all-to-all
-                # would move 1/N of the bytes, but ncclSend/Recv-based all_to_all_single ran at
-                # ~1.4 GB/s per rank on the 8-GPU box — 5.6 of a 7.5 s run — while ring collectives
-                # reach > 200 GB/s; measured in round 2, profiles/r02_block_parallel.md.)
+                # would move 1/N of the bytes, but ncclSend/Recv-based all_to_all_single was measured
+                # two orders of magnitude slower per rank than the ring collectives.)
                 scratch = None
                 for j in range(w):
                     b = k + j

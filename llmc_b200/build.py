@@ -1,4 +1,4 @@
-"""Build libllmc_b200.so (the C-ABI CUDA library) in-tree with nvcc for sm_100a.
+"""Build libllmc_b200.so (the C-ABI CUDA library) in-tree with nvcc for sm_90a (H100).
 
 The library has NO torch / Python dependency: plain `nvcc -shared`, static cudart, the driver
 API (cuTensorMapEncodeTiled) resolved at run time through cudaGetDriverEntryPoint so that
@@ -16,7 +16,7 @@ LIB_NAME = 'libllmc_b200.so'
 LIB_PATH = os.path.join(HERE, LIB_NAME)
 
 NVCC_FLAGS = [
-    '-gencode', 'arch=compute_100a,code=sm_100a',
+    '-gencode', 'arch=compute_90a,code=sm_90a',
     '-O3', '-std=c++17', '-lineinfo',
     '-Xcompiler', '-fPIC',
     '--expt-relaxed-constexpr',
@@ -76,7 +76,7 @@ def build(force=False, verbose=False):
             sys.stderr.write(txt)
     if failed:
         raise RuntimeError('nvcc compilation failed')
-    cmd = [nvcc, '-shared', '-cudart', 'static', '-gencode', 'arch=compute_100a,code=sm_100a',
+    cmd = [nvcc, '-shared', '-cudart', 'static', '-gencode', 'arch=compute_90a,code=sm_90a',
            '-o', LIB_PATH] + objs + ['-ldl']
     subprocess.check_call(cmd)
     with open(stamp, 'w') as fh:

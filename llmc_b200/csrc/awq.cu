@@ -367,7 +367,7 @@ extern "C" int llmc_awq_clip(const void* w, int64_t R, int64_t C, const void* x,
     LLMC_CHECK_CUDA(cudaFuncSetAttribute(awq_clip_err_kernel<LLMC_F16>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
     LLMC_CHECK_CUDA(cudaFuncSetAttribute(awq_clip_err_kernel<LLMC_BF16>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
   });
-  // row slices so that ng * slices ~ a few waves of 148 CTAs
+  // row slices so that ng * slices ~ a few waves of kNumSMs CTAs
   int slices = (4 * kNumSMs + ng - 1) / ng;
   if (slices > (R + 7) / 8) slices = static_cast<int>((R + 7) / 8);
   if (slices < 1) slices = 1;

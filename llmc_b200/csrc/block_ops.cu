@@ -1,7 +1,7 @@
 // block_ops.cu — the elementwise glue of a Llama-shaped decoder block during calibration
 // (F2 of SURVEY.md §8(a): block_forward, base_blockwise_quantization.py:367-390).  The reference
 // runs the HF module, i.e. ~12 eager kernels per norm / rotary / activation with fp32
-// temporaries; over 128 x 2048 calibration tokens that is ~100 ms per block of pure HBM traffic.
+// temporaries, i.e. several extra HBM round trips of the activations per op.
 // Each op here is one pass.  Semantics are those of the HF modules the reference wraps:
 //   rmsnorm : LlamaRMSNorm.forward  — x.float(); x * rsqrt(mean(x^2) + eps); weight * x.to(T)
 //   rope    : apply_rotary_pos_emb  — q * cos + rotate_half(q) * sin, evaluated in T

@@ -145,7 +145,7 @@ diag_kernel(float* __restrict__ G, int64_t n, int64_t k0, int nb, float* __restr
 
 // ---- diag_kernel_v2: the same contract as diag_kernel, blocked by 32 ------------------------------
 // The v1 kernel above is one long sequential sweep whose shared-memory traffic (two LDS per FMA,
-// 2-way conflicts in the inverse) made it 180 us per block — 11 % of a calibration step.  v2 factors
+// 2-way conflicts in the inverse) made it the slowest link of the factorisation chain.  v2 factors
 // 32x32 diagonal sub-blocks in registers (warp shuffles), solves the sub-panel with one thread per
 // row in registers, applies the trailing update with 4x4 register tiles, and builds L^-1 from 32x32
 // block products (X_ij = -X_ii * sum_k L_ik X_kj).  Rows/cols >= nb are padded with the identity so
@@ -469,7 +469,7 @@ extern "C" int llmc_chol_inv_upper(float* A, int64_t C, void* workspace, int64_t
   if (lookahead) {
     // ================= look-ahead schedule (round 2) ==========================================
     // The factorisation's dependent chain is  diag(k) -> panel solve(k) -> update of column block
-    // k+1  (~100 us per 128 columns, 1..112 CTAs wide); everything else — 90 % of the flops — is
+    // k+1  (1..112 CTAs wide); everything else — 90 % of the flops — is
     // off that chain.  Streams (created once per device):
     //   hi    highest priority : the chain.  Inside a super-panel of 4 blocks it is LEFT-looking
     //                            (column block j receives the rank-128*(j-j0) update of its

@@ -1,4 +1,4 @@
-// common.cuh — shared device/host helpers for libllmc_b200.so (sm_100a only).
+// common.cuh — shared device/host helpers for libllmc_b200.so (sm_90a only).
 #pragma once
 
 #include <cuda_runtime.h>
@@ -13,7 +13,7 @@
 
 namespace llmc {
 
-constexpr int kNumSMs = 148;  // B200: 2 dies x 74 SMs
+constexpr int kNumSMs = 132;  // H100 SXM
 
 // ---- error plumbing --------------------------------------------------------------------
 void set_last_error(const char* fmt, ...);

@@ -1,10 +1,13 @@
-// gemm.cu — K3 (Hessian SYRK) and K6 (fake-quant forward GEMM) on tcgen05 tensor cores.
+// gemm.cu — K3 (Hessian SYRK) and K6 (fake-quant forward GEMM) on Hopper wgmma tensor cores.
 //
-// One persistent, warp-specialised kernel template (1 CTA per SM):
-//   warp 0     TMA producer  (cp.async.bulk.tensor -> 128B-swizzled smem ring, mbarrier tx)
-//   warp 1     MMA issuer    (one elected thread, tcgen05.mma kind::f16, fp32 accum in TMEM)
-//   warps 2-5  epilogue      (tcgen05.ld TMEM -> registers -> global), double-buffered TMEM
-// Tile 128(M) x 256(N) x 64(K), 4-stage ring (48 KB / stage), 2 x 256 TMEM columns.
+// One persistent, warp-specialised kernel template (1 CTA per SM, 3 warpgroups):
+//   warpgroup 0     TMA producer (one thread: cp.async.bulk.tensor -> 128B-swizzled smem ring,
+//                   mbarrier transaction counts)
+//   warpgroups 1-2  consumers: each owns 64 rows of the 128 x 256 tile and issues
+//                   wgmma.mma_async m64n128k16 (two per 16-deep K step, one per 128-column half)
+//                   with fp32 accumulators in registers, then stores its rows from registers.
+// Tile 128(M) x 256(N) x 64(K), 4-stage ring (48 KB / stage).  A consumer keeps one wgmma group
+// in flight and frees a ring stage as soon as the group that read it has retired.
 //
 //  * GEMM  (llmc_gemm_bf16):  Y[M,N] = X[M,K] . W[N,K]^T (+bias) — both operands K-major.
 //      Replaces F.linear in FakeQuantLinear / EffcientFakeQuantLinear.forward
@@ -28,9 +31,7 @@ constexpr int kBBytes = BN * BK * 2;                 // 32 KB
 constexpr int kStageBytes = kABytes + kBBytes;       // 48 KB
 constexpr int kBoxBytes = 64 * 64 * 2;               // SYRK box: 64 tokens x 64 channels
 constexpr int kSmemBytes = kStages * kStageBytes + 1024 /*align slack*/ + 256 /*barriers*/;
-constexpr int kThreads = 192;
-constexpr int kTmemCols = 512;
-
+constexpr int kThreads = 384;
 struct GemmParams {
   int64_t M, N, K;          // GEMM: Y[M,N]; SYRK: M = N = C, K = T
   void* out;                // GEMM: Y (bf16/fp16) ; SYRK: partial slabs fp32 [splits][C][C]
@@ -56,7 +57,7 @@ __device__ __forceinline__ Unit decode_unit(const GemmParams& p, int u) {
     // Grouped rasterisation: weights are swept in groups of `gn` n-tiles (<= ~32 MB, L2 resident),
     // all m-tiles per group, n fastest inside the group.  Activations are re-read N/(256*gn)
     // times from HBM, weights once; n-fastest over a 14336-row weight would instead stream the
-    // whole 117 MB weight through L2 once per 148-tile wave.
+    // whole 117 MB weight through L2 once per 132-tile wave.
     const int m_tiles = p.num_tiles / p.n_tiles_n;
     const int per_group = p.gn * m_tiles;
     const int g = u / per_group;
@@ -69,7 +70,7 @@ __device__ __forceinline__ Unit decode_unit(const GemmParams& p, int u) {
     t.split = 0;
   } else {
     // tile fastest, split slowest: concurrent CTAs stream the same token range (L2 reuse).
-    // Tiles are visited in super-rows of `gn` m-blocks, n-major inside a super-row, so the 148
+    // Tiles are visited in super-rows of `gn` m-blocks, n-major inside a super-row, so the 132
     // tiles of a wave form a compact patch of H and touch ~4.6K channels of X per k-block instead
     // of all C (X is streamed from HBM once per wave).
     int tile = u % p.num_tiles;
@@ -100,42 +101,31 @@ __device__ __forceinline__ Unit decode_unit(const GemmParams& p, int u) {
 
 template <bool kSyrk, bool kBf16>
 __global__ void __launch_bounds__(kThreads, 1)
-umma_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
-                 const GemmParams p) {
+wgmma_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
+                  const GemmParams p) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) &
                                              ~static_cast<uintptr_t>(1023));
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + kStages * kStageBytes);
   uint64_t* empty_bar = full_bar + kStages;
-  uint64_t* tmem_full = empty_bar + kStages;
-  uint64_t* tmem_empty = tmem_full + 2;
-  uint32_t* tmem_ptr = reinterpret_cast<uint32_t*>(tmem_empty + 2);
 
-  const int warp = threadIdx.x >> 5;
-  const int lane = threadIdx.x & 31;
+  const int wg = threadIdx.x >> 7;
+  const int tid = threadIdx.x & 127;
 
-  if (warp == 0 && lane == 0) {
+  if (threadIdx.x == 0) {
     prefetch_tmap(&tmA);
     prefetch_tmap(&tmB);
     for (int s = 0; s < kStages; ++s) {
       mbar_init(&full_bar[s], 1);
-      mbar_init(&empty_bar[s], 1);
-    }
-    for (int s = 0; s < 2; ++s) {
-      mbar_init(&tmem_full[s], 1);
-      mbar_init(&tmem_empty[s], 4);   // one arrive per epilogue warp
+      mbar_init(&empty_bar[s], 2);    // one arrive per consumer warpgroup
     }
     fence_barrier_init();
   }
-  if (warp == 1) tmem_alloc(tmem_ptr, kTmemCols);
-  tcgen05_fence_before();
   __syncthreads();
-  tcgen05_fence_after();
-  const uint32_t tmem_base = *tmem_ptr;
 
-  if (warp == 0) {
+  if (wg == 0) {
     // ===================== TMA producer =====================
-    if (lane == 0) {
+    if (tid == 0) {
       int stage = 0;
       uint32_t phase = 0;
       for (int u = blockIdx.x; u < p.num_units; u += gridDim.x) {
@@ -163,119 +153,100 @@ umma_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
         }
       }
     }
-  } else if (warp == 1) {
-    // ===================== MMA issuer =====================
-    constexpr uint32_t idesc = make_idesc_f16(kBf16 ? 1 : 0, kSyrk ? 1 : 0, kSyrk ? 1 : 0, BM, BN);
-    int stage = 0;
-    uint32_t phase = 0;
-    int as = 0;
-    uint32_t aphase = 0;
-    for (int u = blockIdx.x; u < p.num_units; u += gridDim.x) {
-      const Unit t = decode_unit<kSyrk>(p, u);
-      mbar_wait(&tmem_empty[as], aphase ^ 1);
-      tcgen05_fence_after();
-      const uint32_t d_tmem = tmem_base + as * BN;
-      for (int kb = t.kb0; kb < t.kb1; ++kb) {
-        mbar_wait(&full_bar[stage], phase);
-        tcgen05_fence_after();
-        if (lane == 0) {
-          const uint32_t a_addr = smem_u32(smem + stage * kStageBytes);
-          const uint32_t b_addr = a_addr + kABytes;
-#pragma unroll
-          for (int k = 0; k < BK / 16; ++k) {
-            uint64_t adesc, bdesc;
-            if constexpr (!kSyrk) {
-              adesc = make_smem_desc(a_addr + k * 32, 16, 1024);
-              bdesc = make_smem_desc(b_addr + k * 32, 16, 1024);
-            } else {
-              adesc = make_smem_desc(a_addr + k * 2048, kBoxBytes, 1024);
-              bdesc = make_smem_desc(b_addr + k * 2048, kBoxBytes, 1024);
-            }
-            umma_f16(d_tmem, adesc, bdesc, idesc, (kb > t.kb0 || k > 0) ? 1u : 0u);
-          }
-          umma_commit(&empty_bar[stage]);                    // frees the smem slot
-          if (kb == t.kb1 - 1) umma_commit(&tmem_full[as]);  // accumulator complete
-        }
-        __syncwarp();
-        if (++stage == kStages) { stage = 0; phase ^= 1; }
-      }
-      if (t.kb1 <= t.kb0 && lane == 0) umma_commit(&tmem_full[as]);  // empty K range (never)
-      as ^= 1;
-      if (as == 0) aphase ^= 1;
-    }
-  } else {
-    // ===================== epilogue (warps 2..5) =====================
-    const int q = warp & 3;                       // TMEM lane quarter this warp may access
-    int as = 0;
-    uint32_t aphase = 0;
-    for (int u = blockIdx.x; u < p.num_units; u += gridDim.x) {
-      const Unit t = decode_unit<kSyrk>(p, u);
-      mbar_wait(&tmem_full[as], aphase);
-      tcgen05_fence_after();
-      const int64_t row = static_cast<int64_t>(t.m_blk) * BM + q * 32 + lane;
-      const uint32_t taddr0 = tmem_base + (static_cast<uint32_t>(q * 32) << 16) + as * BN;
-#pragma unroll 1
-      for (int c = 0; c < BN; c += 32) {
-        uint32_t r[32];
-        tmem_ld_32x32b_x32(taddr0 + c, r);
-        tmem_ld_wait();
-        const int64_t col0 = static_cast<int64_t>(t.n_blk) * BN + c;
-        if (row < p.M && col0 < p.N) {
-          if constexpr (kSyrk) {
-            float* o = reinterpret_cast<float*>(p.out) +
-                       (static_cast<int64_t>(t.split) * p.M + row) * p.ld_out + col0;
-            if (col0 + 32 <= p.N) {
-#pragma unroll
-              for (int i = 0; i < 32; i += 4)
-                *reinterpret_cast<uint4*>(o + i) = make_uint4(r[i], r[i + 1], r[i + 2], r[i + 3]);
-            } else {
-              for (int i = 0; i < 32 && col0 + i < p.N; ++i) o[i] = __uint_as_float(r[i]);
-            }
-          } else {
-            uint16_t* o = reinterpret_cast<uint16_t*>(p.out) + row * p.ld_out + col0;
-            const uint16_t* bs = reinterpret_cast<const uint16_t*>(p.bias);
-            const bool full = (col0 + 32 <= p.N) && ((p.ld_out & 7) == 0);
-            uint32_t pk[16];
-#pragma unroll
-            for (int i = 0; i < 32; i += 2) {
-              float v0 = __uint_as_float(r[i]), v1 = __uint_as_float(r[i + 1]);
-              if (bs != nullptr) {
-                // F.linear adds the bias in fp32 before the single rounding to the out dtype
-                if (col0 + i < p.N) v0 += kBf16 ? __uint_as_float(static_cast<uint32_t>(bs[col0 + i]) << 16)
-                                                : __half2float(__ushort_as_half(bs[col0 + i]));
-                if (col0 + i + 1 < p.N) v1 += kBf16 ? __uint_as_float(static_cast<uint32_t>(bs[col0 + i + 1]) << 16)
-                                                    : __half2float(__ushort_as_half(bs[col0 + i + 1]));
-              }
-              if constexpr (kBf16) {
-                __nv_bfloat162 h = __floats2bfloat162_rn(v0, v1);
-                pk[i >> 1] = *reinterpret_cast<uint32_t*>(&h);
-              } else {
-                __half2 h = __floats2half2_rn(v0, v1);
-                pk[i >> 1] = *reinterpret_cast<uint32_t*>(&h);
-              }
-            }
-            if (full) {
-#pragma unroll
-              for (int i = 0; i < 16; i += 4)
-                *reinterpret_cast<uint4*>(o + 2 * i) = make_uint4(pk[i], pk[i + 1], pk[i + 2], pk[i + 3]);
-            } else {
-              for (int i = 0; i < 32 && col0 + i < p.N; ++i)
-                o[i] = static_cast<uint16_t>((i & 1) ? (pk[i >> 1] >> 16) : (pk[i >> 1] & 0xffffu));
-            }
-          }
-        }
-      }
-      tcgen05_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&tmem_empty[as]);
-      as ^= 1;
-      if (as == 0) aphase ^= 1;
-    }
+    return;
   }
 
-  tcgen05_fence_before();
-  __syncthreads();
-  if (warp == 1) tmem_dealloc(tmem_base, kTmemCols);
+  // ===================== consumers (warpgroups 1, 2): rows 64 * c .. 64 * c + 63 =====================
+  const int c = wg - 1;
+  const int lane = tid & 31;
+  int stage = 0;
+  uint32_t phase = 0;
+  for (int u = blockIdx.x; u < p.num_units; u += gridDim.x) {
+    const Unit t = decode_unit<kSyrk>(p, u);
+    float acc0[64], acc1[64];                    // columns [0, 128) and [128, 256) of the tile
+#pragma unroll
+    for (int i = 0; i < 64; ++i) { acc0[i] = 0.f; acc1[i] = 0.f; }
+    int prev = -1;
+    for (int kb = t.kb0; kb < t.kb1; ++kb) {
+      mbar_wait(&full_bar[stage], phase);
+      wgmma_fence();
+      const uint32_t a_addr = smem_u32(smem + stage * kStageBytes);
+      const uint32_t b_addr = a_addr + kABytes;
+#pragma unroll
+      for (int k = 0; k < BK / 16; ++k) {
+        uint64_t adesc, bdesc0, bdesc1;
+        if constexpr (!kSyrk) {
+          adesc = make_smem_desc(a_addr + c * 64 * 128 + k * 32, 16, 1024);
+          bdesc0 = make_smem_desc(b_addr + k * 32, 16, 1024);
+          bdesc1 = make_smem_desc(b_addr + 128 * 128 + k * 32, 16, 1024);
+        } else {
+          adesc = make_smem_desc(a_addr + c * kBoxBytes + k * 2048, kBoxBytes, 1024);
+          bdesc0 = make_smem_desc(b_addr + k * 2048, kBoxBytes, 1024);
+          bdesc1 = make_smem_desc(b_addr + 2 * kBoxBytes + k * 2048, kBoxBytes, 1024);
+        }
+        const uint32_t accum = (kb > t.kb0 || k > 0) ? 1u : 0u;
+        wgmma_m64n128k16<kBf16, kSyrk ? 1 : 0, kSyrk ? 1 : 0>(acc0, adesc, bdesc0, accum);
+        wgmma_m64n128k16<kBf16, kSyrk ? 1 : 0, kSyrk ? 1 : 0>(acc1, adesc, bdesc1, accum);
+      }
+      wgmma_commit();
+      wgmma_wait<1>();                           // the group that read stage `prev` has retired
+      if (prev >= 0 && tid == 0) mbar_arrive(&empty_bar[prev]);
+      prev = stage;
+      if (++stage == kStages) { stage = 0; phase ^= 1; }
+    }
+    wgmma_wait<0>();
+    fence_acc(acc0);
+    fence_acc(acc1);
+    if (prev >= 0 && tid == 0) mbar_arrive(&empty_bar[prev]);
+
+    // ---- epilogue straight from the accumulator registers ----
+    const int64_t row0 = static_cast<int64_t>(t.m_blk) * BM + c * 64 + (tid >> 5) * 16 + (lane >> 2);
+    auto store_half = [&](const float (&acc)[64], int h) {
+#pragma unroll
+      for (int j = 0; j < 16; ++j) {
+        const int64_t col = static_cast<int64_t>(t.n_blk) * BN + h * 128 + 8 * j + 2 * (lane & 3);
+        if (col >= p.N) continue;
+#pragma unroll
+        for (int i = 0; i < 2; ++i) {
+          const int64_t row = row0 + 8 * i;
+          if (row >= p.M) continue;
+          float v0 = acc[4 * j + 2 * i], v1 = acc[4 * j + 2 * i + 1];
+          const bool pair = col + 1 < p.N;
+          if constexpr (kSyrk) {
+            float* o = reinterpret_cast<float*>(p.out) +
+                       (static_cast<int64_t>(t.split) * p.M + row) * p.ld_out + col;
+            if (pair) *reinterpret_cast<float2*>(o) = make_float2(v0, v1);
+            else o[0] = v0;
+          } else {
+            uint16_t* o = reinterpret_cast<uint16_t*>(p.out) + row * p.ld_out + col;
+            const uint16_t* bs = reinterpret_cast<const uint16_t*>(p.bias);
+            if (bs != nullptr) {
+              // F.linear adds the bias in fp32 before the single rounding to the out dtype
+              v0 += kBf16 ? __uint_as_float(static_cast<uint32_t>(bs[col]) << 16)
+                          : __half2float(__ushort_as_half(bs[col]));
+              if (pair) v1 += kBf16 ? __uint_as_float(static_cast<uint32_t>(bs[col + 1]) << 16)
+                                    : __half2float(__ushort_as_half(bs[col + 1]));
+            }
+            uint32_t pk;
+            if constexpr (kBf16) {
+              __nv_bfloat162 hv = __floats2bfloat162_rn(v0, v1);
+              pk = *reinterpret_cast<uint32_t*>(&hv);
+            } else {
+              __half2 hv = __floats2half2_rn(v0, v1);
+              pk = *reinterpret_cast<uint32_t*>(&hv);
+            }
+            if (pair && (p.ld_out & 1) == 0) *reinterpret_cast<uint32_t*>(o) = pk;
+            else {
+              o[0] = static_cast<uint16_t>(pk & 0xffffu);
+              if (pair) o[1] = static_cast<uint16_t>(pk >> 16);
+            }
+          }
+        }
+      }
+    };
+    store_half(acc0, 0);
+    store_half(acc1, 1);
+  }
 }
 
 // ---- SYRK finalize: H = a*H + b*sum_s P_s on the upper triangle, mirrored -----------------------
@@ -358,7 +329,7 @@ int encode_tmap_2d_b16(CUtensorMap* out, const void* base, uint64_t rows, uint64
 }
 
 int encode_tmap_2d_f32(CUtensorMap* out, const void* base, uint64_t rows, uint64_t cols,
-                       uint64_t ld_elems, uint32_t box_rows, uint32_t box_cols, int atom32b) {
+                       uint64_t ld_elems, uint32_t box_rows, uint32_t box_cols) {
   PFN_tmapEncodeTiled fn = get_encode_fn();
   if (!fn) return LLMC_ECUDA;
   cuuint64_t dims[2] = {cols, rows};
@@ -366,8 +337,7 @@ int encode_tmap_2d_f32(CUtensorMap* out, const void* base, uint64_t rows, uint64
   cuuint32_t box[2] = {box_cols, box_rows};
   cuuint32_t estr[2] = {1, 1};
   CUresult r = fn(out, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, const_cast<void*>(base), dims, strides,
-                  box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                  atom32b ? CU_TENSOR_MAP_SWIZZLE_128B_ATOM_32B : CU_TENSOR_MAP_SWIZZLE_128B,
+                  box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
                   CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS) {
     set_last_error("cuTensorMapEncodeTiled(f32) failed with CUresult %d (rows %llu cols %llu ld %llu)",
@@ -403,9 +373,9 @@ int encode_tmap_2d_i32_noswizzle(CUtensorMap* out, const void* base, uint64_t ro
 }
 
 template <bool kSyrk, bool kBf16>
-static int launch_umma(const CUtensorMap& tmA, const CUtensorMap& tmB, const GemmParams& p,
+static int launch_wgmma(const CUtensorMap& tmA, const CUtensorMap& tmB, const GemmParams& p,
                        cudaStream_t st) {
-  auto kern = umma_gemm_kernel<kSyrk, kBf16>;
+  auto kern = wgmma_gemm_kernel<kSyrk, kBf16>;
   LLMC_ONCE_PER_DEVICE({
     LLMC_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemBytes));
   });
@@ -430,7 +400,7 @@ static SyrkPlan plan_syrk(int64_t T, int64_t C) {
   }
   s.num_tiles = tiles;
   s.kb_total = static_cast<int>((T + BK - 1) / BK);
-  // choose the split-K factor that best fills whole waves of 148 CTAs
+  // choose the split-K factor that best fills whole waves of kNumSMs CTAs
   int best = 1;
   double best_eff = 0.0;
   for (int sp = 1; sp <= 16; ++sp) {
@@ -482,8 +452,8 @@ extern "C" int llmc_gemm_bf16(const void* x, const void* w, const void* bias, vo
     p.gn = static_cast<int>(gn);
   }
   cudaStream_t st = static_cast<cudaStream_t>(stream);
-  return dtype == LLMC_BF16 ? launch_umma<false, true>(tmA, tmB, p, st)
-                            : launch_umma<false, false>(tmA, tmB, p, st);
+  return dtype == LLMC_BF16 ? launch_wgmma<false, true>(tmA, tmB, p, st)
+                            : launch_wgmma<false, false>(tmA, tmB, p, st);
 }
 
 extern "C" int64_t llmc_syrk_workspace_bytes(int64_t T, int64_t C) {
@@ -516,10 +486,10 @@ extern "C" int llmc_syrk_accum(const void* x, int64_t T, int64_t C, int dtype, f
   p.num_units = s.num_tiles * s.splits;
   p.kb_total = s.kb_total;
   p.kb_per_split = s.kb_per_split;
-  p.gn = 12;                      // 12 m-blocks (1536 rows) x ~12 n-tiles ~ one wave of 148 tiles
+  p.gn = 12;                      // 12 m-blocks (1536 rows) x ~11 n-tiles ~ one wave of 132 tiles
   cudaStream_t st = static_cast<cudaStream_t>(stream);
-  int rc = dtype == LLMC_BF16 ? launch_umma<true, true>(tmX, tmX, p, st)
-                              : launch_umma<true, false>(tmX, tmX, p, st);
+  int rc = dtype == LLMC_BF16 ? launch_wgmma<true, true>(tmX, tmX, p, st)
+                              : launch_wgmma<true, false>(tmX, tmX, p, st);
   if (rc) return rc;
   // gptq.py:283-290: H *= n/(n+b); H += (sqrt(2/(n+b)) X)^T (sqrt(2/(n+b)) X)
   const float fa = static_cast<float>(n / (n + b));

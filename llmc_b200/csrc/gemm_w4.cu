@@ -1,24 +1,26 @@
-// gemm_w4.cu — K6: fake-quant forward on PACKED INT4 weights, dequantisation fused into the
-// tcgen05 operand pipeline.
+// gemm_w4.cu — K6: fake-quant forward on PACKED INT4 / INT8 weights, dequantisation fused into
+// the wgmma operand pipeline.
 //
 //   Y[M,N] = X[M,K] . dequant(Wq)[N,K]^T (+ bias),   dequant(n,k) = rT( fp32((code - zero) * scale) )
 //
 // which is bit-for-bit the bf16/fp16 weight the reference materialises in FakeQuantLinear /
 // EffcientFakeQuantLinear (llmc/compression/quantization/module_utils.py:626-643, 722-741) before
-// F.linear — so the result equals llmc_gemm_bf16 on that materialised weight exactly (same tile
-// shape, same K order), while the weight stream from HBM is 4.25 bits instead of 16 per element.
+// F.linear — so the result equals llmc_gemm_bf16 on that materialised weight exactly (the same
+// m64n128k16 wgmma per output element, same K order), while the weight stream from HBM is 4.25
+// bits instead of 16 per element.
 //
-// Pipeline per 64-deep K step, TWO rings so that the TMA latency is covered by a deep, cheap ring
-// and the dequantised tile by a short one:
-//   ring L (4 x 24 KB): X tile [128 x 64] bf16 (swizzle 128B) + packed W tile [256 x 8] int32
-//   ring B (3 x 32 KB): the dequantised, 128B-swizzled UMMA B tile
-//   warp 0       TMA into ring L
-//   warps 6..13  dequant (one weight row per thread): nibble -> fp32 via the 2^23 magic constant,
-//                (q - z) * s in fp32, round to bf16/fp16, 16-byte stores into ring B,
-//                fence.proxy.async; the group's scale/zero for the NEXT step is prefetched
-//   warp 1       MMA issuer (tcgen05.mma kind::f16, 128 x 256 x 16, fp32 accumulators in TMEM);
-//                its commit frees the ring-L stage (X consumed) and the ring-B stage
-//   warps 2..5   epilogue (tcgen05.ld -> bias -> bf16/fp16 -> global), double-buffered TMEM
+// Tile 128(M) x 128(N) x 64(K).  Pipeline per K step, TWO rings so that the TMA latency is covered
+// by a deep, cheap ring and the dequantised tile by a short one:
+//   ring L (6 x 20 KB): X tile [128 x 64] bf16 (swizzle 128B) + packed W tile [128 x 8] int32
+//   ring B (3 x 16 KB): the dequantised, 128B-swizzled wgmma B tile
+//   warps 0 .. 4NG-1   dequant, NG groups of four warps taking every NG-th K step (one weight row
+//                      per thread): nibble -> fp32 via the 2^23 magic constant, (q - z) * s in
+//                      fp32, round to bf16/fp16, 16-byte stores into ring B, fence.proxy.async;
+//                      the group's scale/zero for its NEXT step is prefetched
+//   warpgroups NG, NG+1  consumers: 64 rows each, wgmma m64n128k16 with fp32 register
+//                      accumulators; retiring a step's wgmma group frees its ring-L and ring-B
+//                      stages; epilogue (bias -> bf16/fp16 -> global) from registers
+//   warp 4NG + 8       TMA into ring L
 // Weight layout: LLMC_OUT_PACK_VLLM of UNSIGNED codes — 8 nibbles per int32 along K, nibble i =
 // element 8*w + i; scales / zeros fp32 [N, K/group] (zeros NULL => 2^(bit-1), the symmetric
 // +8 offset of module_utils.py:842-844).
@@ -32,24 +34,22 @@ using namespace tc;
 
 namespace w4 {
 
-constexpr int BM = 128, BN = 256, BK = 64;
-// ring B (dequantised W tile) depth and dequant warps are template parameters now: NG groups of
-// four warps take every NG-th K step (see the kernel), ring B is max(3, NG) deep
+constexpr int BM = 128, BN = 128, BK = 64;
 constexpr int kABytes = BM * BK * 2;          // 16 KB
-constexpr int kBBytes = BN * BK * 2;          // 32 KB dequantised
-// per weight width: INT4 -> 8 KB packed tile, 4-deep ring L; INT8 -> 16 KB packed tile, 3-deep
+constexpr int kBBytes = BN * BK * 2;          // 16 KB dequantised
+// per weight width: INT4 -> 4 KB packed tile, INT8 -> 8 KB
 template <int kBits, int NG> struct Cfg {
   static constexpr int kPBytes = BN * BK * kBits / 8;
   static constexpr int kLBytes = kABytes + kPBytes;
   static constexpr int kBStages = NG > 3 ? NG : 3;
-  static constexpr int kLStages = (kBits == 4 && NG <= 2) ? 4 : 3;
+  static constexpr int kLStages = 6;
   static constexpr int kSmemBytes = kLStages * kLBytes + kBStages * kBBytes + 1024 + 256;
   static constexpr int kWordsPerRow = BK * kBits / 32;      // int32 per row of the packed tile
   static constexpr int kDequantWarps = 4 * NG;
-  static constexpr int kThreads = (6 + kDequantWarps) * 32;
+  static constexpr int kConsumerWarp0 = kDequantWarps;      // first warp of the consumer warpgroups
+  static constexpr int kTmaWarp = kDequantWarps + 8;
+  static constexpr int kThreads = (kTmaWarp + 1) * 32;
 };
-constexpr int kTmemCols = 512;
-
 struct Params {
   int64_t M, N, K;
   void* out;
@@ -125,32 +125,24 @@ w4a16_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
   uint64_t* emptyL = fullL + kLStages;
   uint64_t* readyB = emptyL + kLStages;          // dequantised B tile written
   uint64_t* emptyB = readyB + kBStages;
-  uint64_t* tmem_full = emptyB + kBStages;
-  uint64_t* tmem_empty = tmem_full + 2;
-  uint32_t* tmem_ptr = reinterpret_cast<uint32_t*>(tmem_empty + 2);
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
 
-  if (warp == 0 && lane == 0) {
+  if (threadIdx.x == 0) {
     prefetch_tmap(&tmA);
     prefetch_tmap(&tmP);
     for (int s = 0; s < kLStages; ++s) {
       mbar_init(&fullL[s], 1);
-      mbar_init(&emptyL[s], 1 + 4);                   // MMA commit (X) + the step's dequant group (4 warps)
+      mbar_init(&emptyL[s], 2 + 4);                   // both consumer warpgroups + the step's dequant group
     }
     for (int s = 0; s < kBStages; ++s) {
       mbar_init(&readyB[s], 4);
-      mbar_init(&emptyB[s], 1);
+      mbar_init(&emptyB[s], 2);
     }
-    for (int s = 0; s < 2; ++s) { mbar_init(&tmem_full[s], 1); mbar_init(&tmem_empty[s], 4); }
     fence_barrier_init();
   }
-  if (warp == 1) tmem_alloc(tmem_ptr, kTmemCols);
-  tcgen05_fence_before();
   __syncthreads();
-  tcgen05_fence_after();
-  const uint32_t tmem_base = *tmem_ptr;
 
-  if (warp == 0) {
+  if (warp == C::kTmaWarp) {
     // ===================== TMA producer =====================
     if (lane == 0) {
       int sl = 0;
@@ -169,53 +161,86 @@ w4a16_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
         }
       }
     }
-  } else if (warp == 1) {
-    // ===================== MMA issuer =====================
-    constexpr uint32_t idesc = make_idesc_f16(kBf16 ? 1 : 0, 0, 0, BM, BN);
+  } else if (warp >= C::kConsumerWarp0) {
+    // ===================== consumers: rows 64 * c .. 64 * c + 63 of the tile =====================
+    const int c = (warp - C::kConsumerWarp0) >> 2;
+    const int tid = threadIdx.x & 127;
     int sl = 0, sb = 0;
     uint32_t phl = 0, phb = 0;
-    int as = 0;
-    uint32_t aphase = 0;
     for (int u = blockIdx.x; u < p.num_units; u += gridDim.x) {
-      mbar_wait(&tmem_empty[as], aphase ^ 1);
-      tcgen05_fence_after();
-      const uint32_t d_tmem = tmem_base + as * BN;
+      int m_blk, n_blk;
+      decode(p, u, m_blk, n_blk);
+      float acc[64];
+#pragma unroll
+      for (int i = 0; i < 64; ++i) acc[i] = 0.f;
+      int prev_l = -1, prev_b = -1;
       for (int kb = 0; kb < p.kb_total; ++kb) {
         mbar_wait(&fullL[sl], phl);              // X tile landed
         mbar_wait(&readyB[sb], phb);             // W tile dequantised
-        tcgen05_fence_after();
-        if (lane == 0) {
-          const uint32_t a_addr = smem_u32(ringL + sl * kLBytes);
-          const uint32_t b_addr = smem_u32(ringB + sb * kBBytes);
+        wgmma_fence();
+        const uint32_t a_addr = smem_u32(ringL + sl * kLBytes) + c * 64 * 128;
+        const uint32_t b_addr = smem_u32(ringB + sb * kBBytes);
 #pragma unroll
-          for (int k = 0; k < BK / 16; ++k) {
-            const uint64_t adesc = make_smem_desc(a_addr + k * 32, 16, 1024);
-            const uint64_t bdesc = make_smem_desc(b_addr + k * 32, 16, 1024);
-            umma_f16(d_tmem, adesc, bdesc, idesc, (kb > 0 || k > 0) ? 1u : 0u);
-          }
-          umma_commit(&emptyL[sl]);
-          umma_commit(&emptyB[sb]);
-          if (kb == p.kb_total - 1) umma_commit(&tmem_full[as]);
+        for (int k = 0; k < BK / 16; ++k) {
+          const uint64_t adesc = make_smem_desc(a_addr + k * 32, 16, 1024);
+          const uint64_t bdesc = make_smem_desc(b_addr + k * 32, 16, 1024);
+          wgmma_m64n128k16<kBf16, 0, 0>(acc, adesc, bdesc, (kb > 0 || k > 0) ? 1u : 0u);
         }
-        __syncwarp();
+        wgmma_commit();
+        wgmma_wait<1>();                         // the previous step's group has retired
+        if (prev_l >= 0 && tid == 0) {
+          mbar_arrive(&emptyL[prev_l]);
+          mbar_arrive(&emptyB[prev_b]);
+        }
+        prev_l = sl;
+        prev_b = sb;
         if (++sl == kLStages) { sl = 0; phl ^= 1; }
         if (++sb == kBStages) { sb = 0; phb ^= 1; }
       }
-      as ^= 1;
-      if (as == 0) aphase ^= 1;
+      wgmma_wait<0>();
+      fence_acc(acc);
+      if (prev_l >= 0 && tid == 0) {
+        mbar_arrive(&emptyL[prev_l]);
+        mbar_arrive(&emptyB[prev_b]);
+      }
+      // ---- epilogue from the accumulator registers ----
+      const int64_t row0 = static_cast<int64_t>(m_blk) * BM + c * 64 + (tid >> 5) * 16 + (lane >> 2);
+      const uint16_t* bs = reinterpret_cast<const uint16_t*>(p.bias);
+#pragma unroll
+      for (int j = 0; j < 16; ++j) {
+        const int64_t col = static_cast<int64_t>(n_blk) * BN + 8 * j + 2 * (lane & 3);
+        if (col >= p.N) continue;
+        const bool pair = col + 1 < p.N;
+        float b0 = 0.f, b1 = 0.f;
+        if (bs != nullptr) {
+          b0 = kBf16 ? __uint_as_float(static_cast<uint32_t>(bs[col]) << 16)
+                     : __half2float(__ushort_as_half(bs[col]));
+          if (pair) b1 = kBf16 ? __uint_as_float(static_cast<uint32_t>(bs[col + 1]) << 16)
+                               : __half2float(__ushort_as_half(bs[col + 1]));
+        }
+#pragma unroll
+        for (int i = 0; i < 2; ++i) {
+          const int64_t row = row0 + 8 * i;
+          if (row >= p.M) continue;
+          float v0 = acc[4 * j + 2 * i], v1 = acc[4 * j + 2 * i + 1];
+          if (bs != nullptr) { v0 += b0; v1 += b1; }
+          const uint32_t pk = pack2<kBf16>(v0, v1);
+          uint16_t* o = reinterpret_cast<uint16_t*>(p.out) + row * p.N + col;
+          if (pair && (p.N & 1) == 0) *reinterpret_cast<uint32_t*>(o) = pk;
+          else {
+            o[0] = static_cast<uint16_t>(pk & 0xffffu);
+            if (pair) o[1] = static_cast<uint16_t>(pk >> 16);
+          }
+        }
+      }
     }
-  } else if (warp >= 6) {
-    // ===================== dequant warps (4 * NG): two weight rows per thread =====================
-    // NG groups of four warps take every NG-th K step.  A thread's unpack -> convert -> store chain
-    // for its 128 weights of a tile is ~2300 cycles of dependent latency (round-2 finding: with two
-    // groups the kernel ran at exactly one tile per two such chains, tensor pipe 44 % active, while
-    // only half of the issue slots were used) — more groups in flight, not more instructions per
-    // clock, is what hides it.  Ring B has one stage per group.
-    const int grp = (warp - 6) % NG;
-    const int tig = ((warp - 6) / NG) * 32 + lane;   // 0..127 inside the group
+  } else {
+    // ===================== dequant warps (4 * NG): one weight row per thread =====================
+    // NG groups of four warps take every NG-th K step, so that several groups' dependent
+    // unpack -> convert -> store chains are in flight at once.  Ring B has one stage per group.
+    const int grp = warp % NG;
+    const int row = (warp / NG) * 32 + lane;         // 0..127 inside the group
     uint32_t it = 0;                                 // K steps issued so far (all tiles)
-    // raw group qparams of row n, group gi (no arithmetic on the loaded values here: the loads
-    // must stay in flight while the current step is dequantised)
     // RAW bits of (scale, zero) — widening / arithmetic happens at use (widen below), so the two
     // loads stay in flight across a whole K step
     auto load_qparams = [&](int64_t n, int gi, uint32_t& s, uint32_t& z) {
@@ -239,61 +264,51 @@ w4a16_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
     for (int u = blockIdx.x; u < p.num_units; u += gridDim.x) {
       int m_blk, n_blk;
       decode(p, u, m_blk, n_blk);
-      const int64_t n0 = static_cast<int64_t>(n_blk) * BN + tig;
+      const int64_t n0 = static_cast<int64_t>(n_blk) * BN + row;
       // first K step of this tile that belongs to this group: (it + kb) % NG == grp
       int kb = (grp + NG - static_cast<int>(it % NG)) % NG;
-      uint32_t s_cur[2] = {0u, 0u}, z_cur[2] = {0u, 0u};
-      if (kb < p.kb_total) {
-#pragma unroll
-        for (int h = 0; h < 2; ++h) load_qparams(n0 + h * 128, kb / steps_per_group, s_cur[h], z_cur[h]);
-      }
+      uint32_t s_cur = 0u, z_cur = 0u;
+      if (kb < p.kb_total) load_qparams(n0, kb / steps_per_group, s_cur, z_cur);
       for (; kb < p.kb_total; kb += NG) {
         const uint32_t my = it + kb;
         const int sl = my % kLStages, sb = my % kBStages;
         const uint32_t phl = (my / kLStages) & 1u, phb = (my / kBStages) & 1u;
         // qparams of this group's NEXT step are requested now and consumed next iteration
-        uint32_t s_nxt[2] = {s_cur[0], s_cur[1]}, z_nxt[2] = {z_cur[0], z_cur[1]};
-        if (kb + NG < p.kb_total && (kb + NG) / steps_per_group != kb / steps_per_group) {
-#pragma unroll
-          for (int h = 0; h < 2; ++h)
-            load_qparams(n0 + h * 128, (kb + NG) / steps_per_group, s_nxt[h], z_nxt[h]);
-        }
+        uint32_t s_nxt = s_cur, z_nxt = z_cur;
+        if (kb + NG < p.kb_total && (kb + NG) / steps_per_group != kb / steps_per_group)
+          load_qparams(n0, (kb + NG) / steps_per_group, s_nxt, z_nxt);
         mbar_wait(&fullL[sl], phl);
         mbar_wait(&emptyB[sb], phb ^ 1);
         const uint8_t* pk = ringL + sl * kLBytes + kABytes;
         uint8_t* bt = ringB + sb * kBBytes;
+        const float z_c = have_zeros ? widen(z_cur) : p.zero_default;
+        const float zm_cur = 8388608.0f + z_c;        // (2^23 + q) - (2^23 + z) = q - z exactly
+        const float s_c = (n0 < p.N) ? widen(s_cur) : 0.f;
+        if constexpr (kBits == 8) {
+          // INT8: 64-byte rows, TMA SWIZZLE_64B: 16-byte chunk c of row r sits at c ^ ((r >> 1) & 3).
+          // byte -> fp32 through the 2^23 magic (0x4B0000nn), (q - z) * s in fp32, one rounding;
+          // bf16 has no exact packed form for 8-bit codes (128 + q needs 9 bits), so both qparam
+          // flavours take this path (same value: the product of two T numbers rounds once).
+          const int sw8 = (row >> 1) & 3;
 #pragma unroll
-        for (int h = 0; h < 2; ++h) {
-          const int row = tig + h * 128;
-          const float z_c = have_zeros ? widen(z_cur[h]) : p.zero_default;
-          const float zm_cur = 8388608.0f + z_c;        // (2^23 + q) - (2^23 + z) = q - z exactly
-          const float s_c = (n0 + h * 128 < p.N) ? widen(s_cur[h]) : 0.f;
-          if constexpr (kBits == 8) {
-            // INT8: 64-byte rows, TMA SWIZZLE_64B: 16-byte chunk c of row r sits at c ^ ((r >> 1) & 3).
-            // byte -> fp32 through the 2^23 magic (0x4B0000nn), (q - z) * s in fp32, one rounding;
-            // bf16 has no exact packed form for 8-bit codes (128 + q needs 9 bits), so both qparam
-            // flavours take this path (same value: the product of two T numbers rounds once).
-            const int sw8 = (row >> 1) & 3;
+          for (int c4 = 0; c4 < 4; ++c4) {
+            const uint4 wv = *reinterpret_cast<const uint4*>(pk + row * 64 + ((c4 ^ sw8) << 4));
+            const uint32_t wd[4] = {wv.x, wv.y, wv.z, wv.w};
 #pragma unroll
-            for (int c4 = 0; c4 < 4; ++c4) {
-              const uint4 wv = *reinterpret_cast<const uint4*>(pk + row * 64 + ((c4 ^ sw8) << 4));
-              const uint32_t wd[4] = {wv.x, wv.y, wv.z, wv.w};
+            for (int hh = 0; hh < 2; ++hh) {
+              float v[8];
 #pragma unroll
-              for (int hh = 0; hh < 2; ++hh) {
-                float v[8];
-#pragma unroll
-                for (int j = 0; j < 4; ++j) {
-                  v[j] = fmul_rn(__uint_as_float(__byte_perm(wd[2 * hh], 0x4B000000u, 0x7650u + j)) - zm_cur, s_c);
-                  v[4 + j] = fmul_rn(__uint_as_float(__byte_perm(wd[2 * hh + 1], 0x4B000000u, 0x7650u + j)) - zm_cur, s_c);
-                }
-                const uint4 o = make_uint4(pack2<kBf16>(v[0], v[1]), pack2<kBf16>(v[2], v[3]),
-                                           pack2<kBf16>(v[4], v[5]), pack2<kBf16>(v[6], v[7]));
-                const int c = c4 * 2 + hh;
-                *reinterpret_cast<uint4*>(bt + row * 128 + ((c ^ (row & 7)) << 4)) = o;
+              for (int j = 0; j < 4; ++j) {
+                v[j] = fmul_rn(__uint_as_float(__byte_perm(wd[2 * hh], 0x4B000000u, 0x7650u + j)) - zm_cur, s_c);
+                v[4 + j] = fmul_rn(__uint_as_float(__byte_perm(wd[2 * hh + 1], 0x4B000000u, 0x7650u + j)) - zm_cur, s_c);
               }
+              const uint4 o = make_uint4(pack2<kBf16>(v[0], v[1]), pack2<kBf16>(v[2], v[3]),
+                                         pack2<kBf16>(v[4], v[5]), pack2<kBf16>(v[6], v[7]));
+              const int c = c4 * 2 + hh;
+              *reinterpret_cast<uint4*>(bt + row * 128 + ((c ^ (row & 7)) << 4)) = o;
             }
-            continue;
           }
+        } else {
           // packed tile is TMA-swizzled (32B): half h of row r sits at half h ^ ((r >> 2) & 1)
           const int sw = ((row >> 2) & 1) << 4;
           const uint4 w0 = *reinterpret_cast<const uint4*>(pk + row * 32 + sw);
@@ -322,9 +337,8 @@ w4a16_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
           } else {
 #pragma unroll
             for (int c = 0; c < 8; ++c) {            // one 16-byte chunk = 8 elements = one word
-              // The integer pipe is the scarce resource (64 lanes vs 128 fp32 lanes per SM and
-              // clock): split the word into even / odd nibbles once, then ONE byte-permute per
-              // element builds the fp32 bit pattern 0x4B0000nn = 2^23 + nibble.
+              // split the word into even / odd nibbles once, then ONE byte-permute per element
+              // builds the fp32 bit pattern 0x4B0000nn = 2^23 + nibble
               const uint32_t w = words[c];
               const uint32_t ev = w & 0x0F0F0F0Fu;           // nibbles 0,2,4,6 in bytes 0..3
               const uint32_t od = (w >> 4) & 0x0F0F0F0Fu;    // nibbles 1,3,5,7
@@ -348,65 +362,12 @@ w4a16_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
           mbar_arrive(&readyB[sb]);
           mbar_arrive(&emptyL[sl]);                // packed tile consumed
         }
-#pragma unroll
-        for (int h = 0; h < 2; ++h) { s_cur[h] = s_nxt[h]; z_cur[h] = z_nxt[h]; }
+        s_cur = s_nxt;
+        z_cur = z_nxt;
       }
       it += static_cast<uint32_t>(p.kb_total);
     }
-  } else {
-    // ===================== epilogue (warps 2..5) =====================
-    const int q = warp & 3;
-    int as = 0;
-    uint32_t aphase = 0;
-    for (int u = blockIdx.x; u < p.num_units; u += gridDim.x) {
-      int m_blk, n_blk;
-      decode(p, u, m_blk, n_blk);
-      mbar_wait(&tmem_full[as], aphase);
-      tcgen05_fence_after();
-      const int64_t row = static_cast<int64_t>(m_blk) * BM + q * 32 + lane;
-      const uint32_t taddr0 = tmem_base + (static_cast<uint32_t>(q * 32) << 16) + as * BN;
-#pragma unroll 1
-      for (int c = 0; c < BN; c += 32) {
-        uint32_t r[32];
-        tmem_ld_32x32b_x32(taddr0 + c, r);
-        tmem_ld_wait();
-        const int64_t col0 = static_cast<int64_t>(n_blk) * BN + c;
-        if (row < p.M && col0 < p.N) {
-          uint16_t* o = reinterpret_cast<uint16_t*>(p.out) + row * p.N + col0;
-          const uint16_t* bs = reinterpret_cast<const uint16_t*>(p.bias);
-          const bool full = (col0 + 32 <= p.N) && ((p.N & 7) == 0);
-          uint32_t pk[16];
-#pragma unroll
-          for (int i = 0; i < 32; i += 2) {
-            float v0 = __uint_as_float(r[i]), v1 = __uint_as_float(r[i + 1]);
-            if (bs != nullptr) {
-              if (col0 + i < p.N) v0 += kBf16 ? __uint_as_float(static_cast<uint32_t>(bs[col0 + i]) << 16)
-                                              : __half2float(__ushort_as_half(bs[col0 + i]));
-              if (col0 + i + 1 < p.N) v1 += kBf16 ? __uint_as_float(static_cast<uint32_t>(bs[col0 + i + 1]) << 16)
-                                                  : __half2float(__ushort_as_half(bs[col0 + i + 1]));
-            }
-            pk[i >> 1] = pack2<kBf16>(v0, v1);
-          }
-          if (full) {
-#pragma unroll
-            for (int i = 0; i < 16; i += 4)
-              *reinterpret_cast<uint4*>(o + 2 * i) = make_uint4(pk[i], pk[i + 1], pk[i + 2], pk[i + 3]);
-          } else {
-            for (int i = 0; i < 32 && col0 + i < p.N; ++i)
-              o[i] = static_cast<uint16_t>((i & 1) ? (pk[i >> 1] >> 16) : (pk[i >> 1] & 0xffffu));
-          }
-        }
-      }
-      tcgen05_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&tmem_empty[as]);
-      as ^= 1;
-      if (as == 0) aphase ^= 1;
-    }
   }
-  tcgen05_fence_before();
-  __syncthreads();
-  if (warp == 1) tmem_dealloc(tmem_base, kTmemCols);
 }
 
 }  // namespace w4
@@ -480,9 +441,7 @@ static int gemm_wNa16_ng(const void* x, const int32_t* wq, const void* scales, c
   return LLMC_OK;
 }
 
-// Two dequant groups.  (A four-group variant — the template parameter NG exists for it — was
-// tried in round 2 on the theory that the per-thread unpack chain, not issue bandwidth, limits the
-// kernel: it was slower, 728 vs 871 TFLOP/s, and is not instantiated.)
+// Two dequant groups (eight warps, one weight row per thread and K step).
 template <int kBits>
 static int gemm_wNa16(const void* x, const int32_t* wq, const void* scales, const void* zeros,
                       int qparam_dtype, const void* bias, void* y, int64_t M, int64_t N, int64_t K,

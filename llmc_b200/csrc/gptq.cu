@@ -379,7 +379,7 @@ gptq_inblock_kernel(InblockArgs a) {
 
 // ---- in-block column loop, v2: eight lanes per weight row ----------------------------------------------
 // v1 above gives one thread a whole row: 128 CTAs' worth of parallelism does not exist for
-// R = 4096 (32 CTAs on 148 SMs, one warp per scheduler, IPC 0.23 per warp, 85 us per block).
+// R = 4096 (32 CTAs, one warp per scheduler).
 // v2 spreads a row over 8 lanes (lane l owns columns l, l+8, ...), 32 rows per CTA, 256 threads,
 // two CTAs per SM:
 //   * per 8-column sub-block each lane keeps ITS column in a register; the eight sequential
@@ -401,7 +401,7 @@ constexpr int kInblockV2Smem = (IR * WP + GB * EP + GB * HP2 + 2 * GB) * 4;
 // rounded quotient (Markstein), provided nothing under/overflows: x, s and r with exponents in
 // [2^-40, 2^41) keep q and both residuals normal (x = 0 is exact as well).  Anything else takes
 // div.rn, kept OUT of line: inlined, its ~10-instruction sequence sat on the dependent chain of
-// every column step whether or not it was needed (profiles/r01c_hot_gptq_inblock_v2.md).
+// every column step whether or not it was needed.
 __device__ __noinline__ float div_exact_slow(float x, float s) { return fdiv_rn(x, s); }
 
 __device__ __forceinline__ bool exp_mid(float v) {
@@ -765,13 +765,13 @@ spqr_inblock_kernel(SpqrArgs a) {
 
 // ---- SpQR in-block kernel, 16 lanes per weight row ----------------------------------------------------------
 // spqr_inblock_kernel above gives a row to ONE thread: 32 CTAs for R = 4096, one warp per scheduler,
-// 887 us per 128-column block (profiles/r02_microbench_spqr.txt).  Here a row is spread over 16 lanes
+// latency bound.  Here a row is spread over 16 lanes
 // (16 rows per CTA, 256 threads, two CTAs per SM): lane j evaluates the leave-one-out cases j,
 // j + 16, ... of a group, every lane recomputes the cheap group statistics, and after the (redundant)
 // quantise -> err step of a column each lane applies the rank-1 update to the later columns it owns.
 // The three phases are spqr::lanes_* of spqr_row.cuh — bit-identical to row_block() by construction,
-// checked on the host (lock-step emulation) by the CPU tests and on the GPU against the kernel above
-// (1000 x 1024, g16: 6.8 -> 1.2 ms).  Lanes talk through the row's
+// checked on the host (lock-step emulation) by the CPU tests and on the GPU against the kernel above.
+// Lanes talk through the row's
 // shared-memory storage, with __syncwarp() between phases.
 constexpr int SL = 16;            // lanes per row
 constexpr int SR = 16;            // rows per CTA
@@ -1011,9 +1011,9 @@ static int sweep_schedule(float* W, const float* Hinv, int64_t R, int64_t C, int
   const bool groups_fit = group <= GB || kSuperPanel % group == 0 || group % kSuperPanel == 0;
   const int64_t sp_width = (tensor_trailing && groups_fit) ? kSuperPanel : GB;
   // ---- look-ahead schedule ------------------------------------------------------------------
-  // The sweep's dependent chain is  in-block kernel -> in-panel update -> next in-block kernel
-  // (~90 us per 128 columns); the rank-512 update of everything beyond a super-panel is 25-35 % of
-  // the sweep's time at R >= 4096 and is NOT on that chain beyond the next 512 columns.  So at a
+  // The sweep's dependent chain is  in-block kernel -> in-panel update -> next in-block kernel;
+  // the rank-512 update of everything beyond a super-panel is a large share of the sweep's work
+  // at R >= 4096 and is NOT on that chain beyond the next 512 columns.  So at a
   // super-panel boundary the chain (high-priority stream) updates the next super-panel's columns
   // only, and the rest goes to a low-priority stream, one tile per CTA, overlapping the next
   // panel's chain.  Every column receives its panel updates in the same order as before (events),

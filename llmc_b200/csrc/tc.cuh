@@ -1,6 +1,6 @@
-// tc.cuh — sm_100a building blocks: mbarrier, TMA (cp.async.bulk.tensor), tcgen05 (UMMA +
-// TMEM).  Hand-written inline PTX; bit layouts follow the PTX ISA "tcgen05" chapter
-// (cross-checked against cute/arch/mma_sm100_desc.hpp field tables).
+// tc.cuh — sm_90a building blocks: mbarrier, TMA (cp.async.bulk.tensor) and warpgroup MMA
+// (wgmma.mma_async, fp32 accumulators in registers).  Hand-written inline PTX; descriptor bit
+// layouts follow the PTX ISA "asynchronous warpgroup level matrix" chapter.
 #pragma once
 
 #include <cuda.h>  // CUtensorMap (types only; the driver entry point is resolved at run time)
@@ -12,19 +12,6 @@ namespace tc {
 
 __device__ __forceinline__ uint32_t smem_u32(const void* p) {
   return static_cast<uint32_t>(__cvta_generic_to_shared(p));
-}
-
-__device__ __forceinline__ bool elect_one() {
-  uint32_t pred = 0;
-  asm volatile(
-      "{\n"
-      ".reg .b32 rx;\n"
-      ".reg .pred px;\n"
-      "elect.sync rx|px, 0xffffffff;\n"
-      "selp.b32 %0, 1, 0, px;\n"
-      "}\n"
-      : "=r"(pred));
-  return pred != 0;
 }
 
 // ---- mbarrier ---------------------------------------------------------------------------
@@ -42,7 +29,8 @@ __device__ __forceinline__ void mbar_expect_tx(uint64_t* bar, uint32_t bytes) {
 __device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
   asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
 }
-// Bounded wait: a protocol bug must trap (kernel error) instead of hanging the GPU.
+// Bounded wait: a protocol bug must trap (kernel error) instead of hanging the GPU.  No printf on
+// the timeout path: a function call inside a wgmma loop makes ptxas serialise every wgmma.
 __device__ __forceinline__ bool mbar_try_wait(uint32_t addr, uint32_t parity) {
   uint32_t done = 0;
   asm volatile(
@@ -66,15 +54,11 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
   if (mbar_try_wait(addr, parity)) return;
   const uint64_t t0 = globaltimer_ns();
   while (!mbar_try_wait(addr, parity)) {
-    if (globaltimer_ns() - t0 > 5000000000ull) {  // 5 s: far beyond any legitimate wait
-      printf("llmc_b200: mbarrier wait timed out (block %d thread %d bar %u parity %u)\n",
-             blockIdx.x, threadIdx.x, addr, parity);
-      __trap();
-    }
+    if (globaltimer_ns() - t0 > 5000000000ull) __trap();  // 5 s: far beyond any legitimate wait
   }
 }
 
-// generic-proxy writes to smem -> visible to the async proxy (UMMA / TMA reads)
+// generic-proxy writes to smem -> visible to the async proxy (wgmma / TMA reads)
 __device__ __forceinline__ void fence_proxy_async_smem() {
   asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
 }
@@ -94,92 +78,77 @@ __device__ __forceinline__ void tma_load_2d(void* dst, const CUtensorMap* m, uin
       : "memory");
 }
 
-// ---- TMEM ---------------------------------------------------------------------------------
-__device__ __forceinline__ void tmem_alloc(uint32_t* dst_smem, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(
-                   smem_u32(dst_smem)),
-               "r"(ncols)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols)
-               : "memory");
-}
-__device__ __forceinline__ void tcgen05_fence_before() {
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-}
-__device__ __forceinline__ void tcgen05_fence_after() {
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-}
-// MMA completion -> mbarrier (implies fence::before_thread_sync)
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::
-                   "r"(smem_u32(bar))
-               : "memory");
-}
-
-// 32 lanes x 32 consecutive fp32 columns -> 32 registers per thread (thread = lane = row)
-__device__ __forceinline__ void tmem_ld_32x32b_x32(uint32_t taddr, uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]),
-        "=r"(r[7]), "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]),
-        "=r"(r[14]), "=r"(r[15]), "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]),
-        "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]), "=r"(r[25]),
-        "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait() {
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-}
-
-// ---- UMMA descriptors ------------------------------------------------------------------------
+// ---- wgmma ----------------------------------------------------------------------------------
 // Shared-memory matrix descriptor (64 bit):
 //   [0,14)  start address >> 4        [16,30) leading-dim byte offset >> 4
-//   [32,46) stride-dim byte offset >> 4   [46,48) version = 1 (Blackwell)
-//   [49,52) base offset = 0           [61,64) layout: 0 none, 2 = SWIZZLE_128B
+//   [32,46) stride-dim byte offset >> 4   [49,52) base offset = 0   [62,64) 1 = SWIZZLE_128B
 // K-major, SWIZZLE_128B (rows of 128 B, 8-row 1024-B atoms, as written by TMA):
 //   SBO = 1024 (next 8 rows), LBO unused (encoded 1).
 // MN-major, SWIZZLE_128B (128-B rows hold 64 MN-contiguous elements of one K index):
 //   SBO = 1024 (next 8 K indices), LBO = byte distance between 64-element MN atoms.
-// 32-bit MN-major operands (tf32) are the exception: the only supported swizzled layout is
-// layout type 1 = SWIZZLE_128B_BASE32B (32-byte swizzle atoms, 4-row K groups -> SBO = 512),
-// written by TMA with CU_TENSOR_MAP_SWIZZLE_128B_ATOM_32B.
 __device__ __forceinline__ uint64_t make_smem_desc(uint32_t saddr, uint32_t lbo_bytes,
-                                                   uint32_t sbo_bytes, uint32_t layout = 2) {
+                                                   uint32_t sbo_bytes) {
   uint64_t d = 0;
   d |= static_cast<uint64_t>((saddr >> 4) & 0x3fffu);
   d |= static_cast<uint64_t>((lbo_bytes >> 4) & 0x3fffu) << 16;
   d |= static_cast<uint64_t>((sbo_bytes >> 4) & 0x3fffu) << 32;
-  d |= static_cast<uint64_t>(1) << 46;  // version
-  d |= static_cast<uint64_t>(layout) << 61;  // 2 = SWIZZLE_128B, 1 = SWIZZLE_128B_BASE32B
+  d |= static_cast<uint64_t>(1) << 62;  // SWIZZLE_128B
   return d;
 }
 
-// Instruction descriptor for kind::f16 (fp16/bf16 inputs, fp32 accumulate):
-//   [4,6) D format: 1 = f32      [7,10) A format: 0 = f16, 1 = bf16     [10,13) B format
-//   [15] A major: 0 = K, 1 = MN  [16] B major     [17,23) N >> 3        [24,29) M >> 4
-__host__ __device__ constexpr uint32_t make_idesc_f16(int bf16, int a_mn, int b_mn, int M, int N) {
-  return (1u << 4) | (static_cast<uint32_t>(bf16) << 7) | (static_cast<uint32_t>(bf16) << 10) |
-         (static_cast<uint32_t>(a_mn) << 15) | (static_cast<uint32_t>(b_mn) << 16) |
-         (static_cast<uint32_t>(N >> 3) << 17) | (static_cast<uint32_t>(M >> 4) << 24);
+__device__ __forceinline__ void wgmma_fence() {
+  asm volatile("wgmma.fence.sync.aligned;" ::: "memory");
+}
+__device__ __forceinline__ void wgmma_commit() {
+  asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory");
+}
+template <int N>
+__device__ __forceinline__ void wgmma_wait() {
+  asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory");
+}
+// Keeps the compiler from moving accumulator reads / writes across an in-flight wgmma.
+__device__ __forceinline__ void fence_acc(float (&d)[64]) {
+#pragma unroll
+  for (int i = 0; i < 64; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
 
-// D[tmem] (+)= A[smem] * B[smem], issued by ONE thread.
-__device__ __forceinline__ void umma_f16(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc,
-                                         uint32_t idesc, uint32_t accumulate) {
+// D[64 x 128] (+)= A[64 x 16] * B[128 x 16]^T, issued by one warpgroup; trans = operand MN-major.
+// Accumulator fragment of thread t (warp w = t / 32 of the group, lane l):
+//   d[4 j + 2 i + c] = D[16 w + l / 4 + 8 i][8 j + 2 (l % 4) + c],  j < 16, i, c < 2.
+template <int kTransA, int kTransB>
+__device__ __forceinline__ void wgmma_m64n128k16_bf16(float (&d)[64], uint64_t adesc, uint64_t bdesc,
+                                         uint32_t accumulate) {
   asm volatile(
       "{\n"
       ".reg .pred p;\n"
-      "setp.ne.b32 p, %4, 0;\n"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n"
-      "}\n" ::"r"(tmem_d),
-      "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
+      "setp.ne.b32 p, %66, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, "
+      "%64, %65, p, 1, 1, %67, %68;\n"
+      "}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+      : "l"(adesc), "l"(bdesc), "r"(accumulate), "n"(kTransA), "n"(kTransB));
+}
+template <int kTransA, int kTransB>
+__device__ __forceinline__ void wgmma_m64n128k16_f16(float (&d)[64], uint64_t adesc, uint64_t bdesc,
+                                         uint32_t accumulate) {
+  asm volatile(
+      "{\n"
+      ".reg .pred p;\n"
+      "setp.ne.b32 p, %66, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n128k16.f32.f16.f16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, "
+      "%64, %65, p, 1, 1, %67, %68;\n"
+      "}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+      : "l"(adesc), "l"(bdesc), "r"(accumulate), "n"(kTransA), "n"(kTransB));
+}
+
+template <bool kBf16, int kTransA, int kTransB>
+__device__ __forceinline__ void wgmma_m64n128k16(float (&d)[64], uint64_t adesc, uint64_t bdesc,
+                                                 uint32_t accumulate) {
+  if constexpr (kBf16) wgmma_m64n128k16_bf16<kTransA, kTransB>(d, adesc, bdesc, accumulate);
+  else wgmma_m64n128k16_f16<kTransA, kTransB>(d, adesc, bdesc, accumulate);
 }
 
 }  // namespace tc

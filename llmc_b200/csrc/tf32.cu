@@ -1,22 +1,25 @@
-// tf32.cu — fp32-accurate rank-K updates on tcgen05 tensor cores ("3xTF32").
+// tf32.cu — fp32-accurate rank-K updates on tensor cores ("3xTF32").
 //
 //   C[M,N]  <-  C - A * B      (mode 0)      or      C <- A * B      (mode 1)
 //
 // with fp32 A, B given as pre-split pairs (hi = tf32(x), lo = tf32(x - hi)) and the product
-// evaluated as  A_hi*B_hi + A_lo*B_hi + A_hi*B_lo  (three kind::tf32 MMAs accumulating into the
-// same fp32 TMEM tile; the dropped A_lo*B_lo term is ~2^-22 relative).  This is the workhorse for
+// evaluated as  A_hi*B_hi + A_lo*B_hi + A_hi*B_lo  (three tf32 MMAs accumulating into the same
+// fp32 accumulators; the dropped A_lo*B_lo term is ~2^-22 relative).  This is the workhorse for
 // every fp32 GEMM-shaped step of GPTQ that the reference runs as cuBLAS SGEMM / cuSOLVER:
 //   * W[:, i2:] -= Err1 @ Hinv[i1:i2, i2:]                        (gptq.py:244)
 //   * the trailing updates of the blocked Cholesky and of the triangular inverse that replace
 //     torch.linalg.cholesky / cholesky_inverse / cholesky(upper) (gptq.py:172-174).
-// K is small (128 per call), so these are HBM-bound read-modify-write sweeps over C; the three
-// MMAs per k-step are free under that roof.
+// K is small (128 per call), so these are read-modify-write sweeps over C.
 //
 // Operand layouts (per operand flag):
 //   K-major : element (i, k) at base[i*ld + k]   (rows = M or N index, K contiguous)
 //   MN-major: element (i, k) at base[k*ld + i]   (rows = K index, M or N contiguous)
-// Same warp-specialised structure as gemm.cu (TMA producer / MMA issuer / 4 epilogue warps,
-// double-buffered 2 x 256-column TMEM accumulators), tile 128 x 256, 32 k per stage, 2 stages.
+// The GPTQ weight update has BOTH operands MN-major, which Hopper's wgmma cannot read for tf32
+// (tf32 wgmma operands must be K-major), so the MMAs are warp-level mma.sync m16n8k8 whose
+// fragments are gathered from shared memory in either layout.
+// Structure: one TMA producer warp fills a 3-stage ring of 128B-swizzled tiles (mbarrier
+// transaction counts); eight MMA warps (2 x 4, 64 x 32 each) compute a 128 x 128 tile with fp32
+// register accumulators and write it back with the fused epilogue.
 #include "tc.cuh"
 
 namespace llmc {
@@ -25,16 +28,15 @@ using namespace tc;
 
 namespace t3 {
 
-constexpr int BM = 128, BN = 256, BK = 32;     // BK tf32 elements = 128 bytes
-constexpr int kStages = 2;
+constexpr int BM = 128, BN = 128, BK = 32;     // BK tf32 elements = 128 bytes
+constexpr int kStages = 3;
 constexpr int kABytes = BM * BK * 4;             // 16 KB (per hi / lo)
-constexpr int kBBytes = BN * BK * 4;             // 32 KB
-constexpr int kStageBytes = 2 * (kABytes + kBBytes);   // 96 KB
+constexpr int kBBytes = BN * BK * 4;             // 16 KB
+constexpr int kStageBytes = 2 * (kABytes + kBBytes);   // 64 KB
 constexpr int kBoxBytes = 32 * BK * 4;           // MN-major box: 32 MN x 32 K rows = 4 KB
 constexpr int kSmemBytes = kStages * kStageBytes + 1024 + 256;
-constexpr int kThreads = 192;
-constexpr int kTmemCols = 512;
-
+constexpr int kMmaWarps = 8;
+constexpr int kThreads = (kMmaWarps + 1) * 32;   // + the TMA warp
 struct Params {
   int64_t M, N;
   int K;
@@ -57,7 +59,7 @@ __device__ __forceinline__ void decode(const Params& p, int u, int& m_blk, int& 
     return;
   }
   // lower-triangle tiles of row-block mi: n_blk in [0, cnt(mi)) with
-  // cnt = number of 256-wide column tiles whose first column <= last row of the block
+  // cnt = number of BN-wide column tiles whose first column <= last row of the block
   int mi = 0;
   for (;; ++mi) {
     const int64_t last_row = p.row_off + static_cast<int64_t>(mi) * BM + BM - 1;
@@ -71,29 +73,32 @@ __device__ __forceinline__ void decode(const Params& p, int u, int& m_blk, int& 
   n_blk = u;
 }
 
-// Instruction descriptor kind::tf32: D f32 (1<<4), A/B format 2 = TF32.
-__host__ __device__ constexpr uint32_t idesc_tf32(int a_mn, int b_mn) {
-  return (1u << 4) | (2u << 7) | (2u << 10) | (static_cast<uint32_t>(a_mn) << 15) |
-         (static_cast<uint32_t>(b_mn) << 16) | (static_cast<uint32_t>(BN >> 3) << 17) |
-         (static_cast<uint32_t>(BM >> 4) << 24);
-}
-
-__device__ __forceinline__ void umma_tf32(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc,
-                                          uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n"
-      ".reg .pred p;\n"
-      "setp.ne.b32 p, %4, 0;\n"
-      "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n"
-      "}\n" ::"r"(tmem_d),
-      "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-
 __device__ __forceinline__ float to_tf32(float x) {
   uint32_t r;
   asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(r) : "f"(x));
   return __uint_as_float(r);
+}
+
+// byte offset of element (i, k) inside an operand tile as TMA wrote it (SWIZZLE_128B: 16-byte
+// chunk c of a 128-byte row r sits at chunk c ^ (r & 7))
+template <bool kMn>
+__device__ __forceinline__ uint32_t tile_off(int i, int k) {
+  if constexpr (!kMn)   // rows = i, 32 k per 128-byte row
+    return i * 128 + ((((k >> 2) ^ (i & 7)) << 4) | ((k & 3) << 2));
+  else                  // boxes of 32 i; rows = k
+    return (i >> 5) * kBoxBytes + k * 128 + (((((i & 31) >> 2) ^ (k & 7)) << 4) | ((i & 3) << 2));
+}
+
+__device__ __forceinline__ uint32_t lds_u32(const uint8_t* base, uint32_t off) {
+  return *reinterpret_cast<const uint32_t*>(base + off);
+}
+
+__device__ __forceinline__ void mma_tf32(float (&d)[4], const uint32_t (&a)[4], const uint32_t (&b)[2]) {
+  asm volatile(
+      "mma.sync.aligned.m16n8k8.row.col.f32.tf32.tf32.f32 {%0, %1, %2, %3}, {%4, %5, %6, %7}, "
+      "{%8, %9}, {%0, %1, %2, %3};"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b[0]), "r"(b[1]));
 }
 
 template <bool kAmn, bool kBmn>
@@ -106,25 +111,18 @@ tf32x3_kernel(const __grid_constant__ CUtensorMap tmAhi, const __grid_constant__
                                              ~static_cast<uintptr_t>(1023));
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + kStages * kStageBytes);
   uint64_t* empty_bar = full_bar + kStages;
-  uint64_t* tmem_full = empty_bar + kStages;
-  uint64_t* tmem_empty = tmem_full + 2;
-  uint32_t* tmem_ptr = reinterpret_cast<uint32_t*>(tmem_empty + 2);
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int kb_total = (p.K + BK - 1) / BK;
 
-  if (warp == 0 && lane == 0) {
+  if (threadIdx.x == 0) {
     prefetch_tmap(&tmAhi); prefetch_tmap(&tmAlo); prefetch_tmap(&tmBhi); prefetch_tmap(&tmBlo);
-    for (int s = 0; s < kStages; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], 1); }
-    for (int s = 0; s < 2; ++s) { mbar_init(&tmem_full[s], 1); mbar_init(&tmem_empty[s], 4); }
+    for (int s = 0; s < kStages; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], kMmaWarps); }
     fence_barrier_init();
   }
-  if (warp == 1) tmem_alloc(tmem_ptr, kTmemCols);
-  tcgen05_fence_before();
   __syncthreads();
-  tcgen05_fence_after();
-  const uint32_t tmem_base = *tmem_ptr;
 
-  if (warp == 0) {
+  if (warp == kMmaWarps) {
+    // ===================== TMA producer =====================
     if (lane == 0) {
       int stage = 0;
       uint32_t phase = 0;
@@ -162,127 +160,105 @@ tf32x3_kernel(const __grid_constant__ CUtensorMap tmAhi, const __grid_constant__
         }
       }
     }
-  } else if (warp == 1) {
-    constexpr uint32_t idesc = idesc_tf32(kAmn ? 1 : 0, kBmn ? 1 : 0);
-    int stage = 0;
-    uint32_t phase = 0;
-    int as = 0;
-    uint32_t aphase = 0;
-    for (int u = blockIdx.x; u < p.num_units; u += gridDim.x) {
-      mbar_wait(&tmem_empty[as], aphase ^ 1);
-      tcgen05_fence_after();
-      const uint32_t d_tmem = tmem_base + as * BN;
-      for (int kb = 0; kb < kb_total; ++kb) {
-        mbar_wait(&full_bar[stage], phase);
-        tcgen05_fence_after();
-        if (lane == 0) {
-          const uint32_t ahi = smem_u32(smem + stage * kStageBytes);
-          const uint32_t alo = ahi + kABytes;
-          const uint32_t bhi = alo + kABytes;
-          const uint32_t blo = bhi + kBBytes;
+    return;
+  }
+
+  // ===================== MMA warps: warp (wm, wn) owns rows 64 wm .. +63, cols 32 wn .. +31 =====
+  const int wm = warp >> 2, wn = warp & 3;
+  const int g = lane >> 2, t = lane & 3;
+  int stage = 0;
+  uint32_t phase = 0;
+  for (int u = blockIdx.x; u < p.num_units; u += gridDim.x) {
+    int m_blk, n_blk;
+    decode(p, u, m_blk, n_blk);
+    float acc[4][4][4];
 #pragma unroll
-          for (int k = 0; k < BK / 8; ++k) {
-            // K-major: 8 tf32 = 32 B along the swizzled 128-B row; MN-major: one 8-row atom
-            const uint32_t aoff = kAmn ? k * 1024 : k * 32;
-            const uint32_t boff = kBmn ? k * 1024 : k * 32;
-            const uint32_t albo = kAmn ? kBoxBytes : 16, blbo = kBmn ? kBoxBytes : 16;
-            // MN-major tf32: SWIZZLE_128B_BASE32B, K groups of 4 rows (512 B)
-            const uint32_t asbo = kAmn ? 512 : 1024, bsbo = kBmn ? 512 : 1024;
-            const uint32_t alay = kAmn ? 1 : 2, blay = kBmn ? 1 : 2;
-            const uint64_t dah = make_smem_desc(ahi + aoff, albo, asbo, alay);
-            const uint64_t dal = make_smem_desc(alo + aoff, albo, asbo, alay);
-            const uint64_t dbh = make_smem_desc(bhi + boff, blbo, bsbo, blay);
-            const uint64_t dbl = make_smem_desc(blo + boff, blbo, bsbo, blay);
-            umma_tf32(d_tmem, dah, dbh, idesc, (kb > 0 || k > 0) ? 1u : 0u);
-            umma_tf32(d_tmem, dal, dbh, idesc, 1u);
-            umma_tf32(d_tmem, dah, dbl, idesc, 1u);
-          }
-          umma_commit(&empty_bar[stage]);
-          if (kb == kb_total - 1) umma_commit(&tmem_full[as]);
-        }
-        __syncwarp();
-        if (++stage == kStages) { stage = 0; phase ^= 1; }
-      }
-      as ^= 1;
-      if (as == 0) aphase ^= 1;
-    }
-  } else {
-    const int q = warp & 3;
-    int as = 0;
-    uint32_t aphase = 0;
-    for (int u = blockIdx.x; u < p.num_units; u += gridDim.x) {
-      int m_blk, n_blk;
-      decode(p, u, m_blk, n_blk);
-      mbar_wait(&tmem_full[as], aphase);
-      tcgen05_fence_after();
-      const int64_t row = static_cast<int64_t>(m_blk) * BM + q * 32 + lane;
-      const uint32_t taddr0 = tmem_base + (static_cast<uint32_t>(q * 32) << 16) + as * BN;
+    for (int a = 0; a < 4; ++a)
+#pragma unroll
+      for (int b = 0; b < 4; ++b)
+#pragma unroll
+        for (int c = 0; c < 4; ++c) acc[a][b][c] = 0.f;
+    for (int kb = 0; kb < kb_total; ++kb) {
+      mbar_wait(&full_bar[stage], phase);
+      const uint8_t* ahi = smem + stage * kStageBytes;
+      const uint8_t* alo = ahi + kABytes;
+      const uint8_t* bhi = alo + kABytes;
+      const uint8_t* blo = bhi + kBBytes;
 #pragma unroll 1
-      for (int c = 0; c < BN; c += 32) {
-        uint32_t r[32];
-        tmem_ld_32x32b_x32(taddr0 + c, r);
-        tmem_ld_wait();
-        const int64_t col0 = static_cast<int64_t>(n_blk) * BN + c;
-        if (row < p.M && col0 < p.N) {
-          float* cp = p.C + row * p.ldc + col0;
-          const bool vec = (col0 + 32 <= p.N) && ((reinterpret_cast<uintptr_t>(cp) & 15) == 0);
-          float v[32];
+      for (int kk = 0; kk < BK; kk += 8) {
+        uint32_t fbh[4][2], fbl[4][2];
+#pragma unroll
+        for (int nt = 0; nt < 4; ++nt) {
+          const int j = wn * 32 + nt * 8 + g;
+          const uint32_t o0 = tile_off<kBmn>(j, kk + t), o1 = tile_off<kBmn>(j, kk + t + 4);
+          fbh[nt][0] = lds_u32(bhi, o0); fbh[nt][1] = lds_u32(bhi, o1);
+          fbl[nt][0] = lds_u32(blo, o0); fbl[nt][1] = lds_u32(blo, o1);
+        }
+#pragma unroll
+        for (int mt = 0; mt < 4; ++mt) {
+          const int i0 = wm * 64 + mt * 16 + g;
+          const uint32_t o0 = tile_off<kAmn>(i0, kk + t), o1 = tile_off<kAmn>(i0 + 8, kk + t);
+          const uint32_t o2 = tile_off<kAmn>(i0, kk + t + 4), o3 = tile_off<kAmn>(i0 + 8, kk + t + 4);
+          const uint32_t fah[4] = {lds_u32(ahi, o0), lds_u32(ahi, o1), lds_u32(ahi, o2), lds_u32(ahi, o3)};
+          const uint32_t fal[4] = {lds_u32(alo, o0), lds_u32(alo, o1), lds_u32(alo, o2), lds_u32(alo, o3)};
+#pragma unroll
+          for (int nt = 0; nt < 4; ++nt) {
+            mma_tf32(acc[mt][nt], fah, fbh[nt]);
+            mma_tf32(acc[mt][nt], fal, fbh[nt]);
+            mma_tf32(acc[mt][nt], fah, fbl[nt]);
+          }
+        }
+      }
+      __syncwarp();
+      if (lane == 0) mbar_arrive(&empty_bar[stage]);
+      if (++stage == kStages) { stage = 0; phase ^= 1; }
+    }
+
+    // ---- epilogue: fragment element (mt, nt, 2 i + c) = C[row g + 8 i][col 2 t + c] ----
+#pragma unroll
+    for (int mt = 0; mt < 4; ++mt) {
+#pragma unroll
+      for (int i = 0; i < 2; ++i) {
+        const int64_t row = static_cast<int64_t>(m_blk) * BM + wm * 64 + mt * 16 + g + 8 * i;
+        if (row >= p.M) continue;
+#pragma unroll
+        for (int nt = 0; nt < 4; ++nt) {
+          const int64_t col = static_cast<int64_t>(n_blk) * BN + wn * 32 + nt * 8 + 2 * t;
+          if (col >= p.N) continue;
+          const bool pair = col + 1 < p.N;
+          float* cp = p.C + row * p.ldc + col;
+          const bool vec = pair && (reinterpret_cast<uintptr_t>(cp) & 7) == 0;
+          float v0 = acc[mt][nt][2 * i], v1 = acc[mt][nt][2 * i + 1];
           if (p.mode == 0) {
             if (vec) {
-#pragma unroll
-              for (int i = 0; i < 32; i += 4) {
-                const float4 o = *reinterpret_cast<const float4*>(cp + i);
-                v[i] = o.x - __uint_as_float(r[i]);
-                v[i + 1] = o.y - __uint_as_float(r[i + 1]);
-                v[i + 2] = o.z - __uint_as_float(r[i + 2]);
-                v[i + 3] = o.w - __uint_as_float(r[i + 3]);
-              }
+              const float2 o = *reinterpret_cast<const float2*>(cp);
+              v0 = o.x - v0;
+              v1 = o.y - v1;
             } else {
-              for (int i = 0; i < 32; ++i)
-                v[i] = (col0 + i < p.N) ? cp[i] - __uint_as_float(r[i]) : 0.f;
+              v0 = cp[0] - v0;
+              if (pair) v1 = cp[1] - v1;
             }
-          } else {
-#pragma unroll
-            for (int i = 0; i < 32; ++i) v[i] = __uint_as_float(r[i]);
           }
-          if (vec) {
-#pragma unroll
-            for (int i = 0; i < 32; i += 4)
-              *reinterpret_cast<float4*>(cp + i) = make_float4(v[i], v[i + 1], v[i + 2], v[i + 3]);
-          } else {
-            for (int i = 0; i < 32 && col0 + i < p.N; ++i) cp[i] = v[i];
+          if (vec) *reinterpret_cast<float2*>(cp) = make_float2(v0, v1);
+          else {
+            cp[0] = v0;
+            if (pair) cp[1] = v1;
           }
-          if (p.Chi != nullptr && (row < p.split_rows || col0 < p.split_cols)) {
-            float* hp = p.Chi + row * p.ldc + col0;
-            float* lp = p.Clo + row * p.ldc + col0;
-            if (vec && ((reinterpret_cast<uintptr_t>(hp) | reinterpret_cast<uintptr_t>(lp)) & 15) == 0) {
-#pragma unroll
-              for (int i = 0; i < 32; i += 4) {
-                const float4 h = make_float4(to_tf32(v[i]), to_tf32(v[i + 1]), to_tf32(v[i + 2]), to_tf32(v[i + 3]));
-                *reinterpret_cast<float4*>(hp + i) = h;
-                *reinterpret_cast<float4*>(lp + i) = make_float4(to_tf32(v[i] - h.x), to_tf32(v[i + 1] - h.y),
-                                                                 to_tf32(v[i + 2] - h.z), to_tf32(v[i + 3] - h.w));
-              }
-            } else {
-              for (int i = 0; i < 32 && col0 + i < p.N; ++i) {
-                const float h = to_tf32(v[i]);
-                hp[i] = h;
-                lp[i] = to_tf32(v[i] - h);
-              }
+          if (p.Chi != nullptr && (row < p.split_rows || col < p.split_cols)) {
+            float* hp = p.Chi + row * p.ldc + col;
+            float* lp = p.Clo + row * p.ldc + col;
+            const float h0 = to_tf32(v0), h1 = to_tf32(v1);
+            hp[0] = h0;
+            lp[0] = to_tf32(v0 - h0);
+            if (pair) {
+              hp[1] = h1;
+              lp[1] = to_tf32(v1 - h1);
             }
           }
         }
       }
-      tcgen05_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&tmem_empty[as]);
-      as ^= 1;
-      if (as == 0) aphase ^= 1;
     }
   }
-  tcgen05_fence_before();
-  __syncthreads();
-  if (warp == 1) tmem_dealloc(tmem_base, kTmemCols);
 }
 
 __global__ void __launch_bounds__(256)
@@ -303,7 +279,7 @@ split_tf32_kernel(const float* __restrict__ x, int64_t rows, int64_t cols, int64
 
 // rows x cols fp32 matrix, row stride ld; 128-byte swizzle => box_cols must be 32.
 int encode_tmap_2d_f32(CUtensorMap* out, const void* base, uint64_t rows, uint64_t cols,
-                       uint64_t ld_elems, uint32_t box_rows, uint32_t box_cols, int atom32b);
+                       uint64_t ld_elems, uint32_t box_rows, uint32_t box_cols);
 
 // One 3xTF32 update.  a_mn / b_mn: operand is MN-major (element (i,k) at base[k*ld + i]).
 // split_rows / split_cols restrict where the tf32 split of the result (Chi/Clo) is written: rows
@@ -339,8 +315,8 @@ int tf32x3_update_ex(const float* Ahi, const float* Alo, int a_mn, int64_t lda, 
 
 // one_tile_per_cta != 0: grid = number of tiles, every CTA computes one tile and exits.  Bulk
 // updates launched on a LOW-priority stream this way give their SMs back at tile granularity
-// (~20 us), so the short kernels of a latency-bound chain on a high-priority stream (blocked
-// Cholesky look-ahead, chol.cu) never wait behind a persistent 148-CTA grid.
+// (one 128 x 128 tile), so the short kernels of a latency-bound chain on a high-priority stream (blocked
+// Cholesky look-ahead, chol.cu) never wait behind a persistent grid that fills every SM.
 int tf32x3_update_grid(const float* Ahi, const float* Alo, int a_mn, int64_t lda, const float* Bhi,
                        const float* Blo, int b_mn, int64_t ldb, float* C, int64_t ldc, int64_t M,
                        int64_t N, int K, int mode, int tri, int64_t row_off, int64_t col_off,
@@ -356,18 +332,18 @@ int tf32x3_update_grid(const float* Ahi, const float* Alo, int a_mn, int64_t lda
   CUtensorMap tah, tal, tbh, tbl;
   int rc;
   if (!a_mn) {
-    if ((rc = encode_tmap_2d_f32(&tah, Ahi, M, K, lda, BM, BK, 0))) return rc;
-    if ((rc = encode_tmap_2d_f32(&tal, Alo, M, K, lda, BM, BK, 0))) return rc;
+    if ((rc = encode_tmap_2d_f32(&tah, Ahi, M, K, lda, BM, BK))) return rc;
+    if ((rc = encode_tmap_2d_f32(&tal, Alo, M, K, lda, BM, BK))) return rc;
   } else {
-    if ((rc = encode_tmap_2d_f32(&tah, Ahi, K, M, lda, BK, 32, 1))) return rc;
-    if ((rc = encode_tmap_2d_f32(&tal, Alo, K, M, lda, BK, 32, 1))) return rc;
+    if ((rc = encode_tmap_2d_f32(&tah, Ahi, K, M, lda, BK, 32))) return rc;
+    if ((rc = encode_tmap_2d_f32(&tal, Alo, K, M, lda, BK, 32))) return rc;
   }
   if (!b_mn) {
-    if ((rc = encode_tmap_2d_f32(&tbh, Bhi, N, K, ldb, BN, BK, 0))) return rc;
-    if ((rc = encode_tmap_2d_f32(&tbl, Blo, N, K, ldb, BN, BK, 0))) return rc;
+    if ((rc = encode_tmap_2d_f32(&tbh, Bhi, N, K, ldb, BN, BK))) return rc;
+    if ((rc = encode_tmap_2d_f32(&tbl, Blo, N, K, ldb, BN, BK))) return rc;
   } else {
-    if ((rc = encode_tmap_2d_f32(&tbh, Bhi, K, N, ldb, BK, 32, 1))) return rc;
-    if ((rc = encode_tmap_2d_f32(&tbl, Blo, K, N, ldb, BK, 32, 1))) return rc;
+    if ((rc = encode_tmap_2d_f32(&tbh, Bhi, K, N, ldb, BK, 32))) return rc;
+    if ((rc = encode_tmap_2d_f32(&tbl, Blo, K, N, ldb, BK, 32))) return rc;
   }
   Params p{};
   p.M = M; p.N = N; p.K = K; p.C = C; p.ldc = ldc; p.Chi = Chi; p.Clo = Clo;

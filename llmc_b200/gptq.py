@@ -1,10 +1,10 @@
-"""GPTQ — mirror of llmc/compression/quantization/gptq.py (class GPTQ :21-478) on the B200
+"""GPTQ — mirror of llmc/compression/quantization/gptq.py (class GPTQ :21-478) on the CUDA
 kernels.  Same YAML knobs (`special: actorder, static_groups, percdamp, blocksize,
 true_sequential, chunk_num`), same hook / subset flow, same `buf_*` hand-off to
 FakeQuantLinear / the real-quant packers.
 
 What differs from the reference is only HOW the numbers are produced:
-  * add_batch        -> one tcgen05 SYRK per hooked batch (gptq_ops.hessian_add_batch); the
+  * add_batch        -> one wgmma SYRK per hooked batch (gptq_ops.hessian_add_batch); the
                         per-batch all_reduce of H (gptq.py:292-295) becomes ONE all_reduce per
                         layer before it is used (same mean, linear in H);
   * layer_transform  -> prepare gather kernel, Cholesky triple, one fused column-block sweep
@@ -145,7 +145,7 @@ class GPTQ(BaseBlockwiseQuantization):
         else:
             self._init_layers(linears, subsets)
 
-    # ---- B200-first block execution: ONE progressive pass instead of five forwards ------------------
+    # ---- GPU-first block execution: ONE progressive pass instead of five forwards ------------------
     def progressive_ok(self, block):
         """The staged whole-batch pass reproduces the reference's schedule in two cases:
           true_sequential + quant_out       : every linear sees the output of the already-quantised

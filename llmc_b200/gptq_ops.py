@@ -1,4 +1,4 @@
-"""GPTQ layer math on the B200 kernels — the tensor-level pieces of
+"""GPTQ layer math on the CUDA kernels — the tensor-level pieces of
 llmc/compression/quantization/gptq.py (add_batch :253-295, process_hessian_and_weights
 :128-176, weight_transform :198-244) behind small functions; llmc_b200/gptq.py wires them into
 the reference's class / hook structure.
@@ -32,7 +32,7 @@ def free_workspaces():
 def hessian_add_batch(H, nsamples, inp):
     """gptq.py:253-290 for nn.Linear inputs.  H [C,C] fp32 updated in place:
     H <- H*n/(n+b) + 2/(n+b) * X^T X with X = inp.reshape(-1, C); returns the new nsamples.
-    One tcgen05 SYRK launch (csrc/gemm.cu) instead of an fp32 SGEMM on X.float()."""
+    One wgmma SYRK launch (csrc/gemm.cu) instead of an fp32 SGEMM on X.float()."""
     require_cuda(H, inp)
     if inp.dim() == 2:
         inp = inp.unsqueeze(0)
@@ -81,7 +81,7 @@ def chol_inv_upper(Hp, backend='b200', inplace=False, return_info=False):
     """gptq.py:172-174: U = cholesky(cholesky_inverse(cholesky(Hp)), upper=True).
 
     backend 'b200' (default): csrc/chol.cu — one reverse-ordered blocked factorisation + one
-    blocked triangular inverse, all O(C^3) work as 3xTF32 rank-128 updates on tcgen05.
+    blocked triangular inverse, all O(C^3) work as 3xTF32 rank-128 updates on tensor cores.
     backend 'cusolver': the reference's three library calls, kept only so tests can compare the
     two (never used by the algorithms).
     return_info: also return the device int32[1] status flag (0 = positive-definite, k = the

@@ -16,7 +16,7 @@ from .prof import TIMER
 
 
 def linear_forward(x, weight, bias=None):
-    """F.linear on the tcgen05 GEMM (csrc/gemm.cu) — y = x @ weight.T (+ bias)."""
+    """F.linear on the wgmma GEMM (csrc/gemm.cu) — y = x @ weight.T (+ bias)."""
     require_cuda(x, weight)
     if x.dtype != weight.dtype:
         raise TypeError(f'activation dtype {x.dtype} != weight dtype {weight.dtype}')
@@ -121,7 +121,7 @@ class OriginFloatLinear(nn.Module):
 class LlmcFp8Linear(nn.Module):
     """module_utils.py:130-191 — holder of a 128x128 block-FP8 checkpoint weight (`weight` fp8 +
     `weight_scale_inv` fp32 [ceil(out/bs), ceil(in/bs)]).  Forward = the reference's non-Triton branch
-    (:171-178): dequantise ONCE to bf16 (llmc_fp8_block_dequant) and run the tcgen05 GEMM."""
+    (:171-178): dequantise ONCE to bf16 (llmc_fp8_block_dequant) and run the wgmma GEMM."""
 
     def __init__(self, in_features, out_features, bias, block_size):
         super().__init__()
@@ -230,9 +230,9 @@ def pack_unsigned_codes(codes, bits, signed):
 class EffcientFakeQuantLinear(nn.Module):
     """module_utils.py:681-759 — eval-time wrapper: w_qdq applied once in `new`.
 
-    B200 extension (K6): when the weight quantizer is a plain INT4 / INT8 group or channel
+    Extension (K6): when the weight quantizer is a plain INT4 / INT8 group or channel
     quantizer, `new` keeps the PACKED codes + group qparams instead of the dequantised weight and
-    the forward runs the fused dequant -> tcgen05 GEMM (csrc/gemm_w4.cu) — bit-identical to F.linear
+    the forward runs the fused dequant -> wgmma GEMM (csrc/gemm_w4.cu) — bit-identical to F.linear
     on the materialised weight (tests/test_gpu_gemm_w4.py), at 4.25 / 8.25 instead of 16 bits per
     weight in HBM.  `.weight` then dequantises on demand.  LLMC_B200_FUSED_DEQUANT=0 disables it."""
 

@@ -23,8 +23,8 @@ class KernelTimer:
             yield
             return
         # Event.record() without a stream resolves "the current device" through
-        # torch.cuda.is_available() -> cudaGetDeviceCount on every call (≈1 ms of host time each on
-        # this image); an explicit stream object avoids that.
+        # torch.cuda.is_available() -> cudaGetDeviceCount on every call (host time on every
+        # record); an explicit stream object avoids that.
         st = torch.cuda.current_stream(torch.cuda.current_device())
         s = torch.cuda.Event(enable_timing=True)
         e = torch.cuda.Event(enable_timing=True)

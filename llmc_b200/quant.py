@@ -3,7 +3,7 @@
 Same constructor kwargs, method names, argument meaning, return shapes/dtypes and error
 behaviour as the reference's `BaseQuantizer` / `IntegerQuantizer` (quant.py:46-960) and
 `FloatQuantizer` (:963-1229), so `quant.weight` / `quant.act` YAML dicts construct them
-unchanged (base_blockwise_quantization.py:150-179).  The arithmetic runs in the sm_100a
+unchanged (base_blockwise_quantization.py:150-179).  The arithmetic runs in the sm_90a
 kernels of libllmc_b200.so (csrc/quant.cu) through the C ABI; tensors must live on a CUDA
 device — there is no CPU path here (the CPU restatement is oracle/, test-only).
 """
@@ -44,7 +44,7 @@ class BaseQuantizer(object):
         if kwargs.get('ste', False) or kwargs.get('ste_all', False):
             raise NotImplementedError(
                 'straight-through rounding is a training-time feature (quant.py:63-71); the '
-                'B200 kernels implement inference-time round-half-even only')
+                'the CUDA kernels implement inference-time round-half-even only')
         self.round_func = torch.round
         self.ste_all = False
         self.round_zp = kwargs.get('round_zp', True)
@@ -440,7 +440,7 @@ class IntegerQuantizer(BaseQuantizer):
             zeros = torch.tensor(0.0)
         # qmax / qmin stay 0-dim HOST tensors (the reference moves them to the device): they are
         # kernel arguments here, and a pageable H2D copy of a scalar is a synchronous cudaMemcpy
-        # that makes the host lose its lead over the GPU (0.5 ms of idle GPU per call, measured)
+        # that makes the host lose its lead over the GPU (the GPU idles for every such call)
         return reshaped, scales, zeros, self.qmax, self.qmin
 
     def quant(self, tensor, scales, zeros, qmax, qmin):
@@ -528,7 +528,7 @@ class IntegerQuantizer(BaseQuantizer):
         return q_weight.T if transpose else q_weight
 
     def fake_quant_weight_static(self, weight, args):
-        """quant.py:785-831; `args['gmap']` (int32 [C]) is the B200 extension that fuses
+        """quant.py:785-831; `args['gmap']` (int32 [C]) is an extension of this library that fuses
         GPTQ's act-order gather (gptq.py:427-450) into the same pass."""
         if 'int_indices' in args or 'rounding' in args:
             raise NotImplementedError('int_indices / TesseraQ rounding (quant.py:786-799)')
@@ -642,7 +642,7 @@ class IntegerQuantizer(BaseQuantizer):
         return self._finish_real(t, scales, zeros, osf)
 
     def real_quant_pack_vllm_dynamic(self, weight):
-        """B200 fast path for VllmRealQuantLinear.quant_pack (module_utils.py:821-862):
+        """Fast path for VllmRealQuantLinear.quant_pack (module_utils.py:821-862):
         quantise + pack in ONE pass (the reference round-trips int32 codes through numpy)."""
         assert self.granularity in ('per_group', 'per_channel') and self.bit in (4, 8)
         src = weight.contiguous()

@@ -27,7 +27,7 @@ class FloatQuantizer(BaseQuantizer):
         self.use_qtorch = self.kwargs.get('use_qtorch')
         if not self.use_qtorch:
             raise NotImplementedError('FloatQuantizer without use_qtorch (quant.py:1005-1027 log2 '
-                                      'emulation) has no B200 kernel; every shipped fp8 YAML sets it')
+                                      'emulation) has no CUDA kernel here; every shipped fp8 YAML sets it')
         if self.bit not in _FP8:
             raise NotImplementedError(f'{self.bit}: only e4m3 / e5m2 have hardware conversions '
                                       '(e2m1/e3m2/e4m7 of quant.py:982-988 are not built)')

@@ -7,7 +7,7 @@ a threshold unquantised (an unstructured outlier mask).
 Same YAML knobs (`special: actorder, percdamp, blocksize, true_sequential, relative_threshold,
 simplified_outliers, scale: {...}, zero: {...}`), same `buf_*` hand-off to FakeQuantLinear.
 What runs where:
-  * Hessians              -> the tcgen05 SYRK of GPTQ (spqr.py:270-299 is gptq.py:253-295);
+  * Hessians              -> the wgmma SYRK of GPTQ (spqr.py:270-299 is gptq.py:253-295);
   * Cholesky triple       -> llmc_chol_inv_upper;
   * weight_transform      -> llmc_spqr_colblock (csrc/gptq.cu: one thread per weight row through
                              csrc/spqr_row.cuh, super-panel trailing updates on 3xTF32 tensor cores);

@@ -39,7 +39,7 @@ SHAPES = {
 
 
 class B200Linear(nn.Linear):
-    """nn.Linear whose forward is the tcgen05 GEMM (csrc/gemm.cu) on CUDA tensors."""
+    """nn.Linear whose forward is the wgmma GEMM (csrc/gemm.cu) on CUDA tensors."""
 
     def forward(self, x):
         if x.is_cuda:

@@ -6,7 +6,7 @@ oracle/ref_harness.py).  Build container only (needs /root/reference):
     python oracle/gen_e2e_golden.py
 
 The fixtures hold the initial weights, token ids and the reference's results, so the `-m gpu`
-tests (tests/test_gpu_e2e.py) can run the B200 pipeline on the same inputs.
+tests (tests/test_gpu_e2e.py) can run the GPU pipeline on the same inputs.
 """
 import os
 import sys

@@ -1,12 +1,12 @@
 """Block-parallel GPTQ calibration benchmark — BASELINE.json north_star's multi-GPU split and
-configs[3] ("GPTQ W4A16 on Llama-3-70B-shaped weights, layer-parallel across 8xB200 with NCCL
+configs[3] ("GPTQ W4A16 on Llama-3-70B-shaped weights, layer-parallel across 8 GPUs with NCCL
 activation broadcast").
 
     python -m torch.distributed.run --nproc-per-node N scripts/bench_block_parallel.py \
         --model llama-3-70b --layers 16 --samples 128 --seq-len 2048
 
 Runs llmc_b200.block_parallel.BlockParallelRunner over `--layers` decoder blocks of the shape model
-(every block has the same cost; a prefix keeps weights + activations inside one B200's HBM and the
+(every block has the same cost; a prefix keeps weights + activations inside one GPU's HBM and the
 run inside the GPU budget) with the GPTQ YAML of configs/gptq_w_only.yml except `quant_out: False`,
 `true_sequential: False` — the setting in which blocks are independent given their fp inputs
 (SURVEY.md 8(e)).  Timing: barrier + synchronize around the whole run, CUDA events, max over

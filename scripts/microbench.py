@@ -1,4 +1,4 @@
-"""Kernel-level timings on one B200 (CUDA events, warm-up, inputs larger than L2 or L2 flushed).
+"""Kernel-level timings on one GPU (CUDA events, warm-up, inputs larger than L2 or L2 flushed).
 Writes gpurun_out/microbench.json.  Not the headline bench (bench.py); used to steer tuning."""
 import json
 import os
@@ -194,10 +194,10 @@ if 'prof' in only:
     x = torch.randn(32768, 4096, device='cuda').bfloat16()
     w = (torch.randn(4096, 4096, device='cuda') * 0.02).bfloat16()
     for _ in range(3):
-        linear_forward(x, w)                                   # umma_gemm_kernel<false,true>
+        linear_forward(x, w)                                   # wgmma_gemm_kernel<false,true>
     H = torch.zeros(4096, 4096, device='cuda')
     for _ in range(3):
-        ops.hessian_add_batch(H, 1, x.unsqueeze(0))            # umma_gemm_kernel<true,true> + finalize
+        ops.hessian_add_batch(H, 1, x.unsqueeze(0))            # wgmma_gemm_kernel<true,true> + finalize
     wq = (torch.randn(14336, 4096, device='cuda') * 0.02).bfloat16()
     q = IntegerQuantizer(4, False, 'per_group', group_size=128)
     for _ in range(3):

@@ -20,8 +20,7 @@ def _load(golden_dir):
     return torch.load(os.path.join(golden_dir, 'awq_kat.pt'), weights_only=False)
 
 
-# Loss-curve bar = SURVEY 8(c)'s 1e-3 relative.  Measured on the B200 (round 2, PARITY.md):
-# 2.1e-5 (fp16 v2), 6.2e-5 (bf16 v1), 2.6e-4 (bf16 v2 W8 per-channel); identical arg-min in all.
+# Loss-curve bar = SURVEY 8(c)'s 1e-3 relative.
 BAR = {0: 1e-3, 1: 1e-3, 2: 1e-3}
 
 

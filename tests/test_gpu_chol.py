@@ -90,7 +90,7 @@ def test_chol_reports_non_spd():
 
 
 def test_gptq_raises_on_non_spd_hessian():
-    """ADVICE r1: the reference raises from torch.linalg.cholesky (gptq.py:172); the B200 path must
+    """ADVICE r1: the reference raises from torch.linalg.cholesky (gptq.py:172); the GPU path must
     not sweep NaNs into layer.weight silently."""
     import pytest as _pt
     from llmc_b200.blockwise import AttrDict

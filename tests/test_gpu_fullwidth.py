@@ -49,7 +49,7 @@ def test_fullwidth_hessian_cholesky_sweep(golden_dir):
     c = _setup(golden_dir)
     k, W, X = c['k'], c['W'], c['X']
     C = k['C']
-    # G2: 8 add_batch calls of [1, 2048, 14336] (gptq.py:253-290) on the tcgen05 SYRK
+    # G2: 8 add_batch calls of [1, 2048, 14336] (gptq.py:253-290) on the wgmma SYRK
     H = torch.zeros(C, C, device='cuda')
     n = 0
     for b in range(k['NB']):

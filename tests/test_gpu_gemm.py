@@ -1,4 +1,4 @@
-"""GPU parity for the tcgen05 kernels: GEMM (fake-quant forward) and SYRK (GPTQ Hessian).
+"""GPU parity for the wgmma kernels: GEMM (fake-quant forward) and SYRK (GPTQ Hessian).
 Floating point: compared with an fp32/fp64 torch reference of the same op; tolerance stated
 per test (north_star: 1e-3 relative on the Hessian)."""
 import pytest

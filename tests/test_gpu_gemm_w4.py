@@ -1,4 +1,4 @@
-"""GPU: the fused dequant->GEMM (packed INT4 weights) must equal the tcgen05 GEMM on the
+"""GPU: the fused dequant->GEMM (packed INT4 weights) must equal the wgmma GEMM on the
 materialised fake-quant weight BIT FOR BIT (same tiles, same K order, identical operand bits),
 for RTN-style (model dtype) and GPTQ-style (fp32) scales, sym and asym."""
 import pytest
@@ -65,7 +65,7 @@ def test_fused_with_fp32_gptq_scales_and_bias():
 @pytest.mark.parametrize('M,N,K', [(128, 256, 128), (300, 520, 512), (2048, 4096, 4096)])
 def test_w8a16_fused_equals_materialised(dtype, sym, gran, g, M, N, K, native):
     """llmc_gemm_w8a16 (INT8 weights, W8A16 — rtn_w8a16.yml / per-channel W8): bit for bit the
-    tcgen05 GEMM on the materialised fake-quant weight."""
+    wgmma GEMM on the materialised fake-quant weight."""
     from llmc_b200.module_utils import linear_forward, linear_forward_w4, pack_unsigned_codes
     from llmc_b200.quant import IntegerQuantizer
     torch.manual_seed(M + N + K + int(sym))

@@ -1,4 +1,4 @@
-"""GPU parity: the sm_100a quantize / pack kernels (through the C ABI, via the reference-shaped
+"""GPU parity: the sm_90a quantize / pack kernels (through the C ABI, via the reference-shaped
 Python classes) against the oracle and the reference-generated golden fixtures.
 Bar: bit-exact for codes, packed words, zeros; scales bit-exact too (tolerance 0)."""
 import os

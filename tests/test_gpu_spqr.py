@@ -4,7 +4,7 @@ and against the CPU oracle.
 
 Bars: a 128-column problem involves no GEMM between blocks -> tmp / mask / scales / zeros bit-exact;
 multi-block layers see the 3xTF32 trailing update instead of the reference's fp32 GEMM -> 1e-4 on tmp,
->= 99.5 % equal mask bits; from (W, H) through the B200 Hessian-free path (the golden H) and
+>= 99.5 % equal mask bits; from (W, H) through the GPU Hessian-free path (the golden H) and
 llmc_chol_inv_upper -> 1e-3 on the loss."""
 import math
 import os

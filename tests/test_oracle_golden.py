@@ -185,14 +185,33 @@ def test_awq_search_and_clip(golden_dir):
         assert _eq(ao.apply_clip(c['w'], c['best_max'], c['clip_sym'], c['best_min']), c['clipped'])
 
 
+# relative L2 distance of the oracle's block-0 output from the reference's: 0 (bit-identical) at 4
+# and 8 CPU threads, 1.5e-2 at 1 thread (another MKL blocking flips group roundings); a wrong block
+# forward or quant_out pass is off by O(1)
+BLOCK0_OUT_REL = 5e-2
+# Block 1's o / gate / up / down see inputs the oracle computes itself through block 1's quantised
+# prefix with the host's bf16 CPU kernels.  Measured worst deviation: 9.2e-4 on an 8-core host
+# (1 - 16 threads), 2.5e-3 (down_proj) on a 16-core host; the reference itself moves block 0's
+# down_proj by 8.8e-4 between those two hosts.  Twice the worst measured value:
+BLOCK1_LATER_REL = 5e-3
+
+
 def test_block_oracle_reproduces_reference_pipeline(golden_dir):
     """oracle/block_oracle.py (the five-forward GPTQ schedule of one decoder block, also the CPU
-    arm of bench.py) against the reference's own end-to-end run on the tiny Llama
-    (tests/golden/e2e_gptq_llama.pt): per-layer Losses.sum() of BOTH blocks — block 1 only matches
-    if block 0's quantised output (the quant_out pass) is right."""
+    arm of bench.py) against the reference's own end-to-end run on the tiny Llama: per-layer
+    Losses.sum() of BOTH blocks, at 2e-3 wherever the layer's input is the reference's own.  Block 0 starts from the embeddings
+    (tests/golden/e2e_gptq_llama.pt).  Block 1 starts from the input the reference itself gave it
+    (tests/golden/e2e_gptq_block1.npz, oracle/gen_block1_golden.py): that input is block 0's bf16
+    output computed by CPU kernels whose roundings depend on the CPU and its thread count, and GPTQ
+    amplifies such roundings.  The oracle's own block-0 output must still agree with it."""
+    import numpy as np
     from oracle import block_oracle as bo
     d = _load(golden_dir, 'e2e_gptq_llama.pt')
     sd = _load(golden_dir, d['init'])['sd0']
+    b1 = np.load(os.path.join(golden_dir, 'e2e_gptq_block1.npz'))
+    x1 = torch.from_numpy(b1['x1'].view(np.int16)).view(torch.bfloat16)
+    ref_losses = [{k: v for k, v in d['losses'].items() if k.startswith('0.')},
+                  dict(zip(b1['loss_names'].tolist(), b1['losses'].tolist()))]
     x = [torch.nn.functional.embedding(d['calib_ids'][i:i + 1], sd['model.embed_tokens.weight'])
          for i in range(d['calib_ids'].shape[0])]
     for blk in range(2):
@@ -200,11 +219,17 @@ def test_block_oracle_reproduces_reference_pipeline(golden_dir):
              for n in bo.LINEARS}
         W['ln1'] = sd[f'model.layers.{blk}.input_layernorm.weight']
         W['ln2'] = sd[f'model.layers.{blk}.post_attention_layernorm.weight']
+        if blk == 1:
+            out0 = torch.cat(x, dim=0).float()
+            rel = ((out0 - x1.float()).norm() / x1.float().norm()).item()
+            assert rel < BLOCK0_OUT_REL, rel
+            x = list(torch.split(x1, 1, dim=0))
         x, _, info = bo.gptq_block(W, x, heads=4, kv_heads=2)
         for n in bo.LINEARS:
             mod = 'self_attn' if n in ('q_proj', 'k_proj', 'v_proj', 'o_proj') else 'mlp'
-            ref = d['losses'][f'{blk}.{mod}.{n}']
-            assert info[n]['loss'] == pytest.approx(ref, rel=2e-3), (blk, n, info[n]['loss'], ref)
+            ref = ref_losses[blk][f'{blk}.{mod}.{n}']
+            rel = 2e-3 if blk == 0 or n in ('q_proj', 'k_proj', 'v_proj') else BLOCK1_LATER_REL
+            assert info[n]['loss'] == pytest.approx(ref, rel=rel), (blk, n, info[n]['loss'], ref)
 
 
 def test_range_oracle_matches_reference(golden_dir):
