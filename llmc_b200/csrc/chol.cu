@@ -13,24 +13,6 @@
 #include "tc.cuh"
 
 namespace llmc {
-
-int tf32x3_update(const float* Ahi, const float* Alo, int a_mn, int64_t lda, const float* Bhi,
-                  const float* Blo, int b_mn, int64_t ldb, float* C, int64_t ldc, int64_t M,
-                  int64_t N, int K, int mode, int tri, int64_t row_off, int64_t col_off,
-                  float* Chi, float* Clo, cudaStream_t st);
-int tf32x3_update_ex(const float* Ahi, const float* Alo, int a_mn, int64_t lda, const float* Bhi,
-                     const float* Blo, int b_mn, int64_t ldb, float* C, int64_t ldc, int64_t M,
-                     int64_t N, int K, int mode, int tri, int64_t row_off, int64_t col_off,
-                     float* Chi, float* Clo, int64_t split_rows, int64_t split_cols,
-                     cudaStream_t st);
-int tf32x3_update_grid(const float* Ahi, const float* Alo, int a_mn, int64_t lda, const float* Bhi,
-                       const float* Blo, int b_mn, int64_t ldb, float* C, int64_t ldc, int64_t M,
-                       int64_t N, int K, int mode, int tri, int64_t row_off, int64_t col_off,
-                       float* Chi, float* Clo, int64_t split_rows, int64_t split_cols,
-                       int one_tile_per_cta, cudaStream_t st);
-int split_tf32(const float* x, int64_t rows, int64_t cols, int64_t ld, float* hi, float* lo,
-               int64_t ld_out, cudaStream_t st);
-
 namespace ch {
 
 constexpr int NB = 128;
@@ -63,98 +45,17 @@ reverse_upper_kernel(const float* __restrict__ Y, float* __restrict__ U, int64_t
   }
 }
 
-// One CTA: factor the nb x nb diagonal block at G[k0][k0] (lower), invert the factor.
-//   G block <- L_kk (lower part), D <- L_kk^-1 (nb x nb, row-major, ld NB, zero above the diagonal
-//   and zero padded to 128), Dhi/Dlo its tf32 split.  info[0] = k0 + j + 1 on a non-positive pivot.
-__global__ void __launch_bounds__(256, 1)
-diag_kernel(float* __restrict__ G, int64_t n, int64_t k0, int nb, float* __restrict__ D,
-            float* __restrict__ Dhi, float* __restrict__ Dlo, int* __restrict__ info) {
-  extern __shared__ float sm[];
-  float* S = sm;                 // [NB][LDS] the block / L
-  float* X = sm + NB * LDS;      // [NB][LDS] L^-1
-  const int tid = threadIdx.x;
-  for (int idx = tid; idx < NB * NB; idx += 256) {
-    const int i = idx >> 7, j = idx & 127;
-    float v = 0.f;
-    if (i < nb && j < nb && j <= i) v = G[(k0 + i) * n + k0 + j];
-    S[i * LDS + j] = v;
-    X[i * LDS + j] = 0.f;
-  }
-  __syncthreads();
-  // Left-looking column Cholesky: thread i owns row i (conflict-free padded rows, row j is a
-  // broadcast read).  L[i][j] = (A[i][j] - sum_{k<j} L[i][k] L[j][k]) / L[j][j].
-  {
-    const int i = tid;
-    for (int j = 0; j < nb; ++j) {
-      float v = 0.f;
-      if (i >= j && i < nb) {
-        float a0 = 0.f, a1 = 0.f, a2 = 0.f, a3 = 0.f;
-        const float* ri = S + i * LDS;
-        const float* rj = S + j * LDS;
-        int k = 0;
-        for (; k + 3 < j; k += 4) {
-          a0 = fmaf(ri[k], rj[k], a0);
-          a1 = fmaf(ri[k + 1], rj[k + 1], a1);
-          a2 = fmaf(ri[k + 2], rj[k + 2], a2);
-          a3 = fmaf(ri[k + 3], rj[k + 3], a3);
-        }
-        for (; k < j; ++k) a0 = fmaf(ri[k], rj[k], a0);
-        v = ri[j] - ((a0 + a1) + (a2 + a3));
-      }
-      // (column j is only written below; the dot products above read columns < j, final already)
-      if (i == j) {
-        if (!(v > 0.f) && info[0] == 0) info[0] = static_cast<int>(k0) + j + 1;
-        S[j * LDS + j] = sqrtf(fmaxf(v, 1e-30f));
-      }
-      __syncthreads();
-      if (i > j && i < nb) S[i * LDS + j] = v / S[j * LDS + j];
-      // row j+1's column j is written by thread j+1 and read by all in the next iteration
-      __syncthreads();
-    }
-  }
-  // X = L^-1: thread c owns column c (unit-stride across threads), forward substitution with
-  // four partial sums per entry to break the FMA dependency chain
-  if (tid < nb) {
-    const int c = tid;
-    X[c * LDS + c] = 1.0f / S[c * LDS + c];
-    for (int i = c + 1; i < nb; ++i) {
-      float a0 = 0.f, a1 = 0.f, a2 = 0.f, a3 = 0.f;
-      const float* ri = S + i * LDS;
-      int k = c;
-      for (; k + 3 < i; k += 4) {
-        a0 = fmaf(ri[k], X[k * LDS + c], a0);
-        a1 = fmaf(ri[k + 1], X[(k + 1) * LDS + c], a1);
-        a2 = fmaf(ri[k + 2], X[(k + 2) * LDS + c], a2);
-        a3 = fmaf(ri[k + 3], X[(k + 3) * LDS + c], a3);
-      }
-      for (; k < i; ++k) a0 = fmaf(ri[k], X[k * LDS + c], a0);
-      X[i * LDS + c] = -((a0 + a1) + (a2 + a3)) / ri[i];
-    }
-  }
-  __syncthreads();
-  for (int idx = tid; idx < NB * NB; idx += 256) {
-    const int i = idx >> 7, j = idx & 127;
-    if (i < nb && j < nb && j <= i) G[(k0 + i) * n + k0 + j] = S[i * LDS + j];
-    const float x = X[i * LDS + j];
-    D[idx] = x;
-    const float h = tf32r(x);
-    Dhi[idx] = h;
-    Dlo[idx] = tf32r(x - h);
-  }
-}
-
-// ---- diag_kernel_v2: the same contract as diag_kernel, blocked by 32 ------------------------------
-// The v1 kernel above is one long sequential sweep whose shared-memory traffic (two LDS per FMA,
-// 2-way conflicts in the inverse) made it the slowest link of the factorisation chain.  v2 factors
-// 32x32 diagonal sub-blocks in registers (warp shuffles), solves the sub-panel with one thread per
-// row in registers, applies the trailing update with 4x4 register tiles, and builds L^-1 from 32x32
-// block products (X_ij = -X_ii * sum_k L_ik X_kj).  Rows/cols >= nb are padded with the identity so
-// every loop runs at the full 128.
+// One CTA: factor the nb x nb diagonal block at G[k0][k0] (lower) and invert the factor, blocked by
+// 32: 32x32 diagonal sub-blocks are factored in registers (warp shuffles), the sub-panel is solved
+// with one thread per row in registers, the trailing update uses 4x4 register tiles, and L^-1 is
+// built from 32x32 block products (X_ij = -X_ii * sum_k L_ik X_kj).  Rows/cols >= nb are padded
+// with the identity so every loop runs at the full 128.  G block <- L_kk; Y / Yhi / Ylo block <-
+// L_kk^-1 and its tf32 split (ld n).  info[0] = k0 + j + 1 on a non-positive pivot.
 constexpr int SBK = 32;
 
 __global__ void __launch_bounds__(256, 1)
-diag_kernel_v2(float* __restrict__ G, int64_t n, int64_t k0, int nb, float* __restrict__ Y,
-               float* __restrict__ Yhi, float* __restrict__ Ylo, int* __restrict__ info) {
+diag_kernel(float* __restrict__ G, int64_t n, int64_t k0, int nb, float* __restrict__ Y,
+            float* __restrict__ Yhi, float* __restrict__ Ylo, int* __restrict__ info) {
   extern __shared__ float sm[];
   float* S = sm;                 // [NB][LDS]
   float* X = sm + NB * LDS;      // [NB][LDS]
@@ -359,20 +260,6 @@ diag_kernel_v2(float* __restrict__ G, int64_t n, int64_t k0, int nb, float* __re
   }
 }
 
-// copy the nb x nb block D (ld NB) into Y / Yhi / Ylo at (k0, k0)
-__global__ void __launch_bounds__(256)
-place_diag_kernel(const float* __restrict__ D, const float* __restrict__ Dhi,
-                  const float* __restrict__ Dlo, float* __restrict__ Y, float* __restrict__ Yhi,
-                  float* __restrict__ Ylo, int64_t n, int64_t k0, int nb) {
-  for (int idx = threadIdx.x + blockIdx.x * blockDim.x; idx < nb * nb; idx += blockDim.x * gridDim.x) {
-    const int i = idx / nb, j = idx - i * nb;
-    const int64_t o = (k0 + i) * n + k0 + j;
-    Y[o] = D[i * NB + j];
-    Yhi[o] = Dhi[i * NB + j];
-    Ylo[o] = Dlo[i * NB + j];
-  }
-}
-
 }  // namespace ch
 }  // namespace llmc
 
@@ -380,9 +267,8 @@ using namespace llmc;
 
 extern "C" int64_t llmc_chol_workspace_bytes(int64_t C) {
   if (C <= 0) return 0;
-  const int64_t nbk = (C + ch::NB - 1) / ch::NB;
-  // G, Lhi, Llo, Y, Yhi, Ylo (C^2 each) + per-block D, Dhi, Dlo (128^2 each)
-  return (6 * C * C + 3 * nbk * ch::NB * ch::NB) * 4 + 256;
+  // G, Lhi, Llo, Y, Yhi, Ylo (C^2 each)
+  return 6 * C * C * 4 + 256;
 }
 
 extern "C" int llmc_chol_inv_upper(float* A, int64_t C, void* workspace, int64_t workspace_bytes,
@@ -401,17 +287,10 @@ extern "C" int llmc_chol_inv_upper(float* A, int64_t C, void* workspace, int64_t
   float* Y = Llo + nn;
   float* Yhi = Y + nn;
   float* Ylo = Yhi + nn;
-  float* D = Ylo + nn;
-  float* Dhi = D + nbk * NB * NB;
-  float* Dlo = Dhi + nbk * NB * NB;
   const int diag_smem = 2 * NB * LDS * 4;
   LLMC_ONCE_PER_DEVICE({
     LLMC_CHECK_CUDA(cudaFuncSetAttribute(diag_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, diag_smem));
-    LLMC_CHECK_CUDA(cudaFuncSetAttribute(diag_kernel_v2, cudaFuncAttributeMaxDynamicSharedMemorySize, diag_smem));
   });
-  // LLMC_B200_CHOL_DIAG_V1=1: the unblocked diagonal kernel, for A/B runs
-  const char* v1_env = getenv("LLMC_B200_CHOL_DIAG_V1");
-  const bool use_v1 = (v1_env != nullptr && v1_env[0] == '1');
   // Side stream + events for the inverse chain (process-wide, created once; the call stays
   // asynchronous with respect to the host and ordered on `stream` through the final join).
   // (per device; one host thread per device is assumed, like everywhere in this library)
@@ -434,21 +313,8 @@ extern "C" int llmc_chol_inv_upper(float* A, int64_t C, void* workspace, int64_t
   }
   cudaStream_t side = side_of[dev_id];
   cudaEvent_t ev_join = join_of[dev_id];
-  // LLMC_B200_CHOL_ONE_STREAM=1 keeps the inverse chain on the caller's stream (A/B runs only)
-  const char* one_env = getenv("LLMC_B200_CHOL_ONE_STREAM");
-  const bool one_stream = one_env != nullptr && one_env[0] == '1';
-  cudaStream_t s2 = one_stream ? st : side;
-  while (static_cast<int64_t>(ev.size()) < nbk) {
-    cudaEvent_t e;
-    LLMC_CHECK_CUDA(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
-    ev.push_back(e);
-  }
-  // super-panel width for the lazy trailing updates (LLMC_B200_CHOL_SP=1..8 blocks, default 4)
-  int64_t spw = 4 * NB;
-  if (const char* e = getenv("LLMC_B200_CHOL_SP")) {
-    const int v = atoi(e);
-    if (v >= 1 && v <= 8) spw = static_cast<int64_t>(v) * NB;
-  }
+  // super-panel width of the lazy trailing updates: 4 blocks
+  constexpr int64_t spw = 4 * NB;
   LLMC_CHECK_CUDA(cudaMemsetAsync(info, 0, sizeof(int), st));
   LLMC_CHECK_CUDA(cudaMemsetAsync(Y, 0, nn * sizeof(float), st));
   // the rank-512 inverse update reads Yhi/Ylo over whole super-panel rows: the part above the
@@ -463,11 +329,9 @@ extern "C" int llmc_chol_inv_upper(float* A, int64_t C, void* workspace, int64_t
   reverse_kernel<<<(int)blocks, 256, 0, st>>>(A, G, n);
   LLMC_CHECK_LAUNCH();
 
-  // LLMC_B200_CHOL_LOOKAHEAD=0 selects the round-1 schedule below (A/B runs only)
-  const char* la_env = getenv("LLMC_B200_CHOL_LOOKAHEAD");
-  const bool lookahead = !(la_env != nullptr && la_env[0] == '0') && !use_v1 && !one_stream && n > spw;
-  if (lookahead) {
-    // ================= look-ahead schedule (round 2) ==========================================
+  // More than one super-panel: the look-ahead schedule; otherwise the serial schedule below.
+  if (n > spw) {
+    // ================= look-ahead schedule ====================================================
     // The factorisation's dependent chain is  diag(k) -> panel solve(k) -> update of column block
     // k+1  (1..112 CTAs wide); everything else — 90 % of the flops — is
     // off that chain.  Streams (created once per device):
@@ -515,7 +379,6 @@ extern "C" int llmc_chol_inv_upper(float* A, int64_t C, void* workspace, int64_t
     std::vector<cudaEvent_t>& evIB = evIB_of[dev_id];   // inverse bulk of super-panel s done (s3)
     LLMC_CHECK_CUDA(cudaEventRecord(fork_of[dev_id], st));
     LLMC_CHECK_CUDA(cudaStreamWaitEvent(hi, fork_of[dev_id], 0));
-    const int64_t nsp = (n + spw - 1) / spw;
     for (int64_t kb = 0; kb < nbk; ++kb) {
       const int64_t k0 = kb * NB;
       const int nb = static_cast<int>((n - k0) < NB ? (n - k0) : NB);
@@ -535,7 +398,7 @@ extern "C" int llmc_chol_inv_upper(float* A, int64_t C, void* workspace, int64_t
                                       Llo + k0 * n + k0, INT64_MAX, INT64_MAX, hi))
           return rc;
       }
-      diag_kernel_v2<<<1, 256, diag_smem, hi>>>(G, n, k0, nb, Y, Yhi, Ylo, info);
+      diag_kernel<<<1, 256, diag_smem, hi>>>(G, n, k0, nb, Y, Yhi, Ylo, info);
       LLMC_CHECK_LAUNCH();
       const float* Xh = Yhi + k0 * n + k0;
       const float* Xl = Ylo + k0 * n + k0;
@@ -615,7 +478,6 @@ extern "C" int llmc_chol_inv_upper(float* A, int64_t C, void* workspace, int64_t
         LLMC_CHECK_CUDA(cudaEventRecord(evIB[sidx], s3));
       }
     }
-    (void)nsp;
     cudaStream_t all[4] = {hi, bulk, si, s3};
     for (int i = 0; i < 4; ++i) {
       LLMC_CHECK_CUDA(cudaEventRecord(j_of[dev_id][i], all[i]));
@@ -626,25 +488,16 @@ extern "C" int llmc_chol_inv_upper(float* A, int64_t C, void* workspace, int64_t
     return LLMC_OK;
   }
 
+  // ================= serial schedule (n <= spw: one super-panel) ==============================
   // ---- factor: G = L L^T (lower, in place), Lhi/Llo = split of the sub-diagonal panels ----
   for (int64_t kb = 0; kb < nbk; ++kb) {
     const int64_t k0 = kb * NB;
     const int nb = static_cast<int>((n - k0) < NB ? (n - k0) : NB);
-    float* Dk = D + kb * NB * NB;
-    float* Dkh = Dhi + kb * NB * NB;
-    float* Dkl = Dlo + kb * NB * NB;
-    if (use_v1) {
-      diag_kernel<<<1, 256, diag_smem, st>>>(G, n, k0, nb, Dk, Dkh, Dkl, info);
-      LLMC_CHECK_LAUNCH();
-      place_diag_kernel<<<16, 256, 0, st>>>(Dk, Dkh, Dkl, Y, Yhi, Ylo, n, k0, nb);
-    } else {
-      diag_kernel_v2<<<1, 256, diag_smem, st>>>(G, n, k0, nb, Y, Yhi, Ylo, info);
-    }
+    diag_kernel<<<1, 256, diag_smem, st>>>(G, n, k0, nb, Y, Yhi, Ylo, info);
     LLMC_CHECK_LAUNCH();
-    // L_kk^-1 as a GEMM operand: v2 leaves it in the diagonal block of Yhi/Ylo (ld n)
-    const float* Xh = use_v1 ? Dkh : Yhi + k0 * n + k0;
-    const float* Xl = use_v1 ? Dkl : Ylo + k0 * n + k0;
-    const int64_t ldx = use_v1 ? NB : n;
+    // L_kk^-1 as a GEMM operand: the diagonal block of Yhi/Ylo (ld n)
+    const float* Xh = Yhi + k0 * n + k0;
+    const float* Xl = Ylo + k0 * n + k0;
     const int64_t r0 = k0 + nb;
     const int64_t m = n - r0;
     float* P = G + r0 * n + k0;          // panel [m x nb], ld n
@@ -654,60 +507,39 @@ extern "C" int llmc_chol_inv_upper(float* A, int64_t C, void* workspace, int64_t
       // the split of panel 0 is made here; later panels get theirs from the trailing update below
       if (kb == 0)
         if (int rc = split_tf32(P, m, nb, n, Ph, Pl, n, st)) return rc;
-      // P <- P * L_kk^-T : out[i][j] = sum_k P[i][k] * Dk[j][k]   (both K-major), + split
-      if (int rc = tf32x3_update(Ph, Pl, 0, n, Xh, Xl, 0, ldx, P, n, m, nb, nb, 1, 0, 0, 0, Ph, Pl, st))
+      // P <- P * L_kk^-T : out[i][j] = sum_k P[i][k] * X[j][k]   (both K-major), + split
+      if (int rc = tf32x3_update(Ph, Pl, 0, n, Xh, Xl, 0, n, P, n, m, nb, nb, 1, 0, 0, 0, Ph, Pl, st))
         return rc;
     }
-    LLMC_CHECK_CUDA(cudaEventRecord(ev[kb], st));          // L panel kb, D_kb and Y_kk are final
-    // Trailing updates are lazy per super-panel [sp0, sp1) of kSuperBlocks blocks: a block updates
-    // only the super-panel's remaining columns (rank 128); everything beyond the super-panel
-    // gets one rank-512 update when its last block is done — a quarter of the read-modify-write
-    // traffic.  Both emit the tf32 split of the next panel (their first 128 columns).
-    const int64_t sp0 = (k0 / spw) * spw;
-    const int64_t sp1 = (sp0 + spw < n) ? sp0 + spw : n;
-    if (m > 0 && r0 < sp1) {
-      // G[r0:, r0:sp1] -= P P[r0:sp1]^T  (lower tiles only)
-      if (int rc = tf32x3_update_ex(Ph, Pl, 0, n, Ph, Pl, 0, n, G + r0 * n + r0, n, m, sp1 - r0, nb, 0,
+    LLMC_CHECK_CUDA(cudaEventRecord(ev[kb], st));          // L panel kb and Y_kk are final
+    if (m > 0) {
+      // G[r0:, r0:] -= P P^T  (lower tiles only); emits the tf32 split of the next panel
+      if (int rc = tf32x3_update_ex(Ph, Pl, 0, n, Ph, Pl, 0, n, G + r0 * n + r0, n, m, m, nb, 0,
                                     1, 0, 0, Lhi + r0 * n + r0, Llo + r0 * n + r0, 0, NB, st))
-        return rc;
-    } else if (m > 0) {
-      // G[sp1:, sp1:] -= L[sp1:, sp0:sp1] L[sp1:, sp0:sp1]^T
-      const float* Ah = Lhi + sp1 * n + sp0;
-      const float* Al = Llo + sp1 * n + sp0;
-      if (int rc = tf32x3_update_ex(Ah, Al, 0, n, Ah, Al, 0, n, G + sp1 * n + sp1, n, n - sp1, n - sp1,
-                                    static_cast<int>(sp1 - sp0), 0, 1, 0, 0, Lhi + sp1 * n + sp1,
-                                    Llo + sp1 * n + sp1, 0, NB, st))
         return rc;
     }
 
     // ---- inverse step kb on the side stream: Y = L^-1 (lower).  T' (stored in Y below the
-    //      diagonal blocks) accumulates -sum_{k<i} L_ik Y_k ;  Y_i = D_i T'_i.  It needs panel kb
+    //      diagonal blocks) accumulates -sum_{k<i} L_ik Y_k ;  Y_i = Y_ii T'_i.  It needs panel kb
     //      of L only, so it overlaps the factorisation's trailing update and later steps. ----
-    LLMC_CHECK_CUDA(cudaStreamWaitEvent(s2, ev[kb], 0));
+    LLMC_CHECK_CUDA(cudaStreamWaitEvent(side, ev[kb], 0));
     if (kb > 0) {
       float* T = Y + k0 * n;             // rows k0..k0+nb, cols 0..k0; split emitted by step kb-1
       float* Th = Yhi + k0 * n;
       float* Tl = Ylo + k0 * n;
-      // Y[k rows, 0:k0] = D_k (K-major: D[m][kk]) * T' (MN-major: element (col, kk) at T[kk*n + col])
-      if (int rc = tf32x3_update(Xh, Xl, 0, ldx, Th, Tl, 1, n, T, n, nb, k0, nb, 1, 0, 0, 0, Th, Tl, s2))
+      // Y[k rows, 0:k0] = Y_kk (K-major) * T' (MN-major: element (col, kk) at T[kk*n + col])
+      if (int rc = tf32x3_update(Xh, Xl, 0, n, Th, Tl, 1, n, T, n, nb, k0, nb, 1, 0, 0, 0, Th, Tl, side))
         return rc;
     }
-    if (m > 0 && r0 < sp1) {
-      // T'[r0:sp1, 0:r0] -= L[r0:sp1, kblock] * Y[k rows, 0:r0]; emits the split of the next T' rows
+    if (m > 0) {
+      // T'[r0:, 0:r0] -= L[r0:, kblock] * Y[k rows, 0:r0]; emits the split of the next T' rows
       if (int rc = tf32x3_update_ex(Lhi + r0 * n + k0, Llo + r0 * n + k0, 0, n, Yhi + k0 * n,
-                                    Ylo + k0 * n, 1, n, Y + r0 * n, n, sp1 - r0, r0, nb, 0, 0, 0, 0,
-                                    Yhi + r0 * n, Ylo + r0 * n, NB, 0, s2))
-        return rc;
-    } else if (m > 0) {
-      // T'[sp1:, 0:sp1] -= L[sp1:, sp0:sp1] * Y[sp0:sp1, 0:sp1]
-      if (int rc = tf32x3_update_ex(Lhi + sp1 * n + sp0, Llo + sp1 * n + sp0, 0, n, Yhi + sp0 * n,
-                                    Ylo + sp0 * n, 1, n, Y + sp1 * n, n, n - sp1, sp1,
-                                    static_cast<int>(sp1 - sp0), 0, 0, 0, 0, Yhi + sp1 * n,
-                                    Ylo + sp1 * n, NB, 0, s2))
+                                    Ylo + k0 * n, 1, n, Y + r0 * n, n, m, r0, nb, 0, 0, 0, 0,
+                                    Yhi + r0 * n, Ylo + r0 * n, NB, 0, side))
         return rc;
     }
   }
-  LLMC_CHECK_CUDA(cudaEventRecord(ev_join, s2));
+  LLMC_CHECK_CUDA(cudaEventRecord(ev_join, side));
   LLMC_CHECK_CUDA(cudaStreamWaitEvent(st, ev_join, 0));
   reverse_upper_kernel<<<(int)blocks, 256, 0, st>>>(Y, A, n);
   LLMC_CHECK_LAUNCH();

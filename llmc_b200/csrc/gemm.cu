@@ -308,65 +308,22 @@ static PFN_tmapEncodeTiled get_encode_fn() {
   return fn;
 }
 
-int encode_tmap_2d_b16(CUtensorMap* out, const void* base, uint64_t rows, uint64_t cols,
-                       uint64_t ld_elems, uint32_t box_rows, uint32_t box_cols) {
+int encode_tmap_2d(CUtensorMap* out, const void* base, CUtensorMapDataType dtype, uint32_t elem_bytes,
+                   uint64_t rows, uint64_t cols, uint64_t ld_elems, uint32_t box_rows,
+                   uint32_t box_cols, CUtensorMapSwizzle swizzle) {
   PFN_tmapEncodeTiled fn = get_encode_fn();
   if (!fn) return LLMC_ECUDA;
   cuuint64_t dims[2] = {cols, rows};
-  cuuint64_t strides[1] = {ld_elems * 2};
+  cuuint64_t strides[1] = {ld_elems * elem_bytes};
   cuuint32_t box[2] = {box_cols, box_rows};
   cuuint32_t estr[2] = {1, 1};
-  CUresult r = fn(out, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void*>(base), dims, strides,
-                  box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
-                  CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  CUresult r = fn(out, dtype, 2, const_cast<void*>(base), dims, strides, box, estr,
+                  CU_TENSOR_MAP_INTERLEAVE_NONE, swizzle, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                  CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS) {
-    set_last_error("cuTensorMapEncodeTiled failed with CUresult %d (rows %llu cols %llu ld %llu)",
-                   (int)r, (unsigned long long)rows, (unsigned long long)cols,
+    set_last_error("cuTensorMapEncodeTiled failed with CUresult %d (dtype %d rows %llu cols %llu ld %llu)",
+                   (int)r, (int)dtype, (unsigned long long)rows, (unsigned long long)cols,
                    (unsigned long long)ld_elems);
-    return LLMC_ECUDA;
-  }
-  return LLMC_OK;
-}
-
-int encode_tmap_2d_f32(CUtensorMap* out, const void* base, uint64_t rows, uint64_t cols,
-                       uint64_t ld_elems, uint32_t box_rows, uint32_t box_cols) {
-  PFN_tmapEncodeTiled fn = get_encode_fn();
-  if (!fn) return LLMC_ECUDA;
-  cuuint64_t dims[2] = {cols, rows};
-  cuuint64_t strides[1] = {ld_elems * 4};
-  cuuint32_t box[2] = {box_cols, box_rows};
-  cuuint32_t estr[2] = {1, 1};
-  CUresult r = fn(out, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, const_cast<void*>(base), dims, strides,
-                  box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
-                  CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (r != CUDA_SUCCESS) {
-    set_last_error("cuTensorMapEncodeTiled(f32) failed with CUresult %d (rows %llu cols %llu ld %llu)",
-                   (int)r, (unsigned long long)rows, (unsigned long long)cols,
-                   (unsigned long long)ld_elems);
-    return LLMC_ECUDA;
-  }
-  return LLMC_OK;
-}
-
-// swizzle32: CU_TENSOR_MAP_SWIZZLE_32B (box_cols must be 8 = 32 bytes): the 16-byte half of a
-// 32-byte row is XORed with bit 2 of the row index, which makes one-row-per-thread 16-byte
-// shared-memory loads conflict free.
-int encode_tmap_2d_i32_noswizzle(CUtensorMap* out, const void* base, uint64_t rows, uint64_t cols,
-                                 uint64_t ld_elems, uint32_t box_rows, uint32_t box_cols,
-                                 int swizzle32) {
-  PFN_tmapEncodeTiled fn = get_encode_fn();
-  if (!fn) return LLMC_ECUDA;
-  cuuint64_t dims[2] = {cols, rows};
-  cuuint64_t strides[1] = {ld_elems * 4};
-  cuuint32_t box[2] = {box_cols, box_rows};
-  cuuint32_t estr[2] = {1, 1};
-  CUresult r = fn(out, CU_TENSOR_MAP_DATA_TYPE_INT32, 2, const_cast<void*>(base), dims, strides, box,
-                  estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                  swizzle32 == 2 ? CU_TENSOR_MAP_SWIZZLE_64B
-                                 : (swizzle32 ? CU_TENSOR_MAP_SWIZZLE_32B : CU_TENSOR_MAP_SWIZZLE_NONE),
-                  CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (r != CUDA_SUCCESS) {
-    set_last_error("cuTensorMapEncodeTiled(i32) failed with CUresult %d", (int)r);
     return LLMC_ECUDA;
   }
   return LLMC_OK;
@@ -431,8 +388,12 @@ extern "C" int llmc_gemm_bf16(const void* x, const void* w, const void* bias, vo
     return LLMC_EALIGN;
   }
   CUtensorMap tmA, tmB;
-  if (int rc = encode_tmap_2d_b16(&tmA, x, M, K, K, BM, BK)) return rc;
-  if (int rc = encode_tmap_2d_b16(&tmB, w, N, K, K, BN, BK)) return rc;
+  if (int rc = encode_tmap_2d(&tmA, x, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, M, K, K, BM, BK,
+                              CU_TENSOR_MAP_SWIZZLE_128B))
+    return rc;
+  if (int rc = encode_tmap_2d(&tmB, w, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, N, K, K, BN, BK,
+                              CU_TENSOR_MAP_SWIZZLE_128B))
+    return rc;
   GemmParams p{};
   p.M = M; p.N = N; p.K = K;
   p.out = y; p.bias = bias; p.ld_out = N;
@@ -476,7 +437,9 @@ extern "C" int llmc_syrk_accum(const void* x, int64_t T, int64_t C, int dtype, f
                  "syrk: workspace too small (%lld < %lld)", (long long)workspace_bytes,
                  (long long)(static_cast<int64_t>(s.splits) * C * C * 4));
   CUtensorMap tmX;
-  if (int rc = encode_tmap_2d_b16(&tmX, x, T, C, C, 64, 64)) return rc;
+  if (int rc = encode_tmap_2d(&tmX, x, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, T, C, C, 64, 64,
+                              CU_TENSOR_MAP_SWIZZLE_128B))
+    return rc;
   GemmParams p{};
   p.M = C; p.N = C; p.K = T;
   p.out = workspace; p.bias = nullptr; p.ld_out = C;

@@ -372,12 +372,6 @@ w4a16_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
 
 }  // namespace w4
 
-int encode_tmap_2d_b16(CUtensorMap* out, const void* base, uint64_t rows, uint64_t cols,
-                       uint64_t ld_elems, uint32_t box_rows, uint32_t box_cols);
-int encode_tmap_2d_i32_noswizzle(CUtensorMap* out, const void* base, uint64_t rows, uint64_t cols,
-                                 uint64_t ld_elems, uint32_t box_rows, uint32_t box_cols,
-                                 int swizzle32);
-
 }  // namespace llmc
 
 using namespace llmc;
@@ -404,9 +398,11 @@ static int gemm_wNa16_ng(const void* x, const int32_t* wq, const void* scales, c
   constexpr int wpr = C::kWordsPerRow;
   constexpr int kThreads = C::kThreads;
   CUtensorMap tmA, tmP;
-  if (int rc = encode_tmap_2d_b16(&tmA, x, M, K, K, BM, BK)) return rc;
-  if (int rc = encode_tmap_2d_i32_noswizzle(&tmP, wq, N, K * kBits / 32, K * kBits / 32, BN, wpr,
-                                            kBits == 4 ? 1 : 2))
+  if (int rc = encode_tmap_2d(&tmA, x, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, M, K, K, BM, BK,
+                              CU_TENSOR_MAP_SWIZZLE_128B))
+    return rc;
+  if (int rc = encode_tmap_2d(&tmP, wq, CU_TENSOR_MAP_DATA_TYPE_INT32, 4, N, K * kBits / 32, K * kBits / 32,
+                              BN, wpr, kBits == 4 ? CU_TENSOR_MAP_SWIZZLE_32B : CU_TENSOR_MAP_SWIZZLE_64B))
     return rc;
   Params p{};
   p.M = M; p.N = N; p.K = K; p.out = y; p.bias = bias;

@@ -3,15 +3,16 @@
 // Replaces GPTQ.process_hessian_and_weights (dead columns, act-order gather, damping;
 // llmc/compression/quantization/gptq.py:128-171) and GPTQ.weight_transform (:198-244) with
 // search_column_qparams (:358-366).  The reference spends ~15 tiny launches per COLUMN; here a
-// 128-column block is one launch of `gptq_inblock_kernel` (rows are independent: one thread
-// owns one weight row, the 128x128 Hinv block and the row tile live in shared memory) followed
-// by one fp32 `trailing_update_kernel` (W[:, i2:] -= Err1 @ Hinv[i1:i2, i2:], :244).
+// 128-column block is one launch of `gptq_inblock_kernel` (rows are independent: eight lanes
+// share one weight row, 32 rows per CTA, the row tile and the 128x128 Hinv block live in shared
+// memory) followed by the trailing update W[:, i2:] -= Err1 @ Hinv[i1:i2, i2:] (:244) as a 3xTF32
+// GEMM (tf32.cu), or the fp32 `trailing_update_kernel` where the operands do not allow TMA.
 //
 // Numerics: fp32 throughout like the reference (gptq.py:135).  Inside a block every op is
 // rounded exactly like torch (separate multiply and subtract for the rank-1 updates, :240;
-// IEEE divides), so single-block problems are bit-exact; across blocks only the summation
-// order of the 128-deep trailing dot products differs from the CPU BLAS.
-#include "common.cuh"
+// correctly rounded divides), so single-block problems are bit-exact; across blocks only the
+// summation order of the 128-deep trailing dot products differs from the CPU BLAS.
+#include "tc.cuh"
 #include "spqr_row.cuh"
 
 namespace llmc {
@@ -22,9 +23,6 @@ constexpr int GB = 128;          // gptq blocksize (gptq_w_only.yml: blocksize 1
 // ONE rank-512 update.  Same terms as gptq.py:244 block by block, grouped differently (fp32
 // summation order only), and a quarter of the read-modify-write traffic over W.
 constexpr int kSuperPanel = 4 * GB;
-constexpr int SB = 16;           // register sub-block inside the 128-column block
-constexpr int kPad = GB + 1;
-constexpr int HP = GB + 4;       // pitch of the transposed Hinv block (16-byte aligned rows)
 
 // ---- prepare -----------------------------------------------------------------------------------------
 __global__ void __launch_bounds__(256)
@@ -108,13 +106,6 @@ __device__ __forceinline__ float load_q(const void* p, int dt, int64_t i) {
   return DType<LLMC_BF16>::load(p, i);
 }
 
-// fp32-faithful quant-dequant of one value (quant.py:699-717 on fp32 tensors).
-__device__ __forceinline__ float qdq_f32(float w, float s, float z, float qmin, float qmax) {
-  float q = rintf(fdiv_rn(w, s)) + z;
-  q = fminf(fmaxf(q, qmin), qmax);
-  return fmul_rn(q - z, s);
-}
-
 __device__ __forceinline__ void qparams_f32(float mn, float mx, int sym, float qmin, float qmax,
                                             float& s, float& z) {
   if (sym) {
@@ -129,272 +120,20 @@ __device__ __forceinline__ void qparams_f32(float mn, float mx, int sym, float q
   }
 }
 
-__global__ void __launch_bounds__(GB, 1)
-gptq_inblock_kernel(InblockArgs a) {
-  extern __shared__ float sm[];
-  float* Wt = sm;                        // [128 cols][129]  current (lazily updated) weights
-  float* Et = Wt + GB * kPad;            // [128 cols][129]  err (Err1 transposed)
-  float* Ht = Et + GB * kPad;            // [128 j][HP]      Ht[j][i] = Hinv1[i][j]
-  const int tid = threadIdx.x;
-  const int64_t r0 = static_cast<int64_t>(blockIdx.x) * GB;
-  const int64_t row = r0 + tid;
-  const int cnt = a.count;
-
-  // Tile loads: 16-byte coalesced loads, eight in flight per thread (the scalar one-at-a-time
-  // version spent ~47 % of the kernel stalled on global latency), transposed into shared memory.
-  {
-    const bool vec = (cnt == GB) && ((a.C & 3) == 0) && ((reinterpret_cast<uintptr_t>(a.W) & 15) == 0) &&
-                     ((reinterpret_cast<uintptr_t>(a.Hinv) & 15) == 0);
-    if (vec) {
-      constexpr int kBatch = 8;
-      // W tile: 128 rows x 32 float4; item = row * 32 + c4
-      for (int base = 0; base < GB * 32; base += GB * kBatch) {
-        float4 v[kBatch];
-#pragma unroll
-        for (int b = 0; b < kBatch; ++b) {
-          const int item = base + b * GB + tid;
-          const int rr = item >> 5, c4 = item & 31;
-          const int64_t r = r0 + rr;
-          v[b] = (r < a.R) ? *reinterpret_cast<const float4*>(&a.W[r * a.C + a.i1 + c4 * 4])
-                           : make_float4(0.f, 0.f, 0.f, 0.f);
-        }
-#pragma unroll
-        for (int b = 0; b < kBatch; ++b) {
-          const int item = base + b * GB + tid;
-          const int rr = item >> 5, c = (item & 31) * 4;
-          Wt[(c + 0) * kPad + rr] = v[b].x;
-          Wt[(c + 1) * kPad + rr] = v[b].y;
-          Wt[(c + 2) * kPad + rr] = v[b].z;
-          Wt[(c + 3) * kPad + rr] = v[b].w;
-        }
-      }
-      // Hinv block: row i, float4 over j -> Ht[j][i], upper triangle only
-      for (int base = 0; base < GB * 32; base += GB * kBatch) {
-        float4 v[kBatch];
-#pragma unroll
-        for (int b = 0; b < kBatch; ++b) {
-          const int item = base + b * GB + tid;
-          const int i = item >> 5, j4 = item & 31;
-          v[b] = *reinterpret_cast<const float4*>(
-              &a.Hinv[(static_cast<int64_t>(a.i1) + i) * a.C + a.i1 + j4 * 4]);
-        }
-#pragma unroll
-        for (int b = 0; b < kBatch; ++b) {
-          const int item = base + b * GB + tid;
-          const int i = item >> 5, j = (item & 31) * 4;
-          Ht[(j + 0) * HP + i] = (j + 0 >= i) ? v[b].x : 0.f;
-          Ht[(j + 1) * HP + i] = (j + 1 >= i) ? v[b].y : 0.f;
-          Ht[(j + 2) * HP + i] = (j + 2 >= i) ? v[b].z : 0.f;
-          Ht[(j + 3) * HP + i] = (j + 3 >= i) ? v[b].w : 0.f;
-        }
-      }
-    } else {
-      const int warp = tid >> 5, lane = tid & 31;
-      for (int rr = warp; rr < GB; rr += 4) {
-        const int64_t r = r0 + rr;
-        for (int c = lane; c < GB; c += 32) {
-          float v = 0.f;
-          if (r < a.R && c < cnt) v = a.W[r * a.C + a.i1 + c];
-          Wt[c * kPad + rr] = v;
-        }
-      }
-      for (int i = warp; i < GB; i += 4)
-        for (int j = lane; j < GB; j += 32) {
-          float v = 0.f;
-          if (i < cnt && j < cnt && j >= i)
-            v = a.Hinv[(static_cast<int64_t>(a.i1) + i) * a.C + a.i1 + j];
-          Ht[j * HP + i] = v;
-        }
-    }
-  }
-  __syncthreads();
-  const bool live = row < a.R;
-
-  // ---- qparams of the groups that start inside this block (gptq.py:215-223) ----
-  // searched on W as it stands at block entry (the reference indexes the global W, not the
-  // in-block clone W1).  Kept in registers for group >= 128, recomputed per group otherwise.
-  float s_cur = 1.f, z_cur = 0.f;
-  const bool dynamic = !a.static_groups;
-  const int gsz = static_cast<int>(a.group < GB ? a.group : GB);   // columns per group inside the block
-  if (dynamic && live) {
-    if (a.group >= GB) {
-      if ((a.i1 % a.group) == 0) {
-        float mn = INFINITY, mx = -INFINITY;
-        const int64_t gend = min(static_cast<int64_t>(a.i1) + a.group, a.C);
-        if (gend - a.i1 <= cnt) {
-          for (int c = 0; c < cnt; ++c) { const float v = Wt[c * kPad + tid]; mn = fminf(mn, v); mx = fmaxf(mx, v); }
-        } else {
-          for (int64_t c = a.i1; c < gend; ++c) { const float v = a.W[row * a.C + c]; mn = fminf(mn, v); mx = fmaxf(mx, v); }
-        }
-        qparams_f32(mn, mx, a.sym, a.qmin, a.qmax, s_cur, z_cur);
-        const int64_t gi = a.i1 / a.group;
-        reinterpret_cast<float*>(a.scales)[row * a.ng + gi] = s_cur;
-        if (!a.sym) reinterpret_cast<float*>(a.zeros)[row * a.ng + gi] = z_cur;
-      } else {
-        const int64_t gi = a.i1 / a.group;    // group opened by an earlier block
-        s_cur = reinterpret_cast<const float*>(a.scales)[row * a.ng + gi];
-        z_cur = a.sym ? 0.f : reinterpret_cast<const float*>(a.zeros)[row * a.ng + gi];
-      }
-    }
-  } else if (!dynamic && live && a.group >= a.C) {
-    s_cur = load_q(a.scales, a.q_dtype, row);                 // per_channel
-    z_cur = a.zeros ? load_q(a.zeros, a.q_dtype, row) : 0.f;
-  }
-  // small groups: compute all in-block group qparams up front into registers (<= 8 groups)
-  float s_small[8], z_small[8];
-  if (dynamic && a.group < GB) {
-#pragma unroll
-    for (int g = 0; g < 8; ++g) {
-      s_small[g] = 1.f; z_small[g] = 0.f;
-      if (g * gsz < cnt && live) {
-        float mn = INFINITY, mx = -INFINITY;
-        const int cend = min((g + 1) * gsz, cnt);
-        for (int c = g * gsz; c < cend; ++c) { const float v = Wt[c * kPad + tid]; mn = fminf(mn, v); mx = fmaxf(mx, v); }
-        qparams_f32(mn, mx, a.sym, a.qmin, a.qmax, s_small[g], z_small[g]);
-        const int64_t gi = (a.i1 + g * gsz) / a.group;
-        reinterpret_cast<float*>(a.scales)[row * a.ng + gi] = s_small[g];
-        if (!a.sym) reinterpret_cast<float*>(a.zeros)[row * a.ng + gi] = z_small[g];
-      }
-    }
-  }
-
-  float loss = 0.f;
-  for (int sb = 0; sb < cnt; sb += SB) {
-    float w[SB], e[SB], ss[SB], zz[SB];
-    // qparams for the sub-block's columns
-#pragma unroll
-    for (int k = 0; k < SB; ++k) {
-      const int c = sb + k;
-      ss[k] = s_cur; zz[k] = z_cur;
-      if (dynamic && a.group < GB) {
-        const int g = c / gsz;
-        // static register indexing through a switch-free select (g <= 7)
-        float sv = s_small[0], zv = z_small[0];
-#pragma unroll
-        for (int t = 1; t < 8; ++t) { if (g == t) { sv = s_small[t]; zv = z_small[t]; } }
-        ss[k] = sv; zz[k] = zv;
-      } else if (!dynamic && a.group < a.C && live && c < cnt) {
-        const int64_t idx = static_cast<int64_t>(a.i1) + c;
-        const int64_t gi = a.gmap ? a.gmap[idx] : idx / a.group;     // gptq.py:225-227
-        ss[k] = load_q(a.scales, a.q_dtype, row * a.ng + gi);
-        zz[k] = a.zeros ? load_q(a.zeros, a.q_dtype, row * a.ng + gi) : 0.f;
-      }
-      w[k] = Wt[c * kPad + tid];
-    }
-    // sequential part: quantise column, propagate inside the sub-block (registers)
-#pragma unroll
-    for (int k = 0; k < SB; ++k) {
-      const int c = sb + k;
-      const float d = Ht[c * HP + c];                      // Hinv1[c][c]
-      const float q = qdq_f32(w[k], ss[k], zz[k], a.qmin, a.qmax);
-      const float diff = fsub_rn(w[k], q);
-      float err = 0.f;
-      if (c < cnt) {
-        loss += fdiv_rn(fmul_rn(diff, diff), fmul_rn(2.f, fmul_rn(d, d)));   // :238
-        err = fdiv_rn(diff, d);                                               // :239
-      }
-      e[k] = err;
-#pragma unroll
-      for (int k2 = k + 1; k2 < SB; ++k2)
-        w[k2] = fsub_rn(w[k2], fmul_rn(err, Ht[(sb + k2) * HP + c]));          // :240
-    }
-    // record tmp (pre-rounding compensated weight, :237) and Err1 (:241)
-#pragma unroll
-    for (int k = 0; k < SB; ++k) {
-      const int c = sb + k;
-      Wt[c * kPad + tid] = w[k];
-      Et[c * kPad + tid] = e[k];
-    }
-    // lazy propagation to the remaining columns of the block, in the reference's order
-    // (each column's 16 updates are a dependent chain by definition; four columns are kept in
-    // flight so the chains overlap)
-    int j = sb + SB;
-    for (; j + 3 < cnt; j += 4) {
-      float v0 = Wt[(j + 0) * kPad + tid], v1 = Wt[(j + 1) * kPad + tid];
-      float v2 = Wt[(j + 2) * kPad + tid], v3 = Wt[(j + 3) * kPad + tid];
-      const float4* h0 = reinterpret_cast<const float4*>(&Ht[(j + 0) * HP + sb]);
-      const float4* h1 = reinterpret_cast<const float4*>(&Ht[(j + 1) * HP + sb]);
-      const float4* h2 = reinterpret_cast<const float4*>(&Ht[(j + 2) * HP + sb]);
-      const float4* h3 = reinterpret_cast<const float4*>(&Ht[(j + 3) * HP + sb]);
-#pragma unroll
-      for (int k4 = 0; k4 < SB / 4; ++k4) {
-        const float4 a = h0[k4], b = h1[k4], c = h2[k4], d = h3[k4];
-        v0 = fsub_rn(v0, fmul_rn(e[4 * k4 + 0], a.x)); v1 = fsub_rn(v1, fmul_rn(e[4 * k4 + 0], b.x));
-        v2 = fsub_rn(v2, fmul_rn(e[4 * k4 + 0], c.x)); v3 = fsub_rn(v3, fmul_rn(e[4 * k4 + 0], d.x));
-        v0 = fsub_rn(v0, fmul_rn(e[4 * k4 + 1], a.y)); v1 = fsub_rn(v1, fmul_rn(e[4 * k4 + 1], b.y));
-        v2 = fsub_rn(v2, fmul_rn(e[4 * k4 + 1], c.y)); v3 = fsub_rn(v3, fmul_rn(e[4 * k4 + 1], d.y));
-        v0 = fsub_rn(v0, fmul_rn(e[4 * k4 + 2], a.z)); v1 = fsub_rn(v1, fmul_rn(e[4 * k4 + 2], b.z));
-        v2 = fsub_rn(v2, fmul_rn(e[4 * k4 + 2], c.z)); v3 = fsub_rn(v3, fmul_rn(e[4 * k4 + 2], d.z));
-        v0 = fsub_rn(v0, fmul_rn(e[4 * k4 + 3], a.w)); v1 = fsub_rn(v1, fmul_rn(e[4 * k4 + 3], b.w));
-        v2 = fsub_rn(v2, fmul_rn(e[4 * k4 + 3], c.w)); v3 = fsub_rn(v3, fmul_rn(e[4 * k4 + 3], d.w));
-      }
-      Wt[(j + 0) * kPad + tid] = v0; Wt[(j + 1) * kPad + tid] = v1;
-      Wt[(j + 2) * kPad + tid] = v2; Wt[(j + 3) * kPad + tid] = v3;
-    }
-    for (; j < cnt; ++j) {
-      float v = Wt[j * kPad + tid];
-      const float4* hp = reinterpret_cast<const float4*>(&Ht[j * HP + sb]);
-#pragma unroll
-      for (int k4 = 0; k4 < SB / 4; ++k4) {
-        const float4 h = hp[k4];
-        v = fsub_rn(v, fmul_rn(e[4 * k4 + 0], h.x));
-        v = fsub_rn(v, fmul_rn(e[4 * k4 + 1], h.y));
-        v = fsub_rn(v, fmul_rn(e[4 * k4 + 2], h.z));
-        v = fsub_rn(v, fmul_rn(e[4 * k4 + 3], h.w));
-      }
-      Wt[j * kPad + tid] = v;
-    }
-  }
-  if (live) a.losses[row] += loss;
-  __syncthreads();
-  // coalesced write-back: tmp[:, i1:i2] (row-major) and Err1 transposed ([k][row], k-major so
-  // the trailing GEMM reads its A operand with unit stride)
-  {
-    const int warp = tid >> 5, lane = tid & 31;
-    for (int rr = warp; rr < GB; rr += 4) {
-      const int64_t r = r0 + rr;
-      if (r >= a.R) break;
-      for (int c = lane; c < cnt; c += 32) {
-        // tmp[:, invperm] (gptq.py:186-188) fused as a scatter: permuted column i1+c goes back
-        // to original column perm[i1+c]
-        const int64_t oc = a.out_perm ? a.out_perm[a.i1 + c] : static_cast<int64_t>(a.i1) + c;
-        a.tmp[r * a.C + oc] = Wt[c * kPad + rr];
-      }
-    }
-    for (int c = warp; c < GB; c += 4)
-      for (int rr = lane; rr < GB; rr += 32) {
-        const float ev = (c < cnt) ? Et[c * kPad + rr] : 0.f;
-        const int64_t o = static_cast<int64_t>(c) * a.Rpad + r0 + rr;
-        a.err[o] = ev;
-        uint32_t hb;                                   // tf32 split for the 3xTF32 trailing GEMM
-        asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(hb) : "f"(ev));
-        const float h = __uint_as_float(hb);
-        uint32_t lb;
-        asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(lb) : "f"(ev - h));
-        a.err_hi[o] = h;
-        a.err_lo[o] = __uint_as_float(lb);
-      }
-  }
-}
-
-// ---- in-block column loop, v2: eight lanes per weight row ----------------------------------------------
-// v1 above gives one thread a whole row: 128 CTAs' worth of parallelism does not exist for
-// R = 4096 (32 CTAs, one warp per scheduler).
-// v2 spreads a row over 8 lanes (lane l owns columns l, l+8, ...), 32 rows per CTA, 256 threads,
-// two CTAs per SM:
+// A row is spread over 8 lanes (lane l owns columns l, l+8, ...), 32 rows per CTA, 256 threads,
+// two CTAs per SM (one thread per row would give R = 4096 only 32 CTAs, one warp per scheduler):
 //   * per 8-column sub-block each lane keeps ITS column in a register; the eight sequential
 //     quantise -> err -> rank-1 steps exchange `err` with one width-8 shuffle each;
 //   * the other columns of the row stay in shared memory and receive the sub-block's eight
-//     updates lazily, in the reference's order (same op sequence per element as gptq.py:240, so
-//     results are bit-identical to v1);
+//     updates lazily, in the reference's order (same op sequence per element as gptq.py:240);
 //   * x / s with s fixed is evaluated as a reciprocal multiply plus two FMA corrections
 //     (div_by below), which is the correctly rounded quotient, at a third of div.rn's cost.
 constexpr int IR = 32;            // rows per CTA
 constexpr int IL = 8;             // lanes per row
 constexpr int WP = GB + 8;        // pitch of the row-major W tile: 4 rows x 8 lanes hit 32 banks
 constexpr int EP = IR + 1;        // pitch of the transposed err tile
-constexpr int HP2 = GB + 4;       // pitch of the row-major Hinv block
-constexpr int kInblockV2Smem = (IR * WP + GB * EP + GB * HP2 + 2 * GB) * 4;
+constexpr int HP = GB + 4;        // pitch of the row-major Hinv block
+constexpr int kInblockSmem = (IR * WP + GB * EP + GB * HP + 2 * GB) * 4;
 
 // RN(x / s) given r = RN(1 / s).  q1 is a faithful quotient (residual-corrected once), and the
 // second correction of a faithful quotient with a correctly rounded reciprocal is the correctly
@@ -438,12 +177,12 @@ __device__ __forceinline__ float group8_max(float v) {
 }
 
 __global__ void __launch_bounds__(IR * IL, 2)
-gptq_inblock_kernel_v2(InblockArgs a) {
+gptq_inblock_kernel(InblockArgs a) {
   extern __shared__ float sm[];
   float* Wr = sm;                        // [32 rows][136]   current (lazily updated) weights
   float* Et = Wr + IR * WP;              // [128 cols][33]   err (Err1 transposed)
   float* Hs = Et + GB * EP;              // [128 j][132]     Hs[j][k] = Hinv1[j][k]
-  float* dd = Hs + GB * HP2;             // [128] Hinv1[c][c]
+  float* dd = Hs + GB * HP;              // [128] Hinv1[c][c]
   float* rd = dd + GB;                   // [128] RN(1 / Hinv1[c][c])
   const int tid = threadIdx.x, rg = tid >> 3, l = tid & 7;
   const int warp = tid >> 5, lane = tid & 31;
@@ -484,7 +223,7 @@ gptq_inblock_kernel_v2(InblockArgs a) {
         for (int b = 0; b < 8; ++b) {
           const int item = base + b * (IR * IL) + tid;
           const int i = item >> 5, j4 = item & 31;
-          *reinterpret_cast<float4*>(&Hs[i * HP2 + j4 * 4]) = v[b];
+          *reinterpret_cast<float4*>(&Hs[i * HP + j4 * 4]) = v[b];
         }
       }
     } else {
@@ -495,14 +234,14 @@ gptq_inblock_kernel_v2(InblockArgs a) {
       }
       for (int idx = tid; idx < GB * GB; idx += IR * IL) {
         const int i = idx >> 7, j = idx & 127;
-        Hs[i * HP2 + j] = (i < cnt && j < cnt) ? a.Hinv[(static_cast<int64_t>(a.i1) + i) * a.C + a.i1 + j]
+        Hs[i * HP + j] = (i < cnt && j < cnt) ? a.Hinv[(static_cast<int64_t>(a.i1) + i) * a.C + a.i1 + j]
                                                : 0.f;
       }
     }
   }
   __syncthreads();
   if (tid < GB) {
-    const float d = (tid < cnt) ? Hs[tid * HP2 + tid] : 1.f;
+    const float d = (tid < cnt) ? Hs[tid * HP + tid] : 1.f;
     dd[tid] = d;
     rd[tid] = __frcp_rn(d);
   }
@@ -583,7 +322,7 @@ gptq_inblock_kernel_v2(InblockArgs a) {
     float wc = Wr[rg * WP + c_own];
     float hd[IL];
 #pragma unroll
-    for (int jj = 0; jj < IL; ++jj) hd[jj] = Hs[(cb + jj) * HP2 + c_own];
+    for (int jj = 0; jj < IL; ++jj) hd[jj] = Hs[(cb + jj) * HP + c_own];
     const float d = dd[c_own], rdv = rd[c_own];
     const bool d_ok = exp_mid(d) && exp_mid(rdv);
     float ev[IL];
@@ -608,22 +347,22 @@ gptq_inblock_kernel_v2(InblockArgs a) {
     for (; mp + 3 < nsb; mp += 4) {
       float w0 = Wr[rg * WP + (mp + 0) * IL + l], w1 = Wr[rg * WP + (mp + 1) * IL + l];
       float w2 = Wr[rg * WP + (mp + 2) * IL + l], w3 = Wr[rg * WP + (mp + 3) * IL + l];
-      const float* hp = Hs + cb * HP2 + mp * IL + l;
+      const float* hp = Hs + cb * HP + mp * IL + l;
 #pragma unroll
       for (int jj = 0; jj < IL; ++jj) {
-        w0 = fsub_rn(w0, fmul_rn(ev[jj], hp[jj * HP2]));
-        w1 = fsub_rn(w1, fmul_rn(ev[jj], hp[jj * HP2 + IL]));
-        w2 = fsub_rn(w2, fmul_rn(ev[jj], hp[jj * HP2 + 2 * IL]));
-        w3 = fsub_rn(w3, fmul_rn(ev[jj], hp[jj * HP2 + 3 * IL]));
+        w0 = fsub_rn(w0, fmul_rn(ev[jj], hp[jj * HP]));
+        w1 = fsub_rn(w1, fmul_rn(ev[jj], hp[jj * HP + IL]));
+        w2 = fsub_rn(w2, fmul_rn(ev[jj], hp[jj * HP + 2 * IL]));
+        w3 = fsub_rn(w3, fmul_rn(ev[jj], hp[jj * HP + 3 * IL]));
       }
       Wr[rg * WP + (mp + 0) * IL + l] = w0; Wr[rg * WP + (mp + 1) * IL + l] = w1;
       Wr[rg * WP + (mp + 2) * IL + l] = w2; Wr[rg * WP + (mp + 3) * IL + l] = w3;
     }
     for (; mp < nsb; ++mp) {
       float w0 = Wr[rg * WP + mp * IL + l];
-      const float* hp = Hs + cb * HP2 + mp * IL + l;
+      const float* hp = Hs + cb * HP + mp * IL + l;
 #pragma unroll
-      for (int jj = 0; jj < IL; ++jj) w0 = fsub_rn(w0, fmul_rn(ev[jj], hp[jj * HP2]));
+      for (int jj = 0; jj < IL; ++jj) w0 = fsub_rn(w0, fmul_rn(ev[jj], hp[jj * HP]));
       Wr[rg * WP + mp * IL + l] = w0;
     }
   }
@@ -660,12 +399,11 @@ gptq_inblock_kernel_v2(InblockArgs a) {
 
 
 // ---- SpQR in-block kernel (spqr.py:215-268) ------------------------------------------------------------------
-// Same role as gptq_inblock_kernel for the SpQR sweep: one thread owns one weight row of the
-// 128-column block (rows are independent), the row tile / Hinv block / Err1 / outlier mask live in
-// shared memory, and ALL arithmetic is spqr::row_block() of spqr_row.cuh — the function the CPU tests
-// run on the host against the oracle.  Per group of `gs` columns: leave-one-out outlier search
-// (gs * (gs - 1) quantise-dequantise evaluations per row), bilevel (scale / zero) quantisation; per
-// column: quantise, unstructured outlier mask, rank-1 update of the block's remaining columns.
+// Same role as gptq_inblock_kernel for the SpQR sweep (rows are independent): the row tile / Hinv
+// block / Err1 / outlier mask live in shared memory.  Per group of `gs` columns: leave-one-out
+// outlier search (gs * (gs - 1) quantise-dequantise evaluations per row), bilevel (scale / zero)
+// quantisation; per column: quantise, unstructured outlier mask, rank-1 update of the block's
+// remaining columns.
 struct SpqrArgs {
   float* W;
   const float* Hinv;
@@ -684,104 +422,22 @@ struct SpqrArgs {
   float* err; float* err_hi; float* err_lo;
 };
 
-constexpr int kSpqrMaskPitch = GB + 16;
-constexpr int kSpqrSmem = (2 * GB * kPad + GB * HP) * 4 + GB * kSpqrMaskPitch;
-
-__global__ void __launch_bounds__(GB, 1)
-spqr_inblock_kernel(SpqrArgs a) {
-  extern __shared__ float sm[];
-  float* Wt = sm;                       // [col][row]  pitch kPad
-  float* Et = Wt + GB * kPad;           // [col][row]
-  float* Ht = Et + GB * kPad;           // Ht[j * HP + i] = Hinv1[i][j], upper triangle
-  uint8_t* Mt = reinterpret_cast<uint8_t*>(Ht + GB * HP);   // [col][row] pitch kSpqrMaskPitch
-  const int tid = threadIdx.x;
-  const int64_t r0 = static_cast<int64_t>(blockIdx.x) * GB;
-  const int64_t row = r0 + tid;
-  const int cnt = a.count;
-  {
-    const int warp = tid >> 5, lane = tid & 31;
-    for (int rr = warp; rr < GB; rr += 4) {
-      const int64_t r = r0 + rr;
-      for (int c = lane; c < GB; c += 32) {
-        float v = 0.f;
-        if (r < a.R && c < cnt) v = a.W[r * a.C + a.i1 + c];
-        Wt[c * kPad + rr] = v;
-      }
-    }
-    for (int i = warp; i < GB; i += 4)
-      for (int j = lane; j < GB; j += 32) {
-        float v = (i == j) ? 1.f : 0.f;
-        if (i < cnt && j < cnt && j >= i)
-          v = a.Hinv[(static_cast<int64_t>(a.i1) + i) * a.C + a.i1 + j];
-        Ht[j * HP + i] = v;
-      }
-    for (int idx = tid; idx < GB * kSpqrMaskPitch; idx += GB) Mt[idx] = 0;
-    for (int idx = tid; idx < GB * kPad; idx += GB) Et[idx] = 0.f;
-  }
-  __syncthreads();
-  if (row < a.R) {
-    spqr::Cfg cfg = a.cfg;
-    cfg.thr = a.thr[0];
-    cfg.has_thr = !isinf(cfg.thr);
-    cfg.outliers = (!a.simplified && cfg.has_thr) ? 1 : 0;
-    float s_out[GB / 16], z_out[GB / 16];
-    const float loss = spqr::row_block(Wt + tid, kPad, Ht, 1, HP, cnt, cfg, Et + tid, kPad,
-                                       Mt + tid, kSpqrMaskPitch, s_out, z_out);
-    a.losses[row] += loss;
-    const int64_t g0 = a.i1 / cfg.gs;
-    for (int g = 0; g * cfg.gs < cnt; ++g) {
-      a.scales[row * a.ng + g0 + g] = s_out[g];
-      a.zeros[row * a.ng + g0 + g] = z_out[g];
-    }
-  }
-  __syncthreads();
-  {
-    const int warp = tid >> 5, lane = tid & 31;
-    for (int rr = warp; rr < GB; rr += 4) {
-      const int64_t r = r0 + rr;
-      if (r >= a.R) break;
-      for (int c = lane; c < cnt; c += 32) {
-        // tmp[:, invperm] / mask[:, invperm] (spqr.py:163-165) fused as a scatter
-        const int64_t oc = a.out_perm ? a.out_perm[a.i1 + c] : static_cast<int64_t>(a.i1) + c;
-        a.tmp[r * a.C + oc] = Wt[c * kPad + rr];
-        a.mask[r * a.C + oc] = Mt[c * kSpqrMaskPitch + rr];
-      }
-    }
-    for (int c = warp; c < GB; c += 4)
-      for (int rr = lane; rr < GB; rr += 32) {
-        const float ev = (c < cnt) ? Et[c * kPad + rr] : 0.f;
-        const int64_t o = static_cast<int64_t>(c) * a.Rpad + r0 + rr;
-        a.err[o] = ev;
-        uint32_t hb, lb;                                   // tf32 split for the 3xTF32 trailing GEMM
-        asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(hb) : "f"(ev));
-        const float h = __uint_as_float(hb);
-        asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(lb) : "f"(ev - h));
-        a.err_hi[o] = h;
-        a.err_lo[o] = __uint_as_float(lb);
-      }
-  }
-}
-
-
-// ---- SpQR in-block kernel, 16 lanes per weight row ----------------------------------------------------------
-// spqr_inblock_kernel above gives a row to ONE thread: 32 CTAs for R = 4096, one warp per scheduler,
-// latency bound.  Here a row is spread over 16 lanes
-// (16 rows per CTA, 256 threads, two CTAs per SM): lane j evaluates the leave-one-out cases j,
-// j + 16, ... of a group, every lane recomputes the cheap group statistics, and after the (redundant)
-// quantise -> err step of a column each lane applies the rank-1 update to the later columns it owns.
-// The three phases are spqr::lanes_* of spqr_row.cuh — bit-identical to row_block() by construction,
-// checked on the host (lock-step emulation) by the CPU tests and on the GPU against the kernel above.
-// Lanes talk through the row's
-// shared-memory storage, with __syncwarp() between phases.
+// A row is spread over 16 lanes (16 rows per CTA, 256 threads, two CTAs per SM; one thread per row
+// would give R = 4096 only 32 CTAs, one warp per scheduler): lane j evaluates the leave-one-out
+// cases j, j + 16, ... of a group, every lane recomputes the cheap group statistics, and after the
+// (redundant) quantise -> err step of a column each lane applies the rank-1 update to the later
+// columns it owns.  The three phases are spqr::lanes_* of spqr_row.cuh, which the CPU tests run on
+// the host in lock step against the oracle.  Lanes talk through the row's shared-memory storage,
+// with __syncwarp() between phases.
 constexpr int SL = 16;            // lanes per row
 constexpr int SR = 16;            // rows per CTA
 constexpr int SWP = GB + 16;      // pitch of a W row: the two rows of a warp sit 16 banks apart
 constexpr int SHP = GB + 4;       // pitch of the row-major Hinv block
 constexpr int SEP = SR + 1;       // pitch of the transposed err tile
-constexpr int kSpqrLanesSmem = (SR * SWP + GB * SHP + GB * SEP) * 4 + 2 * SR * GB;
+constexpr int kSpqrSmem = (SR * SWP + GB * SHP + GB * SEP) * 4 + 2 * SR * GB;
 
 __global__ void __launch_bounds__(SR * SL, 2)
-spqr_inblock_lanes_kernel(SpqrArgs a) {
+spqr_inblock_kernel(SpqrArgs a) {
   extern __shared__ float sm[];
   float* Ws = sm;                        // [row][col]   current (in place updated) weights
   float* Hs = Ws + SR * SWP;             // [i][j]       Hinv1, upper triangle
@@ -968,20 +624,6 @@ extern "C" int llmc_gptq_prepare(const float* H, int64_t C, const int64_t* perm,
   return LLMC_OK;
 }
 
-namespace llmc {
-int tf32x3_update(const float* Ahi, const float* Alo, int a_mn, int64_t lda, const float* Bhi,
-                  const float* Blo, int b_mn, int64_t ldb, float* C, int64_t ldc, int64_t M,
-                  int64_t N, int K, int mode, int tri, int64_t row_off, int64_t col_off,
-                  float* Chi, float* Clo, cudaStream_t st);
-int tf32x3_update_grid(const float* Ahi, const float* Alo, int a_mn, int64_t lda, const float* Bhi,
-                       const float* Blo, int b_mn, int64_t ldb, float* C, int64_t ldc, int64_t M,
-                       int64_t N, int K, int mode, int tri, int64_t row_off, int64_t col_off,
-                       float* Chi, float* Clo, int64_t split_rows, int64_t split_cols,
-                       int one_tile_per_cta, cudaStream_t st);
-int split_tf32(const float* x, int64_t rows, int64_t cols, int64_t ld, float* hi, float* lo,
-               int64_t ld_out, cudaStream_t st);
-}  // namespace llmc
-
 // The schedule shared by the GPTQ and SpQR sweeps: in-block kernel per 128 columns (launched by
 // `launch_inblock(i1, count, err, err_hi, err_lo, stream)`), lazy trailing updates per super-panel
 // and the look-ahead split of the bulk update.  `wide_dynamic_group`: the in-block kernel reads
@@ -1140,16 +782,11 @@ extern "C" int llmc_gptq_colblock(float* W, const float* Hinv, int64_t R, int64_
   LLMC_CHECK_ARG(static_groups || q_dtype == LLMC_F32, "gptq_colblock: dynamic groups write fp32 qparams");
   LLMC_CHECK_ARG(workspace_bytes >= llmc_gptq_workspace_bytes(R, C), "gptq_colblock: workspace too small");
   cudaStream_t st = static_cast<cudaStream_t>(stream);
-  const int in_smem = (2 * GB * kPad + GB * HP) * 4;       // 199,680 B
   const int tr_smem = 2 * TT * TT * 4;                     // 131,072 B
   LLMC_ONCE_PER_DEVICE({
-    LLMC_CHECK_CUDA(cudaFuncSetAttribute(gptq_inblock_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, in_smem));
     LLMC_CHECK_CUDA(cudaFuncSetAttribute(trailing_update_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, tr_smem));
-    LLMC_CHECK_CUDA(cudaFuncSetAttribute(gptq_inblock_kernel_v2, cudaFuncAttributeMaxDynamicSharedMemorySize, kInblockV2Smem));
+    LLMC_CHECK_CUDA(cudaFuncSetAttribute(gptq_inblock_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kInblockSmem));
   });
-  // LLMC_B200_INBLOCK_V1=1 selects the thread-per-row kernel (A/B comparisons in tests only)
-  const char* v1env = getenv("LLMC_B200_INBLOCK_V1");
-  const bool inblock_v1 = v1env != nullptr && v1env[0] == '1';
   LLMC_CHECK_CUDA(cudaMemsetAsync(losses, 0, R * sizeof(float), st));
   InblockArgs a{};
   a.W = W; a.Hinv = Hinv; a.R = R; a.C = C;
@@ -1159,14 +796,12 @@ extern "C" int llmc_gptq_colblock(float* W, const float* Hinv, int64_t R, int64_
   a.static_groups = static_groups; a.gmap = gmap;
   a.scales = scales; a.zeros = sym ? nullptr : zeros; a.q_dtype = q_dtype;
   a.tmp = tmp; a.out_perm = out_perm; a.losses = losses;
-  const unsigned row_blocks = static_cast<unsigned>((R + GB - 1) / GB);
-  a.Rpad = static_cast<int64_t>(row_blocks) * GB;
+  a.Rpad = ((R + GB - 1) / GB) * GB;
   const bool wide = !static_groups && group > kSuperPanel;
   return sweep_schedule(W, Hinv, R, C, group, wide, workspace, st,
                         [&](int i1, int count, float* err, float* err_hi, float* err_lo, cudaStream_t cs) -> int {
     a.i1 = i1; a.count = count; a.err = err; a.err_hi = err_hi; a.err_lo = err_lo;
-    if (inblock_v1) gptq_inblock_kernel<<<row_blocks, GB, in_smem, cs>>>(a);
-    else gptq_inblock_kernel_v2<<<static_cast<unsigned>(a.Rpad / IR), IR * IL, kInblockV2Smem, cs>>>(a);
+    gptq_inblock_kernel<<<static_cast<unsigned>(a.Rpad / IR), IR * IL, kInblockSmem, cs>>>(a);
     LLMC_CHECK_LAUNCH();
     return LLMC_OK;
   });
@@ -1199,7 +834,6 @@ extern "C" int llmc_spqr_colblock(float* W, const float* Hinv, int64_t R, int64_
   const int tr_smem = 2 * TT * TT * 4;
   LLMC_ONCE_PER_DEVICE({
     LLMC_CHECK_CUDA(cudaFuncSetAttribute(spqr_inblock_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kSpqrSmem));
-    LLMC_CHECK_CUDA(cudaFuncSetAttribute(spqr_inblock_lanes_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kSpqrLanesSmem));
     LLMC_CHECK_CUDA(cudaFuncSetAttribute(trailing_update_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, tr_smem));
   });
   LLMC_CHECK_CUDA(cudaMemsetAsync(losses, 0, R * sizeof(float), st));
@@ -1212,18 +846,11 @@ extern "C" int llmc_spqr_colblock(float* W, const float* Hinv, int64_t R, int64_
   a.cfg.gs = static_cast<int>(group);
   a.thr = threshold; a.simplified = simplified_outliers;
   a.scales = scales; a.zeros = zeros; a.tmp = tmp; a.mask = mask; a.out_perm = out_perm; a.losses = losses;
-  const unsigned row_blocks = static_cast<unsigned>((R + GB - 1) / GB);
-  a.Rpad = static_cast<int64_t>(row_blocks) * GB;
-  // the 16-lanes-per-row kernel is the default (bit-identical to the thread-per-row kernel and
-  // 5-6x faster: tests/test_gpu_spqr.py::test_lane_kernel_bit_identical_to_row_kernel);
-  // LLMC_B200_SPQR_KERNEL=row selects the thread-per-row kernel (A/B comparisons in tests only)
-  const char* kenv = getenv("LLMC_B200_SPQR_KERNEL");
-  const bool row_kernel = kenv != nullptr && kenv[0] == 'r';
+  a.Rpad = ((R + GB - 1) / GB) * GB;
   return sweep_schedule(W, Hinv, R, C, group, false, workspace, st,
                         [&](int i1, int count, float* err, float* err_hi, float* err_lo, cudaStream_t cs) -> int {
     a.i1 = i1; a.count = count; a.err = err; a.err_hi = err_hi; a.err_lo = err_lo;
-    if (row_kernel) spqr_inblock_kernel<<<row_blocks, GB, kSpqrSmem, cs>>>(a);
-    else spqr_inblock_lanes_kernel<<<static_cast<unsigned>(a.Rpad / SR), SR * SL, kSpqrLanesSmem, cs>>>(a);
+    spqr_inblock_kernel<<<static_cast<unsigned>(a.Rpad / SR), SR * SL, kSpqrSmem, cs>>>(a);
     LLMC_CHECK_LAUNCH();
     return LLMC_OK;
   });

@@ -7,8 +7,6 @@
 // HBM-bound integer/byte work: one pass over W with 16-byte loads, qparams in registers,
 // 4..32-byte stores.  Bit-exactness against torch comes from reproducing torch's rounding
 // points ("T-faithful", common.cuh) — see DESIGN.md §numerics.
-#include <stdlib.h>
-
 #include "common.cuh"
 
 namespace llmc {
@@ -852,8 +850,6 @@ static int launch_fast(const QuantArgs& a, int mode, int bits, int64_t total_gro
 
 // Which (mode, bits) of the fast kernel serves this call, or -1.
 static int fast_mode(const QuantArgs& a, int dtype) {
-  static const bool off = [] { const char* e = getenv("LLMC_B200_QUANT_FAST"); return e && e[0] == '0'; }();
-  if (off) return -1;
   if (a.ld != a.cols && !(a.ng == 1 && a.ld % 8 == 0)) return -1;      // groups need dense rows
   if (a.col_scale != nullptr && !((a.group == 64 || a.group == 128) && a.ld == a.cols)) return -1;
   if (dtype != LLMC_F16 && dtype != LLMC_BF16) return -1;

@@ -6,9 +6,10 @@
 // arithmetic plus sums over <= group_size elements.  This header restates that chain in IEEE fp32
 // with one rounding per torch op (no FMA contraction: __f*_rn on the device; compile the host side
 // with -ffp-contract=off) and sums in ascending index order.  The CUDA kernel (gptq.cu:
-// spqr_inblock_kernel) calls spqr_row_block() with shared-memory strides; tests/ build the same
-// function for the host CPU and compare it bit-for-bit with oracle/spqr_oracle.py, so the device
-// arithmetic is pinned before it ever runs on a GPU.
+// spqr_inblock_kernel) spreads a row over 16 lanes and runs the lanes_* functions with
+// shared-memory strides.  row_block() is the single-thread form of the same arithmetic.  tests/
+// build both for the host CPU (the lanes in lock step) and compare them bit for bit with
+// oracle/spqr_oracle.py, so the device arithmetic is pinned before it ever runs on a GPU.
 #pragma once
 #include <cmath>
 #include <math.h>

@@ -153,10 +153,30 @@ __device__ __forceinline__ void wgmma_m64n128k16(float (&d)[64], uint64_t adesc,
 
 }  // namespace tc
 
-// ---- host: tensor-map encoding through the driver entry point ---------------------------------
-// rows x cols matrix of 2-byte elements, row stride ld_elems; box = box_cols (inner) x box_rows,
-// 128-byte swizzle (box_cols * 2 must be 128).
-int encode_tmap_2d_b16(CUtensorMap* out, const void* base, uint64_t rows, uint64_t cols,
-                       uint64_t ld_elems, uint32_t box_rows, uint32_t box_cols);
+// ---- host helpers shared across translation units ---------------------------------------------
+// gemm.cu: tensor-map encoding through the driver entry point.  rows x cols matrix of elem_bytes
+// elements, row stride ld_elems; box = box_cols (inner) x box_rows.  A swizzled box row must be
+// exactly the swizzle span (128-byte swizzle: box_cols * elem_bytes == 128).
+int encode_tmap_2d(CUtensorMap* out, const void* base, CUtensorMapDataType dtype, uint32_t elem_bytes,
+                   uint64_t rows, uint64_t cols, uint64_t ld_elems, uint32_t box_rows,
+                   uint32_t box_cols, CUtensorMapSwizzle swizzle);
+
+// tf32.cu: 3xTF32 rank-K updates (see there) and the tf32 split hi = tf32(x), lo = tf32(x - hi).
+int tf32x3_update(const float* Ahi, const float* Alo, int a_mn, int64_t lda, const float* Bhi,
+                  const float* Blo, int b_mn, int64_t ldb, float* C, int64_t ldc, int64_t M,
+                  int64_t N, int K, int mode, int tri, int64_t row_off, int64_t col_off,
+                  float* Chi, float* Clo, cudaStream_t st);
+int tf32x3_update_ex(const float* Ahi, const float* Alo, int a_mn, int64_t lda, const float* Bhi,
+                     const float* Blo, int b_mn, int64_t ldb, float* C, int64_t ldc, int64_t M,
+                     int64_t N, int K, int mode, int tri, int64_t row_off, int64_t col_off,
+                     float* Chi, float* Clo, int64_t split_rows, int64_t split_cols,
+                     cudaStream_t st);
+int tf32x3_update_grid(const float* Ahi, const float* Alo, int a_mn, int64_t lda, const float* Bhi,
+                       const float* Blo, int b_mn, int64_t ldb, float* C, int64_t ldc, int64_t M,
+                       int64_t N, int K, int mode, int tri, int64_t row_off, int64_t col_off,
+                       float* Chi, float* Clo, int64_t split_rows, int64_t split_cols,
+                       int one_tile_per_cta, cudaStream_t st);
+int split_tf32(const float* x, int64_t rows, int64_t cols, int64_t ld, float* hi, float* lo,
+               int64_t ld_out, cudaStream_t st);
 
 }  // namespace llmc

@@ -278,24 +278,16 @@ split_tf32_kernel(const float* __restrict__ x, int64_t rows, int64_t cols, int64
 }  // namespace t3
 
 // rows x cols fp32 matrix, row stride ld; 128-byte swizzle => box_cols must be 32.
-int encode_tmap_2d_f32(CUtensorMap* out, const void* base, uint64_t rows, uint64_t cols,
-                       uint64_t ld_elems, uint32_t box_rows, uint32_t box_cols);
+static int encode_tmap_2d_f32(CUtensorMap* out, const void* base, uint64_t rows, uint64_t cols,
+                              uint64_t ld_elems, uint32_t box_rows, uint32_t box_cols) {
+  return encode_tmap_2d(out, base, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, rows, cols, ld_elems, box_rows,
+                        box_cols, CU_TENSOR_MAP_SWIZZLE_128B);
+}
 
 // One 3xTF32 update.  a_mn / b_mn: operand is MN-major (element (i,k) at base[k*ld + i]).
 // split_rows / split_cols restrict where the tf32 split of the result (Chi/Clo) is written: rows
 // [0, split_rows) and columns [0, split_cols) of C (multiples of 32).  The blocked Cholesky uses
 // this to get the split of the *next* panel for free from the trailing update.
-int tf32x3_update_ex(const float* Ahi, const float* Alo, int a_mn, int64_t lda, const float* Bhi,
-                     const float* Blo, int b_mn, int64_t ldb, float* C, int64_t ldc, int64_t M,
-                     int64_t N, int K, int mode, int tri, int64_t row_off, int64_t col_off,
-                     float* Chi, float* Clo, int64_t split_rows, int64_t split_cols,
-                     cudaStream_t st);
-int tf32x3_update_grid(const float* Ahi, const float* Alo, int a_mn, int64_t lda, const float* Bhi,
-                       const float* Blo, int b_mn, int64_t ldb, float* C, int64_t ldc, int64_t M,
-                       int64_t N, int K, int mode, int tri, int64_t row_off, int64_t col_off,
-                       float* Chi, float* Clo, int64_t split_rows, int64_t split_cols,
-                       int one_tile_per_cta, cudaStream_t st);
-
 int tf32x3_update(const float* Ahi, const float* Alo, int a_mn, int64_t lda, const float* Bhi,
                   const float* Blo, int b_mn, int64_t ldb, float* C, int64_t ldc, int64_t M,
                   int64_t N, int K, int mode, int tri, int64_t row_off, int64_t col_off,

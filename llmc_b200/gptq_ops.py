@@ -4,7 +4,6 @@ llmc/compression/quantization/gptq.py (add_batch :253-295, process_hessian_and_w
 the reference's class / hook structure.
 """
 import math
-import os
 
 import torch
 
@@ -87,8 +86,6 @@ def chol_inv_upper(Hp, backend='b200', inplace=False, return_info=False):
     return_info: also return the device int32[1] status flag (0 = positive-definite, k = the
     leading minor of order k is not); the caller owns checking it (GPTQ.check_factorizations)."""
     C = Hp.shape[0]
-    if os.environ.get('LLMC_B200_CHOL') == 'cusolver':      # A/B switch for debugging only
-        backend = 'cusolver'
     if backend == 'cusolver':
         with TIMER.span('cholesky_triple(cusolver)', flops=4.0 / 3.0 * C ** 3):
             L = torch.linalg.cholesky(Hp)

@@ -1,5 +1,6 @@
-"""Debug: per-layer comparison of the hook schedule vs the progressive schedule on tiny-llama,
-under the A/B switches LLMC_B200_CHOL=cusolver / LLMC_B200_SIMT_TRAILING=1."""
+"""Debug: per-layer comparison of the hook schedule vs the progressive schedule on tiny-llama
+(LLMC_B200_SIMT_TRAILING=1 forces the fp32 CUDA-core trailing update), then the blocked Cholesky
+against chol_inv_upper(backend='cusolver')."""
 import copy
 import os
 import sys
@@ -11,7 +12,7 @@ sys.path.insert(0, os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(
 from test_gpu_framework import GPTQ_CFG, _run_gptq  # noqa: E402
 from llmc_b200 import gptq_ops as ops  # noqa: E402
 
-print('CHOL', os.environ.get('LLMC_B200_CHOL'), 'SIMT', os.environ.get('LLMC_B200_SIMT_TRAILING'))
+print('SIMT', os.environ.get('LLMC_B200_SIMT_TRAILING'))
 m1, a1 = _run_gptq(False)
 m2, a2 = _run_gptq(True)
 for bi, (b1, b2) in enumerate(zip(m1.get_blocks(), m2.get_blocks())):

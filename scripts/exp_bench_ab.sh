@@ -21,7 +21,6 @@ for v in "$@"; do
     NOTIMER) run NOTIMER LLMC_BENCH_TIMER=0 ;;
     SYNC) run SYNC LLMC_BENCH_STEP_SYNC=1 ;;
     NOTIMER_SYNC) run NOTIMER_SYNC LLMC_BENCH_TIMER=0 LLMC_BENCH_STEP_SYNC=1 ;;
-    ONESTREAM) run ONESTREAM LLMC_B200_CHOL_ONE_STREAM=1 ;;
     EXPAND) run EXPAND PYTORCH_CUDA_ALLOC_CONF=expandable_segments:True ;;
   esac
 done

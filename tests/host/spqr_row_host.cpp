@@ -1,7 +1,9 @@
 // Host build of llmc_b200/csrc/spqr_row.cuh for tests/test_oracle_golden.py: the SAME source the
 // CUDA kernel spqr_inblock_kernel compiles for the device, driven row by row on the CPU so that
 // its arithmetic can be compared bit for bit with oracle/spqr_oracle.py (and, through it, with
-// the reference-generated goldens).  Build: g++ -O2 -ffp-contract=off -shared -fPIC.
+// the reference-generated goldens).  The kernel runs the lanes_* functions (emulated in lock step
+// below); row_block() is their single-thread form, pinned to the oracle the same way.
+// Build: g++ -O2 -ffp-contract=off -shared -fPIC.
 #include "spqr_row.cuh"
 
 static spqr::QCfg qcfg(int bit, int sym, int round_zp) {

@@ -89,8 +89,8 @@ def test_error_behaviour_of_the_solver_and_gemm_entry_points():
     assert lib.llmc_gemm_f32x3(p, p, 0, 128, p, p, 0, 128, p, 128, 128, 128, 128, 3, 0, null) == -1
     assert 'mode must be 0' in last()
     assert lib.llmc_b200_error_string(-1).decode() == 'invalid argument'
-    # workspace sizing is pure arithmetic: 6 C^2 + 3 (C/128) 128^2 floats; (3*512*Rpad + 2 C^2) floats
-    assert lib.llmc_chol_workspace_bytes(4096) == (6 * 4096 ** 2 + 3 * 32 * 128 * 128) * 4 + 256
+    # workspace sizing is pure arithmetic: 6 C^2 floats; (3*512*Rpad + 2 C^2) floats
+    assert lib.llmc_chol_workspace_bytes(4096) == 6 * 4096 ** 2 * 4 + 256
     assert lib.llmc_gptq_workspace_bytes(4000, 4096) == (6 * 512 * 4096 + 2 * 4096 ** 2) * 4
     assert lib.llmc_b200_abi_version() == 1
 

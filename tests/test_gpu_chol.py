@@ -57,7 +57,7 @@ def test_f32x3_exact_on_integers_and_lower_only():
     assert torch.equal(c[low], ref[low]), 'lower triangle must be exact on small integers'
 
 
-@pytest.mark.parametrize('C', [128, 256, 1024, 4096, 1096])
+@pytest.mark.parametrize('C', [128, 256, 512, 1024, 4096, 1096])
 def test_chol_inv_upper_matches_cusolver_and_definition(C):
     from llmc_b200 import gptq_ops as ops
     torch.manual_seed(C)

@@ -121,33 +121,36 @@ def test_single_block_bit_exact_vs_oracle():
         assert torch.allclose(losses.cpu(), L_o.sum(1), rtol=1e-5, atol=0)
 
 
+@pytest.mark.parametrize('sym', [False, True])
 @pytest.mark.parametrize('group', [128, 64, 32, 256])
-def test_inblock_v2_equals_v1(group, monkeypatch):
-    """The eight-lanes-per-row kernel applies the same rounded op sequence to every element as the
-    thread-per-row kernel (and uses reciprocal+FMA-corrected division instead of div.rn), so tmp,
-    scales and zeros must be bit-identical across several 128-column blocks; R is not a multiple
-    of 32 and some columns are dead (exact zeros)."""
+def test_inblock_bit_exact_vs_oracle_across_blocks(group, sym):
+    """Hinv is the oracle's upper factor with every entry outside its 128 x 128 diagonal blocks set
+    to zero: each diagonal block is still an upper factor with a positive diagonal, and the
+    trailing updates W[:, i2:] -= Err1 @ 0 leave W unchanged on both sides.  So every 128-column
+    block of a multi-block layer starts from the same W, and the in-block kernel (eight lanes per
+    row, reciprocal + two FMA corrections instead of div.rn) must reproduce the oracle bit for bit
+    in every block: tmp, scales, zeros.  R is not a multiple of 32; a dead column gives exact
+    zeros (x == 0); one block of weights scaled by 1e-13 puts the quotients outside the Markstein
+    range, so they take div.rn."""
     from llmc_b200 import gptq_ops as ops
     torch.manual_seed(11)
     R, C, T = 333, 512, 1024
-    W = (torch.randn(R, C) * 0.02).bfloat16()
+    W = torch.randn(R, C) * 0.02
     W[:, 7] = 0
-    X = (torch.randn(1, T, C) * torch.exp(torch.randn(C))).bfloat16()
-    H, _ = go.hessian([X], C)
-    Wp, Hinv, perm = go.prepare(W, H, True, 0.01)
-    outs = []
-    for v1 in ('1', '0'):
-        monkeypatch.setenv('LLMC_B200_INBLOCK_V1', v1)
-        for sym in (False, True):
-            outs.append((v1, sym, ops.weight_transform(Wp.cuda().clone(), Hinv.cuda(), 4, sym, group)))
-    monkeypatch.delenv('LLMC_B200_INBLOCK_V1')
-    half = len(outs) // 2
-    for (_, sym, a), (_, _, b) in zip(outs[:half], outs[half:]):
-        assert torch.equal(a[0], b[0]), (group, sym, (a[0] != b[0]).float().mean().item())
-        assert torch.equal(a[2], b[2])
-        if not sym:
-            assert torch.equal(a[3], b[3])
-        assert torch.allclose(a[1], b[1], rtol=1e-5, atol=0)
+    X = torch.randn(1, T, C) * torch.exp(torch.randn(C))
+    X[..., 7] = 0
+    H, _ = go.hessian([X.bfloat16()], C)
+    Wp, Hinv, _ = go.prepare(W, H, True, 0.01)
+    Wp[:, 256:384] *= 1e-13
+    b = torch.arange(C) // 128
+    Hinv = torch.where(b[:, None] == b[None, :], Hinv, torch.zeros(()))
+    tmp_o, L_o, groups = go.weight_transform(Wp, Hinv, 4, sym, 'per_group', group)
+    tmp, losses, scales, zeros = ops.weight_transform(Wp.cuda(), Hinv.cuda(), 4, sym, group)
+    assert torch.equal(tmp.cpu(), tmp_o), (tmp.cpu() != tmp_o).float().mean().item()
+    assert torch.equal(scales.cpu(), torch.cat([g[0] for g in groups], 1))
+    if not sym:
+        assert torch.equal(zeros.cpu(), torch.cat([g[1] for g in groups], 1))
+    assert torch.allclose(losses.cpu(), L_o.sum(1), rtol=1e-5, atol=0)
 
 
 @pytest.mark.parametrize('R,C,group,static', [(4096, 4096, 128, False), (1000, 2560, 128, True),

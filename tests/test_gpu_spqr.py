@@ -169,19 +169,16 @@ def test_model_width_properties():
     assert float(((dq - tp).abs() / s)[inside].max()) <= 0.5 + 1e-3
 
 
-def test_lane_kernel_bit_identical_to_row_kernel(golden_dir, monkeypatch):
-    """The 16-lanes-per-row in-block kernel (the default) against the thread-per-row kernel
-    (LLMC_B200_SPQR_KERNEL=row): same per-element operation sequences (spqr_row.cuh: lanes_* vs row_block, equal on the
-    host by tests/test_oracle_golden.py), so every output must be bit-identical — on the reference
-    layers and on a 1000 x 1024 layer with act-order scatter; timings of both go to gpurun_out/."""
-    import json
-    import time
+def test_inblock_kernel_bit_exact_vs_oracle_across_blocks(golden_dir):
+    """The in-block kernel (16 lanes per row) against the oracle in every 128-column block of
+    multi-block layers: Hinv is restricted to its 128 x 128 diagonal blocks (each still an upper
+    factor with a positive diagonal), so the trailing updates W[:, i2:] -= Err1 @ 0 leave W
+    unchanged on both sides and every block starts from the same W.  tmp, mask, scales, zeros and
+    per-row losses must be bit-identical — on the reference layers in full and on a 1000 x 1024
+    group-16 layer (R not a multiple of 16) whose tmp / mask are scattered back through its
+    act-order permutation."""
     from llmc_b200 import gptq_ops as ops
-    cases = []
-    for c in _kat(golden_dir):
-        wcfg, l2c = _cfgs(c)
-        cases.append((c['name'], c['Wp'].cuda(), c['Hinv'].cuda(), wcfg, l2c, c['special']['relative_threshold'],
-                      c['special']['simplified_outliers'], None))
+    cases = [dict(c, perm=None) for c in _kat(golden_dir)]
     torch.manual_seed(9)
     R, C = 1000, 1024
     W = torch.randn(R, C, device='cuda') * 0.02
@@ -190,26 +187,25 @@ def test_lane_kernel_bit_identical_to_row_kernel(golden_dir, monkeypatch):
     ops.hessian_add_batch(H, 0, (torch.randn(1, 4096, C, device='cuda') * torch.exp(torch.randn(C, device='cuda') * 0.7)).bfloat16())
     perm = torch.argsort(torch.diag(H), descending=True)
     Wp, Hp = ops.prepare(W.bfloat16(), H, perm, 1.0)
-    cases.append(('rand_1000x1024', Wp, ops.chol_inv_upper(Hp), (4, False, False, 16), (3, False, False), 0.2, False, perm))
-    times = {}
-    for name, Wp, Hinv, wcfg, l2c, rel, simp, op in cases:
-        thr = ops.spqr_threshold(Wp, Hinv, rel)
-        outs = {}
-        for kern in ('row', 'lanes'):
-            monkeypatch.setenv('LLMC_B200_SPQR_KERNEL', kern)
-            ops.spqr_transform(Wp.clone(), Hinv, wcfg, l2c, l2c, thr, simp, out_perm=op)
-            torch.cuda.synchronize()
-            t0 = time.perf_counter()
-            outs[kern] = ops.spqr_transform(Wp.clone(), Hinv, wcfg, l2c, l2c, thr, simp, out_perm=op)
-            torch.cuda.synchronize()
-            times[f'{name}_{kern}_ms'] = (time.perf_counter() - t0) * 1e3
-        monkeypatch.delenv('LLMC_B200_SPQR_KERNEL')
-        for a, b in zip(outs['row'], outs['lanes']):
-            assert torch.equal(a, b), name
-    out = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), 'gpurun_out')
-    try:
-        os.makedirs(out, exist_ok=True)
-        with open(os.path.join(out, 'spqr_kernels.json'), 'w') as fh:
-            json.dump(times, fh, indent=1)
-    except OSError:
-        pass
+    l2 = dict(bit=3, symmetric=False, round_zp=False)
+    cases.append(dict(name='rand_1000x1024', Wp=Wp.cpu(), Hinv=ops.chol_inv_upper(Hp).cpu(), perm=perm.cpu(),
+                      weight_kwargs=dict(bit=4, symmetric=False, round_zp=False, group_size=16),
+                      special=dict(relative_threshold=0.2, simplified_outliers=False), level2=l2))
+    for c in cases:
+        wcfg, l2c = _cfgs(c)
+        Wp, Hinv, perm, simp = c['Wp'], c['Hinv'], c['perm'], c['special']['simplified_outliers']
+        b = torch.arange(Hinv.shape[0]) // 128
+        Hinv = torch.where(b[:, None] == b[None, :], Hinv, torch.zeros(()))
+        thr = so.threshold_of(Wp, Hinv, c['special']['relative_threshold'])
+        cfg = so.make_cfg(c['weight_kwargs'], c['special'], c['level2'], c['level2'], thr)
+        tmp_o, mask_o, S_o, Z_o, loss_o = so.weight_transform(Wp, Hinv, cfg)
+        thr_t = torch.tensor([thr], dtype=torch.float32, device='cuda')
+        tmp, mask, losses, S, Z = (t.cpu() for t in ops.spqr_transform(
+            Wp.cuda(), Hinv.cuda(), wcfg, l2c, l2c, thr_t, simp,
+            out_perm=perm.cuda() if perm is not None else None))
+        if perm is not None:
+            tmp, mask = tmp[:, perm], mask[:, perm]
+        assert torch.equal(tmp, tmp_o), c['name']
+        assert torch.equal(mask, mask_o), c['name']
+        assert torch.equal(S, S_o) and torch.equal(Z, Z_o), c['name']
+        assert torch.equal(losses, loss_o), c['name']
