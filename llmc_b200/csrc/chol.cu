@@ -8,8 +8,6 @@
 // Work: C^3/3 (factor) + C^3/3 (inverse) flops instead of the reference's potrf + potri + potrf
 // (4/3 C^3), and every O(C^3) part is a 128-deep rank update executed by the 3xTF32 tensor-core
 // kernel of tf32.cu (fp32-accurate); only the 128x128 diagonal blocks run on CUDA cores.
-#include <vector>
-
 #include "tc.cuh"
 
 namespace llmc {
@@ -287,32 +285,17 @@ extern "C" int llmc_chol_inv_upper(float* A, int64_t C, void* workspace, int64_t
   float* Y = Llo + nn;
   float* Yhi = Y + nn;
   float* Ylo = Yhi + nn;
+  const SplitMatrix L{Lhi, Llo, n};    // tf32 split of L's sub-diagonal panels
+  const SplitMatrix Ys{Yhi, Ylo, n};   // tf32 split of Y = L^-1
   const int diag_smem = 2 * NB * LDS * 4;
   LLMC_ONCE_PER_DEVICE({
     LLMC_CHECK_CUDA(cudaFuncSetAttribute(diag_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, diag_smem));
   });
-  // Side stream + events for the inverse chain (process-wide, created once; the call stays
-  // asynchronous with respect to the host and ordered on `stream` through the final join).
-  // (per device; one host thread per device is assumed, like everywhere in this library)
-  constexpr int kMaxDev = 64;
-  static cudaStream_t side_of[kMaxDev] = {};
-  static cudaEvent_t join_of[kMaxDev] = {};
-  static std::vector<cudaEvent_t> ev_of[kMaxDev];
-  int dev_id = 0;
-  LLMC_CHECK_CUDA(cudaGetDevice(&dev_id));
-  dev_id &= kMaxDev - 1;
-  if (side_of[dev_id] == nullptr) {
-    LLMC_CHECK_CUDA(cudaStreamCreateWithFlags(&side_of[dev_id], cudaStreamNonBlocking));
-    LLMC_CHECK_CUDA(cudaEventCreateWithFlags(&join_of[dev_id], cudaEventDisableTiming));
-  }
-  std::vector<cudaEvent_t>& ev = ev_of[dev_id];
-  while (static_cast<int64_t>(ev.size()) < nbk) {
-    cudaEvent_t e;
-    LLMC_CHECK_CUDA(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
-    ev.push_back(e);
-  }
-  cudaStream_t side = side_of[dev_id];
-  cudaEvent_t ev_join = join_of[dev_id];
+  // Side streams + events (common.cuh); the call stays asynchronous with respect to the host and
+  // ordered on `stream` through the final join.
+  SideStreams* side = nullptr;
+  if (int rc = side_streams(nbk + 1, &side)) return rc;
+  cudaEvent_t* ev = side->ev[0].data();   // L panel kb and Y_kk final
   // super-panel width of the lazy trailing updates: 4 blocks
   constexpr int64_t spw = 4 * NB;
   LLMC_CHECK_CUDA(cudaMemsetAsync(info, 0, sizeof(int), st));
@@ -329,12 +312,47 @@ extern "C" int llmc_chol_inv_upper(float* A, int64_t C, void* workspace, int64_t
   reverse_kernel<<<(int)blocks, 256, 0, st>>>(A, G, n);
   LLMC_CHECK_LAUNCH();
 
+  auto width = [n](int64_t k0) { return static_cast<int>((n - k0) < NB ? (n - k0) : NB); };
+  // Step kb of the factorisation on stream s, once column block kb is up to date: factor and invert
+  // the diagonal block, then the panel below it.  ev[kb] marks L panel kb and Y_kk final.
+  auto factor_block = [&](int64_t kb, cudaStream_t s) -> int {
+    const int64_t k0 = kb * NB;
+    const int nb = width(k0);
+    const int64_t r0 = k0 + nb;
+    const int64_t m = n - r0;
+    diag_kernel<<<1, 256, diag_smem, s>>>(G, n, k0, nb, Y, Yhi, Ylo, info);
+    LLMC_CHECK_LAUNCH();
+    if (m > 0) {
+      float* P = G + r0 * n + k0;          // panel [m x nb], ld n
+      // the split of panel 0 is made here; later panels get theirs from the trailing updates
+      if (kb == 0)
+        if (int rc = split_tf32(P, m, nb, n, Lhi + r0 * n + k0, Llo + r0 * n + k0, n, s)) return rc;
+      // P <- P * L_kk^-T : out[i][j] = sum_k P[i][k] * X[j][k]  (both K-major; X = L_kk^-1 is the
+      // diagonal block of Yhi/Ylo), + split
+      if (int rc = tf32x3_update(
+              Tf32x3Update{L.at(r0, k0), Ys.at(k0, k0), P, n, m, nb, nb}.overwrite().split_into(L, r0, k0), s))
+        return rc;
+    }
+    LLMC_CHECK_CUDA(cudaEventRecord(ev[kb], s));
+    return LLMC_OK;
+  };
+  // Row step kb of the inverse on stream s, after ev[kb]: Y[k rows, 0:k0] = Y_kk (K-major) * T'
+  // (MN-major: element (col, kk) at T[kk*n + col]); the split of T' was emitted by step kb-1.
+  auto inverse_row = [&](int64_t kb, cudaStream_t s) -> int {
+    LLMC_CHECK_CUDA(cudaStreamWaitEvent(s, ev[kb], 0));
+    if (kb == 0) return LLMC_OK;
+    const int64_t k0 = kb * NB;
+    const int nb = width(k0);
+    return tf32x3_update(
+        Tf32x3Update{Ys.at(k0, k0), Ys.at_mn(k0, 0), Y + k0 * n, n, nb, k0, nb}.overwrite().split_into(Ys, k0, 0), s);
+  };
+
   // More than one super-panel: the look-ahead schedule; otherwise the serial schedule below.
   if (n > spw) {
     // ================= look-ahead schedule ====================================================
     // The factorisation's dependent chain is  diag(k) -> panel solve(k) -> update of column block
     // k+1  (1..112 CTAs wide); everything else — 90 % of the flops — is
-    // off that chain.  Streams (created once per device):
+    // off that chain.  Side streams:
     //   hi    highest priority : the chain.  Inside a super-panel of 4 blocks it is LEFT-looking
     //                            (column block j receives the rank-128*(j-j0) update of its
     //                            super-panel's earlier panels right before it is factored); at a
@@ -344,44 +362,19 @@ extern "C" int llmc_chol_inv_upper(float* A, int64_t C, void* workspace, int64_t
     //                            chain needs next (A': the following 512 columns, event evA), then
     //                            everything beyond (B).  One tile per CTA, so SMs return to the
     //                            chain within a tile time.
-    //   s2    middle priority  : the inverse chain (needs panel k of L only), with its own bulk
+    //   si    middle priority  : the inverse chain (needs panel k of L only), with its own bulk
     //                            stream s3 for the rows beyond the next super-panel.
     // Every column block receives its updates in a fixed order (events), so the result does not
     // depend on timing.
-    static cudaStream_t hi_of[kMaxDev] = {}, bulk_of[kMaxDev] = {}, s3_of[kMaxDev] = {}, s2p_of[kMaxDev] = {};
-    static cudaEvent_t fork_of[kMaxDev] = {}, j_of[kMaxDev][4] = {};
-    static std::vector<cudaEvent_t> evA_of[kMaxDev], evI_of[kMaxDev], evIB_of[kMaxDev];
-    if (hi_of[dev_id] == nullptr) {
-      int least = 0, greatest = 0;
-      LLMC_CHECK_CUDA(cudaDeviceGetStreamPriorityRange(&least, &greatest));
-      const int mid = (greatest < least) ? greatest + 1 : greatest;
-      LLMC_CHECK_CUDA(cudaStreamCreateWithPriority(&hi_of[dev_id], cudaStreamNonBlocking, greatest));
-      LLMC_CHECK_CUDA(cudaStreamCreateWithPriority(&s2p_of[dev_id], cudaStreamNonBlocking, mid));
-      LLMC_CHECK_CUDA(cudaStreamCreateWithPriority(&bulk_of[dev_id], cudaStreamNonBlocking, least));
-      LLMC_CHECK_CUDA(cudaStreamCreateWithPriority(&s3_of[dev_id], cudaStreamNonBlocking, least));
-      LLMC_CHECK_CUDA(cudaEventCreateWithFlags(&fork_of[dev_id], cudaEventDisableTiming));
-      for (int i = 0; i < 4; ++i) LLMC_CHECK_CUDA(cudaEventCreateWithFlags(&j_of[dev_id][i], cudaEventDisableTiming));
-    }
-    auto grow = [&](std::vector<cudaEvent_t>& v) -> int {
-      while (static_cast<int64_t>(v.size()) < nbk + 1) {
-        cudaEvent_t e;
-        LLMC_CHECK_CUDA(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
-        v.push_back(e);
-      }
-      return LLMC_OK;
-    };
-    if (int rc = grow(evA_of[dev_id])) return rc;
-    if (int rc = grow(evI_of[dev_id])) return rc;
-    if (int rc = grow(evIB_of[dev_id])) return rc;
-    cudaStream_t hi = hi_of[dev_id], bulk = bulk_of[dev_id], si = s2p_of[dev_id], s3 = s3_of[dev_id];
-    std::vector<cudaEvent_t>& evA = evA_of[dev_id];     // A' of super-panel s done (bulk)
-    std::vector<cudaEvent_t>& evI = evI_of[dev_id];     // inverse chain reached the end of super-panel s
-    std::vector<cudaEvent_t>& evIB = evIB_of[dev_id];   // inverse bulk of super-panel s done (s3)
-    LLMC_CHECK_CUDA(cudaEventRecord(fork_of[dev_id], st));
-    LLMC_CHECK_CUDA(cudaStreamWaitEvent(hi, fork_of[dev_id], 0));
+    cudaStream_t hi = side->stream[kChain], bulk = side->stream[kBulk];
+    cudaStream_t si = side->stream[kInverse], s3 = side->stream[kInverseBulk];
+    cudaEvent_t* evA = side->ev[1].data();    // A' of super-panel s done (bulk)
+    cudaEvent_t* evI = side->ev[2].data();    // inverse chain reached the end of super-panel s
+    cudaEvent_t* evIB = side->ev[3].data();   // inverse bulk of super-panel s done (s3)
+    if (int rc = side->fork(st, {kChain})) return rc;
     for (int64_t kb = 0; kb < nbk; ++kb) {
       const int64_t k0 = kb * NB;
-      const int nb = static_cast<int>((n - k0) < NB ? (n - k0) : NB);
+      const int nb = width(k0);
       const int64_t sidx = k0 / spw;
       const int64_t sp0 = sidx * spw;
       const int64_t sp1 = (sp0 + spw < n) ? sp0 + spw : n;
@@ -392,155 +385,98 @@ extern "C" int llmc_chol_inv_upper(float* A, int64_t C, void* workspace, int64_t
         if (sidx > 0 && k0 == sp0 + NB)      // columns sp0+128.. of this super-panel come from A' of the previous one
           LLMC_CHECK_CUDA(cudaStreamWaitEvent(hi, evA[sidx - 1], 0));
         // G[k0:, k0:k0+nb] -= L[k0:, sp0:k0] L[k0:k0+nb, sp0:k0]^T ; emits the split of the block
-        if (int rc = tf32x3_update_ex(Lhi + k0 * n + sp0, Llo + k0 * n + sp0, 0, n, Lhi + k0 * n + sp0,
-                                      Llo + k0 * n + sp0, 0, n, G + k0 * n + k0, n, n - k0, nb,
-                                      static_cast<int>(k0 - sp0), 0, 0, 0, 0, Lhi + k0 * n + k0,
-                                      Llo + k0 * n + k0, INT64_MAX, INT64_MAX, hi))
+        if (int rc = tf32x3_update(Tf32x3Update{L.at(k0, sp0), L.at(k0, sp0), G + k0 * n + k0, n, n - k0, nb,
+                                                k0 - sp0}.split_into(L, k0, k0), hi))
           return rc;
       }
-      diag_kernel<<<1, 256, diag_smem, hi>>>(G, n, k0, nb, Y, Yhi, Ylo, info);
-      LLMC_CHECK_LAUNCH();
-      const float* Xh = Yhi + k0 * n + k0;
-      const float* Xl = Ylo + k0 * n + k0;
-      float* P = G + r0 * n + k0;
-      float* Ph = Lhi + r0 * n + k0;
-      float* Pl = Llo + r0 * n + k0;
-      if (m > 0) {
-        if (kb == 0)
-          if (int rc = split_tf32(P, m, nb, n, Ph, Pl, n, hi)) return rc;
-        if (int rc = tf32x3_update(Ph, Pl, 0, n, Xh, Xl, 0, n, P, n, m, nb, nb, 1, 0, 0, 0, Ph, Pl, hi))
-          return rc;
-      }
-      LLMC_CHECK_CUDA(cudaEventRecord(ev[kb], hi));        // L panel kb, Y_kk final
+      if (int rc = factor_block(kb, hi)) return rc;
       if (m > 0 && r0 == sp1) {
         // ---- super-panel boundary: rank-(sp1-sp0) update of G[sp1:, sp1:] in three pieces ----
-        const int kk = static_cast<int>(sp1 - sp0);
-        const float* Ah = Lhi + sp1 * n + sp0;
-        const float* Al = Llo + sp1 * n + sp0;
+        const int64_t kk = sp1 - sp0;
+        const SplitOperand Lsp = L.at(sp1, sp0);   // L[sp1:, sp0:sp1]
         const int64_t w1 = (n - sp1) < NB ? (n - sp1) : NB;
         // chain: the next column block (also waits for what earlier bulk pieces wrote there)
         if (sidx > 0) LLMC_CHECK_CUDA(cudaStreamWaitEvent(hi, evA[sidx - 1], 0));
-        if (int rc = tf32x3_update_ex(Ah, Al, 0, n, Ah, Al, 0, n, G + sp1 * n + sp1, n, n - sp1, w1, kk, 0,
-                                      0, 0, 0, Lhi + sp1 * n + sp1, Llo + sp1 * n + sp1, INT64_MAX,
-                                      INT64_MAX, hi))
+        if (int rc = tf32x3_update(
+                Tf32x3Update{Lsp, Lsp, G + sp1 * n + sp1, n, n - sp1, w1, kk}.split_into(L, sp1, sp1), hi))
           return rc;
         // bulk: A' = columns [sp1+128, sp1+128+spw), then B = the rest; lower tiles only
         LLMC_CHECK_CUDA(cudaStreamWaitEvent(bulk, ev[kb], 0));
         const int64_t ca = sp1 + NB;
         const int64_t cb = (ca + spw < n) ? ca + spw : n;
         if (ca < n) {
-          if (int rc = tf32x3_update_grid(Ah, Al, 0, n, Lhi + ca * n + sp0, Llo + ca * n + sp0, 0, n,
-                                          G + sp1 * n + ca, n, n - sp1, cb - ca, kk, 0, 1, sp1, ca,
-                                          nullptr, nullptr, 0, 0, 1, bulk))
+          if (int rc = tf32x3_update(Tf32x3Update{Lsp, L.at(ca, sp0), G + sp1 * n + ca, n, n - sp1, cb - ca, kk}
+                                         .lower_tiles(sp1, ca).tile_per_cta(), bulk))
             return rc;
         }
         LLMC_CHECK_CUDA(cudaEventRecord(evA[sidx], bulk));
         if (cb < n) {
-          if (int rc = tf32x3_update_grid(Ah, Al, 0, n, Lhi + cb * n + sp0, Llo + cb * n + sp0, 0, n,
-                                          G + sp1 * n + cb, n, n - sp1, n - cb, kk, 0, 1, sp1, cb,
-                                          nullptr, nullptr, 0, 0, 1, bulk))
+          if (int rc = tf32x3_update(Tf32x3Update{Lsp, L.at(cb, sp0), G + sp1 * n + cb, n, n - sp1, n - cb, kk}
+                                         .lower_tiles(sp1, cb).tile_per_cta(), bulk))
             return rc;
         }
       }
       // ---- inverse chain (si): Y = L^-1, one block row per panel ----
-      LLMC_CHECK_CUDA(cudaStreamWaitEvent(si, ev[kb], 0));
-      if (kb > 0) {
-        float* T = Y + k0 * n;
-        float* Th = Yhi + k0 * n;
-        float* Tl = Ylo + k0 * n;
-        if (int rc = tf32x3_update(Xh, Xl, 0, n, Th, Tl, 1, n, T, n, nb, k0, nb, 1, 0, 0, 0, Th, Tl, si))
-          return rc;
-      }
+      if (int rc = inverse_row(kb, si)) return rc;
       if (m > 0 && r0 < sp1) {
-        if (int rc = tf32x3_update_ex(Lhi + r0 * n + k0, Llo + r0 * n + k0, 0, n, Yhi + k0 * n,
-                                      Ylo + k0 * n, 1, n, Y + r0 * n, n, sp1 - r0, r0, nb, 0, 0, 0, 0,
-                                      Yhi + r0 * n, Ylo + r0 * n, NB, 0, si))
+        if (int rc = tf32x3_update(Tf32x3Update{L.at(r0, k0), Ys.at_mn(k0, 0), Y + r0 * n, n, sp1 - r0, r0, nb}
+                                       .split_into(Ys, r0, 0).split_first_rows(NB), si))
           return rc;
       } else if (m > 0) {
         // T'[sp1:, 0:sp1] -= L[sp1:, sp0:sp1] Y[sp0:sp1, 0:sp1]: the next super-panel's rows on the
         // chain, the rows beyond on s3 (they are next touched by the following boundary's pieces,
         // which wait for evIB)
-        const int kk = static_cast<int>(sp1 - sp0);
+        const int64_t kk = sp1 - sp0;
         const int64_t ra = (sp1 + spw < n) ? sp1 + spw : n;
         if (sidx > 0) LLMC_CHECK_CUDA(cudaStreamWaitEvent(si, evIB[sidx - 1], 0));
-        if (int rc = tf32x3_update_ex(Lhi + sp1 * n + sp0, Llo + sp1 * n + sp0, 0, n, Yhi + sp0 * n,
-                                      Ylo + sp0 * n, 1, n, Y + sp1 * n, n, ra - sp1, sp1, kk, 0, 0, 0, 0,
-                                      Yhi + sp1 * n, Ylo + sp1 * n, NB, 0, si))
+        if (int rc = tf32x3_update(Tf32x3Update{L.at(sp1, sp0), Ys.at_mn(sp0, 0), Y + sp1 * n, n, ra - sp1, sp1, kk}
+                                       .split_into(Ys, sp1, 0).split_first_rows(NB), si))
           return rc;
         LLMC_CHECK_CUDA(cudaEventRecord(evI[sidx], si));
         LLMC_CHECK_CUDA(cudaStreamWaitEvent(s3, evI[sidx], 0));
         if (ra < n) {
-          if (int rc = tf32x3_update_grid(Lhi + ra * n + sp0, Llo + ra * n + sp0, 0, n, Yhi + sp0 * n,
-                                          Ylo + sp0 * n, 1, n, Y + ra * n, n, n - ra, sp1, kk, 0, 0, 0, 0,
-                                          nullptr, nullptr, 0, 0, 1, s3))
+          if (int rc = tf32x3_update(Tf32x3Update{L.at(ra, sp0), Ys.at_mn(sp0, 0), Y + ra * n, n, n - ra, sp1, kk}
+                                         .tile_per_cta(), s3))
             return rc;
         }
         LLMC_CHECK_CUDA(cudaEventRecord(evIB[sidx], s3));
       }
     }
-    cudaStream_t all[4] = {hi, bulk, si, s3};
-    for (int i = 0; i < 4; ++i) {
-      LLMC_CHECK_CUDA(cudaEventRecord(j_of[dev_id][i], all[i]));
-      LLMC_CHECK_CUDA(cudaStreamWaitEvent(st, j_of[dev_id][i], 0));
-    }
+    if (int rc = side->join(st, {kChain, kBulk, kInverse, kInverseBulk})) return rc;
     reverse_upper_kernel<<<(int)blocks, 256, 0, st>>>(Y, A, n);
     LLMC_CHECK_LAUNCH();
     return LLMC_OK;
   }
 
   // ================= serial schedule (n <= spw: one super-panel) ==============================
+  // The factorisation runs on `stream`, the inverse steps on the least-priority side stream.
+  cudaStream_t inv = side->stream[kBulk];
   // ---- factor: G = L L^T (lower, in place), Lhi/Llo = split of the sub-diagonal panels ----
   for (int64_t kb = 0; kb < nbk; ++kb) {
     const int64_t k0 = kb * NB;
-    const int nb = static_cast<int>((n - k0) < NB ? (n - k0) : NB);
-    diag_kernel<<<1, 256, diag_smem, st>>>(G, n, k0, nb, Y, Yhi, Ylo, info);
-    LLMC_CHECK_LAUNCH();
-    // L_kk^-1 as a GEMM operand: the diagonal block of Yhi/Ylo (ld n)
-    const float* Xh = Yhi + k0 * n + k0;
-    const float* Xl = Ylo + k0 * n + k0;
+    const int nb = width(k0);
     const int64_t r0 = k0 + nb;
     const int64_t m = n - r0;
-    float* P = G + r0 * n + k0;          // panel [m x nb], ld n
-    float* Ph = Lhi + r0 * n + k0;
-    float* Pl = Llo + r0 * n + k0;
-    if (m > 0) {
-      // the split of panel 0 is made here; later panels get theirs from the trailing update below
-      if (kb == 0)
-        if (int rc = split_tf32(P, m, nb, n, Ph, Pl, n, st)) return rc;
-      // P <- P * L_kk^-T : out[i][j] = sum_k P[i][k] * X[j][k]   (both K-major), + split
-      if (int rc = tf32x3_update(Ph, Pl, 0, n, Xh, Xl, 0, n, P, n, m, nb, nb, 1, 0, 0, 0, Ph, Pl, st))
-        return rc;
-    }
-    LLMC_CHECK_CUDA(cudaEventRecord(ev[kb], st));          // L panel kb and Y_kk are final
+    if (int rc = factor_block(kb, st)) return rc;
     if (m > 0) {
       // G[r0:, r0:] -= P P^T  (lower tiles only); emits the tf32 split of the next panel
-      if (int rc = tf32x3_update_ex(Ph, Pl, 0, n, Ph, Pl, 0, n, G + r0 * n + r0, n, m, m, nb, 0,
-                                    1, 0, 0, Lhi + r0 * n + r0, Llo + r0 * n + r0, 0, NB, st))
+      if (int rc = tf32x3_update(Tf32x3Update{L.at(r0, k0), L.at(r0, k0), G + r0 * n + r0, n, m, m, nb}
+                                     .lower_tiles(0, 0).split_into(L, r0, r0).split_first_cols(NB), st))
         return rc;
     }
 
     // ---- inverse step kb on the side stream: Y = L^-1 (lower).  T' (stored in Y below the
     //      diagonal blocks) accumulates -sum_{k<i} L_ik Y_k ;  Y_i = Y_ii T'_i.  It needs panel kb
     //      of L only, so it overlaps the factorisation's trailing update and later steps. ----
-    LLMC_CHECK_CUDA(cudaStreamWaitEvent(side, ev[kb], 0));
-    if (kb > 0) {
-      float* T = Y + k0 * n;             // rows k0..k0+nb, cols 0..k0; split emitted by step kb-1
-      float* Th = Yhi + k0 * n;
-      float* Tl = Ylo + k0 * n;
-      // Y[k rows, 0:k0] = Y_kk (K-major) * T' (MN-major: element (col, kk) at T[kk*n + col])
-      if (int rc = tf32x3_update(Xh, Xl, 0, n, Th, Tl, 1, n, T, n, nb, k0, nb, 1, 0, 0, 0, Th, Tl, side))
-        return rc;
-    }
+    if (int rc = inverse_row(kb, inv)) return rc;
     if (m > 0) {
       // T'[r0:, 0:r0] -= L[r0:, kblock] * Y[k rows, 0:r0]; emits the split of the next T' rows
-      if (int rc = tf32x3_update_ex(Lhi + r0 * n + k0, Llo + r0 * n + k0, 0, n, Yhi + k0 * n,
-                                    Ylo + k0 * n, 1, n, Y + r0 * n, n, m, r0, nb, 0, 0, 0, 0,
-                                    Yhi + r0 * n, Ylo + r0 * n, NB, 0, side))
+      if (int rc = tf32x3_update(Tf32x3Update{L.at(r0, k0), Ys.at_mn(k0, 0), Y + r0 * n, n, m, r0, nb}
+                                     .split_into(Ys, r0, 0).split_first_rows(NB), inv))
         return rc;
     }
   }
-  LLMC_CHECK_CUDA(cudaEventRecord(ev_join, side));
-  LLMC_CHECK_CUDA(cudaStreamWaitEvent(st, ev_join, 0));
+  if (int rc = side->join(st, {kBulk})) return rc;
   reverse_upper_kernel<<<(int)blocks, 256, 0, st>>>(Y, A, n);
   LLMC_CHECK_LAUNCH();
   return LLMC_OK;

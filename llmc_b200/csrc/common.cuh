@@ -7,7 +7,9 @@
 #include <stdint.h>
 #include <stdio.h>
 
+#include <initializer_list>
 #include <mutex>
+#include <vector>
 
 #include "../../include/llmc_b200.h"
 
@@ -60,6 +62,35 @@ void count_launch(int n);
       once_mask_ |= once_bit_;                                       \
     }                                                                \
   } while (0)
+
+// ---- side streams ------------------------------------------------------------------------
+// The look-ahead schedules of the blocked Cholesky (chol.cu) and of the GPTQ / SpQR sweep
+// (gptq.cu) run a latency-bound chain and the bulk updates off that chain on side streams of
+// different priorities.  One set per device, created on first use, serves both.  Sharing it is
+// sound only because every call forks from the caller's stream before its first side-stream
+// launch and joins every side stream it used back into the caller's stream before it returns: its
+// side-stream work starts after everything enqueued on the caller's stream before the call and
+// ends before anything enqueued after it, so calls never overlap on a side stream.  Records and
+// waits take effect at enqueue time, so one host thread per device is assumed, like everywhere in
+// this library.
+enum SideStream {
+  kChain,          // greatest priority
+  kInverse,        // the next priority: the Cholesky's inverse chain
+  kBulk,           // least priority (the default priority of a stream)
+  kInverseBulk,    // least priority
+  kNumSideStreams
+};
+struct SideStreams {
+  cudaStream_t stream[kNumSideStreams];
+  cudaEvent_t fork_ev, join_ev[kNumSideStreams];
+  std::vector<cudaEvent_t> ev[4];   // grow-only; each array serves one purpose within a call
+  // `to` wait for everything enqueued on st so far
+  int fork(cudaStream_t st, std::initializer_list<SideStream> to);
+  // st waits for everything enqueued on `from` so far
+  int join(cudaStream_t st, std::initializer_list<SideStream> from);
+};
+// This device's side streams, with at least n_events events in every ev[] array.
+int side_streams(int64_t n_events, SideStreams** out);
 
 // ---- dtype helpers ---------------------------------------------------------------------
 // "T-faithful" arithmetic: torch eager evaluates every elementwise op on fp16/bf16 tensors

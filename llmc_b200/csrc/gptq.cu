@@ -523,6 +523,7 @@ spqr_inblock_kernel(SpqrArgs a) {
 // ---- trailing update: W[:, n0:] -= Err[R,128] @ Hinv[i1:i1+128, n0:] ---------------------------------------
 // fp32 SIMT GEMM, 128x128 tile, 8x8 per thread, K = 128 resident in shared memory.
 constexpr int TT = 128;
+constexpr int kTrailingSmem = 2 * TT * TT * 4;   // 131,072 B
 __global__ void __launch_bounds__(256, 1)
 trailing_update_kernel(float* __restrict__ W, int64_t R, int64_t Rpad, int64_t C, const float* __restrict__ Err,
                        const float* __restrict__ Hinv, int i1, int kcount, int64_t n0) {
@@ -632,15 +633,19 @@ extern "C" int llmc_gptq_prepare(const float* H, int64_t C, const int64_t* perm,
 template <class F>
 static int sweep_schedule(float* W, const float* Hinv, int64_t R, int64_t C, int64_t group,
                           bool wide_dynamic_group, void* workspace, cudaStream_t st, F&& launch_inblock) {
-  const int tr_smem = 2 * TT * TT * 4;                     // 131,072 B
+  LLMC_ONCE_PER_DEVICE({
+    LLMC_CHECK_CUDA(cudaFuncSetAttribute(trailing_update_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kTrailingSmem));
+  });
   const int64_t Rpad = ((R + GB - 1) / GB) * GB;
   // [512][Rpad] x {err, hi, lo}, two sets selected by the parity of the super-panel
   float* const err_set[2] = {reinterpret_cast<float*>(workspace),
                              reinterpret_cast<float*>(workspace) + 3 * kSuperPanel * Rpad};
   float* Hh = err_set[1] + 3 * kSuperPanel * Rpad;
   float* Hl = Hh + C * C;
-  // trailing updates on tensor cores (3xTF32) when the shapes allow TMA; fp32 SIMT otherwise
-  // LLMC_B200_SIMT_TRAILING=1 forces the fp32 CUDA-core kernel (A/B comparisons in tests only)
+  const SplitMatrix Hs{Hh, Hl, C};    // tf32 split of Hinv
+  // trailing updates on tensor cores (3xTF32) when the shapes allow TMA; fp32 SIMT otherwise.
+  // LLMC_B200_SIMT_TRAILING=1 forces the fp32 CUDA-core kernel everywhere: a second summation
+  // order for scripts/check_spqr_summation_order.py, whose measurements PARITY.md records.
   static const bool force_simt = getenv("LLMC_B200_SIMT_TRAILING") != nullptr;
   const bool tensor_trailing = !force_simt && (C % 8 == 0) && aligned16(W) && aligned16(Hinv) &&
                                aligned16(workspace);
@@ -667,30 +672,17 @@ static int sweep_schedule(float* W, const float* Hinv, int64_t R, int64_t C, int
   //  updating: those sweeps keep the serial schedule)
   const bool lookahead = !la_off && tensor_trailing && sp_width == kSuperPanel && C > 2 * kSuperPanel &&
                          !wide_dynamic_group;
-  constexpr int kMaxDev = 64;
-  static cudaStream_t hi_of[kMaxDev] = {}, bulk_of[kMaxDev] = {};
-  static cudaEvent_t fork_of[kMaxDev] = {}, join_of[kMaxDev][2] = {}, panel_of[kMaxDev][2] = {}, bulkdone_of[kMaxDev][2] = {};
   cudaStream_t chain = st, bulk = st;
-  int dev_id = 0;
+  SideStreams* side = nullptr;
+  cudaEvent_t* panel_done = nullptr;   // per parity: the panel's errors are complete (chain)
+  cudaEvent_t* bulk_done = nullptr;    // per parity: the panel's bulk update is done (bulk)
   if (lookahead) {
-    LLMC_CHECK_CUDA(cudaGetDevice(&dev_id));
-    dev_id &= kMaxDev - 1;
-    if (hi_of[dev_id] == nullptr) {
-      int least = 0, greatest = 0;
-      LLMC_CHECK_CUDA(cudaDeviceGetStreamPriorityRange(&least, &greatest));
-      LLMC_CHECK_CUDA(cudaStreamCreateWithPriority(&hi_of[dev_id], cudaStreamNonBlocking, greatest));
-      LLMC_CHECK_CUDA(cudaStreamCreateWithPriority(&bulk_of[dev_id], cudaStreamNonBlocking, least));
-      LLMC_CHECK_CUDA(cudaEventCreateWithFlags(&fork_of[dev_id], cudaEventDisableTiming));
-      for (int i = 0; i < 2; ++i) {
-        LLMC_CHECK_CUDA(cudaEventCreateWithFlags(&join_of[dev_id][i], cudaEventDisableTiming));
-        LLMC_CHECK_CUDA(cudaEventCreateWithFlags(&panel_of[dev_id][i], cudaEventDisableTiming));
-        LLMC_CHECK_CUDA(cudaEventCreateWithFlags(&bulkdone_of[dev_id][i], cudaEventDisableTiming));
-      }
-    }
-    chain = hi_of[dev_id];
-    bulk = bulk_of[dev_id];
-    LLMC_CHECK_CUDA(cudaEventRecord(fork_of[dev_id], st));
-    LLMC_CHECK_CUDA(cudaStreamWaitEvent(chain, fork_of[dev_id], 0));
+    if (int rc = side_streams(2, &side)) return rc;
+    chain = side->stream[kChain];
+    bulk = side->stream[kBulk];
+    panel_done = side->ev[0].data();
+    bulk_done = side->ev[1].data();
+    if (int rc = side->fork(st, {kChain})) return rc;
   }
   bool bulk_pending[2] = {false, false};        // a bulk update of that parity has been enqueued
   for (int64_t i1 = 0; i1 < C; i1 += GB) {
@@ -699,60 +691,49 @@ static int sweep_schedule(float* W, const float* Hinv, int64_t R, int64_t C, int
     const int64_t sp1 = (sp0 + sp_width < C) ? sp0 + sp_width : C;
     const int par = static_cast<int>((i1 / sp_width) & 1);
     float* err_base = err_set[par];
-    float* errh_base = err_base + kSuperPanel * Rpad;
-    float* errl_base = errh_base + kSuperPanel * Rpad;
+    // the tf32 split of the super-panel's errors, row j - sp0 for column j
+    const SplitMatrix E{err_base + kSuperPanel * Rpad, err_base + 2 * kSuperPanel * Rpad, Rpad};
     const int b_i1 = static_cast<int>(i1);
     const int b_count = static_cast<int>(i2 - i1);
     float* const b_err = err_base + (i1 - sp0) * Rpad;
-    float* const b_err_hi = errh_base + (i1 - sp0) * Rpad;
-    float* const b_err_lo = errl_base + (i1 - sp0) * Rpad;
-    if (int rc = launch_inblock(b_i1, b_count, b_err, b_err_hi, b_err_lo, chain)) return rc;
+    if (int rc = launch_inblock(b_i1, b_count, b_err, E.hi + (i1 - sp0) * Rpad, E.lo + (i1 - sp0) * Rpad, chain))
+      return rc;
+    // W[:, n0:n1] -= Err1[:, k0:k1] @ Hinv[k0:k1, n0:n1]   (gptq.py:244) for columns k0..k1 of this
+    // super-panel: A = Err1^T (MN-major, ld Rpad), B = Hinv rows (MN-major, ld C)
+    auto trailing = [&](int64_t k0, int64_t k1, int64_t n0, int64_t n1) {
+      return Tf32x3Update{E.at_mn(k0 - sp0, 0), Hs.at_mn(k0, n0), W + n0, C, R, n1 - n0, k1 - k0};
+    };
     if (i2 < C && tensor_trailing) {
-      // W[:, i2:] -= Err1 @ Hinv[i1:i2, i2:]   (gptq.py:244): A = Err1^T (MN-major, ld Rpad),
-      // B = Hinv rows (MN-major, ld C).  Inside the super-panel: this block's errors onto the
-      // super-panel's remaining columns; at its end: all of its errors onto everything beyond.
+      // Inside the super-panel: this block's errors onto the super-panel's remaining columns; at its
+      // end: all of its errors onto everything beyond.
       if (i2 < sp1) {
-        if (int rc = tf32x3_update(b_err_hi, b_err_lo, 1, Rpad, Hh + i1 * C + i2, Hl + i1 * C + i2,
-                                   1, C, W + i2, C, R, sp1 - i2, b_count, 0, 0, 0, 0, nullptr, nullptr, chain))
-          return rc;
+        if (int rc = tf32x3_update(trailing(i1, i2, i2, sp1), chain)) return rc;
       } else if (!lookahead) {
-        if (int rc = tf32x3_update(errh_base, errl_base, 1, Rpad, Hh + sp0 * C + sp1, Hl + sp0 * C + sp1,
-                                   1, C, W + sp1, C, R, C - sp1, static_cast<int>(sp1 - sp0), 0, 0, 0, 0,
-                                   nullptr, nullptr, chain))
-          return rc;
+        if (int rc = tf32x3_update(trailing(sp0, sp1, sp1, C), chain)) return rc;
       } else {
-        const int kk = static_cast<int>(sp1 - sp0);
         const int64_t nx1 = (sp1 + sp_width < C) ? sp1 + sp_width : C;
         // the errors of this panel are complete: the bulk piece may start (after the previous one)
-        LLMC_CHECK_CUDA(cudaEventRecord(panel_of[dev_id][par], chain));
+        LLMC_CHECK_CUDA(cudaEventRecord(panel_done[par], chain));
         // chain: the next super-panel's columns, last written by the previous panel's bulk piece
-        if (bulk_pending[par ^ 1]) LLMC_CHECK_CUDA(cudaStreamWaitEvent(chain, bulkdone_of[dev_id][par ^ 1], 0));
-        if (int rc = tf32x3_update(errh_base, errl_base, 1, Rpad, Hh + sp0 * C + sp1, Hl + sp0 * C + sp1,
-                                   1, C, W + sp1, C, R, nx1 - sp1, kk, 0, 0, 0, 0, nullptr, nullptr, chain))
-          return rc;
+        if (bulk_pending[par ^ 1]) LLMC_CHECK_CUDA(cudaStreamWaitEvent(chain, bulk_done[par ^ 1], 0));
+        if (int rc = tf32x3_update(trailing(sp0, sp1, sp1, nx1), chain)) return rc;
         // bulk: everything beyond.  After this wait the chain goes on to write the OTHER error set,
         // which the previous bulk piece (just waited for) was the last reader of.
         if (nx1 < C) {
-          LLMC_CHECK_CUDA(cudaStreamWaitEvent(bulk, panel_of[dev_id][par], 0));
-          if (int rc = tf32x3_update_grid(errh_base, errl_base, 1, Rpad, Hh + sp0 * C + nx1, Hl + sp0 * C + nx1,
-                                          1, C, W + nx1, C, R, C - nx1, kk, 0, 0, 0, 0, nullptr, nullptr,
-                                          0, 0, 1, bulk))
-            return rc;
-          LLMC_CHECK_CUDA(cudaEventRecord(bulkdone_of[dev_id][par], bulk));
+          LLMC_CHECK_CUDA(cudaStreamWaitEvent(bulk, panel_done[par], 0));
+          if (int rc = tf32x3_update(trailing(sp0, sp1, nx1, C).tile_per_cta(), bulk)) return rc;
+          LLMC_CHECK_CUDA(cudaEventRecord(bulk_done[par], bulk));
           bulk_pending[par] = true;
         }
       }
     } else if (i2 < C) {
       dim3 grid(static_cast<unsigned>((C - i2 + TT - 1) / TT), static_cast<unsigned>((R + TT - 1) / TT));
-      trailing_update_kernel<<<grid, 256, tr_smem, chain>>>(W, R, Rpad, C, b_err, Hinv, b_i1, b_count, i2);
+      trailing_update_kernel<<<grid, 256, kTrailingSmem, chain>>>(W, R, Rpad, C, b_err, Hinv, b_i1, b_count, i2);
       LLMC_CHECK_LAUNCH();
     }
   }
   if (lookahead) {
-    LLMC_CHECK_CUDA(cudaEventRecord(join_of[dev_id][0], chain));
-    LLMC_CHECK_CUDA(cudaEventRecord(join_of[dev_id][1], bulk));
-    LLMC_CHECK_CUDA(cudaStreamWaitEvent(st, join_of[dev_id][0], 0));
-    LLMC_CHECK_CUDA(cudaStreamWaitEvent(st, join_of[dev_id][1], 0));
+    if (int rc = side->join(st, {kChain, kBulk})) return rc;
   }
   return LLMC_OK;
 }
@@ -782,9 +763,7 @@ extern "C" int llmc_gptq_colblock(float* W, const float* Hinv, int64_t R, int64_
   LLMC_CHECK_ARG(static_groups || q_dtype == LLMC_F32, "gptq_colblock: dynamic groups write fp32 qparams");
   LLMC_CHECK_ARG(workspace_bytes >= llmc_gptq_workspace_bytes(R, C), "gptq_colblock: workspace too small");
   cudaStream_t st = static_cast<cudaStream_t>(stream);
-  const int tr_smem = 2 * TT * TT * 4;                     // 131,072 B
   LLMC_ONCE_PER_DEVICE({
-    LLMC_CHECK_CUDA(cudaFuncSetAttribute(trailing_update_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, tr_smem));
     LLMC_CHECK_CUDA(cudaFuncSetAttribute(gptq_inblock_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kInblockSmem));
   });
   LLMC_CHECK_CUDA(cudaMemsetAsync(losses, 0, R * sizeof(float), st));
@@ -831,10 +810,8 @@ extern "C" int llmc_spqr_colblock(float* W, const float* Hinv, int64_t R, int64_
                  (long long)group, (long long)C);
   LLMC_CHECK_ARG(workspace_bytes >= llmc_gptq_workspace_bytes(R, C), "spqr_colblock: workspace too small");
   cudaStream_t st = static_cast<cudaStream_t>(stream);
-  const int tr_smem = 2 * TT * TT * 4;
   LLMC_ONCE_PER_DEVICE({
     LLMC_CHECK_CUDA(cudaFuncSetAttribute(spqr_inblock_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kSpqrSmem));
-    LLMC_CHECK_CUDA(cudaFuncSetAttribute(trailing_update_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, tr_smem));
   });
   LLMC_CHECK_CUDA(cudaMemsetAsync(losses, 0, R * sizeof(float), st));
   SpqrArgs a{};

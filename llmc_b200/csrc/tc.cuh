@@ -162,20 +162,56 @@ int encode_tmap_2d(CUtensorMap* out, const void* base, CUtensorMapDataType dtype
                    uint32_t box_cols, CUtensorMapSwizzle swizzle);
 
 // tf32.cu: 3xTF32 rank-K updates (see there) and the tf32 split hi = tf32(x), lo = tf32(x - hi).
-int tf32x3_update(const float* Ahi, const float* Alo, int a_mn, int64_t lda, const float* Bhi,
-                  const float* Blo, int b_mn, int64_t ldb, float* C, int64_t ldc, int64_t M,
-                  int64_t N, int K, int mode, int tri, int64_t row_off, int64_t col_off,
-                  float* Chi, float* Clo, cudaStream_t st);
-int tf32x3_update_ex(const float* Ahi, const float* Alo, int a_mn, int64_t lda, const float* Bhi,
-                     const float* Blo, int b_mn, int64_t ldb, float* C, int64_t ldc, int64_t M,
-                     int64_t N, int K, int mode, int tri, int64_t row_off, int64_t col_off,
-                     float* Chi, float* Clo, int64_t split_rows, int64_t split_cols,
-                     cudaStream_t st);
-int tf32x3_update_grid(const float* Ahi, const float* Alo, int a_mn, int64_t lda, const float* Bhi,
-                       const float* Blo, int b_mn, int64_t ldb, float* C, int64_t ldc, int64_t M,
-                       int64_t N, int K, int mode, int tri, int64_t row_off, int64_t col_off,
-                       float* Chi, float* Clo, int64_t split_rows, int64_t split_cols,
-                       int one_tile_per_cta, cudaStream_t st);
+// A GEMM operand held as its tf32 split: element (i, k) at [i * ld + k] (K-major) or, mn = true,
+// at [k * ld + i] (MN-major); i indexes M (operand A) or N (operand B).
+struct SplitOperand {
+  const float* hi;
+  const float* lo;
+  int64_t ld;
+  bool mn;
+};
+// An fp32 matrix held as its tf32 split with row stride ld.  at / at_mn: the operand whose element
+// (i, k) is the matrix element (row + i, col + k) / (row + k, col + i).
+struct SplitMatrix {
+  float* hi;
+  float* lo;
+  int64_t ld;
+  SplitOperand at(int64_t row, int64_t col) const {
+    return {hi + row * ld + col, lo + row * ld + col, ld, false};
+  }
+  SplitOperand at_mn(int64_t row, int64_t col) const {
+    return {hi + row * ld + col, lo + row * ld + col, ld, true};
+  }
+};
+// C[i][j] -= sum_k A(i, k) B(j, k) for i < M, j < N, k < K; C has row stride ldc.  The optional
+// parts default to off and are set by the chained setters, so one update reads as one statement:
+//   tf32x3_update(Tf32x3Update{A, B, c, ldc, M, N, K}.overwrite().split_into(S, row, col), stream)
+struct Tf32x3Update {
+  SplitOperand a, b;
+  float* c;
+  int64_t ldc, M, N, K;
+  bool assign = false;              // C = A B^T instead of C -= A B^T
+  bool lower = false;               // only the tiles that touch the lower triangle (col <= row),
+  int64_t row_off = 0, col_off = 0; //   C[0][0] being element (row_off, col_off) of the matrix
+  SplitMatrix c_split{};            // tf32 split of the result (ld == ldc) where C's row <
+  int64_t split_rows = INT64_MAX;   //   split_rows or column < split_cols; hi == nullptr: none
+  int64_t split_cols = INT64_MAX;
+  bool one_tile_per_cta = false;    // grid = tile count (see tf32x3_update)
+
+  Tf32x3Update& overwrite() { assign = true; return *this; }
+  Tf32x3Update& lower_tiles(int64_t row0, int64_t col0) {
+    lower = true; row_off = row0; col_off = col0; return *this;
+  }
+  // the split goes to s at (row, col) onward, everywhere unless narrowed by split_first_*
+  Tf32x3Update& split_into(const SplitMatrix& s, int64_t row, int64_t col) {
+    c_split = {s.hi + row * s.ld + col, s.lo + row * s.ld + col, s.ld};
+    return *this;
+  }
+  Tf32x3Update& split_first_rows(int64_t rows) { split_rows = rows; split_cols = 0; return *this; }
+  Tf32x3Update& split_first_cols(int64_t cols) { split_rows = 0; split_cols = cols; return *this; }
+  Tf32x3Update& tile_per_cta() { one_tile_per_cta = true; return *this; }
+};
+int tf32x3_update(const Tf32x3Update& u, cudaStream_t st);
 int split_tf32(const float* x, int64_t rows, int64_t cols, int64_t ld, float* hi, float* lo,
                int64_t ld_out, cudaStream_t st);
 

@@ -277,96 +277,73 @@ split_tf32_kernel(const float* __restrict__ x, int64_t rows, int64_t cols, int64
 
 }  // namespace t3
 
-// rows x cols fp32 matrix, row stride ld; 128-byte swizzle => box_cols must be 32.
-static int encode_tmap_2d_f32(CUtensorMap* out, const void* base, uint64_t rows, uint64_t cols,
-                              uint64_t ld_elems, uint32_t box_rows, uint32_t box_cols) {
-  return encode_tmap_2d(out, base, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, rows, cols, ld_elems, box_rows,
-                        box_cols, CU_TENSOR_MAP_SWIZZLE_128B);
-}
-
-// One 3xTF32 update.  a_mn / b_mn: operand is MN-major (element (i,k) at base[k*ld + i]).
-// split_rows / split_cols restrict where the tf32 split of the result (Chi/Clo) is written: rows
-// [0, split_rows) and columns [0, split_cols) of C (multiples of 32).  The blocked Cholesky uses
-// this to get the split of the *next* panel for free from the trailing update.
-int tf32x3_update(const float* Ahi, const float* Alo, int a_mn, int64_t lda, const float* Bhi,
-                  const float* Blo, int b_mn, int64_t ldb, float* C, int64_t ldc, int64_t M,
-                  int64_t N, int K, int mode, int tri, int64_t row_off, int64_t col_off,
-                  float* Chi, float* Clo, cudaStream_t st) {
-  return tf32x3_update_ex(Ahi, Alo, a_mn, lda, Bhi, Blo, b_mn, ldb, C, ldc, M, N, K, mode, tri,
-                          row_off, col_off, Chi, Clo, INT64_MAX, INT64_MAX, st);
-}
-
-int tf32x3_update_ex(const float* Ahi, const float* Alo, int a_mn, int64_t lda, const float* Bhi,
-                     const float* Blo, int b_mn, int64_t ldb, float* C, int64_t ldc, int64_t M,
-                     int64_t N, int K, int mode, int tri, int64_t row_off, int64_t col_off,
-                     float* Chi, float* Clo, int64_t split_rows, int64_t split_cols,
-                     cudaStream_t st) {
-  return tf32x3_update_grid(Ahi, Alo, a_mn, lda, Bhi, Blo, b_mn, ldb, C, ldc, M, N, K, mode, tri,
-                            row_off, col_off, Chi, Clo, split_rows, split_cols, 0, st);
-}
-
-// one_tile_per_cta != 0: grid = number of tiles, every CTA computes one tile and exits.  Bulk
+// One 3xTF32 update (Tf32x3Update, tc.cuh).  The split of the result can be narrowed to C's first
+// rows or columns (multiples of 32): the blocked Cholesky uses this to get the split of the *next*
+// panel for free from the trailing update.
+// one_tile_per_cta: grid = number of tiles, every CTA computes one tile and exits.  Bulk
 // updates launched on a LOW-priority stream this way give their SMs back at tile granularity
 // (one 128 x 128 tile), so the short kernels of a latency-bound chain on a high-priority stream (blocked
 // Cholesky look-ahead, chol.cu) never wait behind a persistent grid that fills every SM.
-int tf32x3_update_grid(const float* Ahi, const float* Alo, int a_mn, int64_t lda, const float* Bhi,
-                       const float* Blo, int b_mn, int64_t ldb, float* C, int64_t ldc, int64_t M,
-                       int64_t N, int K, int mode, int tri, int64_t row_off, int64_t col_off,
-                       float* Chi, float* Clo, int64_t split_rows, int64_t split_cols,
-                       int one_tile_per_cta, cudaStream_t st) {
+int tf32x3_update(const Tf32x3Update& u, cudaStream_t st) {
   using namespace t3;
-  if (M <= 0 || N <= 0 || K <= 0) return LLMC_OK;
-  if ((lda % 4) || (ldb % 4) || !aligned16(Ahi) || !aligned16(Alo) || !aligned16(Bhi) ||
-      !aligned16(Blo)) {
+  if (u.M <= 0 || u.N <= 0 || u.K <= 0) return LLMC_OK;
+  if ((u.a.ld % 4) || (u.b.ld % 4) || !aligned16(u.a.hi) || !aligned16(u.a.lo) ||
+      !aligned16(u.b.hi) || !aligned16(u.b.lo)) {
     set_last_error("tf32x3_update: operands need 16-byte aligned bases and ld %% 4 == 0");
     return LLMC_EALIGN;
   }
-  CUtensorMap tah, tal, tbh, tbl;
-  int rc;
-  if (!a_mn) {
-    if ((rc = encode_tmap_2d_f32(&tah, Ahi, M, K, lda, BM, BK))) return rc;
-    if ((rc = encode_tmap_2d_f32(&tal, Alo, M, K, lda, BM, BK))) return rc;
-  } else {
-    if ((rc = encode_tmap_2d_f32(&tah, Ahi, K, M, lda, BK, 32))) return rc;
-    if ((rc = encode_tmap_2d_f32(&tal, Alo, K, M, lda, BK, 32))) return rc;
+  if (u.c_split.hi != nullptr && u.c_split.ld != u.ldc) {
+    set_last_error("tf32x3_update: the split of the result must have the result's ld");
+    return LLMC_EINVAL;
   }
-  if (!b_mn) {
-    if ((rc = encode_tmap_2d_f32(&tbh, Bhi, N, K, ldb, BN, BK))) return rc;
-    if ((rc = encode_tmap_2d_f32(&tbl, Blo, N, K, ldb, BN, BK))) return rc;
-  } else {
-    if ((rc = encode_tmap_2d_f32(&tbh, Bhi, K, N, ldb, BK, 32))) return rc;
-    if ((rc = encode_tmap_2d_f32(&tbl, Blo, K, N, ldb, BK, 32))) return rc;
-  }
+  // both halves of an operand with `rows` M or N indices: K-major boxes are box_rows x BK,
+  // MN-major boxes BK x 32 (128-byte swizzle: a box row is 32 fp32)
+  auto encode = [&](CUtensorMap (&tm)[2], const SplitOperand& x, int64_t rows, uint32_t box_rows) -> int {
+    for (int h = 0; h < 2; ++h) {
+      const float* base = h ? x.lo : x.hi;
+      const int rc =
+          x.mn ? encode_tmap_2d(&tm[h], base, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, u.K, rows, x.ld,
+                                BK, 32, CU_TENSOR_MAP_SWIZZLE_128B)
+               : encode_tmap_2d(&tm[h], base, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, rows, u.K, x.ld,
+                                box_rows, BK, CU_TENSOR_MAP_SWIZZLE_128B);
+      if (rc) return rc;
+    }
+    return LLMC_OK;
+  };
+  CUtensorMap ta[2], tb[2];
+  if (int rc = encode(ta, u.a, u.M, BM)) return rc;
+  if (int rc = encode(tb, u.b, u.N, BN)) return rc;
   Params p{};
-  p.M = M; p.N = N; p.K = K; p.C = C; p.ldc = ldc; p.Chi = Chi; p.Clo = Clo;
-  p.mode = mode; p.tri = tri; p.row_off = row_off; p.col_off = col_off;
-  p.split_rows = split_rows; p.split_cols = split_cols;
-  p.n_tiles_m = static_cast<int>((M + BM - 1) / BM);
-  p.n_tiles_n = static_cast<int>((N + BN - 1) / BN);
-  if (!tri) {
+  p.M = u.M; p.N = u.N; p.K = static_cast<int>(u.K); p.C = u.c; p.ldc = u.ldc;
+  p.Chi = u.c_split.hi; p.Clo = u.c_split.lo;
+  p.mode = u.assign ? 1 : 0; p.tri = u.lower ? 1 : 0; p.row_off = u.row_off; p.col_off = u.col_off;
+  p.split_rows = u.split_rows; p.split_cols = u.split_cols;
+  p.n_tiles_m = static_cast<int>((u.M + BM - 1) / BM);
+  p.n_tiles_n = static_cast<int>((u.N + BN - 1) / BN);
+  if (!u.lower) {
     p.num_units = p.n_tiles_m * p.n_tiles_n;
   } else {
     long units = 0;
     for (int mi = 0; mi < p.n_tiles_m; ++mi) {
-      const int64_t last_row = row_off + static_cast<int64_t>(mi) * BM + BM - 1;
-      int64_t cnt = last_row < col_off ? 0 : (last_row - col_off) / BN + 1;
+      const int64_t last_row = u.row_off + static_cast<int64_t>(mi) * BM + BM - 1;
+      int64_t cnt = last_row < u.col_off ? 0 : (last_row - u.col_off) / BN + 1;
       if (cnt > p.n_tiles_n) cnt = p.n_tiles_n;
       units += cnt;
     }
     p.num_units = static_cast<int>(units);
   }
   if (p.num_units == 0) return LLMC_OK;
-  const int grid = (one_tile_per_cta || p.num_units < kNumSMs) ? p.num_units : kNumSMs;
+  const int grid = (u.one_tile_per_cta || p.num_units < kNumSMs) ? p.num_units : kNumSMs;
   LLMC_ONCE_PER_DEVICE({
     LLMC_CHECK_CUDA(cudaFuncSetAttribute(tf32x3_kernel<false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemBytes));
     LLMC_CHECK_CUDA(cudaFuncSetAttribute(tf32x3_kernel<false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemBytes));
     LLMC_CHECK_CUDA(cudaFuncSetAttribute(tf32x3_kernel<true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemBytes));
     LLMC_CHECK_CUDA(cudaFuncSetAttribute(tf32x3_kernel<true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemBytes));
   });
-  if (!a_mn && !b_mn) tf32x3_kernel<false, false><<<grid, kThreads, kSmemBytes, st>>>(tah, tal, tbh, tbl, p);
-  else if (!a_mn && b_mn) tf32x3_kernel<false, true><<<grid, kThreads, kSmemBytes, st>>>(tah, tal, tbh, tbl, p);
-  else if (a_mn && !b_mn) tf32x3_kernel<true, false><<<grid, kThreads, kSmemBytes, st>>>(tah, tal, tbh, tbl, p);
-  else tf32x3_kernel<true, true><<<grid, kThreads, kSmemBytes, st>>>(tah, tal, tbh, tbl, p);
+  if (!u.a.mn && !u.b.mn) tf32x3_kernel<false, false><<<grid, kThreads, kSmemBytes, st>>>(ta[0], ta[1], tb[0], tb[1], p);
+  else if (!u.a.mn) tf32x3_kernel<false, true><<<grid, kThreads, kSmemBytes, st>>>(ta[0], ta[1], tb[0], tb[1], p);
+  else if (!u.b.mn) tf32x3_kernel<true, false><<<grid, kThreads, kSmemBytes, st>>>(ta[0], ta[1], tb[0], tb[1], p);
+  else tf32x3_kernel<true, true><<<grid, kThreads, kSmemBytes, st>>>(ta[0], ta[1], tb[0], tb[1], p);
   LLMC_CHECK_LAUNCH();
   return LLMC_OK;
 }
@@ -399,6 +376,8 @@ extern "C" int llmc_gemm_f32x3(const float* a_hi, const float* a_lo, int a_mn, i
   LLMC_CHECK_ARG(a_hi && a_lo && b_hi && b_lo && c, "gemm_f32x3: null pointer");
   LLMC_CHECK_ARG(M >= 0 && N >= 0 && K > 0 && K % 8 == 0 && K <= (1 << 20), "gemm_f32x3: bad shape (K %% 8 == 0)");
   LLMC_CHECK_ARG(mode == 0 || mode == 1, "gemm_f32x3: mode must be 0 (C -= AB) or 1 (C = AB)");
-  return tf32x3_update(a_hi, a_lo, a_mn, lda, b_hi, b_lo, b_mn, ldb, c, ldc, M, N, (int)K, mode,
-                       lower_only, 0, 0, nullptr, nullptr, static_cast<cudaStream_t>(stream));
+  Tf32x3Update u{{a_hi, a_lo, lda, a_mn != 0}, {b_hi, b_lo, ldb, b_mn != 0}, c, ldc, M, N, K};
+  if (mode == 1) u.overwrite();
+  if (lower_only) u.lower_tiles(0, 0);
+  return tf32x3_update(u, static_cast<cudaStream_t>(stream));
 }
