@@ -59,14 +59,27 @@ def prepare(W, H, actorder, percdamp):
     return W, H, perm
 
 
+def tf32_split(x):
+    """hi = tf32(x), lo = tf32(x - hi) of an fp32 tensor, each rounded like cvt.rna.tf32.f32
+    (nearest, ties away from zero, to 10 mantissa bits): on the int32 view, add 0x1000 to the
+    magnitude and clear the low 13 bits.  This is the split the library's 3xTF32 updates
+    multiply (llmc_b200/csrc/tf32.cu)."""
+    def rna(v):
+        return ((v.contiguous().view(torch.int32) + 0x1000) & -0x2000).view(torch.float32)
+    hi = rna(x)
+    return hi, rna(x - hi)
+
+
 def weight_transform(W, Hinv, bit, sym, granularity, group_size=None, blocksize=128,
-                     static_qparams=None, perm=None):
+                     static_qparams=None, perm=None, trailing_split=False):
     """gptq.py:198-244.  W [R, C] fp32 (permuted), Hinv upper factor.
 
     dynamic groups (static_qparams None, per_group): qparams searched on the compensated
       columns [idx, idx+g) when idx % g == 0 (:215-223, search_column_qparams :358-366);
     static groups / per_channel: static_qparams = (scales, zeros) each a list over groups of
       [R,1] tensors (per_group, indexed perm[idx] // g, :225-227) or a single [R,1] pair.
+    trailing_split: the trailing update multiplies hi + lo of tf32_split(Err1) instead of Err1,
+      as the 3xTF32 kernel does.  The default is the reference's arithmetic.
     Returns (tmp [R,C], Losses [R,C], groups list of (scale, zero)).
     """
     W = W.clone()
@@ -104,6 +117,9 @@ def weight_transform(W, Hinv, bit, sym, granularity, group_size=None, blocksize=
             err1 = (w - q) / d
             W1[:, i:] -= err1.unsqueeze(1).matmul(Hinv1[i, i:].unsqueeze(0))
             Err1[:, i] = err1
+        if trailing_split:
+            hi, lo = tf32_split(Err1)
+            Err1 = hi + lo
         W[:, i2:] -= Err1.matmul(Hinv[i1:i2, i2:])
     return tmp, Losses, [groups[k] for k in sorted(groups)]
 

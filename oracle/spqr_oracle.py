@@ -15,6 +15,8 @@ import math
 
 import torch
 
+from .gptq_oracle import tf32_split
+
 
 def qcfg(bit, sym, round_zp=True):
     """quant.py:661-678."""
@@ -138,9 +140,10 @@ def threshold_of(Wp, Hinv, relative_threshold):
     return float(torch.tensor(thr, dtype=torch.float32)) if not math.isinf(thr) else math.inf
 
 
-def weight_transform(Wp, Hinv, cfg, blocksize=128):
+def weight_transform(Wp, Hinv, cfg, blocksize=128, trailing_split=False):
     """spqr.py:172-268 on the permuted weight.  Returns tmp, mask (uint8), scales, zeros [R, ng],
-    per-row losses."""
+    per-row losses.  trailing_split: the trailing update multiplies hi + lo of the tf32 split of
+    the block's errors, as the 3xTF32 kernel does (gptq_oracle.tf32_split)."""
     W = Wp.clone()
     R, C = W.shape
     gs = cfg['gs']
@@ -155,6 +158,9 @@ def weight_transform(Wp, Hinv, cfg, blocksize=128):
         tmp[:, i1:i2], mask[:, i1:i2] = t, m
         S[:, i1 // gs:i1 // gs + s.shape[1]], Z[:, i1 // gs:i1 // gs + s.shape[1]] = s, z
         losses = losses + l
+        if trailing_split:
+            hi, lo = tf32_split(e)
+            e = hi + lo
         W[:, i2:] -= e.matmul(Hinv[i1:i2, i2:])
     return tmp, mask, S, Z, losses
 
