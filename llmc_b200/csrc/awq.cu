@@ -11,6 +11,7 @@
 // here nothing is materialised.  Arithmetic is T-faithful (common.cuh), reductions accumulate in
 // fp32 like torch and round once.
 #include "common.cuh"
+#include "quant_math.cuh"
 
 namespace llmc {
 
@@ -142,24 +143,11 @@ __device__ __forceinline__ void group_qdq(const float (&cw)[4], int nk, int sym,
     if (lane * 4 + i < nk) { mn = fminf(mn, cw[i]); mx = fmaxf(mx, cw[i]); }
   mn = warp_min(mn);
   mx = warp_max(mx);
-  const float eps = DType<DT>::rT(1e-5f);
   float s, z;
-  if (sym) {
-    float a = fmaxf(fmaxf(fabsf(mx), fabsf(mn)), eps);
-    s = DType<DT>::rT(fdiv_rn(a, qmax));
-    z = 0.f;
-  } else {
-    float d = fmaxf(DType<DT>::rT(fsub_rn(mx, mn)), eps);
-    s = DType<DT>::rT(fdiv_rn(d, fsub_rn(qmax, qmin)));
-    z = DType<DT>::rT(fsub_rn(qmin, rintf(DType<DT>::rT(fdiv_rn(mn, s)))));
-    z = fminf(fmaxf(z, qmin), qmax);
-  }
+  qparams<DType<DT>>(mn, mx, sym, 1, qmin, qmax, s, z);
 #pragma unroll
-  for (int i = 0; i < 4; ++i) {
-    float q = rintf(DType<DT>::rT(fdiv_rn(cw[i], s))) + z;
-    q = fminf(fmaxf(q, qmin), qmax);
-    qw[i] = DType<DT>::rT(fmul_rn(q - z, s));
-  }
+  for (int i = 0; i < 4; ++i)
+    qw[i] = dequant<DType<DT>>(quant_code<DType<DT>>(cw[i], IeeeDiv{s}, z, qmin, qmax), s, z);
 }
 
 template <int DT>
@@ -279,14 +267,6 @@ awq_clip_select_kernel(const void* __restrict__ w, int64_t R, int64_t C, int gro
 
 using namespace llmc;
 
-#define DISPATCH_DT(dt, CALL)                                                        \
-  do {                                                                               \
-    if ((dt) == LLMC_F32) { CALL(LLMC_F32); }                                        \
-    else if ((dt) == LLMC_F16) { CALL(LLMC_F16); }                                   \
-    else if ((dt) == LLMC_BF16) { CALL(LLMC_BF16); }                                 \
-    else { set_last_error("bad dtype %d", (dt)); return LLMC_EINVAL; }               \
-  } while (0)
-
 extern "C" int llmc_absmean_cols(const void* x, int64_t T, int64_t C, int dtype, void* out,
                                  float* workspace, int64_t workspace_floats, void* stream) {
   LLMC_CHECK_ARG(x && out && workspace && T > 0 && C > 0, "absmean_cols: bad argument");
@@ -303,7 +283,7 @@ extern "C" int llmc_absmean_cols(const void* x, int64_t T, int64_t C, int dtype,
   LLMC_CHECK_LAUNCH();                                                                      \
   absmean_stage2<DT><<<static_cast<unsigned>((C + 255) / 256), 256, 0, st>>>(workspace, splits, T, C, out); \
   LLMC_CHECK_LAUNCH()
-  DISPATCH_DT(dtype, CALL);
+  LLMC_DISPATCH_DT("absmean_cols", dtype, CALL);
 #undef CALL
   return LLMC_OK;
 }
@@ -318,7 +298,7 @@ extern "C" int llmc_div_cols(const void* x, const void* s, int64_t T, int64_t C,
   int64_t blocks = (T * (C / 8) + 255) / 256;
   if (blocks > kNumSMs * 32) blocks = kNumSMs * 32;
 #define CALL(DT) div_cols_kernel<DT><<<(int)blocks, 256, 0, st>>>(x, s, T, C, out); LLMC_CHECK_LAUNCH()
-  DISPATCH_DT(dtype, CALL);
+  LLMC_DISPATCH_DT("div_cols", dtype, CALL);
 #undef CALL
   return LLMC_OK;
 }
@@ -332,7 +312,7 @@ extern "C" int llmc_mse(const void* a, const void* b, int64_t n, int dtype, floa
   if (blocks < 1) blocks = 1;
   if (blocks > 1024) blocks = 1024;
 #define CALL(DT) mse_stage1<DT><<<(int)blocks, 256, 0, st>>>(a, b, n, workspace); LLMC_CHECK_LAUNCH()
-  DISPATCH_DT(dtype, CALL);
+  LLMC_DISPATCH_DT("mse", dtype, CALL);
 #undef CALL
   mse_stage2<<<1, 256, 0, st>>>(workspace, (int)blocks, 1.0 / static_cast<double>(n), out);
   LLMC_CHECK_LAUNCH();
@@ -358,8 +338,7 @@ extern "C" int llmc_awq_clip(const void* w, int64_t R, int64_t C, const void* x,
   ClipArgs a{};
   a.w = w; a.x = x; a.R = R; a.C = C; a.group = static_cast<int>(group); a.ng = ng;
   a.sym = sym; a.bit = bit; a.clip_sym = clip_sym;
-  if (sym) { a.qmin = -(float)(1 << (bit - 1)); a.qmax = (float)((1 << (bit - 1)) - 1); }
-  else { a.qmin = 0.f; a.qmax = (float)((1 << bit) - 1); }
+  int_range(bit, sym, a.qmin, a.qmax);
   a.err = workspace;
   const int smem = (kClipMaxTok * (kClipG + 1) + 8 * kClipG) * 4;
   LLMC_ONCE_PER_DEVICE({
@@ -376,7 +355,7 @@ extern "C" int llmc_awq_clip(const void* w, int64_t R, int64_t C, const void* x,
     a.tok0 = static_cast<int>(t0);
     a.ntok = static_cast<int>(ns - t0 < kClipMaxTok ? ns - t0 : kClipMaxTok);
 #define CALL(DT) awq_clip_err_kernel<DT><<<grid, 256, smem, st>>>(a); LLMC_CHECK_LAUNCH()
-    DISPATCH_DT(dtype, CALL);
+    LLMC_DISPATCH_DT("awq_clip", dtype, CALL);
 #undef CALL
   }
   const int64_t total = R * ng;
@@ -384,7 +363,7 @@ extern "C" int llmc_awq_clip(const void* w, int64_t R, int64_t C, const void* x,
   awq_clip_select_kernel<DT><<<static_cast<unsigned>((total + 255) / 256), 256, 0, st>>>(          \
       w, R, C, static_cast<int>(group), ng, clip_sym, workspace, static_cast<int>(ns), best_max, best_min); \
   LLMC_CHECK_LAUNCH()
-  DISPATCH_DT(dtype, CALL);
+  LLMC_DISPATCH_DT("awq_clip", dtype, CALL);
 #undef CALL
   return LLMC_OK;
 }

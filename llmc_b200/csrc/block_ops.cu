@@ -118,14 +118,6 @@ add_kernel(const void* __restrict__ a, const void* __restrict__ b, void* __restr
 
 using namespace llmc;
 
-#define DISPATCH16(dt, CALL)                                                          \
-  do {                                                                                \
-    if ((dt) == LLMC_F16) { CALL(LLMC_F16); }                                         \
-    else if ((dt) == LLMC_BF16) { CALL(LLMC_BF16); }                                  \
-    else if ((dt) == LLMC_F32) { CALL(LLMC_F32); }                                    \
-    else { set_last_error("bad dtype %d", (dt)); return LLMC_EINVAL; }                \
-  } while (0)
-
 extern "C" int llmc_rmsnorm(const void* x, const void* weight, void* y, int64_t rows, int64_t cols,
                             float eps, int dtype, void* stream) {
   LLMC_CHECK_ARG(x && weight && y && rows >= 0 && cols > 0, "rmsnorm: bad argument");
@@ -135,7 +127,7 @@ extern "C" int llmc_rmsnorm(const void* x, const void* weight, void* y, int64_t 
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   int64_t blocks = rows < kNumSMs * 16 ? rows : kNumSMs * 16;
 #define CALL(DT) rmsnorm_kernel<DT><<<(int)blocks, 256, 0, st>>>(x, weight, y, rows, cols, eps); LLMC_CHECK_LAUNCH()
-  DISPATCH16(dtype, CALL);
+  LLMC_DISPATCH_DT("rmsnorm", dtype, CALL);
 #undef CALL
   return LLMC_OK;
 }
@@ -151,7 +143,7 @@ extern "C" int llmc_rope(void* x, const void* cosv, const void* sinv, int64_t B,
   int64_t blocks = (total + 255) / 256;
   if (blocks > kNumSMs * 32) blocks = kNumSMs * 32;
 #define CALL(DT) rope_kernel<DT><<<(int)blocks, 256, 0, st>>>(x, cosv, sinv, B, S, H, D); LLMC_CHECK_LAUNCH()
-  DISPATCH16(dtype, CALL);
+  LLMC_DISPATCH_DT("rope", dtype, CALL);
 #undef CALL
   return LLMC_OK;
 }
@@ -166,7 +158,7 @@ extern "C" int llmc_silu_mul(const void* gate, const void* up, void* y, int64_t 
   int64_t blocks = ((n >> 3) + 255) / 256;
   if (blocks > kNumSMs * 32) blocks = kNumSMs * 32;
 #define CALL(DT) silu_mul_kernel<DT><<<(int)blocks, 256, 0, st>>>(gate, up, y, n >> 3); LLMC_CHECK_LAUNCH()
-  DISPATCH16(dtype, CALL);
+  LLMC_DISPATCH_DT("silu_mul", dtype, CALL);
 #undef CALL
   return LLMC_OK;
 }
@@ -180,7 +172,7 @@ extern "C" int llmc_add(const void* a, const void* b, void* y, int64_t n, int dt
   int64_t blocks = ((n >> 3) + 255) / 256;
   if (blocks > kNumSMs * 32) blocks = kNumSMs * 32;
 #define CALL(DT) add_kernel<DT><<<(int)blocks, 256, 0, st>>>(a, b, y, n >> 3); LLMC_CHECK_LAUNCH()
-  DISPATCH16(dtype, CALL);
+  LLMC_DISPATCH_DT("add", dtype, CALL);
 #undef CALL
   return LLMC_OK;
 }

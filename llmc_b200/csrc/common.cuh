@@ -134,6 +134,28 @@ template <> struct DType<LLMC_BF16> {
   }
 };
 
+// Run-time dtype versions of DType<>::load / store and store8 (an unknown dtype means bf16).
+__device__ __forceinline__ float load_as(int dt, const void* p, int64_t i) {
+  if (dt == LLMC_F32) return DType<LLMC_F32>::load(p, i);
+  if (dt == LLMC_F16) return DType<LLMC_F16>::load(p, i);
+  return DType<LLMC_BF16>::load(p, i);
+}
+__device__ __forceinline__ void store_as(int dt, void* p, int64_t i, float v) {
+  if (dt == LLMC_F32) DType<LLMC_F32>::store(p, i, v);
+  else if (dt == LLMC_F16) DType<LLMC_F16>::store(p, i, v);
+  else DType<LLMC_BF16>::store(p, i, v);
+}
+
+// Host side: run CALL(DT) with DT the compile-time constant of the run-time dtype `dt`; an unknown
+// dtype makes the enclosing entry point fail with LLMC_EINVAL.
+#define LLMC_DISPATCH_DT(what, dt, CALL)                                            \
+  do {                                                                              \
+    if ((dt) == LLMC_F32) { CALL(LLMC_F32); }                                       \
+    else if ((dt) == LLMC_F16) { CALL(LLMC_F16); }                                  \
+    else if ((dt) == LLMC_BF16) { CALL(LLMC_BF16); }                                \
+    else { ::llmc::set_last_error("%s: bad dtype %d", what, (dt)); return LLMC_EINVAL; } \
+  } while (0)
+
 // 8 consecutive elements <-> 8 floats, vectorised (16 B for 2-byte types, 2x16 B for fp32).
 template <int DT>
 __device__ __forceinline__ void load8(const void* base, int64_t idx, float (&v)[8]) {
@@ -182,6 +204,12 @@ __device__ __forceinline__ void store8(void* base, int64_t idx, const float (&v)
     *reinterpret_cast<uint4*>(reinterpret_cast<uint16_t*>(base) + idx) =
         make_uint4(w[0], w[1], w[2], w[3]);
   }
+}
+
+__device__ __forceinline__ void store8_as(int dt, void* base, int64_t idx, const float (&v)[8]) {
+  if (dt == LLMC_F32) store8<LLMC_F32>(base, idx, v);
+  else if (dt == LLMC_F16) store8<LLMC_F16>(base, idx, v);
+  else store8<LLMC_BF16>(base, idx, v);
 }
 
 __device__ __forceinline__ float warp_max(float v, int width = 32) {

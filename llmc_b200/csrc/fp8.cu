@@ -127,16 +127,16 @@ extern "C" int llmc_fp8_quant(const void* w, int64_t rows, int64_t cols, int dty
   if (dynamic) {
     int64_t blocks = rows * a.ng;
     if (blocks > kNumSMs * 32) blocks = kNumSMs * 32;
-    if (dtype == LLMC_F32) fp8_dynamic_kernel<LLMC_F32><<<(int)blocks, 256, 0, st>>>(a);
-    else if (dtype == LLMC_F16) fp8_dynamic_kernel<LLMC_F16><<<(int)blocks, 256, 0, st>>>(a);
-    else fp8_dynamic_kernel<LLMC_BF16><<<(int)blocks, 256, 0, st>>>(a);
+#define CALL(DT) fp8_dynamic_kernel<DT><<<(int)blocks, 256, 0, st>>>(a)
+    LLMC_DISPATCH_DT("fp8_quant", dtype, CALL);
+#undef CALL
   } else {
     LLMC_CHECK_ARG(out_mode != 0, "fp8_quant: static mode needs an output");
     int64_t blocks = (rows * cols + 255) / 256;
     if (blocks > kNumSMs * 32) blocks = kNumSMs * 32;
-    if (dtype == LLMC_F32) fp8_static_kernel<LLMC_F32><<<(int)blocks, 256, 0, st>>>(a);
-    else if (dtype == LLMC_F16) fp8_static_kernel<LLMC_F16><<<(int)blocks, 256, 0, st>>>(a);
-    else fp8_static_kernel<LLMC_BF16><<<(int)blocks, 256, 0, st>>>(a);
+#define CALL(DT) fp8_static_kernel<DT><<<(int)blocks, 256, 0, st>>>(a)
+    LLMC_DISPATCH_DT("fp8_quant", dtype, CALL);
+#undef CALL
   }
   LLMC_CHECK_LAUNCH();
   return LLMC_OK;
@@ -217,10 +217,9 @@ extern "C" int llmc_fp8_block_quant(const void* w, int64_t M, int64_t N, int dty
   const int64_t nb = ((M + block - 1) / block) * ((N + block - 1) / block);
   const int grid = static_cast<int>(nb < kNumSMs * 16 ? nb : kNumSMs * 16);
   const float fmax = e5m2 ? 57344.f : 448.f;
-  if (dtype == LLMC_F32) fp8_block_quant_kernel<LLMC_F32><<<grid, 256, 0, st>>>(w, M, N, block, e5m2, fmax, scales, out_mode, out);
-  else if (dtype == LLMC_F16) fp8_block_quant_kernel<LLMC_F16><<<grid, 256, 0, st>>>(w, M, N, block, e5m2, fmax, scales, out_mode, out);
-  else if (dtype == LLMC_BF16) fp8_block_quant_kernel<LLMC_BF16><<<grid, 256, 0, st>>>(w, M, N, block, e5m2, fmax, scales, out_mode, out);
-  else { set_last_error("fp8_block_quant: bad dtype %d", dtype); return LLMC_EINVAL; }
+#define CALL(DT) fp8_block_quant_kernel<DT><<<grid, 256, 0, st>>>(w, M, N, block, e5m2, fmax, scales, out_mode, out)
+  LLMC_DISPATCH_DT("fp8_block_quant", dtype, CALL);
+#undef CALL
   LLMC_CHECK_LAUNCH();
   return LLMC_OK;
 }

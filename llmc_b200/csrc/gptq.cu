@@ -13,6 +13,7 @@
 // correctly rounded divides), so single-block problems are bit-exact; across blocks only the
 // summation order of the 128-deep trailing dot products differs from the CPU BLAS.
 #include "tc.cuh"
+#include "quant_math.cuh"
 #include "spqr_row.cuh"
 
 namespace llmc {
@@ -100,26 +101,6 @@ struct InblockArgs {
   int64_t Rpad;          // R rounded up to 128
 };
 
-__device__ __forceinline__ float load_q(const void* p, int dt, int64_t i) {
-  if (dt == LLMC_F32) return DType<LLMC_F32>::load(p, i);
-  if (dt == LLMC_F16) return DType<LLMC_F16>::load(p, i);
-  return DType<LLMC_BF16>::load(p, i);
-}
-
-__device__ __forceinline__ void qparams_f32(float mn, float mx, int sym, float qmin, float qmax,
-                                            float& s, float& z) {
-  if (sym) {
-    float a = fmaxf(fmaxf(fabsf(mx), fabsf(mn)), 1e-5f);
-    s = fdiv_rn(a, qmax);
-    z = 0.f;
-  } else {
-    float d = fmaxf(fsub_rn(mx, mn), 1e-5f);
-    s = fdiv_rn(d, fsub_rn(qmax, qmin));
-    z = fsub_rn(qmin, rintf(fdiv_rn(mn, s)));
-    z = fminf(fmaxf(z, qmin), qmax);
-  }
-}
-
 // A row is spread over 8 lanes (lane l owns columns l, l+8, ...), 32 rows per CTA, 256 threads,
 // two CTAs per SM (one thread per row would give R = 4096 only 32 CTAs, one warp per scheduler):
 //   * per 8-column sub-block each lane keeps ITS column in a register; the eight sequential
@@ -127,43 +108,14 @@ __device__ __forceinline__ void qparams_f32(float mn, float mx, int sym, float q
 //   * the other columns of the row stay in shared memory and receive the sub-block's eight
 //     updates lazily, in the reference's order (same op sequence per element as gptq.py:240);
 //   * x / s with s fixed is evaluated as a reciprocal multiply plus two FMA corrections
-//     (div_by below), which is the correctly rounded quotient, at a third of div.rn's cost.
+//     (MarksteinDiv, quant_math.cuh), which is the correctly rounded quotient, at a third of
+//     div.rn's cost.
 constexpr int IR = 32;            // rows per CTA
 constexpr int IL = 8;             // lanes per row
 constexpr int WP = GB + 8;        // pitch of the row-major W tile: 4 rows x 8 lanes hit 32 banks
 constexpr int EP = IR + 1;        // pitch of the transposed err tile
 constexpr int HP = GB + 4;        // pitch of the row-major Hinv block
 constexpr int kInblockSmem = (IR * WP + GB * EP + GB * HP + 2 * GB) * 4;
-
-// RN(x / s) given r = RN(1 / s).  q1 is a faithful quotient (residual-corrected once), and the
-// second correction of a faithful quotient with a correctly rounded reciprocal is the correctly
-// rounded quotient (Markstein), provided nothing under/overflows: x, s and r with exponents in
-// [2^-40, 2^41) keep q and both residuals normal (x = 0 is exact as well).  Anything else takes
-// div.rn, kept OUT of line: inlined, its ~10-instruction sequence sat on the dependent chain of
-// every column step whether or not it was needed.
-__device__ __noinline__ float div_exact_slow(float x, float s) { return fdiv_rn(x, s); }
-
-__device__ __forceinline__ bool exp_mid(float v) {
-  return (((__float_as_uint(v) >> 23) & 0xffu) - 87u) <= 80u;
-}
-
-// sr_ok = exp_mid(s) && exp_mid(r): a property of the divisor, evaluated once by the caller
-__device__ __forceinline__ float div_by(float x, float s, float r, bool sr_ok) {
-  const float q0 = fmul_rn(x, r);
-  float rem = fma_rn(-q0, s, x);
-  const float q1 = fma_rn(rem, r, q0);
-  rem = fma_rn(-q1, s, x);
-  float q2 = fma_rn(rem, r, q1);
-  if (!(sr_ok && (exp_mid(x) || x == 0.f))) q2 = div_exact_slow(x, s);
-  return q2;
-}
-
-__device__ __forceinline__ float qdq_f32_r(float w, float s, float rs, bool s_ok, float z, float qmin,
-                                           float qmax) {
-  float q = rintf(div_by(w, s, rs, s_ok)) + z;
-  q = fminf(fmaxf(q, qmin), qmax);
-  return fmul_rn(q - z, s);
-}
 
 __device__ __forceinline__ float group8_min(float v) {
   v = fminf(v, __shfl_xor_sync(0xffffffffu, v, 1));
@@ -268,7 +220,7 @@ gptq_inblock_kernel(InblockArgs a) {
           mn = 0.f; mx = 0.f;
         }
         mn = group8_min(mn); mx = group8_max(mx);
-        qparams_f32(mn, mx, a.sym, a.qmin, a.qmax, s_cur, z_cur);
+        qparams<F32Round>(mn, mx, a.sym, 1, a.qmin, a.qmax, s_cur, z_cur);
         if (live && l == 0) {
           reinterpret_cast<float*>(a.scales)[row * a.ng + gi] = s_cur;
           if (!a.sym) reinterpret_cast<float*>(a.zeros)[row * a.ng + gi] = z_cur;
@@ -285,7 +237,7 @@ gptq_inblock_kernel(InblockArgs a) {
           const int cend = min((g + 1) * gsz, cnt);
           for (int c = g * gsz + l; c < cend; c += IL) { const float v = Wr[rg * WP + c]; mn = fminf(mn, v); mx = fmaxf(mx, v); }
           mn = group8_min(mn); mx = group8_max(mx);
-          qparams_f32(mn, mx, a.sym, a.qmin, a.qmax, s_small[g], z_small[g]);
+          qparams<F32Round>(mn, mx, a.sym, 1, a.qmin, a.qmax, s_small[g], z_small[g]);
           if (live && l == 0) {
             const int64_t gi = (a.i1 + g * gsz) / a.group;
             reinterpret_cast<float*>(a.scales)[row * a.ng + gi] = s_small[g];
@@ -295,8 +247,8 @@ gptq_inblock_kernel(InblockArgs a) {
       }
     }
   } else if (live && a.group >= a.C) {
-    s_cur = load_q(a.scales, a.q_dtype, row);                 // per_channel
-    z_cur = a.zeros ? load_q(a.zeros, a.q_dtype, row) : 0.f;
+    s_cur = load_as(a.q_dtype, a.scales, row);                 // per_channel
+    z_cur = a.zeros ? load_as(a.q_dtype, a.zeros, row) : 0.f;
   }
   __syncthreads();                         // dd / rd
 
@@ -314,25 +266,24 @@ gptq_inblock_kernel(InblockArgs a) {
     } else if (!dynamic && a.group < a.C && live && col_live) {
       const int64_t idx = static_cast<int64_t>(a.i1) + c_own;
       const int64_t gi = a.gmap ? a.gmap[idx] : idx / a.group;     // gptq.py:225-227
-      s = load_q(a.scales, a.q_dtype, row * a.ng + gi);
-      z = a.zeros ? load_q(a.zeros, a.q_dtype, row * a.ng + gi) : 0.f;
+      s = load_as(a.q_dtype, a.scales, row * a.ng + gi);
+      z = a.zeros ? load_as(a.q_dtype, a.zeros, row * a.ng + gi) : 0.f;
     }
-    const float rs = __frcp_rn(s);
-    const bool s_ok = exp_mid(s) && exp_mid(rs);
+    const MarksteinDiv div_s(s);
     float wc = Wr[rg * WP + c_own];
     float hd[IL];
 #pragma unroll
     for (int jj = 0; jj < IL; ++jj) hd[jj] = Hs[(cb + jj) * HP + c_own];
-    const float d = dd[c_own], rdv = rd[c_own];
-    const bool d_ok = exp_mid(d) && exp_mid(rdv);
+    const float d = dd[c_own];
+    const MarksteinDiv div_d(d, rd[c_own]);
     float ev[IL];
     float my_err = 0.f, my_diff = 0.f;
     // the eight sequential columns of the sub-block: lane jj's column is final at step jj
 #pragma unroll
     for (int jj = 0; jj < IL; ++jj) {
-      const float q = qdq_f32_r(wc, s, rs, s_ok, z, a.qmin, a.qmax);
+      const float q = dequant<F32Round>(quant_code<F32Round>(wc, div_s, z, a.qmin, a.qmax), s, z);
       const float diff = fsub_rn(wc, q);
-      float err = div_by(diff, d, rdv, d_ok);                                       // :239
+      float err = div_d(diff);                                                      // :239
       if (!col_live) err = 0.f;
       const float e = __shfl_sync(0xffffffffu, err, jj, IL);
       ev[jj] = e;
@@ -492,7 +443,7 @@ spqr_inblock_kernel(SpqrArgs a) {
     if (live && lane == 0) {
       Et[col * SEP + rr] = err;
       Ms[rr * GB + col] = m;
-      loss = spqr::add(loss, spqr::mul(err, err));
+      loss = add(loss, mul(err, err));
     }
     __syncwarp();
   }
@@ -612,10 +563,9 @@ extern "C" int llmc_gptq_prepare(const float* H, int64_t C, const int64_t* perm,
   LLMC_CHECK_LAUNCH();
   // W first: it reads the ORIGINAL diagonal of H (dead test), Hp may alias neither H nor W
   if (W != nullptr) {
-    if (w_dtype == LLMC_F32) gather_w_kernel<LLMC_F32><<<(unsigned)R, 256, smem, st>>>(W, R, C, H, perm, Wp);
-    else if (w_dtype == LLMC_F16) gather_w_kernel<LLMC_F16><<<(unsigned)R, 256, smem, st>>>(W, R, C, H, perm, Wp);
-    else if (w_dtype == LLMC_BF16) gather_w_kernel<LLMC_BF16><<<(unsigned)R, 256, smem, st>>>(W, R, C, H, perm, Wp);
-    else { set_last_error("gptq_prepare: bad dtype %d", w_dtype); return LLMC_EINVAL; }
+#define CALL(DT) gather_w_kernel<DT><<<(unsigned)R, 256, smem, st>>>(W, R, C, H, perm, Wp)
+    LLMC_DISPATCH_DT("gptq_prepare", w_dtype, CALL);
+#undef CALL
     LLMC_CHECK_LAUNCH();
   }
   if (Hp != nullptr) {
@@ -770,8 +720,7 @@ extern "C" int llmc_gptq_colblock(float* W, const float* Hinv, int64_t R, int64_
   InblockArgs a{};
   a.W = W; a.Hinv = Hinv; a.R = R; a.C = C;
   a.group = group; a.ng = C / group; a.sym = sym;
-  if (sym) { a.qmin = -(float)(1 << (bit - 1)); a.qmax = (float)((1 << (bit - 1)) - 1); }
-  else { a.qmin = 0.f; a.qmax = (float)((1 << bit) - 1); }
+  int_range(bit, sym, a.qmin, a.qmax);
   a.static_groups = static_groups; a.gmap = gmap;
   a.scales = scales; a.zeros = sym ? nullptr : zeros; a.q_dtype = q_dtype;
   a.tmp = tmp; a.out_perm = out_perm; a.losses = losses;
@@ -788,8 +737,7 @@ extern "C" int llmc_gptq_colblock(float* W, const float* Hinv, int64_t R, int64_
 
 static spqr::QCfg spqr_qcfg(int bit, int sym, int round_zp) {
   spqr::QCfg q{};
-  if (sym) { q.qmin = -static_cast<float>(1 << (bit - 1)); q.qmax = static_cast<float>((1 << (bit - 1)) - 1); }
-  else { q.qmin = 0.f; q.qmax = static_cast<float>((1 << bit) - 1); }
+  int_range(bit, sym, q.qmin, q.qmax);
   q.sym = sym; q.round_zp = round_zp;
   return q;
 }

@@ -32,11 +32,7 @@ pack_awq_kernel(const void* __restrict__ w, int64_t R, int64_t C, const void* __
     if (r < R && c < C) {
       const int64_t g = c / group;
       // scales.t().contiguous().to(torch.float16)  (:1008)
-      float s;
-      if (s_dtype == LLMC_F32) s = DType<LLMC_F32>::load(scales, r * ng + g);
-      else if (s_dtype == LLMC_F16) s = DType<LLMC_F16>::load(scales, r * ng + g);
-      else s = DType<LLMC_BF16>::load(scales, r * ng + g);
-      s = DType<LLMC_F16>::rT(s);
+      const float s = DType<LLMC_F16>::rT(load_as(s_dtype, scales, r * ng + g));
       const float z = static_cast<float>(zeros[r * ng + g]);
       const float sz = DType<LLMC_F16>::rT(fmul_rn(z, s));  // int32 * fp16 -> fp16 (:1011)
       const float x = DType<WT>::load(w, r * C + c);
@@ -79,11 +75,7 @@ pack_awq_qparams_kernel(const void* __restrict__ scales, int s_dtype,
   for (int64_t i = static_cast<int64_t>(blockIdx.x) * blockDim.x + threadIdx.x; i < total;
        i += static_cast<int64_t>(gridDim.x) * blockDim.x) {
     const int64_t g = i / R, r = i - g * R;
-    float s;
-    if (s_dtype == LLMC_F32) s = DType<LLMC_F32>::load(scales, r * ng + g);
-    else if (s_dtype == LLMC_F16) s = DType<LLMC_F16>::load(scales, r * ng + g);
-    else s = DType<LLMC_BF16>::load(scales, r * ng + g);
-    scales_out[i] = __float2half_rn(s);
+    scales_out[i] = __float2half_rn(load_as(s_dtype, scales, r * ng + g));
     if ((r & 7) == 0) {
       const int order[8] = {0, 2, 4, 6, 1, 3, 5, 7};
       uint32_t word = 0;
@@ -112,16 +104,9 @@ extern "C" int llmc_pack_awq(const void* w, int64_t R, int64_t C, int dtype, con
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   const int64_t ng = C / group;
   dim3 grid((unsigned)((C + kTileC - 1) / kTileC), (unsigned)((R + kTileR - 1) / kTileR));
-  if (dtype == LLMC_F16)
-    pack_awq_kernel<LLMC_F16><<<grid, 256, 0, st>>>(w, R, C, scales, s_dtype, zeros, group, ng, qweight);
-  else if (dtype == LLMC_BF16)
-    pack_awq_kernel<LLMC_BF16><<<grid, 256, 0, st>>>(w, R, C, scales, s_dtype, zeros, group, ng, qweight);
-  else if (dtype == LLMC_F32)
-    pack_awq_kernel<LLMC_F32><<<grid, 256, 0, st>>>(w, R, C, scales, s_dtype, zeros, group, ng, qweight);
-  else {
-    set_last_error("pack_awq: bad dtype %d", dtype);
-    return LLMC_EINVAL;
-  }
+#define CALL(DT) pack_awq_kernel<DT><<<grid, 256, 0, st>>>(w, R, C, scales, s_dtype, zeros, group, ng, qweight)
+  LLMC_DISPATCH_DT("pack_awq", dtype, CALL);
+#undef CALL
   LLMC_CHECK_LAUNCH();
   int64_t total = ng * R;
   int64_t blocks = (total + 255) / 256;

@@ -7,7 +7,10 @@
 // HBM-bound integer/byte work: one pass over W with 16-byte loads, qparams in registers,
 // 4..32-byte stores.  Bit-exactness against torch comes from reproducing torch's rounding
 // points ("T-faithful", common.cuh) — see DESIGN.md §numerics.
+#include <type_traits>
+
 #include "common.cuh"
+#include "quant_math.cuh"
 
 namespace llmc {
 
@@ -28,75 +31,10 @@ struct QuantArgs {
   const void* col_scale;   // optional [cols] DT: w' = rT(w * s[c]) first (AWQ, awq.py:39-46)
 };
 
-// torch: tensor.clamp(min=1e-5) converts the python scalar to the tensor dtype first.
+// x / s, correctly rounded to fp32 (then the caller rounds to T): the reciprocal divider for
+// 16-bit operands, the IEEE divide for fp32 (quant_math.cuh).
 template <int DT>
-__device__ __forceinline__ float eps_T() { return DType<DT>::rT(1e-5f); }
-
-// quant.py:545-559 (get_qparams), T-faithful.
-template <int DT>
-__device__ __forceinline__ void compute_qparams(float mn, float mx, int sym, float qmin,
-                                                float qmax, float& s, float& z) {
-  using D = DType<DT>;
-  if (sym) {
-    float a = fmaxf(fabsf(mx), fabsf(mn));
-    a = fmaxf(a, eps_T<DT>());
-    s = D::rT(fdiv_rn(a, qmax));
-    z = 0.f;
-  } else {
-    float d = D::rT(fsub_rn(mx, mn));
-    d = fmaxf(d, eps_T<DT>());
-    s = D::rT(fdiv_rn(d, fsub_rn(qmax, qmin)));
-    float t = rintf(D::rT(fdiv_rn(mn, s)));
-    z = D::rT(fsub_rn(qmin, t));
-    z = fminf(fmaxf(z, qmin), qmax);
-  }
-}
-
-// x / s, correctly rounded to fp32 (then the caller rounds to T).
-// For 16-bit T both x and s carry <= 11 significant bits, so q0 = RN(x*r), r = RN(1/s),
-// followed by one exact-remainder correction is the correctly rounded quotient (the
-// remainder x - q0*s is exact in fp32 and the corrected value is within 2^-47 of x/s while
-// fp32 rounding boundaries are >= 2^-36 away; DESIGN.md).  fp32 uses the IEEE divide.
-template <int DT>
-struct Divider {
-  float s, r;
-  __device__ __forceinline__ explicit Divider(float s_) : s(s_), r(fdiv_rn(1.0f, s_)) {}
-  __device__ __forceinline__ float operator()(float x) const {
-    if constexpr (DT == LLMC_F32) {
-      return fdiv_rn(x, s);
-    } else {
-      float q0 = fmul_rn(x, r);
-      float rem = fma_rn(-q0, s, x);
-      return fma_rn(rem, r, q0);
-    }
-  }
-};
-
-// quant.py:699-701: clamp(round(x / s) + z, qmin, qmax)  — returns the integer-valued code.
-template <int DT, int DV = DT>
-__device__ __forceinline__ float quant_code(float x, const Divider<DV>& div, float z,
-                                            float qmin, float qmax) {
-  float q = rintf(DType<DT>::rT(div(x)));
-  q = q + z;  // integers: exact whenever the result survives the clamp
-  return fminf(fmaxf(q, qmin), qmax);
-}
-
-// round_zp = False (quant.py:702-707, HQQ's real-valued zero-points):
-//   clamp(round(x / s.clamp_min(1e-9) + z), qmin, qmax) — the zero-point goes INSIDE the rounding.
-// `div` must have been built from the clamped scale.
-template <int DT, int DV = DT>
-__device__ __forceinline__ float quant_code_zp(float x, const Divider<DV>& div, float z,
-                                               float qmin, float qmax) {
-  float t = DType<DT>::rT(div(x));
-  t = DType<DT>::rT(fadd_rn(t, z));
-  return fminf(fmaxf(rintf(t), qmin), qmax);
-}
-
-// quant.py:710-712: (q - z) * s
-template <int DT>
-__device__ __forceinline__ float dequant_val(float q, float s, float z) {
-  return DType<DT>::rT(fmul_rn(q - z, s));
-}
+using Divider = std::conditional_t<DT == LLMC_F32, IeeeDiv, RecipDiv>;
 
 // Emit 8 consecutive codes/values of row r starting at column c (c % 8 == 0).
 template <int DT>
@@ -106,11 +44,8 @@ __device__ __forceinline__ void emit8(const QuantArgs& a, int64_t r, int64_t c,
     case LLMC_OUT_QDQ: {
       float y[8];
 #pragma unroll
-      for (int i = 0; i < 8; ++i) y[i] = dequant_val<DT>(q[i], s, z);
-      int64_t idx = r * a.ld_out + c;
-      if (a.out_dtype == LLMC_F32) store8<LLMC_F32>(a.out, idx, y);
-      else if (a.out_dtype == LLMC_F16) store8<LLMC_F16>(a.out, idx, y);
-      else store8<LLMC_BF16>(a.out, idx, y);
+      for (int i = 0; i < 8; ++i) y[i] = dequant<DType<DT>>(q[i], s, z);
+      store8_as(a.out_dtype, a.out, r * a.ld_out + c, y);
       break;
     }
     case LLMC_OUT_CODES_I8:
@@ -196,20 +131,20 @@ quant_dynamic_warp_kernel(QuantArgs a, int lpg, int64_t total_groups) {
     mn = warp_min(mn, lpg);
     mx = warp_max(mx, lpg);
     float s, z;
-    compute_qparams<DT>(mn, mx, a.sym, a.qmin, a.qmax, s, z);
+    qparams<DType<DT>>(mn, mx, a.sym, 1, a.qmin, a.qmax, s, z);
     if (active && sub == 0) {
       D::store(a.scales, g, s);
       if (!a.sym && a.zeros) D::store(a.zeros, g, z);
     }
     if (a.out_mode == LLMC_OUT_NONE) continue;
-    const Divider<DT> div(s);
+    const Divider<DT> div{s};
 #pragma unroll
     for (int c = 0; c < CH; ++c) {
       const int ch = c * lpg + sub;
       if (active && ch < chunks) {
         float q[8];
 #pragma unroll
-        for (int i = 0; i < 8; ++i) q[i] = quant_code<DT>(v[c][i], div, z, a.qmin, a.qmax);
+        for (int i = 0; i < 8; ++i) q[i] = quant_code<DType<DT>>(v[c][i], div, z, a.qmin, a.qmax);
         emit8<DT>(a, r, col0 + ch * 8, q, s, z);
       }
     }
@@ -254,13 +189,13 @@ quant_dynamic_block_kernel(QuantArgs a, int64_t total_groups) {
     }
     block_minmax(mn, mx);
     float s, z;
-    compute_qparams<DT>(mn, mx, a.sym, a.qmin, a.qmax, s, z);
+    qparams<DType<DT>>(mn, mx, a.sym, 1, a.qmin, a.qmax, s, z);
     if (threadIdx.x == 0) {
       D::store(a.scales, g, s);
       if (!a.sym && a.zeros) D::store(a.zeros, g, z);
     }
     if (a.out_mode == LLMC_OUT_NONE) continue;
-    const Divider<DT> div(s);
+    const Divider<DT> div{s};
     for (int ch = threadIdx.x; ch < chunks; ch += blockDim.x) {
       float v[8], q[8];
       load8<DT>(a.w, base + ch * 8, v);
@@ -271,7 +206,7 @@ quant_dynamic_block_kernel(QuantArgs a, int64_t total_groups) {
         for (int i = 0; i < 8; ++i) v[i] = D::rT(fmul_rn(v[i], cs[i]));
       }
 #pragma unroll
-      for (int i = 0; i < 8; ++i) q[i] = quant_code<DT>(v[i], div, z, a.qmin, a.qmax);
+      for (int i = 0; i < 8; ++i) q[i] = quant_code<DType<DT>>(v[i], div, z, a.qmin, a.qmax);
       emit8<DT>(a, r, j * a.group + ch * 8, q, s, z);
     }
   }
@@ -293,7 +228,7 @@ qparams_generic_kernel(QuantArgs a, int64_t total_groups) {
     }
     block_minmax(mn, mx);
     float s, z;
-    compute_qparams<DT>(mn, mx, a.sym, a.qmin, a.qmax, s, z);
+    qparams<DType<DT>>(mn, mx, a.sym, 1, a.qmin, a.qmax, s, z);
     if (threadIdx.x == 0) {
       D::store(a.scales, g, s);
       if (!a.sym && a.zeros) D::store(a.zeros, g, z);
@@ -343,7 +278,7 @@ quant_static_kernel(StaticArgs a) {
     const int off = 1 << (a.bit - 1);
     int64_t last_g = -1;
     float s = 1.f, z = 0.f;
-    Divider<LLMC_DV> div(1.f);
+    Divider<LLMC_DV> div{1.f};
     for (int i = 0; i < a.unit; ++i) {
       const int64_t c = c0 + i;
       if (c >= a.cols) break;
@@ -351,19 +286,15 @@ quant_static_kernel(StaticArgs a) {
       if (g != last_g) {
         s = DType<QT>::load(a.scales, r * a.q_row_stride + g);
         z = a.zeros ? DType<QT>::load(a.zeros, r * a.q_row_stride + g) : 0.f;
-        div = Divider<LLMC_DV>(a.zp_inside ? fmaxf(s, 1e-9f) : s);
+        div = Divider<LLMC_DV>{a.zp_inside ? fmaxf(s, 1e-9f) : s};
         last_g = g;
       }
       const float x = load_w<WT>(a.w, r * a.ld + c);
-      const float q = a.zp_inside ? quant_code_zp<CT, LLMC_DV>(x, div, z, a.qmin, a.qmax)
-                                  : quant_code<CT, LLMC_DV>(x, div, z, a.qmin, a.qmax);
+      const float q = a.zp_inside ? quant_code_zp<DType<CT>>(x, div, z, a.qmin, a.qmax)
+                                  : quant_code<DType<CT>>(x, div, z, a.qmin, a.qmax);
       switch (a.out_mode) {
         case LLMC_OUT_QDQ: {
-          const float y = dequant_val<CT>(q, s, z);
-          const int64_t idx = r * a.ld_out + c;
-          if (a.out_dtype == LLMC_F32) DType<LLMC_F32>::store(a.out, idx, y);
-          else if (a.out_dtype == LLMC_F16) DType<LLMC_F16>::store(a.out, idx, y);
-          else DType<LLMC_BF16>::store(a.out, idx, y);
+          store_as(a.out_dtype, a.out, r * a.ld_out + c, dequant<DType<CT>>(q, s, z));
           break;
         }
         case LLMC_OUT_CODES_I8:
@@ -402,11 +333,11 @@ quant_static_vec8_kernel(StaticArgs a, QuantArgs e) {
       const int64_t g = c0 / a.group;
       const float s = DType<QT>::load(a.scales, r * a.q_row_stride + g);
       const float z = a.zeros ? DType<QT>::load(a.zeros, r * a.q_row_stride + g) : 0.f;
-      const Divider<LLMC_DV> div(a.zp_inside ? fmaxf(s, 1e-9f) : s);
+      const Divider<LLMC_DV> div{a.zp_inside ? fmaxf(s, 1e-9f) : s};
 #pragma unroll
       for (int i = 0; i < 8; ++i)
-        q[i] = a.zp_inside ? quant_code_zp<CT, LLMC_DV>(x[i], div, z, a.qmin, a.qmax)
-                           : quant_code<CT, LLMC_DV>(x[i], div, z, a.qmin, a.qmax);
+        q[i] = a.zp_inside ? quant_code_zp<DType<CT>>(x[i], div, z, a.qmin, a.qmax)
+                           : quant_code<DType<CT>>(x[i], div, z, a.qmin, a.qmax);
       emit8<CT>(e, r, c0, q, s, z);
     } else {
       // act-order gather: every column may belong to a different group; only QDQ/CODES.
@@ -416,16 +347,13 @@ quant_static_vec8_kernel(StaticArgs a, QuantArgs e) {
         const int64_t g = a.gmap[c0 + i];
         const float s = DType<QT>::load(a.scales, r * a.q_row_stride + g);
         const float z = a.zeros ? DType<QT>::load(a.zeros, r * a.q_row_stride + g) : 0.f;
-        const Divider<LLMC_DV> div(a.zp_inside ? fmaxf(s, 1e-9f) : s);
-        q[i] = a.zp_inside ? quant_code_zp<CT, LLMC_DV>(x[i], div, z, a.qmin, a.qmax)
-                           : quant_code<CT, LLMC_DV>(x[i], div, z, a.qmin, a.qmax);
-        y[i] = dequant_val<CT>(q[i], s, z);
+        const Divider<LLMC_DV> div{a.zp_inside ? fmaxf(s, 1e-9f) : s};
+        q[i] = a.zp_inside ? quant_code_zp<DType<CT>>(x[i], div, z, a.qmin, a.qmax)
+                           : quant_code<DType<CT>>(x[i], div, z, a.qmin, a.qmax);
+        y[i] = dequant<DType<CT>>(q[i], s, z);
       }
       if (a.out_mode == LLMC_OUT_QDQ) {
-        const int64_t idx = r * a.ld_out + c0;
-        if (a.out_dtype == LLMC_F32) store8<LLMC_F32>(a.out, idx, y);
-        else if (a.out_dtype == LLMC_F16) store8<LLMC_F16>(a.out, idx, y);
-        else store8<LLMC_BF16>(a.out, idx, y);
+        store8_as(a.out_dtype, a.out, r * a.ld_out + c0, y);
       } else {
         emit8<CT>(e, r, c0, q, 1.f, 0.f);
       }
@@ -661,7 +589,7 @@ quant_group_fast_kernel(QuantArgs a, int64_t total_groups) {
       const float mn = fminf(lo_f<DT>(mn2), hi_f<DT>(mn2));
       const float mx = fmaxf(lo_f<DT>(mx2), hi_f<DT>(mx2));
       float s, z;
-      compute_qparams<DT>(mn, mx, a.sym, a.qmin, a.qmax, s, z);
+      qparams<DType<DT>>(mn, mx, a.sym, 1, a.qmin, a.qmax, s, z);
       DType<DT>::store(a.scales, g, s);
       if (!a.sym && a.zeros) DType<DT>::store(a.zeros, g, z);
       if constexpr (MODE != M_NONE) {
@@ -672,7 +600,7 @@ quant_group_fast_kernel(QuantArgs a, int64_t total_groups) {
         // bounds is clamp(rint + z, qmin, qmax); the float BITS of the clamped v are
         // 0x4B400000 + (code + OFFE - o), which the integer packing below consumes directly
         // (multiply-add chain, the constant parts subtracted once per word).
-        const Divider<DT> div(s);
+        const Divider<DT> div{s};
         float Ce, vlo, vhi;
         uint32_t ob;
         fast_consts<MODE, BITS>(z, a.qmin, a.qmax, a.sym, Ce, vlo, vhi, ob);
@@ -770,13 +698,13 @@ quant_row_fast_kernel(QuantArgs a) {
     const float mn = fminf(lo_f<DT>(mn2), hi_f<DT>(mn2));
     const float mx = fmaxf(lo_f<DT>(mx2), hi_f<DT>(mx2));
     float s, z;
-    compute_qparams<DT>(mn, mx, a.sym, a.qmin, a.qmax, s, z);
+    qparams<DType<DT>>(mn, mx, a.sym, 1, a.qmin, a.qmax, s, z);
     if (t == 0) {
       DType<DT>::store(a.scales, r, s);
       if (!a.sym && a.zeros) DType<DT>::store(a.zeros, r, z);
     }
     if constexpr (MODE != M_NONE) {
-      const Divider<DT> div(s);
+      const Divider<DT> div{s};
       float Ce, vlo, vhi;
       uint32_t ob;
       fast_consts<MODE, BITS>(z, a.qmin, a.qmax, a.sym, Ce, vlo, vhi, ob);
@@ -997,8 +925,7 @@ extern "C" int llmc_quant_dynamic(const void* w, int64_t rows, int64_t cols, int
   a.group = group; a.ng = cols / group;
   a.sym = sym; a.bit = bit;
   if (use_range) { a.qmin = (float)qmin; a.qmax = (float)qmax; }
-  else if (sym) { a.qmin = -(float)(1 << (bit - 1)); a.qmax = (float)((1 << (bit - 1)) - 1); }
-  else { a.qmin = 0.f; a.qmax = (float)((1 << bit) - 1); }
+  else int_range(bit, sym, a.qmin, a.qmax);
   a.scales = scales; a.zeros = zeros; a.col_scale = col_scale;
   a.out_mode = out_mode; a.out = out;
   a.ld_out = (out_mode == LLMC_OUT_QDQ) ? (ld_out > 0 ? ld_out : cols) : cols;
@@ -1010,24 +937,22 @@ extern "C" int llmc_quant_dynamic(const void* w, int64_t rows, int64_t cols, int
   const bool vec_ok = pack_fast && (group % 8 == 0) && (ld % 8 == 0) && aligned16(w) &&
                       (out == nullptr || aligned16(out)) &&
                       (out_mode != LLMC_OUT_QDQ || a.ld_out % 8 == 0);
-  int rc = LLMC_EUNSUPPORTED;
   if (col_scale != nullptr && !(vec_ok && aligned16(col_scale))) {
     set_last_error("quant_dynamic: col_scale needs the vectorised path (group, ld %% 8 == 0, aligned)");
     return LLMC_EUNSUPPORTED;
   }
   if (vec_ok) {
-    if (dtype == LLMC_F32) rc = launch_dynamic<LLMC_F32>(a, true, st);
-    else if (dtype == LLMC_F16) rc = launch_dynamic<LLMC_F16>(a, true, st);
-    else rc = launch_dynamic<LLMC_BF16>(a, true, st);
-    return rc;
+#define CALL(DT) return launch_dynamic<DT>(a, true, st)
+    LLMC_DISPATCH_DT("quant_dynamic", dtype, CALL);
+#undef CALL
   }
   // generic: qparams kernel, then the scalar static kernel
   {
     int64_t total_groups = rows * a.ng;
     int64_t blocks = total_groups < kNumSMs * 32 ? total_groups : kNumSMs * 32;
-    if (dtype == LLMC_F32) qparams_generic_kernel<LLMC_F32><<<(int)blocks, 256, 0, st>>>(a, total_groups);
-    else if (dtype == LLMC_F16) qparams_generic_kernel<LLMC_F16><<<(int)blocks, 256, 0, st>>>(a, total_groups);
-    else qparams_generic_kernel<LLMC_BF16><<<(int)blocks, 256, 0, st>>>(a, total_groups);
+#define CALL(DT) qparams_generic_kernel<DT><<<(int)blocks, 256, 0, st>>>(a, total_groups)
+    LLMC_DISPATCH_DT("quant_dynamic", dtype, CALL);
+#undef CALL
     LLMC_CHECK_LAUNCH();
   }
   if (out_mode == LLMC_OUT_NONE) return LLMC_OK;
@@ -1092,19 +1017,11 @@ extern "C" int llmc_minmax_tensor(const void* w, int64_t n, int dtype, void* mm,
   int64_t blocks = ((n >> 3) + 255) / 256;
   if (blocks < 1) blocks = 1;
   if (blocks > 1024) blocks = 1024;
-  if (dtype == LLMC_F32) {
-    minmax_stage1<LLMC_F32><<<(int)blocks, 256, 0, st>>>(w, n, workspace);
-    minmax_stage2<LLMC_F32><<<1, 256, 0, st>>>(workspace, (int)blocks, mm);
-  } else if (dtype == LLMC_F16) {
-    minmax_stage1<LLMC_F16><<<(int)blocks, 256, 0, st>>>(w, n, workspace);
-    minmax_stage2<LLMC_F16><<<1, 256, 0, st>>>(workspace, (int)blocks, mm);
-  } else if (dtype == LLMC_BF16) {
-    minmax_stage1<LLMC_BF16><<<(int)blocks, 256, 0, st>>>(w, n, workspace);
-    minmax_stage2<LLMC_BF16><<<1, 256, 0, st>>>(workspace, (int)blocks, mm);
-  } else {
-    set_last_error("minmax_tensor: bad dtype %d", dtype);
-    return LLMC_EINVAL;
-  }
+#define CALL(DT)                                                                \
+  minmax_stage1<DT><<<(int)blocks, 256, 0, st>>>(w, n, workspace);              \
+  minmax_stage2<DT><<<1, 256, 0, st>>>(workspace, (int)blocks, mm)
+  LLMC_DISPATCH_DT("minmax_tensor", dtype, CALL);
+#undef CALL
   LLMC_CHECK_LAUNCH();
   return LLMC_OK;
 }

@@ -151,10 +151,7 @@ extern "C" int llmc_mse_range(const void* w, int64_t rows, int64_t cols, int dty
 #define CALL(DT)                                                                                  \
   rg::mse_range_kernel<DT><<<(int)grid_x, rg::kThreads, smem, st>>>(                              \
       w, rows, cols, sym, (float)qmin, (float)qmax, steps, grid, norm, kCacheCols, min_out, max_out)
-  if (dtype == LLMC_F32) CALL(LLMC_F32);
-  else if (dtype == LLMC_F16) CALL(LLMC_F16);
-  else if (dtype == LLMC_BF16) CALL(LLMC_BF16);
-  else { set_last_error("mse_range: bad dtype %d", dtype); return LLMC_EINVAL; }
+  LLMC_DISPATCH_DT("mse_range", dtype, CALL);
 #undef CALL
   LLMC_CHECK_LAUNCH();
   return LLMC_OK;
@@ -172,10 +169,7 @@ extern "C" int llmc_histc(const void* x, int64_t n, int dtype, int bins, float l
   if (blocks > kNumSMs * 8) blocks = kNumSMs * 8;
   const int smem = bins * 4;
 #define CALL(DT) rg::histc_kernel<DT><<<(int)blocks, 256, smem, st>>>(x, n, lo, hi, bins, hist)
-  if (dtype == LLMC_F32) CALL(LLMC_F32);
-  else if (dtype == LLMC_F16) CALL(LLMC_F16);
-  else if (dtype == LLMC_BF16) CALL(LLMC_BF16);
-  else { set_last_error("histc: bad dtype %d", dtype); return LLMC_EINVAL; }
+  LLMC_DISPATCH_DT("histc", dtype, CALL);
 #undef CALL
   LLMC_CHECK_LAUNCH();
   return LLMC_OK;

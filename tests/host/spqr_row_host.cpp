@@ -1,37 +1,20 @@
-// Host build of llmc_b200/csrc/spqr_row.cuh for tests/test_oracle_golden.py: the SAME source the
-// CUDA kernel spqr_inblock_kernel compiles for the device, driven row by row on the CPU so that
-// its arithmetic can be compared bit for bit with oracle/spqr_oracle.py (and, through it, with
-// the reference-generated goldens).  The kernel runs the lanes_* functions (emulated in lock step
-// below); row_block() is their single-thread form, pinned to the oracle the same way.
+// Host build of llmc_b200/csrc/spqr_row.cuh (and the quant_math.cuh it includes) for
+// tests/test_oracle_golden.py: the SAME source the CUDA kernel spqr_inblock_kernel compiles for the
+// device, driven row by row on the CPU so that its arithmetic can be compared bit for bit with
+// oracle/spqr_oracle.py (and, through it, with the reference-generated goldens).  The lanes_*
+// functions the kernel runs are emulated in lock step below; nl = 1 is the single-thread form.
 // Build: g++ -O2 -ffp-contract=off -shared -fPIC.
+#include <cmath>
+
 #include "spqr_row.cuh"
+
+using namespace llmc;
 
 static spqr::QCfg qcfg(int bit, int sym, int round_zp) {
   spqr::QCfg q{};
-  if (sym) { q.qmin = -static_cast<float>(1 << (bit - 1)); q.qmax = static_cast<float>((1 << (bit - 1)) - 1); }
-  else { q.qmin = 0.f; q.qmax = static_cast<float>((1 << bit) - 1); }
+  int_range(bit, sym, q.qmin, q.qmax);
   q.sym = sym; q.round_zp = round_zp;
   return q;
-}
-
-extern "C" void spqr_row_block_host(float* W, const float* Hb, int R, int cnt, int gs, int bit, int sym,
-                                    int round_zp, int s_bit, int s_sym, int s_rzp, int z_bit, int z_sym,
-                                    int z_rzp, float thr, int simplified, float* err, uint8_t* mask,
-                                    float* S, float* Z, float* loss) {
-  spqr::Cfg c{};
-  c.w = qcfg(bit, sym, round_zp);
-  c.loo = qcfg(bit, sym, 0);
-  c.sc = qcfg(s_bit, s_sym, s_rzp);
-  c.zc = qcfg(z_bit, z_sym, z_rzp);
-  c.gs = gs;
-  c.thr = thr;
-  c.has_thr = !std::isinf(thr);
-  c.outliers = (!simplified && c.has_thr) ? 1 : 0;
-  const int ng = (cnt + gs - 1) / gs;
-  for (int r = 0; r < R; ++r)
-    loss[r] = spqr::row_block(W + static_cast<long>(r) * cnt, 1, Hb, cnt, 1, cnt, c, err + static_cast<long>(r) * cnt, 1,
-                              mask + static_cast<long>(r) * cnt, 1, S + static_cast<long>(r) * ng,
-                              Z + static_cast<long>(r) * ng);
 }
 
 // Lock-step emulation of the lane-parallel kernel: every phase runs for lane = 0 .. nl-1 before the
@@ -78,7 +61,7 @@ extern "C" void spqr_row_block_lanes_host(float* W, const float* Hb, int R, int 
       }
       err[static_cast<long>(r) * cnt + col] = e0;
       mask[static_cast<long>(r) * cnt + col] = m0;
-      l = spqr::add(l, spqr::mul(e0, e0));
+      l = add(l, mul(e0, e0));
     }
     loss[r] = l;
   }

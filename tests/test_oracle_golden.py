@@ -330,7 +330,7 @@ def _build_spqr_host(tmp_path):
     return ctypes.CDLL(so_path)
 
 
-def _spqr_host_block(lib, Wb, Hb, wk, l2s, l2z, thr, simplified, lanes=0):
+def _spqr_host_block(lib, Wb, Hb, wk, l2s, l2z, thr, simplified, lanes):
     import ctypes
     P = ctypes.c_void_p
     R, cnt = Wb.shape
@@ -345,20 +345,18 @@ def _spqr_host_block(lib, Wb, Hb, wk, l2s, l2z, thr, simplified, lanes=0):
             l2z['bit'], int(l2z['symmetric']), int(l2z.get('round_zp', True)), ctypes.c_float(thr),
             int(simplified))
     tail = (P(err.data_ptr()), P(mask.data_ptr()), P(S.data_ptr()), P(Z.data_ptr()), P(loss.data_ptr()))
-    if lanes:
-        # lock-step emulation of the lane-parallel kernel (spqr_row.cuh: lanes_*)
-        lib.spqr_row_block_lanes_host(*head, int(lanes), *tail)
-    else:
-        lib.spqr_row_block_host(*head, *tail)
+    # lock-step emulation of the lane-parallel kernel (spqr_row.cuh: lanes_*)
+    lib.spqr_row_block_lanes_host(*head, int(lanes), *tail)
     return W, err, mask, S, Z, loss
 
 
-def test_spqr_device_row_code_on_the_host_matches_oracle(golden_dir, tmp_path):
+def test_spqr_device_lane_code_on_the_host_matches_oracle(golden_dir, tmp_path):
     """llmc_b200/csrc/spqr_row.cuh is the arithmetic of the CUDA kernel spqr_inblock_kernel.  Built
     for the HOST (tests/host/spqr_row_host.cpp, -ffp-contract=off) it must agree bit for bit with
     the oracle — on the reference-generated layers and on a seeded 128-column block with other
     second-level configurations — so the device code is pinned without a GPU.  `lanes`: the
-    lane-parallel form the kernel actually runs (16 lanes per row), emulated in lock step."""
+    lane-parallel form the kernel runs (16 lanes per row), emulated in lock step; one lane is the
+    single-thread form."""
     from oracle import spqr_oracle as so
     lib = _build_spqr_host(tmp_path)
     kat = _load(golden_dir, 'spqr_kat.pt')
@@ -366,7 +364,7 @@ def test_spqr_device_row_code_on_the_host_matches_oracle(golden_dir, tmp_path):
         cfg = _spqr_cfg(c, so)
         cnt = min(128, c['Wp'].shape[1])
         ref = so.row_block(c['Wp'][:, :cnt], c['Hinv'][:cnt, :cnt], cfg)
-        for lanes in (0, 16, 8):
+        for lanes in (1, 16, 8):
             got = _spqr_host_block(lib, c['Wp'][:, :cnt], c['Hinv'][:cnt, :cnt], c['weight_kwargs'],
                                    c['level2'], c['level2'], cfg['thr'], c['special']['simplified_outliers'],
                                    lanes=lanes)
@@ -388,7 +386,7 @@ def test_spqr_device_row_code_on_the_host_matches_oracle(golden_dir, tmp_path):
         thr = so.threshold_of(W, Hinv, rel)
         cfg = so.make_cfg(wk, sp, l2s, l2z, thr)
         ref = so.row_block(W, Hinv, cfg)
-        for lanes in (0, 16):
+        for lanes in (1, 16):
             got = _spqr_host_block(lib, W, Hinv, wk, l2s, l2z, thr, False, lanes=lanes)
             for a, b in zip(got, ref):
                 assert torch.equal(a, b), (bit, gs, lanes)
