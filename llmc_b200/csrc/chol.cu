@@ -16,12 +16,6 @@ namespace ch {
 constexpr int NB = 128;
 constexpr int LDS = NB + 1;
 
-__device__ __forceinline__ float tf32r(float x) {
-  uint32_t r;
-  asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(r) : "f"(x));
-  return __uint_as_float(r);
-}
-
 // G[i][j] = H[n-1-i][n-1-j]
 __global__ void __launch_bounds__(256)
 reverse_kernel(const float* __restrict__ H, float* __restrict__ G, int64_t n) {
@@ -250,10 +244,10 @@ diag_kernel(float* __restrict__ G, int64_t n, int64_t k0, int nb, float* __restr
       const int64_t o = (k0 + i) * n + k0 + j;
       G[o] = S[i * LDS + j];
       const float x = X[i * LDS + j];
-      const float h = tf32r(x);
+      const float2 s = tf32_split(x);
       Y[o] = x;
-      Yhi[o] = h;
-      Ylo[o] = tf32r(x - h);
+      Yhi[o] = s.x;
+      Ylo[o] = s.y;
     }
   }
 }

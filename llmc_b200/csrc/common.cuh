@@ -156,7 +156,40 @@ __device__ __forceinline__ void store_as(int dt, void* p, int64_t i, float v) {
     else { ::llmc::set_last_error("%s: bad dtype %d", what, (dt)); return LLMC_EINVAL; } \
   } while (0)
 
+// ---- 16-bit pairs ----------------------------------------------------------------------
+// Two fp16 / bf16 (DT) values in one 32-bit word, the first in the low half.  Packing rounds each
+// float once (cvt.rn.{f16,bf16}x2); widening is exact.
+template <int DT>
+__device__ __forceinline__ uint32_t pack_pair(float a, float b) {
+  if constexpr (DT == LLMC_BF16) {
+    const __nv_bfloat162 h = __floats2bfloat162_rn(a, b);
+    return *reinterpret_cast<const uint32_t*>(&h);
+  } else {
+    const __half2 h = __floats2half2_rn(a, b);
+    return *reinterpret_cast<const uint32_t*>(&h);
+  }
+}
+// a lone 16-bit value (a bias element, a qparam in the activation dtype)
+template <int DT>
+__device__ __forceinline__ float widen16(uint16_t x) {
+  if constexpr (DT == LLMC_BF16) return __uint_as_float(static_cast<uint32_t>(x) << 16);
+  else return __half2float(__ushort_as_half(x));
+}
+template <int DT>
+__device__ __forceinline__ float pair_lo(uint32_t w) {
+  if constexpr (DT == LLMC_BF16) return __uint_as_float(w << 16);
+  else return widen16<DT>(static_cast<uint16_t>(w & 0xffffu));
+}
+template <int DT>
+__device__ __forceinline__ float pair_hi(uint32_t w) {
+  if constexpr (DT == LLMC_BF16) return __uint_as_float(w & 0xffff0000u);
+  else return widen16<DT>(static_cast<uint16_t>(w >> 16));
+}
+
 // 8 consecutive elements <-> 8 floats, vectorised (16 B for 2-byte types, 2x16 B for fp32).
+// load8 writes its widening out rather than calling pair_lo / pair_hi: with the calls, ptxas
+// allocates registers differently in callers (an 8-byte spill in quant_dynamic_warp_kernel<bf16>,
+// three more registers in rope_kernel).
 template <int DT>
 __device__ __forceinline__ void load8(const void* base, int64_t idx, float (&v)[8]) {
   if constexpr (DT == LLMC_F32) {
@@ -192,15 +225,7 @@ __device__ __forceinline__ void store8(void* base, int64_t idx, const float (&v)
   } else {
     uint32_t w[4];
 #pragma unroll
-    for (int i = 0; i < 4; ++i) {
-      if constexpr (DT == LLMC_BF16) {
-        __nv_bfloat162 h = __floats2bfloat162_rn(v[2 * i], v[2 * i + 1]);
-        w[i] = *reinterpret_cast<uint32_t*>(&h);
-      } else {
-        __half2 h = __floats2half2_rn(v[2 * i], v[2 * i + 1]);
-        w[i] = *reinterpret_cast<uint32_t*>(&h);
-      }
-    }
+    for (int i = 0; i < 4; ++i) w[i] = pack_pair<DT>(v[2 * i], v[2 * i + 1]);
     *reinterpret_cast<uint4*>(reinterpret_cast<uint16_t*>(base) + idx) =
         make_uint4(w[0], w[1], w[2], w[3]);
   }

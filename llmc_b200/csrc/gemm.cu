@@ -54,17 +54,7 @@ template <bool kSyrk>
 __device__ __forceinline__ Unit decode_unit(const GemmParams& p, int u) {
   Unit t;
   if constexpr (!kSyrk) {
-    // Grouped rasterisation: weights are swept in groups of `gn` n-tiles (<= ~32 MB, L2 resident),
-    // all m-tiles per group, n fastest inside the group.  Activations are re-read N/(256*gn)
-    // times from HBM, weights once; n-fastest over a 14336-row weight would instead stream the
-    // whole 117 MB weight through L2 once per 132-tile wave.
-    const int m_tiles = p.num_tiles / p.n_tiles_n;
-    const int per_group = p.gn * m_tiles;
-    const int g = u / per_group;
-    const int rem = u - g * per_group;
-    const int gsz = min(p.gn, p.n_tiles_n - g * p.gn);
-    t.m_blk = rem / gsz;
-    t.n_blk = g * p.gn + (rem - t.m_blk * gsz);
+    grouped_tile(u, p.num_tiles / p.n_tiles_n, p.n_tiles_n, p.gn, t.m_blk, t.n_blk);
     t.kb0 = 0;
     t.kb1 = p.kb_total;
     t.split = 0;
@@ -200,52 +190,35 @@ wgmma_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
     if (prev >= 0 && tid == 0) mbar_arrive(&empty_bar[prev]);
 
     // ---- epilogue straight from the accumulator registers ----
-    const int64_t row0 = static_cast<int64_t>(t.m_blk) * BM + c * 64 + (tid >> 5) * 16 + (lane >> 2);
-    auto store_half = [&](const float (&acc)[64], int h) {
+    if constexpr (!kSyrk) {
+      constexpr int DT = kBf16 ? LLMC_BF16 : LLMC_F16;
+      const int64_t row0 = static_cast<int64_t>(t.m_blk) * BM + c * 64;
+      const int64_t col0 = static_cast<int64_t>(t.n_blk) * BN;
+      store_linear_m64n128<DT>(acc0, row0, col0, p.M, p.N, p.ld_out, p.bias, p.out);
+      store_linear_m64n128<DT>(acc1, row0, col0 + 128, p.M, p.N, p.ld_out, p.bias, p.out);
+    } else {
+      // fp32 partial slab `t.split` of the split-K sum
+      const int64_t row0 = static_cast<int64_t>(t.m_blk) * BM + c * 64 + (tid >> 5) * 16 + (lane >> 2);
+      auto store_half = [&](const float (&acc)[64], int h) {
 #pragma unroll
-      for (int j = 0; j < 16; ++j) {
-        const int64_t col = static_cast<int64_t>(t.n_blk) * BN + h * 128 + 8 * j + 2 * (lane & 3);
-        if (col >= p.N) continue;
+        for (int j = 0; j < 16; ++j) {
+          const int64_t col = static_cast<int64_t>(t.n_blk) * BN + h * 128 + 8 * j + 2 * (lane & 3);
+          if (col >= p.N) continue;
 #pragma unroll
-        for (int i = 0; i < 2; ++i) {
-          const int64_t row = row0 + 8 * i;
-          if (row >= p.M) continue;
-          float v0 = acc[4 * j + 2 * i], v1 = acc[4 * j + 2 * i + 1];
-          const bool pair = col + 1 < p.N;
-          if constexpr (kSyrk) {
+          for (int i = 0; i < 2; ++i) {
+            const int64_t row = row0 + 8 * i;
+            if (row >= p.M) continue;
+            const float v0 = acc[4 * j + 2 * i], v1 = acc[4 * j + 2 * i + 1];
             float* o = reinterpret_cast<float*>(p.out) +
                        (static_cast<int64_t>(t.split) * p.M + row) * p.ld_out + col;
-            if (pair) *reinterpret_cast<float2*>(o) = make_float2(v0, v1);
+            if (col + 1 < p.N) *reinterpret_cast<float2*>(o) = make_float2(v0, v1);
             else o[0] = v0;
-          } else {
-            uint16_t* o = reinterpret_cast<uint16_t*>(p.out) + row * p.ld_out + col;
-            const uint16_t* bs = reinterpret_cast<const uint16_t*>(p.bias);
-            if (bs != nullptr) {
-              // F.linear adds the bias in fp32 before the single rounding to the out dtype
-              v0 += kBf16 ? __uint_as_float(static_cast<uint32_t>(bs[col]) << 16)
-                          : __half2float(__ushort_as_half(bs[col]));
-              if (pair) v1 += kBf16 ? __uint_as_float(static_cast<uint32_t>(bs[col + 1]) << 16)
-                                    : __half2float(__ushort_as_half(bs[col + 1]));
-            }
-            uint32_t pk;
-            if constexpr (kBf16) {
-              __nv_bfloat162 hv = __floats2bfloat162_rn(v0, v1);
-              pk = *reinterpret_cast<uint32_t*>(&hv);
-            } else {
-              __half2 hv = __floats2half2_rn(v0, v1);
-              pk = *reinterpret_cast<uint32_t*>(&hv);
-            }
-            if (pair && (p.ld_out & 1) == 0) *reinterpret_cast<uint32_t*>(o) = pk;
-            else {
-              o[0] = static_cast<uint16_t>(pk & 0xffffu);
-              if (pair) o[1] = static_cast<uint16_t>(pk >> 16);
-            }
           }
         }
-      }
-    };
-    store_half(acc0, 0);
-    store_half(acc1, 1);
+      };
+      store_half(acc0, 0);
+      store_half(acc1, 1);
+    }
   }
 }
 
@@ -405,13 +378,7 @@ extern "C" int llmc_gemm_bf16(const void* x, const void* w, const void* bias, vo
   p.splits = 1;
   p.kb_total = static_cast<int>((K + BK - 1) / BK);
   p.kb_per_split = p.kb_total;
-  {
-    const int64_t tile_bytes = static_cast<int64_t>(BN) * K * 2;      // one n-tile of weights
-    int64_t gn = (32ll << 20) / (tile_bytes > 0 ? tile_bytes : 1);
-    if (gn < 1) gn = 1;
-    if (gn > p.n_tiles_n) gn = p.n_tiles_n;
-    p.gn = static_cast<int>(gn);
-  }
+  p.gn = l2_group_width(static_cast<int64_t>(BN) * K * 2, p.n_tiles_n);   // K > 0: one n-tile's bytes
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   return dtype == LLMC_BF16 ? launch_wgmma<false, true>(tmA, tmB, p, st)
                             : launch_wgmma<false, false>(tmA, tmB, p, st);

@@ -13,14 +13,14 @@
 // by a deep, cheap ring and the dequantised tile by a short one:
 //   ring L (6 x 20 KB): X tile [128 x 64] bf16 (swizzle 128B) + packed W tile [128 x 8] int32
 //   ring B (3 x 16 KB): the dequantised, 128B-swizzled wgmma B tile
-//   warps 0 .. 4NG-1   dequant, NG groups of four warps taking every NG-th K step (one weight row
-//                      per thread): nibble -> fp32 via the 2^23 magic constant, (q - z) * s in
+//   warps 0-7          dequant, NG = 2 groups of four warps taking alternate K steps (one weight
+//                      row per thread): nibble -> fp32 via the 2^23 magic constant, (q - z) * s in
 //                      fp32, round to bf16/fp16, 16-byte stores into ring B, fence.proxy.async;
 //                      the group's scale/zero for its NEXT step is prefetched
-//   warpgroups NG, NG+1  consumers: 64 rows each, wgmma m64n128k16 with fp32 register
+//   warpgroups 2, 3    consumers: 64 rows each, wgmma m64n128k16 with fp32 register
 //                      accumulators; retiring a step's wgmma group frees its ring-L and ring-B
 //                      stages; epilogue (bias -> bf16/fp16 -> global) from registers
-//   warp 4NG + 8       TMA into ring L
+//   warp 16            TMA into ring L  (17 warps, 544 threads)
 // Weight layout: LLMC_OUT_PACK_VLLM of UNSIGNED codes — 8 nibbles per int32 along K, nibble i =
 // element 8*w + i; scales / zeros fp32 [N, K/group] (zeros NULL => 2^(bit-1), the symmetric
 // +8 offset of module_utils.py:842-844).
@@ -37,11 +37,12 @@ namespace w4 {
 constexpr int BM = 128, BN = 128, BK = 64;
 constexpr int kABytes = BM * BK * 2;          // 16 KB
 constexpr int kBBytes = BN * BK * 2;          // 16 KB dequantised
+constexpr int NG = 2;                         // dequant groups of four warps
 // per weight width: INT4 -> 4 KB packed tile, INT8 -> 8 KB
-template <int kBits, int NG> struct Cfg {
+template <int kBits> struct Cfg {
   static constexpr int kPBytes = BN * BK * kBits / 8;
   static constexpr int kLBytes = kABytes + kPBytes;
-  static constexpr int kBStages = NG > 3 ? NG : 3;
+  static constexpr int kBStages = 3;
   static constexpr int kLStages = 6;
   static constexpr int kSmemBytes = kLStages * kLBytes + kBStages * kBBytes + 1024 + 256;
   static constexpr int kWordsPerRow = BK * kBits / 32;      // int32 per row of the packed tile
@@ -63,27 +64,6 @@ struct Params {
   float zero_default;
   int n_tiles_n, num_units, kb_total, gn;
 };
-
-__device__ __forceinline__ void decode(const Params& p, int u, int& m_blk, int& n_blk) {
-  const int m_tiles = p.num_units / p.n_tiles_n;
-  const int per_group = p.gn * m_tiles;
-  const int g = u / per_group;
-  const int rem = u - g * per_group;
-  const int gsz = min(p.gn, p.n_tiles_n - g * p.gn);
-  m_blk = rem / gsz;
-  n_blk = g * p.gn + (rem - m_blk * gsz);
-}
-
-template <bool kBf16>
-__device__ __forceinline__ uint32_t pack2(float a, float b) {
-  if constexpr (kBf16) {
-    __nv_bfloat162 h = __floats2bfloat162_rn(a, b);
-    return *reinterpret_cast<uint32_t*>(&h);
-  } else {
-    __half2 h = __floats2half2_rn(a, b);
-    return *reinterpret_cast<uint32_t*>(&h);
-  }
-}
 
 // (a & b) | c in one LOP3
 __device__ __forceinline__ uint32_t and_or(uint32_t a, uint32_t b, uint32_t c) {
@@ -108,11 +88,12 @@ __device__ __forceinline__ uint32_t sub_mul2(uint32_t x2, uint32_t zm2, uint32_t
   }
 }
 
-template <bool kBf16, int kBits, int NG>
-__global__ void __launch_bounds__(Cfg<kBits, NG>::kThreads, 1)
+template <bool kBf16, int kBits>
+__global__ void __launch_bounds__(Cfg<kBits>::kThreads, 1)
 w4a16_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmP,
                   const Params p) {
-  using C = Cfg<kBits, NG>;
+  using C = Cfg<kBits>;
+  constexpr int DT = kBf16 ? LLMC_BF16 : LLMC_F16;
   constexpr int kLStages = C::kLStages;
   constexpr int kLBytes = C::kLBytes;
   constexpr int kBStages = C::kBStages;
@@ -149,7 +130,7 @@ w4a16_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
       uint32_t phl = 0;
       for (int u = blockIdx.x; u < p.num_units; u += gridDim.x) {
         int m_blk, n_blk;
-        decode(p, u, m_blk, n_blk);
+        grouped_tile(u, p.num_units / p.n_tiles_n, p.n_tiles_n, p.gn, m_blk, n_blk);
         for (int kb = 0; kb < p.kb_total; ++kb) {
           mbar_wait(&emptyL[sl], phl ^ 1);
           uint8_t* a_dst = ringL + sl * kLBytes;
@@ -169,7 +150,7 @@ w4a16_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
     uint32_t phl = 0, phb = 0;
     for (int u = blockIdx.x; u < p.num_units; u += gridDim.x) {
       int m_blk, n_blk;
-      decode(p, u, m_blk, n_blk);
+      grouped_tile(u, p.num_units / p.n_tiles_n, p.n_tiles_n, p.gn, m_blk, n_blk);
       float acc[64];
 #pragma unroll
       for (int i = 0; i < 64; ++i) acc[i] = 0.f;
@@ -204,40 +185,13 @@ w4a16_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
         mbar_arrive(&emptyB[prev_b]);
       }
       // ---- epilogue from the accumulator registers ----
-      const int64_t row0 = static_cast<int64_t>(m_blk) * BM + c * 64 + (tid >> 5) * 16 + (lane >> 2);
-      const uint16_t* bs = reinterpret_cast<const uint16_t*>(p.bias);
-#pragma unroll
-      for (int j = 0; j < 16; ++j) {
-        const int64_t col = static_cast<int64_t>(n_blk) * BN + 8 * j + 2 * (lane & 3);
-        if (col >= p.N) continue;
-        const bool pair = col + 1 < p.N;
-        float b0 = 0.f, b1 = 0.f;
-        if (bs != nullptr) {
-          b0 = kBf16 ? __uint_as_float(static_cast<uint32_t>(bs[col]) << 16)
-                     : __half2float(__ushort_as_half(bs[col]));
-          if (pair) b1 = kBf16 ? __uint_as_float(static_cast<uint32_t>(bs[col + 1]) << 16)
-                               : __half2float(__ushort_as_half(bs[col + 1]));
-        }
-#pragma unroll
-        for (int i = 0; i < 2; ++i) {
-          const int64_t row = row0 + 8 * i;
-          if (row >= p.M) continue;
-          float v0 = acc[4 * j + 2 * i], v1 = acc[4 * j + 2 * i + 1];
-          if (bs != nullptr) { v0 += b0; v1 += b1; }
-          const uint32_t pk = pack2<kBf16>(v0, v1);
-          uint16_t* o = reinterpret_cast<uint16_t*>(p.out) + row * p.N + col;
-          if (pair && (p.N & 1) == 0) *reinterpret_cast<uint32_t*>(o) = pk;
-          else {
-            o[0] = static_cast<uint16_t>(pk & 0xffffu);
-            if (pair) o[1] = static_cast<uint16_t>(pk >> 16);
-          }
-        }
-      }
+      store_linear_m64n128<DT>(acc, static_cast<int64_t>(m_blk) * BM + c * 64,
+                               static_cast<int64_t>(n_blk) * BN, p.M, p.N, p.N, p.bias, p.out);
     }
   } else {
     // ===================== dequant warps (4 * NG): one weight row per thread =====================
-    // NG groups of four warps take every NG-th K step, so that several groups' dependent
-    // unpack -> convert -> store chains are in flight at once.  Ring B has one stage per group.
+    // NG groups of four warps take every NG-th K step, so that both groups' dependent
+    // unpack -> convert -> store chains are in flight at once.
     const int grp = warp % NG;
     const int row = (warp / NG) * 32 + lane;         // 0..127 inside the group
     uint32_t it = 0;                                 // K steps issued so far (all tiles)
@@ -257,13 +211,13 @@ w4a16_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
     };
     auto widen = [&](uint32_t raw) -> float {
       if (!p.qparam_native) return __uint_as_float(raw);
-      return kBf16 ? __uint_as_float(raw << 16) : __half2float(__ushort_as_half(static_cast<uint16_t>(raw)));
+      return widen16<DT>(static_cast<uint16_t>(raw));
     };
     const bool have_zeros = p.zeros != nullptr;
     const int steps_per_group = static_cast<int>(p.group / BK);
     for (int u = blockIdx.x; u < p.num_units; u += gridDim.x) {
       int m_blk, n_blk;
-      decode(p, u, m_blk, n_blk);
+      grouped_tile(u, p.num_units / p.n_tiles_n, p.n_tiles_n, p.gn, m_blk, n_blk);
       const int64_t n0 = static_cast<int64_t>(n_blk) * BN + row;
       // first K step of this tile that belongs to this group: (it + kb) % NG == grp
       int kb = (grp + NG - static_cast<int>(it % NG)) % NG;
@@ -302,8 +256,8 @@ w4a16_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
                 v[j] = fmul_rn(__uint_as_float(__byte_perm(wd[2 * hh], 0x4B000000u, 0x7650u + j)) - zm_cur, s_c);
                 v[4 + j] = fmul_rn(__uint_as_float(__byte_perm(wd[2 * hh + 1], 0x4B000000u, 0x7650u + j)) - zm_cur, s_c);
               }
-              const uint4 o = make_uint4(pack2<kBf16>(v[0], v[1]), pack2<kBf16>(v[2], v[3]),
-                                         pack2<kBf16>(v[4], v[5]), pack2<kBf16>(v[6], v[7]));
+              const uint4 o = make_uint4(pack_pair<DT>(v[0], v[1]), pack_pair<DT>(v[2], v[3]),
+                                         pack_pair<DT>(v[4], v[5]), pack_pair<DT>(v[6], v[7]));
               const int c = c4 * 2 + hh;
               *reinterpret_cast<uint4*>(bt + row * 128 + ((c ^ (row & 7)) << 4)) = o;
             }
@@ -318,9 +272,9 @@ w4a16_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
             // packed path: 0x6400|q = 1024+q (fp16) / 0x4300|q = 128+q (bf16), two weights per
             // register; (magic+q) - (magic+z) and * s are one HSUB2 + one HMUL2 per pair
             constexpr uint32_t kMagic2 = kBf16 ? 0x43004300u : 0x64006400u;
-            const uint32_t s2 = pack2<kBf16>(s_c, s_c);                          // exact: s is a T value
-            const uint32_t zm2 = pack2<kBf16>((kBf16 ? 128.f : 1024.f) + z_c,
-                                              (kBf16 ? 128.f : 1024.f) + z_c);        // exact: <= 8 bits
+            const uint32_t s2 = pack_pair<DT>(s_c, s_c);                          // exact: s is a T value
+            const uint32_t zm2 = pack_pair<DT>((kBf16 ? 128.f : 1024.f) + z_c,
+                                               (kBf16 ? 128.f : 1024.f) + z_c);       // exact: <= 8 bits
 #pragma unroll
             for (int c = 0; c < 8; ++c) {
               const uint32_t w = words[c];
@@ -350,8 +304,8 @@ w4a16_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
                 v[2 * j] = fmul_rn(__uint_as_float(be) - zm_cur, s_c);
                 v[2 * j + 1] = fmul_rn(__uint_as_float(bo) - zm_cur, s_c);
               }
-              const uint4 o = make_uint4(pack2<kBf16>(v[0], v[1]), pack2<kBf16>(v[2], v[3]),
-                                         pack2<kBf16>(v[4], v[5]), pack2<kBf16>(v[6], v[7]));
+              const uint4 o = make_uint4(pack_pair<DT>(v[0], v[1]), pack_pair<DT>(v[2], v[3]),
+                                         pack_pair<DT>(v[4], v[5]), pack_pair<DT>(v[6], v[7]));
               *reinterpret_cast<uint4*>(bt + row * 128 + ((c ^ (row & 7)) << 4)) = o;
             }
           }
@@ -376,8 +330,8 @@ w4a16_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
 
 using namespace llmc;
 
-template <int kBits, int NG>
-static int gemm_wNa16_ng(const void* x, const int32_t* wq, const void* scales, const void* zeros,
+template <int kBits>
+static int gemm_wNa16(const void* x, const int32_t* wq, const void* scales, const void* zeros,
                       int qparam_dtype, const void* bias, void* y, int64_t M, int64_t N, int64_t K,
                       int64_t group, int dtype, int q_transposed, void* stream, const char* name) {
   using namespace w4;
@@ -394,7 +348,7 @@ static int gemm_wNa16_ng(const void* x, const int32_t* wq, const void* scales, c
     set_last_error("%s: K=%lld must be a multiple of 64 and pointers 16-byte aligned", name, (long long)K);
     return LLMC_EALIGN;
   }
-  using C = Cfg<kBits, NG>;
+  using C = Cfg<kBits>;
   constexpr int wpr = C::kWordsPerRow;
   constexpr int kThreads = C::kThreads;
   CUtensorMap tmA, tmP;
@@ -417,33 +371,23 @@ static int gemm_wNa16_ng(const void* x, const int32_t* wq, const void* scales, c
   LLMC_CHECK_ARG(mt * p.n_tiles_n < (1ll << 31), "%s: too many tiles", name);
   p.num_units = static_cast<int>(mt * p.n_tiles_n);
   p.kb_total = static_cast<int>(K / BK);
-  {
-    int64_t gn = (32ll << 20) / (static_cast<int64_t>(BN) * K * kBits / 8 + 1);
-    if (gn < 1) gn = 1;
-    if (gn > p.n_tiles_n) gn = p.n_tiles_n;
-    p.gn = static_cast<int>(gn);
-  }
+  // One byte over the packed n-tile's size, so that the tile order, and with it the measured
+  // timing, stays as it is: the width is one n-tile narrower than 32 MB allows when the tile bytes
+  // divide 32 MB exactly (W8 at K = 4096: 63 n-tiles, not 64).  The width changes no output, only
+  // L2 traffic; change it only together with a measurement.
+  p.gn = l2_group_width(static_cast<int64_t>(BN) * K * kBits / 8 + 1, p.n_tiles_n);
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   constexpr int smem = C::kSmemBytes;
   static_assert(smem <= 227 * 1024, "shared memory budget");
   LLMC_ONCE_PER_DEVICE({
-    LLMC_CHECK_CUDA(cudaFuncSetAttribute(w4a16_gemm_kernel<true, kBits, NG>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-    LLMC_CHECK_CUDA(cudaFuncSetAttribute(w4a16_gemm_kernel<false, kBits, NG>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+    LLMC_CHECK_CUDA(cudaFuncSetAttribute(w4a16_gemm_kernel<true, kBits>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+    LLMC_CHECK_CUDA(cudaFuncSetAttribute(w4a16_gemm_kernel<false, kBits>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
   });
   const int grid = p.num_units < kNumSMs ? p.num_units : kNumSMs;
-  if (dtype == LLMC_BF16) w4a16_gemm_kernel<true, kBits, NG><<<grid, kThreads, smem, st>>>(tmA, tmP, p);
-  else w4a16_gemm_kernel<false, kBits, NG><<<grid, kThreads, smem, st>>>(tmA, tmP, p);
+  if (dtype == LLMC_BF16) w4a16_gemm_kernel<true, kBits><<<grid, kThreads, smem, st>>>(tmA, tmP, p);
+  else w4a16_gemm_kernel<false, kBits><<<grid, kThreads, smem, st>>>(tmA, tmP, p);
   LLMC_CHECK_LAUNCH();
   return LLMC_OK;
-}
-
-// Two dequant groups (eight warps, one weight row per thread and K step).
-template <int kBits>
-static int gemm_wNa16(const void* x, const int32_t* wq, const void* scales, const void* zeros,
-                      int qparam_dtype, const void* bias, void* y, int64_t M, int64_t N, int64_t K,
-                      int64_t group, int dtype, int q_transposed, void* stream, const char* name) {
-  return gemm_wNa16_ng<kBits, 2>(x, wq, scales, zeros, qparam_dtype, bias, y, M, N, K, group, dtype,
-                                 q_transposed, stream, name);
 }
 
 extern "C" int llmc_gemm_w4a16(const void* x, const int32_t* wq, const void* scales,

@@ -338,12 +338,9 @@ gptq_inblock_kernel(InblockArgs a) {
       const float evv = (c < cnt) ? Et[c * EP + lane] : 0.f;
       const int64_t o = static_cast<int64_t>(c) * a.Rpad + r0 + lane;
       a.err[o] = evv;
-      uint32_t hb, lb;                                   // tf32 split for the 3xTF32 trailing GEMM
-      asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(hb) : "f"(evv));
-      const float h = __uint_as_float(hb);
-      asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(lb) : "f"(evv - h));
-      a.err_hi[o] = h;
-      a.err_lo[o] = __uint_as_float(lb);
+      const float2 s = tf32_split(evv);                  // for the 3xTF32 trailing GEMM
+      a.err_hi[o] = s.x;
+      a.err_lo[o] = s.y;
     }
   }
 }
@@ -462,12 +459,9 @@ spqr_inblock_kernel(SpqrArgs a) {
     const float ev = (c < cnt) ? Et[c * SEP + r] : 0.f;
     const int64_t o = static_cast<int64_t>(c) * a.Rpad + r0 + r;
     a.err[o] = ev;
-    uint32_t hb, lb;
-    asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(hb) : "f"(ev));
-    const float h = __uint_as_float(hb);
-    asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(lb) : "f"(ev - h));
-    a.err_hi[o] = h;
-    a.err_lo[o] = __uint_as_float(lb);
+    const float2 s = tf32_split(ev);
+    a.err_hi[o] = s.x;
+    a.err_lo[o] = s.y;
   }
 }
 

@@ -437,26 +437,6 @@ __device__ __forceinline__ uint32_t max2(uint32_t a, uint32_t b) {
     return *reinterpret_cast<const uint32_t*>(&r);
   }
 }
-template <int DT>
-__device__ __forceinline__ float lo_f(uint32_t w) {
-  if constexpr (DT == LLMC_BF16) return __uint_as_float(w << 16);
-  else return __half2float(__ushort_as_half(static_cast<uint16_t>(w & 0xffffu)));
-}
-template <int DT>
-__device__ __forceinline__ float hi_f(uint32_t w) {
-  if constexpr (DT == LLMC_BF16) return __uint_as_float(w & 0xffff0000u);
-  else return __half2float(__ushort_as_half(static_cast<uint16_t>(w >> 16)));
-}
-template <int DT>
-__device__ __forceinline__ uint32_t pack_T(float a, float b) {
-  if constexpr (DT == LLMC_BF16) {
-    const __nv_bfloat162 h = __floats2bfloat162_rn(a, b);
-    return *reinterpret_cast<const uint32_t*>(&h);
-  } else {
-    const __half2 h = __floats2half2_rn(a, b);
-    return *reinterpret_cast<const uint32_t*>(&h);
-  }
-}
 
 // The per-chunk tail shared by the two fast kernels: 8 packed T values -> QDQ chunk | packed codes.
 //   v = yb + Ce does rint, + zero and the storage offset in one float add (see the kernel comment).
@@ -469,16 +449,16 @@ __device__ __forceinline__ void fast_tail(const uint4& xin, const Divider<DT>& d
 #pragma unroll
   for (int i = 0; i < 4; ++i) {
     // rT(x / s): exact quotient, then ONE rounding to T for the pair (cvt.rn.{bf16,f16}x2)
-    const uint32_t yb = pack_T<DT>(div(lo_f<DT>(wd[i])), div(hi_f<DT>(wd[i])));
-    v[2 * i] = fminf(fmaxf(fadd_rn(lo_f<DT>(yb), Ce), vlo), vhi);
-    v[2 * i + 1] = fminf(fmaxf(fadd_rn(hi_f<DT>(yb), Ce), vlo), vhi);
+    const uint32_t yb = pack_pair<DT>(div(pair_lo<DT>(wd[i])), div(pair_hi<DT>(wd[i])));
+    v[2 * i] = fminf(fmaxf(fadd_rn(pair_lo<DT>(yb), Ce), vlo), vhi);
+    v[2 * i + 1] = fminf(fmaxf(fadd_rn(pair_hi<DT>(yb), Ce), vlo), vhi);
   }
   if constexpr (MODE == M_QDQ) {
     // (q - z) = v - Ce exactly; * s rounds once to T (quant.py:710-712)
-    out.x = pack_T<DT>(fmul_rn(v[0] - Ce, s), fmul_rn(v[1] - Ce, s));
-    out.y = pack_T<DT>(fmul_rn(v[2] - Ce, s), fmul_rn(v[3] - Ce, s));
-    out.z = pack_T<DT>(fmul_rn(v[4] - Ce, s), fmul_rn(v[5] - Ce, s));
-    out.w = pack_T<DT>(fmul_rn(v[6] - Ce, s), fmul_rn(v[7] - Ce, s));
+    out.x = pack_pair<DT>(fmul_rn(v[0] - Ce, s), fmul_rn(v[1] - Ce, s));
+    out.y = pack_pair<DT>(fmul_rn(v[2] - Ce, s), fmul_rn(v[3] - Ce, s));
+    out.z = pack_pair<DT>(fmul_rn(v[4] - Ce, s), fmul_rn(v[5] - Ce, s));
+    out.w = pack_pair<DT>(fmul_rn(v[6] - Ce, s), fmul_rn(v[7] - Ce, s));
   } else if constexpr (MODE == M_PACK && BITS == 4) {
     // sym: nibble_i = code_i + 8 in [0, 15]; word = sum nibble_i * 16^i.
     // asym: the codes are packed plain (C) and the reference's (code + 8) << 4i, OR-ed
@@ -574,10 +554,10 @@ quant_group_fast_kernel(QuantArgs a, int64_t total_groups) {
 #pragma unroll
         for (int c = 0; c < CPG; ++c) {
           const uint4 sv = __ldg(cs + c);
-          x[c].x = pack_T<DT>(fmul_rn(lo_f<DT>(x[c].x), lo_f<DT>(sv.x)), fmul_rn(hi_f<DT>(x[c].x), hi_f<DT>(sv.x)));
-          x[c].y = pack_T<DT>(fmul_rn(lo_f<DT>(x[c].y), lo_f<DT>(sv.y)), fmul_rn(hi_f<DT>(x[c].y), hi_f<DT>(sv.y)));
-          x[c].z = pack_T<DT>(fmul_rn(lo_f<DT>(x[c].z), lo_f<DT>(sv.z)), fmul_rn(hi_f<DT>(x[c].z), hi_f<DT>(sv.z)));
-          x[c].w = pack_T<DT>(fmul_rn(lo_f<DT>(x[c].w), lo_f<DT>(sv.w)), fmul_rn(hi_f<DT>(x[c].w), hi_f<DT>(sv.w)));
+          x[c].x = pack_pair<DT>(fmul_rn(pair_lo<DT>(x[c].x), pair_lo<DT>(sv.x)), fmul_rn(pair_hi<DT>(x[c].x), pair_hi<DT>(sv.x)));
+          x[c].y = pack_pair<DT>(fmul_rn(pair_lo<DT>(x[c].y), pair_lo<DT>(sv.y)), fmul_rn(pair_hi<DT>(x[c].y), pair_hi<DT>(sv.y)));
+          x[c].z = pack_pair<DT>(fmul_rn(pair_lo<DT>(x[c].z), pair_lo<DT>(sv.z)), fmul_rn(pair_hi<DT>(x[c].z), pair_hi<DT>(sv.z)));
+          x[c].w = pack_pair<DT>(fmul_rn(pair_lo<DT>(x[c].w), pair_lo<DT>(sv.w)), fmul_rn(pair_hi<DT>(x[c].w), pair_hi<DT>(sv.w)));
         }
       }
       uint32_t mn2 = x[0].x, mx2 = x[0].x;
@@ -586,8 +566,8 @@ quant_group_fast_kernel(QuantArgs a, int64_t total_groups) {
         mn2 = min2<DT>(min2<DT>(mn2, x[c].x), min2<DT>(x[c].y, min2<DT>(x[c].z, x[c].w)));
         mx2 = max2<DT>(max2<DT>(mx2, x[c].x), max2<DT>(x[c].y, max2<DT>(x[c].z, x[c].w)));
       }
-      const float mn = fminf(lo_f<DT>(mn2), hi_f<DT>(mn2));
-      const float mx = fmaxf(lo_f<DT>(mx2), hi_f<DT>(mx2));
+      const float mn = fminf(pair_lo<DT>(mn2), pair_hi<DT>(mn2));
+      const float mx = fmaxf(pair_lo<DT>(mx2), pair_hi<DT>(mx2));
       float s, z;
       qparams<DType<DT>>(mn, mx, a.sym, 1, a.qmin, a.qmax, s, z);
       DType<DT>::store(a.scales, g, s);
@@ -695,8 +675,8 @@ quant_row_fast_kernel(QuantArgs a) {
 #pragma unroll
     for (int w = 1; w < 8; ++w) { mn2 = min2<DT>(mn2, smn[w]); mx2 = max2<DT>(mx2, smx[w]); }
     __syncthreads();
-    const float mn = fminf(lo_f<DT>(mn2), hi_f<DT>(mn2));
-    const float mx = fmaxf(lo_f<DT>(mx2), hi_f<DT>(mx2));
+    const float mn = fminf(pair_lo<DT>(mn2), pair_hi<DT>(mn2));
+    const float mx = fmaxf(pair_lo<DT>(mx2), pair_hi<DT>(mx2));
     float s, z;
     qparams<DType<DT>>(mn, mx, a.sym, 1, a.qmin, a.qmax, s, z);
     if (t == 0) {

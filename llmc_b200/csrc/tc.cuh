@@ -151,6 +151,58 @@ __device__ __forceinline__ void wgmma_m64n128k16(float (&d)[64], uint64_t adesc,
   else wgmma_m64n128k16_f16<kTransA, kTransB>(d, adesc, bdesc, accumulate);
 }
 
+// ---- forward GEMMs (gemm.cu, gemm_w4.cu) -------------------------------------------------------
+// L2-grouped tile order: the weights are swept in groups of `gn` n-tiles (<= ~32 MB, L2 resident,
+// see l2_group_width), all m-tiles per group, n fastest inside the group.  Activations are re-read
+// once per group from HBM, weights once; n-fastest over a 14336-row weight would instead stream
+// the whole 117 MB weight through L2 once per 132-tile wave.
+__device__ __forceinline__ void grouped_tile(int u, int m_tiles, int n_tiles, int gn, int& m_blk,
+                                             int& n_blk) {
+  const int per_group = gn * m_tiles;
+  const int g = u / per_group;
+  const int rem = u - g * per_group;
+  const int gsz = min(gn, n_tiles - g * gn);
+  m_blk = rem / gsz;
+  n_blk = g * gn + (rem - m_blk * gsz);
+}
+
+// The F.linear epilogue: stores this thread's part of an m64n128 accumulator fragment (layout at
+// wgmma_m64n128k16_bf16) whose element (0, 0) is Y[row0][col0] of the DT matrix Y[M, N] with row
+// stride ld.  The bias (DT, may be null) is added in fp32 before the single rounding, as F.linear
+// does.  Column pairs are stored as one 32-bit word when ld is even, element by element otherwise.
+template <int DT>
+__device__ __forceinline__ void store_linear_m64n128(const float (&acc)[64], int64_t row0,
+                                                     int64_t col0, int64_t M, int64_t N, int64_t ld,
+                                                     const void* bias, void* out) {
+  const int tid = threadIdx.x & 127, lane = threadIdx.x & 31;
+  const uint16_t* bs = static_cast<const uint16_t*>(bias);
+#pragma unroll
+  for (int j = 0; j < 16; ++j) {
+    const int64_t col = col0 + 8 * j + 2 * (lane & 3);
+    if (col >= N) continue;
+    const bool pair = col + 1 < N;
+    float b0 = 0.f, b1 = 0.f;                    // loaded once per column pair
+    if (bs != nullptr) {
+      b0 = widen16<DT>(bs[col]);
+      if (pair) b1 = widen16<DT>(bs[col + 1]);
+    }
+#pragma unroll
+    for (int i = 0; i < 2; ++i) {
+      const int64_t row = row0 + (tid >> 5) * 16 + (lane >> 2) + 8 * i;
+      if (row >= M) continue;
+      float v0 = acc[4 * j + 2 * i], v1 = acc[4 * j + 2 * i + 1];
+      if (bs != nullptr) { v0 += b0; v1 += b1; }
+      const uint32_t pk = pack_pair<DT>(v0, v1);
+      uint16_t* o = static_cast<uint16_t*>(out) + row * ld + col;
+      if (pair && (ld & 1) == 0) *reinterpret_cast<uint32_t*>(o) = pk;
+      else {
+        o[0] = static_cast<uint16_t>(pk & 0xffffu);
+        if (pair) o[1] = static_cast<uint16_t>(pk >> 16);
+      }
+    }
+  }
+}
+
 }  // namespace tc
 
 // ---- host helpers shared across translation units ---------------------------------------------
@@ -161,7 +213,28 @@ int encode_tmap_2d(CUtensorMap* out, const void* base, CUtensorMapDataType dtype
                    uint64_t rows, uint64_t cols, uint64_t ld_elems, uint32_t box_rows,
                    uint32_t box_cols, CUtensorMapSwizzle swizzle);
 
+// Width in n-tiles of a group of tc::grouped_tile: as many n-tiles of weights as 32 MB of L2
+// holds, given the bytes one n-tile takes (divisor > 0), and at least one, at most n_tiles.
+inline int l2_group_width(int64_t divisor, int n_tiles) {
+  int64_t gn = (32ll << 20) / divisor;
+  if (gn < 1) gn = 1;
+  if (gn > n_tiles) gn = n_tiles;
+  return static_cast<int>(gn);
+}
+
 // tf32.cu: 3xTF32 rank-K updates (see there) and the tf32 split hi = tf32(x), lo = tf32(x - hi).
+// tf32_split(x) is that split of one element (.x = hi, .y = lo), tf32 rounding to nearest with
+// ties away from zero (cvt.rna); hi + lo carries x to ~2^-22 relative.  The 3xTF32 update's error
+// bound and the oracle's tf32_split assume exactly this format.
+__device__ __forceinline__ float tf32_rna(float x) {
+  uint32_t r;
+  asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(r) : "f"(x));
+  return __uint_as_float(r);
+}
+__device__ __forceinline__ float2 tf32_split(float x) {
+  const float hi = tf32_rna(x);
+  return make_float2(hi, tf32_rna(x - hi));
+}
 // A GEMM operand held as its tf32 split: element (i, k) at [i * ld + k] (K-major) or, mn = true,
 // at [k * ld + i] (MN-major); i indexes M (operand A) or N (operand B).
 struct SplitOperand {

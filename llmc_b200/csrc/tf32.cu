@@ -73,12 +73,6 @@ __device__ __forceinline__ void decode(const Params& p, int u, int& m_blk, int& 
   n_blk = u;
 }
 
-__device__ __forceinline__ float to_tf32(float x) {
-  uint32_t r;
-  asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(r) : "f"(x));
-  return __uint_as_float(r);
-}
-
 // byte offset of element (i, k) inside an operand tile as TMA wrote it (SWIZZLE_128B: 16-byte
 // chunk c of a 128-byte row r sits at chunk c ^ (r & 7))
 template <bool kMn>
@@ -247,12 +241,13 @@ tf32x3_kernel(const __grid_constant__ CUtensorMap tmAhi, const __grid_constant__
           if (p.Chi != nullptr && (row < p.split_rows || col < p.split_cols)) {
             float* hp = p.Chi + row * p.ldc + col;
             float* lp = p.Clo + row * p.ldc + col;
-            const float h0 = to_tf32(v0), h1 = to_tf32(v1);
-            hp[0] = h0;
-            lp[0] = to_tf32(v0 - h0);
+            const float2 s0 = tf32_split(v0);
+            hp[0] = s0.x;
+            lp[0] = s0.y;
             if (pair) {
-              hp[1] = h1;
-              lp[1] = to_tf32(v1 - h1);
+              const float2 s1 = tf32_split(v1);
+              hp[1] = s1.x;
+              lp[1] = s1.y;
             }
           }
         }
@@ -268,10 +263,9 @@ split_tf32_kernel(const float* __restrict__ x, int64_t rows, int64_t cols, int64
   for (int64_t i = static_cast<int64_t>(blockIdx.x) * blockDim.x + threadIdx.x; i < total;
        i += static_cast<int64_t>(gridDim.x) * blockDim.x) {
     const int64_t r = i / cols, c = i - r * cols;
-    const float v = x[r * ld + c];
-    const float h = to_tf32(v);
-    hi[r * ld_out + c] = h;
-    lo[r * ld_out + c] = to_tf32(v - h);
+    const float2 s = tf32_split(x[r * ld + c]);
+    hi[r * ld_out + c] = s.x;
+    lo[r * ld_out + c] = s.y;
   }
 }
 

@@ -14,7 +14,8 @@ def _lin(x, w, b=None):
 
 @pytest.mark.parametrize('dtype', [torch.bfloat16, torch.float16])
 @pytest.mark.parametrize('M,N,K', [(128, 256, 64), (256, 512, 128), (2048, 4096, 4096),
-                                   (1000, 768, 3072), (77, 264, 200), (4096, 1024, 4096)])
+                                   (1000, 768, 3072), (77, 264, 200), (4096, 1024, 4096),
+                                   (77, 263, 200)])
 def test_gemm_matches_fp32_reference(dtype, M, N, K):
     torch.manual_seed(M + N + K)
     x = torch.randn(M, K, device='cuda').to(dtype)

@@ -21,7 +21,8 @@ def _pack_unsigned(codes_u):
 @pytest.mark.parametrize('dtype', [torch.bfloat16, torch.float16])
 @pytest.mark.parametrize('sym', [True, False])
 @pytest.mark.parametrize('M,N,K,g', [(128, 256, 128, 128), (300, 520, 512, 128), (2048, 4096, 4096, 128),
-                                     (512, 1024, 1024, 64), (4096, 14336, 4096, 128)])
+                                     (512, 1024, 1024, 64), (4096, 14336, 4096, 128),
+                                     (300, 519, 512, 128)])
 def test_fused_equals_materialised(dtype, sym, M, N, K, g, native):
     """native: qparams handed over in the activation dtype -> packed half2 / bf16x2 dequant;
     otherwise as fp32 -> fp32 dequant.  Both must reproduce the materialised weight bit for bit."""
