@@ -73,18 +73,106 @@ __device__ __forceinline__ void decode(const Params& p, int u, int& m_blk, int& 
   n_blk = u;
 }
 
-// byte offset of element (i, k) inside an operand tile as TMA wrote it (SWIZZLE_128B: 16-byte
-// chunk c of a 128-byte row r sits at chunk c ^ (r & 7))
-template <bool kMn>
-__device__ __forceinline__ uint32_t tile_off(int i, int k) {
-  if constexpr (!kMn)   // rows = i, 32 k per 128-byte row
-    return i * 128 + ((((k >> 2) ^ (i & 7)) << 4) | ((k & 3) << 2));
-  else                  // boxes of 32 i; rows = k
-    return (i >> 5) * kBoxBytes + k * 128 + (((((i & 31) >> 2) ^ (k & 7)) << 4) | ((i & 3) << 2));
+// Operand tiles as TMA wrote them (SWIZZLE_128B: 16-byte chunk c of a 128-byte row r sits at
+// chunk c ^ (r & 7)), every tile 1024-byte aligned:
+//   K-major : element (i, k) at  i * 128 + (((k / 4) ^ (i % 8)) * 16) + (k % 4) * 4
+//   MN-major: element (i, k) at  (i / 32) * kBoxBytes + k * 128 + ((((i % 32) / 4) ^ (k % 8)) * 16) + (i % 4) * 4
+// The mma.m16n8k8 tf32 fragments of lane (g = lane / 4, t = lane % 4) are
+//   A: a0 = (g, t), a1 = (g + 8, t), a2 = (g, t + 4), a3 = (g + 8, t + 4)     (i, k)
+//   B: b0 = (g, t), b1 = (g, t + 4)
+// K-major: an 8 x 4 block of tf32 (8 rows of one 16-byte chunk) is, read as b16, exactly one
+// ldmatrix 8 x 8 matrix with the (g, t) element in lane 4 g + t, so A is one ldmatrix.x4 and two B
+// fragments are another; the 8 row addresses of each matrix hit 8 different chunks (conflict free).
+// MN-major: 32-bit loads.  For a k8 step kk (kk % 8 == 0) the swizzle term k % 8 does not depend
+// on kk, so each lane's offsets are fixed and a k step only adds kk * 128.
+__device__ __forceinline__ void ldsm_x4(uint32_t (&r)[4], uint32_t addr) {
+  asm volatile("ldmatrix.sync.aligned.m8n8.x4.shared.b16 {%0, %1, %2, %3}, [%4];"
+               : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3])
+               : "r"(addr)
+               : "memory");
 }
 
-__device__ __forceinline__ uint32_t lds_u32(const uint8_t* base, uint32_t off) {
-  return *reinterpret_cast<const uint32_t*>(base + off);
+__device__ __forceinline__ uint32_t lds_u32(uint32_t addr) {
+  uint32_t v;
+  asm volatile("ld.shared.b32 %0, [%1];" : "=r"(v) : "r"(addr) : "memory");
+  return v;
+}
+
+__device__ __forceinline__ void prefetch_l2(const void* p) {
+  asm volatile("prefetch.global.L2 [%0];" ::"l"(p));
+}
+
+// Per-lane byte offsets of this warp's fragments inside an operand tile.
+//   A K-major : a[s]  = ldmatrix row address for k8 step s (rows 64 wm + .., mt adds mt * 2048)
+//   A MN-major: a[ih] = element (64 wm + g + 8 ih, t); (mt, kh, s) only add constants
+//   B K-major : b[s]  = ldmatrix row address for k8 step s (cols 32 wn + .., pair np adds np * 2048)
+//   B MN-major: b[nt] = element (32 wn + 8 nt + g, t); kh = 1 is b[nt ^ 2] + 512
+template <bool kAmn, bool kBmn>
+struct LaneOffsets {
+  uint32_t a[4], b[4];
+  __device__ __forceinline__ LaneOffsets(int wm, int wn, int lane) {
+    const int g = lane >> 2, t = lane & 3, r = lane & 7;
+#pragma unroll
+    for (int s = 0; s < 4; ++s) {
+      if constexpr (!kAmn) {
+        const int row = wm * 64 + r + 8 * ((lane >> 3) & 1);
+        a[s] = row * 128 + (((2 * s + (lane >> 4)) ^ r) << 4);
+      } else {
+        a[s] = s < 2 ? wm * 2 * kBoxBytes + t * 128 + ((((2 * s + (g >> 2)) ^ t)) << 4) + (g & 3) * 4 : 0;
+      }
+      if constexpr (!kBmn) {
+        const int row = wn * 32 + r + 8 * (lane >> 4);
+        b[s] = row * 128 + (((2 * s + ((lane >> 3) & 1)) ^ r) << 4);
+      } else {
+        b[s] = wn * kBoxBytes + t * 128 + (((2 * s) ^ (g >> 2) ^ t) << 4) + (g & 3) * 4;
+      }
+    }
+  }
+};
+
+// A fragment (hi and lo) of k8 step s for the warp's 16-row block mt (both compile-time after
+// unrolling)
+template <bool kMn>
+__device__ __forceinline__ void load_a(uint32_t (&fa)[2][4], uint32_t hi, uint32_t lo,
+                                       const uint32_t (&off)[4], int mt, int s) {
+  if constexpr (!kMn) {
+    ldsm_x4(fa[0], hi + mt * 2048 + off[s]);
+    ldsm_x4(fa[1], lo + mt * 2048 + off[s]);
+  } else {
+#pragma unroll
+    for (int q = 0; q < 4; ++q) {   // q = ih + 2 kh
+      const int ih = q & 1, kh = q >> 1;
+      const uint32_t o = off[ih] + (mt >> 1) * kBoxBytes + kh * 512 + (((mt & 1) ^ kh) << 6) + s * 1024;
+      fa[0][q] = lds_u32(hi + o);
+      fa[1][q] = lds_u32(lo + o);
+    }
+  }
+}
+
+// B fragments (hi and lo) of k8 step s for the warp's four 8-column blocks
+template <bool kMn>
+__device__ __forceinline__ void load_b(uint32_t (&fb)[4][2][2], uint32_t hi, uint32_t lo,
+                                       const uint32_t (&off)[4], int s) {
+  if constexpr (!kMn) {
+#pragma unroll
+    for (int np = 0; np < 2; ++np) {
+      uint32_t h[4], l[4];
+      ldsm_x4(h, hi + np * 2048 + off[s]);
+      ldsm_x4(l, lo + np * 2048 + off[s]);
+#pragma unroll
+      for (int q = 0; q < 2; ++q) {
+        fb[2 * np + q][0][0] = h[2 * q]; fb[2 * np + q][0][1] = h[2 * q + 1];
+        fb[2 * np + q][1][0] = l[2 * q]; fb[2 * np + q][1][1] = l[2 * q + 1];
+      }
+    }
+  } else {
+#pragma unroll
+    for (int nt = 0; nt < 4; ++nt) {
+      const uint32_t o0 = off[nt] + s * 1024, o1 = off[nt ^ 2] + 512 + s * 1024;
+      fb[nt][0][0] = lds_u32(hi + o0); fb[nt][0][1] = lds_u32(hi + o1);
+      fb[nt][1][0] = lds_u32(lo + o0); fb[nt][1][1] = lds_u32(lo + o1);
+    }
+  }
 }
 
 __device__ __forceinline__ void mma_tf32(float (&d)[4], const uint32_t (&a)[4], const uint32_t (&b)[2]) {
@@ -100,9 +188,12 @@ __global__ void __launch_bounds__(kThreads, 1)
 tf32x3_kernel(const __grid_constant__ CUtensorMap tmAhi, const __grid_constant__ CUtensorMap tmAlo,
               const __grid_constant__ CUtensorMap tmBhi, const __grid_constant__ CUtensorMap tmBlo,
               const Params p) {
-  extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) &
-                                             ~static_cast<uintptr_t>(1023));
+  extern __shared__ __align__(1024) uint8_t smem_raw[];
+  // 1024-byte aligned ring (swizzle atoms).  Offsetting the array keeps `smem` a pointer the
+  // compiler knows to be shared; the MMA warps address the ring by 32-bit shared addresses.
+  const uint32_t raw = smem_u32(smem_raw);
+  uint8_t* smem = smem_raw + (((raw + 1023u) & ~1023u) - raw);
+  const uint32_t ring = smem_u32(smem);
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + kStages * kStageBytes);
   uint64_t* empty_bar = full_bar + kStages;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -110,7 +201,7 @@ tf32x3_kernel(const __grid_constant__ CUtensorMap tmAhi, const __grid_constant__
 
   if (threadIdx.x == 0) {
     prefetch_tmap(&tmAhi); prefetch_tmap(&tmAlo); prefetch_tmap(&tmBhi); prefetch_tmap(&tmBlo);
-    for (int s = 0; s < kStages; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], kMmaWarps); }
+    for (int s = 0; s < kStages; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], 1); }
     fence_barrier_init();
   }
   __syncthreads();
@@ -160,11 +251,27 @@ tf32x3_kernel(const __grid_constant__ CUtensorMap tmAhi, const __grid_constant__
   // ===================== MMA warps: warp (wm, wn) owns rows 64 wm .. +63, cols 32 wn .. +31 =====
   const int wm = warp >> 2, wn = warp & 3;
   const int g = lane >> 2, t = lane & 3;
+  const LaneOffsets<kAmn, kBmn> off(wm, wn, lane);
   int stage = 0;
   uint32_t phase = 0;
   for (int u = blockIdx.x; u < p.num_units; u += gridDim.x) {
     int m_blk, n_blk;
     decode(p, u, m_blk, n_blk);
+    const int64_t row0 = static_cast<int64_t>(m_blk) * BM + wm * 64;
+    const int64_t col0 = static_cast<int64_t>(n_blk) * BN + wn * 32;
+    if (p.mode == 0 && col0 < p.N) {
+      // pull this warp's 64 x 32 block of C into L2 while the MMAs run: two rows per lane, the
+      // first and last column of each (a row segment spans at most two 128-byte lines)
+      const int64_t last = (col0 + 31 < p.N ? col0 + 31 : p.N - 1) - col0;
+#pragma unroll
+      for (int r = 0; r < 2; ++r) {
+        const int64_t row = row0 + 2 * lane + r;
+        if (row < p.M) {
+          prefetch_l2(p.C + row * p.ldc + col0);
+          prefetch_l2(p.C + row * p.ldc + col0 + last);
+        }
+      }
+    }
     float acc[4][4][4];
 #pragma unroll
     for (int a = 0; a < 4; ++a)
@@ -174,56 +281,80 @@ tf32x3_kernel(const __grid_constant__ CUtensorMap tmAhi, const __grid_constant__
         for (int c = 0; c < 4; ++c) acc[a][b][c] = 0.f;
     for (int kb = 0; kb < kb_total; ++kb) {
       mbar_wait(&full_bar[stage], phase);
-      const uint8_t* ahi = smem + stage * kStageBytes;
-      const uint8_t* alo = ahi + kABytes;
-      const uint8_t* bhi = alo + kABytes;
-      const uint8_t* blo = bhi + kBBytes;
-#pragma unroll 1
-      for (int kk = 0; kk < BK; kk += 8) {
-        uint32_t fbh[4][2], fbl[4][2];
+      const uint32_t ahi = ring + stage * kStageBytes, alo = ahi + kABytes;
+      const uint32_t bhi = alo + kABytes, blo = bhi + kBBytes;
+      // Fragments are double-buffered: B per k8 step (s), A per (s, 16-row block mt), so the next
+      // fragments load while the current ones feed the MMAs.  Every accumulator sees hi*hi,
+      // lo*hi, hi*lo per k8 step, k ascending.
+      uint32_t fa[2][2][4], fb[2][4][2][2];
+      load_b<kBmn>(fb[0], bhi, blo, off.b, 0);
+      load_a<kAmn>(fa[0], ahi, alo, off.a, 0, 0);
 #pragma unroll
-        for (int nt = 0; nt < 4; ++nt) {
-          const int j = wn * 32 + nt * 8 + g;
-          const uint32_t o0 = tile_off<kBmn>(j, kk + t), o1 = tile_off<kBmn>(j, kk + t + 4);
-          fbh[nt][0] = lds_u32(bhi, o0); fbh[nt][1] = lds_u32(bhi, o1);
-          fbl[nt][0] = lds_u32(blo, o0); fbl[nt][1] = lds_u32(blo, o1);
-        }
+      for (int s = 0; s < BK / 8; ++s) {
 #pragma unroll
         for (int mt = 0; mt < 4; ++mt) {
-          const int i0 = wm * 64 + mt * 16 + g;
-          const uint32_t o0 = tile_off<kAmn>(i0, kk + t), o1 = tile_off<kAmn>(i0 + 8, kk + t);
-          const uint32_t o2 = tile_off<kAmn>(i0, kk + t + 4), o3 = tile_off<kAmn>(i0 + 8, kk + t + 4);
-          const uint32_t fah[4] = {lds_u32(ahi, o0), lds_u32(ahi, o1), lds_u32(ahi, o2), lds_u32(ahi, o3)};
-          const uint32_t fal[4] = {lds_u32(alo, o0), lds_u32(alo, o1), lds_u32(alo, o2), lds_u32(alo, o3)};
+          const int q = 4 * s + mt;
+          if (mt == 0 && s + 1 < BK / 8) load_b<kBmn>(fb[(s + 1) & 1], bhi, blo, off.b, s + 1);
+          if (q + 1 < BK / 2) load_a<kAmn>(fa[(q + 1) & 1], ahi, alo, off.a, (q + 1) & 3, (q + 1) >> 2);
 #pragma unroll
           for (int nt = 0; nt < 4; ++nt) {
-            mma_tf32(acc[mt][nt], fah, fbh[nt]);
-            mma_tf32(acc[mt][nt], fal, fbh[nt]);
-            mma_tf32(acc[mt][nt], fah, fbl[nt]);
+            mma_tf32(acc[mt][nt], fa[q & 1][0], fb[s & 1][nt][0]);
+            mma_tf32(acc[mt][nt], fa[q & 1][1], fb[s & 1][nt][0]);
+            mma_tf32(acc[mt][nt], fa[q & 1][0], fb[s & 1][nt][1]);
           }
         }
       }
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&empty_bar[stage]);
+      // Free the stage only once every MMA thread's reads of it are performed.  ptxas schedules
+      // the arrive above MMAs whose fragment loads may still be in flight, and neither the
+      // arrive nor a warp sync waits for them; bar.sync does (it orders all prior shared-memory
+      // accesses of the participating threads before it).
+      asm volatile("bar.sync 1, %0;" ::"n"(kMmaWarps * 32) : "memory");
+      if (threadIdx.x == 0) mbar_arrive(&empty_bar[stage]);
       if (++stage == kStages) { stage = 0; phase ^= 1; }
     }
 
     // ---- epilogue: fragment element (mt, nt, 2 i + c) = C[row g + 8 i][col 2 t + c] ----
+    // A warp whose 64 x 32 block lies inside C with 8-byte aligned pairs reads all of it before
+    // the first store and folds it into the accumulators (C - acc, one rounding as below); the
+    // stores could alias the reads, so interleaved the compiler would wait out one memory round
+    // trip per element pair.  Ragged or misaligned blocks read each pair right before its store.
+    const bool folded = p.mode == 0 && row0 + 64 <= p.M && col0 + 32 <= p.N && (p.ldc & 1) == 0 &&
+                        (reinterpret_cast<uintptr_t>(p.C) & 7) == 0;
+    if (folded) {
+      float2 old[4][2][4];
+#pragma unroll
+      for (int mt = 0; mt < 4; ++mt)
+#pragma unroll
+        for (int i = 0; i < 2; ++i) {
+          const float* cp = p.C + (row0 + mt * 16 + g + 8 * i) * p.ldc + col0 + 2 * t;
+#pragma unroll
+          for (int nt = 0; nt < 4; ++nt) old[mt][i][nt] = *reinterpret_cast<const float2*>(cp + nt * 8);
+        }
+#pragma unroll
+      for (int mt = 0; mt < 4; ++mt)
+#pragma unroll
+        for (int i = 0; i < 2; ++i)
+#pragma unroll
+          for (int nt = 0; nt < 4; ++nt) {
+            acc[mt][nt][2 * i] = old[mt][i][nt].x - acc[mt][nt][2 * i];
+            acc[mt][nt][2 * i + 1] = old[mt][i][nt].y - acc[mt][nt][2 * i + 1];
+          }
+    }
 #pragma unroll
     for (int mt = 0; mt < 4; ++mt) {
 #pragma unroll
       for (int i = 0; i < 2; ++i) {
-        const int64_t row = static_cast<int64_t>(m_blk) * BM + wm * 64 + mt * 16 + g + 8 * i;
+        const int64_t row = row0 + mt * 16 + g + 8 * i;
         if (row >= p.M) continue;
 #pragma unroll
         for (int nt = 0; nt < 4; ++nt) {
-          const int64_t col = static_cast<int64_t>(n_blk) * BN + wn * 32 + nt * 8 + 2 * t;
+          const int64_t col = col0 + nt * 8 + 2 * t;
           if (col >= p.N) continue;
           const bool pair = col + 1 < p.N;
           float* cp = p.C + row * p.ldc + col;
           const bool vec = pair && (reinterpret_cast<uintptr_t>(cp) & 7) == 0;
           float v0 = acc[mt][nt][2 * i], v1 = acc[mt][nt][2 * i + 1];
-          if (p.mode == 0) {
+          if (p.mode == 0 && !folded) {
             if (vec) {
               const float2 o = *reinterpret_cast<const float2*>(cp);
               v0 = o.x - v0;
@@ -241,13 +372,17 @@ tf32x3_kernel(const __grid_constant__ CUtensorMap tmAhi, const __grid_constant__
           if (p.Chi != nullptr && (row < p.split_rows || col < p.split_cols)) {
             float* hp = p.Chi + row * p.ldc + col;
             float* lp = p.Clo + row * p.ldc + col;
-            const float2 s0 = tf32_split(v0);
-            hp[0] = s0.x;
-            lp[0] = s0.y;
-            if (pair) {
-              const float2 s1 = tf32_split(v1);
-              hp[1] = s1.x;
-              lp[1] = s1.y;
+            const float2 s0 = tf32_split(v0), s1 = tf32_split(v1);
+            if (vec && ((reinterpret_cast<uintptr_t>(hp) | reinterpret_cast<uintptr_t>(lp)) & 7) == 0) {
+              *reinterpret_cast<float2*>(hp) = make_float2(s0.x, s1.x);
+              *reinterpret_cast<float2*>(lp) = make_float2(s0.y, s1.y);
+            } else {
+              hp[0] = s0.x;
+              lp[0] = s0.y;
+              if (pair) {
+                hp[1] = s1.x;
+                lp[1] = s1.y;
+              }
             }
           }
         }
