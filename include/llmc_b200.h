@@ -356,14 +356,36 @@ int llmc_fp8_quant(const void* w, int64_t rows, int64_t cols, int dtype, int64_t
  *       (fp32, written to scales [ceil(M/block), ceil(N/block)]), q = fp8(x.float() / scale);
  *       out_mode 0 scales only | 1 QDQ (`dtype`) | 2 fp8 bytes.
  *   llmc_fp8_block_dequant  weight_cast_to_bf16 (quant.py:18-29): bf16(fp8.float() * scale_inv).
- *   (The reference's Triton act_quant / fp8_gemm pair, kernel.py:31-53, 141-242, is not built: the
- *   forward of LlmcFp8Linear dequantises once and runs the bf16 wgmma GEMM, the reference's own
- *   non-Triton branch, module_utils.py:171-178.)
+ *   (LlmcFp8Linear dequantises once with llmc_fp8_block_dequant and runs the bf16 wgmma GEMM — the
+ *   reference's non-Hopper branch, module_utils.py:171-178 — unless its USE_FP8GEMM_KERNEL switch
+ *   selects the FP8 tensor-core forward below.)
  * ------------------------------------------------------------------------------------ */
 int llmc_fp8_block_quant(const void* w, int64_t M, int64_t N, int dtype, int block, int e5m2,
                          float* scales, int out_mode, void* out, void* stream);
 int llmc_fp8_block_dequant(const void* w_fp8, int64_t M, int64_t N, int block, int e5m2,
                            const float* scale_inv, void* out_bf16, void* stream);
+
+/* ------------------------------------------------------------------------------------
+ * Block-FP8 linear forward on the FP8 tensor cores: the reference's Triton act_quant / fp8_gemm
+ *   pair (kernel.py:7-53, 153-242) behind block_wise_fp8_forward_func (module_utils.py:40-45).
+ *   llmc_fp8_act_quant  (csrc/fp8.cu) x [rows, K] `dtype`, K % 128 == 0: per contiguous group of 128
+ *       elements s = max|x| / 448 and y = e4m3(x / s), both divisions the approximate div.full.f32
+ *       the reference's kernel compiles to, the cast cvt.rn.satfinite; y [rows, K] e4m3 bytes,
+ *       scales [rows, K/128] fp32.  No clamp: an all-zero group gives s = 0 and NaN codes.
+ *   llmc_gemm_fp8_block (csrc/gemm_fp8.cu) out[M, N] = sum over 128-deep K blocks kb, ascending,
+ *       acc = fma(dot_kb * a_s[m, kb], b_s[n / 128, kb], acc), the dot on wgmma e4m3 (Hopper's
+ *       reduced-precision accumulator, fresh per K block).  a [M, K], b [N, K] e4m3 (K-major),
+ *       a_s [M, K/128], b_s [ceil(N/128), K/128] fp32; K % 128 == 0, N >= 1, M == 0 is a no-op.
+ *       out_dtype LLMC_F32: out = acc (fp8_gemm's default-dtype output; bias must be NULL).
+ *       out_dtype LLMC_BF16: out = bf16(acc), or with a bias [N] of `bias_dtype` (F32 / F16 / BF16)
+ *       bf16(float(bf16(acc)) + float(bias)) — the rounding, then the bias, as module_utils.py:42-44.
+ *       Each output element's arithmetic does not depend on M, N or the tile schedule.
+ * ------------------------------------------------------------------------------------ */
+int llmc_fp8_act_quant(const void* x, int64_t rows, int64_t K, int dtype, void* y, float* scales,
+                       void* stream);
+int llmc_gemm_fp8_block(const void* a, const float* a_s, const void* b, const float* b_s,
+                        const void* bias, int bias_dtype, void* out, int out_dtype, int64_t M,
+                        int64_t N, int64_t K, void* stream);
 
 /* ------------------------------------------------------------------------------------
  * Block-forward glue (csrc/block_ops.cu) for F2 block_forward

@@ -235,3 +235,85 @@ extern "C" int llmc_fp8_block_dequant(const void* w_fp8, int64_t M, int64_t N, i
   LLMC_CHECK_LAUNCH();
   return LLMC_OK;
 }
+
+// ---- 1 x 128 activation quantiser: act_quant (kernel.py:7-53), the input side of fp8_gemm ----------
+// Per contiguous group of 128 elements, in fp32: s = max|x| / 448, y = e4m3(x / s).  The reference's
+// Triton kernel compiles both divisions on sm_90 to the approximate `div.full.f32` (<= 2 ulp), not
+// IEEE div.rn, the max to `max.f32` and the cast to `cvt.rn.satfinite.e4m3x2.f32`; the same
+// instructions are issued here, so scales and codes match the reference's bit for bit on the same
+// hardware.  Reproduced quirk: unlike weight_cast_to_fp8 there is no clamp(min=1e-5), so an
+// all-zero group gets s = 0 and NaN codes (0 / 0), which fp8_gemm spreads over its output row.
+// Half a warp per group, 8 elements per lane: one 16-byte load (two for fp32), one 8-byte store.
+namespace llmc {
+
+__device__ __forceinline__ float div_full(float a, float b) {
+  float r;
+  asm("div.full.f32 %0, %1, %2;" : "=f"(r) : "f"(a), "f"(b));
+  return r;
+}
+
+// two e4m3 codes in one 16-bit word, `lo` in the low byte (the lower address)
+__device__ __forceinline__ uint32_t e4m3x2(float lo, float hi) {
+  uint16_t r;
+  asm("cvt.rn.satfinite.e4m3x2.f32 %0, %1, %2;" : "=h"(r) : "f"(hi), "f"(lo));
+  return r;
+}
+
+template <int DT>
+__global__ void __launch_bounds__(256)
+fp8_act_quant_kernel(const void* __restrict__ x, int64_t groups, uint8_t* __restrict__ y,
+                     float* __restrict__ scales) {
+  // the loop bound is uniform across a warp (both halves shuffle together)
+  const int64_t warp = (static_cast<int64_t>(blockIdx.x) * blockDim.x + threadIdx.x) >> 5;
+  const int64_t nwarps = (static_cast<int64_t>(gridDim.x) * blockDim.x) >> 5;
+  const int half = (threadIdx.x >> 4) & 1, sub = threadIdx.x & 15;
+  for (int64_t g0 = 2 * warp; g0 < groups; g0 += 2 * nwarps) {
+    const int64_t g = g0 + half;
+    const bool live = g < groups;
+    const int64_t base = g * 128 + sub * 8;
+    float v[8];
+    if (live) load8<DT>(x, base, v);
+    else {
+#pragma unroll
+      for (int i = 0; i < 8; ++i) v[i] = 0.f;
+    }
+    float mx = 0.f;
+#pragma unroll
+    for (int i = 0; i < 8; ++i) mx = fmaxf(mx, fabsf(v[i]));
+    mx = warp_max(mx, 16);
+    const float s = div_full(mx, 448.f);
+    if (!live) continue;
+    uint32_t w[2];
+#pragma unroll
+    for (int h = 0; h < 2; ++h)
+      w[h] = e4m3x2(div_full(v[4 * h], s), div_full(v[4 * h + 1], s)) |
+             (e4m3x2(div_full(v[4 * h + 2], s), div_full(v[4 * h + 3], s)) << 16);
+    *reinterpret_cast<uint2*>(y + base) = make_uint2(w[0], w[1]);
+    if (sub == 0) scales[g] = s;
+  }
+}
+
+}  // namespace llmc
+
+extern "C" int llmc_fp8_act_quant(const void* x, int64_t rows, int64_t K, int dtype, void* y,
+                                  float* scales, void* stream) {
+  LLMC_CHECK_ARG(rows >= 0 && K >= 1, "fp8_act_quant: bad shape rows=%lld K=%lld", (long long)rows,
+                 (long long)K);
+  LLMC_CHECK_ARG(K % 128 == 0, "fp8_act_quant: K=%lld must be a multiple of 128", (long long)K);
+  LLMC_CHECK_ARG(dtype >= LLMC_F32 && dtype <= LLMC_BF16, "fp8_act_quant: bad dtype %d", dtype);
+  if (rows == 0) return LLMC_OK;
+  LLMC_CHECK_ARG(x && y && scales, "fp8_act_quant: null pointer");
+  if (!aligned16(x) || !aligned16(y)) {
+    set_last_error("fp8_act_quant: x and y must be 16-byte aligned");
+    return LLMC_EALIGN;
+  }
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  const int64_t groups = rows * (K / 128);
+  int64_t blocks = (groups + 15) / 16;                 // 16 groups per 256-thread block
+  if (blocks > kNumSMs * 16) blocks = kNumSMs * 16;
+#define CALL(DT) fp8_act_quant_kernel<DT><<<(int)blocks, 256, 0, st>>>(x, groups, reinterpret_cast<uint8_t*>(y), scales)
+  LLMC_DISPATCH_DT("fp8_act_quant", dtype, CALL);
+#undef CALL
+  LLMC_CHECK_LAUNCH();
+  return LLMC_OK;
+}

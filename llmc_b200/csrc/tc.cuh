@@ -144,6 +144,24 @@ __device__ __forceinline__ void wgmma_m64n128k16_f16(float (&d)[64], uint64_t ad
       : "l"(adesc), "l"(bdesc), "r"(accumulate), "n"(kTransA), "n"(kTransB));
 }
 
+// D[64 x 128] (+)= A[64 x 32] * B[128 x 32]^T on e4m3 operands, issued by one warpgroup.  8-bit
+// operands are read K-major only (no transpose immediates); fragment layout as above.  The Hopper
+// tensor core keeps a reduced-precision fp32 accumulator for 8-bit inputs, so long K runs are
+// promoted into a full fp32 register sum by the caller (gemm_fp8.cu).
+__device__ __forceinline__ void wgmma_m64n128k32_e4m3(float (&d)[64], uint64_t adesc, uint64_t bdesc,
+                                                      uint32_t accumulate) {
+  asm volatile(
+      "{\n"
+      ".reg .pred p;\n"
+      "setp.ne.b32 p, %66, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n128k32.f32.e4m3.e4m3 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, "
+      "%64, %65, p, 1, 1;\n"
+      "}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+      : "l"(adesc), "l"(bdesc), "r"(accumulate));
+}
+
 template <bool kBf16, int kTransA, int kTransB>
 __device__ __forceinline__ void wgmma_m64n128k16(float (&d)[64], uint64_t adesc, uint64_t bdesc,
                                                  uint32_t accumulate) {
@@ -151,7 +169,7 @@ __device__ __forceinline__ void wgmma_m64n128k16(float (&d)[64], uint64_t adesc,
   else wgmma_m64n128k16_f16<kTransA, kTransB>(d, adesc, bdesc, accumulate);
 }
 
-// ---- forward GEMMs (gemm.cu, gemm_w4.cu) -------------------------------------------------------
+// ---- forward GEMMs (gemm.cu, gemm_w4.cu, gemm_fp8.cu) ------------------------------------------
 // L2-grouped tile order: the weights are swept in groups of `gn` n-tiles (<= ~32 MB, L2 resident,
 // see l2_group_width), all m-tiles per group, n fastest inside the group.  Activations are re-read
 // once per group from HBM, weights once; n-fastest over a 14336-row weight would instead stream

@@ -69,6 +69,20 @@ def linear_forward_w4(x, wq, scales, zeros, group, bias=None, bits=4, qparams_t=
     return y.reshape(*x.shape[:-1], N)
 
 
+# Counterpart of the reference's USE_FP8GEMM_TRITON_KERNEL (module_utils.py:14-20): when set,
+# LlmcFp8Linear keeps its weight in fp8 and runs block_wise_fp8_forward_func on the FP8 tensor cores.
+# Off by default: the forward then dequantises once and runs the bf16 GEMM, as it always has here.
+USE_FP8GEMM_KERNEL = False
+
+
+def block_wise_fp8_forward_func(x, w, w_scale, block_size, bias):
+    """module_utils.py:40-45: y = bf16(fp8_gemm(act_quant(x))) (+ bias after the rounding), as one
+    act_quant pass and one FP8 GEMM whose bf16 epilogue adds the bias (csrc/gemm_fp8.cu)."""
+    from .quant_float import act_quant, gemm_fp8_block
+    xq, scale = act_quant(x, block_size)
+    return gemm_fp8_block(xq, scale, w, w_scale, torch.bfloat16, bias)
+
+
 def _copy_bufs(dst, ori_module):
     for name, buf in ori_module.named_buffers():
         if name.startswith('buf_'):
@@ -98,9 +112,19 @@ class OriginFloatLinear(nn.Module):
         if getattr(self, 'buf_rotate', False):
             raise NotImplementedError('online rotation (QuaRot) is out of scope (SURVEY §2 #12)')
         self.buf_rotate = False
+        # :413-419: a block-FP8 weight (LlmcFp8Linear) keeps its scales and runs the FP8 forward
+        if self.weight.data.dtype == torch.float8_e4m3fn:
+            self.fp8_forward = True
+            self.weight_scale_inv = ori_module.weight_scale_inv
+            self.block_size = ori_module.block_size
+        else:
+            self.fp8_forward = False
 
     @torch.no_grad()
     def forward(self, x):
+        if self.fp8_forward:
+            return block_wise_fp8_forward_func(x, self.weight, self.weight_scale_inv, self.block_size,
+                                               self.bias)
         return linear_forward(x, self.weight, self.bias)
 
     @classmethod
@@ -115,13 +139,16 @@ class OriginFloatLinear(nn.Module):
     def __repr__(self):
         return (f'OriginFloatLinear(in_features={self.in_features},'
                 f'out_features={self.out_features}, bias={self.bias is not None},'
-                f'online_rotate={self.buf_rotate})')
+                f'online_rotate={self.buf_rotate},'
+                f'fp8_forward={self.fp8_forward})')
 
 
 class LlmcFp8Linear(nn.Module):
     """module_utils.py:130-191 — holder of a 128x128 block-FP8 checkpoint weight (`weight` fp8 +
-    `weight_scale_inv` fp32 [ceil(out/bs), ceil(in/bs)]).  Forward = the reference's non-Triton branch
-    (:171-178): dequantise ONCE to bf16 (llmc_fp8_block_dequant) and run the wgmma GEMM."""
+    `weight_scale_inv` fp32 [ceil(out/bs), ceil(in/bs)]).  Forward, by default, = the reference's
+    non-Hopper branch (:171-178): dequantise ONCE to bf16 (llmc_fp8_block_dequant) and run the wgmma
+    GEMM.  With USE_FP8GEMM_KERNEL set (the reference's Hopper branch, :157-166) the weight stays fp8
+    and every forward runs block_wise_fp8_forward_func."""
 
     def __init__(self, in_features, out_features, bias, block_size):
         super().__init__()
@@ -138,6 +165,9 @@ class LlmcFp8Linear(nn.Module):
     @torch.no_grad()
     def forward(self, x):
         if self.weight.data.dtype == torch.float8_e4m3fn:
+            if USE_FP8GEMM_KERNEL:
+                return block_wise_fp8_forward_func(x, self.weight.data, self.weight_scale_inv.data,
+                                                   self.block_size, self.bias)
             from .quant_float import weight_cast_to_bf16
             self.weight.data = weight_cast_to_bf16(self.weight.data, self.weight_scale_inv.data,
                                                    self.block_size)
@@ -152,7 +182,7 @@ class LlmcFp8Linear(nn.Module):
         return (f'LlmcFp8Linear(in_features={self.in_features}, out_features={self.out_features}, '
                 f'bias={self.bias is not None}, weight_shape={self.weight.shape}, '
                 f'weight_dtype={self.weight.dtype}, block_size={self.block_size}, '
-                'use_fp8gemm_triton_kernel=False)')
+                f'use_fp8gemm_triton_kernel={USE_FP8GEMM_KERNEL})')
 
 
 class FakeQuantLinear(nn.Module):

@@ -193,6 +193,78 @@ def weight_cast_to_fp8(weight, block_size):
     return fp8_weight, fp8_scale
 
 
+_FP8_BLOCK_ONLY_128 = ('block_size={}: the block-FP8 forward is built for 128 only — the reference '
+                       "hard-wires fp8_gemm's K step and scale index to 128 (kernel.py:143, 196)")
+
+
+def act_quant(x, block_size=128):
+    """kernel.py:31-53 -> (e4m3 tensor of x's shape, fp32 scales [*x.shape[:-1], K/128]).
+
+    Per contiguous group of 128 elements s = max|x| / 448 and y = e4m3(x / s), with the approximate
+    division the reference's kernel compiles to (csrc/fp8.cu).  An all-zero group gives s = 0 and NaN
+    codes, as in the reference.  x: bf16, fp16 or fp32, any leading dims."""
+    if block_size != 128:
+        raise NotImplementedError(_FP8_BLOCK_ONLY_128.format(block_size))
+    require_cuda(x)
+    K = x.shape[-1]
+    if K % block_size:
+        raise ValueError(f'Last dimension size must be divisible by block_size (block_size={block_size})')
+    xc = x if x.is_contiguous() else x.contiguous()
+    y = torch.empty(x.shape, dtype=torch.uint8, device=x.device)
+    s = torch.empty((*x.shape[:-1], K // block_size), dtype=torch.float32, device=x.device)
+    rows = x.numel() // K if K else 0
+    if rows:
+        with TIMER.span('fp8_act_quant', nbytes=(x.element_size() + 1 + 4.0 / block_size) * rows * K):
+            call('llmc_fp8_act_quant', ptr(xc), rows, K, dtype_enum(x.dtype), ptr(y), ptr(s),
+                 stream_ptr(x.device))
+    return y.view(torch.float8_e4m3fn), s
+
+
+def gemm_fp8_block(a, a_s, b, b_s, out_dtype, bias=None):
+    """llmc_gemm_fp8_block: a [..., K] e4m3 with a_s [..., K/128], b [N, K] e4m3 with
+    b_s [ceil(N/128), K/128] -> [..., N] of out_dtype (fp32, or bf16 with an optional bias added
+    after the rounding)."""
+    require_cuda(a, a_s, b, b_s, bias)
+    if a.dtype != torch.float8_e4m3fn or b.dtype != torch.float8_e4m3fn:
+        raise TypeError(f'fp8 GEMM operands must be float8_e4m3fn (got {a.dtype}, {b.dtype})')
+    K = a.shape[-1]
+    N = b.shape[0]
+    if b.dim() != 2 or b.shape[1] != K:
+        raise ValueError(f'weight shape {tuple(b.shape)} does not match K={K}')
+    if K % 128:
+        raise ValueError(f'K={K} must be a multiple of 128')
+    a2 = a.reshape(-1, K)
+    a2 = a2 if a2.is_contiguous() else a2.contiguous()
+    M = a2.shape[0]
+    sa = a_s.reshape(M, K // 128).to(torch.float32).contiguous()
+    sb = b_s.to(torch.float32).contiguous()
+    if tuple(sb.shape) != (-(-N // 128), K // 128):
+        raise ValueError(f'weight scales {tuple(sb.shape)} != [ceil(N/128), K/128] = '
+                         f'[{-(-N // 128)}, {K // 128}]')
+    bc = b if b.is_contiguous() else b.contiguous()
+    bt = None
+    if bias is not None:
+        bt = bias.contiguous()
+        if bt.dtype not in (torch.float32, torch.float16, torch.bfloat16) or bt.numel() != N:
+            raise ValueError(f'bias must be [N={N}] fp32 / fp16 / bf16 (got {bt.dtype} {tuple(bt.shape)})')
+    y = torch.empty((M, N), dtype=out_dtype, device=a.device)
+    with TIMER.span('gemm_fp8_block', flops=2.0 * M * N * K,
+                    nbytes=float(M * K + N * K) + 4.0 * (M + N / 128) * K / 128 + y.element_size() * M * N):
+        call('llmc_gemm_fp8_block', ptr(a2.view(torch.uint8)), ptr(sa), ptr(bc.view(torch.uint8)), ptr(sb),
+             ptr(bt), dtype_enum(bt.dtype) if bt is not None else 0, ptr(y), dtype_enum(out_dtype),
+             M, N, K, stream_ptr(a.device))
+    return y.reshape(*a.shape[:-1], N)
+
+
+def fp8_gemm(a, a_s, b, b_s):
+    """kernel.py:217-242: block-scaled e4m3 GEMM on the FP8 tensor cores -> [..., N] of
+    torch.get_default_dtype() (fp32 unless changed; bf16 is also built)."""
+    dt = torch.get_default_dtype()
+    if dt not in (torch.float32, torch.bfloat16):
+        raise NotImplementedError(f'fp8_gemm output dtype {dt}: only fp32 and bf16 are built')
+    return gemm_fp8_block(a, a_s, b, b_s, dt)
+
+
 def weight_cast_to_bf16(weight, scale, block_size):
     """quant.py:18-29: block-FP8 checkpoint weight -> bf16."""
     require_cuda(weight, scale)

@@ -17,8 +17,10 @@ try:
     PEAKS = json.load(open(os.path.join(os.path.dirname(__file__), '..', 'MEASURED_PEAKS.json')))
 except Exception:
     pass
-HBM = PEAKS.get('hbm_gbs', 6650.0)
-TF = PEAKS.get('bf16_tflops', 1590.0)
+# H100 SXM data sheet (dense, 700 W card): 3.35 TB/s HBM3, 989 TFLOP/s bf16, 1,979 TFLOP/s fp8
+HBM = PEAKS.get('hbm_gbs', 3350.0)
+TF = PEAKS.get('bf16_tflops', 989.0)
+TF_FP8 = PEAKS.get('fp8_tflops', 1979.0)
 
 flush = torch.empty(256 * 1024 * 1024, dtype=torch.uint8, device='cuda')
 
@@ -41,7 +43,22 @@ def timeit(fn, iters=5, warm=2, do_flush=True):
     return ts[len(ts) // 2]
 
 
-res = {}
+def _device():
+    """The card every number of this run was measured on, and its power limit."""
+    import subprocess
+    d = {'name': torch.cuda.get_device_name(0)}
+    try:
+        out = subprocess.run(['nvidia-smi', '--query-gpu=power.limit,clocks.max.sm',
+                              '--format=csv,noheader', '-i', '0'], capture_output=True, text=True,
+                             timeout=30).stdout.strip()
+        d['power_limit'], d['max_sm_clock'] = [v.strip() for v in out.split(',')]
+    except Exception as e:                                   # noqa: BLE001
+        d['power_limit'] = f'unknown ({type(e).__name__})'
+    return d
+
+
+res = {'_device': _device()}
+print('device', res['_device'], flush=True)
 
 
 def rec(name, ms, **kw):
@@ -185,6 +202,51 @@ if 'awq' in only:
         dt = time.perf_counter() - t0
         rec(f'awq_block_llama2_7b_rep{rep}', dt * 1e3, layers_per_s=7 / dt)
         del algo, model, inp
+
+if 'fp8' in only:
+    # The block-FP8 linear forward (act_quant + gemm_fp8_block, csrc/fp8.cu + csrc/gemm_fp8.cu) next
+    # to the dequant-once path (llmc_fp8_block_dequant + llmc_gemm_bf16) and, where this
+    # torch / cuBLAS build takes it, torch._scaled_mm with 1 x 128 / 128 x 128 block scales.
+    from llmc_b200.quant_float import act_quant, gemm_fp8_block, weight_cast_to_bf16, weight_cast_to_fp8
+    shapes = [(1536, 7168), (18432, 7168), (7168, 18432), (2048, 7168), (7168, 2048),   # DeepSeek-V3
+              (14336, 4096), (4096, 14336)]                                          # Llama-3-8B
+    scaled_mm = None
+    for M in (16384, 4096):
+        for (N, K) in shapes:
+            tag = f'{M}x{N}x{K}'
+            x = torch.randn(M, K, device='cuda').bfloat16()
+            w = (torch.randn(N, K, device='cuda') * 0.02).bfloat16()
+            wq, ws = weight_cast_to_fp8(w, 128)
+            xq, xs = act_quant(x)
+            fl = 2.0 * M * N * K
+            ms = timeit(lambda: act_quant(x))
+            by = M * K * (2 + 1 + 4 / 128)
+            rec(f'fp8_act_quant_{M}x{K}', ms, gbs=by / ms / 1e6, frac_hbm=by / ms / 1e6 / HBM)
+            ms_g = timeit(lambda: gemm_fp8_block(xq, xs, wq, ws, torch.bfloat16), do_flush=False)
+            rec(f'gemm_fp8_block_{tag}', ms_g, tflops=fl / ms_g / 1e9, frac_fp8=fl / ms_g / 1e9 / TF_FP8)
+            ms_f = timeit(lambda: gemm_fp8_block(*act_quant(x), wq, ws, torch.bfloat16), do_flush=False)
+            rec(f'fp8_forward_{tag}', ms_f, tflops=fl / ms_f / 1e9)
+            wd = weight_cast_to_bf16(wq, ws, 128)
+            ms_b = timeit(lambda: linear_forward(x, wd), do_flush=False)
+            ms_d = timeit(lambda: weight_cast_to_bf16(wq, ws, 128))
+            rec(f'dequant_once_bf16_gemm_{tag}', ms_b, tflops=fl / ms_b / 1e9, frac_bf16=fl / ms_b / 1e9 / TF,
+                dequant_ms=round(ms_d, 4), fp8_forward_speedup=ms_b / ms_f)
+            if scaled_mm is None or scaled_mm is True:
+                try:
+                    # 1 x 128 activation scales and 128 x 128 weight scales, both outer-dim-major
+                    sa = xs.t().contiguous().t()
+                    sb = ws.t().contiguous().t()
+                    f = lambda: torch._scaled_mm(xq, wq.t(), scale_a=sa, scale_b=sb.t(),  # noqa: E731
+                                                 out_dtype=torch.bfloat16)
+                    f()
+                    ms_s = timeit(f, do_flush=False)
+                    rec(f'torch_scaled_mm_block_{tag}', ms_s, tflops=fl / ms_s / 1e9)
+                    scaled_mm = True
+                except Exception as e:                       # noqa: BLE001
+                    scaled_mm = False
+                    rec('torch_scaled_mm_block', 0.0, status='unsupported',
+                        error=f'{type(e).__name__}: {str(e).splitlines()[0][:200]}')
+            del x, w, wq, ws, xq, xs, wd
 
 os.makedirs('gpurun_out', exist_ok=True)
 json.dump(res, open('gpurun_out/microbench.json', 'w'), indent=1)
