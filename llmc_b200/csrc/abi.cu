@@ -1,7 +1,10 @@
-// abi.cu — version / error reporting of the C ABI (include/llmc_b200.h).
+// abi.cu — version / error reporting of the C ABI (include/llmc_b200.h) and the launch
+// bookkeeping every entry point shares.
 #include <atomic>
+#include <set>
 #include <stdarg.h>
 #include <string.h>
+#include <utility>
 
 #include "common.cuh"
 
@@ -18,6 +21,18 @@ void set_last_error(const char* fmt, ...) {
 
 static std::atomic<long long> g_launches{0};
 void count_launch(int n) { g_launches.fetch_add(n, std::memory_order_relaxed); }
+
+int opt_in_smem(const void* kernel, int bytes) {
+  static std::mutex mutex;
+  static std::set<std::pair<int, const void*>> done;
+  int dev = 0;
+  LLMC_CHECK_CUDA(cudaGetDevice(&dev));
+  std::lock_guard<std::mutex> guard(mutex);
+  if (done.count({dev, kernel})) return LLMC_OK;
+  LLMC_CHECK_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes));
+  done.insert({dev, kernel});
+  return LLMC_OK;
+}
 
 }  // namespace llmc
 

@@ -341,11 +341,8 @@ extern "C" int llmc_awq_clip(const void* w, int64_t R, int64_t C, const void* x,
   int_range(bit, sym, a.qmin, a.qmax);
   a.err = workspace;
   const int smem = (kClipMaxTok * (kClipG + 1) + 8 * kClipG) * 4;
-  LLMC_ONCE_PER_DEVICE({
-    LLMC_CHECK_CUDA(cudaFuncSetAttribute(awq_clip_err_kernel<LLMC_F32>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-    LLMC_CHECK_CUDA(cudaFuncSetAttribute(awq_clip_err_kernel<LLMC_F16>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-    LLMC_CHECK_CUDA(cudaFuncSetAttribute(awq_clip_err_kernel<LLMC_BF16>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-  });
+  for (auto kern : {awq_clip_err_kernel<LLMC_F32>, awq_clip_err_kernel<LLMC_F16>, awq_clip_err_kernel<LLMC_BF16>})
+    if (int rc = opt_in_smem(kern, smem)) return rc;
   // row slices so that ng * slices ~ a few waves of kNumSMs CTAs
   int slices = (4 * kNumSMs + ng - 1) / ng;
   if (slices > (R + 7) / 8) slices = static_cast<int>((R + 7) / 8);

@@ -282,9 +282,7 @@ extern "C" int llmc_chol_inv_upper(float* A, int64_t C, void* workspace, int64_t
   const SplitMatrix L{Lhi, Llo, n};    // tf32 split of L's sub-diagonal panels
   const SplitMatrix Ys{Yhi, Ylo, n};   // tf32 split of Y = L^-1
   const int diag_smem = 2 * NB * LDS * 4;
-  LLMC_ONCE_PER_DEVICE({
-    LLMC_CHECK_CUDA(cudaFuncSetAttribute(diag_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, diag_smem));
-  });
+  if (int rc = opt_in_smem(diag_kernel, diag_smem)) return rc;
   // Side streams + events (common.cuh); the call stays asynchronous with respect to the host and
   // ordered on `stream` through the final join.
   SideStreams* side = nullptr;

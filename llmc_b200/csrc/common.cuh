@@ -46,22 +46,33 @@ void count_launch(int n);
     LLMC_CHECK_CUDA(cudaGetLastError());    \
   } while (0)
 
-// Function attributes (opt-in dynamic shared memory) are per DEVICE: run `body` the first time
-// this call site is reached on each device (a process normally drives one GPU, but nothing here
-// should break when it drives several).  `body` may `return` an error code.
-#define LLMC_ONCE_PER_DEVICE(body)                                   \
-  do {                                                               \
-    static std::mutex once_mutex_;                                   \
-    static uint64_t once_mask_ = 0;                                  \
-    int once_dev_ = 0;                                               \
-    if (cudaGetDevice(&once_dev_) != cudaSuccess) once_dev_ = 0;     \
-    std::lock_guard<std::mutex> once_guard_(once_mutex_);            \
-    const uint64_t once_bit_ = 1ull << (once_dev_ & 63);             \
-    if (!(once_mask_ & once_bit_)) {                                 \
-      body;                                                          \
-      once_mask_ |= once_bit_;                                       \
-    }                                                                \
-  } while (0)
+// Opts `kernel` in to `bytes` of dynamic shared memory beyond the default 48 KB.  Function
+// attributes are per DEVICE, so this sets the attribute the first time each (device, kernel) is
+// seen (a process normally drives one GPU, but nothing here should break when it drives several);
+// `bytes` is the most any launch of the kernel uses.
+int opt_in_smem(const void* kernel, int bytes);
+template <class... P>
+int opt_in_smem(void (*kernel)(P...), int bytes) {
+  return opt_in_smem(reinterpret_cast<const void*>(kernel), bytes);
+}
+
+// A persistent kernel's CTAs take its `count` units of work in turn (u = blockIdx.x; u +=
+// gridDim.x).  launch_persistent runs it on one CTA per SM, or on fewer when there are fewer units;
+// cta_per_unit runs one CTA per unit instead (see tf32x3_update).
+struct Units {
+  int count;
+  bool cta_per_unit;
+  Units(int n, bool one_cta_each = false) : count(n), cta_per_unit(one_cta_each) {}
+};
+template <class... P, class... A>
+int launch_persistent(void (*kernel)(P...), Units units, int threads, int smem, cudaStream_t st,
+                      A... args) {
+  if (int rc = opt_in_smem(kernel, smem)) return rc;
+  const int grid = (units.cta_per_unit || units.count < kNumSMs) ? units.count : kNumSMs;
+  kernel<<<grid, threads, smem, st>>>(args...);
+  LLMC_CHECK_LAUNCH();
+  return LLMC_OK;
+}
 
 // ---- side streams ------------------------------------------------------------------------
 // The look-ahead schedules of the blocked Cholesky (chol.cu) and of the GPTQ / SpQR sweep

@@ -6,8 +6,8 @@
 //   warpgroups 1-2  consumers: each owns 64 rows of the 128 x 256 tile and issues
 //                   wgmma.mma_async m64n128k16 (two per 16-deep K step, one per 128-column half)
 //                   with fp32 accumulators in registers, then stores its rows from registers.
-// Tile 128(M) x 256(N) x 64(K), 4-stage ring (48 KB / stage).  A consumer keeps one wgmma group
-// in flight and frees a ring stage as soon as the group that read it has retired.
+// Tile 128(M) x 256(N) x 64(K), 4-stage tc::Ring (48 KB / stage).  A consumer keeps one wgmma
+// group in flight and frees a ring stage as soon as the group that read it has retired.
 //
 //  * GEMM  (llmc_gemm_bf16):  Y[M,N] = X[M,K] . W[N,K]^T (+bias) — both operands K-major.
 //      Replaces F.linear in FakeQuantLinear / EffcientFakeQuantLinear.forward
@@ -30,7 +30,7 @@ constexpr int kABytes = BM * BK * 2;                 // 16 KB
 constexpr int kBBytes = BN * BK * 2;                 // 32 KB
 constexpr int kStageBytes = kABytes + kBBytes;       // 48 KB
 constexpr int kBoxBytes = 64 * 64 * 2;               // SYRK box: 64 tokens x 64 channels
-constexpr int kSmemBytes = kStages * kStageBytes + 1024 /*align slack*/ + 256 /*barriers*/;
+constexpr int kSmemBytes = ring_smem_bytes(kStages * kStageBytes);
 constexpr int kThreads = 384;
 struct GemmParams {
   int64_t M, N, K;          // GEMM: Y[M,N]; SYRK: M = N = C, K = T
@@ -94,10 +94,8 @@ __global__ void __launch_bounds__(kThreads, 1)
 wgmma_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                   const GemmParams p) {
   extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) &
-                                             ~static_cast<uintptr_t>(1023));
-  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + kStages * kStageBytes);
-  uint64_t* empty_bar = full_bar + kStages;
+  uint8_t* smem = ring_base(smem_raw);
+  const Ring<kStages> ring(smem + kStages * kStageBytes);
 
   const int wg = threadIdx.x >> 7;
   const int tid = threadIdx.x & 127;
@@ -105,10 +103,7 @@ wgmma_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
   if (threadIdx.x == 0) {
     prefetch_tmap(&tmA);
     prefetch_tmap(&tmB);
-    for (int s = 0; s < kStages; ++s) {
-      mbar_init(&full_bar[s], 1);
-      mbar_init(&empty_bar[s], 2);    // one arrive per consumer warpgroup
-    }
+    ring.init(1, 2);                  // empty: one arrive per consumer warpgroup
     fence_barrier_init();
   }
   __syncthreads();
@@ -116,30 +111,28 @@ wgmma_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
   if (wg == 0) {
     // ===================== TMA producer =====================
     if (tid == 0) {
-      int stage = 0;
-      uint32_t phase = 0;
+      PipeState<kStages> ps;
       for (int u = blockIdx.x; u < p.num_units; u += gridDim.x) {
         const Unit t = decode_unit<kSyrk>(p, u);
         for (int kb = t.kb0; kb < t.kb1; ++kb) {
-          mbar_wait(&empty_bar[stage], phase ^ 1);
-          uint8_t* a_dst = smem + stage * kStageBytes;
+          ring.wait_empty(ps);
+          uint8_t* a_dst = smem + ps.stage * kStageBytes;
           uint8_t* b_dst = a_dst + kABytes;
-          mbar_expect_tx(&full_bar[stage], kStageBytes);
+          uint64_t* bar = &ring.full[ps.stage];
+          ring.expect_tx(ps, kStageBytes);
           if constexpr (!kSyrk) {
-            tma_load_2d(a_dst, &tmA, &full_bar[stage], kb * BK, t.m_blk * BM);
-            tma_load_2d(b_dst, &tmB, &full_bar[stage], kb * BK, t.n_blk * BN);
+            tma_load_2d(a_dst, &tmA, bar, kb * BK, t.m_blk * BM);
+            tma_load_2d(b_dst, &tmB, bar, kb * BK, t.n_blk * BN);
           } else {
             // X[T, C]: coordinate 0 = channel, coordinate 1 = token; box = 64 ch x 64 tok
 #pragma unroll
             for (int i = 0; i < BM / 64; ++i)
-              tma_load_2d(a_dst + i * kBoxBytes, &tmA, &full_bar[stage], t.m_blk * BM + i * 64,
-                          kb * BK);
+              tma_load_2d(a_dst + i * kBoxBytes, &tmA, bar, t.m_blk * BM + i * 64, kb * BK);
 #pragma unroll
             for (int i = 0; i < BN / 64; ++i)
-              tma_load_2d(b_dst + i * kBoxBytes, &tmA, &full_bar[stage], t.n_blk * BN + i * 64,
-                          kb * BK);
+              tma_load_2d(b_dst + i * kBoxBytes, &tmA, bar, t.n_blk * BN + i * 64, kb * BK);
           }
-          if (++stage == kStages) { stage = 0; phase ^= 1; }
+          ps.advance();
         }
       }
     }
@@ -148,9 +141,7 @@ wgmma_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
 
   // ===================== consumers (warpgroups 1, 2): rows 64 * c .. 64 * c + 63 =====================
   const int c = wg - 1;
-  const int lane = tid & 31;
-  int stage = 0;
-  uint32_t phase = 0;
+  PipeState<kStages> ps;
   for (int u = blockIdx.x; u < p.num_units; u += gridDim.x) {
     const Unit t = decode_unit<kSyrk>(p, u);
     float acc0[64], acc1[64];                    // columns [0, 128) and [128, 256) of the tile
@@ -158,9 +149,9 @@ wgmma_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
     for (int i = 0; i < 64; ++i) { acc0[i] = 0.f; acc1[i] = 0.f; }
     int prev = -1;
     for (int kb = t.kb0; kb < t.kb1; ++kb) {
-      mbar_wait(&full_bar[stage], phase);
+      ring.wait_full(ps);
       wgmma_fence();
-      const uint32_t a_addr = smem_u32(smem + stage * kStageBytes);
+      const uint32_t a_addr = smem_u32(smem + ps.stage * kStageBytes);
       const uint32_t b_addr = a_addr + kABytes;
 #pragma unroll
       for (int k = 0; k < BK / 16; ++k) {
@@ -180,44 +171,28 @@ wgmma_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
       }
       wgmma_commit();
       wgmma_wait<1>();                           // the group that read stage `prev` has retired
-      if (prev >= 0 && tid == 0) mbar_arrive(&empty_bar[prev]);
-      prev = stage;
-      if (++stage == kStages) { stage = 0; phase ^= 1; }
+      if (prev >= 0 && tid == 0) ring.release(prev);
+      prev = ps.stage;
+      ps.advance();
     }
     wgmma_wait<0>();
     fence_acc(acc0);
     fence_acc(acc1);
-    if (prev >= 0 && tid == 0) mbar_arrive(&empty_bar[prev]);
+    if (prev >= 0 && tid == 0) ring.release(prev);
 
     // ---- epilogue straight from the accumulator registers ----
+    const int64_t row0 = static_cast<int64_t>(t.m_blk) * BM + c * 64;
+    const int64_t col0 = static_cast<int64_t>(t.n_blk) * BN;
     if constexpr (!kSyrk) {
       constexpr int DT = kBf16 ? LLMC_BF16 : LLMC_F16;
-      const int64_t row0 = static_cast<int64_t>(t.m_blk) * BM + c * 64;
-      const int64_t col0 = static_cast<int64_t>(t.n_blk) * BN;
       store_linear_m64n128<DT>(acc0, row0, col0, p.M, p.N, p.ld_out, p.bias, p.out);
       store_linear_m64n128<DT>(acc1, row0, col0 + 128, p.M, p.N, p.ld_out, p.bias, p.out);
     } else {
       // fp32 partial slab `t.split` of the split-K sum
-      const int64_t row0 = static_cast<int64_t>(t.m_blk) * BM + c * 64 + (tid >> 5) * 16 + (lane >> 2);
-      auto store_half = [&](const float (&acc)[64], int h) {
-#pragma unroll
-        for (int j = 0; j < 16; ++j) {
-          const int64_t col = static_cast<int64_t>(t.n_blk) * BN + h * 128 + 8 * j + 2 * (lane & 3);
-          if (col >= p.N) continue;
-#pragma unroll
-          for (int i = 0; i < 2; ++i) {
-            const int64_t row = row0 + 8 * i;
-            if (row >= p.M) continue;
-            const float v0 = acc[4 * j + 2 * i], v1 = acc[4 * j + 2 * i + 1];
-            float* o = reinterpret_cast<float*>(p.out) +
-                       (static_cast<int64_t>(t.split) * p.M + row) * p.ld_out + col;
-            if (col + 1 < p.N) *reinterpret_cast<float2*>(o) = make_float2(v0, v1);
-            else o[0] = v0;
-          }
-        }
-      };
-      store_half(acc0, 0);
-      store_half(acc1, 1);
+      float* slab = static_cast<float*>(p.out) + static_cast<int64_t>(t.split) * p.M * p.ld_out;
+      __builtin_assume((p.ld_out & 1) == 0);   // ld_out = C, a multiple of 8: all pairs are float2
+      store_f32_m64n128(acc0, row0, col0, p.M, p.N, p.ld_out, slab);
+      store_f32_m64n128(acc1, row0, col0 + 128, p.M, p.N, p.ld_out, slab);
     }
   }
 }
@@ -302,19 +277,6 @@ int encode_tmap_2d(CUtensorMap* out, const void* base, CUtensorMapDataType dtype
   return LLMC_OK;
 }
 
-template <bool kSyrk, bool kBf16>
-static int launch_wgmma(const CUtensorMap& tmA, const CUtensorMap& tmB, const GemmParams& p,
-                       cudaStream_t st) {
-  auto kern = wgmma_gemm_kernel<kSyrk, kBf16>;
-  LLMC_ONCE_PER_DEVICE({
-    LLMC_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemBytes));
-  });
-  int grid = p.num_units < kNumSMs ? p.num_units : kNumSMs;
-  kern<<<grid, kThreads, kSmemBytes, st>>>(tmA, tmB, p);
-  LLMC_CHECK_LAUNCH();
-  return LLMC_OK;
-}
-
 struct SyrkPlan {
   int n_tiles_n, num_tiles, splits, kb_total, kb_per_split;
 };
@@ -380,8 +342,9 @@ extern "C" int llmc_gemm_bf16(const void* x, const void* w, const void* bias, vo
   p.kb_per_split = p.kb_total;
   p.gn = l2_group_width(static_cast<int64_t>(BN) * K * 2, p.n_tiles_n);   // K > 0: one n-tile's bytes
   cudaStream_t st = static_cast<cudaStream_t>(stream);
-  return dtype == LLMC_BF16 ? launch_wgmma<false, true>(tmA, tmB, p, st)
-                            : launch_wgmma<false, false>(tmA, tmB, p, st);
+  return launch_persistent(dtype == LLMC_BF16 ? wgmma_gemm_kernel<false, true>
+                                              : wgmma_gemm_kernel<false, false>,
+                           p.num_units, kThreads, kSmemBytes, st, tmA, tmB, p);
 }
 
 extern "C" int64_t llmc_syrk_workspace_bytes(int64_t T, int64_t C) {
@@ -418,8 +381,9 @@ extern "C" int llmc_syrk_accum(const void* x, int64_t T, int64_t C, int dtype, f
   p.kb_per_split = s.kb_per_split;
   p.gn = 12;                      // 12 m-blocks (1536 rows) x ~11 n-tiles ~ one wave of 132 tiles
   cudaStream_t st = static_cast<cudaStream_t>(stream);
-  int rc = dtype == LLMC_BF16 ? launch_wgmma<true, true>(tmX, tmX, p, st)
-                              : launch_wgmma<true, false>(tmX, tmX, p, st);
+  int rc = launch_persistent(dtype == LLMC_BF16 ? wgmma_gemm_kernel<true, true>
+                                                : wgmma_gemm_kernel<true, false>,
+                             p.num_units, kThreads, kSmemBytes, st, tmX, tmX, p);
   if (rc) return rc;
   // gptq.py:283-290: H *= n/(n+b); H += (sqrt(2/(n+b)) X)^T (sqrt(2/(n+b)) X)
   const float fa = static_cast<float>(n / (n + b));

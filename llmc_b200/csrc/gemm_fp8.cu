@@ -42,7 +42,7 @@ constexpr int kBM = 128, kBN = 128, kBK = 128;
 constexpr int kStages = 6;
 constexpr int kTileBytes = kBM * kBK;                  // 16 KB of e4m3 (kBN == kBM)
 constexpr int kStageBytes = 2 * kTileBytes;            // 32 KB
-constexpr int kSmemBytes = kStages * kStageBytes + 1024 /*align slack*/ + 256 /*barriers*/;
+constexpr int kSmemBytes = ring_smem_bytes(kStages * kStageBytes);
 constexpr int kThreads = 384;
 
 struct Fp8GemmParams {
@@ -62,6 +62,11 @@ __global__ void __launch_bounds__(kThreads, 1)
 fp8_block_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                       const Fp8GemmParams p) {
   extern __shared__ uint8_t smem_raw[];
+  // The ring is reached only through TMA and wgmma descriptors, so the generic address costs
+  // nothing here.  tc::ring_base and tc::Ring's init, waits and release are not used: with either,
+  // ptxas schedules the descriptor setup between the fence and the first wgmma of each K block,
+  // which the wgmma_wait<0> per K block serialises (5-13 % slower at M = 4096 / 16384 with
+  // DeepSeek-V3 and Llama-3-8B widths, H100 SXM at 700 W).
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) &
                                              ~static_cast<uintptr_t>(1023));
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + kStages * kStageBytes);
@@ -84,18 +89,17 @@ fp8_block_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_cons
   if (wg == 0) {
     // ===================== TMA producer =====================
     if (tid == 0) {
-      int stage = 0;
-      uint32_t phase = 0;
+      PipeState<kStages> ps;
       for (int u = blockIdx.x; u < p.num_tiles; u += gridDim.x) {
         int m_blk, n_blk;
         grouped_tile(u, p.m_tiles, p.n_tiles, p.gn, m_blk, n_blk);
         for (int kb = 0; kb < p.kb_total; ++kb) {
-          mbar_wait(&empty_bar[stage], phase ^ 1);
-          uint8_t* a_dst = smem + stage * kStageBytes;
-          mbar_expect_tx(&full_bar[stage], kStageBytes);
-          tma_load_2d(a_dst, &tmA, &full_bar[stage], kb * kBK, m_blk * kBM);
-          tma_load_2d(a_dst + kTileBytes, &tmB, &full_bar[stage], kb * kBK, n_blk * kBN);
-          if (++stage == kStages) { stage = 0; phase ^= 1; }
+          mbar_wait(&empty_bar[ps.stage], ps.phase ^ 1);
+          uint8_t* a_dst = smem + ps.stage * kStageBytes;
+          mbar_expect_tx(&full_bar[ps.stage], kStageBytes);
+          tma_load_2d(a_dst, &tmA, &full_bar[ps.stage], kb * kBK, m_blk * kBM);
+          tma_load_2d(a_dst + kTileBytes, &tmB, &full_bar[ps.stage], kb * kBK, n_blk * kBN);
+          ps.advance();
         }
       }
     }
@@ -105,8 +109,7 @@ fp8_block_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_cons
   // ===================== consumers (warpgroups 1, 2): tile rows 64 c .. 64 c + 63 =====================
   const int c = wg - 1;
   const int lane = tid & 31;
-  int stage = 0;
-  uint32_t phase = 0;
+  PipeState<kStages> ps;
   float d[64];                                   // the dot of one K block
 #pragma unroll
   for (int i = 0; i < 64; ++i) d[i] = 0.f;
@@ -125,9 +128,9 @@ fp8_block_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_cons
     for (int i = 0; i < 64; ++i) acc[i] = 0.f;
     for (int kb = 0; kb < p.kb_total; ++kb) {
       const float sa0 = __ldg(as_lo + kb), sa1 = __ldg(as_hi + kb), sb = __ldg(bs + kb);
-      mbar_wait(&full_bar[stage], phase);
+      mbar_wait(&full_bar[ps.stage], ps.phase);
       wgmma_fence();
-      const uint32_t a_addr = smem_u32(smem + stage * kStageBytes);
+      const uint32_t a_addr = smem_u32(smem + ps.stage * kStageBytes);
       const uint32_t b_addr = a_addr + kTileBytes;
 #pragma unroll
       for (int k = 0; k < kBK / 32; ++k) {
@@ -138,8 +141,8 @@ fp8_block_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_cons
       wgmma_commit();
       wgmma_wait<0>();
       fence_acc(d);
-      if (tid == 0) mbar_arrive(&empty_bar[stage]);
-      if (++stage == kStages) { stage = 0; phase ^= 1; }
+      if (tid == 0) mbar_arrive(&empty_bar[ps.stage]);
+      ps.advance();
       // promotion: d[4 j + 2 i + e] belongs to row r_lo + 8 i
 #pragma unroll
       for (int j = 0; j < 16; ++j) {
@@ -175,48 +178,14 @@ fp8_block_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_cons
             const float v0 = fadd_rn(DType<LLMC_BF16>::rT(acc[4 * j + 2 * i]), b0);
             const float v1 = fadd_rn(DType<LLMC_BF16>::rT(acc[4 * j + 2 * i + 1]), b1);
             const uint32_t pk = pack_pair<LLMC_BF16>(v0, v1);
-            uint16_t* o = static_cast<uint16_t*>(p.out) + row * p.N + col;
-            if (pair && (p.N & 1) == 0) *reinterpret_cast<uint32_t*>(o) = pk;
-            else {
-              o[0] = static_cast<uint16_t>(pk & 0xffffu);
-              if (pair) o[1] = static_cast<uint16_t>(pk >> 16);
-            }
+            store_pair16(static_cast<uint16_t*>(p.out) + row * p.N + col, pk, pair, p.N);
           }
         }
       }
     } else {
-#pragma unroll
-      for (int j = 0; j < 16; ++j) {
-        const int64_t col = col0 + 8 * j + 2 * (lane & 3);
-        if (col >= p.N) continue;
-#pragma unroll
-        for (int i = 0; i < 2; ++i) {
-          const int64_t row = r_lo + 8 * i;
-          if (row >= p.M) continue;
-          float* o = static_cast<float*>(p.out) + row * p.N + col;
-          const float v0 = acc[4 * j + 2 * i], v1 = acc[4 * j + 2 * i + 1];
-          if (col + 1 < p.N && (p.N & 1) == 0) *reinterpret_cast<float2*>(o) = make_float2(v0, v1);
-          else {
-            o[0] = v0;
-            if (col + 1 < p.N) o[1] = v1;
-          }
-        }
-      }
+      store_f32_m64n128(acc, row0, col0, p.M, p.N, p.N, static_cast<float*>(p.out));
     }
   }
-}
-
-template <bool kBf16Out>
-int launch_fp8_gemm(const CUtensorMap& tmA, const CUtensorMap& tmB, const Fp8GemmParams& p,
-                    cudaStream_t st) {
-  auto kern = fp8_block_gemm_kernel<kBf16Out>;
-  LLMC_ONCE_PER_DEVICE({
-    LLMC_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemBytes));
-  });
-  const int grid = p.num_tiles < kNumSMs ? p.num_tiles : kNumSMs;
-  kern<<<grid, kThreads, kSmemBytes, st>>>(tmA, tmB, p);
-  LLMC_CHECK_LAUNCH();
-  return LLMC_OK;
 }
 
 }  // namespace
@@ -262,6 +231,7 @@ extern "C" int llmc_gemm_fp8_block(const void* a, const float* a_s, const void* 
   p.gn = l2_group_width(static_cast<int64_t>(kBN) * K, p.n_tiles);   // one n-tile's weight bytes
   p.bias_dt = bias_dtype;
   cudaStream_t st = static_cast<cudaStream_t>(stream);
-  return out_dtype == LLMC_BF16 ? launch_fp8_gemm<true>(tmA, tmB, p, st)
-                                : launch_fp8_gemm<false>(tmA, tmB, p, st);
+  return launch_persistent(out_dtype == LLMC_BF16 ? fp8_block_gemm_kernel<true>
+                                                  : fp8_block_gemm_kernel<false>,
+                           p.num_tiles, kThreads, kSmemBytes, st, tmA, tmB, p);
 }

@@ -9,10 +9,11 @@
 // m64n128k16 wgmma per output element, same K order), while the weight stream from HBM is 4.25
 // bits instead of 16 per element.
 //
-// Tile 128(M) x 128(N) x 64(K).  Pipeline per K step, TWO rings so that the TMA latency is covered
-// by a deep, cheap ring and the dequantised tile by a short one:
+// Tile 128(M) x 128(N) x 64(K).  Pipeline per K step, TWO tc::Rings so that the TMA latency is
+// covered by a deep, cheap ring and the dequantised tile by a short one:
 //   ring L (6 x 20 KB): X tile [128 x 64] bf16 (swizzle 128B) + packed W tile [128 x 8] int32
-//   ring B (3 x 16 KB): the dequantised, 128B-swizzled wgmma B tile
+//   ring B (3 x 16 KB): the dequantised, 128B-swizzled wgmma B tile; its full barrier counts the
+//                       four warps of the dequant group that wrote it
 //   warps 0-7          dequant, NG = 2 groups of four warps taking alternate K steps (one weight
 //                      row per thread): nibble -> fp32 via the 2^23 magic constant, (q - z) * s in
 //                      fp32, round to bf16/fp16, 16-byte stores into ring B, fence.proxy.async;
@@ -44,7 +45,7 @@ template <int kBits> struct Cfg {
   static constexpr int kLBytes = kABytes + kPBytes;
   static constexpr int kBStages = 3;
   static constexpr int kLStages = 6;
-  static constexpr int kSmemBytes = kLStages * kLBytes + kBStages * kBBytes + 1024 + 256;
+  static constexpr int kSmemBytes = ring_smem_bytes(kLStages * kLBytes + kBStages * kBBytes);
   static constexpr int kWordsPerRow = BK * kBits / 32;      // int32 per row of the packed tile
   static constexpr int kDequantWarps = 4 * NG;
   static constexpr int kConsumerWarp0 = kDequantWarps;      // first warp of the consumer warpgroups
@@ -98,27 +99,17 @@ w4a16_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
   constexpr int kLBytes = C::kLBytes;
   constexpr int kBStages = C::kBStages;
   extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) &
-                                             ~static_cast<uintptr_t>(1023));
-  uint8_t* ringL = smem;
-  uint8_t* ringB = smem + kLStages * kLBytes;
-  uint64_t* fullL = reinterpret_cast<uint64_t*>(ringB + kBStages * kBBytes);
-  uint64_t* emptyL = fullL + kLStages;
-  uint64_t* readyB = emptyL + kLStages;          // dequantised B tile written
-  uint64_t* emptyB = readyB + kBStages;
+  uint8_t* ringL = ring_base(smem_raw);
+  uint8_t* ringB = ringL + kLStages * kLBytes;
+  const Ring<kLStages> ring_l(ringB + kBStages * kBBytes);
+  const Ring<kBStages> ring_b(ring_l.end());      // full: the dequantised B tile is written
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
 
   if (threadIdx.x == 0) {
     prefetch_tmap(&tmA);
     prefetch_tmap(&tmP);
-    for (int s = 0; s < kLStages; ++s) {
-      mbar_init(&fullL[s], 1);
-      mbar_init(&emptyL[s], 2 + 4);                   // both consumer warpgroups + the step's dequant group
-    }
-    for (int s = 0; s < kBStages; ++s) {
-      mbar_init(&readyB[s], 4);
-      mbar_init(&emptyB[s], 2);
-    }
+    ring_l.init(1, 2 + 4);            // empty: both consumer warpgroups + the step's dequant group
+    ring_b.init(4, 2);
     fence_barrier_init();
   }
   __syncthreads();
@@ -126,19 +117,18 @@ w4a16_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
   if (warp == C::kTmaWarp) {
     // ===================== TMA producer =====================
     if (lane == 0) {
-      int sl = 0;
-      uint32_t phl = 0;
+      PipeState<kLStages> sl;
       for (int u = blockIdx.x; u < p.num_units; u += gridDim.x) {
         int m_blk, n_blk;
         grouped_tile(u, p.num_units / p.n_tiles_n, p.n_tiles_n, p.gn, m_blk, n_blk);
         for (int kb = 0; kb < p.kb_total; ++kb) {
-          mbar_wait(&emptyL[sl], phl ^ 1);
-          uint8_t* a_dst = ringL + sl * kLBytes;
+          ring_l.wait_empty(sl);
+          uint8_t* a_dst = ringL + sl.stage * kLBytes;
           uint8_t* p_dst = a_dst + kABytes;
-          mbar_expect_tx(&fullL[sl], kLBytes);
-          tma_load_2d(a_dst, &tmA, &fullL[sl], kb * BK, m_blk * BM);
-          tma_load_2d(p_dst, &tmP, &fullL[sl], kb * C::kWordsPerRow, n_blk * BN);
-          if (++sl == kLStages) { sl = 0; phl ^= 1; }
+          ring_l.expect_tx(sl, kLBytes);
+          tma_load_2d(a_dst, &tmA, &ring_l.full[sl.stage], kb * BK, m_blk * BM);
+          tma_load_2d(p_dst, &tmP, &ring_l.full[sl.stage], kb * C::kWordsPerRow, n_blk * BN);
+          sl.advance();
         }
       }
     }
@@ -146,8 +136,8 @@ w4a16_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
     // ===================== consumers: rows 64 * c .. 64 * c + 63 of the tile =====================
     const int c = (warp - C::kConsumerWarp0) >> 2;
     const int tid = threadIdx.x & 127;
-    int sl = 0, sb = 0;
-    uint32_t phl = 0, phb = 0;
+    PipeState<kLStages> sl;
+    PipeState<kBStages> sb;
     for (int u = blockIdx.x; u < p.num_units; u += gridDim.x) {
       int m_blk, n_blk;
       grouped_tile(u, p.num_units / p.n_tiles_n, p.n_tiles_n, p.gn, m_blk, n_blk);
@@ -156,11 +146,11 @@ w4a16_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
       for (int i = 0; i < 64; ++i) acc[i] = 0.f;
       int prev_l = -1, prev_b = -1;
       for (int kb = 0; kb < p.kb_total; ++kb) {
-        mbar_wait(&fullL[sl], phl);              // X tile landed
-        mbar_wait(&readyB[sb], phb);             // W tile dequantised
+        ring_l.wait_full(sl);                    // X tile landed
+        ring_b.wait_full(sb);                    // W tile dequantised
         wgmma_fence();
-        const uint32_t a_addr = smem_u32(ringL + sl * kLBytes) + c * 64 * 128;
-        const uint32_t b_addr = smem_u32(ringB + sb * kBBytes);
+        const uint32_t a_addr = smem_u32(ringL + sl.stage * kLBytes) + c * 64 * 128;
+        const uint32_t b_addr = smem_u32(ringB + sb.stage * kBBytes);
 #pragma unroll
         for (int k = 0; k < BK / 16; ++k) {
           const uint64_t adesc = make_smem_desc(a_addr + k * 32, 16, 1024);
@@ -170,19 +160,19 @@ w4a16_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
         wgmma_commit();
         wgmma_wait<1>();                         // the previous step's group has retired
         if (prev_l >= 0 && tid == 0) {
-          mbar_arrive(&emptyL[prev_l]);
-          mbar_arrive(&emptyB[prev_b]);
+          ring_l.release(prev_l);
+          ring_b.release(prev_b);
         }
-        prev_l = sl;
-        prev_b = sb;
-        if (++sl == kLStages) { sl = 0; phl ^= 1; }
-        if (++sb == kBStages) { sb = 0; phb ^= 1; }
+        prev_l = sl.stage;
+        prev_b = sb.stage;
+        sl.advance();
+        sb.advance();
       }
       wgmma_wait<0>();
       fence_acc(acc);
       if (prev_l >= 0 && tid == 0) {
-        mbar_arrive(&emptyL[prev_l]);
-        mbar_arrive(&emptyB[prev_b]);
+        ring_l.release(prev_l);
+        ring_b.release(prev_b);
       }
       // ---- epilogue from the accumulator registers ----
       store_linear_m64n128<DT>(acc, static_cast<int64_t>(m_blk) * BM + c * 64,
@@ -224,17 +214,16 @@ w4a16_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
       uint32_t s_cur = 0u, z_cur = 0u;
       if (kb < p.kb_total) load_qparams(n0, kb / steps_per_group, s_cur, z_cur);
       for (; kb < p.kb_total; kb += NG) {
-        const uint32_t my = it + kb;
-        const int sl = my % kLStages, sb = my % kBStages;
-        const uint32_t phl = (my / kLStages) & 1u, phb = (my / kBStages) & 1u;
+        const auto sl = PipeState<kLStages>::at(it + kb);
+        const auto sb = PipeState<kBStages>::at(it + kb);
         // qparams of this group's NEXT step are requested now and consumed next iteration
         uint32_t s_nxt = s_cur, z_nxt = z_cur;
         if (kb + NG < p.kb_total && (kb + NG) / steps_per_group != kb / steps_per_group)
           load_qparams(n0, (kb + NG) / steps_per_group, s_nxt, z_nxt);
-        mbar_wait(&fullL[sl], phl);
-        mbar_wait(&emptyB[sb], phb ^ 1);
-        const uint8_t* pk = ringL + sl * kLBytes + kABytes;
-        uint8_t* bt = ringB + sb * kBBytes;
+        ring_l.wait_full(sl);
+        ring_b.wait_empty(sb);
+        const uint8_t* pk = ringL + sl.stage * kLBytes + kABytes;
+        uint8_t* bt = ringB + sb.stage * kBBytes;
         const float z_c = have_zeros ? widen(z_cur) : p.zero_default;
         const float zm_cur = 8388608.0f + z_c;        // (2^23 + q) - (2^23 + z) = q - z exactly
         const float s_c = (n0 < p.N) ? widen(s_cur) : 0.f;
@@ -313,8 +302,8 @@ w4a16_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
         fence_proxy_async_smem();
         __syncwarp();
         if (lane == 0) {
-          mbar_arrive(&readyB[sb]);
-          mbar_arrive(&emptyL[sl]);                // packed tile consumed
+          mbar_arrive(&ring_b.full[sb.stage]);
+          ring_l.release(sl.stage);                // packed tile consumed
         }
         s_cur = s_nxt;
         z_cur = z_nxt;
@@ -350,7 +339,6 @@ static int gemm_wNa16(const void* x, const int32_t* wq, const void* scales, cons
   }
   using C = Cfg<kBits>;
   constexpr int wpr = C::kWordsPerRow;
-  constexpr int kThreads = C::kThreads;
   CUtensorMap tmA, tmP;
   if (int rc = encode_tmap_2d(&tmA, x, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, M, K, K, BM, BK,
                               CU_TENSOR_MAP_SWIZZLE_128B))
@@ -379,15 +367,9 @@ static int gemm_wNa16(const void* x, const int32_t* wq, const void* scales, cons
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   constexpr int smem = C::kSmemBytes;
   static_assert(smem <= 227 * 1024, "shared memory budget");
-  LLMC_ONCE_PER_DEVICE({
-    LLMC_CHECK_CUDA(cudaFuncSetAttribute(w4a16_gemm_kernel<true, kBits>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-    LLMC_CHECK_CUDA(cudaFuncSetAttribute(w4a16_gemm_kernel<false, kBits>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-  });
-  const int grid = p.num_units < kNumSMs ? p.num_units : kNumSMs;
-  if (dtype == LLMC_BF16) w4a16_gemm_kernel<true, kBits><<<grid, kThreads, smem, st>>>(tmA, tmP, p);
-  else w4a16_gemm_kernel<false, kBits><<<grid, kThreads, smem, st>>>(tmA, tmP, p);
-  LLMC_CHECK_LAUNCH();
-  return LLMC_OK;
+  return launch_persistent(dtype == LLMC_BF16 ? w4a16_gemm_kernel<true, kBits>
+                                              : w4a16_gemm_kernel<false, kBits>,
+                           p.num_units, C::kThreads, smem, st, tmA, tmP, p);
 }
 
 extern "C" int llmc_gemm_w4a16(const void* x, const int32_t* wq, const void* scales,

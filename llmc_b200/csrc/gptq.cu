@@ -547,12 +547,9 @@ extern "C" int llmc_gptq_prepare(const float* H, int64_t C, const int64_t* perm,
                  (long long)C);
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   const int smem = static_cast<int>(C * 4);
-  LLMC_ONCE_PER_DEVICE({
-    LLMC_CHECK_CUDA(cudaFuncSetAttribute(gather_h_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
-    LLMC_CHECK_CUDA(cudaFuncSetAttribute(gather_w_kernel<LLMC_F32>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
-    LLMC_CHECK_CUDA(cudaFuncSetAttribute(gather_w_kernel<LLMC_F16>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
-    LLMC_CHECK_CUDA(cudaFuncSetAttribute(gather_w_kernel<LLMC_BF16>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
-  });
+  if (int rc = opt_in_smem(gather_h_kernel, 200 * 1024)) return rc;
+  for (auto kern : {gather_w_kernel<LLMC_F32>, gather_w_kernel<LLMC_F16>, gather_w_kernel<LLMC_BF16>})
+    if (int rc = opt_in_smem(kern, 200 * 1024)) return rc;
   diag_mean_kernel<<<1, 256, 0, st>>>(H, C, percdamp, diag_scratch);
   LLMC_CHECK_LAUNCH();
   // W first: it reads the ORIGINAL diagonal of H (dead test), Hp may alias neither H nor W
@@ -577,9 +574,7 @@ extern "C" int llmc_gptq_prepare(const float* H, int64_t C, const int64_t* perm,
 template <class F>
 static int sweep_schedule(float* W, const float* Hinv, int64_t R, int64_t C, int64_t group,
                           bool wide_dynamic_group, void* workspace, cudaStream_t st, F&& launch_inblock) {
-  LLMC_ONCE_PER_DEVICE({
-    LLMC_CHECK_CUDA(cudaFuncSetAttribute(trailing_update_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kTrailingSmem));
-  });
+  if (int rc = opt_in_smem(trailing_update_kernel, kTrailingSmem)) return rc;
   const int64_t Rpad = ((R + GB - 1) / GB) * GB;
   // [512][Rpad] x {err, hi, lo}, two sets selected by the parity of the super-panel
   float* const err_set[2] = {reinterpret_cast<float*>(workspace),
@@ -707,9 +702,7 @@ extern "C" int llmc_gptq_colblock(float* W, const float* Hinv, int64_t R, int64_
   LLMC_CHECK_ARG(static_groups || q_dtype == LLMC_F32, "gptq_colblock: dynamic groups write fp32 qparams");
   LLMC_CHECK_ARG(workspace_bytes >= llmc_gptq_workspace_bytes(R, C), "gptq_colblock: workspace too small");
   cudaStream_t st = static_cast<cudaStream_t>(stream);
-  LLMC_ONCE_PER_DEVICE({
-    LLMC_CHECK_CUDA(cudaFuncSetAttribute(gptq_inblock_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kInblockSmem));
-  });
+  if (int rc = opt_in_smem(gptq_inblock_kernel, kInblockSmem)) return rc;
   LLMC_CHECK_CUDA(cudaMemsetAsync(losses, 0, R * sizeof(float), st));
   InblockArgs a{};
   a.W = W; a.Hinv = Hinv; a.R = R; a.C = C;
@@ -752,9 +745,7 @@ extern "C" int llmc_spqr_colblock(float* W, const float* Hinv, int64_t R, int64_
                  (long long)group, (long long)C);
   LLMC_CHECK_ARG(workspace_bytes >= llmc_gptq_workspace_bytes(R, C), "spqr_colblock: workspace too small");
   cudaStream_t st = static_cast<cudaStream_t>(stream);
-  LLMC_ONCE_PER_DEVICE({
-    LLMC_CHECK_CUDA(cudaFuncSetAttribute(spqr_inblock_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kSpqrSmem));
-  });
+  if (int rc = opt_in_smem(spqr_inblock_kernel, kSpqrSmem)) return rc;
   LLMC_CHECK_CUDA(cudaMemsetAsync(losses, 0, R * sizeof(float), st));
   SpqrArgs a{};
   a.W = W; a.Hinv = Hinv; a.R = R; a.C = C; a.ng = C / group;

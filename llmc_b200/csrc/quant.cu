@@ -740,9 +740,7 @@ static int launch_fast(const QuantArgs& a, int mode, int bits, int64_t total_gro
 #define QF_GO(MODE, BITS)                                                                          \
   do {                                                                                             \
     auto kern = quant_group_fast_kernel<DT, G, MODE, BITS>;                                        \
-    LLMC_ONCE_PER_DEVICE({                                                                         \
-      LLMC_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem)); \
-    });                                                                                            \
+    if (int rc = opt_in_smem(kern, smem)) return rc;                                               \
     kern<<<grid, TG, smem, st>>>(a, total_groups);                                                 \
   } while (0)
   if (mode == M_NONE) QF_GO(M_NONE, 4);

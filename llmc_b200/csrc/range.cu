@@ -142,11 +142,8 @@ extern "C" int llmc_mse_range(const void* w, int64_t rows, int64_t cols, int dty
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   constexpr int kCacheCols = 24 * 1024;                      // 96 KB of fp32
   const int smem = (cols <= kCacheCols ? static_cast<int>(cols) : 0) * 4;
-  LLMC_ONCE_PER_DEVICE({
-    LLMC_CHECK_CUDA(cudaFuncSetAttribute(rg::mse_range_kernel<LLMC_F32>, cudaFuncAttributeMaxDynamicSharedMemorySize, kCacheCols * 4));
-    LLMC_CHECK_CUDA(cudaFuncSetAttribute(rg::mse_range_kernel<LLMC_F16>, cudaFuncAttributeMaxDynamicSharedMemorySize, kCacheCols * 4));
-    LLMC_CHECK_CUDA(cudaFuncSetAttribute(rg::mse_range_kernel<LLMC_BF16>, cudaFuncAttributeMaxDynamicSharedMemorySize, kCacheCols * 4));
-  });
+  for (auto kern : {rg::mse_range_kernel<LLMC_F32>, rg::mse_range_kernel<LLMC_F16>, rg::mse_range_kernel<LLMC_BF16>})
+    if (int rc = opt_in_smem(kern, kCacheCols * 4)) return rc;
   const int64_t grid_x = rows < static_cast<int64_t>(kNumSMs) * 16 ? rows : static_cast<int64_t>(kNumSMs) * 16;
 #define CALL(DT)                                                                                  \
   rg::mse_range_kernel<DT><<<(int)grid_x, rg::kThreads, smem, st>>>(                              \

@@ -78,6 +78,64 @@ __device__ __forceinline__ void tma_load_2d(void* dst, const CUtensorMap* m, uin
       : "memory");
 }
 
+// ---- TMA rings ------------------------------------------------------------------------------
+// A ring is kStages shared-memory stages that a producer fills and consumers drain, with two
+// mbarriers per stage placed after the kernel's ring data: full[s] completes when stage s holds
+// its data (TMA transaction bytes, or the producer's arrivals), empty[s] when every consumer has
+// released it.  Each role walks the stages in the same order with its own PipeState; the n-th use
+// of a stage waits for parity n & 1, and the producer's first pass over the ring waits on the
+// parity before that, which a freshly initialised barrier reports complete.
+
+// 1024-byte aligned start of the rings (a 128-byte swizzle atom is 8 rows = 1024 bytes) in the
+// kernel's dynamic shared memory.  Offsetting the extern array, instead of rounding its address as
+// an integer, keeps the result a pointer the compiler knows to be shared: plain loads and stores
+// through it compile to LDS / STS, not generic LD / ST.
+__device__ __forceinline__ uint8_t* ring_base(uint8_t* smem_raw) {
+  const uint32_t raw = smem_u32(smem_raw);
+  return smem_raw + ((0u - raw) & 1023u);
+}
+// Dynamic shared memory of a kernel whose rings take ring_bytes: the alignment slack above and
+// 256 bytes for the barriers (two per stage, at most 16 stages in all).
+constexpr int ring_smem_bytes(int ring_bytes) { return ring_bytes + 1024 + 256; }
+
+template <int kStages>
+struct PipeState {
+  int stage = 0;
+  uint32_t phase = 0;
+  __device__ __forceinline__ void advance() {
+    if (++stage == kStages) { stage = 0; phase ^= 1; }
+  }
+  // the state after i advances from the start
+  __device__ __forceinline__ static PipeState at(uint32_t i) {
+    return {static_cast<int>(i % kStages), (i / kStages) & 1u};
+  }
+};
+
+template <int kStages>
+struct Ring {
+  using State = PipeState<kStages>;
+  uint64_t* full;                   // full[kStages], followed by empty[kStages]
+  __device__ __forceinline__ explicit Ring(void* bars) : full(static_cast<uint64_t*>(bars)) {}
+  __device__ __forceinline__ void* end() const { return full + 2 * kStages; }
+  // by one thread, followed by fence_barrier_init and a CTA barrier
+  __device__ __forceinline__ void init(uint32_t full_count, uint32_t empty_count) const {
+    for (int s = 0; s < kStages; ++s) {
+      mbar_init(&full[s], full_count);
+      mbar_init(&full[kStages + s], empty_count);
+    }
+  }
+  __device__ __forceinline__ void wait_full(const State& st) const {
+    mbar_wait(&full[st.stage], st.phase);
+  }
+  __device__ __forceinline__ void wait_empty(const State& st) const {
+    mbar_wait(&full[kStages + st.stage], st.phase ^ 1);
+  }
+  __device__ __forceinline__ void expect_tx(const State& st, uint32_t bytes) const {
+    mbar_expect_tx(&full[st.stage], bytes);
+  }
+  __device__ __forceinline__ void release(int stage) const { mbar_arrive(&full[kStages + stage]); }
+};
+
 // ---- wgmma ----------------------------------------------------------------------------------
 // Shared-memory matrix descriptor (64 bit):
 //   [0,14)  start address >> 4        [16,30) leading-dim byte offset >> 4
@@ -184,10 +242,46 @@ __device__ __forceinline__ void grouped_tile(int u, int m_tiles, int n_tiles, in
   n_blk = g * gn + (rem - m_blk * gsz);
 }
 
-// The F.linear epilogue: stores this thread's part of an m64n128 accumulator fragment (layout at
-// wgmma_m64n128k16_bf16) whose element (0, 0) is Y[row0][col0] of the DT matrix Y[M, N] with row
-// stride ld.  The bias (DT, may be null) is added in fp32 before the single rounding, as F.linear
-// does.  Column pairs are stored as one 32-bit word when ld is even, element by element otherwise.
+// Stores the 16-bit pair pk (pack_pair) of columns col, col + 1 at o = &Y[row][col], the second
+// element only if `pair`: one 32-bit word when ld is even (o is then 4-byte aligned), element by
+// element otherwise.
+__device__ __forceinline__ void store_pair16(uint16_t* o, uint32_t pk, bool pair, int64_t ld) {
+  if (pair && (ld & 1) == 0) *reinterpret_cast<uint32_t*>(o) = pk;
+  else {
+    o[0] = static_cast<uint16_t>(pk & 0xffffu);
+    if (pair) o[1] = static_cast<uint16_t>(pk >> 16);
+  }
+}
+
+// Stores this thread's part of an m64n128 accumulator fragment (layout at wgmma_m64n128k16_bf16)
+// whose element (0, 0) is Y[row0][col0] of the fp32 matrix Y[M, N] with row stride ld.  Column
+// pairs are stored as one 8-byte word when ld is even, element by element otherwise.
+__device__ __forceinline__ void store_f32_m64n128(const float (&acc)[64], int64_t row0, int64_t col0,
+                                                  int64_t M, int64_t N, int64_t ld, float* out) {
+  const int tid = threadIdx.x & 127, lane = threadIdx.x & 31;
+#pragma unroll
+  for (int j = 0; j < 16; ++j) {
+    const int64_t col = col0 + 8 * j + 2 * (lane & 3);
+    if (col >= N) continue;
+    const bool pair = col + 1 < N;
+#pragma unroll
+    for (int i = 0; i < 2; ++i) {
+      const int64_t row = row0 + (tid >> 5) * 16 + (lane >> 2) + 8 * i;
+      if (row >= M) continue;
+      const float v0 = acc[4 * j + 2 * i], v1 = acc[4 * j + 2 * i + 1];
+      float* o = out + row * ld + col;
+      if (pair && (ld & 1) == 0) *reinterpret_cast<float2*>(o) = make_float2(v0, v1);
+      else {
+        o[0] = v0;
+        if (pair) o[1] = v1;
+      }
+    }
+  }
+}
+
+// The F.linear epilogue: stores this thread's part of an m64n128 accumulator fragment whose
+// element (0, 0) is Y[row0][col0] of the DT matrix Y[M, N] with row stride ld.  The bias (DT, may
+// be null) is added in fp32 before the single rounding, as F.linear does.
 template <int DT>
 __device__ __forceinline__ void store_linear_m64n128(const float (&acc)[64], int64_t row0,
                                                      int64_t col0, int64_t M, int64_t N, int64_t ld,
@@ -210,13 +304,7 @@ __device__ __forceinline__ void store_linear_m64n128(const float (&acc)[64], int
       if (row >= M) continue;
       float v0 = acc[4 * j + 2 * i], v1 = acc[4 * j + 2 * i + 1];
       if (bs != nullptr) { v0 += b0; v1 += b1; }
-      const uint32_t pk = pack_pair<DT>(v0, v1);
-      uint16_t* o = static_cast<uint16_t*>(out) + row * ld + col;
-      if (pair && (ld & 1) == 0) *reinterpret_cast<uint32_t*>(o) = pk;
-      else {
-        o[0] = static_cast<uint16_t>(pk & 0xffffu);
-        if (pair) o[1] = static_cast<uint16_t>(pk >> 16);
-      }
+      store_pair16(static_cast<uint16_t*>(out) + row * ld + col, pack_pair<DT>(v0, v1), pair, ld);
     }
   }
 }

@@ -17,7 +17,7 @@
 // The GPTQ weight update has BOTH operands MN-major, which Hopper's wgmma cannot read for tf32
 // (tf32 wgmma operands must be K-major), so the MMAs are warp-level mma.sync m16n8k8 whose
 // fragments are gathered from shared memory in either layout.
-// Structure: one TMA producer warp fills a 3-stage ring of 128B-swizzled tiles (mbarrier
+// Structure: one TMA producer warp fills a 3-stage tc::Ring of 128B-swizzled tiles (mbarrier
 // transaction counts); eight MMA warps (2 x 4, 64 x 32 each) compute a 128 x 128 tile with fp32
 // register accumulators and write it back with the fused epilogue.
 #include "tc.cuh"
@@ -34,7 +34,7 @@ constexpr int kABytes = BM * BK * 4;             // 16 KB (per hi / lo)
 constexpr int kBBytes = BN * BK * 4;             // 16 KB
 constexpr int kStageBytes = 2 * (kABytes + kBBytes);   // 64 KB
 constexpr int kBoxBytes = 32 * BK * 4;           // MN-major box: 32 MN x 32 K rows = 4 KB
-constexpr int kSmemBytes = kStages * kStageBytes + 1024 + 256;
+constexpr int kSmemBytes = ring_smem_bytes(kStages * kStageBytes);
 constexpr int kMmaWarps = 8;
 constexpr int kThreads = (kMmaWarps + 1) * 32;   // + the TMA warp
 struct Params {
@@ -189,19 +189,14 @@ tf32x3_kernel(const __grid_constant__ CUtensorMap tmAhi, const __grid_constant__
               const __grid_constant__ CUtensorMap tmBhi, const __grid_constant__ CUtensorMap tmBlo,
               const Params p) {
   extern __shared__ __align__(1024) uint8_t smem_raw[];
-  // 1024-byte aligned ring (swizzle atoms).  Offsetting the array keeps `smem` a pointer the
-  // compiler knows to be shared; the MMA warps address the ring by 32-bit shared addresses.
-  const uint32_t raw = smem_u32(smem_raw);
-  uint8_t* smem = smem_raw + (((raw + 1023u) & ~1023u) - raw);
-  const uint32_t ring = smem_u32(smem);
-  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + kStages * kStageBytes);
-  uint64_t* empty_bar = full_bar + kStages;
+  uint8_t* smem = ring_base(smem_raw);
+  const Ring<kStages> ring(smem + kStages * kStageBytes);
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int kb_total = (p.K + BK - 1) / BK;
 
   if (threadIdx.x == 0) {
     prefetch_tmap(&tmAhi); prefetch_tmap(&tmAlo); prefetch_tmap(&tmBhi); prefetch_tmap(&tmBlo);
-    for (int s = 0; s < kStages; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], 1); }
+    ring.init(1, 1);
     fence_barrier_init();
   }
   __syncthreads();
@@ -209,39 +204,39 @@ tf32x3_kernel(const __grid_constant__ CUtensorMap tmAhi, const __grid_constant__
   if (warp == kMmaWarps) {
     // ===================== TMA producer =====================
     if (lane == 0) {
-      int stage = 0;
-      uint32_t phase = 0;
+      PipeState<kStages> ps;
       for (int u = blockIdx.x; u < p.num_units; u += gridDim.x) {
         int m_blk, n_blk;
         decode(p, u, m_blk, n_blk);
         for (int kb = 0; kb < kb_total; ++kb) {
-          mbar_wait(&empty_bar[stage], phase ^ 1);
-          uint8_t* ahi = smem + stage * kStageBytes;
+          ring.wait_empty(ps);
+          uint8_t* ahi = smem + ps.stage * kStageBytes;
           uint8_t* alo = ahi + kABytes;
           uint8_t* bhi = alo + kABytes;
           uint8_t* blo = bhi + kBBytes;
-          mbar_expect_tx(&full_bar[stage], kStageBytes);
+          uint64_t* bar = &ring.full[ps.stage];
+          ring.expect_tx(ps, kStageBytes);
           if constexpr (!kAmn) {
-            tma_load_2d(ahi, &tmAhi, &full_bar[stage], kb * BK, m_blk * BM);
-            tma_load_2d(alo, &tmAlo, &full_bar[stage], kb * BK, m_blk * BM);
+            tma_load_2d(ahi, &tmAhi, bar, kb * BK, m_blk * BM);
+            tma_load_2d(alo, &tmAlo, bar, kb * BK, m_blk * BM);
           } else {
 #pragma unroll
             for (int i = 0; i < BM / 32; ++i) {
-              tma_load_2d(ahi + i * kBoxBytes, &tmAhi, &full_bar[stage], m_blk * BM + i * 32, kb * BK);
-              tma_load_2d(alo + i * kBoxBytes, &tmAlo, &full_bar[stage], m_blk * BM + i * 32, kb * BK);
+              tma_load_2d(ahi + i * kBoxBytes, &tmAhi, bar, m_blk * BM + i * 32, kb * BK);
+              tma_load_2d(alo + i * kBoxBytes, &tmAlo, bar, m_blk * BM + i * 32, kb * BK);
             }
           }
           if constexpr (!kBmn) {
-            tma_load_2d(bhi, &tmBhi, &full_bar[stage], kb * BK, n_blk * BN);
-            tma_load_2d(blo, &tmBlo, &full_bar[stage], kb * BK, n_blk * BN);
+            tma_load_2d(bhi, &tmBhi, bar, kb * BK, n_blk * BN);
+            tma_load_2d(blo, &tmBlo, bar, kb * BK, n_blk * BN);
           } else {
 #pragma unroll
             for (int i = 0; i < BN / 32; ++i) {
-              tma_load_2d(bhi + i * kBoxBytes, &tmBhi, &full_bar[stage], n_blk * BN + i * 32, kb * BK);
-              tma_load_2d(blo + i * kBoxBytes, &tmBlo, &full_bar[stage], n_blk * BN + i * 32, kb * BK);
+              tma_load_2d(bhi + i * kBoxBytes, &tmBhi, bar, n_blk * BN + i * 32, kb * BK);
+              tma_load_2d(blo + i * kBoxBytes, &tmBlo, bar, n_blk * BN + i * 32, kb * BK);
             }
           }
-          if (++stage == kStages) { stage = 0; phase ^= 1; }
+          ps.advance();
         }
       }
     }
@@ -252,8 +247,7 @@ tf32x3_kernel(const __grid_constant__ CUtensorMap tmAhi, const __grid_constant__
   const int wm = warp >> 2, wn = warp & 3;
   const int g = lane >> 2, t = lane & 3;
   const LaneOffsets<kAmn, kBmn> off(wm, wn, lane);
-  int stage = 0;
-  uint32_t phase = 0;
+  PipeState<kStages> ps;
   for (int u = blockIdx.x; u < p.num_units; u += gridDim.x) {
     int m_blk, n_blk;
     decode(p, u, m_blk, n_blk);
@@ -280,8 +274,9 @@ tf32x3_kernel(const __grid_constant__ CUtensorMap tmAhi, const __grid_constant__
 #pragma unroll
         for (int c = 0; c < 4; ++c) acc[a][b][c] = 0.f;
     for (int kb = 0; kb < kb_total; ++kb) {
-      mbar_wait(&full_bar[stage], phase);
-      const uint32_t ahi = ring + stage * kStageBytes, alo = ahi + kABytes;
+      ring.wait_full(ps);
+      // the MMA warps address the ring by 32-bit shared addresses
+      const uint32_t ahi = smem_u32(smem + ps.stage * kStageBytes), alo = ahi + kABytes;
       const uint32_t bhi = alo + kABytes, blo = bhi + kBBytes;
       // Fragments are double-buffered: B per k8 step (s), A per (s, 16-row block mt), so the next
       // fragments load while the current ones feed the MMAs.  Every accumulator sees hi*hi,
@@ -309,8 +304,8 @@ tf32x3_kernel(const __grid_constant__ CUtensorMap tmAhi, const __grid_constant__
       // arrive nor a warp sync waits for them; bar.sync does (it orders all prior shared-memory
       // accesses of the participating threads before it).
       asm volatile("bar.sync 1, %0;" ::"n"(kMmaWarps * 32) : "memory");
-      if (threadIdx.x == 0) mbar_arrive(&empty_bar[stage]);
-      if (++stage == kStages) { stage = 0; phase ^= 1; }
+      if (threadIdx.x == 0) ring.release(ps.stage);
+      ps.advance();
     }
 
     // ---- epilogue: fragment element (mt, nt, 2 i + c) = C[row g + 8 i][col 2 t + c] ----
@@ -462,19 +457,10 @@ int tf32x3_update(const Tf32x3Update& u, cudaStream_t st) {
     p.num_units = static_cast<int>(units);
   }
   if (p.num_units == 0) return LLMC_OK;
-  const int grid = (u.one_tile_per_cta || p.num_units < kNumSMs) ? p.num_units : kNumSMs;
-  LLMC_ONCE_PER_DEVICE({
-    LLMC_CHECK_CUDA(cudaFuncSetAttribute(tf32x3_kernel<false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemBytes));
-    LLMC_CHECK_CUDA(cudaFuncSetAttribute(tf32x3_kernel<false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemBytes));
-    LLMC_CHECK_CUDA(cudaFuncSetAttribute(tf32x3_kernel<true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemBytes));
-    LLMC_CHECK_CUDA(cudaFuncSetAttribute(tf32x3_kernel<true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemBytes));
-  });
-  if (!u.a.mn && !u.b.mn) tf32x3_kernel<false, false><<<grid, kThreads, kSmemBytes, st>>>(ta[0], ta[1], tb[0], tb[1], p);
-  else if (!u.a.mn) tf32x3_kernel<false, true><<<grid, kThreads, kSmemBytes, st>>>(ta[0], ta[1], tb[0], tb[1], p);
-  else if (!u.b.mn) tf32x3_kernel<true, false><<<grid, kThreads, kSmemBytes, st>>>(ta[0], ta[1], tb[0], tb[1], p);
-  else tf32x3_kernel<true, true><<<grid, kThreads, kSmemBytes, st>>>(ta[0], ta[1], tb[0], tb[1], p);
-  LLMC_CHECK_LAUNCH();
-  return LLMC_OK;
+  const auto kern = !u.a.mn ? (!u.b.mn ? tf32x3_kernel<false, false> : tf32x3_kernel<false, true>)
+                            : (!u.b.mn ? tf32x3_kernel<true, false> : tf32x3_kernel<true, true>);
+  return launch_persistent(kern, {p.num_units, u.one_tile_per_cta}, kThreads, kSmemBytes, st, ta[0],
+                           ta[1], tb[0], tb[1], p);
 }
 
 int split_tf32(const float* x, int64_t rows, int64_t cols, int64_t ld, float* hi, float* lo,
