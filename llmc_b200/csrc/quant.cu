@@ -438,6 +438,15 @@ __device__ __forceinline__ uint32_t max2(uint32_t a, uint32_t b) {
   }
 }
 
+// Group (min, max) from the packed pair reductions.  Like the scalar kernels' reductions, which start
+// from +inf / -inf and drop NaN, an all-NaN group yields (+inf, -inf): the packed min of NaN pairs
+// stays NaN, and the +-inf operands make the final fminf / fmaxf return the same identity.
+template <int DT>
+__device__ __forceinline__ void group_range(uint32_t mn2, uint32_t mx2, float& mn, float& mx) {
+  mn = fminf(fminf(pair_lo<DT>(mn2), pair_hi<DT>(mn2)), INFINITY);
+  mx = fmaxf(fmaxf(pair_lo<DT>(mx2), pair_hi<DT>(mx2)), -INFINITY);
+}
+
 // The per-chunk tail shared by the two fast kernels: 8 packed T values -> QDQ chunk | packed codes.
 //   v = yb + Ce does rint, + zero and the storage offset in one float add (see the kernel comment).
 template <int DT, int MODE, int BITS>
@@ -566,8 +575,8 @@ quant_group_fast_kernel(QuantArgs a, int64_t total_groups) {
         mn2 = min2<DT>(min2<DT>(mn2, x[c].x), min2<DT>(x[c].y, min2<DT>(x[c].z, x[c].w)));
         mx2 = max2<DT>(max2<DT>(mx2, x[c].x), max2<DT>(x[c].y, max2<DT>(x[c].z, x[c].w)));
       }
-      const float mn = fminf(pair_lo<DT>(mn2), pair_hi<DT>(mn2));
-      const float mx = fmaxf(pair_lo<DT>(mx2), pair_hi<DT>(mx2));
+      float mn, mx;
+      group_range<DT>(mn2, mx2, mn, mx);
       float s, z;
       qparams<DType<DT>>(mn, mx, a.sym, 1, a.qmin, a.qmax, s, z);
       DType<DT>::store(a.scales, g, s);
@@ -675,8 +684,8 @@ quant_row_fast_kernel(QuantArgs a) {
 #pragma unroll
     for (int w = 1; w < 8; ++w) { mn2 = min2<DT>(mn2, smn[w]); mx2 = max2<DT>(mx2, smx[w]); }
     __syncthreads();
-    const float mn = fminf(pair_lo<DT>(mn2), pair_hi<DT>(mn2));
-    const float mx = fmaxf(pair_lo<DT>(mx2), pair_hi<DT>(mx2));
+    float mn, mx;
+    group_range<DT>(mn2, mx2, mn, mx);
     float s, z;
     qparams<DType<DT>>(mn, mx, a.sym, 1, a.qmin, a.qmax, s, z);
     if (t == 0) {
@@ -754,6 +763,15 @@ static int launch_fast(const QuantArgs& a, int mode, int bits, int64_t total_gro
   return LLMC_OK;
 }
 
+// fast_tail packs codes as `bits`-bit fields: plain for asymmetric, offset-binary for symmetric
+// quantisers.  A use_range wider than that field (asym qmin < 0, sym beyond [-2^(b-1), 2^(b-1) - 1])
+// would borrow or carry across fields in the multiply-add chain; emit8 packs those correctly.
+static bool codes_fit_field(const QuantArgs& a, int bits) {
+  float lo, hi;
+  int_range(bits, a.sym, lo, hi);
+  return a.qmin >= lo && a.qmax <= hi;
+}
+
 // Which (mode, bits) of the fast kernel serves this call, or -1.
 static int fast_mode(const QuantArgs& a, int dtype) {
   if (a.ld != a.cols && !(a.ng == 1 && a.ld % 8 == 0)) return -1;      // groups need dense rows
@@ -768,9 +786,9 @@ static int fast_mode(const QuantArgs& a, int dtype) {
     case LLMC_OUT_QDQ: return (a.out_dtype == dtype && (a.ld_out == a.cols || a.ng == 1)) ? M_QDQ : -1;
     // asymmetric codes + the +2^(bit-1) storage offset overflow their field and the reference ORs
     // the overlapping bits (module_utils.py:842-856): fast_tail reproduces that on the packed word
-    case LLMC_OUT_PACK_VLLM: return (a.bit == 4 || a.bit == 8) ? M_PACK : -1;
+    case LLMC_OUT_PACK_VLLM: return (a.bit == 4 || a.bit == 8) && codes_fit_field(a, a.bit) ? M_PACK : -1;
     case LLMC_OUT_CODES_I8:
-    case LLMC_OUT_CODES_U8: return a.bit == 8 ? M_CODES8 : -1;
+    case LLMC_OUT_CODES_U8: return a.bit == 8 && codes_fit_field(a, 8) ? M_CODES8 : -1;
     default: return -1;
   }
 }

@@ -77,10 +77,11 @@ LLMC_HD float quant_code_zp(float x, const Div& div, float z, float qmin, float 
   return fminf(fmaxf(rintf(t), qmin), qmax);
 }
 
-// quant.py:710-712: (q - z) * s
+// quant.py:710-712: (q - z) * s, both ops rounded to T.  q - z is exact for integer zero-points;
+// the real-valued ones of round_zp = false need its rounding.
 template <class Round>
 LLMC_HD float dequant(float q, float s, float z) {
-  return Round::rT(mul(q - z, s));
+  return Round::rT(mul(Round::rT(sub(q, z)), s));
 }
 
 // ---- dividers: x / s for a fixed s, correctly rounded to fp32 ---------------------------------
@@ -95,6 +96,10 @@ struct IeeeDiv {
 // followed by one exact-remainder correction is the correctly rounded quotient (the remainder
 // x - q0*s is exact in fp32 and the corrected value is within 2^-47 of x/s while fp32 rounding
 // boundaries are >= 2^-36 away; DESIGN.md §3).  Not exact for wider operands.
+// Domain: finite quotients.  Where IEEE gives a non-finite quotient of a finite x — |x / s| beyond
+// fp32 range (bf16 only) or s = inf (a group holding +-inf) — this returns NaN (inf - inf, 0 * inf),
+// which the clamp of quant_code turns into qmin instead of the IEEE code.  A guard for it measured
+// slower than run-to-run noise on the row kernel, so the divider stays as is.
 struct RecipDiv {
   float s, r;
   __device__ __forceinline__ explicit RecipDiv(float s_) : s(s_), r(dvd(1.0f, s_)) {}

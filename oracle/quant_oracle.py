@@ -22,8 +22,11 @@ import numpy as np
 import torch
 
 
-def int_range(bit, sym):
-    """quant.py:665-677 -> (qmin, qmax) as 0-dim tensors with the reference's dtypes."""
+def int_range(bit, sym, qrange=None):
+    """quant.py:665-677 -> (qmin, qmax) as 0-dim tensors with the reference's dtypes.  `qrange`
+    is the quantizer's `int_range: [qmin, qmax]` option (quant.py:665-666)."""
+    if qrange is not None:
+        return torch.tensor(qrange[0]), torch.tensor(qrange[1])
     if sym:
         return torch.tensor(-(2 ** (bit - 1))), torch.tensor(2 ** (bit - 1) - 1)
     return torch.tensor(0.0), torch.tensor(2 ** bit - 1)
@@ -45,9 +48,9 @@ def minmax(t, granularity):
     return t.amin(dim=-1, keepdim=True), t.amax(dim=-1, keepdim=True)
 
 
-def qparams(min_val, max_val, bit, sym, round_zp=True):
-    """quant.py:545-559."""
-    qmin, qmax = int_range(bit, sym)
+def qparams(min_val, max_val, bit, sym, round_zp=True, qrange=None):
+    """quant.py:545-559 (qmin / qmax moved to the device of the range, :547-548)."""
+    qmin, qmax = (t.to(min_val.device) for t in int_range(bit, sym, qrange))
     if sym:
         abs_max = torch.max(max_val.abs(), min_val.abs()).clamp(min=1e-5)
         return abs_max / qmax, torch.tensor(0.0), qmax, qmin
@@ -58,8 +61,10 @@ def qparams(min_val, max_val, bit, sym, round_zp=True):
     return scales, zeros, qmax, qmin
 
 
-def quant(t, scales, zeros, qmax, qmin):
-    """quant.py:699-701."""
+def quant(t, scales, zeros, qmax, qmin, round_zp=True):
+    """quant.py:699-708; round_zp=False adds the real-valued zero-point before the rounding."""
+    if not round_zp:
+        return torch.clamp(torch.round(t / scales.clamp_min(1e-9) + zeros), qmin, qmax)
     return torch.clamp(torch.round(t / scales) + zeros, qmin, qmax)
 
 
@@ -68,17 +73,17 @@ def dequant(q, scales, zeros):
     return (q - zeros) * scales
 
 
-def tensor_qparams(w, bit, sym, granularity, group_size=None):
+def tensor_qparams(w, bit, sym, granularity, group_size=None, qrange=None):
     """quant.py:690-697 -> (grouped view, scales, zeros, qmax, qmin)."""
     t = group_view(w, granularity, group_size)
     mn, mx = minmax(t, granularity)
-    s, z, qmax, qmin = qparams(mn, mx, bit, sym)
+    s, z, qmax, qmin = qparams(mn, mx, bit, sym, qrange=qrange)
     return t, s, z, qmax, qmin
 
 
-def fake_quant_dynamic(w, bit, sym, granularity, group_size=None):
+def fake_quant_dynamic(w, bit, sym, granularity, group_size=None, qrange=None):
     """quant.py:833-869 (no int_indices / dim / current_bit)."""
-    t, s, z, qmax, qmin = tensor_qparams(w, bit, sym, granularity, group_size)
+    t, s, z, qmax, qmin = tensor_qparams(w, bit, sym, granularity, group_size, qrange)
     y = dequant(quant(t, s, z, qmax, qmin), s, z)
     return y.reshape(w.shape).to(w.dtype)
 
@@ -90,6 +95,16 @@ def fake_quant_static(w, scales, zeros, qmax, qmin, granularity, group_size=None
     return y.reshape(w.shape).to(w.dtype)
 
 
+def quant_static_gmap(w, scales, zeros, gmap, qmax, qmin, round_zp=True):
+    """Static qparams [R, ng] applied through a column -> group map (gptq.py:424-452: act-order
+    quantises W[:, perm] group by group, so column c of W uses group invperm[c] // group_size).
+    -> (codes, dequantised values), both in the promoted dtype of w and the qparams."""
+    s = scales[:, gmap]
+    z = zeros[:, gmap] if torch.is_tensor(zeros) and zeros.dim() else zeros
+    q = quant(w, s, z, qmax, qmin, round_zp)
+    return q, dequant(q, s, z)
+
+
 def code_dtype(bit, sym):
     """quant.py:890-896."""
     if bit == 8:
@@ -97,9 +112,9 @@ def code_dtype(bit, sym):
     return torch.int32
 
 
-def real_quant_dynamic(w, bit, sym, granularity, group_size=None):
+def real_quant_dynamic(w, bit, sym, granularity, group_size=None, qrange=None):
     """quant.py:916-953 -> (codes, scales [R, ng] | [1], zeros | None)."""
-    t, s, z, qmax, qmin = tensor_qparams(w, bit, sym, granularity, group_size)
+    t, s, z, qmax, qmin = tensor_qparams(w, bit, sym, granularity, group_size, qrange)
     codes = quant(t, s, z, qmax, qmin).reshape(w.shape).to(code_dtype(bit, sym))
     shape = 1 if granularity == 'per_tensor' else (w.shape[0], -1)
     zeros = None if sym else z.to(code_dtype(bit, sym)).view(shape)

@@ -23,7 +23,7 @@ def _q(bit, sym, gran, gs=None, **kw):
 
 
 def _same(a, b):
-    a = a.cpu()
+    a = a.to(b.device)
     assert a.shape == b.shape, (a.shape, b.shape)
     assert a.dtype == b.dtype, (a.dtype, b.dtype)
     if not torch.equal(a, b):
@@ -91,25 +91,31 @@ def test_golden_pack(golden_dir):
         _same(qzeros, c['qzeros'])
 
 
-SHAPES = [(4096, 4096), (1024, 4096), (3072, 768), (14336, 4096)]
+# (bit, sym, granularity, group) -> (rows, cols): every case at its own model shape, widths 768,
+# 3072, 4096 and 14336
+SHAPES = {
+    (4, False, 'per_group', 128): (4096, 4096), (4, True, 'per_group', 128): (14336, 4096),
+    (8, True, 'per_channel', None): (4096, 14336), (4, True, 'per_group', 64): (3072, 768),
+    (8, False, 'per_group', 256): (768, 3072), (3, False, 'per_group', 128): (4096, 14336),
+    (4, False, 'per_tensor', None): (1024, 4096), (8, True, 'per_group', 512): (1024, 3072),
+    # asymmetric PACK on the fast kernels (the reference's overflowing +2^(bit-1) offset)
+    (8, False, 'per_group', 128): (3072, 768), (4, False, 'per_group', 64): (14336, 4096),
+    (4, False, 'per_channel', None): (3072, 768), (8, False, 'per_channel', None): (1024, 3072)}
 
 
 @pytest.mark.parametrize('dtype', [torch.float16, torch.bfloat16, torch.float32])
-@pytest.mark.parametrize('bit,sym,gran,gs', [
-    (4, False, 'per_group', 128), (4, True, 'per_group', 128), (8, True, 'per_channel', None),
-    (4, True, 'per_group', 64), (8, False, 'per_group', 256), (3, False, 'per_group', 128),
-    (4, False, 'per_tensor', None), (8, True, 'per_group', 512),
-    # asymmetric PACK on the fast kernels (the reference's overflowing +2^(bit-1) offset)
-    (8, False, 'per_group', 128), (4, False, 'per_group', 64), (4, False, 'per_channel', None),
-    (8, False, 'per_channel', None)])
+@pytest.mark.parametrize('bit,sym,gran,gs', list(SHAPES))
 def test_oracle_full_shapes(dtype, bit, sym, gran, gs):
-    """Seeded random weights at model shapes; every output bit-exact vs the CPU oracle."""
+    """Seeded random weights at model shapes (widths 768, 3072, 4096 and 14336); every output
+    bit-exact vs the oracle.  The oracle runs on CUDA tensors (pinned to the CPU oracle by
+    test_gpu_quant_paths.py::test_cuda_oracle_equals_cpu_oracle), except per_tensor: torch's CUDA
+    kernels round a 0-dim scale to the tensor dtype, its CPU kernels (the parity target) do not."""
     torch.manual_seed(1234 + bit)
-    rows, cols = SHAPES[(bit + (gs or 0)) % len(SHAPES)]
-    rows = min(rows, 1024)                           # keep the CPU oracle to seconds
+    rows, cols = SHAPES[(bit, sym, gran, gs)]
+    dev = 'cpu' if gran == 'per_tensor' else 'cuda'
     w = (torch.randn(rows, cols) * 0.02)
     w[:, ::97] *= 6
-    w = w.to(dtype)
+    w = w.to(dtype).to(dev)
     q = _q(bit, sym, gran, gs)
     wc = w.cuda()
     codes, s, z = q.real_quant_weight_dynamic(wc)
@@ -123,7 +129,7 @@ def test_oracle_full_shapes(dtype, bit, sym, gran, gs):
     _same(q.fake_quant_weight_dynamic(wc), qo.fake_quant_dynamic(w, bit, sym, gran, gs))
     if gran != 'per_tensor' and bit in (4, 8):
         packed, ps, _ = q.real_quant_pack_vllm_dynamic(wc)
-        opacked, _ = qo.pack_vllm(ocodes, os_, bit)
+        opacked, _ = qo.pack_vllm(ocodes.cpu(), os_.cpu(), bit)
         _same(packed, opacked)
 
 
