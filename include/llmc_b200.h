@@ -204,7 +204,8 @@ int llmc_gptq_prepare(const float* H, int64_t C, const int64_t* perm, float perc
  *       U = cholesky( cholesky_inverse( cholesky(H) ), upper )
  *   computed as U = R^-1 where H = R R^T, R upper triangular (one reverse-ordered
  *   factorisation + one triangular inverse instead of potrf + potri + potrf; DESIGN.md).
- *   A  [C, C] fp32 in: SPD H (full); out: U in the upper triangle, zeros below.
+ *   A  [C, C] fp32 in: SPD H; only its upper triangle (diagonal included) is read;
+ *                 out: U in the upper triangle, zeros below.
  *   info: device int[1]: 0 if H is positive-definite, else k = the order of the first leading minor
  *         of the index-REVERSED matrix J H J that is not positive (the factorisation runs bottom-up).
  *   C must be a multiple of 8.  The inverse chain runs on a library-owned side stream (one per
