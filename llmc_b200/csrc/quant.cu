@@ -14,20 +14,56 @@
 
 namespace llmc {
 
+// Where and how a quantiser writes its results (out_mode LLMC_OUT_*).  Kernels take it as a
+// parameter of its own.  Nested in QuantArgs / StaticArgs, it makes nvcc 12.9 address the whole
+// parameter struct through a register, and every kernel that takes one compiles differently; the
+// tuned fast kernels lose up to a third of their instructions (quant_group_fast_kernel<fp16, 128,
+// PACK, 4>: 3920 -> 2768), a change to their speed that is not measured.  A separate parameter
+// keeps the code a flat parameter struct gives them.
+struct OutDesc {
+  int mode;
+  void* ptr;
+  int64_t ld;              // QDQ row stride (elements)
+  int dtype;               // QDQ dtype
+  int bit;
+  int64_t cols;            // CODES_*: row stride (elements)
+  int64_t packed_cols;     // PACK_VLLM: words per row
+};
+
+// Validates the output arguments of a quantiser call on `cols` columns and describes them in o.
+static int make_out(int mode, void* ptr, int64_t ld_out, int dtype, int bit, int64_t cols,
+                    OutDesc& o) {
+  if (mode < LLMC_OUT_NONE || mode > LLMC_OUT_PACK_VLLM) {
+    set_last_error("bad out_mode %d", mode);
+    return LLMC_EINVAL;
+  }
+  if (mode != LLMC_OUT_NONE && ptr == nullptr) {
+    set_last_error("out is NULL for out_mode %d", mode);
+    return LLMC_EINVAL;
+  }
+  if (bit < 2 || bit > 8) {
+    set_last_error("bit %d outside 2..8", bit);
+    return LLMC_EINVAL;
+  }
+  const int pf = 32 / bit;
+  o.ptr = ptr;
+  o.ld = (mode == LLMC_OUT_QDQ && ld_out > 0) ? ld_out : cols;
+  o.cols = cols;
+  o.packed_cols = (cols + pf - 1) / pf;
+  o.mode = mode;
+  o.dtype = dtype;
+  o.bit = bit;
+  return LLMC_OK;
+}
+
 struct QuantArgs {
   const void* w;
   int64_t rows, cols, ld;
   int64_t group, ng;       // elements per group, groups per row
   float qmin, qmax;
   int sym;
-  int bit;
   void* scales;            // [rows*ng] DT  (dynamic: out)
   void* zeros;             // [rows*ng] DT  (dynamic: out, asym only)
-  int out_mode;
-  void* out;
-  int64_t ld_out;          // QDQ row stride (elements)
-  int out_dtype;
-  int64_t packed_cols;     // PACK_VLLM: words per row
   const void* col_scale;   // optional [cols] DT: w' = rT(w * s[c]) first (AWQ, awq.py:39-46)
 };
 
@@ -36,54 +72,55 @@ struct QuantArgs {
 template <int DT>
 using Divider = std::conditional_t<DT == LLMC_F32, IeeeDiv, RecipDiv>;
 
+// Field i of a vLLM-packed word (module_utils.py:842-856): (code + off).to(uint8) << bit * i.  The
+// byte is wider than a field when bit < 8; the fields are OR-ed as the reference does.
+__device__ __forceinline__ uint32_t vllm_field(int code, int off, int bit, int i) {
+  return (static_cast<uint32_t>(code + off) & 0xffu) << (bit * i);
+}
+
+// 8 codes as the bytes (code + off), the first in the low byte of .x.
+__device__ __forceinline__ uint2 bytes8(const float (&q)[8], int off) {
+  uint32_t lo = 0, hi = 0;
+#pragma unroll
+  for (int i = 0; i < 4; ++i) {
+    lo |= vllm_field(static_cast<int>(q[i]), off, 8, i);
+    hi |= vllm_field(static_cast<int>(q[i + 4]), off, 8, i);
+  }
+  return make_uint2(lo, hi);
+}
+
 // Emit 8 consecutive codes/values of row r starting at column c (c % 8 == 0).
 template <int DT>
-__device__ __forceinline__ void emit8(const QuantArgs& a, int64_t r, int64_t c,
+__device__ __forceinline__ void emit8(const OutDesc& o, int64_t r, int64_t c,
                                       const float (&q)[8], float s, float z) {
-  switch (a.out_mode) {
+  switch (o.mode) {
     case LLMC_OUT_QDQ: {
       float y[8];
 #pragma unroll
       for (int i = 0; i < 8; ++i) y[i] = dequant<DType<DT>>(q[i], s, z);
-      store8_as(a.out_dtype, a.out, r * a.ld_out + c, y);
+      store8_as(o.dtype, o.ptr, r * o.ld + c, y);
       break;
     }
     case LLMC_OUT_CODES_I8:
-    case LLMC_OUT_CODES_U8: {
-      uint32_t lo = 0, hi = 0;
-#pragma unroll
-      for (int i = 0; i < 4; ++i) {
-        lo |= (static_cast<uint32_t>(static_cast<int>(q[i])) & 0xffu) << (8 * i);
-        hi |= (static_cast<uint32_t>(static_cast<int>(q[i + 4])) & 0xffu) << (8 * i);
-      }
-      *reinterpret_cast<uint2*>(reinterpret_cast<uint8_t*>(a.out) + r * a.cols + c) =
-          make_uint2(lo, hi);
+    case LLMC_OUT_CODES_U8:
+      *reinterpret_cast<uint2*>(reinterpret_cast<uint8_t*>(o.ptr) + r * o.cols + c) = bytes8(q, 0);
       break;
-    }
     case LLMC_OUT_CODES_I32: {
-      int4* p = reinterpret_cast<int4*>(reinterpret_cast<int32_t*>(a.out) + r * a.cols + c);
+      int4* p = reinterpret_cast<int4*>(reinterpret_cast<int32_t*>(o.ptr) + r * o.cols + c);
       p[0] = make_int4((int)q[0], (int)q[1], (int)q[2], (int)q[3]);
       p[1] = make_int4((int)q[4], (int)q[5], (int)q[6], (int)q[7]);
       break;
     }
     case LLMC_OUT_PACK_VLLM: {
-      // module_utils.py:842-856: (code + 2^(bit-1)).to(uint8) << bit*i, OR-ed.
-      const int off = 1 << (a.bit - 1);
-      int32_t* o = reinterpret_cast<int32_t*>(a.out) + r * a.packed_cols;
-      if (a.bit == 4) {
-        uint32_t wd = 0;
+      const int off = 1 << (o.bit - 1);
+      int32_t* wd = reinterpret_cast<int32_t*>(o.ptr) + r * o.packed_cols;
+      if (o.bit == 4) {
+        uint32_t w4 = 0;
 #pragma unroll
-        for (int i = 0; i < 8; ++i)
-          wd |= (static_cast<uint32_t>(static_cast<int>(q[i]) + off) & 0xffu) << (4 * i);
-        o[c >> 3] = static_cast<int32_t>(wd);
+        for (int i = 0; i < 8; ++i) w4 |= vllm_field(static_cast<int>(q[i]), off, 4, i);
+        wd[c >> 3] = static_cast<int32_t>(w4);
       } else {  // bit == 8
-        uint32_t lo = 0, hi = 0;
-#pragma unroll
-        for (int i = 0; i < 4; ++i) {
-          lo |= (static_cast<uint32_t>(static_cast<int>(q[i]) + off) & 0xffu) << (8 * i);
-          hi |= (static_cast<uint32_t>(static_cast<int>(q[i + 4]) + off) & 0xffu) << (8 * i);
-        }
-        *reinterpret_cast<uint2*>(o + (c >> 2)) = make_uint2(lo, hi);
+        *reinterpret_cast<uint2*>(wd + (c >> 2)) = bytes8(q, off);
       }
       break;
     }
@@ -91,11 +128,28 @@ __device__ __forceinline__ void emit8(const QuantArgs& a, int64_t r, int64_t c,
   }
 }
 
+// AWQ: the 8 values v of columns c.. become rT(v * col_scale[c..]) when there is a col_scale.
+template <int DT>
+__device__ __forceinline__ void awq_prescale8(const void* col_scale, int64_t c, float (&v)[8]) {
+  if (col_scale == nullptr) return;
+  float cs[8];
+  load8<DT>(col_scale, c, cs);
+#pragma unroll
+  for (int i = 0; i < 8; ++i) v[i] = DType<DT>::rT(fmul_rn(v[i], cs[i]));
+}
+
+// The dynamic kernels' qparams of group g: the scale, and the zero-point when asymmetric.
+template <int DT>
+__device__ __forceinline__ void store_qparams(void* scales, void* zeros, int sym, int64_t g, float s,
+                                              float z) {
+  DType<DT>::store(scales, g, s);
+  if (!sym && zeros) DType<DT>::store(zeros, g, z);
+}
+
 // ---- fast path: a sub-warp of LPG lanes owns one group; CH 8-element chunks per lane -----
 template <int DT, int CH>
 __global__ void __launch_bounds__(256)
-quant_dynamic_warp_kernel(QuantArgs a, int lpg, int64_t total_groups) {
-  using D = DType<DT>;
+quant_dynamic_warp_kernel(QuantArgs a, OutDesc o, int lpg, int64_t total_groups) {
   const int lane = threadIdx.x & 31;
   const int sub = lane & (lpg - 1);
   const int gpw = 32 / lpg;                       // groups per warp
@@ -118,12 +172,7 @@ quant_dynamic_warp_kernel(QuantArgs a, int lpg, int64_t total_groups) {
       const int ch = c * lpg + sub;
       if (active && ch < chunks) {
         load8<DT>(a.w, r * a.ld + col0 + ch * 8, v[c]);
-        if (a.col_scale != nullptr) {
-          float cs[8];
-          load8<DT>(a.col_scale, col0 + ch * 8, cs);
-#pragma unroll
-          for (int i = 0; i < 8; ++i) v[c][i] = D::rT(fmul_rn(v[c][i], cs[i]));
-        }
+        awq_prescale8<DT>(a.col_scale, col0 + ch * 8, v[c]);
 #pragma unroll
         for (int i = 0; i < 8; ++i) { mn = fminf(mn, v[c][i]); mx = fmaxf(mx, v[c][i]); }
       }
@@ -132,11 +181,8 @@ quant_dynamic_warp_kernel(QuantArgs a, int lpg, int64_t total_groups) {
     mx = warp_max(mx, lpg);
     float s, z;
     qparams<DType<DT>>(mn, mx, a.sym, 1, a.qmin, a.qmax, s, z);
-    if (active && sub == 0) {
-      D::store(a.scales, g, s);
-      if (!a.sym && a.zeros) D::store(a.zeros, g, z);
-    }
-    if (a.out_mode == LLMC_OUT_NONE) continue;
+    if (active && sub == 0) store_qparams<DT>(a.scales, a.zeros, a.sym, g, s, z);
+    if (o.mode == LLMC_OUT_NONE) continue;
     const Divider<DT> div{s};
 #pragma unroll
     for (int c = 0; c < CH; ++c) {
@@ -145,7 +191,7 @@ quant_dynamic_warp_kernel(QuantArgs a, int lpg, int64_t total_groups) {
         float q[8];
 #pragma unroll
         for (int i = 0; i < 8; ++i) q[i] = quant_code<DType<DT>>(v[c][i], div, z, a.qmin, a.qmax);
-        emit8<DT>(a, r, col0 + ch * 8, q, s, z);
+        emit8<DT>(o, r, col0 + ch * 8, q, s, z);
       }
     }
   }
@@ -168,8 +214,7 @@ __device__ __forceinline__ void block_minmax(float& mn, float& mx) {
 // ---- large groups (per_channel / per_token rows): one CTA per group, second pass from L2 ---
 template <int DT>
 __global__ void __launch_bounds__(256)
-quant_dynamic_block_kernel(QuantArgs a, int64_t total_groups) {
-  using D = DType<DT>;
+quant_dynamic_block_kernel(QuantArgs a, OutDesc o, int64_t total_groups) {
   const int chunks = static_cast<int>(a.group >> 3);
   for (int64_t g = blockIdx.x; g < total_groups; g += gridDim.x) {
     const int64_t r = g / a.ng, j = g - r * a.ng;
@@ -178,36 +223,23 @@ quant_dynamic_block_kernel(QuantArgs a, int64_t total_groups) {
     for (int ch = threadIdx.x; ch < chunks; ch += blockDim.x) {
       float v[8];
       load8<DT>(a.w, base + ch * 8, v);
-      if (a.col_scale != nullptr) {
-        float cs[8];
-        load8<DT>(a.col_scale, j * a.group + ch * 8, cs);
-#pragma unroll
-        for (int i = 0; i < 8; ++i) v[i] = D::rT(fmul_rn(v[i], cs[i]));
-      }
+      awq_prescale8<DT>(a.col_scale, j * a.group + ch * 8, v);
 #pragma unroll
       for (int i = 0; i < 8; ++i) { mn = fminf(mn, v[i]); mx = fmaxf(mx, v[i]); }
     }
     block_minmax(mn, mx);
     float s, z;
     qparams<DType<DT>>(mn, mx, a.sym, 1, a.qmin, a.qmax, s, z);
-    if (threadIdx.x == 0) {
-      D::store(a.scales, g, s);
-      if (!a.sym && a.zeros) D::store(a.zeros, g, z);
-    }
-    if (a.out_mode == LLMC_OUT_NONE) continue;
+    if (threadIdx.x == 0) store_qparams<DT>(a.scales, a.zeros, a.sym, g, s, z);
+    if (o.mode == LLMC_OUT_NONE) continue;
     const Divider<DT> div{s};
     for (int ch = threadIdx.x; ch < chunks; ch += blockDim.x) {
       float v[8], q[8];
       load8<DT>(a.w, base + ch * 8, v);
-      if (a.col_scale != nullptr) {
-        float cs[8];
-        load8<DT>(a.col_scale, j * a.group + ch * 8, cs);
-#pragma unroll
-        for (int i = 0; i < 8; ++i) v[i] = D::rT(fmul_rn(v[i], cs[i]));
-      }
+      awq_prescale8<DT>(a.col_scale, j * a.group + ch * 8, v);
 #pragma unroll
       for (int i = 0; i < 8; ++i) q[i] = quant_code<DType<DT>>(v[i], div, z, a.qmin, a.qmax);
-      emit8<DT>(a, r, j * a.group + ch * 8, q, s, z);
+      emit8<DT>(o, r, j * a.group + ch * 8, q, s, z);
     }
   }
 }
@@ -216,23 +248,19 @@ quant_dynamic_block_kernel(QuantArgs a, int64_t total_groups) {
 template <int DT>
 __global__ void __launch_bounds__(256)
 qparams_generic_kernel(QuantArgs a, int64_t total_groups) {
-  using D = DType<DT>;
   for (int64_t g = blockIdx.x; g < total_groups; g += gridDim.x) {
     const int64_t r = g / a.ng, j = g - r * a.ng;
     const int64_t base = r * a.ld + j * a.group;
     float mn = INFINITY, mx = -INFINITY;
     for (int64_t i = threadIdx.x; i < a.group; i += blockDim.x) {
-      float v = D::load(a.w, base + i);
+      float v = DType<DT>::load(a.w, base + i);
       mn = fminf(mn, v);
       mx = fmaxf(mx, v);
     }
     block_minmax(mn, mx);
     float s, z;
     qparams<DType<DT>>(mn, mx, a.sym, 1, a.qmin, a.qmax, s, z);
-    if (threadIdx.x == 0) {
-      D::store(a.scales, g, s);
-      if (!a.sym && a.zeros) D::store(a.zeros, g, z);
-    }
+    if (threadIdx.x == 0) store_qparams<DT>(a.scales, a.zeros, a.sym, g, s, z);
   }
 }
 
@@ -246,13 +274,7 @@ struct StaticArgs {
   int64_t group;
   const int32_t* gmap;     // optional column -> group index
   float qmin, qmax;
-  int bit;
-  int out_mode;
-  void* out;
-  int64_t ld_out;
-  int out_dtype;
-  int64_t packed_cols;
-  int unit;                // elements per thread (8, or 32/bit for PACK with odd widths)
+  int unit;                // scalar kernel: elements per thread (8, or 32/bit for PACK_VLLM)
   int zp_inside;           // round_zp False: zero-point added before rounding, scale clamped at 1e-9
 };
 
@@ -262,12 +284,15 @@ __device__ __forceinline__ float load_w(const void* p, int64_t i) { return DType
 // CT = rounding dtype of every op (normally promote(w dtype, qparam dtype)); WT = weight storage
 // dtype; QT = qparam storage dtype.  CT == WT != QT == fp32 is torch's CPU "scalar operand"
 // path: a 0-dim fp32 scale keeps its fp32 value while results round to the tensor dtype.
-// The reciprocal-based divide is only exact when x and s both have <= 11 significant bits.
-#define LLMC_DV ((WT == QT && WT == CT) ? CT : LLMC_F32)
+// The reciprocal-based divide is only exact when x and s both have <= 11 significant bits, so the
+// static kernels divide in fp32 unless all three dtypes agree.
+template <int CT, int WT, int QT>
+constexpr int kStaticDivDT = (WT == QT && WT == CT) ? CT : LLMC_F32;
 // QT (qparam storage) == CT unless CT is fp32 and qparams are 16-bit, handled by QT.
 template <int CT, int WT, int QT>
 __global__ void __launch_bounds__(256)
-quant_static_kernel(StaticArgs a) {
+quant_static_kernel(StaticArgs a, OutDesc o) {
+  using Div = Divider<kStaticDivDT<CT, WT, QT>>;
   const int64_t units_per_row = (a.cols + a.unit - 1) / a.unit;
   const int64_t total = a.rows * units_per_row;
   for (int64_t u = static_cast<int64_t>(blockIdx.x) * blockDim.x + threadIdx.x; u < total;
@@ -275,10 +300,10 @@ quant_static_kernel(StaticArgs a) {
     const int64_t r = u / units_per_row;
     const int64_t c0 = (u - r * units_per_row) * a.unit;
     uint32_t word = 0;
-    const int off = 1 << (a.bit - 1);
+    const int off = 1 << (o.bit - 1);
     int64_t last_g = -1;
     float s = 1.f, z = 0.f;
-    Divider<LLMC_DV> div{1.f};
+    Div div{1.f};
     for (int i = 0; i < a.unit; ++i) {
       const int64_t c = c0 + i;
       if (c >= a.cols) break;
@@ -286,33 +311,33 @@ quant_static_kernel(StaticArgs a) {
       if (g != last_g) {
         s = DType<QT>::load(a.scales, r * a.q_row_stride + g);
         z = a.zeros ? DType<QT>::load(a.zeros, r * a.q_row_stride + g) : 0.f;
-        div = Divider<LLMC_DV>{a.zp_inside ? fmaxf(s, 1e-9f) : s};
+        div = Div{a.zp_inside ? fmaxf(s, 1e-9f) : s};
         last_g = g;
       }
       const float x = load_w<WT>(a.w, r * a.ld + c);
       const float q = a.zp_inside ? quant_code_zp<DType<CT>>(x, div, z, a.qmin, a.qmax)
                                   : quant_code<DType<CT>>(x, div, z, a.qmin, a.qmax);
-      switch (a.out_mode) {
+      switch (o.mode) {
         case LLMC_OUT_QDQ: {
-          store_as(a.out_dtype, a.out, r * a.ld_out + c, dequant<DType<CT>>(q, s, z));
+          store_as(o.dtype, o.ptr, r * o.ld + c, dequant<DType<CT>>(q, s, z));
           break;
         }
         case LLMC_OUT_CODES_I8:
         case LLMC_OUT_CODES_U8:
-          reinterpret_cast<uint8_t*>(a.out)[r * a.cols + c] =
+          reinterpret_cast<uint8_t*>(o.ptr)[r * o.cols + c] =
               static_cast<uint8_t>(static_cast<int>(q));
           break;
         case LLMC_OUT_CODES_I32:
-          reinterpret_cast<int32_t*>(a.out)[r * a.cols + c] = static_cast<int>(q);
+          reinterpret_cast<int32_t*>(o.ptr)[r * o.cols + c] = static_cast<int>(q);
           break;
         case LLMC_OUT_PACK_VLLM:
-          word |= (static_cast<uint32_t>(static_cast<int>(q) + off) & 0xffu) << (a.bit * i);
+          word |= vllm_field(static_cast<int>(q), off, o.bit, i);
           break;
         default: break;
       }
     }
-    if (a.out_mode == LLMC_OUT_PACK_VLLM)
-      reinterpret_cast<int32_t*>(a.out)[r * a.packed_cols + c0 / a.unit] =
+    if (o.mode == LLMC_OUT_PACK_VLLM)
+      reinterpret_cast<int32_t*>(o.ptr)[r * o.packed_cols + c0 / a.unit] =
           static_cast<int32_t>(word);
   }
 }
@@ -320,7 +345,8 @@ quant_static_kernel(StaticArgs a) {
 // vectorised static path: 8 aligned columns per thread, one group per 8 columns unless gmap.
 template <int CT, int WT, int QT>
 __global__ void __launch_bounds__(256)
-quant_static_vec8_kernel(StaticArgs a, QuantArgs e) {
+quant_static_vec8_kernel(StaticArgs a, OutDesc o) {
+  using Div = Divider<kStaticDivDT<CT, WT, QT>>;
   const int64_t units_per_row = a.cols >> 3;
   const int64_t total = a.rows * units_per_row;
   for (int64_t u = static_cast<int64_t>(blockIdx.x) * blockDim.x + threadIdx.x; u < total;
@@ -333,12 +359,12 @@ quant_static_vec8_kernel(StaticArgs a, QuantArgs e) {
       const int64_t g = c0 / a.group;
       const float s = DType<QT>::load(a.scales, r * a.q_row_stride + g);
       const float z = a.zeros ? DType<QT>::load(a.zeros, r * a.q_row_stride + g) : 0.f;
-      const Divider<LLMC_DV> div{a.zp_inside ? fmaxf(s, 1e-9f) : s};
+      const Div div{a.zp_inside ? fmaxf(s, 1e-9f) : s};
 #pragma unroll
       for (int i = 0; i < 8; ++i)
         q[i] = a.zp_inside ? quant_code_zp<DType<CT>>(x[i], div, z, a.qmin, a.qmax)
                            : quant_code<DType<CT>>(x[i], div, z, a.qmin, a.qmax);
-      emit8<CT>(e, r, c0, q, s, z);
+      emit8<CT>(o, r, c0, q, s, z);
     } else {
       // act-order gather: every column may belong to a different group; only QDQ/CODES.
       float y[8];
@@ -347,15 +373,15 @@ quant_static_vec8_kernel(StaticArgs a, QuantArgs e) {
         const int64_t g = a.gmap[c0 + i];
         const float s = DType<QT>::load(a.scales, r * a.q_row_stride + g);
         const float z = a.zeros ? DType<QT>::load(a.zeros, r * a.q_row_stride + g) : 0.f;
-        const Divider<LLMC_DV> div{a.zp_inside ? fmaxf(s, 1e-9f) : s};
+        const Div div{a.zp_inside ? fmaxf(s, 1e-9f) : s};
         q[i] = a.zp_inside ? quant_code_zp<DType<CT>>(x[i], div, z, a.qmin, a.qmax)
                            : quant_code<DType<CT>>(x[i], div, z, a.qmin, a.qmax);
         y[i] = dequant<DType<CT>>(q[i], s, z);
       }
-      if (a.out_mode == LLMC_OUT_QDQ) {
-        store8_as(a.out_dtype, a.out, r * a.ld_out + c0, y);
+      if (o.mode == LLMC_OUT_QDQ) {
+        store8_as(o.dtype, o.ptr, r * o.ld + c0, y);
       } else {
-        emit8<CT>(e, r, c0, q, 1.f, 0.f);
+        emit8<CT>(o, r, c0, q, 1.f, 0.f);
       }
     }
   }
@@ -512,7 +538,7 @@ __device__ __forceinline__ void fast_consts(float z, float qmin, float qmax, int
 
 template <int DT, int G, int MODE, int BITS>
 __global__ void __launch_bounds__(TG)
-quant_group_fast_kernel(QuantArgs a, int64_t total_groups) {
+quant_group_fast_kernel(QuantArgs a, OutDesc out, int64_t total_groups) {
   constexpr int CPG = G / 8;               // 16-byte chunks per group
   constexpr int RB = G * 2;                // bytes per group row
   constexpr int TILE = TG * RB;
@@ -579,8 +605,7 @@ quant_group_fast_kernel(QuantArgs a, int64_t total_groups) {
       group_range<DT>(mn2, mx2, mn, mx);
       float s, z;
       qparams<DType<DT>>(mn, mx, a.sym, 1, a.qmin, a.qmax, s, z);
-      DType<DT>::store(a.scales, g, s);
-      if (!a.sym && a.zeros) DType<DT>::store(a.zeros, g, z);
+      store_qparams<DT>(a.scales, a.zeros, a.sym, g, s, z);
       if constexpr (MODE != M_NONE) {
         // Tail of the chain after the exact division, with the rounding done by ONE float add:
         //   v = yb + Ce,  Ce = 1.5*2^23 + (z - o) + OFFE  (o = parity of z, OFFE = even storage offset)
@@ -604,11 +629,11 @@ quant_group_fast_kernel(QuantArgs a, int64_t total_groups) {
           }
         }
         if constexpr (MODE == M_PACK && BITS == 4) {
-          uint4* o = reinterpret_cast<uint4*>(reinterpret_cast<int32_t*>(a.out) + g * (G / 8));
+          uint4* o = reinterpret_cast<uint4*>(reinterpret_cast<int32_t*>(out.ptr) + g * (G / 8));
 #pragma unroll
           for (int c = 0; c < CPG; c += 4) o[c / 4] = make_uint4(x[c].x, x[c + 1].x, x[c + 2].x, x[c + 3].x);
         } else if constexpr (MODE == M_PACK || MODE == M_CODES8) {
-          uint4* o = reinterpret_cast<uint4*>(reinterpret_cast<uint8_t*>(a.out) + g * G);
+          uint4* o = reinterpret_cast<uint4*>(reinterpret_cast<uint8_t*>(out.ptr) + g * G);
 #pragma unroll
           for (int c = 0; c < CPG; c += 2) o[c / 2] = make_uint4(x[c].x, x[c].y, x[c + 1].x, x[c + 1].y);
         }
@@ -618,7 +643,7 @@ quant_group_fast_kernel(QuantArgs a, int64_t total_groups) {
       __syncthreads();
       const int64_t nvalid = (total_groups - g0) < TG ? (total_groups - g0) : TG;
       const int nchunks = static_cast<int>(nvalid) * CPG;
-      uint8_t* dst = reinterpret_cast<uint8_t*>(a.out) + g0 * RB;
+      uint8_t* dst = reinterpret_cast<uint8_t*>(out.ptr) + g0 * RB;
 #pragma unroll
       for (int k = 0; k < CPG; ++k) {
         const int q = k * TG + t;
@@ -639,7 +664,7 @@ quant_group_fast_kernel(QuantArgs a, int64_t total_groups) {
 // same fast tail.  Coalesced 16-byte loads and 8/16-byte stores; no shared-memory staging needed.
 template <int DT, int MODE, int BITS, int CH>
 __global__ void __launch_bounds__(256, CH == 4 ? 4 : 6)
-quant_row_fast_kernel(QuantArgs a) {
+quant_row_fast_kernel(QuantArgs a, OutDesc out) {
   __shared__ uint32_t smn[8], smx[8];
   const int t = threadIdx.x, lane = t & 31, warp = t >> 5;
   const int chunks = static_cast<int>(a.cols >> 3);
@@ -688,10 +713,7 @@ quant_row_fast_kernel(QuantArgs a) {
     group_range<DT>(mn2, mx2, mn, mx);
     float s, z;
     qparams<DType<DT>>(mn, mx, a.sym, 1, a.qmin, a.qmax, s, z);
-    if (t == 0) {
-      DType<DT>::store(a.scales, r, s);
-      if (!a.sym && a.zeros) DType<DT>::store(a.zeros, r, z);
-    }
+    if (t == 0) store_qparams<DT>(a.scales, a.zeros, a.sym, r, s, z);
     if constexpr (MODE != M_NONE) {
       const Divider<DT> div{s};
       float Ce, vlo, vhi;
@@ -704,11 +726,11 @@ quant_row_fast_kernel(QuantArgs a) {
           uint4 o;
           fast_tail<DT, MODE, BITS>(x[c], div, s, Ce, vlo, vhi, ob, a.sym, o);
           if constexpr (MODE == M_QDQ) {
-            reinterpret_cast<uint4*>(reinterpret_cast<uint16_t*>(a.out) + r * a.ld_out)[ch] = o;
+            reinterpret_cast<uint4*>(reinterpret_cast<uint16_t*>(out.ptr) + r * out.ld)[ch] = o;
           } else if constexpr (MODE == M_PACK && BITS == 4) {
-            (reinterpret_cast<uint32_t*>(a.out) + r * a.packed_cols)[ch] = o.x;
+            (reinterpret_cast<uint32_t*>(out.ptr) + r * out.packed_cols)[ch] = o.x;
           } else {
-            reinterpret_cast<uint2*>(reinterpret_cast<uint8_t*>(a.out) + r * a.cols)[ch] = make_uint2(o.x, o.y);
+            reinterpret_cast<uint2*>(reinterpret_cast<uint8_t*>(out.ptr) + r * a.cols)[ch] = make_uint2(o.x, o.y);
           }
         }
       }
@@ -718,47 +740,45 @@ quant_row_fast_kernel(QuantArgs a) {
   }
 }
 
+// f(MODE, BITS) with the fast kernels' compile-time output mode and field width as
+// std::integral_constant arguments.  BITS is 4 for NONE and QDQ and 8 for CODES8.
+template <class F>
+static auto with_mode_bits(int mode, int bits, F&& f) {
+  using std::integral_constant;
+  if (mode == M_NONE) return f(integral_constant<int, M_NONE>(), integral_constant<int, 4>());
+  if (mode == M_QDQ) return f(integral_constant<int, M_QDQ>(), integral_constant<int, 4>());
+  if (mode == M_CODES8) return f(integral_constant<int, M_CODES8>(), integral_constant<int, 8>());
+  if (bits == 4) return f(integral_constant<int, M_PACK>(), integral_constant<int, 4>());
+  return f(integral_constant<int, M_PACK>(), integral_constant<int, 8>());
+}
+
 template <int DT>
-static int launch_row_fast(const QuantArgs& a, int mode, int bits, cudaStream_t st) {
+static int launch_row_fast(const QuantArgs& a, const OutDesc& o, int mode, int bits, cudaStream_t st) {
   // chunk slots per thread: 2 up to 4096 columns (6 resident CTAs per SM), 4 up to 8192 (4 CTAs)
   const bool small = a.cols <= 4096;
   const int64_t cap = static_cast<int64_t>(kNumSMs) * (small ? 6 : 4);
   const int grid = static_cast<int>(a.rows < cap ? a.rows : cap);
-#define QR_GO(MODE, BITS)                                                              \
-  do {                                                                                 \
-    if (small) quant_row_fast_kernel<DT, MODE, BITS, 2><<<grid, 256, 0, st>>>(a);      \
-    else quant_row_fast_kernel<DT, MODE, BITS, 4><<<grid, 256, 0, st>>>(a);            \
-  } while (0)
-  if (mode == M_NONE) QR_GO(M_NONE, 4);
-  else if (mode == M_QDQ) QR_GO(M_QDQ, 4);
-  else if (mode == M_PACK && bits == 4) QR_GO(M_PACK, 4);
-  else if (mode == M_PACK && bits == 8) QR_GO(M_PACK, 8);
-  else if (mode == M_CODES8) QR_GO(M_CODES8, 8);
-  else return LLMC_EUNSUPPORTED;
-#undef QR_GO
+  auto kern = with_mode_bits(mode, bits, [small](auto m, auto b) {
+    constexpr int MODE = decltype(m)::value, BITS = decltype(b)::value;
+    return small ? &quant_row_fast_kernel<DT, MODE, BITS, 2> : &quant_row_fast_kernel<DT, MODE, BITS, 4>;
+  });
+  kern<<<grid, 256, 0, st>>>(a, o);
   LLMC_CHECK_LAUNCH();
   return LLMC_OK;
 }
 
 template <int DT, int G>
-static int launch_fast(const QuantArgs& a, int mode, int bits, int64_t total_groups, cudaStream_t st) {
+static int launch_fast(const QuantArgs& a, const OutDesc& o, int mode, int bits, int64_t total_groups,
+                       cudaStream_t st) {
   constexpr int smem = 2 * TG * G * 2;
   const int64_t n_tiles = (total_groups + TG - 1) / TG;
   const int64_t cap = static_cast<int64_t>(kNumSMs) * (G == 128 ? 3 : 6);
   const int grid = static_cast<int>(n_tiles < cap ? n_tiles : cap);
-#define QF_GO(MODE, BITS)                                                                          \
-  do {                                                                                             \
-    auto kern = quant_group_fast_kernel<DT, G, MODE, BITS>;                                        \
-    if (int rc = opt_in_smem(kern, smem)) return rc;                                               \
-    kern<<<grid, TG, smem, st>>>(a, total_groups);                                                 \
-  } while (0)
-  if (mode == M_NONE) QF_GO(M_NONE, 4);
-  else if (mode == M_QDQ) QF_GO(M_QDQ, 4);
-  else if (mode == M_PACK && bits == 4) QF_GO(M_PACK, 4);
-  else if (mode == M_PACK && bits == 8) QF_GO(M_PACK, 8);
-  else if (mode == M_CODES8) QF_GO(M_CODES8, 8);
-  else return LLMC_EUNSUPPORTED;
-#undef QF_GO
+  auto kern = with_mode_bits(mode, bits, [](auto m, auto b) {
+    return &quant_group_fast_kernel<DT, G, decltype(m)::value, decltype(b)::value>;
+  });
+  if (int rc = opt_in_smem(kern, smem)) return rc;
+  kern<<<grid, TG, smem, st>>>(a, o, total_groups);
   LLMC_CHECK_LAUNCH();
   return LLMC_OK;
 }
@@ -772,97 +792,33 @@ static bool codes_fit_field(const QuantArgs& a, int bits) {
   return a.qmin >= lo && a.qmax <= hi;
 }
 
-// Which (mode, bits) of the fast kernel serves this call, or -1.
-static int fast_mode(const QuantArgs& a, int dtype) {
-  if (a.ld != a.cols && !(a.ng == 1 && a.ld % 8 == 0)) return -1;      // groups need dense rows
-  if (a.col_scale != nullptr && !((a.group == 64 || a.group == 128) && a.ld == a.cols)) return -1;
-  if (dtype != LLMC_F16 && dtype != LLMC_BF16) return -1;
-  const bool row_kind = a.ng == 1 && a.group == a.cols && a.cols >= 512 && a.cols <= 8192 && a.cols % 8 == 0;
-  if (a.group != 64 && a.group != 128 && !row_kind) return -1;
-  if (a.rows * a.ng >= (1ll << 40)) return -1;
-  if (row_kind && a.out_mode == LLMC_OUT_QDQ && (a.ld_out % 8 != 0)) return -1;
-  switch (a.out_mode) {
-    case LLMC_OUT_NONE: return M_NONE;
-    case LLMC_OUT_QDQ: return (a.out_dtype == dtype && (a.ld_out == a.cols || a.ng == 1)) ? M_QDQ : -1;
-    // asymmetric codes + the +2^(bit-1) storage offset overflow their field and the reference ORs
-    // the overlapping bits (module_utils.py:842-856): fast_tail reproduces that on the packed word
-    case LLMC_OUT_PACK_VLLM: return (a.bit == 4 || a.bit == 8) && codes_fit_field(a, a.bit) ? M_PACK : -1;
-    case LLMC_OUT_CODES_I8:
-    case LLMC_OUT_CODES_U8: return a.bit == 8 && codes_fit_field(a, 8) ? M_CODES8 : -1;
-    default: return -1;
-  }
-}
-
 }  // namespace qf
 
-template <int DT>
-static int launch_dynamic(const QuantArgs& a, bool vec_ok, cudaStream_t st) {
-  const int64_t total_groups = a.rows * a.ng;
-  if (total_groups == 0 || a.cols == 0) return LLMC_OK;
-  if constexpr (DT != LLMC_F32) {
-    const int fm = vec_ok ? qf::fast_mode(a, DT) : -1;
-    if (fm >= 0) {
-      if (a.group == 128 && a.ld == a.cols) return qf::launch_fast<DT, 128>(a, fm, a.bit, total_groups, st);
-      if (a.group == 64 && a.ld == a.cols) return qf::launch_fast<DT, 64>(a, fm, a.bit, total_groups, st);
-      if (a.ng == 1) return qf::launch_row_fast<DT>(a, fm, a.bit, st);
-    }
-  }
-  if (vec_ok && a.group <= 1024) {
-    // 32 elements (4 x 16-byte loads in flight) per lane wherever the group allows it: the
-    // per-group scalar work (qparams: four IEEE divides) is then amortised over 4x more
-    // elements — with 8 elements per lane the kernel was issue-bound at ~1.1 warp-instr/element.
-    const int64_t chunks = a.group >> 3;
-    int lpg = 1;
-    while (lpg * 4 < chunks) lpg *= 2;               // smallest power of two with <= 4 chunks/lane
-    const int ch = static_cast<int>((chunks + lpg - 1) / lpg);
-    if (total_groups >= (1ll << 31)) {
-      set_last_error("quant_dynamic: %lld groups exceed the 2^31 limit", (long long)total_groups);
-      return LLMC_EUNSUPPORTED;
-    }
-    const int64_t warps_needed = (total_groups + (32 / lpg) - 1) / (32 / lpg);
-    int64_t blocks = (warps_needed + 7) / 8;
-    const int64_t cap = static_cast<int64_t>(kNumSMs) * 16;
-    if (blocks > cap) blocks = cap;
-    if (ch == 1) quant_dynamic_warp_kernel<DT, 1><<<(int)blocks, 256, 0, st>>>(a, lpg, total_groups);
-    else if (ch == 2) quant_dynamic_warp_kernel<DT, 2><<<(int)blocks, 256, 0, st>>>(a, lpg, total_groups);
-    else quant_dynamic_warp_kernel<DT, 4><<<(int)blocks, 256, 0, st>>>(a, lpg, total_groups);
-  } else if (vec_ok) {
-    int64_t blocks = total_groups;
-    const int64_t cap = static_cast<int64_t>(kNumSMs) * 32;
-    if (blocks > cap) blocks = cap;
-    quant_dynamic_block_kernel<DT><<<(int)blocks, 256, 0, st>>>(a, total_groups);
-  } else {
-    return LLMC_EUNSUPPORTED;  // caller falls back to qparams_generic + static generic
-  }
-  LLMC_CHECK_LAUNCH();
-  return LLMC_OK;
-}
-
 template <int CT, int WT, int QT>
-static int launch_static_t(const StaticArgs& s, const QuantArgs& e, bool vec_ok, cudaStream_t st) {
-  if (s.rows == 0 || s.cols == 0) return LLMC_OK;
+static int launch_static_t(StaticArgs s, const OutDesc& o, bool vec_ok, cudaStream_t st) {
+  const int64_t cap = static_cast<int64_t>(kNumSMs) * 32;
   if (vec_ok) {
     int64_t total = s.rows * (s.cols >> 3);
     int64_t blocks = (total + 255) / 256;
-    const int64_t cap = static_cast<int64_t>(kNumSMs) * 32;
     if (blocks > cap) blocks = cap;
-    quant_static_vec8_kernel<CT, WT, QT><<<(int)blocks, 256, 0, st>>>(s, e);
+    quant_static_vec8_kernel<CT, WT, QT><<<(int)blocks, 256, 0, st>>>(s, o);
   } else {
+    // a thread per packed word, or per 8 columns
+    s.unit = (o.mode == LLMC_OUT_PACK_VLLM) ? 32 / o.bit : 8;
     int64_t total = s.rows * ((s.cols + s.unit - 1) / s.unit);
     int64_t blocks = (total + 255) / 256;
-    const int64_t cap = static_cast<int64_t>(kNumSMs) * 32;
     if (blocks > cap) blocks = cap;
-    quant_static_kernel<CT, WT, QT><<<(int)blocks, 256, 0, st>>>(s);
+    quant_static_kernel<CT, WT, QT><<<(int)blocks, 256, 0, st>>>(s, o);
   }
   LLMC_CHECK_LAUNCH();
   return LLMC_OK;
 }
 
-static int launch_static(const StaticArgs& s, const QuantArgs& e, int w_dtype, int q_dtype,
+static int launch_static(const StaticArgs& s, const OutDesc& o, int w_dtype, int q_dtype,
                          int round_dtype, bool vec_ok, cudaStream_t st) {
   const int ct = round_dtype >= 0 ? round_dtype : promote(w_dtype, q_dtype);
 #define CASE(CT, WT, QT) \
-  if (ct == CT && w_dtype == WT && q_dtype == QT) return launch_static_t<CT, WT, QT>(s, e, vec_ok, st);
+  if (ct == CT && w_dtype == WT && q_dtype == QT) return launch_static_t<CT, WT, QT>(s, o, vec_ok, st);
   CASE(LLMC_F32, LLMC_F32, LLMC_F32)
   CASE(LLMC_F16, LLMC_F16, LLMC_F16)
   CASE(LLMC_BF16, LLMC_BF16, LLMC_BF16)
@@ -879,20 +835,122 @@ static int launch_static(const StaticArgs& s, const QuantArgs& e, int w_dtype, i
   return LLMC_EUNSUPPORTED;
 }
 
-static int check_out_mode(int out_mode, int bit, const void* out) {
-  if (out_mode < LLMC_OUT_NONE || out_mode > LLMC_OUT_PACK_VLLM) {
-    set_last_error("bad out_mode %d", out_mode);
-    return LLMC_EINVAL;
+// The kernel that serves a llmc_quant_dynamic call.
+struct DynPlan {
+  enum Kernel { kFast128, kFast64, kRow, kWarp, kBlock, kGeneric } kernel;
+  int mode, bits;          // kFast128, kFast64, kRow: qf::M_* and the packed field width
+  int lpg, ch;             // kWarp: lanes per group, 8-element chunks per lane
+};
+
+// plan_dynamic picks it from the validated arguments a and o (w of dtype):
+//
+//   vectorisable  16-bit  fast output  group 128 | 64, ld == cols              quant_group_fast_kernel<G>
+//                                      group == cols: 512..8192 columns, or    quant_row_fast_kernel
+//                                        64 | 128 with ld > cols (padded rows)
+//   vectorisable  any                  group <= 1024 (< 2^31 groups)           quant_dynamic_warp_kernel<CH>
+//                                      group > 1024                            quant_dynamic_block_kernel
+//   otherwise                                                                  qparams_generic_kernel, then
+//                                                                              quant_static_kernel
+//
+// vectorisable: group and ld multiples of 8, w and out 16-byte aligned, a QDQ ld_out multiple of 8,
+// PACK_VLLM at 4 or 8 bits only.  A col_scale needs a vectorisable call and 16-byte alignment
+// (else LLMC_EUNSUPPORTED), and rules out the row kernel.
+// fast output: fewer than 2^40 groups, and out_mode NONE; QDQ in w's dtype with ld_out == cols or
+// one group per row; PACK_VLLM at 4 or 8 bits, CODES_I8 / U8 at 8 bits, whose [qmin, qmax] fits
+// the field (qf::codes_fit_field).
+static int plan_dynamic(const QuantArgs& a, const OutDesc& o, int dtype, DynPlan& p) {
+  const bool vec = (o.mode != LLMC_OUT_PACK_VLLM || o.bit == 4 || o.bit == 8) && a.group % 8 == 0 &&
+                   a.ld % 8 == 0 && aligned16(a.w) && (o.ptr == nullptr || aligned16(o.ptr)) &&
+                   (o.mode != LLMC_OUT_QDQ || o.ld % 8 == 0);
+  if (a.col_scale != nullptr && !(vec && aligned16(a.col_scale))) {
+    set_last_error("quant_dynamic: col_scale needs the vectorised path (group, ld %% 8 == 0, aligned)");
+    return LLMC_EUNSUPPORTED;
   }
-  if (out_mode != LLMC_OUT_NONE && out == nullptr) {
-    set_last_error("out is NULL for out_mode %d", out_mode);
-    return LLMC_EINVAL;
+  p = DynPlan{};
+  if (!vec) {
+    p.kernel = DynPlan::kGeneric;
+    return LLMC_OK;
   }
-  if (bit < 2 || bit > 8) {
-    set_last_error("bit %d outside 2..8", bit);
-    return LLMC_EINVAL;
+  const int64_t total_groups = a.rows * a.ng;
+  int mode = -1, bits = 4;
+  switch (o.mode) {
+    case LLMC_OUT_NONE: mode = qf::M_NONE; break;
+    case LLMC_OUT_QDQ:
+      if (o.dtype == dtype && (o.ld == a.cols || a.ng == 1)) mode = qf::M_QDQ;
+      break;
+    // asymmetric codes + the +2^(bit-1) storage offset overflow their field and the reference ORs
+    // the overlapping bits (module_utils.py:842-856): fast_tail reproduces that on the packed word
+    case LLMC_OUT_PACK_VLLM:
+      if ((o.bit == 4 || o.bit == 8) && qf::codes_fit_field(a, o.bit)) { mode = qf::M_PACK; bits = o.bit; }
+      break;
+    case LLMC_OUT_CODES_I8:
+    case LLMC_OUT_CODES_U8:
+      if (o.bit == 8 && qf::codes_fit_field(a, 8)) { mode = qf::M_CODES8; bits = 8; }
+      break;
+    default: break;
+  }
+  const bool g64_128 = a.group == 64 || a.group == 128;
+  const bool tile = g64_128 && a.ld == a.cols;
+  const bool row = a.ng == 1 && a.col_scale == nullptr && (g64_128 || (a.cols >= 512 && a.cols <= 8192));
+  if (dtype != LLMC_F32 && mode >= 0 && total_groups < (1ll << 40) && (tile || row)) {
+    p.kernel = !tile ? DynPlan::kRow : a.group == 128 ? DynPlan::kFast128 : DynPlan::kFast64;
+    p.mode = mode;
+    p.bits = bits;
+  } else if (a.group <= 1024) {
+    if (total_groups >= (1ll << 31)) {
+      set_last_error("quant_dynamic: %lld groups exceed the 2^31 limit", (long long)total_groups);
+      return LLMC_EUNSUPPORTED;
+    }
+    // 32 elements (4 x 16-byte loads in flight) per lane wherever the group allows it: the
+    // per-group scalar work (qparams: four IEEE divides) is then amortised over 4x more
+    // elements — with 8 elements per lane the kernel was issue-bound at ~1.1 warp-instr/element.
+    const int64_t chunks = a.group >> 3;
+    p.kernel = DynPlan::kWarp;
+    p.lpg = 1;
+    while (p.lpg * 4 < chunks) p.lpg *= 2;           // smallest power of two with <= 4 chunks/lane
+    p.ch = static_cast<int>((chunks + p.lpg - 1) / p.lpg);
+  } else {
+    p.kernel = DynPlan::kBlock;
   }
   return LLMC_OK;
+}
+
+template <int DT>
+static int launch_dynamic(const QuantArgs& a, const OutDesc& o, const DynPlan& p, cudaStream_t st) {
+  const int64_t total_groups = a.rows * a.ng;
+  if constexpr (DT != LLMC_F32) {
+    if (p.kernel == DynPlan::kFast128) return qf::launch_fast<DT, 128>(a, o, p.mode, p.bits, total_groups, st);
+    if (p.kernel == DynPlan::kFast64) return qf::launch_fast<DT, 64>(a, o, p.mode, p.bits, total_groups, st);
+    if (p.kernel == DynPlan::kRow) return qf::launch_row_fast<DT>(a, o, p.mode, p.bits, st);
+  }
+  if (p.kernel == DynPlan::kWarp) {
+    const int64_t warps_needed = (total_groups + (32 / p.lpg) - 1) / (32 / p.lpg);
+    int64_t blocks = (warps_needed + 7) / 8;
+    const int64_t cap = static_cast<int64_t>(kNumSMs) * 16;
+    if (blocks > cap) blocks = cap;
+    if (p.ch == 1) quant_dynamic_warp_kernel<DT, 1><<<(int)blocks, 256, 0, st>>>(a, o, p.lpg, total_groups);
+    else if (p.ch == 2) quant_dynamic_warp_kernel<DT, 2><<<(int)blocks, 256, 0, st>>>(a, o, p.lpg, total_groups);
+    else quant_dynamic_warp_kernel<DT, 4><<<(int)blocks, 256, 0, st>>>(a, o, p.lpg, total_groups);
+    LLMC_CHECK_LAUNCH();
+    return LLMC_OK;
+  }
+  const int64_t cap = static_cast<int64_t>(kNumSMs) * 32;
+  const int blocks = static_cast<int>(total_groups < cap ? total_groups : cap);
+  if (p.kernel == DynPlan::kBlock) {
+    quant_dynamic_block_kernel<DT><<<blocks, 256, 0, st>>>(a, o, total_groups);
+    LLMC_CHECK_LAUNCH();
+    return LLMC_OK;
+  }
+  // generic: qparams, then the scalar static kernel with them
+  qparams_generic_kernel<DT><<<blocks, 256, 0, st>>>(a, total_groups);
+  LLMC_CHECK_LAUNCH();
+  if (o.mode == LLMC_OUT_NONE) return LLMC_OK;
+  StaticArgs s{};
+  s.w = a.w; s.rows = a.rows; s.cols = a.cols; s.ld = a.ld;
+  s.scales = a.scales; s.zeros = a.sym ? nullptr : a.zeros;
+  s.q_row_stride = a.ng; s.group = a.group;
+  s.qmin = a.qmin; s.qmax = a.qmax;
+  return launch_static_t<DT, DT, DT>(s, o, false, st);
 }
 
 }  // namespace llmc
@@ -913,54 +971,21 @@ extern "C" int llmc_quant_dynamic(const void* w, int64_t rows, int64_t cols, int
                  "quant_dynamic: cols %lld not divisible by group %lld", (long long)cols,
                  (long long)group);
   LLMC_CHECK_ARG(sym || zeros, "quant_dynamic: zeros is NULL for asymmetric quantisation");
-  if (int rc = check_out_mode(out_mode, bit, out)) return rc;
-  cudaStream_t st = static_cast<cudaStream_t>(stream);
-
+  OutDesc o;
+  if (int rc = make_out(out_mode, out, ld_out, out_dtype, bit, cols, o)) return rc;
   QuantArgs a{};
   a.w = w; a.rows = rows; a.cols = cols; a.ld = ld;
   a.group = group; a.ng = cols / group;
-  a.sym = sym; a.bit = bit;
+  a.sym = sym;
   if (use_range) { a.qmin = (float)qmin; a.qmax = (float)qmax; }
   else int_range(bit, sym, a.qmin, a.qmax);
   a.scales = scales; a.zeros = zeros; a.col_scale = col_scale;
-  a.out_mode = out_mode; a.out = out;
-  a.ld_out = (out_mode == LLMC_OUT_QDQ) ? (ld_out > 0 ? ld_out : cols) : cols;
-  a.out_dtype = out_dtype;
-  const int pf = 32 / bit;
-  a.packed_cols = (cols + pf - 1) / pf;
-
-  const bool pack_fast = out_mode != LLMC_OUT_PACK_VLLM || bit == 4 || bit == 8;
-  const bool vec_ok = pack_fast && (group % 8 == 0) && (ld % 8 == 0) && aligned16(w) &&
-                      (out == nullptr || aligned16(out)) &&
-                      (out_mode != LLMC_OUT_QDQ || a.ld_out % 8 == 0);
-  if (col_scale != nullptr && !(vec_ok && aligned16(col_scale))) {
-    set_last_error("quant_dynamic: col_scale needs the vectorised path (group, ld %% 8 == 0, aligned)");
-    return LLMC_EUNSUPPORTED;
-  }
-  if (vec_ok) {
-#define CALL(DT) return launch_dynamic<DT>(a, true, st)
-    LLMC_DISPATCH_DT("quant_dynamic", dtype, CALL);
+  DynPlan p;
+  if (int rc = plan_dynamic(a, o, dtype, p)) return rc;
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+#define CALL(DT) return launch_dynamic<DT>(a, o, p, st)
+  LLMC_DISPATCH_DT("quant_dynamic", dtype, CALL);
 #undef CALL
-  }
-  // generic: qparams kernel, then the scalar static kernel
-  {
-    int64_t total_groups = rows * a.ng;
-    int64_t blocks = total_groups < kNumSMs * 32 ? total_groups : kNumSMs * 32;
-#define CALL(DT) qparams_generic_kernel<DT><<<(int)blocks, 256, 0, st>>>(a, total_groups)
-    LLMC_DISPATCH_DT("quant_dynamic", dtype, CALL);
-#undef CALL
-    LLMC_CHECK_LAUNCH();
-  }
-  if (out_mode == LLMC_OUT_NONE) return LLMC_OK;
-  StaticArgs s{};
-  s.w = w; s.rows = rows; s.cols = cols; s.ld = ld;
-  s.scales = scales; s.zeros = sym ? nullptr : zeros;
-  s.q_row_stride = a.ng; s.group = group; s.gmap = nullptr;
-  s.qmin = a.qmin; s.qmax = a.qmax; s.bit = bit;
-  s.out_mode = out_mode; s.out = out; s.ld_out = a.ld_out; s.out_dtype = out_dtype;
-  s.packed_cols = a.packed_cols;
-  s.unit = (out_mode == LLMC_OUT_PACK_VLLM) ? pf : 8;
-  return launch_static(s, a, dtype, dtype, -1, false, st);
 }
 
 extern "C" int llmc_quant_static(const void* w, int64_t rows, int64_t cols, int64_t ld,
@@ -978,31 +1003,20 @@ extern "C" int llmc_quant_static(const void* w, int64_t rows, int64_t cols, int6
   const int zp_inside = (out_mode & LLMC_OUT_FLAG_ZP_INSIDE) ? 1 : 0;
   out_mode &= ~LLMC_OUT_FLAG_ZP_INSIDE;
   LLMC_CHECK_ARG(out_mode != LLMC_OUT_NONE, "quant_static: out_mode NONE makes no sense");
-  if (int rc = check_out_mode(out_mode, bit, out)) return rc;
-  cudaStream_t st = static_cast<cudaStream_t>(stream);
-  const int pf = 32 / bit;
-
+  OutDesc o;
+  if (int rc = make_out(out_mode, out, ld_out, out_dtype, bit, cols, o)) return rc;
   StaticArgs s{};
   s.w = w; s.rows = rows; s.cols = cols; s.ld = ld;
   s.scales = scales; s.zeros = zeros;
   s.q_row_stride = q_row_stride; s.group = group; s.gmap = gmap;
-  s.qmin = (float)qmin; s.qmax = (float)qmax; s.bit = bit;
-  s.out_mode = out_mode; s.out = out;
-  s.ld_out = (out_mode == LLMC_OUT_QDQ) ? (ld_out > 0 ? ld_out : cols) : cols;
-  s.out_dtype = out_dtype;
-  s.packed_cols = (cols + pf - 1) / pf;
-  s.unit = (out_mode == LLMC_OUT_PACK_VLLM) ? pf : 8;
+  s.qmin = (float)qmin; s.qmax = (float)qmax;
   s.zp_inside = zp_inside;
-
-  QuantArgs e{};
-  e.rows = rows; e.cols = cols; e.bit = bit; e.out_mode = out_mode; e.out = out;
-  e.ld_out = s.ld_out; e.out_dtype = out_dtype; e.packed_cols = s.packed_cols;
 
   const bool pack_fast = out_mode != LLMC_OUT_PACK_VLLM || ((bit == 4 || bit == 8) && !gmap);
   const bool vec_ok = pack_fast && (cols % 8 == 0) && (ld % 8 == 0) && aligned16(w) &&
                       aligned16(out) && (gmap || group % 8 == 0) &&
-                      (out_mode != LLMC_OUT_QDQ || s.ld_out % 8 == 0);
-  return launch_static(s, e, w_dtype, q_dtype, round_dtype, vec_ok, st);
+                      (out_mode != LLMC_OUT_QDQ || o.ld % 8 == 0);
+  return launch_static(s, o, w_dtype, q_dtype, round_dtype, vec_ok, static_cast<cudaStream_t>(stream));
 }
 
 extern "C" int llmc_minmax_tensor(const void* w, int64_t n, int dtype, void* mm,
@@ -1015,10 +1029,11 @@ extern "C" int llmc_minmax_tensor(const void* w, int64_t n, int dtype, void* mm,
   if (blocks > 1024) blocks = 1024;
 #define CALL(DT)                                                                \
   minmax_stage1<DT><<<(int)blocks, 256, 0, st>>>(w, n, workspace);              \
-  minmax_stage2<DT><<<1, 256, 0, st>>>(workspace, (int)blocks, mm)
+  LLMC_CHECK_LAUNCH();                                                          \
+  minmax_stage2<DT><<<1, 256, 0, st>>>(workspace, (int)blocks, mm);             \
+  LLMC_CHECK_LAUNCH()
   LLMC_DISPATCH_DT("minmax_tensor", dtype, CALL);
 #undef CALL
-  LLMC_CHECK_LAUNCH();
   return LLMC_OK;
 }
 
@@ -1037,9 +1052,7 @@ pack_vllm_codes_kernel(const CodeT* __restrict__ codes, int64_t rows, int64_t co
     uint32_t word = 0;
     for (int i = 0; i < pf; ++i) {
       const int64_t c = pc * pf + i;
-      if (c < cols)
-        word |= (static_cast<uint32_t>(static_cast<int>(codes[r * cols + c]) + off) & 0xffu)
-                << (bit * i);
+      if (c < cols) word |= vllm_field(static_cast<int>(codes[r * cols + c]), off, bit, i);
     }
     out[u] = static_cast<int32_t>(word);
   }
