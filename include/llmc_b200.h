@@ -222,8 +222,9 @@ int llmc_chol_inv_upper(float* A, int64_t C, void* workspace, int64_t workspace_
  *   llmc_gemm_f32x3:  C[M,N] = (mode 1) or C -= (mode 0)  A * B  with
  *       A(i,k) = a[i*lda + k] (a_mn = 0, K-major)  or  a[k*lda + i] (a_mn = 1, MN-major)
  *       B(j,k) = b[j*ldb + k] (b_mn = 0)           or  b[k*ldb + j] (b_mn = 1)
- *     evaluated as A_hi*B_hi + A_lo*B_hi + A_hi*B_lo on mma.sync tf32 with fp32 register
- *     accumulation; lower_only != 0 restricts the update to tiles touching col <= row.
+ *     evaluated as A_hi*B_hi + A_lo*B_hi + A_hi*B_lo per k8 step with fp32 register
+ *     accumulation, on wgmma tf32 when both operands are K-major and on mma.sync tf32 otherwise
+ *     (the same bits); lower_only != 0 restricts the update to tiles touching col <= row.
  *   These replace the fp32 cuBLAS SGEMMs of gptq.py:244 and the potrf/potri updates of :172-174.
  * ------------------------------------------------------------------------------------ */
 int llmc_split_tf32(const float* x, int64_t rows, int64_t cols, int64_t ld, float* hi,

@@ -26,14 +26,21 @@ reverse_kernel(const float* __restrict__ H, float* __restrict__ G, int64_t n) {
   }
 }
 
-// U[i][j] = j >= i ? Y[n-1-i][n-1-j] : 0
+// U[i][j] = j >= i ? Y[n-1-i][n-1-j] = Z[n-1-j][n-1-i] : 0, for Z = Y^T; 32 x 32 tiles through
+// shared memory, so both the reads of Z and the writes of U are row segments
 __global__ void __launch_bounds__(256)
-reverse_upper_kernel(const float* __restrict__ Y, float* __restrict__ U, int64_t n) {
-  const int64_t total = n * n;
-  for (int64_t idx = static_cast<int64_t>(blockIdx.x) * blockDim.x + threadIdx.x; idx < total;
-       idx += static_cast<int64_t>(gridDim.x) * blockDim.x) {
-    const int64_t i = idx / n, j = idx - i * n;
-    U[idx] = (j >= i) ? Y[total - 1 - idx] : 0.f;
+reverse_upper_kernel(const float* __restrict__ Z, float* __restrict__ U, int64_t n) {
+  __shared__ float tile[32][33];
+  const int tx = threadIdx.x & 31, ty = threadIdx.x >> 5;
+  const int64_t i0 = static_cast<int64_t>(blockIdx.y) * 32, j0 = static_cast<int64_t>(blockIdx.x) * 32;
+  for (int jj = ty; jj < 32; jj += 8) {
+    const int64_t i = i0 + tx, j = j0 + jj;
+    tile[jj][tx] = (i < n && j < n && j >= i) ? Z[(n - 1 - j) * n + (n - 1 - i)] : 0.f;
+  }
+  __syncthreads();
+  for (int ii = ty; ii < 32; ii += 8) {
+    const int64_t i = i0 + ii, j = j0 + tx;
+    if (i < n && j < n) U[i * n + j] = tile[tx][ii];
   }
 }
 
@@ -41,13 +48,15 @@ reverse_upper_kernel(const float* __restrict__ Y, float* __restrict__ U, int64_t
 // 32: 32x32 diagonal sub-blocks are factored in registers (warp shuffles), the sub-panel is solved
 // with one thread per row in registers, the trailing update uses 4x4 register tiles, and L^-1 is
 // built from 32x32 block products (X_ij = -X_ii * sum_k L_ik X_kj).  Rows/cols >= nb are padded
-// with the identity so every loop runs at the full 128.  G block <- L_kk; Y / Yhi / Ylo block <-
-// L_kk^-1 and its tf32 split (ld n).  info[0] = k0 + j + 1 on a non-positive pivot.
+// with the identity so every loop runs at the full 128.  G block <- L_kk; Lhi / Llo block <- the
+// tf32 split of L_kk^-1; Z / Zhi / Zlo block <- L_kk^-T and its split (ld n).  info[0] = k0 + j + 1
+// on a non-positive pivot.
 constexpr int SBK = 32;
 
 __global__ void __launch_bounds__(256, 1)
-diag_kernel(float* __restrict__ G, int64_t n, int64_t k0, int nb, float* __restrict__ Y,
-            float* __restrict__ Yhi, float* __restrict__ Ylo, int* __restrict__ info) {
+diag_kernel(float* __restrict__ G, int64_t n, int64_t k0, int nb, float* __restrict__ Z,
+            float* __restrict__ Zhi, float* __restrict__ Zlo, float* __restrict__ Lhi,
+            float* __restrict__ Llo, int* __restrict__ info) {
   extern __shared__ float sm[];
   float* S = sm;                 // [NB][LDS]
   float* X = sm + NB * LDS;      // [NB][LDS]
@@ -237,17 +246,23 @@ diag_kernel(float* __restrict__ G, int64_t n, int64_t k0, int nb, float* __restr
   }
   for (int idx = tid; idx < NB * NB; idx += 256) {
     const int i = idx >> 7, j = idx & 127;
-    if (i < nb && j <= i) {
-      // L_kk, and the diagonal block of Y = L^-1 with its tf32 split.  The GEMMs that multiply by
-      // L_kk^-1 read it from Yhi/Ylo in place (ld n); the part above the diagonal is zero from
-      // the memsets at the start of llmc_chol_inv_upper.
+    if (i < nb && j < nb) {
+      // L_kk and the tf32 split of X = L_kk^-1 in the diagonal block of Lhi/Llo, where the GEMMs
+      // that multiply by X read it (K-major, ld n), zero above the diagonal; and the diagonal
+      // block of Z = Y^T = L^-T with its tf32 split, (i, j) = X[j][i] for j >= i (the part below
+      // the diagonal is zero from the memsets at the start of llmc_chol_inv_upper).
       const int64_t o = (k0 + i) * n + k0 + j;
-      G[o] = S[i * LDS + j];
-      const float x = X[i * LDS + j];
-      const float2 s = tf32_split(x);
-      Y[o] = x;
-      Yhi[o] = s.x;
-      Ylo[o] = s.y;
+      if (j <= i) G[o] = S[i * LDS + j];
+      const float2 s = tf32_split(j <= i ? X[i * LDS + j] : 0.f);
+      Lhi[o] = s.x;
+      Llo[o] = s.y;
+      if (j >= i) {
+        const float z = X[j * LDS + i];
+        const float2 t = tf32_split(z);
+        Z[o] = z;
+        Zhi[o] = t.x;
+        Zlo[o] = t.y;
+      }
     }
   }
 }
@@ -259,7 +274,7 @@ using namespace llmc;
 
 extern "C" int64_t llmc_chol_workspace_bytes(int64_t C) {
   if (C <= 0) return 0;
-  // G, Lhi, Llo, Y, Yhi, Ylo (C^2 each)
+  // G, Lhi, Llo, Z, Zhi, Zlo (C^2 each)
   return 6 * C * C * 4 + 256;
 }
 
@@ -276,43 +291,47 @@ extern "C" int llmc_chol_inv_upper(float* A, int64_t C, void* workspace, int64_t
   float* G = reinterpret_cast<float*>(workspace);
   float* Lhi = G + nn;
   float* Llo = Lhi + nn;
-  float* Y = Llo + nn;
-  float* Yhi = Y + nn;
-  float* Ylo = Yhi + nn;
-  const SplitMatrix L{Lhi, Llo, n};    // tf32 split of L's sub-diagonal panels
-  const SplitMatrix Ys{Yhi, Ylo, n};   // tf32 split of Y = L^-1
+  float* Z = Llo + nn;
+  float* Zhi = Z + nn;
+  float* Zlo = Zhi + nn;
+  // tf32 split of L's sub-diagonal panels, and of L_kk^-1 in the diagonal blocks
+  const SplitMatrix L{Lhi, Llo, n};
+  // tf32 split of Z = Y^T = L^-T.  The inverse is kept transposed so that every update of it reads
+  // both operands K-major: Y[r0:, 0:r0] -= L[r0:, k] Y[k, 0:r0] is Z[0:r0, r0:] -= Z[0:r0, k] L[r0:, k]^T.
+  const SplitMatrix Zs{Zhi, Zlo, n};
   const int diag_smem = 2 * NB * LDS * 4;
   if (int rc = opt_in_smem(diag_kernel, diag_smem)) return rc;
   // Side streams + events (common.cuh); the call stays asynchronous with respect to the host and
   // ordered on `stream` through the final join.
   SideStreams* side = nullptr;
   if (int rc = side_streams(nbk + 1, &side)) return rc;
-  cudaEvent_t* ev = side->ev[0].data();   // L panel kb and Y_kk final
+  cudaEvent_t* ev = side->ev[0].data();   // L panel kb and L_kk^-1 final
   // super-panel width of the lazy trailing updates: 4 blocks
   constexpr int64_t spw = 4 * NB;
   LLMC_CHECK_CUDA(cudaMemsetAsync(info, 0, sizeof(int), st));
-  LLMC_CHECK_CUDA(cudaMemsetAsync(Y, 0, nn * sizeof(float), st));
-  // the rank-512 inverse update reads Yhi/Ylo over whole super-panel rows: the part above the
-  // diagonal blocks inside each super-panel square is never written, so it must be zero
+  LLMC_CHECK_CUDA(cudaMemsetAsync(Z, 0, nn * sizeof(float), st));
+  // the inverse updates read Zhi/Zlo over whole super-panel columns: the part below the diagonal
+  // (blocks) inside each super-panel square is never written, so it must be zero
   for (int64_t s0 = 0; s0 < n; s0 += spw) {
     const int64_t w = (s0 + spw < n) ? spw : n - s0;
-    LLMC_CHECK_CUDA(cudaMemset2DAsync(Yhi + s0 * n + s0, n * sizeof(float), 0, w * sizeof(float), w, st));
-    LLMC_CHECK_CUDA(cudaMemset2DAsync(Ylo + s0 * n + s0, n * sizeof(float), 0, w * sizeof(float), w, st));
+    LLMC_CHECK_CUDA(cudaMemset2DAsync(Zhi + s0 * n + s0, n * sizeof(float), 0, w * sizeof(float), w, st));
+    LLMC_CHECK_CUDA(cudaMemset2DAsync(Zlo + s0 * n + s0, n * sizeof(float), 0, w * sizeof(float), w, st));
   }
   int64_t blocks = (nn + 255) / 256;
   if (blocks > kNumSMs * 16) blocks = kNumSMs * 16;
   reverse_kernel<<<(int)blocks, 256, 0, st>>>(A, G, n);
   LLMC_CHECK_LAUNCH();
+  const dim3 tiles32(static_cast<unsigned>((n + 31) / 32), static_cast<unsigned>((n + 31) / 32));
 
   auto width = [n](int64_t k0) { return static_cast<int>((n - k0) < NB ? (n - k0) : NB); };
   // Step kb of the factorisation on stream s, once column block kb is up to date: factor and invert
-  // the diagonal block, then the panel below it.  ev[kb] marks L panel kb and Y_kk final.
+  // the diagonal block, then the panel below it.  ev[kb] marks L panel kb and L_kk^-1 final.
   auto factor_block = [&](int64_t kb, cudaStream_t s) -> int {
     const int64_t k0 = kb * NB;
     const int nb = width(k0);
     const int64_t r0 = k0 + nb;
     const int64_t m = n - r0;
-    diag_kernel<<<1, 256, diag_smem, s>>>(G, n, k0, nb, Y, Yhi, Ylo, info);
+    diag_kernel<<<1, 256, diag_smem, s>>>(G, n, k0, nb, Z, Zhi, Zlo, Lhi, Llo, info);
     LLMC_CHECK_LAUNCH();
     if (m > 0) {
       float* P = G + r0 * n + k0;          // panel [m x nb], ld n
@@ -320,23 +339,24 @@ extern "C" int llmc_chol_inv_upper(float* A, int64_t C, void* workspace, int64_t
       if (kb == 0)
         if (int rc = split_tf32(P, m, nb, n, Lhi + r0 * n + k0, Llo + r0 * n + k0, n, s)) return rc;
       // P <- P * L_kk^-T : out[i][j] = sum_k P[i][k] * X[j][k]  (both K-major; X = L_kk^-1 is the
-      // diagonal block of Yhi/Ylo), + split
+      // diagonal block of Lhi/Llo), + split
       if (int rc = tf32x3_update(
-              Tf32x3Update{L.at(r0, k0), Ys.at(k0, k0), P, n, m, nb, nb}.overwrite().split_into(L, r0, k0), s))
+              Tf32x3Update{L.at(r0, k0), L.at(k0, k0), P, n, m, nb, nb}.overwrite().split_into(L, r0, k0), s))
         return rc;
     }
     LLMC_CHECK_CUDA(cudaEventRecord(ev[kb], s));
     return LLMC_OK;
   };
-  // Row step kb of the inverse on stream s, after ev[kb]: Y[k rows, 0:k0] = Y_kk (K-major) * T'
-  // (MN-major: element (col, kk) at T[kk*n + col]); the split of T' was emitted by step kb-1.
+  // Row step kb of the inverse on stream s, after ev[kb]: Y[k rows, 0:k0] = Y_kk T'[k rows, 0:k0],
+  // kept transposed: Z[0:k0, k cols] = T'^T Y_kk^T (T'^T = Z[0:k0, k cols], Y_kk = the diagonal
+  // block of Lhi/Llo, both K-major); the split of T'^T was emitted by step kb-1.
   auto inverse_row = [&](int64_t kb, cudaStream_t s) -> int {
     LLMC_CHECK_CUDA(cudaStreamWaitEvent(s, ev[kb], 0));
     if (kb == 0) return LLMC_OK;
     const int64_t k0 = kb * NB;
     const int nb = width(k0);
     return tf32x3_update(
-        Tf32x3Update{Ys.at(k0, k0), Ys.at_mn(k0, 0), Y + k0 * n, n, nb, k0, nb}.overwrite().split_into(Ys, k0, 0), s);
+        Tf32x3Update{Zs.at(0, k0), L.at(k0, k0), Z + k0, n, k0, nb, nb}.overwrite().split_into(Zs, 0, k0).transpose(), s);
   };
 
   // More than one super-panel: the look-ahead schedule; otherwise the serial schedule below.
@@ -408,34 +428,34 @@ extern "C" int llmc_chol_inv_upper(float* A, int64_t C, void* workspace, int64_t
             return rc;
         }
       }
-      // ---- inverse chain (si): Y = L^-1, one block row per panel ----
+      // ---- inverse chain (si): Y = L^-1 as Z = Y^T, one block column per panel ----
       if (int rc = inverse_row(kb, si)) return rc;
       if (m > 0 && r0 < sp1) {
-        if (int rc = tf32x3_update(Tf32x3Update{L.at(r0, k0), Ys.at_mn(k0, 0), Y + r0 * n, n, sp1 - r0, r0, nb}
-                                       .split_into(Ys, r0, 0).split_first_rows(NB), si))
+        if (int rc = tf32x3_update(Tf32x3Update{Zs.at(0, k0), L.at(r0, k0), Z + r0, n, r0, sp1 - r0, nb}
+                                       .split_into(Zs, 0, r0).split_first_cols(NB).transpose(), si))
           return rc;
       } else if (m > 0) {
-        // T'[sp1:, 0:sp1] -= L[sp1:, sp0:sp1] Y[sp0:sp1, 0:sp1]: the next super-panel's rows on the
-        // chain, the rows beyond on s3 (they are next touched by the following boundary's pieces,
-        // which wait for evIB)
+        // T'[sp1:, 0:sp1] -= L[sp1:, sp0:sp1] Y[sp0:sp1, 0:sp1], as its transpose: the next
+        // super-panel's columns on the chain, the columns beyond on s3 (they are next touched by
+        // the following boundary's pieces, which wait for evIB)
         const int64_t kk = sp1 - sp0;
         const int64_t ra = (sp1 + spw < n) ? sp1 + spw : n;
         if (sidx > 0) LLMC_CHECK_CUDA(cudaStreamWaitEvent(si, evIB[sidx - 1], 0));
-        if (int rc = tf32x3_update(Tf32x3Update{L.at(sp1, sp0), Ys.at_mn(sp0, 0), Y + sp1 * n, n, ra - sp1, sp1, kk}
-                                       .split_into(Ys, sp1, 0).split_first_rows(NB), si))
+        if (int rc = tf32x3_update(Tf32x3Update{Zs.at(0, sp0), L.at(sp1, sp0), Z + sp1, n, sp1, ra - sp1, kk}
+                                       .split_into(Zs, 0, sp1).split_first_cols(NB).transpose(), si))
           return rc;
         LLMC_CHECK_CUDA(cudaEventRecord(evI[sidx], si));
         LLMC_CHECK_CUDA(cudaStreamWaitEvent(s3, evI[sidx], 0));
         if (ra < n) {
-          if (int rc = tf32x3_update(Tf32x3Update{L.at(ra, sp0), Ys.at_mn(sp0, 0), Y + ra * n, n, n - ra, sp1, kk}
-                                         .tile_per_cta(), s3))
+          if (int rc = tf32x3_update(Tf32x3Update{Zs.at(0, sp0), L.at(ra, sp0), Z + ra, n, sp1, n - ra, kk}
+                                         .tile_per_cta().transpose(), s3))
             return rc;
         }
         LLMC_CHECK_CUDA(cudaEventRecord(evIB[sidx], s3));
       }
     }
     if (int rc = side->join(st, {kChain, kBulk, kInverse, kInverseBulk})) return rc;
-    reverse_upper_kernel<<<(int)blocks, 256, 0, st>>>(Y, A, n);
+    reverse_upper_kernel<<<tiles32, 256, 0, st>>>(Z, A, n);
     LLMC_CHECK_LAUNCH();
     return LLMC_OK;
   }
@@ -457,19 +477,21 @@ extern "C" int llmc_chol_inv_upper(float* A, int64_t C, void* workspace, int64_t
         return rc;
     }
 
-    // ---- inverse step kb on the side stream: Y = L^-1 (lower).  T' (stored in Y below the
-    //      diagonal blocks) accumulates -sum_{k<i} L_ik Y_k ;  Y_i = Y_ii T'_i.  It needs panel kb
-    //      of L only, so it overlaps the factorisation's trailing update and later steps. ----
+    // ---- inverse step kb on the side stream: Y = L^-1 (lower), kept as Z = Y^T.  T' (stored in
+    //      Y below the diagonal blocks, in Z above them) accumulates -sum_{k<i} L_ik Y_k ;
+    //      Y_i = Y_ii T'_i.  It needs panel kb of L only, so it overlaps the factorisation's
+    //      trailing update and later steps. ----
     if (int rc = inverse_row(kb, inv)) return rc;
     if (m > 0) {
-      // T'[r0:, 0:r0] -= L[r0:, kblock] * Y[k rows, 0:r0]; emits the split of the next T' rows
-      if (int rc = tf32x3_update(Tf32x3Update{L.at(r0, k0), Ys.at_mn(k0, 0), Y + r0 * n, n, m, r0, nb}
-                                     .split_into(Ys, r0, 0).split_first_rows(NB), inv))
+      // T'[r0:, 0:r0] -= L[r0:, kblock] * Y[k rows, 0:r0] as Z[0:r0, r0:] -= Z[0:r0, k cols] *
+      // L[r0:, kblock]^T; emits the split of the next T' rows (Z columns)
+      if (int rc = tf32x3_update(Tf32x3Update{Zs.at(0, k0), L.at(r0, k0), Z + r0, n, r0, m, nb}
+                                     .split_into(Zs, 0, r0).split_first_cols(NB).transpose(), inv))
         return rc;
     }
   }
   if (int rc = side->join(st, {kBulk})) return rc;
-  reverse_upper_kernel<<<(int)blocks, 256, 0, st>>>(Y, A, n);
+  reverse_upper_kernel<<<tiles32, 256, 0, st>>>(Z, A, n);
   LLMC_CHECK_LAUNCH();
   return LLMC_OK;
 }

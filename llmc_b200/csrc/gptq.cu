@@ -96,7 +96,7 @@ struct InblockArgs {
   const int64_t* out_perm;  // optional: scatter tmp columns back to the original order
   float* losses;         // [R] accumulated
   float* err;            // [128, Rpad] out (Err1 transposed)
-  float* err_hi;         // tf32 split of err
+  float* err_hi;         // tf32 split of Err1, not transposed: row r at err_hi[r * kSuperPanel]
   float* err_lo;
   int64_t Rpad;          // R rounded up to 128
 };
@@ -323,8 +323,9 @@ gptq_inblock_kernel(InblockArgs a) {
   if (live && l == 0) a.losses[row] += loss;
   __syncthreads();
   // write-back: tmp[:, invperm] (gptq.py:186-188) fused as a scatter — permuted column i1+c goes
-  // back to original column perm[i1+c] — and Err1 transposed ([k][row], so the trailing GEMM
-  // reads its A operand with unit stride) with its tf32 split
+  // back to original column perm[i1+c] — Err1 transposed ([k][row], so the SIMT trailing kernel
+  // reads it with unit stride) and its tf32 split row by row (the K-major A operand of the 3xTF32
+  // trailing GEMM)
   for (int rr = warp; rr < IR; rr += (IR * IL) / 32) {
     const int64_t r = r0 + rr;
     if (r >= a.R) break;
@@ -334,11 +335,13 @@ gptq_inblock_kernel(InblockArgs a) {
     }
   }
   if (r0 + lane < a.Rpad) {
-    for (int c = warp; c < GB; c += (IR * IL) / 32) {
-      const float evv = (c < cnt) ? Et[c * EP + lane] : 0.f;
-      const int64_t o = static_cast<int64_t>(c) * a.Rpad + r0 + lane;
-      a.err[o] = evv;
-      const float2 s = tf32_split(evv);                  // for the 3xTF32 trailing GEMM
+    for (int c = warp; c < GB; c += (IR * IL) / 32)
+      a.err[static_cast<int64_t>(c) * a.Rpad + r0 + lane] = (c < cnt) ? Et[c * EP + lane] : 0.f;
+  }
+  for (int rr = warp; rr < IR; rr += (IR * IL) / 32) {
+    for (int c = lane; c < GB; c += 32) {
+      const float2 s = tf32_split((c < cnt) ? Et[c * EP + rr] : 0.f);
+      const int64_t o = (r0 + rr) * kSuperPanel + c;
       a.err_hi[o] = s.x;
       a.err_lo[o] = s.y;
     }
@@ -456,10 +459,12 @@ spqr_inblock_kernel(SpqrArgs a) {
   }
   for (int idx = tid; idx < GB * SR; idx += SR * SL) {
     const int c = idx / SR, r = idx % SR;
-    const float ev = (c < cnt) ? Et[c * SEP + r] : 0.f;
-    const int64_t o = static_cast<int64_t>(c) * a.Rpad + r0 + r;
-    a.err[o] = ev;
-    const float2 s = tf32_split(ev);
+    a.err[static_cast<int64_t>(c) * a.Rpad + r0 + r] = (c < cnt) ? Et[c * SEP + r] : 0.f;
+  }
+  for (int idx = tid; idx < SR * GB; idx += SR * SL) {   // split row by row, as gptq_inblock_kernel
+    const int r = idx >> 7, c = idx & 127;
+    const float2 s = tf32_split((c < cnt) ? Et[c * SEP + r] : 0.f);
+    const int64_t o = (r0 + r) * kSuperPanel + c;
     a.err_hi[o] = s.x;
     a.err_lo[o] = s.y;
   }
@@ -576,12 +581,12 @@ static int sweep_schedule(float* W, const float* Hinv, int64_t R, int64_t C, int
                           bool wide_dynamic_group, void* workspace, cudaStream_t st, F&& launch_inblock) {
   if (int rc = opt_in_smem(trailing_update_kernel, kTrailingSmem)) return rc;
   const int64_t Rpad = ((R + GB - 1) / GB) * GB;
-  // [512][Rpad] x {err, hi, lo}, two sets selected by the parity of the super-panel
+  // {err [512][Rpad], hi, lo [Rpad][512]}, two sets selected by the parity of the super-panel
   float* const err_set[2] = {reinterpret_cast<float*>(workspace),
                              reinterpret_cast<float*>(workspace) + 3 * kSuperPanel * Rpad};
   float* Hh = err_set[1] + 3 * kSuperPanel * Rpad;
   float* Hl = Hh + C * C;
-  const SplitMatrix Hs{Hh, Hl, C};    // tf32 split of Hinv
+  const SplitMatrix Hts{Hh, Hl, C};   // tf32 split of Hinv^T
   // trailing updates on tensor cores (3xTF32) when the shapes allow TMA; fp32 SIMT otherwise.
   // LLMC_B200_SIMT_TRAILING=1 forces the fp32 CUDA-core kernel everywhere: a second summation
   // order for scripts/check_spqr_summation_order.py, whose measurements PARITY.md records.
@@ -589,7 +594,7 @@ static int sweep_schedule(float* W, const float* Hinv, int64_t R, int64_t C, int
   const bool tensor_trailing = !force_simt && (C % 8 == 0) && aligned16(W) && aligned16(Hinv) &&
                                aligned16(workspace);
   if (tensor_trailing && C > GB) {
-    if (int rc = split_tf32(Hinv, C, C, C, Hh, Hl, C, st)) return rc;
+    if (int rc = split_tf32_transposed(Hinv, C, C, C, Hh, Hl, C, st)) return rc;
   }
   // super-panel width: 512 on the tensor path, one block (the reference's schedule) otherwise
   // (a dynamic group is searched on W[:, start : start+group] at its first column, so a group
@@ -630,17 +635,17 @@ static int sweep_schedule(float* W, const float* Hinv, int64_t R, int64_t C, int
     const int64_t sp1 = (sp0 + sp_width < C) ? sp0 + sp_width : C;
     const int par = static_cast<int>((i1 / sp_width) & 1);
     float* err_base = err_set[par];
-    // the tf32 split of the super-panel's errors, row j - sp0 for column j
-    const SplitMatrix E{err_base + kSuperPanel * Rpad, err_base + 2 * kSuperPanel * Rpad, Rpad};
+    // the tf32 split of the super-panel's errors, column j - sp0 for column j
+    const SplitMatrix E{err_base + kSuperPanel * Rpad, err_base + 2 * kSuperPanel * Rpad, kSuperPanel};
     const int b_i1 = static_cast<int>(i1);
     const int b_count = static_cast<int>(i2 - i1);
     float* const b_err = err_base + (i1 - sp0) * Rpad;
-    if (int rc = launch_inblock(b_i1, b_count, b_err, E.hi + (i1 - sp0) * Rpad, E.lo + (i1 - sp0) * Rpad, chain))
+    if (int rc = launch_inblock(b_i1, b_count, b_err, E.hi + (i1 - sp0), E.lo + (i1 - sp0), chain))
       return rc;
     // W[:, n0:n1] -= Err1[:, k0:k1] @ Hinv[k0:k1, n0:n1]   (gptq.py:244) for columns k0..k1 of this
-    // super-panel: A = Err1^T (MN-major, ld Rpad), B = Hinv rows (MN-major, ld C)
+    // super-panel: A = Err1 (K-major, ld 512), B = Hinv^T rows (K-major, ld C)
     auto trailing = [&](int64_t k0, int64_t k1, int64_t n0, int64_t n1) {
-      return Tf32x3Update{E.at_mn(k0 - sp0, 0), Hs.at_mn(k0, n0), W + n0, C, R, n1 - n0, k1 - k0};
+      return Tf32x3Update{E.at(0, k0 - sp0), Hts.at(n0, k0), W + n0, C, R, n1 - n0, k1 - k0};
     };
     if (i2 < C && tensor_trailing) {
       // Inside the super-panel: this block's errors onto the super-panel's remaining columns; at its
@@ -678,9 +683,9 @@ static int sweep_schedule(float* W, const float* Hinv, int64_t R, int64_t C, int
 }
 
 extern "C" int64_t llmc_gptq_workspace_bytes(int64_t R, int64_t C) {
-  // Err1^T + its tf32 split for TWO super-panels ([512, Rpad] x 3 each: the bulk trailing update
-  // of panel p reads its errors while the chain of panel p+1 writes the other set) and the tf32
-  // split of Hinv ([C, C] x 2)
+  // Err1^T + the tf32 split of Err1 for TWO super-panels (512 x Rpad x 3 each: the bulk trailing
+  // update of panel p reads its errors while the chain of panel p+1 writes the other set) and the
+  // tf32 split of Hinv^T ([C, C] x 2)
   const int64_t rpad = ((R + GB - 1) / GB) * GB;
   return (6 * kSuperPanel * rpad + 2 * C * C) * 4;
 }

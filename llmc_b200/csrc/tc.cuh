@@ -220,6 +220,23 @@ __device__ __forceinline__ void wgmma_m64n128k32_e4m3(float (&d)[64], uint64_t a
       : "l"(adesc), "l"(bdesc), "r"(accumulate));
 }
 
+// D[64 x 128] += A[64 x 8] * B[128 x 8]^T on tf32 operands, issued by one warpgroup.  tf32 operands
+// are read K-major only (no transpose immediates); fragment layout as above.  Always accumulates:
+// the 3xTF32 update (tf32.cu) starts from zeroed accumulators, so an exact-zero sum keeps the
+// sign 0.f + ... gives it.
+__device__ __forceinline__ void wgmma_m64n128k8_tf32(float (&d)[64], uint64_t adesc, uint64_t bdesc) {
+  asm volatile(
+      "{\n"
+      ".reg .pred p;\n"
+      "setp.ne.b32 p, 1, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n128k8.f32.tf32.tf32 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, "
+      "%64, %65, p, 1, 1;\n"
+      "}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+      : "l"(adesc), "l"(bdesc));
+}
+
 template <bool kBf16, int kTransA, int kTransB>
 __device__ __forceinline__ void wgmma_m64n128k16(float (&d)[64], uint64_t adesc, uint64_t bdesc,
                                                  uint32_t accumulate) {
@@ -349,17 +366,14 @@ struct SplitOperand {
   int64_t ld;
   bool mn;
 };
-// An fp32 matrix held as its tf32 split with row stride ld.  at / at_mn: the operand whose element
-// (i, k) is the matrix element (row + i, col + k) / (row + k, col + i).
+// An fp32 matrix held as its tf32 split with row stride ld.  at: the K-major operand whose element
+// (i, k) is the matrix element (row + i, col + k).
 struct SplitMatrix {
   float* hi;
   float* lo;
   int64_t ld;
   SplitOperand at(int64_t row, int64_t col) const {
     return {hi + row * ld + col, lo + row * ld + col, ld, false};
-  }
-  SplitOperand at_mn(int64_t row, int64_t col) const {
-    return {hi + row * ld + col, lo + row * ld + col, ld, true};
   }
 };
 // C[i][j] -= sum_k A(i, k) B(j, k) for i < M, j < N, k < K; C has row stride ldc.  The optional
@@ -376,8 +390,13 @@ struct Tf32x3Update {
   int64_t split_rows = INT64_MAX;   //   split_rows or column < split_cols; hi == nullptr: none
   int64_t split_cols = INT64_MAX;
   bool one_tile_per_cta = false;    // grid = tile count (see tf32x3_update)
+  bool transposed = false;          // C holds the transpose of the updated matrix (see transpose())
 
   Tf32x3Update& overwrite() { assign = true; return *this; }
+  // C^T -= B A^T written as C -= A B^T: the cross terms are issued as A_hi*B_lo, then A_lo*B_hi,
+  // the order C^T's own update would issue them in, so either form gives the same bits.
+  // K-major operands only.
+  Tf32x3Update& transpose() { transposed = true; return *this; }
   Tf32x3Update& lower_tiles(int64_t row0, int64_t col0) {
     lower = true; row_off = row0; col_off = col0; return *this;
   }
@@ -393,5 +412,8 @@ struct Tf32x3Update {
 int tf32x3_update(const Tf32x3Update& u, cudaStream_t st);
 int split_tf32(const float* x, int64_t rows, int64_t cols, int64_t ld, float* hi, float* lo,
                int64_t ld_out, cudaStream_t st);
+// the split of x^T: hi/lo[c * ld_out + r] for x[r * ld + c]
+int split_tf32_transposed(const float* x, int64_t rows, int64_t cols, int64_t ld, float* hi, float* lo,
+                          int64_t ld_out, cudaStream_t st);
 
 }  // namespace llmc

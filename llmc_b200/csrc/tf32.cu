@@ -14,12 +14,16 @@
 // Operand layouts (per operand flag):
 //   K-major : element (i, k) at base[i*ld + k]   (rows = M or N index, K contiguous)
 //   MN-major: element (i, k) at base[k*ld + i]   (rows = K index, M or N contiguous)
-// The GPTQ weight update has BOTH operands MN-major, which Hopper's wgmma cannot read for tf32
-// (tf32 wgmma operands must be K-major), so the MMAs are warp-level mma.sync m16n8k8 whose
-// fragments are gathered from shared memory in either layout.
-// Structure: one TMA producer warp fills a 3-stage tc::Ring of 128B-swizzled tiles (mbarrier
-// transaction counts); eight MMA warps (2 x 4, 64 x 32 each) compute a 128 x 128 tile with fp32
-// register accumulators and write it back with the fused epilogue.
+// Hopper's tf32 wgmma reads K-major operands only.  Every caller in the library holds both
+// operands K-major (the sweep keeps the split of Err1 and of Hinv^T, the Cholesky inverse keeps
+// L^-T), and those calls run on tf32x3_wgmma_kernel.  A call with an MN-major operand (possible
+// through llmc_gemm_f32x3 only) runs on tf32x3_kernel, whose warp-level mma.sync m16n8k8 gathers
+// its fragments from shared memory in either layout.  Both issue the same three terms per k8
+// step in the same order and give the same bits.
+// Structure: one TMA producer thread fills a 3-stage tc::Ring of 128B-swizzled tiles (mbarrier
+// transaction counts); two consumer warpgroups (wgmma) or eight MMA warps (mma.sync, 2 x 4 of
+// 64 x 32) compute a 128 x 128 tile with fp32 register accumulators and write it back with the
+// shared epilogue, store_result.
 #include "tc.cuh"
 
 namespace llmc {
@@ -181,6 +185,47 @@ __device__ __forceinline__ void mma_tf32(float (&d)[4], const uint32_t (&a)[4], 
       "{%8, %9}, {%0, %1, %2, %3};"
       : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
       : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b[0]), "r"(b[1]));
+}
+
+// Stores the result pair (v0, v1) of C[row][col], C[row][col + 1] (the second only if col + 1 < N),
+// and its tf32 split where asked.  mode 0 and not `folded`: v0, v1 are the products and are
+// subtracted from C here; otherwise they are the final values.
+__device__ __forceinline__ void store_result(const Params& p, int64_t row, int64_t col, float v0,
+                                             float v1, bool folded) {
+  const bool pair = col + 1 < p.N;
+  float* cp = p.C + row * p.ldc + col;
+  const bool vec = pair && (reinterpret_cast<uintptr_t>(cp) & 7) == 0;
+  if (p.mode == 0 && !folded) {
+    if (vec) {
+      const float2 o = *reinterpret_cast<const float2*>(cp);
+      v0 = o.x - v0;
+      v1 = o.y - v1;
+    } else {
+      v0 = cp[0] - v0;
+      if (pair) v1 = cp[1] - v1;
+    }
+  }
+  if (vec) *reinterpret_cast<float2*>(cp) = make_float2(v0, v1);
+  else {
+    cp[0] = v0;
+    if (pair) cp[1] = v1;
+  }
+  if (p.Chi != nullptr && (row < p.split_rows || col < p.split_cols)) {
+    float* hp = p.Chi + row * p.ldc + col;
+    float* lp = p.Clo + row * p.ldc + col;
+    const float2 s0 = tf32_split(v0), s1 = tf32_split(v1);
+    if (vec && ((reinterpret_cast<uintptr_t>(hp) | reinterpret_cast<uintptr_t>(lp)) & 7) == 0) {
+      *reinterpret_cast<float2*>(hp) = make_float2(s0.x, s1.x);
+      *reinterpret_cast<float2*>(lp) = make_float2(s0.y, s1.y);
+    } else {
+      hp[0] = s0.x;
+      lp[0] = s0.y;
+      if (pair) {
+        hp[1] = s1.x;
+        lp[1] = s1.y;
+      }
+    }
+  }
 }
 
 template <bool kAmn, bool kBmn>
@@ -345,42 +390,150 @@ tf32x3_kernel(const __grid_constant__ CUtensorMap tmAhi, const __grid_constant__
         for (int nt = 0; nt < 4; ++nt) {
           const int64_t col = col0 + nt * 8 + 2 * t;
           if (col >= p.N) continue;
-          const bool pair = col + 1 < p.N;
-          float* cp = p.C + row * p.ldc + col;
-          const bool vec = pair && (reinterpret_cast<uintptr_t>(cp) & 7) == 0;
-          float v0 = acc[mt][nt][2 * i], v1 = acc[mt][nt][2 * i + 1];
-          if (p.mode == 0 && !folded) {
-            if (vec) {
-              const float2 o = *reinterpret_cast<const float2*>(cp);
-              v0 = o.x - v0;
-              v1 = o.y - v1;
-            } else {
-              v0 = cp[0] - v0;
-              if (pair) v1 = cp[1] - v1;
-            }
-          }
-          if (vec) *reinterpret_cast<float2*>(cp) = make_float2(v0, v1);
-          else {
-            cp[0] = v0;
-            if (pair) cp[1] = v1;
-          }
-          if (p.Chi != nullptr && (row < p.split_rows || col < p.split_cols)) {
-            float* hp = p.Chi + row * p.ldc + col;
-            float* lp = p.Clo + row * p.ldc + col;
-            const float2 s0 = tf32_split(v0), s1 = tf32_split(v1);
-            if (vec && ((reinterpret_cast<uintptr_t>(hp) | reinterpret_cast<uintptr_t>(lp)) & 7) == 0) {
-              *reinterpret_cast<float2*>(hp) = make_float2(s0.x, s1.x);
-              *reinterpret_cast<float2*>(lp) = make_float2(s0.y, s1.y);
-            } else {
-              hp[0] = s0.x;
-              lp[0] = s0.y;
-              if (pair) {
-                hp[1] = s1.x;
-                lp[1] = s1.y;
-              }
-            }
-          }
+          store_result(p, row, col, acc[mt][nt][2 * i], acc[mt][nt][2 * i + 1], folded);
         }
+      }
+    }
+  }
+}
+
+// ---- K-major x K-major: wgmma ---------------------------------------------------------------
+// Warpgroup 0 is the TMA producer (one thread), warpgroups 1 and 2 each own 64 rows x 128 columns
+// of the 128 x 128 tile and issue wgmma m64n128k8 straight from the swizzled ring: a 32-float
+// row is one 128-byte swizzle span, so k8 step s is +32 bytes in the descriptor.  Per k8 step
+// three wgmmas into one zeroed accumulator, hi*hi, lo*hi, hi*lo (kSwap: hi*hi, hi*lo, lo*hi, see
+// Tf32x3Update::transpose), k ascending: the order of tf32x3_kernel's mma.sync.  A consumer keeps
+// one wgmma group in flight and frees a stage once the group that read it has retired.
+constexpr int kWgThreads = 384;
+
+template <bool kSwap>
+__global__ void __launch_bounds__(kWgThreads, 1)
+tf32x3_wgmma_kernel(const __grid_constant__ CUtensorMap tmAhi, const __grid_constant__ CUtensorMap tmAlo,
+                    const __grid_constant__ CUtensorMap tmBhi, const __grid_constant__ CUtensorMap tmBlo,
+                    const Params p) {
+  extern __shared__ __align__(1024) uint8_t smem_raw[];
+  uint8_t* smem = ring_base(smem_raw);
+  const Ring<kStages> ring(smem + kStages * kStageBytes);
+  const int wg = threadIdx.x >> 7, tid = threadIdx.x & 127;
+  const int kb_total = (p.K + BK - 1) / BK;
+
+  if (threadIdx.x == 0) {
+    prefetch_tmap(&tmAhi); prefetch_tmap(&tmAlo); prefetch_tmap(&tmBhi); prefetch_tmap(&tmBlo);
+    ring.init(1, 2);                  // empty: one arrive per consumer warpgroup
+    fence_barrier_init();
+  }
+  __syncthreads();
+
+  if (wg == 0) {
+    // ===================== TMA producer =====================
+    if (tid == 0) {
+      PipeState<kStages> ps;
+      for (int u = blockIdx.x; u < p.num_units; u += gridDim.x) {
+        int m_blk, n_blk;
+        decode(p, u, m_blk, n_blk);
+        for (int kb = 0; kb < kb_total; ++kb) {
+          ring.wait_empty(ps);
+          uint8_t* ahi = smem + ps.stage * kStageBytes;
+          uint64_t* bar = &ring.full[ps.stage];
+          ring.expect_tx(ps, kStageBytes);
+          tma_load_2d(ahi, &tmAhi, bar, kb * BK, m_blk * BM);
+          tma_load_2d(ahi + kABytes, &tmAlo, bar, kb * BK, m_blk * BM);
+          tma_load_2d(ahi + 2 * kABytes, &tmBhi, bar, kb * BK, n_blk * BN);
+          tma_load_2d(ahi + 2 * kABytes + kBBytes, &tmBlo, bar, kb * BK, n_blk * BN);
+          ps.advance();
+        }
+      }
+    }
+    return;
+  }
+
+  // ===================== consumers: warpgroup c owns rows 64 c .. 64 c + 63 =====================
+  const int c = wg - 1;
+  const int lane = tid & 31, g = lane >> 2, t = lane & 3;
+  PipeState<kStages> ps;
+  for (int u = blockIdx.x; u < p.num_units; u += gridDim.x) {
+    int m_blk, n_blk;
+    decode(p, u, m_blk, n_blk);
+    const int64_t row0 = static_cast<int64_t>(m_blk) * BM + c * 64;
+    const int64_t col0 = static_cast<int64_t>(n_blk) * BN;
+    if (p.mode == 0) {
+      // pull this warpgroup's 64 x 128 block of C into L2 while the MMAs run: per row four
+      // 32-column segments, the first and last column of each (a segment spans at most two lines)
+#pragma unroll
+      for (int r = 0; r < 2; ++r) {
+        const int q = 2 * tid + r;                // (row, segment) = (q / 4, q % 4)
+        const int64_t row = row0 + (q >> 2), c0 = col0 + 32 * (q & 3);
+        if (row < p.M && c0 < p.N) {
+          const int64_t last = (c0 + 31 < p.N ? c0 + 31 : p.N - 1);
+          prefetch_l2(p.C + row * p.ldc + c0);
+          prefetch_l2(p.C + row * p.ldc + last);
+        }
+      }
+    }
+    float acc[64];
+#pragma unroll
+    for (int i = 0; i < 64; ++i) acc[i] = 0.f;
+    int prev = -1;
+    for (int kb = 0; kb < kb_total; ++kb) {
+      ring.wait_full(ps);
+      wgmma_fence();
+      const uint32_t ahi = smem_u32(smem + ps.stage * kStageBytes) + c * 64 * 128, alo = ahi + kABytes;
+      const uint32_t bhi = smem_u32(smem + ps.stage * kStageBytes) + 2 * kABytes, blo = bhi + kBBytes;
+#pragma unroll
+      for (int s = 0; s < BK / 8; ++s) {
+        const uint64_t dah = make_smem_desc(ahi + s * 32, 16, 1024), dal = make_smem_desc(alo + s * 32, 16, 1024);
+        const uint64_t dbh = make_smem_desc(bhi + s * 32, 16, 1024), dbl = make_smem_desc(blo + s * 32, 16, 1024);
+        wgmma_m64n128k8_tf32(acc, dah, dbh);
+        if constexpr (!kSwap) {
+          wgmma_m64n128k8_tf32(acc, dal, dbh);
+          wgmma_m64n128k8_tf32(acc, dah, dbl);
+        } else {
+          wgmma_m64n128k8_tf32(acc, dah, dbl);
+          wgmma_m64n128k8_tf32(acc, dal, dbh);
+        }
+      }
+      wgmma_commit();
+      wgmma_wait<1>();                           // the group that read stage `prev` has retired
+      if (prev >= 0 && tid == 0) ring.release(prev);
+      prev = ps.stage;
+      ps.advance();
+    }
+    wgmma_wait<0>();
+    fence_acc(acc);
+    if (prev >= 0 && tid == 0) ring.release(prev);
+
+    // ---- epilogue: acc[4 j + 2 i + e] = C[row 16 w + g + 8 i][col 8 j + 2 t + e] ----
+    // As in tf32x3_kernel: a block inside C with 8-byte aligned pairs is read whole before the
+    // first store and folded into the accumulators; ragged or misaligned blocks read each pair
+    // right before its store.
+    const int64_t rw = row0 + 16 * (tid >> 5) + g;
+    const bool folded = p.mode == 0 && row0 + 64 <= p.M && col0 + BN <= p.N && (p.ldc & 1) == 0 &&
+                        (reinterpret_cast<uintptr_t>(p.C) & 7) == 0;
+    if (folded) {
+      float2 old[16][2];
+#pragma unroll
+      for (int i = 0; i < 2; ++i) {
+        const float* cp = p.C + (rw + 8 * i) * p.ldc + col0 + 2 * t;
+#pragma unroll
+        for (int j = 0; j < 16; ++j) old[j][i] = *reinterpret_cast<const float2*>(cp + 8 * j);
+      }
+#pragma unroll
+      for (int j = 0; j < 16; ++j)
+#pragma unroll
+        for (int i = 0; i < 2; ++i) {
+          acc[4 * j + 2 * i] = old[j][i].x - acc[4 * j + 2 * i];
+          acc[4 * j + 2 * i + 1] = old[j][i].y - acc[4 * j + 2 * i + 1];
+        }
+    }
+#pragma unroll
+    for (int i = 0; i < 2; ++i) {
+      const int64_t row = rw + 8 * i;
+      if (row >= p.M) continue;
+#pragma unroll
+      for (int j = 0; j < 16; ++j) {
+        const int64_t col = col0 + 8 * j + 2 * t;
+        if (col >= p.N) continue;
+        store_result(p, row, col, acc[4 * j + 2 * i], acc[4 * j + 2 * i + 1], folded);
       }
     }
   }
@@ -397,6 +550,25 @@ split_tf32_kernel(const float* __restrict__ x, int64_t rows, int64_t cols, int64
     hi[r * ld_out + c] = s.x;
     lo[r * ld_out + c] = s.y;
   }
+}
+
+// hi/lo[c * ld_out + r] = tf32_split(x[r * ld + c]): 32 x 32 tiles through shared memory, so
+// both the reads and the writes are row segments
+__global__ void __launch_bounds__(256)
+split_tf32_t_kernel(const float* __restrict__ x, int64_t rows, int64_t cols, int64_t ld,
+                    float* __restrict__ hi, float* __restrict__ lo, int64_t ld_out) {
+  __shared__ float tile[32][33];
+  const int tx = threadIdx.x & 31, ty = threadIdx.x >> 5;
+  const int64_t r0 = static_cast<int64_t>(blockIdx.y) * 32, c0 = static_cast<int64_t>(blockIdx.x) * 32;
+  for (int i = ty; i < 32; i += 8)
+    if (r0 + i < rows && c0 + tx < cols) tile[i][tx] = x[(r0 + i) * ld + c0 + tx];
+  __syncthreads();
+  for (int i = ty; i < 32; i += 8)
+    if (c0 + i < cols && r0 + tx < rows) {
+      const float2 s = tf32_split(tile[tx][i]);
+      hi[(c0 + i) * ld_out + r0 + tx] = s.x;
+      lo[(c0 + i) * ld_out + r0 + tx] = s.y;
+    }
 }
 
 }  // namespace t3
@@ -418,6 +590,10 @@ int tf32x3_update(const Tf32x3Update& u, cudaStream_t st) {
   }
   if (u.c_split.hi != nullptr && u.c_split.ld != u.ldc) {
     set_last_error("tf32x3_update: the split of the result must have the result's ld");
+    return LLMC_EINVAL;
+  }
+  if (u.transposed && (u.a.mn || u.b.mn)) {
+    set_last_error("tf32x3_update: a transposed update needs K-major operands");
     return LLMC_EINVAL;
   }
   // both halves of an operand with `rows` M or N indices: K-major boxes are box_rows x BK,
@@ -457,10 +633,13 @@ int tf32x3_update(const Tf32x3Update& u, cudaStream_t st) {
     p.num_units = static_cast<int>(units);
   }
   if (p.num_units == 0) return LLMC_OK;
-  const auto kern = !u.a.mn ? (!u.b.mn ? tf32x3_kernel<false, false> : tf32x3_kernel<false, true>)
+  const Units units{p.num_units, u.one_tile_per_cta};
+  if (!u.a.mn && !u.b.mn)
+    return launch_persistent(u.transposed ? tf32x3_wgmma_kernel<true> : tf32x3_wgmma_kernel<false>, units,
+                             kWgThreads, kSmemBytes, st, ta[0], ta[1], tb[0], tb[1], p);
+  const auto kern = !u.a.mn ? tf32x3_kernel<false, true>
                             : (!u.b.mn ? tf32x3_kernel<true, false> : tf32x3_kernel<true, true>);
-  return launch_persistent(kern, {p.num_units, u.one_tile_per_cta}, kThreads, kSmemBytes, st, ta[0],
-                           ta[1], tb[0], tb[1], p);
+  return launch_persistent(kern, units, kThreads, kSmemBytes, st, ta[0], ta[1], tb[0], tb[1], p);
 }
 
 int split_tf32(const float* x, int64_t rows, int64_t cols, int64_t ld, float* hi, float* lo,
@@ -469,6 +648,15 @@ int split_tf32(const float* x, int64_t rows, int64_t cols, int64_t ld, float* hi
   int64_t blocks = (rows * cols + 255) / 256;
   if (blocks > kNumSMs * 16) blocks = kNumSMs * 16;
   t3::split_tf32_kernel<<<(int)blocks, 256, 0, st>>>(x, rows, cols, ld, hi, lo, ld_out);
+  LLMC_CHECK_LAUNCH();
+  return LLMC_OK;
+}
+
+int split_tf32_transposed(const float* x, int64_t rows, int64_t cols, int64_t ld, float* hi, float* lo,
+                          int64_t ld_out, cudaStream_t st) {
+  if (rows <= 0 || cols <= 0) return LLMC_OK;
+  const dim3 grid(static_cast<unsigned>((cols + 31) / 32), static_cast<unsigned>((rows + 31) / 32));
+  t3::split_tf32_t_kernel<<<grid, 256, 0, st>>>(x, rows, cols, ld, hi, lo, ld_out);
   LLMC_CHECK_LAUNCH();
   return LLMC_OK;
 }

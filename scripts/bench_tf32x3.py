@@ -10,7 +10,7 @@ bytes of C read and written (8 per computed element).  Operands are compact (ld 
 the workload reads them out of larger matrices, which TMA loads in the same 128-byte rows.
 
 With several --lib, each shape is timed with every library in turn (alternating, same inputs),
-and the outputs of one seeded call are compared bit for bit across the libraries.  The card name
+and the outputs of one seeded call per mode are compared bit for bit across the libraries.  The card name
 and power limit are printed with the numbers.
 """
 import argparse
@@ -35,14 +35,15 @@ SHAPES = [
     ('chol14336 factor chain K=128', 7168, 128, 128, 0, 0, 0),       # G[k0:, k0:k0+128], k0 = 7168
     ('chol14336 factor chain K=256', 7168, 128, 256, 0, 0, 0),
     ('chol14336 factor chain K=384', 7168, 128, 384, 0, 0, 0),
-    ('chol14336 inverse bulk', 7168, 7168, 512, 0, 1, 0),            # L[sp1:, ..] x Y[sp0:sp1, 0:sp1]
-    ('sweep 4096x14336 bulk', 4096, 13312, 512, 1, 1, 0),
-    ('sweep 4096x14336 bulk', 4096, 6656, 512, 1, 1, 0),
-    ('sweep 4096x14336 chain', 4096, 512, 512, 1, 1, 0),
-    ('sweep 4096x14336 in-panel', 4096, 384, 128, 1, 1, 0),
-    ('sweep 28672x4096 bulk', 28672, 3072, 512, 1, 1, 0),
-    ('sweep 28672x4096 chain', 28672, 512, 512, 1, 1, 0),
-    ('sweep 28672x4096 in-panel', 28672, 384, 128, 1, 1, 0),
+    ('chol14336 inverse bulk', 7168, 7168, 512, 0, 0, 0),            # Z[0:sp1, sp0:sp1] x L[sp1:, ..]
+    ('chol14336 inverse chain', 7168, 128, 128, 0, 0, 0),            # Z[0:k0, k-block] x Y_kk
+    ('sweep 4096x14336 bulk', 4096, 13312, 512, 0, 0, 0),             # Err1 x Hinv^T[n0:, k-block]
+    ('sweep 4096x14336 bulk', 4096, 6656, 512, 0, 0, 0),
+    ('sweep 4096x14336 chain', 4096, 512, 512, 0, 0, 0),
+    ('sweep 4096x14336 in-panel', 4096, 384, 128, 0, 0, 0),
+    ('sweep 28672x4096 bulk', 28672, 3072, 512, 0, 0, 0),
+    ('sweep 28672x4096 chain', 28672, 512, 512, 0, 0, 0),
+    ('sweep 28672x4096 in-panel', 28672, 384, 128, 0, 0, 0),
 ]
 
 
@@ -130,14 +131,17 @@ def main():
         tiles = lower_tiles(M, N) if lower else None
         elems = tiles * BM * BN if lower else M * N
         flop = 2.0 * elems * K
-        # one seeded call per library from the same C, compared bit for bit
-        outs = []
-        for lib in libs:
-            c = case.c0.clone()
-            case.call(lib, c)
-            outs.append(c)
-        same = all(torch.equal(outs[0], o) for o in outs[1:])
-        del outs
+        # one seeded call per library and mode (0: C -= AB from the same C, 1: C = AB), compared
+        # bit for bit
+        same = True
+        for mode in (0, 1):
+            outs = []
+            for lib in libs:
+                c = case.c0.clone()
+                case.call(lib, c, mode)
+                outs.append(c)
+            same = same and all(torch.equal(outs[0], o) for o in outs[1:])
+            del outs
         t1 = time_call(case, libs[0], 1)
         reps = max(5, min(200, int(0.15 / max(t1 * 1e-3, 1e-6))))
         ms = [[] for _ in libs]
