@@ -29,7 +29,7 @@
 extern "C" {
 #endif
 
-#define LLMC_B200_ABI_VERSION 1
+#define LLMC_B200_ABI_VERSION 2
 
 /* dtypes */
 enum { LLMC_F32 = 0, LLMC_F16 = 1, LLMC_BF16 = 2 };
@@ -220,19 +220,17 @@ int llmc_chol_inv_upper(float* A, int64_t C, void* workspace, int64_t workspace_
  * fp32-accurate tensor-core GEMM building block ("3xTF32", csrc/tf32.cu) used by K4 and K5:
  *   llmc_split_tf32:  hi = tf32(x), lo = tf32(x - hi)            (x, hi, lo: [rows, cols], ld)
  *   llmc_gemm_f32x3:  C[M,N] = (mode 1) or C -= (mode 0)  A * B  with
- *       A(i,k) = a[i*lda + k] (a_mn = 0, K-major)  or  a[k*lda + i] (a_mn = 1, MN-major)
- *       B(j,k) = b[j*ldb + k] (b_mn = 0)           or  b[k*ldb + j] (b_mn = 1)
+ *       A(i,k) = a[i*lda + k],  B(j,k) = b[j*ldb + k]     (both K-major)
  *     evaluated as A_hi*B_hi + A_lo*B_hi + A_hi*B_lo per k8 step with fp32 register
- *     accumulation, on wgmma tf32 when both operands are K-major and on mma.sync tf32 otherwise
- *     (the same bits); lower_only != 0 restricts the update to tiles touching col <= row.
+ *     accumulation on wgmma tf32; lower_only != 0 restricts the update to tiles touching
+ *     col <= row.
  *   These replace the fp32 cuBLAS SGEMMs of gptq.py:244 and the potrf/potri updates of :172-174.
  * ------------------------------------------------------------------------------------ */
 int llmc_split_tf32(const float* x, int64_t rows, int64_t cols, int64_t ld, float* hi,
                     float* lo, void* stream);
-int llmc_gemm_f32x3(const float* a_hi, const float* a_lo, int a_mn, int64_t lda,
-                    const float* b_hi, const float* b_lo, int b_mn, int64_t ldb, float* c,
-                    int64_t ldc, int64_t M, int64_t N, int64_t K, int mode, int lower_only,
-                    void* stream);
+int llmc_gemm_f32x3(const float* a_hi, const float* a_lo, int64_t lda, const float* b_hi,
+                    const float* b_lo, int64_t ldb, float* c, int64_t ldc, int64_t M, int64_t N,
+                    int64_t K, int mode, int lower_only, void* stream);
 
 /* ------------------------------------------------------------------------------------
  * K5  llmc_gptq_colblock — replaces GPTQ.weight_transform (gptq.py:198-244) incl.

@@ -55,8 +55,8 @@ SIGNATURES = {
     'llmc_chol_workspace_bytes': (c_i64, [c_i64]),
     'llmc_chol_inv_upper': (c_int, [c_vp, c_i64, c_vp, c_i64, c_vp, c_vp]),
     'llmc_split_tf32': (c_int, [c_vp, c_i64, c_i64, c_i64, c_vp, c_vp, c_vp]),
-    'llmc_gemm_f32x3': (c_int, [c_vp, c_vp, c_int, c_i64, c_vp, c_vp, c_int, c_i64, c_vp, c_i64,
-                                c_i64, c_i64, c_i64, c_int, c_int, c_vp]),
+    'llmc_gemm_f32x3': (c_int, [c_vp, c_vp, c_i64, c_vp, c_vp, c_i64, c_vp, c_i64, c_i64, c_i64,
+                                c_i64, c_int, c_int, c_vp]),
     'llmc_gptq_workspace_bytes': (c_i64, [c_i64, c_i64]),
     'llmc_gptq_colblock': (c_int, [c_vp, c_vp, c_i64, c_i64, c_i64, c_int, c_int, c_int, c_vp,
                                    c_vp, c_vp, c_int, c_vp, c_vp, c_vp, c_vp, c_i64, c_vp]),

@@ -358,13 +358,12 @@ __device__ __forceinline__ float2 tf32_split(float x) {
   const float hi = tf32_rna(x);
   return make_float2(hi, tf32_rna(x - hi));
 }
-// A GEMM operand held as its tf32 split: element (i, k) at [i * ld + k] (K-major) or, mn = true,
-// at [k * ld + i] (MN-major); i indexes M (operand A) or N (operand B).
+// A GEMM operand held as its tf32 split, K-major: element (i, k) at [i * ld + k]; i indexes M
+// (operand A) or N (operand B).
 struct SplitOperand {
   const float* hi;
   const float* lo;
   int64_t ld;
-  bool mn;
 };
 // An fp32 matrix held as its tf32 split with row stride ld.  at: the K-major operand whose element
 // (i, k) is the matrix element (row + i, col + k).
@@ -373,7 +372,7 @@ struct SplitMatrix {
   float* lo;
   int64_t ld;
   SplitOperand at(int64_t row, int64_t col) const {
-    return {hi + row * ld + col, lo + row * ld + col, ld, false};
+    return {hi + row * ld + col, lo + row * ld + col, ld};
   }
 };
 // C[i][j] -= sum_k A(i, k) B(j, k) for i < M, j < N, k < K; C has row stride ldc.  The optional
@@ -395,7 +394,6 @@ struct Tf32x3Update {
   Tf32x3Update& overwrite() { assign = true; return *this; }
   // C^T -= B A^T written as C -= A B^T: the cross terms are issued as A_hi*B_lo, then A_lo*B_hi,
   // the order C^T's own update would issue them in, so either form gives the same bits.
-  // K-major operands only.
   Tf32x3Update& transpose() { transposed = true; return *this; }
   Tf32x3Update& lower_tiles(int64_t row0, int64_t col0) {
     lower = true; row_off = row0; col_off = col0; return *this;

@@ -28,22 +28,22 @@ from llmc_b200 import _lib  # noqa: E402
 
 BM = BN = 128
 
-# (name, M, N, K, a_mn, b_mn, lower_only); see chol.cu (look-ahead schedule) and gptq.cu (sweep)
+# (name, M, N, K, lower_only); see chol.cu (look-ahead schedule) and gptq.cu (sweep)
 SHAPES = [
-    ('chol14336 factor bulk (lower)', 13824, 13824, 512, 0, 0, 1),   # L[sp1:, sp0:sp1] twice, sp1 = 512
-    ('chol14336 factor bulk (lower)', 7168, 7168, 512, 0, 0, 1),     # sp1 = 7168
-    ('chol14336 factor chain K=128', 7168, 128, 128, 0, 0, 0),       # G[k0:, k0:k0+128], k0 = 7168
-    ('chol14336 factor chain K=256', 7168, 128, 256, 0, 0, 0),
-    ('chol14336 factor chain K=384', 7168, 128, 384, 0, 0, 0),
-    ('chol14336 inverse bulk', 7168, 7168, 512, 0, 0, 0),            # Z[0:sp1, sp0:sp1] x L[sp1:, ..]
-    ('chol14336 inverse chain', 7168, 128, 128, 0, 0, 0),            # Z[0:k0, k-block] x Y_kk
-    ('sweep 4096x14336 bulk', 4096, 13312, 512, 0, 0, 0),             # Err1 x Hinv^T[n0:, k-block]
-    ('sweep 4096x14336 bulk', 4096, 6656, 512, 0, 0, 0),
-    ('sweep 4096x14336 chain', 4096, 512, 512, 0, 0, 0),
-    ('sweep 4096x14336 in-panel', 4096, 384, 128, 0, 0, 0),
-    ('sweep 28672x4096 bulk', 28672, 3072, 512, 0, 0, 0),
-    ('sweep 28672x4096 chain', 28672, 512, 512, 0, 0, 0),
-    ('sweep 28672x4096 in-panel', 28672, 384, 128, 0, 0, 0),
+    ('chol14336 factor bulk (lower)', 13824, 13824, 512, 1),   # L[sp1:, sp0:sp1] twice, sp1 = 512
+    ('chol14336 factor bulk (lower)', 7168, 7168, 512, 1),     # sp1 = 7168
+    ('chol14336 factor chain K=128', 7168, 128, 128, 0),       # G[k0:, k0:k0+128], k0 = 7168
+    ('chol14336 factor chain K=256', 7168, 128, 256, 0),
+    ('chol14336 factor chain K=384', 7168, 128, 384, 0),
+    ('chol14336 inverse bulk', 7168, 7168, 512, 0),            # Z[0:sp1, sp0:sp1] x L[sp1:, ..]
+    ('chol14336 inverse chain', 7168, 128, 128, 0),            # Z[0:k0, k-block] x Y_kk
+    ('sweep 4096x14336 bulk', 4096, 13312, 512, 0),             # Err1 x Hinv^T[n0:, k-block]
+    ('sweep 4096x14336 bulk', 4096, 6656, 512, 0),
+    ('sweep 4096x14336 chain', 4096, 512, 512, 0),
+    ('sweep 4096x14336 in-panel', 4096, 384, 128, 0),
+    ('sweep 28672x4096 bulk', 28672, 3072, 512, 0),
+    ('sweep 28672x4096 chain', 28672, 512, 512, 0),
+    ('sweep 28672x4096 in-panel', 28672, 384, 128, 0),
 ]
 
 
@@ -74,26 +74,24 @@ class Case:
     which matches tf32_split only approximately: timing and cross-library equality need inputs,
     not a particular split."""
 
-    def __init__(self, M, N, K, a_mn, b_mn, lower, seed=0):
+    def __init__(self, M, N, K, lower, seed=0):
         g = torch.Generator(device='cuda').manual_seed(seed)
         def split(shape):
             x = torch.randn(*shape, device='cuda', generator=g)
             hi = (x.view(torch.int32) & ~0x1fff).view(torch.float32)
             return hi.contiguous(), (x - hi).contiguous()
-        self.a = split((K, M) if a_mn else (M, K))
-        self.b = split((K, N) if b_mn else (N, K))
-        self.lda = M if a_mn else K
-        self.ldb = N if b_mn else K
+        self.a = split((M, K))
+        self.b = split((N, K))
         self.c0 = torch.randn(M, N, device='cuda', generator=g)
         self.c = self.c0.clone()
-        self.M, self.N, self.K, self.a_mn, self.b_mn, self.lower = M, N, K, a_mn, b_mn, lower
+        self.M, self.N, self.K, self.lower = M, N, K, lower
 
     def call(self, lib, c=None, mode=0):
         c = self.c if c is None else c
         st = ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)
         p = _lib.ptr
-        rc = lib.llmc_gemm_f32x3(p(self.a[0]), p(self.a[1]), self.a_mn, self.lda, p(self.b[0]), p(self.b[1]),
-                                 self.b_mn, self.ldb, p(c), self.N, self.M, self.N, self.K, mode, self.lower, st)
+        rc = lib.llmc_gemm_f32x3(p(self.a[0]), p(self.a[1]), self.K, p(self.b[0]), p(self.b[1]), self.K,
+                                 p(c), self.N, self.M, self.N, self.K, mode, self.lower, st)
         if rc != 0:
             raise RuntimeError('llmc_gemm_f32x3: %s' % lib.llmc_b200_last_error().decode())
 
@@ -126,8 +124,8 @@ def main():
     for i, p in enumerate(paths):
         print(f'# lib{i}: {p}')
     rows = []
-    for sname, M, N, K, a_mn, b_mn, lower in SHAPES:
-        case = Case(M, N, K, a_mn, b_mn, lower)
+    for sname, M, N, K, lower in SHAPES:
+        case = Case(M, N, K, lower)
         tiles = lower_tiles(M, N) if lower else None
         elems = tiles * BM * BN if lower else M * N
         flop = 2.0 * elems * K
@@ -148,7 +146,7 @@ def main():
         for _ in range(args.rounds):
             for i, lib in enumerate(libs):
                 ms[i].append(time_call(case, lib, reps))
-        row = {'shape': sname, 'M': M, 'N': N, 'K': K, 'a_mn': a_mn, 'b_mn': b_mn, 'lower': lower,
+        row = {'shape': sname, 'M': M, 'N': N, 'K': K, 'lower': lower,
                'c_rmw_bytes': 8 * elems, 'reps': reps, 'bitwise_equal': same,
                'ms': [min(m) for m in ms], 'ms_max': [max(m) for m in ms],
                'tflops_fp32eq': [flop / min(m) / 1e9 for m in ms]}

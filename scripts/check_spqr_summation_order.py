@@ -2,7 +2,7 @@
 lands from the reference when only floating-point summation orders change.
 
 The same inputs (tests/golden/e2e_spqr_llama.pt) go through the pipeline four ways:
-  wgmma          the library as shipped (wgmma GEMM / SYRK, mma.sync 3xTF32 trailing update)
+  wgmma          the library as shipped (wgmma GEMM / SYRK, wgmma 3xTF32 trailing update)
   wgmma+simt     the same, trailing update on the fp32 CUDA-core kernel (LLMC_B200_SIMT_TRAILING=1)
   cublas         forwards through torch F.linear (cuBLAS), Hessians as torch fp32 X^T X
   cublas+simt    both substitutions

@@ -269,10 +269,10 @@ if 'prof' in only:
     ops.hessian_add_batch(Hs, 0, torch.randn(1, 8192, 4096, device='cuda').bfloat16())
     Hs += 0.01 * torch.diag(Hs).mean() * torch.eye(4096, device='cuda')
     for _ in range(2):
-        ops.chol_inv_upper(Hs)                                 # tf32x3_kernel, diag_kernel
+        ops.chol_inv_upper(Hs)                                 # tf32x3_wgmma_kernel, diag_kernel
     Wp, Hp = ops.prepare(w, Hs, None, 0.0)
     Hinv = ops.chol_inv_upper(Hp)
-    ops.weight_transform(Wp, Hinv, 4, False, 128)              # gptq_inblock_kernel, tf32x3 (MN/MN)
+    ops.weight_transform(Wp, Hinv, 4, False, 128)              # gptq_inblock_kernel, tf32x3_wgmma_kernel
     torch.cuda.synchronize()
 
 if 'cholq' in only:

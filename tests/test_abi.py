@@ -37,7 +37,7 @@ def test_signature_table_matches_header():
 
 def test_version_and_error_strings(lib):
     lib.llmc_b200_abi_version.restype = ctypes.c_int
-    assert lib.llmc_b200_abi_version() == 1
+    assert lib.llmc_b200_abi_version() == 2
     lib.llmc_b200_error_string.restype = ctypes.c_char_p
     assert lib.llmc_b200_error_string(0) == b'ok'
     assert b'invalid' in lib.llmc_b200_error_string(-1)
@@ -85,14 +85,14 @@ def test_error_behaviour_of_the_solver_and_gemm_entry_points():
     assert 'must divide K=100' in last()
     assert lib.llmc_gemm_w4a16(p, p, p, null, 1, null, p, 128, 256, 128, 128, 2, null) == -1
     assert 'qparam_dtype' in last()
-    assert lib.llmc_gemm_f32x3(p, p, 0, 128, p, p, 0, 128, p, 128, 128, 128, 100, 0, 0, null) == -1
-    assert lib.llmc_gemm_f32x3(p, p, 0, 128, p, p, 0, 128, p, 128, 128, 128, 128, 3, 0, null) == -1
+    assert lib.llmc_gemm_f32x3(p, p, 128, p, p, 128, p, 128, 128, 128, 100, 0, 0, null) == -1
+    assert lib.llmc_gemm_f32x3(p, p, 128, p, p, 128, p, 128, 128, 128, 128, 3, 0, null) == -1
     assert 'mode must be 0' in last()
     assert lib.llmc_b200_error_string(-1).decode() == 'invalid argument'
     # workspace sizing is pure arithmetic: 6 C^2 floats; (3*512*Rpad + 2 C^2) floats
     assert lib.llmc_chol_workspace_bytes(4096) == 6 * 4096 ** 2 * 4 + 256
     assert lib.llmc_gptq_workspace_bytes(4000, 4096) == (6 * 512 * 4096 + 2 * 4096 ** 2) * 4
-    assert lib.llmc_b200_abi_version() == 1
+    assert lib.llmc_b200_abi_version() == 2
 
 
 def test_product_does_not_import_oracle():

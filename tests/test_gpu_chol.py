@@ -1,60 +1,11 @@
-"""GPU: the 3xTF32 tensor-core GEMM block and the blocked Cholesky-inverse built on it.
-Floating point, tolerances stated: fp32-level for the GEMM (3xTF32 drops ~2^-22), 1e-3
-relative on Hinv_U (north_star) — measured far tighter."""
+"""GPU: the blocked Cholesky inverse, built on the 3xTF32 update (tested in test_gpu_tf32x3.py).
+Floating point, tolerance stated: 1e-3 relative on Hinv_U (north_star) — measured far tighter."""
 import ctypes
 
 import pytest
 import torch
 
 pytestmark = pytest.mark.gpu
-
-
-def _split(x):
-    from llmc_b200._lib import call, ptr, stream_ptr
-    hi, lo = torch.empty_like(x), torch.empty_like(x)
-    call('llmc_split_tf32', ptr(x), x.shape[0], x.shape[1], x.shape[1], ptr(hi), ptr(lo),
-         stream_ptr(x.device))
-    return hi, lo
-
-
-def _gemm(a, a_mn, b, b_mn, c, M, N, K, mode, lower=0):
-    from llmc_b200._lib import call, ptr, stream_ptr
-    ah, al = _split(a)
-    bh, bl = _split(b)
-    call('llmc_gemm_f32x3', ptr(ah), ptr(al), a_mn, a.shape[1], ptr(bh), ptr(bl), b_mn, b.shape[1],
-         ptr(c), c.shape[1], M, N, K, mode, lower, stream_ptr(c.device))
-
-
-@pytest.mark.parametrize('a_mn,b_mn', [(0, 0), (0, 1), (1, 0), (1, 1)])
-@pytest.mark.parametrize('M,N,K', [(128, 256, 32), (384, 512, 128), (1000, 776, 128), (4096, 2048, 64)])
-def test_f32x3_all_layouts(a_mn, b_mn, M, N, K):
-    torch.manual_seed(M + N + K + a_mn * 2 + b_mn)
-    A = torch.randn(M, K, device='cuda')
-    B = torch.randn(N, K, device='cuda')
-    a = A.t().contiguous() if a_mn else A
-    b = B.t().contiguous() if b_mn else B
-    C0 = torch.randn(M, N, device='cuda')
-    ref = A.double() @ B.double().t()
-    c = C0.clone()
-    _gemm(a, a_mn, b, b_mn, c, M, N, K, mode=1)
-    err = (c.double() - ref).abs().max().item()
-    assert err <= 2e-6 * K ** 0.5 * ref.abs().max().item() + 1e-6, err
-    c = C0.clone()
-    _gemm(a, a_mn, b, b_mn, c, M, N, K, mode=0)
-    err = (c.double() - (C0.double() - ref)).abs().max().item()
-    assert err <= 2e-6 * K ** 0.5 * ref.abs().max().item() + 1e-6, err
-
-
-def test_f32x3_exact_on_integers_and_lower_only():
-    M = N = 512
-    K = 128
-    A = torch.randint(-8, 9, (M, K), device='cuda').float()
-    C0 = torch.zeros(M, N, device='cuda')
-    c = C0.clone()
-    _gemm(A, 0, A, 0, c, M, N, K, mode=0, lower=1)
-    ref = -(A @ A.t())
-    low = torch.tril(torch.ones(M, N, device='cuda', dtype=torch.bool))
-    assert torch.equal(c[low], ref[low]), 'lower triangle must be exact on small integers'
 
 
 @pytest.mark.parametrize('C', [128, 256, 512, 1024, 4096, 1096])
