@@ -138,7 +138,8 @@ int llmc_minmax_tensor(const void* w, int64_t n, int dtype, void* mm, float* wor
  *     [rows] fp32.  The reference's aliasing of the running range (:165, an improvement shrinks
  *     the base of all later levels) is reproduced.
  *   llmc_histc — torch.histc(x.float(), bins, min=lo, max=hi) for the static histogram observer
- *     (get_static_hist_range, quant.py:462-522): hist [bins] fp32 counts.
+ *     (get_static_hist_range, quant.py:462-522): hist [bins] fp32 counts, each the exact count
+ *     rounded once (deterministic beyond 2^24 per bin); n < 2^32.
  * ------------------------------------------------------------------------------------ */
 int llmc_mse_range(const void* w, int64_t rows, int64_t cols, int dtype, int sym, int qmin,
                    int qmax, int steps, float grid, float norm, float* min_out, float* max_out,

@@ -88,6 +88,7 @@ def scaled_fake_quant(wquantizer, weight, scales):
 
 
 # ---- AutoClipper (auto_clip.py) -----------------------------------------------------------------------
+CLIP_MAX_GROUP = 128          # llmc_awq_clip holds a group in one warp, 4 weights per lane
 class AutoClipper:
     def __init__(self, w_only, wquantizer, aquantizer, clip_version, clip_sym, save_clip,
                  padding_mask):
@@ -99,6 +100,11 @@ class AutoClipper:
             raise NotImplementedError('clip_version v2 (learnable bound factors, auto_clip.py:212-256)')
         if not w_only:
             raise NotImplementedError('auto-clip with activation fake-quant (auto_clip.py:276-281)')
+        if wquantizer.granularity != 'per_group' or wquantizer.group_size > CLIP_MAX_GROUP:
+            # refused here, before the block loop, rather than by llmc_awq_clip at the first layer
+            raise NotImplementedError(
+                f'auto-clip of groups wider than {CLIP_MAX_GROUP} (granularity '
+                f'{wquantizer.granularity}, group_size {getattr(wquantizer, "group_size", None)})')
 
     @torch.no_grad()
     def run(self, block, block_idx, input_feat, n_sample_token):

@@ -99,7 +99,7 @@ mse_stage1(const void* __restrict__ a, const void* __restrict__ b, int64_t n, fl
 }
 
 __global__ void __launch_bounds__(256)
-mse_stage2(const float* __restrict__ ws, int nblocks, double inv_n, float* __restrict__ out) {
+mse_stage2(const float* __restrict__ ws, int nblocks, double n, float* __restrict__ out) {
   __shared__ double red[8];
   double acc = 0.0;
   for (int i = threadIdx.x; i < nblocks; i += blockDim.x) acc += static_cast<double>(ws[i]);
@@ -109,7 +109,9 @@ mse_stage2(const float* __restrict__ ws, int nblocks, double inv_n, float* __res
   if (threadIdx.x == 0) {
     double t = 0.0;
     for (int i = 0; i < 8; ++i) t += red[i];
-    out[0] = static_cast<float>(t * inv_n);
+    // t / n rounded to double and then to fp32 is t / n rounded once to fp32 (53 >= 2 * 24 + 2);
+    // t * (1 / n) would round three times
+    out[0] = static_cast<float>(t / n);
   }
 }
 
@@ -127,7 +129,7 @@ struct ClipArgs {
   const void* x;        // [ns_total, C] sampled tokens
   int64_t R, C;
   int group, ng;
-  int tok0, ntok;       // token chunk [tok0, tok0 + ntok), ntok <= 512
+  int tok0, ntok;       // token chunk [tok0, tok0 + ntok), ntok <= kClipMaxTok
   int sym, bit, clip_sym;
   float qmin, qmax;
   float* err;           // [R, ng, 10] fp32 sums over tokens (accumulated across chunks)
@@ -314,7 +316,7 @@ extern "C" int llmc_mse(const void* a, const void* b, int64_t n, int dtype, floa
 #define CALL(DT) mse_stage1<DT><<<(int)blocks, 256, 0, st>>>(a, b, n, workspace); LLMC_CHECK_LAUNCH()
   LLMC_DISPATCH_DT("mse", dtype, CALL);
 #undef CALL
-  mse_stage2<<<1, 256, 0, st>>>(workspace, (int)blocks, 1.0 / static_cast<double>(n), out);
+  mse_stage2<<<1, 256, 0, st>>>(workspace, (int)blocks, static_cast<double>(n), out);
   LLMC_CHECK_LAUNCH();
   return LLMC_OK;
 }

@@ -7,7 +7,7 @@
 //                   kernels over the whole weight).
 //   llmc_histc      torch.histc for the static histogram observer (quant.py:462-522): counts of
 //                   fp32(x) in `bins` equal bins over [lo, hi] (x == hi -> last bin, values outside
-//                   are ignored).
+//                   are ignored), counted exactly in 32-bit integers and rounded once to fp32.
 //
 // The reference evaluates the mse search on `tensor.float()`: fp32 arithmetic throughout.  One
 // quirk is preserved on purpose (SURVEY App. E style): `best_min_val, best_max_val = _min_val,
@@ -85,7 +85,8 @@ mse_range_kernel(const void* __restrict__ w, int64_t rows, int64_t cols, int sym
       for (int64_t c = tid; c < cols; c += kThreads) {
         const float x = cached ? cache[c] : DType<DT>::load(w, base + c);
         const float q = fminf(fmaxf(rintf(x / s) + z, qmin), qmax);       // quant.py:699-708
-        const float d = fabsf((q - z) * s - x);                          // dequant, q_tensor -= x
+        // dequant (q - z) * s, then q_tensor -= x: two roundings, never one FMA
+        const float d = fabsf(fsub_rn(fmul_rn(fsub_rn(q, z), s), x));
         err += powf(d, norm);
       }
       err = warp_sum(err);
@@ -109,7 +110,7 @@ mse_range_kernel(const void* __restrict__ w, int64_t rows, int64_t cols, int sym
 template <int DT>
 __global__ void __launch_bounds__(256)
 histc_kernel(const void* __restrict__ x, int64_t n, float lo, float hi, int bins,
-             float* __restrict__ hist) {
+             unsigned int* __restrict__ counts) {
   extern __shared__ unsigned int local[];
   for (int b = threadIdx.x; b < bins; b += blockDim.x) local[b] = 0u;
   __syncthreads();
@@ -125,8 +126,18 @@ histc_kernel(const void* __restrict__ x, int64_t n, float lo, float hi, int bins
     }
   }
   __syncthreads();
+  // exact integer totals (n < 2^32): an fp32 sum of the blocks' counts would round, in completion
+  // order, once a bin passes 2^24
   for (int b = threadIdx.x; b < bins; b += blockDim.x)
-    if (local[b]) atomicAdd(&hist[b], static_cast<float>(local[b]));
+    if (local[b]) atomicAdd(&counts[b], local[b]);
+}
+
+// hist holds the uint32 totals bit for bit; replace each by the count rounded once to fp32, like
+// torch.histc's
+__global__ void __launch_bounds__(256)
+histc_finish_kernel(float* __restrict__ hist, int bins) {
+  const int b = blockIdx.x * blockDim.x + threadIdx.x;
+  if (b < bins) hist[b] = __uint2float_rn(__float_as_uint(hist[b]));
 }
 
 }  // namespace rg
@@ -156,18 +167,22 @@ extern "C" int llmc_mse_range(const void* w, int64_t rows, int64_t cols, int dty
 
 extern "C" int llmc_histc(const void* x, int64_t n, int dtype, int bins, float lo, float hi,
                           float* hist, void* stream) {
-  LLMC_CHECK_ARG(x && hist && n >= 0 && bins > 0 && bins <= 8192, "histc: bad argument");
+  LLMC_CHECK_ARG((x || n == 0) && hist && n >= 0 && bins > 0 && bins <= 8192, "histc: bad argument");
+  LLMC_CHECK_ARG(n <= 0xffffffffll, "histc: n = %lld exceeds the 32-bit bin counts", (long long)n);
   LLMC_CHECK_ARG(hi >= lo, "histc: max < min");
   cudaStream_t st = static_cast<cudaStream_t>(stream);
-  LLMC_CHECK_CUDA(cudaMemsetAsync(hist, 0, bins * sizeof(float), st));
+  LLMC_CHECK_CUDA(cudaMemsetAsync(hist, 0, bins * sizeof(float), st));   // 0.0f == 0u
   if (n == 0) return LLMC_OK;
   if (hi == lo) { lo -= 1.f; hi += 1.f; }                   // torch.histc's degenerate-range rule
   int64_t blocks = (n + 255) / 256;
   if (blocks > kNumSMs * 8) blocks = kNumSMs * 8;
   const int smem = bins * 4;
-#define CALL(DT) rg::histc_kernel<DT><<<(int)blocks, 256, smem, st>>>(x, n, lo, hi, bins, hist)
+  unsigned int* counts = reinterpret_cast<unsigned int*>(hist);   // counted in place, then converted
+#define CALL(DT) rg::histc_kernel<DT><<<(int)blocks, 256, smem, st>>>(x, n, lo, hi, bins, counts)
   LLMC_DISPATCH_DT("histc", dtype, CALL);
 #undef CALL
+  LLMC_CHECK_LAUNCH();
+  rg::histc_finish_kernel<<<(bins + 255) / 256, 256, 0, st>>>(hist, bins);
   LLMC_CHECK_LAUNCH();
   return LLMC_OK;
 }

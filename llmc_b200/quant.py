@@ -142,6 +142,10 @@ class BaseQuantizer(object):
         if self.granularity in ('per_tensor', 'per_block') or tensor.dim() != 2:
             raise NotImplementedError('mse range is built for row-wise ranges (per_channel / per_group '
                                       '/ per_head / per_token), the granularities the shipped YAMLs use')
+        if not self.sym and not self.round_zp:
+            # the reference then searches with the unrounded zero-point inside the rounding
+            # (quant.py:557-558, 702-705); llmc_mse_range adds a rounded one after it
+            raise NotImplementedError('calib_algo: mse with round_zp: False')
         require_cuda(tensor)
         t = tensor if tensor.is_contiguous() else tensor.contiguous()
         rows, cols = t.shape

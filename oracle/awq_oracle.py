@@ -75,14 +75,13 @@ def auto_clip_layer(w, x, bit, sym, granularity, group_size, clip_sym=True, n_gr
     w [R, C]; x [..., C].  Returns (best_max [R, ng, 1], best_min [R, ng, 1])."""
     gs = group_size if granularity == 'per_group' else w.shape[1]
     w = w.reshape(w.shape[0], 1, -1, gs)
-    ocb = 256 if w.shape[0] % 256 == 0 else 64
-    assert w.shape[0] % ocb == 0
+    ocb = 256 if w.shape[0] % 256 == 0 else 64     # blocking sizes memory only; the last block may be short
     x = x.view(-1, x.shape[-1])
     x = x.reshape(1, x.shape[0], -1, gs)
     step = max(1, x.shape[1] // n_sample_token)
     x = x[:, 0::step]
     best_max_all, best_min_all = [], []
-    for ib in range(w.shape[0] // ocb):
+    for ib in range(-(-w.shape[0] // ocb)):
         wb = w[ib * ocb:(ib + 1) * ocb]
         org_max = wb.abs().amax(dim=-1, keepdim=True) if clip_sym else wb.amax(dim=-1, keepdim=True)
         org_min = wb.amin(dim=-1, keepdim=True)
