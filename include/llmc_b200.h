@@ -413,6 +413,24 @@ int llmc_gemm_w4a16(const void* x, const int32_t* wq, const void* scales, const 
 int llmc_gemm_w8a16(const void* x, const int32_t* wq, const void* scales, const void* zeros,
                     int qparam_dtype, const void* bias, void* y, int64_t M, int64_t N, int64_t K,
                     int64_t group, int dtype, void* stream);
+/* llmc_gemm_w4a16_gidx / llmc_gemm_w8a16_gidx — the same fused forward with a per-column group
+ *   index: replaces GPTQ.w_qdq with act-order (gptq.py:424-452: W[:, perm] -> qdq in groups of
+ *   the permuted order -> [:, invperm]) followed by F.linear of EffcientFakeQuantLinear
+ *   (module_utils.py:719).  Column k dequantises with group g_idx[k] = invperm[k] / group_size:
+ *   g_idx   [K] int32, 0 <= g_idx[k] < ng (a precondition of the caller, not checked on the device)
+ *   scales / zeros  [N, ng], or [ng, N] when q_transposed != 0, of type `qparam_dtype`
+ *   Arithmetic per element as llmc_gemm_w4a16 (fp32 qparams: one rounding of the fp32 product),
+ *   K in its original order, so the result equals llmc_gemm_bf16 on the materialised weight bit
+ *   for bit; with g_idx[k] = k / group it equals the contiguous call.  K % 64 == 0, 1 <= ng <= K,
+ *   g_idx 16-byte aligned; wq as llmc_gemm_w4a16 / llmc_gemm_w8a16. */
+int llmc_gemm_w4a16_gidx(const void* x, const int32_t* wq, const void* scales, const void* zeros,
+                         int qparam_dtype, const int32_t* g_idx, int64_t ng, int q_transposed,
+                         const void* bias, void* y, int64_t M, int64_t N, int64_t K, int dtype,
+                         void* stream);
+int llmc_gemm_w8a16_gidx(const void* x, const int32_t* wq, const void* scales, const void* zeros,
+                         int qparam_dtype, const int32_t* g_idx, int64_t ng, int q_transposed,
+                         const void* bias, void* y, int64_t M, int64_t N, int64_t K, int dtype,
+                         void* stream);
 
 #ifdef __cplusplus
 }

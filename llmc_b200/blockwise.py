@@ -328,9 +328,12 @@ class BaseBlockwiseQuantization(BlockwiseOpt):
             params['a_qdq'] = (functools.partial(self.a_qdq, aquantizer=self.aquantizer)
                                if not w_only else None)
             params['w_qdq'] = functools.partial(self.w_qdq, wquantizer=self.wquantizer)
-            if type(self).w_qdq is BaseBlockwiseQuantization.w_qdq:
-                # the packed twin of the default w_qdq (algorithms that override w_qdq, e.g. GPTQ with
-                # act-order, keep the materialised path)
+            # the packed twin of w_qdq: only a class that defines w_qdq knows what it materialises,
+            # so the packer is the `w_packed` that same class defines (the base one for RTN / AWQ,
+            # GPTQ's own, act-order included).  A subclass that overrides w_qdq without a w_packed
+            # of its own (SpQR's outlier columns, HQQ) keeps the materialised path.
+            owner = next(c for c in type(self).__mro__ if 'w_qdq' in c.__dict__)
+            if 'w_packed' in owner.__dict__:
                 params['w_qdq'].packed = functools.partial(self.w_packed, wquantizer=self.wquantizer)
         elif mode in _REALQUANT_LINEAR_MAP_:
             params['w_q'] = functools.partial(self.w_q, wquantizer=self.wquantizer)

@@ -25,6 +25,16 @@
 // Weight layout: LLMC_OUT_PACK_VLLM of UNSIGNED codes — 8 nibbles per int32 along K, nibble i =
 // element 8*w + i; scales / zeros fp32 [N, K/group] (zeros NULL => 2^(bit-1), the symmetric
 // +8 offset of module_utils.py:842-844).
+//
+// Group-index form (kGidx, GPTQ act-order): column k uses group g_idx[k] of ng, in any order, so
+// one 64-deep step can touch 64 different groups.  The dequant warps then gather each element's
+// (scale, zero) from global memory (L1 / L2: the qparams of an 8B-model linear are at most 3.7 MB
+// in fp32) instead of holding one pair per step in registers; staging the CTA's 128-row slice of
+// every group in shared memory would take 112 KB at K = 14336, which the ring needs.  The
+// arithmetic per element is the fp32 one, fmul_rn((2^23 + q) - (2^23 + z), s), for both qparam
+// flavours (the product of a small integer and a 16-bit qparam is exact in fp32, so it rounds to
+// the same value as the packed half2 / bf16x2 path).  The ring, the consumers and the epilogue are
+// the contiguous form's; K keeps its order, so the result is still llmc_gemm_bf16's bit for bit.
 #include <stdlib.h>
 
 #include "tc.cuh"
@@ -62,6 +72,7 @@ struct Params {
   int q_transposed;         // qparams stored [ng, N] (a warp's 32 rows = one coalesced segment)
   int64_t group;
   int ng;
+  const int32_t* g_idx;     // [K] group of each column (group-index form only)
   float zero_default;
   int n_tiles_n, num_units, kb_total, gn;
 };
@@ -89,7 +100,7 @@ __device__ __forceinline__ uint32_t sub_mul2(uint32_t x2, uint32_t zm2, uint32_t
   }
 }
 
-template <bool kBf16, int kBits>
+template <bool kBf16, int kBits, bool kGidx>
 __global__ void __launch_bounds__(Cfg<kBits>::kThreads, 1)
 w4a16_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmP,
                   const Params p) {
@@ -212,13 +223,13 @@ w4a16_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
       // first K step of this tile that belongs to this group: (it + kb) % NG == grp
       int kb = (grp + NG - static_cast<int>(it % NG)) % NG;
       uint32_t s_cur = 0u, z_cur = 0u;
-      if (kb < p.kb_total) load_qparams(n0, kb / steps_per_group, s_cur, z_cur);
+      if (!kGidx && kb < p.kb_total) load_qparams(n0, kb / steps_per_group, s_cur, z_cur);
       for (; kb < p.kb_total; kb += NG) {
         const auto sl = PipeState<kLStages>::at(it + kb);
         const auto sb = PipeState<kBStages>::at(it + kb);
         // qparams of this group's NEXT step are requested now and consumed next iteration
         uint32_t s_nxt = s_cur, z_nxt = z_cur;
-        if (kb + NG < p.kb_total && (kb + NG) / steps_per_group != kb / steps_per_group)
+        if (!kGidx && kb + NG < p.kb_total && (kb + NG) / steps_per_group != kb / steps_per_group)
           load_qparams(n0, (kb + NG) / steps_per_group, s_nxt, z_nxt);
         ring_l.wait_full(sl);
         ring_b.wait_empty(sb);
@@ -227,7 +238,45 @@ w4a16_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
         const float z_c = have_zeros ? widen(z_cur) : p.zero_default;
         const float zm_cur = 8388608.0f + z_c;        // (2^23 + q) - (2^23 + z) = q - z exactly
         const float s_c = (n0 < p.N) ? widen(s_cur) : 0.f;
-        if constexpr (kBits == 8) {
+        if constexpr (kGidx) {
+          // this row's packed words of the step, unswizzled: word w holds elements 32/kBits * w ..
+          constexpr int kWords = BK * kBits / 32;
+          uint32_t words[kWords];
+          if constexpr (kBits == 8) {
+            const int sw8 = (row >> 1) & 3;
+#pragma unroll
+            for (int c4 = 0; c4 < 4; ++c4) {
+              const uint4 wv = *reinterpret_cast<const uint4*>(pk + row * 64 + ((c4 ^ sw8) << 4));
+              words[4 * c4] = wv.x; words[4 * c4 + 1] = wv.y; words[4 * c4 + 2] = wv.z; words[4 * c4 + 3] = wv.w;
+            }
+          } else {
+            const int sw = ((row >> 2) & 1) << 4;
+            const uint4 w0 = *reinterpret_cast<const uint4*>(pk + row * 32 + sw);
+            const uint4 w1 = *reinterpret_cast<const uint4*>(pk + row * 32 + (sw ^ 16));
+            words[0] = w0.x; words[1] = w0.y; words[2] = w0.z; words[3] = w0.w;
+            words[4] = w1.x; words[5] = w1.y; words[6] = w1.z; words[7] = w1.w;
+          }
+          const int4* gk = reinterpret_cast<const int4*>(p.g_idx + static_cast<int64_t>(kb) * BK);
+#pragma unroll
+          for (int c = 0; c < 8; ++c) {              // 16-byte output chunk c = elements 8c .. 8c+7
+            const int4 ga = __ldg(gk + 2 * c), gb = __ldg(gk + 2 * c + 1);   // same for every lane
+            const int g[8] = {ga.x, ga.y, ga.z, ga.w, gb.x, gb.y, gb.z, gb.w};
+            uint32_t sr[8], zr[8];
+#pragma unroll
+            for (int e = 0; e < 8; ++e) load_qparams(n0, g[e], sr[e], zr[e]);
+            float v[8];
+#pragma unroll
+            for (int e = 0; e < 8; ++e) {
+              const uint32_t q = kBits == 8 ? (words[2 * c + e / 4] >> (8 * (e % 4))) & 0xFFu
+                                            : (words[c] >> (4 * e)) & 0xFu;
+              const float zm = 8388608.0f + (have_zeros ? widen(zr[e]) : p.zero_default);
+              v[e] = fmul_rn(__uint_as_float(0x4B000000u | q) - zm, widen(sr[e]));
+            }
+            const uint4 o = make_uint4(pack_pair<DT>(v[0], v[1]), pack_pair<DT>(v[2], v[3]),
+                                       pack_pair<DT>(v[4], v[5]), pack_pair<DT>(v[6], v[7]));
+            *reinterpret_cast<uint4*>(bt + row * 128 + ((c ^ (row & 7)) << 4)) = o;
+          }
+        } else if constexpr (kBits == 8) {
           // INT8: 64-byte rows, TMA SWIZZLE_64B: 16-byte chunk c of row r sits at c ^ ((r >> 1) & 3).
           // byte -> fp32 through the 2^23 magic (0x4B0000nn), (q - z) * s in fp32, one rounding;
           // bf16 has no exact packed form for 8-bit codes (128 + q needs 9 bits), so both qparam
@@ -322,7 +371,8 @@ using namespace llmc;
 template <int kBits>
 static int gemm_wNa16(const void* x, const int32_t* wq, const void* scales, const void* zeros,
                       int qparam_dtype, const void* bias, void* y, int64_t M, int64_t N, int64_t K,
-                      int64_t group, int dtype, int q_transposed, void* stream, const char* name) {
+                      int64_t group, const int32_t* g_idx, int64_t ng, int dtype, int q_transposed,
+                      void* stream, const char* name) {
   using namespace w4;
   LLMC_CHECK_ARG(M >= 0 && N >= 0 && K > 0, "%s: bad shape", name);
   if (M == 0 || N == 0) return LLMC_OK;
@@ -330,10 +380,16 @@ static int gemm_wNa16(const void* x, const int32_t* wq, const void* scales, cons
   LLMC_CHECK_ARG(dtype == LLMC_BF16 || dtype == LLMC_F16, "%s: dtype must be bf16 or fp16", name);
   LLMC_CHECK_ARG(qparam_dtype == LLMC_F32 || qparam_dtype == dtype,
                  "%s: qparam_dtype must be fp32 or the activation dtype", name);
-  LLMC_CHECK_ARG(group > 0 && K % group == 0 && group % BK == 0,
-                 "%s: group %lld must divide K=%lld and be a multiple of %d", name, (long long)group,
-                 (long long)K, BK);
-  if (K % 64 != 0 || !aligned16(x) || !aligned16(wq) || !aligned16(y)) {
+  if (g_idx == nullptr) {
+    LLMC_CHECK_ARG(group > 0 && K % group == 0 && group % BK == 0,
+                   "%s: group %lld must divide K=%lld and be a multiple of %d", name, (long long)group,
+                   (long long)K, BK);
+    ng = K / group;
+  } else {
+    LLMC_CHECK_ARG(ng >= 1 && ng <= K, "%s: ng=%lld groups for K=%lld columns", name, (long long)ng,
+                   (long long)K);
+  }
+  if (K % 64 != 0 || !aligned16(x) || !aligned16(wq) || !aligned16(y) || (g_idx && !aligned16(g_idx))) {
     set_last_error("%s: K=%lld must be a multiple of 64 and pointers 16-byte aligned", name, (long long)K);
     return LLMC_EALIGN;
   }
@@ -352,7 +408,8 @@ static int gemm_wNa16(const void* x, const int32_t* wq, const void* scales, cons
   // packed half2 / bf16x2 dequant exists for INT4 only; INT8 widens native qparams to fp32
   p.qparam_native = (qparam_dtype != LLMC_F32) ? 1 : 0;
   p.q_transposed = q_transposed ? 1 : 0;
-  p.group = group; p.ng = static_cast<int>(K / group);
+  p.group = g_idx ? K : group; p.ng = static_cast<int>(ng);
+  p.g_idx = g_idx;
   p.zero_default = static_cast<float>(1 << (kBits - 1));
   p.n_tiles_n = static_cast<int>((N + BN - 1) / BN);
   const int64_t mt = (M + BM - 1) / BM;
@@ -367,9 +424,11 @@ static int gemm_wNa16(const void* x, const int32_t* wq, const void* scales, cons
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   constexpr int smem = C::kSmemBytes;
   static_assert(smem <= 227 * 1024, "shared memory budget");
-  return launch_persistent(dtype == LLMC_BF16 ? w4a16_gemm_kernel<true, kBits>
-                                              : w4a16_gemm_kernel<false, kBits>,
-                           p.num_units, C::kThreads, smem, st, tmA, tmP, p);
+  auto kernel = g_idx ? (dtype == LLMC_BF16 ? w4a16_gemm_kernel<true, kBits, true>
+                                            : w4a16_gemm_kernel<false, kBits, true>)
+                      : (dtype == LLMC_BF16 ? w4a16_gemm_kernel<true, kBits, false>
+                                            : w4a16_gemm_kernel<false, kBits, false>);
+  return launch_persistent(kernel, p.num_units, C::kThreads, smem, st, tmA, tmP, p);
 }
 
 extern "C" int llmc_gemm_w4a16(const void* x, const int32_t* wq, const void* scales,
@@ -378,7 +437,7 @@ extern "C" int llmc_gemm_w4a16(const void* x, const int32_t* wq, const void* sca
                                void* stream) {
   // `group` < 0 selects the TRANSPOSED qparam layout [K/|group|, N] (coalesced per-warp loads)
   return gemm_wNa16<4>(x, wq, scales, zeros, qparam_dtype, bias, y, M, N, K, group < 0 ? -group : group,
-                       dtype, group < 0, stream, "gemm_w4a16");
+                       nullptr, 0, dtype, group < 0, stream, "gemm_w4a16");
 }
 
 // INT8 weights: wq [N, K/4] int32, 4 UNSIGNED codes per word along K (code + 128 for symmetric,
@@ -388,5 +447,25 @@ extern "C" int llmc_gemm_w8a16(const void* x, const int32_t* wq, const void* sca
                                int64_t M, int64_t N, int64_t K, int64_t group, int dtype,
                                void* stream) {
   return gemm_wNa16<8>(x, wq, scales, zeros, qparam_dtype, bias, y, M, N, K, group < 0 ? -group : group,
-                       dtype, group < 0, stream, "gemm_w8a16");
+                       nullptr, 0, dtype, group < 0, stream, "gemm_w8a16");
+}
+
+// Group-index form: column k dequantises with the qparams of group g_idx[k] (0 <= g_idx[k] < ng,
+// the caller's guarantee; not checked on the device).
+extern "C" int llmc_gemm_w4a16_gidx(const void* x, const int32_t* wq, const void* scales,
+                                    const void* zeros, int qparam_dtype, const int32_t* g_idx,
+                                    int64_t ng, int q_transposed, const void* bias, void* y,
+                                    int64_t M, int64_t N, int64_t K, int dtype, void* stream) {
+  LLMC_CHECK_ARG(g_idx != nullptr, "gemm_w4a16_gidx: g_idx is NULL");
+  return gemm_wNa16<4>(x, wq, scales, zeros, qparam_dtype, bias, y, M, N, K, 0, g_idx, ng, dtype,
+                       q_transposed, stream, "gemm_w4a16_gidx");
+}
+
+extern "C" int llmc_gemm_w8a16_gidx(const void* x, const int32_t* wq, const void* scales,
+                                    const void* zeros, int qparam_dtype, const int32_t* g_idx,
+                                    int64_t ng, int q_transposed, const void* bias, void* y,
+                                    int64_t M, int64_t N, int64_t K, int dtype, void* stream) {
+  LLMC_CHECK_ARG(g_idx != nullptr, "gemm_w8a16_gidx: g_idx is NULL");
+  return gemm_wNa16<8>(x, wq, scales, zeros, qparam_dtype, bias, y, M, N, K, 0, g_idx, ng, dtype,
+                       q_transposed, stream, "gemm_w8a16_gidx");
 }

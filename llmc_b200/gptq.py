@@ -446,6 +446,41 @@ class GPTQ(BaseBlockwiseQuantization):
         return wquantizer.fake_quant_weight_static(module.weight.data, args)
 
     @torch.no_grad()
+    def w_packed(self, module, wquantizer):
+        """The packed form of exactly what `w_qdq` materialises, for EffcientFakeQuantLinear: codes of
+        the calibrated fp32 weight (original column order) from the same static quantisation pass
+        w_qdq runs, packed for llmc_gemm_w4a16 / w8a16; qparams as GPTQ stores them (dynamic groups:
+        fp32 in the permuted group order; static groups and per-channel: the model dtype, original
+        order); `g_idx` = invperm // group_size when act-order reorders the groups.  None when the
+        layer does not fit the packed GEMM; it is then materialised as before."""
+        from .module_utils import pack_unsigned_codes
+        from .quant import OUT_CODES_I32, IntegerQuantizer
+        q, w = wquantizer, module.weight.data
+        if not (isinstance(q, IntegerQuantizer) and q.bit in (4, 8) and q.calib_algo == 'minmax'
+                and q.granularity in ('per_group', 'per_channel') and q.round_zp
+                and w.dim() == 2 and w.is_cuda and w.is_floating_point()
+                and self.model_dtype in (torch.float16, torch.bfloat16)):
+            return None
+        R, K = w.shape
+        group = q.group_size if q.granularity == 'per_group' else K
+        if K % 64 or K % group or (not self.need_perm and group % 64):
+            return None
+        scales = module.buf_scales.to(w.device).reshape(R, -1)
+        ng = scales.shape[1]
+        zeros = getattr(module, 'buf_zeros', None) if not q.sym else None
+        if ng != K // group or scales.dtype not in (torch.float32, self.model_dtype):
+            return None
+        if zeros is not None:
+            zeros = zeros.to(device=w.device, dtype=scales.dtype).reshape(R, ng)
+        g_idx = (module.buf_invperm // group).to(torch.int32) if self.need_perm else None
+        codes = torch.empty((R, K), dtype=torch.int32, device=w.device)
+        q._static(w, scales.reshape(-1), zeros, module.buf_qmax, module.buf_qmin, OUT_CODES_I32, codes,
+                  self.model_dtype, ng, group, gmap=g_idx)
+        return dict(qweight=pack_unsigned_codes(codes, q.bit, signed=q.sym), scales=scales.contiguous(),
+                    zeros=None if zeros is None else zeros.contiguous(), bits=q.bit, group=group,
+                    dtype=self.model_dtype, g_idx=g_idx)
+
+    @torch.no_grad()
     def deploy(self, quant_format):
         """gptq.py:454-459."""
         self.check_factorizations(wait=True)

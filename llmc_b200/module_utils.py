@@ -37,13 +37,18 @@ def linear_forward(x, weight, bias=None):
     return y.reshape(*x.shape[:-1], N)
 
 
-def linear_forward_w4(x, wq, scales, zeros, group, bias=None, bits=4, qparams_t=False):
+def linear_forward_w4(x, wq, scales, zeros, group, bias=None, bits=4, qparams_t=False, g_idx=None):
     """Fake-quant forward on PACKED int4 weights (csrc/gemm_w4.cu): y = x @ dequant(wq).T + bias,
     bit-identical to linear_forward(x, rT((code - zero) * scale)) — the materialised weight of
     FakeQuantLinear (module_utils.py:626-643) — while reading 4.25 instead of 16 bits per weight.
 
     wq [N, K/8] int32 (unsigned codes, LLMC_OUT_PACK_VLLM layout), scales [N, K/group] in x.dtype
-    or fp32, zeros likewise or None (None => 8, the symmetric +2^(bit-1) storage offset)."""
+    or fp32, zeros likewise or None (None => 8, the symmetric +2^(bit-1) storage offset).
+
+    g_idx: int32 [K] or None.  When given, column k uses the qparams of group g_idx[k] (GPTQ
+    act-order: groups are contiguous in the permuted order, g_idx = invperm // group_size), the
+    qparams hold ng = scales.numel() // N groups in any order, and `group` is ignored.  Every value
+    must lie in [0, ng); the kernel does not check it."""
     require_cuda(x, wq, scales)
     K = x.shape[-1]
     N = wq.shape[0]
@@ -62,6 +67,19 @@ def linear_forward_w4(x, wq, scales, zeros, group, bias=None, bits=4, qparams_t=
     b = bias.to(x.dtype).contiguous() if bias is not None else None
     y = torch.empty((x2.shape[0], N), dtype=x.dtype, device=x.device)
     M = x2.shape[0]
+    if g_idx is not None:
+        ng = s.numel() // N
+        if s.numel() != N * ng or (z is not None and z.numel() != s.numel()) or ng == 0:
+            raise ValueError(f'qparams of {s.numel()} elements for N={N} rows')
+        if g_idx.dtype != torch.int32 or g_idx.numel() != K or not g_idx.is_cuda:
+            raise ValueError(f'g_idx must be a CUDA int32 tensor of K={K} elements')
+        gi = g_idx.contiguous()
+        with TIMER.span(f'gemm_w{bits}a16_gidx', flops=2.0 * M * N * K,
+                        nbytes=2.0 * M * K + bits / 8.0 * N * K + 8.0 * N * ng + 4.0 * K + 2.0 * M * N):
+            call(f'llmc_gemm_w{bits}a16_gidx', ptr(x2), ptr(wq.contiguous()), ptr(s), ptr(z), dtype_enum(qdt),
+                 ptr(gi), ng, int(bool(qparams_t)), ptr(b), ptr(y), M, N, K, dtype_enum(x.dtype),
+                 stream_ptr(x.device))
+        return y.reshape(*x.shape[:-1], N)
     with TIMER.span(f'gemm_w{bits}a16', flops=2.0 * M * N * K,
                     nbytes=2.0 * M * K + bits / 8.0 * N * K + 8.0 * N * K / group + 2.0 * M * N):
         call(f'llmc_gemm_w{bits}a16', ptr(x2), ptr(wq.contiguous()), ptr(s), ptr(z), dtype_enum(qdt), ptr(b), ptr(y), M, N, K,
@@ -264,7 +282,14 @@ class EffcientFakeQuantLinear(nn.Module):
     quantizer, `new` keeps the PACKED codes + group qparams instead of the dequantised weight and
     the forward runs the fused dequant -> wgmma GEMM (csrc/gemm_w4.cu) — bit-identical to F.linear
     on the materialised weight (tests/test_gpu_gemm_w4.py), at 4.25 / 8.25 instead of 16 bits per
-    weight in HBM.  `.weight` then dequantises on demand.  LLMC_B200_FUSED_DEQUANT=0 disables it."""
+    weight in HBM.  `.weight` then dequantises on demand.  LLMC_B200_FUSED_DEQUANT=0 disables it.
+
+    The packed form comes from the algorithm's `w_packed` twin of its `w_qdq` (RTN / AWQ: the base
+    one; GPTQ: GPTQ.w_packed).  Its qparams keep the dtype the algorithm stores them in — fp32 for
+    GPTQ's dynamic groups, with one rounding of the fp32 product — and `g_idx` (int32 [K], None
+    when groups are contiguous) gives each column's group when GPTQ's act-order makes the groups
+    contiguous only in the permuted column order.  Packed modules are left alone by
+    `convert_dtype`: their codes stay int32 and their qparams keep their dtype."""
 
     def __init__(self, weight, bias, ori_module, a_qdq, packed=None):
         super().__init__()
@@ -282,6 +307,7 @@ class EffcientFakeQuantLinear(nn.Module):
             self.register_buffer('qscales_t', packed['scales'].t().contiguous(), persistent=False)
             self.register_buffer('qzeros_t', packed['zeros'].t().contiguous()
                                  if packed['zeros'] is not None else None, persistent=False)
+            self.register_buffer('g_idx', packed.get('g_idx'))
         self.packed = packed is not None
         if bias is not None:
             self.register_buffer('bias', bias)
@@ -307,6 +333,11 @@ class EffcientFakeQuantLinear(nn.Module):
         N, K = codes.shape
         z = self.qzeros if self.qzeros is not None else float(1 << (bits - 1))
         s = self.qscales
+        if self.g_idx is not None:
+            # column k in group g_idx[k]; (code - zero) * scale in the qparam dtype, one rounding
+            gi = self.g_idx.long()
+            zz = z.reshape(N, -1)[:, gi] if torch.is_tensor(z) else z
+            return ((codes.to(s.dtype) - zz) * s.reshape(N, -1)[:, gi]).to(self.q_dtype)
         c = codes.reshape(N, -1, self.q_group).to(s.dtype)
         zz = z.reshape(N, -1, 1) if torch.is_tensor(z) else z
         return ((c - zz) * s.reshape(N, -1, 1)).reshape(N, K).to(self.q_dtype)
@@ -317,7 +348,7 @@ class EffcientFakeQuantLinear(nn.Module):
             x = self.a_qdq(x, self)
         if self.packed:
             return linear_forward_w4(x, self.qweight, self.qscales_t, self.qzeros_t, self.q_group, self.bias,
-                                     bits=self.q_bits, qparams_t=True)
+                                     bits=self.q_bits, qparams_t=True, g_idx=self.g_idx)
         return linear_forward(x, self.weight, self.bias)
 
     @classmethod

@@ -462,6 +462,11 @@ class SynthModel:
     def convert_dtype(self, dtype):
         for b in self.get_blocks():
             for m in b.modules():
+                if getattr(m, 'packed', False):
+                    # EffcientFakeQuantLinear on packed codes: `.weight` is computed from the codes
+                    # in the model dtype already, and its qparams (fp32 for GPTQ's dynamic groups)
+                    # must keep their dtype
+                    continue
                 if isinstance(m, tuple(_LLMC_LINEAR_TYPES_ + _TRANSFORMERS_LINEAR_TYPES_)):
                     if getattr(m, 'weight', None) is not None and m.weight.is_floating_point():
                         m.weight.data = m.weight.data.to(dtype)

@@ -248,6 +248,43 @@ if 'fp8' in only:
                         error=f'{type(e).__name__}: {str(e).splitlines()[0][:200]}')
             del x, w, wq, ws, xq, xs, wd
 
+if 'w4gidx' in only:
+    # GPTQ act-order deploy (gptq_w_only.yml: W4 asym g128, fp32 qparams, stored [ng, N] as
+    # EffcientFakeQuantLinear hands them over): the group-index GEMM with a random act-order g_idx,
+    # the same kernel with contiguous groups (identity g_idx), the contiguous entry point, and the
+    # bf16 GEMM on the materialised weight.  Llama-3-8B linears at M = 2048 (PPL eval, bs 1) and 16384.
+    from llmc_b200.module_utils import linear_forward_w4, pack_unsigned_codes
+    for M in (2048, 16384):
+        for (N, K) in ((4096, 4096), (1024, 4096), (14336, 4096), (4096, 14336)):
+            tag = f'{M}x{N}x{K}'
+            g = torch.Generator(device='cuda').manual_seed(0)
+            x = torch.randn(M, K, device='cuda', generator=g).bfloat16()
+            codes = torch.randint(0, 16, (N, K), device='cuda', generator=g)
+            packed = pack_unsigned_codes(codes, 4, signed=False)
+            ng = K // 128
+            s = torch.rand(ng, N, device='cuda', generator=g) * 0.004 + 0.001
+            z = torch.randint(0, 16, (ng, N), device='cuda', generator=g).float()
+            perm = torch.randperm(K, device='cuda', generator=g)
+            gi_act = (torch.argsort(perm) // 128).to(torch.int32)
+            gi_id = (torch.arange(K, device='cuda') // 128).to(torch.int32)
+            fl = 2.0 * M * N * K
+            runs = {
+                'gidx_actorder': lambda: linear_forward_w4(x, packed, s, z, 128, qparams_t=True, g_idx=gi_act),
+                'gidx_contiguous': lambda: linear_forward_w4(x, packed, s, z, 128, qparams_t=True, g_idx=gi_id),
+                'w4a16_contiguous': lambda: linear_forward_w4(x, packed, s, z, 128, qparams_t=True),
+            }
+            wd = ((codes.float() - z.t()[:, gi_act.long()]) * s.t()[:, gi_act.long()]).bfloat16()
+            runs['bf16_materialised'] = lambda: linear_forward(x, wd)
+            ms = {}
+            for rep in range(2):                     # alternate the four, keep the faster median
+                for name, fn in runs.items():
+                    t = timeit(fn, iters=10, warm=3, do_flush=False)
+                    ms[name] = min(ms.get(name, t), t)
+            for name, t in ms.items():
+                rec(f'{name}_{tag}', t, tflops=fl / t / 1e9,
+                    vs_actorder=round(ms['gidx_actorder'] / t, 3))
+            del x, codes, packed, s, z, wd
+
 os.makedirs('gpurun_out', exist_ok=True)
 json.dump(res, open('gpurun_out/microbench.json', 'w'), indent=1)
 
