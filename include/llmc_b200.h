@@ -260,6 +260,21 @@ int llmc_gptq_colblock(float* W, const float* Hinv, int64_t R, int64_t C, int64_
                        int64_t workspace_bytes, void* stream);
 
 /* ------------------------------------------------------------------------------------
+ * K5  llmc_gptq_colblock_fp8 — the same sweep on an FP8 grid: FloatQuantizer with
+ *   `use_qtorch: True` (quant.py:963-1081), e5m2 = 0 for e4m3fn (finfo.max 448), 1 for e5m2
+ *   (57344).  Symmetric, zero-point 0, so there are no zeros.  Per column (gptq.py:229-235):
+ *   s == 0 -> 1 (quant.py:1062), q = float_quantize(w / s + 0) * s in fp32, the rounding
+ *   clamped to +-finfo.max then round-to-nearest-even (the cvt.rn.satfinite of llmc_fp8_quant;
+ *   parity with qtorch unpinned).  Dynamic groups: s = max(|max|, |min|).clamp(1e-5) / finfo.max
+ *   in fp32, written to scales [R, ng] in permuted order.  Everything else (W, Hinv, tmp,
+ *   losses, group / static_groups / gmap / q_dtype, out_perm, workspace) as llmc_gptq_colblock.
+ * ------------------------------------------------------------------------------------ */
+int llmc_gptq_colblock_fp8(float* W, const float* Hinv, int64_t R, int64_t C, int64_t group,
+                           int e5m2, int static_groups, const int32_t* gmap, void* scales,
+                           int q_dtype, float* tmp, const int64_t* out_perm, float* losses,
+                           void* workspace, int64_t workspace_bytes, void* stream);
+
+/* ------------------------------------------------------------------------------------
  * K5s llmc_spqr_colblock — SpQR's column sweep (llmc/compression/quantization/spqr.py:172-268,
  *   326-351), the sibling of llmc_gptq_colblock: same Hessian / Cholesky inputs, same block /
  *   super-panel schedule and trailing updates; the in-block step is SpQR's — per group of `group`

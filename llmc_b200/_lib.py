@@ -60,6 +60,8 @@ SIGNATURES = {
     'llmc_gptq_workspace_bytes': (c_i64, [c_i64, c_i64]),
     'llmc_gptq_colblock': (c_int, [c_vp, c_vp, c_i64, c_i64, c_i64, c_int, c_int, c_int, c_vp,
                                    c_vp, c_vp, c_int, c_vp, c_vp, c_vp, c_vp, c_i64, c_vp]),
+    'llmc_gptq_colblock_fp8': (c_int, [c_vp, c_vp, c_i64, c_i64, c_i64, c_int, c_int, c_vp, c_vp,
+                                       c_int, c_vp, c_vp, c_vp, c_vp, c_i64, c_vp]),
     'llmc_spqr_colblock': (c_int, [c_vp, c_vp, c_i64, c_i64, c_i64, c_int, c_int, c_int, c_int, c_int,
                                    c_int, c_int, c_int, c_int, c_vp, c_int, c_vp, c_vp, c_vp, c_vp,
                                    c_vp, c_vp, c_vp, c_i64, c_vp]),

@@ -13,21 +13,9 @@
 #include <cuda_fp8.h>
 
 #include "common.cuh"
+#include "fp8_math.cuh"
 
 namespace llmc {
-
-__device__ __forceinline__ float fp8_round(float v, int e5m2) {
-  if (e5m2) {
-    const __nv_fp8_storage_t b = __nv_cvt_float_to_fp8(v, __NV_SATFINITE, __NV_E5M2);
-    return __half2float(__half(__nv_cvt_fp8_to_halfraw(b, __NV_E5M2)));
-  }
-  const __nv_fp8_storage_t b = __nv_cvt_float_to_fp8(v, __NV_SATFINITE, __NV_E4M3);
-  return __half2float(__half(__nv_cvt_fp8_to_halfraw(b, __NV_E4M3)));
-}
-
-__device__ __forceinline__ uint8_t fp8_bits(float v, int e5m2) {
-  return static_cast<uint8_t>(__nv_cvt_float_to_fp8(v, __NV_SATFINITE, e5m2 ? __NV_E5M2 : __NV_E4M3));
-}
 
 struct Fp8Args {
   const void* w;

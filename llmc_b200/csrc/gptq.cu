@@ -13,6 +13,7 @@
 // correctly rounded divides), so single-block problems are bit-exact; across blocks only the
 // summation order of the 128-deep trailing dot products differs from the CPU BLAS.
 #include "tc.cuh"
+#include "fp8_math.cuh"
 #include "quant_math.cuh"
 #include "spqr_row.cuh"
 
@@ -128,6 +129,24 @@ __device__ __forceinline__ float group8_max(float v) {
   return fmaxf(v, __shfl_xor_sync(0xffffffffu, v, 4));
 }
 
+// The grid a column is rounded onto.  Only the quantise-dequantise of one element differs; the
+// scale search of a dynamic group is the symmetric qparams() on either grid (FloatQuantizer is
+// symmetric with qmax = finfo.max: max(|max|, |min|).clamp(1e-5) / fmax, zero 0; quant.py:549-553).
+enum : int { kGridInt = 0, kGridE4M3 = 1, kGridE5M2 = 2 };
+
+template <int G>
+__device__ __forceinline__ float grid_qdq(float x, const MarksteinDiv& div_s, float s, float z, float qmin,
+                                          float qmax) {
+  if constexpr (G == kGridInt) {
+    return dequant<F32Round>(quant_code<F32Round>(x, div_s, z, qmin, qmax), s, z);
+  } else {
+    // quant.py:1063-1075 in fp32: float_quantize(x / s + 0.0) * s (the + 0.0 turns a -0 quotient
+    // into +0; the zero-point is 0, so (q - 0) * s is q * s)
+    return fmul_rn(fp8_round(fadd_rn(div_s(x), 0.f), G == kGridE5M2), s);
+  }
+}
+
+template <int G>
 __global__ void __launch_bounds__(IR * IL, 2)
 gptq_inblock_kernel(InblockArgs a) {
   extern __shared__ float sm[];
@@ -269,6 +288,7 @@ gptq_inblock_kernel(InblockArgs a) {
       s = load_as(a.q_dtype, a.scales, row * a.ng + gi);
       z = a.zeros ? load_as(a.q_dtype, a.zeros, row * a.ng + gi) : 0.f;
     }
+    if constexpr (G != kGridInt) s = (s == 0.f) ? 1.f : s;   // quant.py:1062: scales[scales == 0] = 1
     const MarksteinDiv div_s(s);
     float wc = Wr[rg * WP + c_own];
     float hd[IL];
@@ -281,7 +301,7 @@ gptq_inblock_kernel(InblockArgs a) {
     // the eight sequential columns of the sub-block: lane jj's column is final at step jj
 #pragma unroll
     for (int jj = 0; jj < IL; ++jj) {
-      const float q = dequant<F32Round>(quant_code<F32Round>(wc, div_s, z, a.qmin, a.qmax), s, z);
+      const float q = grid_qdq<G>(wc, div_s, s, z, a.qmin, a.qmax);
       const float diff = fsub_rn(wc, q);
       float err = div_d(diff);                                                      // :239
       if (!col_live) err = 0.f;
@@ -690,6 +710,30 @@ extern "C" int64_t llmc_gptq_workspace_bytes(int64_t R, int64_t C) {
   return (6 * kSuperPanel * rpad + 2 * C * C) * 4;
 }
 
+// The GPTQ sweep on grid G: `a` carries the grid's qmin / qmax / sym / zeros, the rest is filled in
+// here.  Arguments are validated by the entry points.
+template <int G>
+static int gptq_sweep(InblockArgs a, float* W, const float* Hinv, int64_t R, int64_t C, int64_t group,
+                      int static_groups, const int32_t* gmap, void* scales, int q_dtype, float* tmp,
+                      const int64_t* out_perm, float* losses, void* workspace, cudaStream_t st) {
+  if (int rc = opt_in_smem(gptq_inblock_kernel<G>, kInblockSmem)) return rc;
+  LLMC_CHECK_CUDA(cudaMemsetAsync(losses, 0, R * sizeof(float), st));
+  a.W = W; a.Hinv = Hinv; a.R = R; a.C = C;
+  a.group = group; a.ng = C / group;
+  a.static_groups = static_groups; a.gmap = gmap;
+  a.scales = scales; a.q_dtype = q_dtype;
+  a.tmp = tmp; a.out_perm = out_perm; a.losses = losses;
+  a.Rpad = ((R + GB - 1) / GB) * GB;
+  const bool wide = !static_groups && group > kSuperPanel;
+  return sweep_schedule(W, Hinv, R, C, group, wide, workspace, st,
+                        [&](int i1, int count, float* err, float* err_hi, float* err_lo, cudaStream_t cs) -> int {
+    a.i1 = i1; a.count = count; a.err = err; a.err_hi = err_hi; a.err_lo = err_lo;
+    gptq_inblock_kernel<G><<<static_cast<unsigned>(a.Rpad / IR), IR * IL, kInblockSmem, cs>>>(a);
+    LLMC_CHECK_LAUNCH();
+    return LLMC_OK;
+  });
+}
+
 extern "C" int llmc_gptq_colblock(float* W, const float* Hinv, int64_t R, int64_t C, int64_t group,
                                   int bit, int sym, int static_groups, const int32_t* gmap,
                                   void* scales, void* zeros, int q_dtype, float* tmp,
@@ -706,25 +750,41 @@ extern "C" int llmc_gptq_colblock(float* W, const float* Hinv, int64_t R, int64_
   LLMC_CHECK_ARG(sym || zeros, "gptq_colblock: zeros is NULL for asymmetric quantisation");
   LLMC_CHECK_ARG(static_groups || q_dtype == LLMC_F32, "gptq_colblock: dynamic groups write fp32 qparams");
   LLMC_CHECK_ARG(workspace_bytes >= llmc_gptq_workspace_bytes(R, C), "gptq_colblock: workspace too small");
-  cudaStream_t st = static_cast<cudaStream_t>(stream);
-  if (int rc = opt_in_smem(gptq_inblock_kernel, kInblockSmem)) return rc;
-  LLMC_CHECK_CUDA(cudaMemsetAsync(losses, 0, R * sizeof(float), st));
   InblockArgs a{};
-  a.W = W; a.Hinv = Hinv; a.R = R; a.C = C;
-  a.group = group; a.ng = C / group; a.sym = sym;
+  a.sym = sym;
   int_range(bit, sym, a.qmin, a.qmax);
-  a.static_groups = static_groups; a.gmap = gmap;
-  a.scales = scales; a.zeros = sym ? nullptr : zeros; a.q_dtype = q_dtype;
-  a.tmp = tmp; a.out_perm = out_perm; a.losses = losses;
-  a.Rpad = ((R + GB - 1) / GB) * GB;
-  const bool wide = !static_groups && group > kSuperPanel;
-  return sweep_schedule(W, Hinv, R, C, group, wide, workspace, st,
-                        [&](int i1, int count, float* err, float* err_hi, float* err_lo, cudaStream_t cs) -> int {
-    a.i1 = i1; a.count = count; a.err = err; a.err_hi = err_hi; a.err_lo = err_lo;
-    gptq_inblock_kernel<<<static_cast<unsigned>(a.Rpad / IR), IR * IL, kInblockSmem, cs>>>(a);
-    LLMC_CHECK_LAUNCH();
-    return LLMC_OK;
-  });
+  a.zeros = sym ? nullptr : zeros;
+  return gptq_sweep<kGridInt>(a, W, Hinv, R, C, group, static_groups, gmap, scales, q_dtype, tmp, out_perm,
+                              losses, workspace, static_cast<cudaStream_t>(stream));
+}
+
+extern "C" int llmc_gptq_colblock_fp8(float* W, const float* Hinv, int64_t R, int64_t C, int64_t group,
+                                      int e5m2, int static_groups, const int32_t* gmap, void* scales,
+                                      int q_dtype, float* tmp, const int64_t* out_perm, float* losses,
+                                      void* workspace, int64_t workspace_bytes, void* stream) {
+  LLMC_CHECK_ARG(W && Hinv && tmp && losses && workspace && R > 0 && C > 0, "gptq_colblock_fp8: bad argument");
+  LLMC_CHECK_ARG(e5m2 == 0 || e5m2 == 1, "gptq_colblock_fp8: e5m2 must be 0 (e4m3) or 1 (e5m2), got %d", e5m2);
+  LLMC_CHECK_ARG(group > 0 && group <= C && C % group == 0, "gptq_colblock_fp8: C=%lld %% group=%lld != 0",
+                 (long long)C, (long long)group);
+  LLMC_CHECK_ARG((group >= C) || (group >= GB ? group % GB == 0 : (GB % group == 0 && GB / group <= 8)),
+                 "gptq_colblock_fp8: group %lld must divide or be a multiple of the block size 128 "
+                 "(and be >= 16)", (long long)group);
+  LLMC_CHECK_ARG(scales, "gptq_colblock_fp8: scales is NULL");
+  LLMC_CHECK_ARG(static_groups || q_dtype == LLMC_F32, "gptq_colblock_fp8: dynamic groups write fp32 scales");
+  LLMC_CHECK_ARG(q_dtype >= LLMC_F32 && q_dtype <= LLMC_BF16, "gptq_colblock_fp8: bad q_dtype %d", q_dtype);
+  LLMC_CHECK_ARG(workspace_bytes >= llmc_gptq_workspace_bytes(R, C), "gptq_colblock_fp8: workspace too small");
+  // FloatQuantizer is symmetric (quant.py:966) with [qmin, qmax] = +-finfo.max: qparams() then gives
+  // the reference's scale, and the zero-point is 0
+  InblockArgs a{};
+  a.sym = 1;
+  a.qmax = e5m2 ? 57344.f : 448.f;
+  a.qmin = -a.qmax;
+  a.zeros = nullptr;
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  if (e5m2) return gptq_sweep<kGridE5M2>(a, W, Hinv, R, C, group, static_groups, gmap, scales, q_dtype, tmp,
+                                         out_perm, losses, workspace, st);
+  return gptq_sweep<kGridE4M3>(a, W, Hinv, R, C, group, static_groups, gmap, scales, q_dtype, tmp, out_perm,
+                               losses, workspace, st);
 }
 
 static spqr::QCfg spqr_qcfg(int bit, int sym, int round_zp) {

@@ -54,9 +54,25 @@ class GPTQ(BaseBlockwiseQuantization):
         if sp.get('owq', False):
             raise NotImplementedError('OWQ mixed precision (gptq.py:47-50) is not on the hot path')
         self.owq = False
+        if self.float_grid:
+            # FloatQuantizer itself refuses use_qtorch False (quant.py:1005-1027) and grids other
+            # than e4m3 / e5m2 (:982-988); the sweep covers the granularities of gptq.py:212-227
+            wq = self.wquantizer
+            if wq.granularity not in ('per_channel', 'per_tensor', 'per_group'):
+                raise NotImplementedError(f'GPTQ on an FP8 grid with granularity {wq.granularity} '
+                                          '(gptq.py:212-227 sweeps per_channel / per_tensor / per_group)')
+            if wq.calib_algo != 'minmax':
+                raise NotImplementedError(f'GPTQ on an FP8 grid with calib_algo {wq.calib_algo} '
+                                          '(the sweep searches minmax scales, quant.py:1043-1059)')
         self.chunk_num = sp.get('chunk_num', 1)
         self.need_perm = (self.wquantizer.granularity == 'per_group'
                           and not self.static_groups and self.actorder)
+
+    @property
+    def float_grid(self):
+        """The weights go onto an FP8 grid (FloatQuantizer, llmc_gptq_colblock_fp8)."""
+        from .quant_float import FloatQuantizer
+        return isinstance(self.wquantizer, FloatQuantizer)
 
     # ---- Hessian collection ---------------------------------------------------------------------
     @torch.no_grad()
@@ -369,6 +385,11 @@ class GPTQ(BaseBlockwiseQuantization):
                 layer.buf_scales = scales.reshape(R, ng)[r0:r1].reshape(-1, 1)
                 if not wq.sym:
                     layer.buf_zeros = zeros.reshape(R, ng)[r0:r1].reshape(-1, 1)
+            elif self.float_grid:
+                # FloatQuantizer.quant sets zero scales to 1 IN PLACE (quant.py:1062), and the sweep
+                # hands it the layer's own buf_scales (search_layer_qparams / search_group_qparams,
+                # gptq.py:368-395): a 16-bit scale that underflowed to 0 stays 1 for deploy / export
+                layer.buf_scales.masked_fill_(layer.buf_scales == 0, 1)
 
     def _static_qparams(self, layer, R, ng):
         """The kernel indexes static qparams as [row * ng + group]; expand what
@@ -438,6 +459,13 @@ class GPTQ(BaseBlockwiseQuantization):
     @torch.no_grad()
     def w_qdq(self, module, wquantizer):
         """gptq.py:424-452: W[:, perm] -> static qdq -> model dtype -> [:, invperm], one pass."""
+        if self.float_grid:
+            # the FP8 static kernel has no group map: the column gathers of gptq.py:427-450 as written
+            w = module.weight.data
+            if self.need_perm:
+                w = w[:, module.buf_perm]
+            w = wquantizer.fake_quant_weight_static(w, {'scales': module.buf_scales}).to(self.model_dtype)
+            return w[:, module.buf_invperm] if self.need_perm else w
         args = {'scales': module.buf_scales,
                 'zeros': module.buf_zeros if hasattr(module, 'buf_zeros') else None,
                 'qmax': module.buf_qmax, 'qmin': module.buf_qmin, 'out_dtype': self.model_dtype}

@@ -11,6 +11,7 @@ from ._lib import F32, call, dtype_enum, load, ptr, require_cuda, stream_ptr
 from .prof import TIMER
 
 _ws_cache = {}
+_FP8_GRIDS = {'e4m3': 0, 'e5m2': 1}      # FloatQuantizer.bit -> the e5m2 flag of llmc_gptq_colblock_fp8
 
 
 def _workspace(nbytes, device, tag):
@@ -108,6 +109,8 @@ def weight_transform(Wp, Hinv, bit, sym, group, static_qparams=None, gmap=None, 
     """gptq.py:198-244 (+ :186-193 when out_perm is given).
 
     Wp [R,C] fp32 permuted weights (consumed as scratch), Hinv [C,C] upper factor.
+    bit: an integer width (IntegerQuantizer, llmc_gptq_colblock), or 'e4m3' / 'e5m2'
+      (FloatQuantizer with use_qtorch, llmc_gptq_colblock_fp8: symmetric, no zeros).
     group: group size, or C for per_channel.
     static_qparams: None -> dynamic groups (qparams searched while sweeping, returned fp32
       [R, ng] in permuted column order); else (scales [R*ng], zeros|None) inputs.
@@ -123,6 +126,9 @@ def weight_transform(Wp, Hinv, bit, sym, group, static_qparams=None, gmap=None, 
     R, C = Wp.shape
     ng = C // group
     dev = Wp.device
+    fp8 = bit in _FP8_GRIDS
+    if fp8:
+        sym = True                      # FloatQuantizer is symmetric (quant.py:966)
     tmp = torch.empty_like(Wp)
     losses = torch.empty(R, dtype=torch.float32, device=dev)
     if static_qparams is None:
@@ -137,8 +143,14 @@ def weight_transform(Wp, Hinv, bit, sym, group, static_qparams=None, gmap=None, 
     nbytes = load().llmc_gptq_workspace_bytes(R, C)
     ws = _workspace(nbytes, dev, 'gptq_err')
     op = out_perm.to(torch.int64).contiguous() if out_perm is not None else None
-    with TIMER.span(f'gptq_colblock[{R}x{C}]', flops=float(R) * C * C + float(R) * C * 128,
-                    nbytes=8.0 * R * C + 2.0 * C * C):
+    flops, nbytes = float(R) * C * C + float(R) * C * 128, 8.0 * R * C + 2.0 * C * C
+    if fp8:
+        with TIMER.span(f'gptq_colblock_fp8[{R}x{C}]', flops=flops, nbytes=nbytes):
+            call('llmc_gptq_colblock_fp8', ptr(Wp), ptr(Hinv), R, C, int(group), _FP8_GRIDS[bit],
+                 static, ptr(gmap), ptr(scales), qdt, ptr(tmp), ptr(op), ptr(losses), ptr(ws),
+                 ws.numel(), stream_ptr(dev))
+        return tmp, losses, scales, None
+    with TIMER.span(f'gptq_colblock[{R}x{C}]', flops=flops, nbytes=nbytes):
         call('llmc_gptq_colblock', ptr(Wp), ptr(Hinv), R, C, int(group), int(bit),
              int(bool(sym)), static, ptr(gmap), ptr(scales), ptr(zeros), qdt, ptr(tmp), ptr(op),
              ptr(losses), ptr(ws), ws.numel(), stream_ptr(dev))

@@ -63,6 +63,9 @@ class SpQR(GPTQ):
         if self.quant_config.get('quant_type', 'int-quant') == 'float-quant':
             raise AssertionError('SPQR do not support Float quant now.')           # spqr.py:52-53
         wq = self.wquantizer
+        if self.float_grid:
+            raise NotImplementedError('SpQR on an FP8 weight grid: the reference refuses float quant '
+                                      '(spqr.py:53) and the SpQR kernel is integer only')
         if wq.sym:
             # the reference fails here too: zeros is a 0-dim tensor that zero_quantizer's
             # reshape_tensor cannot index (spqr.py:334, quant.py:614)
