@@ -446,6 +446,24 @@ int llmc_gemm_w8a16_gidx(const void* x, const int32_t* wq, const void* scales, c
                          int qparam_dtype, const int32_t* g_idx, int64_t ng, int q_transposed,
                          const void* bias, void* y, int64_t M, int64_t N, int64_t K, int dtype,
                          void* stream);
+/* llmc_gemm_fp8a16 / llmc_gemm_fp8a16_gidx — the same fused forward for FP8 weights
+ *   (FloatQuantizer's e4m3 / e5m2 fake-quant weights; e5m2 != 0: e5m2, else e4m3):
+ *   Y = X · dequant(Wq)^T (+ bias),  dequant(Wq)[n,k] = rT(fmul_rn(fp32(byte[n,k]), s)), s the
+ *   row's group scale, or 1 where that scale is 0 (quant.py:1062).  This is the QDQ value
+ *   llmc_fp8_quant writes (mode 1) computed from the bytes it writes (mode 2), so the result equals
+ *   llmc_gemm_bf16 on the materialised weight bit for bit.  fp8 value x 16-bit scale is exact in
+ *   fp32; fp32 scales round once in fp32, then to `dtype`.
+ *   wq      the fp8 bytes [N, K] viewed as int32 [N, K/4] (byte i of word w = element 4w + i)
+ *   scales  as llmc_gemm_w8a16 / llmc_gemm_w8a16_gidx (fp32 or `dtype`, [N, ng] or transposed)
+ *   zeros   must be NULL (the grid is symmetric)
+ *   Otherwise as llmc_gemm_w8a16 (group: negative for transposed qparams) / llmc_gemm_w8a16_gidx. */
+int llmc_gemm_fp8a16(const void* x, const int32_t* wq, const void* scales, const void* zeros,
+                     int qparam_dtype, const void* bias, void* y, int64_t M, int64_t N, int64_t K,
+                     int64_t group, int dtype, int e5m2, void* stream);
+int llmc_gemm_fp8a16_gidx(const void* x, const int32_t* wq, const void* scales, const void* zeros,
+                          int qparam_dtype, const int32_t* g_idx, int64_t ng, int q_transposed,
+                          const void* bias, void* y, int64_t M, int64_t N, int64_t K, int dtype,
+                          int e5m2, void* stream);
 
 #ifdef __cplusplus
 }

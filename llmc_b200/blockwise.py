@@ -306,7 +306,10 @@ class BaseBlockwiseQuantization(BlockwiseOpt):
         materialise, or None when this layer / quantizer is not a plain INT4 / INT8 group or channel
         weight quantizer (then the wrapper materialises as before)."""
         from .module_utils import pack_unsigned_codes
+        from .quant_float import FloatQuantizer
         q, w = wquantizer, module.weight
+        if isinstance(q, FloatQuantizer):
+            return self._fp8_packed(module, q)
         if not (isinstance(q, IntegerQuantizer) and q.bit in (4, 8) and q.calib_algo == 'minmax'
                 and q.granularity in ('per_group', 'per_channel') and q.round_zp
                 and w.dim() == 2 and w.is_cuda and w.dtype in (torch.float16, torch.bfloat16)):
@@ -321,6 +324,29 @@ class BaseBlockwiseQuantization(BlockwiseOpt):
         return dict(qweight=pack_unsigned_codes(codes, q.bit, signed=q.sym), scales=scales.contiguous(),
                     zeros=None if zeros is None else zeros.to(scales.dtype).contiguous(),
                     bits=q.bit, group=group, dtype=w.dtype)
+
+    @staticmethod
+    def _fp8_packed(module, q):
+        """w_packed on an e4m3 / e5m2 grid (FloatQuantizer, minmax): the bytes and scales of the very
+        pass fake_quant_weight_dynamic runs (`_dynamic`: byte mode instead of QDQ mode).  per_tensor's
+        fp32 scalar is expanded to one fp32 scale per row; per_channel / per_group keep their scales in
+        the weight dtype.  None for per_block, clipped layers, and K or groups not a multiple of 64."""
+        w = module.weight
+        if not (q.calib_algo == 'minmax' and q.granularity in ('per_tensor', 'per_channel', 'per_group')
+                and w.dim() == 2 and w.is_cuda and w.dtype in (torch.float16, torch.bfloat16)):
+            return None
+        if hasattr(module, 'buf_lowbound_factor') or hasattr(module, 'buf_upbound_factor'):
+            return None
+        N, K = w.shape
+        # FloatQuantizer._layout: a row shorter than the group is one group
+        group = q.group_size if q.granularity == 'per_group' and K >= q.group_size else K
+        if K % 64 or group % 64 or K % group:
+            return None
+        wq, scales = q._dynamic(w.data, 2)
+        if q.granularity == 'per_tensor':
+            scales = scales.reshape(1).float().expand(N, 1)
+        return dict(qweight=wq.reshape(N, K), scales=scales.reshape(N, K // group).contiguous(), zeros=None,
+                    bits=8, group=group, dtype=w.dtype)
 
     def get_replacement_params(self, mode='fake_quant', w_only=False, name=None):
         params = {}

@@ -35,7 +35,16 @@
 // flavours (the product of a small integer and a 16-bit qparam is exact in fp32, so it rounds to
 // the same value as the packed half2 / bf16x2 path).  The ring, the consumers and the epilogue are
 // the contiguous form's; K keeps its order, so the result is still llmc_gemm_bf16's bit for bit.
+//
+// FP8 weight grids (kGrid e4m3 / e5m2, FloatQuantizer's fake-quant weights): the INT8 configuration
+// unchanged — 8 KB packed tile, TMA box and swizzle, rings, consumers, epilogue, tile order — on
+// the fp8 byte tensor [N, K] viewed as int32 [N, K/4] (byte i of word w = element 4w + i, the W8
+// word layout).  Per element: byte -> fp32 (exact, every e4m3 / e5m2 value is an fp16 value),
+// fmul_rn(q, s) with s = 1 where the scale is 0 (quant.py:1062), one rounding to bf16 / fp16 —
+// fp8_emit's QDQ value (csrc/fp8.cu) from the bytes of its byte mode.  No zero-point.
 #include <stdlib.h>
+
+#include <cuda_fp8.h>
 
 #include "tc.cuh"
 
@@ -49,6 +58,8 @@ constexpr int BM = 128, BN = 128, BK = 64;
 constexpr int kABytes = BM * BK * 2;          // 16 KB
 constexpr int kBBytes = BN * BK * 2;          // 16 KB dequantised
 constexpr int NG = 2;                         // dequant groups of four warps
+// the weight grid: integer codes, or e4m3 / e5m2 bytes (8-bit words, no zero-point)
+enum : int { kGridInt = 0, kGridE4M3 = 1, kGridE5M2 = 2 };
 // per weight width: INT4 -> 4 KB packed tile, INT8 -> 8 KB
 template <int kBits> struct Cfg {
   static constexpr int kPBytes = BN * BK * kBits / 8;
@@ -100,7 +111,19 @@ __device__ __forceinline__ uint32_t sub_mul2(uint32_t x2, uint32_t zm2, uint32_t
   }
 }
 
-template <bool kBf16, int kBits, bool kGidx>
+// four fp8 bytes of a word -> fp32, byte i in f[i]; exact through fp16
+template <int G>
+__device__ __forceinline__ void fp8x4_to_f32(uint32_t w, float* f) {
+  constexpr __nv_fp8_interpretation_t kI = G == kGridE5M2 ? __NV_E5M2 : __NV_E4M3;
+  const float2 lo = __half22float2(__half2(__nv_cvt_fp8x2_to_halfraw2(static_cast<__nv_fp8x2_storage_t>(w & 0xFFFFu), kI)));
+  const float2 hi = __half22float2(__half2(__nv_cvt_fp8x2_to_halfraw2(static_cast<__nv_fp8x2_storage_t>(w >> 16), kI)));
+  f[0] = lo.x; f[1] = lo.y; f[2] = hi.x; f[3] = hi.y;
+}
+
+// quant.py:1062: a zero scale dequantises with 1
+__device__ __forceinline__ float fp8_scale(float s) { return s == 0.f ? 1.f : s; }
+
+template <bool kBf16, int kBits, bool kGidx, int kGrid>
 __global__ void __launch_bounds__(Cfg<kBits>::kThreads, 1)
 w4a16_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmP,
                   const Params p) {
@@ -265,12 +288,20 @@ w4a16_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
 #pragma unroll
             for (int e = 0; e < 8; ++e) load_qparams(n0, g[e], sr[e], zr[e]);
             float v[8];
+            if constexpr (kGrid != kGridInt) {
+              float f[8];
+              fp8x4_to_f32<kGrid>(words[2 * c], f);
+              fp8x4_to_f32<kGrid>(words[2 * c + 1], f + 4);
 #pragma unroll
-            for (int e = 0; e < 8; ++e) {
-              const uint32_t q = kBits == 8 ? (words[2 * c + e / 4] >> (8 * (e % 4))) & 0xFFu
-                                            : (words[c] >> (4 * e)) & 0xFu;
-              const float zm = 8388608.0f + (have_zeros ? widen(zr[e]) : p.zero_default);
-              v[e] = fmul_rn(__uint_as_float(0x4B000000u | q) - zm, widen(sr[e]));
+              for (int e = 0; e < 8; ++e) v[e] = fmul_rn(f[e], fp8_scale(widen(sr[e])));
+            } else {
+#pragma unroll
+              for (int e = 0; e < 8; ++e) {
+                const uint32_t q = kBits == 8 ? (words[2 * c + e / 4] >> (8 * (e % 4))) & 0xFFu
+                                              : (words[c] >> (4 * e)) & 0xFu;
+                const float zm = 8388608.0f + (have_zeros ? widen(zr[e]) : p.zero_default);
+                v[e] = fmul_rn(__uint_as_float(0x4B000000u | q) - zm, widen(sr[e]));
+              }
             }
             const uint4 o = make_uint4(pack_pair<DT>(v[0], v[1]), pack_pair<DT>(v[2], v[3]),
                                        pack_pair<DT>(v[4], v[5]), pack_pair<DT>(v[6], v[7]));
@@ -289,10 +320,23 @@ w4a16_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
 #pragma unroll
             for (int hh = 0; hh < 2; ++hh) {
               float v[8];
+              if constexpr (kGrid != kGridInt) {
+                // fp8 bytes: decode, times the scale in fp32
+                float f0[4], f1[4];
+                fp8x4_to_f32<kGrid>(wd[2 * hh], f0);
+                fp8x4_to_f32<kGrid>(wd[2 * hh + 1], f1);
+                const float s_f = fp8_scale(s_c);
 #pragma unroll
-              for (int j = 0; j < 4; ++j) {
-                v[j] = fmul_rn(__uint_as_float(__byte_perm(wd[2 * hh], 0x4B000000u, 0x7650u + j)) - zm_cur, s_c);
-                v[4 + j] = fmul_rn(__uint_as_float(__byte_perm(wd[2 * hh + 1], 0x4B000000u, 0x7650u + j)) - zm_cur, s_c);
+                for (int j = 0; j < 4; ++j) {
+                  v[j] = fmul_rn(f0[j], s_f);
+                  v[4 + j] = fmul_rn(f1[j], s_f);
+                }
+              } else {
+#pragma unroll
+                for (int j = 0; j < 4; ++j) {
+                  v[j] = fmul_rn(__uint_as_float(__byte_perm(wd[2 * hh], 0x4B000000u, 0x7650u + j)) - zm_cur, s_c);
+                  v[4 + j] = fmul_rn(__uint_as_float(__byte_perm(wd[2 * hh + 1], 0x4B000000u, 0x7650u + j)) - zm_cur, s_c);
+                }
               }
               const uint4 o = make_uint4(pack_pair<DT>(v[0], v[1]), pack_pair<DT>(v[2], v[3]),
                                          pack_pair<DT>(v[4], v[5]), pack_pair<DT>(v[6], v[7]));
@@ -368,7 +412,7 @@ w4a16_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
 
 using namespace llmc;
 
-template <int kBits>
+template <int kBits, int kGrid = w4::kGridInt>
 static int gemm_wNa16(const void* x, const int32_t* wq, const void* scales, const void* zeros,
                       int qparam_dtype, const void* bias, void* y, int64_t M, int64_t N, int64_t K,
                       int64_t group, const int32_t* g_idx, int64_t ng, int dtype, int q_transposed,
@@ -424,10 +468,10 @@ static int gemm_wNa16(const void* x, const int32_t* wq, const void* scales, cons
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   constexpr int smem = C::kSmemBytes;
   static_assert(smem <= 227 * 1024, "shared memory budget");
-  auto kernel = g_idx ? (dtype == LLMC_BF16 ? w4a16_gemm_kernel<true, kBits, true>
-                                            : w4a16_gemm_kernel<false, kBits, true>)
-                      : (dtype == LLMC_BF16 ? w4a16_gemm_kernel<true, kBits, false>
-                                            : w4a16_gemm_kernel<false, kBits, false>);
+  auto kernel = g_idx ? (dtype == LLMC_BF16 ? w4a16_gemm_kernel<true, kBits, true, kGrid>
+                                            : w4a16_gemm_kernel<false, kBits, true, kGrid>)
+                      : (dtype == LLMC_BF16 ? w4a16_gemm_kernel<true, kBits, false, kGrid>
+                                            : w4a16_gemm_kernel<false, kBits, false, kGrid>);
   return launch_persistent(kernel, p.num_units, C::kThreads, smem, st, tmA, tmP, p);
 }
 
@@ -468,4 +512,38 @@ extern "C" int llmc_gemm_w8a16_gidx(const void* x, const int32_t* wq, const void
   LLMC_CHECK_ARG(g_idx != nullptr, "gemm_w8a16_gidx: g_idx is NULL");
   return gemm_wNa16<8>(x, wq, scales, zeros, qparam_dtype, bias, y, M, N, K, 0, g_idx, ng, dtype,
                        q_transposed, stream, "gemm_w8a16_gidx");
+}
+
+// FP8 weights (e5m2 != 0: e5m2, else e4m3): wq = the fp8 bytes [N, K] viewed as int32 [N, K/4],
+// scales as llmc_gemm_w8a16, zeros must be NULL.  dequant = rT(fmul_rn(fp32(byte), s)), s = 1
+// where the scale is 0.
+static int gemm_fp8a16(const void* x, const int32_t* wq, const void* scales, const void* zeros,
+                       int qparam_dtype, const void* bias, void* y, int64_t M, int64_t N, int64_t K,
+                       int64_t group, const int32_t* g_idx, int64_t ng, int dtype, int q_transposed,
+                       int e5m2, void* stream, const char* name) {
+  LLMC_CHECK_ARG(zeros == nullptr, "%s: an fp8 grid has no zero-point (zeros must be NULL)", name);
+  LLMC_CHECK_ARG(e5m2 == 0 || e5m2 == 1, "%s: e5m2 must be 0 (e4m3) or 1 (e5m2), got %d", name, e5m2);
+  if (e5m2)
+    return gemm_wNa16<8, w4::kGridE5M2>(x, wq, scales, nullptr, qparam_dtype, bias, y, M, N, K, group, g_idx,
+                                        ng, dtype, q_transposed, stream, name);
+  return gemm_wNa16<8, w4::kGridE4M3>(x, wq, scales, nullptr, qparam_dtype, bias, y, M, N, K, group, g_idx,
+                                      ng, dtype, q_transposed, stream, name);
+}
+
+extern "C" int llmc_gemm_fp8a16(const void* x, const int32_t* wq, const void* scales,
+                                const void* zeros, int qparam_dtype, const void* bias, void* y,
+                                int64_t M, int64_t N, int64_t K, int64_t group, int dtype, int e5m2,
+                                void* stream) {
+  return gemm_fp8a16(x, wq, scales, zeros, qparam_dtype, bias, y, M, N, K, group < 0 ? -group : group,
+                     nullptr, 0, dtype, group < 0, e5m2, stream, "gemm_fp8a16");
+}
+
+extern "C" int llmc_gemm_fp8a16_gidx(const void* x, const int32_t* wq, const void* scales,
+                                     const void* zeros, int qparam_dtype, const int32_t* g_idx,
+                                     int64_t ng, int q_transposed, const void* bias, void* y,
+                                     int64_t M, int64_t N, int64_t K, int dtype, int e5m2,
+                                     void* stream) {
+  LLMC_CHECK_ARG(g_idx != nullptr, "gemm_fp8a16_gidx: g_idx is NULL");
+  return gemm_fp8a16(x, wq, scales, zeros, qparam_dtype, bias, y, M, N, K, 0, g_idx, ng, dtype, q_transposed,
+                     e5m2, stream, "gemm_fp8a16_gidx");
 }

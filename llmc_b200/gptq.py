@@ -484,6 +484,8 @@ class GPTQ(BaseBlockwiseQuantization):
         from .module_utils import pack_unsigned_codes
         from .quant import OUT_CODES_I32, IntegerQuantizer
         q, w = wquantizer, module.weight.data
+        if self.float_grid:
+            return self._fp8_packed_static(module, q)
         if not (isinstance(q, IntegerQuantizer) and q.bit in (4, 8) and q.calib_algo == 'minmax'
                 and q.granularity in ('per_group', 'per_channel') and q.round_zp
                 and w.dim() == 2 and w.is_cuda and w.is_floating_point()
@@ -506,6 +508,37 @@ class GPTQ(BaseBlockwiseQuantization):
                   self.model_dtype, ng, group, gmap=g_idx)
         return dict(qweight=pack_unsigned_codes(codes, q.bit, signed=q.sym), scales=scales.contiguous(),
                     zeros=None if zeros is None else zeros.contiguous(), bits=q.bit, group=group,
+                    dtype=self.model_dtype, g_idx=g_idx)
+
+    def _fp8_packed_static(self, module, q):
+        """w_packed on an e4m3 / e5m2 grid: the bytes of w_qdq's static pass on W[:, perm] (byte mode
+        instead of QDQ mode), gathered back with [:, invperm]; the scales as that pass reads them —
+        buf_scales in the weight's dtype (fp32 until convert_dtype), a per-tensor scale as fp32, one per
+        row — so that fp32(byte) * s rounds once to the model dtype exactly as w_qdq's
+        `.to(model_dtype)` does.  g_idx = invperm // group_size under act-order."""
+        w = module.weight.data
+        if not (q.granularity in ('per_tensor', 'per_channel', 'per_group') and w.dim() == 2 and w.is_cuda
+                and w.dtype in (torch.float32, self.model_dtype)
+                and self.model_dtype in (torch.float16, torch.bfloat16)):
+            return None
+        R, K = w.shape
+        group = q.group_size if q.granularity == 'per_group' else K
+        if K % 64 or K % group or (not self.need_perm and group % 64):
+            return None
+        s = module.buf_scales.to(w.device)
+        if s.numel() == 1:
+            scales = s.reshape(1).float().expand(R, 1).contiguous()
+        else:
+            scales = s.reshape(R, -1).to(w.dtype).contiguous()
+        if scales.shape[1] != K // group:
+            return None
+        src = w[:, module.buf_perm] if self.need_perm else w
+        wq = q._static(src, module.buf_scales, 2).reshape(R, K)
+        g_idx = None
+        if self.need_perm:
+            wq = wq.view(torch.uint8)[:, module.buf_invperm].view(wq.dtype)
+            g_idx = (module.buf_invperm // group).to(torch.int32)
+        return dict(qweight=wq.contiguous(), scales=scales, zeros=None, bits=8, group=group,
                     dtype=self.model_dtype, g_idx=g_idx)
 
     @torch.no_grad()

@@ -87,6 +87,53 @@ def linear_forward_w4(x, wq, scales, zeros, group, bias=None, bits=4, qparams_t=
     return y.reshape(*x.shape[:-1], N)
 
 
+FP8_GRIDS = {torch.float8_e4m3fn: 'e4m3', torch.float8_e5m2: 'e5m2'}
+
+
+def linear_forward_fp8w(x, wq, scales, group, bias=None, qparams_t=False, g_idx=None):
+    """Fake-quant forward on FP8 weights (csrc/gemm_w4.cu, e4m3 / e5m2 grid): y = x @ dequant(wq).T
+    + bias, dequant = rT(fp32(wq) * s) with s = 1 where the scale is 0 — bit-identical to
+    linear_forward on the weight FloatQuantizer materialises (llmc_fp8_quant's QDQ output) while
+    reading 8 bits plus a scale per group instead of 16 bits per weight.
+
+    wq [N, K] float8_e4m3fn / float8_e5m2; scales [N, K/group] (or [K/group, N] with qparams_t) in
+    x.dtype or fp32.  g_idx as in linear_forward_w4."""
+    require_cuda(x, wq, scales)
+    if wq.dtype not in FP8_GRIDS:
+        raise TypeError(f'fp8 weight dtype must be float8_e4m3fn or float8_e5m2, not {wq.dtype}')
+    K = x.shape[-1]
+    N = wq.shape[0]
+    if wq.dim() != 2 or wq.shape[1] != K or K % 4:
+        raise ValueError(f'fp8 weight shape {tuple(wq.shape)} does not match K={K}')
+    e5m2 = int(wq.dtype == torch.float8_e5m2)
+    words = wq.contiguous().view(torch.int32)            # [N, K/4]: byte i of word w = element 4w + i
+    x2 = x.reshape(-1, K)
+    x2 = x2 if x2.is_contiguous() else x2.contiguous()
+    qdt = x.dtype if scales.dtype == x.dtype else torch.float32
+    shape = (-1, N) if qparams_t else (N, -1)
+    s = scales.reshape(shape).to(qdt).contiguous()
+    b = bias.to(x.dtype).contiguous() if bias is not None else None
+    y = torch.empty((x2.shape[0], N), dtype=x.dtype, device=x.device)
+    M = x2.shape[0]
+    if g_idx is not None:
+        ng = s.numel() // N
+        if s.numel() != N * ng or ng == 0:
+            raise ValueError(f'scales of {s.numel()} elements for N={N} rows')
+        if g_idx.dtype != torch.int32 or g_idx.numel() != K or not g_idx.is_cuda:
+            raise ValueError(f'g_idx must be a CUDA int32 tensor of K={K} elements')
+        gi = g_idx.contiguous()
+        with TIMER.span('gemm_fp8a16_gidx', flops=2.0 * M * N * K,
+                        nbytes=2.0 * M * K + 1.0 * N * K + s.element_size() * N * ng + 4.0 * K + 2.0 * M * N):
+            call('llmc_gemm_fp8a16_gidx', ptr(x2), ptr(words), ptr(s), None, dtype_enum(qdt), ptr(gi), ng,
+                 int(bool(qparams_t)), ptr(b), ptr(y), M, N, K, dtype_enum(x.dtype), e5m2, stream_ptr(x.device))
+        return y.reshape(*x.shape[:-1], N)
+    with TIMER.span('gemm_fp8a16', flops=2.0 * M * N * K,
+                    nbytes=2.0 * M * K + 1.0 * N * K + s.element_size() * N * K / group + 2.0 * M * N):
+        call('llmc_gemm_fp8a16', ptr(x2), ptr(words), ptr(s), None, dtype_enum(qdt), ptr(b), ptr(y), M, N, K,
+             int(-group if qparams_t else group), dtype_enum(x.dtype), e5m2, stream_ptr(x.device))
+    return y.reshape(*x.shape[:-1], N)
+
+
 # Counterpart of the reference's USE_FP8GEMM_TRITON_KERNEL (module_utils.py:14-20): when set,
 # LlmcFp8Linear keeps its weight in fp8 and runs block_wise_fp8_forward_func on the FP8 tensor cores.
 # Off by default: the forward then dequantises once and runs the bf16 GEMM, as it always has here.
@@ -289,7 +336,15 @@ class EffcientFakeQuantLinear(nn.Module):
     GPTQ's dynamic groups, with one rounding of the fp32 product — and `g_idx` (int32 [K], None
     when groups are contiguous) gives each column's group when GPTQ's act-order makes the groups
     contiguous only in the permuted column order.  Packed modules are left alone by
-    `convert_dtype`: their codes stay int32 and their qparams keep their dtype."""
+    `convert_dtype`: their codes stay int32 and their qparams keep their dtype.
+
+    FP8 weights (FloatQuantizer on an e4m3 / e5m2 grid) are packed too: `qweight` then holds the
+    fp8 bytes [N, K] themselves (`q_grid` 'e4m3' / 'e5m2'; 'int' for codes), with one scale per row
+    or group and no zero-point, and the forward runs llmc_gemm_fp8a16 — 8 bits plus the scales per
+    weight instead of 16, bit-identical to the materialised forward (tests/test_gpu_gemm_fp8w.py)."""
+
+    # the buffers of the packed form; export_state_dict writes an FP8 module's dense `weight` instead
+    PACKED_BUFFERS = ('qweight', 'qscales', 'qzeros', 'qscales_t', 'qzeros_t', 'g_idx')
 
     def __init__(self, weight, bias, ori_module, a_qdq, packed=None):
         super().__init__()
@@ -303,6 +358,7 @@ class EffcientFakeQuantLinear(nn.Module):
             else:
                 self.qzeros = None
             self.q_bits, self.q_group, self.q_dtype = packed['bits'], packed['group'], packed['dtype']
+            self.q_grid = FP8_GRIDS.get(packed['qweight'].dtype, 'int')
             # [K/group, N] copies for the GEMM (coalesced qparam loads); tiny next to the codes
             self.register_buffer('qscales_t', packed['scales'].t().contiguous(), persistent=False)
             self.register_buffer('qzeros_t', packed['zeros'].t().contiguous()
@@ -326,7 +382,14 @@ class EffcientFakeQuantLinear(nn.Module):
 
     @torch.no_grad()
     def dequantized_weight(self):
-        """rT((code - zero) * scale): the tensor the reference holds in `.weight` (elementwise, exact)."""
+        """rT((code - zero) * scale): the tensor the reference holds in `.weight` (elementwise, exact).
+        FP8 grids: rT(fp32(byte) * scale), a zero scale read as 1, as llmc_fp8_quant's QDQ output."""
+        if self.q_grid != 'int':
+            N, K = self.qweight.shape
+            s = self.qscales.float().reshape(N, -1)
+            s = s.masked_fill(s == 0, 1.0)
+            s = s[:, self.g_idx.long()] if self.g_idx is not None else s.repeat_interleave(self.q_group, dim=1)
+            return (self.qweight.float() * s).to(self.q_dtype)
         bits, pf = self.q_bits, 32 // self.q_bits
         sh = torch.arange(pf, device=self.qweight.device, dtype=torch.int32) * bits
         codes = ((self.qweight.unsqueeze(-1) >> sh) & ((1 << bits) - 1)).reshape(self.qweight.shape[0], -1)
@@ -346,6 +409,9 @@ class EffcientFakeQuantLinear(nn.Module):
     def forward(self, x):
         if self.a_qdq is not None:
             x = self.a_qdq(x, self)
+        if self.packed and self.q_grid != 'int':
+            return linear_forward_fp8w(x, self.qweight, self.qscales_t, self.q_group, self.bias, qparams_t=True,
+                                       g_idx=self.g_idx)
         if self.packed:
             return linear_forward_w4(x, self.qweight, self.qscales_t, self.qzeros_t, self.q_group, self.bias,
                                      bits=self.q_bits, qparams_t=True, g_idx=self.g_idx)
