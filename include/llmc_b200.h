@@ -357,6 +357,9 @@ int llmc_awq_clip(const void* w, int64_t R, int64_t C, const void* x, int64_t ns
  *   the fp8 grid with saturation to the finite max (csrc/fp8.cu header).
  *   dynamic != 0: per (row, group) scale = rT(max(absmax, 1e-5) / finfo.max) written to `scales`
  *                 (dtype), then out_mode 1: QDQ (dtype) | 2: fp8 bytes | 0: scales only.
+ *                 A NaN in a group makes its scale NaN (the absmax propagates NaN, as amax does).
+ *   A scale of 0 (a 16-bit scale that underflowed, or a static 0) quantises with 1 (quant.py:1062);
+ *   the scale written is still 0, and FloatQuantizer exports 1 for it.
  *   dynamic == 0: `scales` is an input: [rows * q_row_stride] dtype, or ONE per-tensor scale
  *                 (q_row_stride 0), fp32 when scale_f32 != 0 (torch's CPU scalar-operand path).
  * ------------------------------------------------------------------------------------ */

@@ -29,6 +29,19 @@ struct Fp8Args {
   void* out;
 };
 
+// The absmax propagates NaN, as the reference's amax / max / clamp do (quant.py:137-140, 550-551):
+// a NaN anywhere in a group makes its scale, and so every output of the group, NaN.  fmaxf would
+// drop it and quantise the rest of the group as if it were absent.
+__device__ __forceinline__ float fmax_nan(float a, float b) {
+  float r;
+  asm("max.NaN.f32 %0, %1, %2;" : "=f"(r) : "f"(a), "f"(b));
+  return r;
+}
+__device__ __forceinline__ float warp_max_nan(float v) {
+  for (int o = 16; o > 0; o >>= 1) v = fmax_nan(v, __shfl_xor_sync(0xffffffffu, v, o));
+  return v;
+}
+
 template <int DT>
 __device__ __forceinline__ void fp8_emit(const Fp8Args& a, int64_t idx, float x, float s, bool scalar) {
   // quant.py:1062: scales[scales == 0] = 1
@@ -56,16 +69,16 @@ fp8_dynamic_kernel(Fp8Args a) {
     const int64_t base = r * a.cols + j * a.group;
     float mx = 0.f;
     for (int64_t i = threadIdx.x; i < a.group; i += blockDim.x)
-      mx = fmaxf(mx, fabsf(DType<DT>::load(a.w, base + i)));
-    mx = warp_max(mx);
+      mx = fmax_nan(mx, fabsf(DType<DT>::load(a.w, base + i)));
+    mx = warp_max_nan(mx);
     if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = mx;
     __syncthreads();
     if (threadIdx.x < 32) {
       float v = threadIdx.x < 8 ? red[threadIdx.x] : 0.f;
-      v = warp_max(v);
+      v = warp_max_nan(v);
       if (threadIdx.x == 0) {
         // quant.py:549-553: abs_max.clamp(min=1e-5) / qmax
-        const float am = fmaxf(v, DType<DT>::rT(1e-5f));
+        const float am = fmax_nan(v, DType<DT>::rT(1e-5f));
         s_sh = DType<DT>::rT(fdiv_rn(am, a.fmax));
         DType<DT>::store(a.scales, g, s_sh);
       }
@@ -152,16 +165,16 @@ fp8_block_quant_kernel(const void* __restrict__ w, int64_t M, int64_t N, int bs,
     float mx = 0.f;
     for (int e = threadIdx.x; e < bs * bs; e += blockDim.x) {
       const int64_t r = r0 + e / bs, c = c0 + e % bs;
-      if (r < M && c < N) mx = fmaxf(mx, fabsf(DType<DT>::load(w, r * N + c)));
+      if (r < M && c < N) mx = fmax_nan(mx, fabsf(DType<DT>::load(w, r * N + c)));
     }
-    mx = warp_max(mx);
+    mx = warp_max_nan(mx);
     if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = mx;
     __syncthreads();
     if (threadIdx.x < 32) {
       float v = threadIdx.x < 8 ? red[threadIdx.x] : 0.f;
-      v = warp_max(v);
+      v = warp_max_nan(v);
       if (threadIdx.x == 0) {
-        s_sh = fdiv_rn(fmaxf(v, 1e-5f), fmax);
+        s_sh = fdiv_rn(fmax_nan(v, 1e-5f), fmax);
         scales[b] = s_sh;
       }
     }

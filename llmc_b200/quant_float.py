@@ -17,6 +17,16 @@ from .quant import BaseQuantizer
 _FP8 = {'e4m3': (torch.float8_e4m3fn, 0), 'e5m2': (torch.float8_e5m2, 1)}
 
 
+def _zeros_to_one(scales):
+    """quant.py:1062 `scales[scales == 0] = 1`, in place on the caller's tensor as in the reference:
+    its quant() changes the scales it is handed, and dequant / real_quant_* go on with those.  A 16-bit
+    scale underflows to 0 for small groups (fp16: absmax / 57344 below ~1.7e-3 on e5m2); such a group
+    is quantised with scale 1, so 1 is the scale its bytes must be exported with."""
+    if torch.is_tensor(scales):
+        scales.masked_fill_(scales == 0, 1)
+    return scales
+
+
 class FloatQuantizer(BaseQuantizer):
     def __init__(self, bit, symmetric, granularity, **kwargs):
         super().__init__(bit, symmetric, granularity, **kwargs)
@@ -32,11 +42,12 @@ class FloatQuantizer(BaseQuantizer):
             raise NotImplementedError(f'{self.bit}: only e4m3 / e5m2 have hardware conversions '
                                       '(e2m1/e3m2/e4m7 of quant.py:982-988 are not built)')
         if 'float_range' in self.kwargs:
-            qmin, qmax = self.kwargs['float_range']
-        else:
-            fi = torch.finfo(_FP8[self.bit][0])
-            qmin, qmax = fi.min, fi.max
-        self.qmax, self.qmin = torch.tensor(qmax), torch.tensor(qmin)
+            # quant.py:979-980 would take qmin / qmax from it, but the kernels here (the quantiser, the
+            # FP8 GPTQ sweep, the fp8 dequant GEMM) all scale to finfo.max and saturate there
+            raise NotImplementedError('FloatQuantizer float_range: only the finfo range of e4m3 / e5m2 '
+                                      'is built (no shipped fp8 YAML sets float_range)')
+        fi = torch.finfo(_FP8[self.bit][0])
+        self.qmax, self.qmin = torch.tensor(fi.max), torch.tensor(fi.min)
         self.dst_nbins = 2 ** self.num_bits
 
     # ---- kernel launcher ----------------------------------------------------------------------
@@ -58,7 +69,10 @@ class FloatQuantizer(BaseQuantizer):
         return out
 
     def _layout(self, tensor):
-        t2d = tensor.reshape(-1, tensor.shape[-1])
+        if self.granularity == 'per_head':                   # quant.py:633-634: one group per head
+            t2d = tensor.reshape(self.head_num, -1)
+        else:
+            t2d = tensor.reshape(-1, tensor.shape[-1])
         t2d = t2d if t2d.is_contiguous() else t2d.contiguous()
         cols = t2d.shape[1]
         if self.granularity == 'per_group' and cols >= self.group_size:
@@ -68,21 +82,26 @@ class FloatQuantizer(BaseQuantizer):
         return t2d, cols
 
     def _dynamic(self, tensor, out_mode):
-        """-> (out, scales [rows*ng, 1] or 0-dim)."""
+        """-> (out, scales [rows*ng, 1] or 0-dim).  out_mode 0 returns get_qparams' scales as they
+        are; the byte mode (2) returns the scales the bytes were quantised with, zeros set to 1
+        (quant.py:1062), which is what real_quant_weight_dynamic exports and the fp8 GEMM reads."""
         if self.calib_algo != 'minmax':
             raise NotImplementedError(f'FloatQuantizer calib_algo={self.calib_algo}')
         if self.granularity == 'per_block':
-            return self._block(tensor, out_mode)
-        t2d, group = self._layout(tensor)
-        if self.granularity == 'per_tensor':
-            mn, mx = self.get_minmax_range(t2d)
-            scales, _, _, _ = self.get_qparams((mn, mx), t2d.device)     # 0-dim (fp32 for T != fp32)
-            s32 = scales.reshape(1).float().contiguous()
-            out = self._run(t2d, t2d.shape[1], 0, s32, out_mode, 0, 1) if out_mode else None
-            return out, scales
-        rows, cols = t2d.shape
-        scales = torch.empty((rows * (cols // group), 1), dtype=t2d.dtype, device=t2d.device)
-        out = self._run(t2d, group, 1, scales, out_mode)
+            out, scales = self._block(tensor, out_mode)
+        else:
+            t2d, group = self._layout(tensor)
+            if self.granularity == 'per_tensor':
+                mn, mx = self.get_minmax_range(t2d)
+                scales, _, _, _ = self.get_qparams((mn, mx), t2d.device)     # 0-dim (fp32 for T != fp32)
+                s32 = scales.reshape(1).float().contiguous()
+                out = self._run(t2d, t2d.shape[1], 0, s32, out_mode, 0, 1) if out_mode else None
+            else:
+                rows, cols = t2d.shape
+                scales = torch.empty((rows * (cols // group), 1), dtype=t2d.dtype, device=t2d.device)
+                out = self._run(t2d, group, 1, scales, out_mode)
+        if out_mode == 2:
+            _zeros_to_one(scales)
         return out, scales
 
     def _block(self, tensor, out_mode):
@@ -108,10 +127,19 @@ class FloatQuantizer(BaseQuantizer):
         return out, scales.view(mb, 1, nb, 1)
 
     def _static(self, tensor, scales, out_mode):
+        """quant.py:1063 `tensor / scales + zeros` with torch's type promotion.  A 0-dim scale, or one of
+        the tensor's dtype T, gives a T quotient (a one-element scale divides in fp32, torch's CPU
+        scalar-operand path).  Scales with dimensions of another dtype promote the quotient, and the
+        QDQ product, to fp32: the tensor is widened to fp32 first, so nothing is rounded to T (out_mode
+        1 then returns fp32, which the callers cast back as the reference's `.to(org_dtype)` does)."""
         t2d, group = self._layout(tensor)
-        s = scales
-        if s.dim() == 0 or s.numel() == 1:
-            s32 = s.reshape(1).to(device=t2d.device, dtype=torch.float32).contiguous()
+        s = scales.to(t2d.device)
+        if s.dim() and s.dtype != t2d.dtype:
+            if torch.promote_types(t2d.dtype, s.dtype) != torch.float32:
+                raise TypeError(f'FloatQuantizer static scales of {s.dtype} for a {t2d.dtype} tensor')
+            t2d = t2d.float()
+        if s.numel() == 1:
+            s32 = s.reshape(1).float().contiguous()
             return self._run(t2d, t2d.shape[1], 0, s32, out_mode, 0, 1)
         s = s.reshape(-1).to(t2d.dtype).contiguous()
         return self._run(t2d, group, 0, s, out_mode, t2d.shape[1] // group, 0)
@@ -127,15 +155,16 @@ class FloatQuantizer(BaseQuantizer):
         return reshaped, scales, torch.tensor(0.0), self.qmax, self.qmin
 
     def quant(self, tensor, scales, zeros, qmax, qmin):
-        """quant.py:1061-1072 -> fp32 tensor of grid values."""
+        """quant.py:1061-1072 -> fp32 tensor of grid values (zero scales set to 1 in place)."""
+        _zeros_to_one(scales)
         return self._static(tensor, scales, 2).float().reshape(tensor.shape)
 
     def dequant(self, tensor, scales, zeros):
         return (tensor - zeros) * scales
 
     def quant_dequant(self, tensor, scales, zeros, qmax, qmin):
-        """quant.py:1078-1081 (result dtype: fp32 * T -> fp32, callers cast back)."""
-        return self._static(tensor, scales, 1).reshape(tensor.shape)
+        """quant.py:1078-1081: the fp32 grid values times the scales -> fp32 (callers cast back)."""
+        return self.dequant(self.quant(tensor, scales, zeros, qmax, qmin), scales, zeros)
 
     def fake_quant_weight_dynamic(self, weight, args={}):
         """quant.py:1142-1159."""
@@ -149,7 +178,7 @@ class FloatQuantizer(BaseQuantizer):
         """quant.py:1111-1140."""
         tr = 'dim' in args and 'ic' in args['dim']
         w = weight.T if tr else weight
-        out = self._static(w, args['scales'], 1).reshape(w.shape).to(w.dtype)
+        out = self._static(w, _zeros_to_one(args['scales']), 1).reshape(w.shape).to(w.dtype)
         return out.T if tr else out
 
     def fake_quant_act_dynamic(self, act, args={}):
@@ -159,7 +188,7 @@ class FloatQuantizer(BaseQuantizer):
 
     def fake_quant_act_static(self, act, args={}):
         """quant.py:1083-1098."""
-        return self._static(act, args['scales'], 1).reshape(act.shape).to(act.dtype)
+        return self._static(act, _zeros_to_one(args['scales']), 1).reshape(act.shape).to(act.dtype)
 
     def _qshape(self, weight, scales):
         if self.granularity == 'per_tensor':
@@ -177,7 +206,7 @@ class FloatQuantizer(BaseQuantizer):
     def real_quant_weight_static(self, weight, args):
         """quant.py:1161-1193."""
         osf = args.pop('output_scale_factor', 1) if 'output_scale_factor' in args else 1
-        out = self._static(weight, args['scales'], 2)
+        out = self._static(weight, _zeros_to_one(args['scales']), 2)
         return out.reshape(weight.shape), self._qshape(weight, args['scales'] * osf), None
 
     def __repr__(self):

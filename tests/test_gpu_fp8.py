@@ -44,7 +44,7 @@ def test_fp8_static_act_per_tensor():
     maxs = torch.stack([x[i].max().float() for i in range(4)]).mean()
     s = torch.max(maxs.abs(), mins.abs()).clamp(min=1e-5) / torch.tensor(448.0)
     assert torch.allclose(sc[0].cpu().float(), s, rtol=1e-6)
-    yo = ((fo.quant(x, sc[0].cpu(), 'e4m3')) * sc[0].cpu()).to(x.dtype)
+    yo = fo.fake_quant_static(x, sc[0].cpu().clone(), 'e4m3', 'per_tensor')
     assert torch.equal(y.cpu(), yo)
 
 
