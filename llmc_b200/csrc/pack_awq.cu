@@ -6,13 +6,17 @@
 // transposes to [C, R] and ORs 8 nibbles per int32 along R in the order {0,2,4,6,1,3,5,7}.
 //
 // One CTA handles a 256(R) x 64(C) tile: coalesced 128-byte reads along C, a transposing
-// shared-memory stage of int8 codes, coalesced 128-byte writes of 32 packed words along R/8.
+// shared-memory stage of int32 codes, coalesced 128-byte writes of 32 packed words along R/8.
+// The codes are staged whole: without a clamp they can leave [0, 15] (and int8), and every bit
+// of a code reaches the word, as the reference's int32 shift + OR does.
 #include "common.cuh"
 
 namespace llmc {
 
 constexpr int kTileR = 256;
 constexpr int kTileC = 64;
+constexpr int kStageRow = kTileR + 1;    // odd row stride: phase 1's column writes hit 32 banks
+constexpr int kStageBytes = kTileC * kStageRow * 4;
 
 // torch promotes (weight dtype, fp16 scales): fp16 stays fp16, bf16/fp32 compute in fp32.
 template <int WT>
@@ -20,7 +24,8 @@ __global__ void __launch_bounds__(256)
 pack_awq_kernel(const void* __restrict__ w, int64_t R, int64_t C, const void* __restrict__ scales,
                 int s_dtype, const int32_t* __restrict__ zeros, int64_t group, int64_t ng,
                 int32_t* __restrict__ qweight) {
-  __shared__ int8_t codes[kTileC][kTileR + 4];
+  extern __shared__ int32_t stage[];
+  int32_t (*codes)[kStageRow] = reinterpret_cast<int32_t (*)[kStageRow]>(stage);
   const int64_t r0 = static_cast<int64_t>(blockIdx.y) * kTileR;
   const int64_t c0 = static_cast<int64_t>(blockIdx.x) * kTileC;
   // phase 1: thread t -> (row = r0 + t/64*?...) ; 256 threads cover 4 rows x 64 cols per step
@@ -45,7 +50,7 @@ pack_awq_kernel(const void* __restrict__ w, int64_t R, int64_t C, const void* __
       }
       v = static_cast<int>(rintf(q));
     }
-    codes[tc][rr] = static_cast<int8_t>(v);
+    codes[tc][rr] = v;
   }
   __syncthreads();
   // phase 2: 64 output rows (c) x 32 words (r/8); thread t -> word (c = t/32 + 8*k, wi = t%32)
@@ -104,7 +109,9 @@ extern "C" int llmc_pack_awq(const void* w, int64_t R, int64_t C, int dtype, con
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   const int64_t ng = C / group;
   dim3 grid((unsigned)((C + kTileC - 1) / kTileC), (unsigned)((R + kTileR - 1) / kTileR));
-#define CALL(DT) pack_awq_kernel<DT><<<grid, 256, 0, st>>>(w, R, C, scales, s_dtype, zeros, group, ng, qweight)
+#define CALL(DT)                                                                                \
+  if (int rc = opt_in_smem(pack_awq_kernel<DT>, kStageBytes)) return rc;                         \
+  pack_awq_kernel<DT><<<grid, 256, kStageBytes, st>>>(w, R, C, scales, s_dtype, zeros, group, ng, qweight)
   LLMC_DISPATCH_DT("pack_awq", dtype, CALL);
 #undef CALL
   LLMC_CHECK_LAUNCH();

@@ -25,6 +25,16 @@ from .blockwise import ALGO_REGISTRY, BaseBlockwiseQuantization
 from .module_utils import _LLMC_LINEAR_TYPES_, _TRANSFORMERS_LINEAR_TYPES_, FakeQuantLinear
 
 
+def norm_into(ln, src, dst):
+    """dst <- ln(src): the fused RMSNorm kernel when `ln` is an RMSNorm it can run (8-wide rows,
+    weight in the activations' dtype), else the module itself."""
+    if hasattr(ln, 'variance_epsilon') and src.shape[-1] % 8 == 0 and ln.weight.dtype == src.dtype:
+        from . import block_ops
+        block_ops.rmsnorm(src, ln.weight.data, ln.variance_epsilon, out=dst)
+    else:
+        dst.copy_(ln(src))
+
+
 @ALGO_REGISTRY
 class GPTQ(BaseBlockwiseQuantization):
     def __init__(self, model, quant_config, input, padding_mask, config, modality='language'):
@@ -231,12 +241,6 @@ class GPTQ(BaseBlockwiseQuantization):
                 yield slice(i, min(i + chunk, N))
 
         from . import block_ops
-
-        def norm_into(ln, src, dst):
-            if hasattr(ln, 'variance_epsilon') and src.shape[-1] % 8 == 0 and ln.weight.dtype == src.dtype:
-                block_ops.rmsnorm(src, ln.weight.data, ln.variance_epsilon, out=dst)
-            else:
-                dst.copy_(ln(src))
 
         x1 = torch.empty_like(X)
         for s in chunks():

@@ -118,7 +118,8 @@ class LlamaMLP(nn.Module):
         self.down_proj = B200Linear(inter, hidden, bias=False)
 
     def act(self, g, u, out=None):
-        if g.is_cuda and g.is_contiguous() and u.is_contiguous() and g.numel() % 8 == 0:
+        if (g.is_cuda and g.is_contiguous() and u.is_contiguous() and u.dtype == g.dtype
+                and g.numel() % 8 == 0):
             from . import block_ops
             return block_ops.silu_mul(g, u, out=out)
         y = F.silu(g) * u
