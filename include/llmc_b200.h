@@ -467,6 +467,34 @@ int llmc_gemm_fp8a16_gidx(const void* x, const int32_t* wq, const void* scales, 
                           int qparam_dtype, const int32_t* g_idx, int64_t ng, int q_transposed,
                           const void* bias, void* y, int64_t M, int64_t N, int64_t K, int dtype,
                           int e5m2, void* stream);
+/* llmc_gemm_w2a16 / llmc_gemm_w3a16 (+ _gidx) — the same fused forward for INT2 / INT3 weights
+ *   (the W2A16 g64 / W3A16 g128 AWQ recipes, GPTQ at 2 or 3 bits), arguments and rules as
+ *   llmc_gemm_w4a16 / llmc_gemm_w4a16_gidx; UNSIGNED codes, zeros NULL -> 2 (W2) / 4 (W3).
+ *   W2: wq [N, K/16] int32, LLMC_OUT_PACK_VLLM (code i of word w = element 16w + i, bits 2i..2i+1).
+ *   W3: wq [ceil(N/2), 12*K/64] int32 — rows 2r and 2r+1 share a row: for each 64-column step s,
+ *       words 12s..12s+5 hold row 2r, 12s+6..12s+11 row 2r+1 (an odd N pads a zero row).  A row's
+ *       six words of a step: word l < 4 the low two bits of codes 16l..16l+15 (code 16l+i in bits
+ *       2i..2i+1), word 4+m the third bits of codes 32m..32m+31 (code 32m+c at bit c with bits 3
+ *       and 4 of c swapped).  Exactly 3 bits per code; llmc_pack_w3_codes writes it.
+ *   Bit for bit llmc_gemm_bf16 on the materialised weight rT((code - zero) * scale). */
+int llmc_gemm_w2a16(const void* x, const int32_t* wq, const void* scales, const void* zeros,
+                    int qparam_dtype, const void* bias, void* y, int64_t M, int64_t N, int64_t K,
+                    int64_t group, int dtype, void* stream);
+int llmc_gemm_w3a16(const void* x, const int32_t* wq, const void* scales, const void* zeros,
+                    int qparam_dtype, const void* bias, void* y, int64_t M, int64_t N, int64_t K,
+                    int64_t group, int dtype, void* stream);
+int llmc_gemm_w2a16_gidx(const void* x, const int32_t* wq, const void* scales, const void* zeros,
+                         int qparam_dtype, const int32_t* g_idx, int64_t ng, int q_transposed,
+                         const void* bias, void* y, int64_t M, int64_t N, int64_t K, int dtype,
+                         void* stream);
+int llmc_gemm_w3a16_gidx(const void* x, const int32_t* wq, const void* scales, const void* zeros,
+                         int qparam_dtype, const int32_t* g_idx, int64_t ng, int q_transposed,
+                         const void* bias, void* y, int64_t M, int64_t N, int64_t K, int dtype,
+                         void* stream);
+/* llmc_pack_w3_codes — the W3 layout above from SIGNED int32 codes [rows, cols] (code - 4 for an
+ *   asymmetric grid, as llmc_pack_vllm_codes takes them), stored as code + 4:
+ *   out [ceil(rows/2), 12*cols/64] int32; cols % 64 == 0. */
+int llmc_pack_w3_codes(const int32_t* codes, int64_t rows, int64_t cols, int32_t* out, void* stream);
 
 #ifdef __cplusplus
 }

@@ -89,6 +89,15 @@ SIGNATURES = {
                                  c_int, c_int, c_vp]),
     'llmc_gemm_fp8a16_gidx': (c_int, [c_vp, c_vp, c_vp, c_vp, c_int, c_vp, c_i64, c_int, c_vp, c_vp, c_i64,
                                       c_i64, c_i64, c_int, c_int, c_vp]),
+    'llmc_gemm_w2a16': (c_int, [c_vp, c_vp, c_vp, c_vp, c_int, c_vp, c_vp, c_i64, c_i64, c_i64, c_i64,
+                                c_int, c_vp]),
+    'llmc_gemm_w3a16': (c_int, [c_vp, c_vp, c_vp, c_vp, c_int, c_vp, c_vp, c_i64, c_i64, c_i64, c_i64,
+                                c_int, c_vp]),
+    'llmc_gemm_w2a16_gidx': (c_int, [c_vp, c_vp, c_vp, c_vp, c_int, c_vp, c_i64, c_int, c_vp, c_vp, c_i64,
+                                     c_i64, c_i64, c_int, c_vp]),
+    'llmc_gemm_w3a16_gidx': (c_int, [c_vp, c_vp, c_vp, c_vp, c_int, c_vp, c_i64, c_int, c_vp, c_vp, c_i64,
+                                     c_i64, c_i64, c_int, c_vp]),
+    'llmc_pack_w3_codes': (c_int, [c_vp, c_i64, c_i64, c_vp, c_vp]),
 }
 
 _lock = threading.Lock()

@@ -303,14 +303,14 @@ class BaseBlockwiseQuantization(BlockwiseOpt):
 
     def w_packed(self, module, wquantizer):
         """K6 hand-off for EffcientFakeQuantLinear: the packed form of exactly what `w_qdq` would
-        materialise, or None when this layer / quantizer is not a plain INT4 / INT8 group or channel
-        weight quantizer (then the wrapper materialises as before)."""
+        materialise, or None when this layer / quantizer is not a plain INT2 / INT3 / INT4 / INT8 group or
+        channel weight quantizer (then the wrapper materialises as before)."""
         from .module_utils import pack_unsigned_codes
         from .quant_float import FloatQuantizer
         q, w = wquantizer, module.weight
         if isinstance(q, FloatQuantizer):
             return self._fp8_packed(module, q)
-        if not (isinstance(q, IntegerQuantizer) and q.bit in (4, 8) and q.calib_algo == 'minmax'
+        if not (isinstance(q, IntegerQuantizer) and q.bit in (2, 3, 4, 8) and q.calib_algo == 'minmax'
                 and q.granularity in ('per_group', 'per_channel') and q.round_zp
                 and w.dim() == 2 and w.is_cuda and w.dtype in (torch.float16, torch.bfloat16)):
             return None

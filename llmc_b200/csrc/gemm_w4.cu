@@ -1,5 +1,5 @@
-// gemm_w4.cu — K6: fake-quant forward on PACKED INT4 / INT8 weights, dequantisation fused into
-// the wgmma operand pipeline.
+// gemm_w4.cu — K6: fake-quant forward on PACKED INT2 / INT3 / INT4 / INT8 weights, dequantisation
+// fused into the wgmma operand pipeline.
 //
 //   Y[M,N] = X[M,K] . dequant(Wq)[N,K]^T (+ bias),   dequant(n,k) = rT( fp32((code - zero) * scale) )
 //
@@ -42,6 +42,25 @@
 // word layout).  Per element: byte -> fp32 (exact, every e4m3 / e5m2 value is an fp16 value),
 // fmul_rn(q, s) with s = 1 where the scale is 0 (quant.py:1062), one rounding to bf16 / fp16 —
 // fp8_emit's QDQ value (csrc/fp8.cu) from the bytes of its byte mode.  No zero-point.
+//
+// INT2 / INT3 weights (kBits 2, 3): the same rings, consumers, epilogue and tile order; only the
+// packed tile and its decode differ.  Both dequant a row's 64 codes of a step as four pair words
+// u(l, j) = code 16l + j in bits 0..2 and code 16l + j + 8 in bits 16..18 (l = 0..3, j = 0..7), so
+// the native-qparam path is the INT4 one — (magic | u) as half2 / bf16x2, one HSUB2 + one HMUL2 —
+// and the fp32 path lifts each half to 0x4B0000nn = 2^23 + code with one byte-permute.
+//   W2: LLMC_OUT_PACK_VLLM, 16 codes per int32 along K, code i of word w (element 16w + i) in bits
+//       2i..2i+1: wq [N, K/16], TMA box [128 rows, 4 words] = 16 B per row, no swizzle (a thread's
+//       16-byte row read is already conflict-free).
+//   W3: 64 codes are 24 B, and a TMA box row must be a multiple of 16 B, so rows 2r and 2r+1 share
+//       one tensor row: wq [ceil(N/2), 12 K/64] int32, words 12 s .. 12 s + 11 = K step s of row 2r
+//       (6 words) then of row 2r+1 (6 words); an odd N pads one all-zero row.  Box [64 row pairs,
+//       12 words] = 48 B, no swizzle; in shared memory row r's 24 bytes of the step sit at 24 r.
+//       The 6 words of a row's step: words 0..3 the low two bits of codes 0..63 in the W2 layout
+//       (code 16l + i in bits 2i..2i+1 of word l), words 4, 5 the third bit of codes 0..31 and
+//       32..63: code 32m + c at bit c' of word 4 + m, c' = c with its bits 3 and 4 swapped (an
+//       involution), so that one shift and one AND move the third bits of codes 16l + j and
+//       16l + j + 8 under bits 2 and 18 of u(l, j).  Exactly 3 bits per code (plus the odd-N row);
+//       llmc_pack_w3_codes writes it.
 #include <stdlib.h>
 
 #include <cuda_fp8.h>
@@ -60,7 +79,7 @@ constexpr int kBBytes = BN * BK * 2;          // 16 KB dequantised
 constexpr int NG = 2;                         // dequant groups of four warps
 // the weight grid: integer codes, or e4m3 / e5m2 bytes (8-bit words, no zero-point)
 enum : int { kGridInt = 0, kGridE4M3 = 1, kGridE5M2 = 2 };
-// per weight width: INT4 -> 4 KB packed tile, INT8 -> 8 KB
+// per weight width: INT2 / INT3 / INT4 -> 2 / 3 / 4 KB packed tile, INT8 -> 8 KB
 template <int kBits> struct Cfg {
   static constexpr int kPBytes = BN * BK * kBits / 8;
   static constexpr int kLBytes = kABytes + kPBytes;
@@ -68,6 +87,7 @@ template <int kBits> struct Cfg {
   static constexpr int kLStages = 6;
   static constexpr int kSmemBytes = ring_smem_bytes(kLStages * kLBytes + kBStages * kBBytes);
   static constexpr int kWordsPerRow = BK * kBits / 32;      // int32 per row of the packed tile
+  static constexpr int kPackRows = kBits == 3 ? 2 : 1;      // weight rows per row of the packed tensor
   static constexpr int kDequantWarps = 4 * NG;
   static constexpr int kConsumerWarp0 = kDequantWarps;      // first warp of the consumer warpgroups
   static constexpr int kTmaWarp = kDequantWarps + 8;
@@ -123,6 +143,34 @@ __device__ __forceinline__ void fp8x4_to_f32(uint32_t w, float* f) {
 // quant.py:1062: a zero scale dequantises with 1
 __device__ __forceinline__ float fp8_scale(float s) { return s == 0.f ? 1.f : s; }
 
+// W2 / W3: a row's words of one K step in the packed tile (header: 4 words of 2-bit planes, W3 two
+// more of third bits).  W3 rows are 24 bytes apart, so the row is read as three 8-byte halves.
+template <int kBits>
+__device__ __forceinline__ void load_lowbit_row(const uint8_t* pk, int row, uint32_t* w) {
+  if constexpr (kBits == 2) {
+    const uint4 v = *reinterpret_cast<const uint4*>(pk + row * 16);
+    w[0] = v.x; w[1] = v.y; w[2] = v.z; w[3] = v.w;
+  } else {
+    const uint2 a = *reinterpret_cast<const uint2*>(pk + row * 24);
+    const uint2 b = *reinterpret_cast<const uint2*>(pk + row * 24 + 8);
+    const uint2 c = *reinterpret_cast<const uint2*>(pk + row * 24 + 16);
+    w[0] = a.x; w[1] = a.y; w[2] = b.x; w[3] = b.y; w[4] = c.x; w[5] = c.y;
+  }
+}
+
+// u(l, j): code 16l + j in bits 0..2, code 16l + j + 8 in bits 16..18 (l, j compile-time after unrolling)
+template <int kBits>
+__device__ __forceinline__ uint32_t lowbit_pair(const uint32_t* w, int l, int j) {
+  uint32_t u = (w[l] >> (2 * j)) & 0x00030003u;
+  if constexpr (kBits == 3) {
+    // third bits of codes 16l + j and 16l + j + 8 sit at bits 8(l & 1) + j and 16 + 8(l & 1) + j
+    const int sh = 8 * (l & 1) + j - 2;
+    const uint32_t h = sh >= 0 ? w[4 + (l >> 1)] >> sh : w[4 + (l >> 1)] << -sh;
+    u = and_or(h, 0x00040004u, u);
+  }
+  return u;
+}
+
 template <bool kBf16, int kBits, bool kGidx, int kGrid>
 __global__ void __launch_bounds__(Cfg<kBits>::kThreads, 1)
 w4a16_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmP,
@@ -161,7 +209,8 @@ w4a16_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
           uint8_t* p_dst = a_dst + kABytes;
           ring_l.expect_tx(sl, kLBytes);
           tma_load_2d(a_dst, &tmA, &ring_l.full[sl.stage], kb * BK, m_blk * BM);
-          tma_load_2d(p_dst, &tmP, &ring_l.full[sl.stage], kb * C::kWordsPerRow, n_blk * BN);
+          tma_load_2d(p_dst, &tmP, &ring_l.full[sl.stage], kb * C::kWordsPerRow * C::kPackRows,
+                      n_blk * (BN / C::kPackRows));
           sl.advance();
         }
       }
@@ -262,7 +311,8 @@ w4a16_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
         const float zm_cur = 8388608.0f + z_c;        // (2^23 + q) - (2^23 + z) = q - z exactly
         const float s_c = (n0 < p.N) ? widen(s_cur) : 0.f;
         if constexpr (kGidx) {
-          // this row's packed words of the step, unswizzled: word w holds elements 32/kBits * w ..
+          // this row's packed words of the step, unswizzled (W4 / W8: word w holds elements 32/kBits * w ..;
+          // W2 / W3: the words of load_lowbit_row)
           constexpr int kWords = BK * kBits / 32;
           uint32_t words[kWords];
           if constexpr (kBits == 8) {
@@ -272,12 +322,14 @@ w4a16_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
               const uint4 wv = *reinterpret_cast<const uint4*>(pk + row * 64 + ((c4 ^ sw8) << 4));
               words[4 * c4] = wv.x; words[4 * c4 + 1] = wv.y; words[4 * c4 + 2] = wv.z; words[4 * c4 + 3] = wv.w;
             }
-          } else {
+          } else if constexpr (kBits == 4) {
             const int sw = ((row >> 2) & 1) << 4;
             const uint4 w0 = *reinterpret_cast<const uint4*>(pk + row * 32 + sw);
             const uint4 w1 = *reinterpret_cast<const uint4*>(pk + row * 32 + (sw ^ 16));
             words[0] = w0.x; words[1] = w0.y; words[2] = w0.z; words[3] = w0.w;
             words[4] = w1.x; words[5] = w1.y; words[6] = w1.z; words[7] = w1.w;
+          } else {
+            load_lowbit_row<kBits>(pk, row, words);
           }
           const int4* gk = reinterpret_cast<const int4*>(p.g_idx + static_cast<int64_t>(kb) * BK);
 #pragma unroll
@@ -297,8 +349,10 @@ w4a16_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
             } else {
 #pragma unroll
               for (int e = 0; e < 8; ++e) {
-                const uint32_t q = kBits == 8 ? (words[2 * c + e / 4] >> (8 * (e % 4))) & 0xFFu
-                                              : (words[c] >> (4 * e)) & 0xFu;
+                uint32_t q;
+                if constexpr (kBits == 8) q = (words[2 * c + e / 4] >> (8 * (e % 4))) & 0xFFu;
+                else if constexpr (kBits == 4) q = (words[c] >> (4 * e)) & 0xFu;
+                else q = (lowbit_pair<kBits>(words, c >> 1, e) >> (16 * (c & 1))) & 0xFFFFu;   // element 8c + e
                 const float zm = 8388608.0f + (have_zeros ? widen(zr[e]) : p.zero_default);
                 v[e] = fmul_rn(__uint_as_float(0x4B000000u | q) - zm, widen(sr[e]));
               }
@@ -342,6 +396,46 @@ w4a16_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
                                          pack_pair<DT>(v[4], v[5]), pack_pair<DT>(v[6], v[7]));
               const int c = c4 * 2 + hh;
               *reinterpret_cast<uint4*>(bt + row * 128 + ((c ^ (row & 7)) << 4)) = o;
+            }
+          }
+        } else if constexpr (kBits < 4) {
+          // INT2 / INT3: pair word u(l, j) -> output chunk 2l from its low halves (elements
+          // 16l .. 16l+7), chunk 2l+1 from its high halves (16l+8 .. 16l+15)
+          uint32_t words[C::kWordsPerRow];
+          load_lowbit_row<kBits>(pk, row, words);
+          if (p.qparam_native) {
+            // as INT4: (magic | u) - (magic + z) is exact, times s rounds once
+            constexpr uint32_t kMagic2 = kBf16 ? 0x43004300u : 0x64006400u;
+            const uint32_t s2 = pack_pair<DT>(s_c, s_c);
+            const uint32_t zm2 = pack_pair<DT>((kBf16 ? 128.f : 1024.f) + z_c, (kBf16 ? 128.f : 1024.f) + z_c);
+#pragma unroll
+            for (int l = 0; l < 4; ++l) {
+              uint32_t r[8];
+#pragma unroll
+              for (int j = 0; j < 8; ++j) r[j] = sub_mul2<kBf16>(lowbit_pair<kBits>(words, l, j) | kMagic2, zm2, s2);
+              const uint4 o0 = make_uint4(__byte_perm(r[0], r[1], 0x5410), __byte_perm(r[2], r[3], 0x5410),
+                                          __byte_perm(r[4], r[5], 0x5410), __byte_perm(r[6], r[7], 0x5410));
+              const uint4 o1 = make_uint4(__byte_perm(r[0], r[1], 0x7632), __byte_perm(r[2], r[3], 0x7632),
+                                          __byte_perm(r[4], r[5], 0x7632), __byte_perm(r[6], r[7], 0x7632));
+              *reinterpret_cast<uint4*>(bt + row * 128 + (((2 * l) ^ (row & 7)) << 4)) = o0;
+              *reinterpret_cast<uint4*>(bt + row * 128 + (((2 * l + 1) ^ (row & 7)) << 4)) = o1;
+            }
+          } else {
+#pragma unroll
+            for (int l = 0; l < 4; ++l) {
+              float v[16];
+#pragma unroll
+              for (int j = 0; j < 8; ++j) {
+                const uint32_t u = lowbit_pair<kBits>(words, l, j);
+                v[j] = fmul_rn(__uint_as_float(__byte_perm(u, 0x4B000000u, 0x7650u)) - zm_cur, s_c);
+                v[8 + j] = fmul_rn(__uint_as_float(__byte_perm(u, 0x4B000000u, 0x7652u)) - zm_cur, s_c);
+              }
+              const uint4 o0 = make_uint4(pack_pair<DT>(v[0], v[1]), pack_pair<DT>(v[2], v[3]),
+                                          pack_pair<DT>(v[4], v[5]), pack_pair<DT>(v[6], v[7]));
+              const uint4 o1 = make_uint4(pack_pair<DT>(v[8], v[9]), pack_pair<DT>(v[10], v[11]),
+                                          pack_pair<DT>(v[12], v[13]), pack_pair<DT>(v[14], v[15]));
+              *reinterpret_cast<uint4*>(bt + row * 128 + (((2 * l) ^ (row & 7)) << 4)) = o0;
+              *reinterpret_cast<uint4*>(bt + row * 128 + (((2 * l + 1) ^ (row & 7)) << 4)) = o1;
             }
           }
         } else {
@@ -439,12 +533,16 @@ static int gemm_wNa16(const void* x, const int32_t* wq, const void* scales, cons
   }
   using C = Cfg<kBits>;
   constexpr int wpr = C::kWordsPerRow;
+  constexpr int pr = C::kPackRows;
+  // W4 / W8 rows are 32 / 64 B and TMA-swizzled; the 16-byte W2 rows and 48-byte W3 row pairs are not
+  constexpr CUtensorMapSwizzle swz = kBits == 4 ? CU_TENSOR_MAP_SWIZZLE_32B
+                                     : kBits == 8 ? CU_TENSOR_MAP_SWIZZLE_64B : CU_TENSOR_MAP_SWIZZLE_NONE;
   CUtensorMap tmA, tmP;
   if (int rc = encode_tmap_2d(&tmA, x, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, M, K, K, BM, BK,
                               CU_TENSOR_MAP_SWIZZLE_128B))
     return rc;
-  if (int rc = encode_tmap_2d(&tmP, wq, CU_TENSOR_MAP_DATA_TYPE_INT32, 4, N, K * kBits / 32, K * kBits / 32,
-                              BN, wpr, kBits == 4 ? CU_TENSOR_MAP_SWIZZLE_32B : CU_TENSOR_MAP_SWIZZLE_64B))
+  if (int rc = encode_tmap_2d(&tmP, wq, CU_TENSOR_MAP_DATA_TYPE_INT32, 4, (N + pr - 1) / pr, K * kBits / 32 * pr,
+                              K * kBits / 32 * pr, BN / pr, wpr * pr, swz))
     return rc;
   Params p{};
   p.M = M; p.N = N; p.K = K; p.out = y; p.bias = bias;
@@ -512,6 +610,90 @@ extern "C" int llmc_gemm_w8a16_gidx(const void* x, const int32_t* wq, const void
   LLMC_CHECK_ARG(g_idx != nullptr, "gemm_w8a16_gidx: g_idx is NULL");
   return gemm_wNa16<8>(x, wq, scales, zeros, qparam_dtype, bias, y, M, N, K, 0, g_idx, ng, dtype,
                        q_transposed, stream, "gemm_w8a16_gidx");
+}
+
+// INT2 weights: wq [N, K/16] (LLMC_OUT_PACK_VLLM, zeros NULL => 2); INT3 weights: wq
+// [ceil(N/2), 12 K/64] in the row-pair layout of the header (llmc_pack_w3_codes, zeros NULL => 4).
+// Otherwise as llmc_gemm_w4a16 / llmc_gemm_w4a16_gidx.
+extern "C" int llmc_gemm_w2a16(const void* x, const int32_t* wq, const void* scales,
+                               const void* zeros, int qparam_dtype, const void* bias, void* y,
+                               int64_t M, int64_t N, int64_t K, int64_t group, int dtype,
+                               void* stream) {
+  return gemm_wNa16<2>(x, wq, scales, zeros, qparam_dtype, bias, y, M, N, K, group < 0 ? -group : group,
+                       nullptr, 0, dtype, group < 0, stream, "gemm_w2a16");
+}
+
+extern "C" int llmc_gemm_w3a16(const void* x, const int32_t* wq, const void* scales,
+                               const void* zeros, int qparam_dtype, const void* bias, void* y,
+                               int64_t M, int64_t N, int64_t K, int64_t group, int dtype,
+                               void* stream) {
+  return gemm_wNa16<3>(x, wq, scales, zeros, qparam_dtype, bias, y, M, N, K, group < 0 ? -group : group,
+                       nullptr, 0, dtype, group < 0, stream, "gemm_w3a16");
+}
+
+extern "C" int llmc_gemm_w2a16_gidx(const void* x, const int32_t* wq, const void* scales,
+                                    const void* zeros, int qparam_dtype, const int32_t* g_idx,
+                                    int64_t ng, int q_transposed, const void* bias, void* y,
+                                    int64_t M, int64_t N, int64_t K, int dtype, void* stream) {
+  LLMC_CHECK_ARG(g_idx != nullptr, "gemm_w2a16_gidx: g_idx is NULL");
+  return gemm_wNa16<2>(x, wq, scales, zeros, qparam_dtype, bias, y, M, N, K, 0, g_idx, ng, dtype,
+                       q_transposed, stream, "gemm_w2a16_gidx");
+}
+
+extern "C" int llmc_gemm_w3a16_gidx(const void* x, const int32_t* wq, const void* scales,
+                                    const void* zeros, int qparam_dtype, const int32_t* g_idx,
+                                    int64_t ng, int q_transposed, const void* bias, void* y,
+                                    int64_t M, int64_t N, int64_t K, int dtype, void* stream) {
+  LLMC_CHECK_ARG(g_idx != nullptr, "gemm_w3a16_gidx: g_idx is NULL");
+  return gemm_wNa16<3>(x, wq, scales, zeros, qparam_dtype, bias, y, M, N, K, 0, g_idx, ng, dtype,
+                       q_transposed, stream, "gemm_w3a16_gidx");
+}
+
+// ---- the INT3 weight layout (header): one thread per output word ----
+namespace llmc {
+namespace w4 {
+__global__ void __launch_bounds__(256)
+pack_w3_codes_kernel(const int32_t* __restrict__ codes, int64_t rows, int64_t cols, int32_t* __restrict__ out) {
+  const int64_t wpp = cols / BK * 12;                       // words per row pair
+  const int64_t total = (rows + 1) / 2 * wpp;
+  for (int64_t u = static_cast<int64_t>(blockIdx.x) * blockDim.x + threadIdx.x; u < total;
+       u += static_cast<int64_t>(gridDim.x) * blockDim.x) {
+    const int64_t pair = u / wpp, rem = u - pair * wpp;
+    const int64_t step = rem / 12;
+    const int w = static_cast<int>(rem % 12);
+    const int64_t r = 2 * pair + w / 6;
+    uint32_t word = 0;
+    if (r < rows) {
+      const int32_t* c = codes + r * cols + step * BK;
+      const int f = w % 6;
+      if (f < 4) {                                          // low two bits of codes 16f .. 16f + 15
+        for (int i = 0; i < 16; ++i) word |= (static_cast<uint32_t>(c[16 * f + i] + 4) & 3u) << (2 * i);
+      } else {                                              // third bits of codes 32m .. 32m + 31
+        const int m = f - 4;
+        for (int b = 0; b < 32; ++b) {
+          const int cc = (b & ~24) | ((b & 8) << 1) | ((b & 16) >> 1);   // b with bits 3 and 4 swapped
+          word |= ((static_cast<uint32_t>(c[32 * m + cc] + 4) >> 2) & 1u) << b;
+        }
+      }
+    }
+    out[u] = static_cast<int32_t>(word);
+  }
+}
+}  // namespace w4
+}  // namespace llmc
+
+// codes [rows, cols] int32, SIGNED (code - 4 for an asymmetric grid, as llmc_pack_vllm_codes takes
+// them); stored as code + 4 in 3 bits.  out [ceil(rows/2), 12 cols/64] int32.
+extern "C" int llmc_pack_w3_codes(const int32_t* codes, int64_t rows, int64_t cols, int32_t* out, void* stream) {
+  LLMC_CHECK_ARG(rows >= 0 && cols >= 0, "pack_w3_codes: bad shape");
+  LLMC_CHECK_ARG(cols % w4::BK == 0, "pack_w3_codes: cols=%lld must be a multiple of %d", (long long)cols, w4::BK);
+  if (rows == 0 || cols == 0) return LLMC_OK;
+  LLMC_CHECK_ARG(codes && out, "pack_w3_codes: null pointer");
+  int64_t blocks = ((rows + 1) / 2 * (cols / w4::BK * 12) + 255) / 256;
+  if (blocks > kNumSMs * 32) blocks = kNumSMs * 32;
+  w4::pack_w3_codes_kernel<<<(int)blocks, 256, 0, static_cast<cudaStream_t>(stream)>>>(codes, rows, cols, out);
+  LLMC_CHECK_LAUNCH();
+  return LLMC_OK;
 }
 
 // FP8 weights (e5m2 != 0: e5m2, else e4m3): wq = the fp8 bytes [N, K] viewed as int32 [N, K/4],

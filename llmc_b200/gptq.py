@@ -481,16 +481,16 @@ class GPTQ(BaseBlockwiseQuantization):
     def w_packed(self, module, wquantizer):
         """The packed form of exactly what `w_qdq` materialises, for EffcientFakeQuantLinear: codes of
         the calibrated fp32 weight (original column order) from the same static quantisation pass
-        w_qdq runs, packed for llmc_gemm_w4a16 / w8a16; qparams as GPTQ stores them (dynamic groups:
-        fp32 in the permuted group order; static groups and per-channel: the model dtype, original
-        order); `g_idx` = invperm // group_size when act-order reorders the groups.  None when the
+        w_qdq runs, packed for llmc_gemm_w2a16 / w3a16 / w4a16 / w8a16; qparams as GPTQ stores them
+        (dynamic groups: fp32 in the permuted group order; static groups and per-channel: the model
+        dtype, original order); `g_idx` = invperm // group_size when act-order reorders the groups.  None when the
         layer does not fit the packed GEMM; it is then materialised as before."""
         from .module_utils import pack_unsigned_codes
         from .quant import OUT_CODES_I32, IntegerQuantizer
         q, w = wquantizer, module.weight.data
         if self.float_grid:
             return self._fp8_packed_static(module, q)
-        if not (isinstance(q, IntegerQuantizer) and q.bit in (4, 8) and q.calib_algo == 'minmax'
+        if not (isinstance(q, IntegerQuantizer) and q.bit in (2, 3, 4, 8) and q.calib_algo == 'minmax'
                 and q.granularity in ('per_group', 'per_channel') and q.round_zp
                 and w.dim() == 2 and w.is_cuda and w.is_floating_point()
                 and self.model_dtype in (torch.float16, torch.bfloat16)):

@@ -45,15 +45,27 @@ def linear_forward_w4(x, wq, scales, zeros, group, bias=None, bits=4, qparams_t=
     wq [N, K/8] int32 (unsigned codes, LLMC_OUT_PACK_VLLM layout), scales [N, K/group] in x.dtype
     or fp32, zeros likewise or None (None => 8, the symmetric +2^(bit-1) storage offset).
 
+    bits 2, 8: wq [N, K*bits/32] in the same layout.  bits 3: wq [ceil(N/2), 3K/16], the row-pair
+    layout of pack_unsigned_codes; N is then read from the 2-D scales ([N, ng], or [ng, N] with
+    qparams_t).
+
     g_idx: int32 [K] or None.  When given, column k uses the qparams of group g_idx[k] (GPTQ
     act-order: groups are contiguous in the permuted order, g_idx = invperm // group_size), the
     qparams hold ng = scales.numel() // N groups in any order, and `group` is ignored.  Every value
     must lie in [0, ng); the kernel does not check it."""
     require_cuda(x, wq, scales)
     K = x.shape[-1]
-    N = wq.shape[0]
-    assert bits in (4, 8)
-    assert wq.dtype == torch.int32 and wq.shape[1] * (32 // bits) == K, (wq.shape, K)
+    if bits not in (2, 3, 4, 8):
+        raise ValueError(f'packed weights are 2, 3, 4 or 8 bits, not {bits}')
+    if bits == 3:
+        if scales.dim() != 2:
+            raise ValueError('3-bit weights need 2-D scales to give N')
+        N = scales.shape[1] if qparams_t else scales.shape[0]
+        assert wq.dtype == torch.int32 and tuple(wq.shape) == ((N + 1) // 2, 3 * K // 16) and K % 64 == 0, \
+            (wq.shape, N, K)
+    else:
+        N = wq.shape[0]
+        assert wq.dtype == torch.int32 and wq.shape[1] * (32 // bits) == K, (wq.shape, K)
     x2 = x.reshape(-1, K)
     x2 = x2 if x2.is_contiguous() else x2.contiguous()
     # qparams already in the activation dtype (RTN / AWQ / exported checkpoints) take the packed
@@ -307,29 +319,55 @@ class FakeQuantLinear(nn.Module):
 
 def pack_unsigned_codes(codes, bits, signed):
     """[N, K] integer codes -> [N, K*bits/32] int32 of UNSIGNED codes, little-end first along K
-    (the weight layout of llmc_gemm_w4a16 / llmc_gemm_w8a16).  llmc_pack_vllm_codes adds the
+    (the weight layout of llmc_gemm_w2a16 / w4a16 / w8a16).  llmc_pack_vllm_codes adds the
     +2^(bits-1) storage offset of module_utils.py:842-844, so asymmetric (already unsigned) codes are
-    shifted down first."""
+    shifted down first.
+
+    bits 3: [ceil(N/2), 3K/16] int32 in the row-pair layout of llmc_gemm_w3a16 (llmc_pack_w3_codes;
+    include/llmc_b200.h), K a multiple of 64."""
     require_cuda(codes)
     c = codes.to(torch.int32)
     if not signed:
         c = c - (1 << (bits - 1))
     c = c.contiguous()
     rows, cols = c.shape
+    if bits == 3:
+        out = torch.empty(((rows + 1) // 2, 3 * cols // 16), dtype=torch.int32, device=c.device)
+        call('llmc_pack_w3_codes', ptr(c), rows, cols, ptr(out), stream_ptr(c.device))
+        return out
     pf = 32 // bits
     out = torch.empty((rows, cols // pf), dtype=torch.int32, device=c.device)
     call('llmc_pack_vllm_codes', ptr(c), 4, rows, cols, int(bits), ptr(out), stream_ptr(c.device))
     return out
 
 
+def unpack_unsigned_codes(packed, bits, rows):
+    """The inverse of pack_unsigned_codes: [rows, K] int32 unsigned codes (elementwise, exact)."""
+    if bits == 3:
+        P, W = packed.shape
+        steps = W // 12
+        # [pair, step, row of the pair, word] -> [row, step, word]
+        words = packed.reshape(P, steps, 2, 6).permute(0, 2, 1, 3).reshape(2 * P, steps, 6)[:rows]
+        i = torch.arange(16, device=packed.device, dtype=torch.int32)
+        lo = ((words[..., :4, None] >> (2 * i)) & 3).reshape(rows, steps, 64)
+        c = torch.arange(32, device=packed.device, dtype=torch.int32)
+        pos = (c & ~24) | ((c & 8) << 1) | ((c & 16) >> 1)      # code 32m + c at bit c with bits 3, 4 swapped
+        hi = ((words[..., 4:, None] >> pos) & 1).reshape(rows, steps, 64)
+        return (lo | (hi << 2)).reshape(rows, steps * 64)
+    pf = 32 // bits
+    sh = torch.arange(pf, device=packed.device, dtype=torch.int32) * bits
+    return ((packed.unsqueeze(-1) >> sh) & ((1 << bits) - 1)).reshape(packed.shape[0], -1)
+
+
 class EffcientFakeQuantLinear(nn.Module):
     """module_utils.py:681-759 — eval-time wrapper: w_qdq applied once in `new`.
 
-    Extension (K6): when the weight quantizer is a plain INT4 / INT8 group or channel
+    Extension (K6): when the weight quantizer is a plain INT2 / INT3 / INT4 / INT8 group or channel
     quantizer, `new` keeps the PACKED codes + group qparams instead of the dequantised weight and
     the forward runs the fused dequant -> wgmma GEMM (csrc/gemm_w4.cu) — bit-identical to F.linear
-    on the materialised weight (tests/test_gpu_gemm_w4.py), at 4.25 / 8.25 instead of 16 bits per
-    weight in HBM.  `.weight` then dequantises on demand.  LLMC_B200_FUSED_DEQUANT=0 disables it.
+    on the materialised weight (tests/test_gpu_gemm_w4.py, tests/test_gpu_gemm_w2w3.py), at e.g.
+    2.5 (W2 g64) / 3.25 (W3 g128) / 4.25 / 8.25 instead of 16 bits per weight in HBM.  `.weight`
+    then dequantises on demand.  LLMC_B200_FUSED_DEQUANT=0 disables it.
 
     The packed form comes from the algorithm's `w_packed` twin of its `w_qdq` (RTN / AWQ: the base
     one; GPTQ: GPTQ.w_packed).  Its qparams keep the dtype the algorithm stores them in — fp32 for
@@ -390,9 +428,8 @@ class EffcientFakeQuantLinear(nn.Module):
             s = s.masked_fill(s == 0, 1.0)
             s = s[:, self.g_idx.long()] if self.g_idx is not None else s.repeat_interleave(self.q_group, dim=1)
             return (self.qweight.float() * s).to(self.q_dtype)
-        bits, pf = self.q_bits, 32 // self.q_bits
-        sh = torch.arange(pf, device=self.qweight.device, dtype=torch.int32) * bits
-        codes = ((self.qweight.unsqueeze(-1) >> sh) & ((1 << bits) - 1)).reshape(self.qweight.shape[0], -1)
+        bits = self.q_bits
+        codes = unpack_unsigned_codes(self.qweight, bits, self.qscales.shape[0])
         N, K = codes.shape
         z = self.qzeros if self.qzeros is not None else float(1 << (bits - 1))
         s = self.qscales
