@@ -495,6 +495,41 @@ int llmc_gemm_w3a16_gidx(const void* x, const int32_t* wq, const void* scales, c
  *   asymmetric grid, as llmc_pack_vllm_codes takes them), stored as code + 4:
  *   out [ceil(rows/2), 12*cols/64] int32; cols % 64 == 0. */
 int llmc_pack_w3_codes(const int32_t* codes, int64_t rows, int64_t cols, int32_t* out, void* stream);
+/* llmc_gemm_w2a16_rz / w3a16_rz / w4a16_rz / w8a16_rz — the same fused forward with REAL-VALUED
+ *   zero-points (HQQ, SpQR: round_zp False), fp32 qparams only:
+ *   dequant(Wq)[n,k] = rT(fmul_rn(fsub_rn(code, z), s)) in fp32, one rounding to `dtype` — the value
+ *   of quant.py:710-717 followed by .to(dtype).  code = the stored unsigned code, minus 2^(bit-1)
+ *   when sym != 0 (the code is exact; the zero-point is never shifted); zeros NULL -> z = 0.
+ *   wq      the layout of each width: W2 / W4 / W8 [N, K*bit/32] LLMC_OUT_PACK_VLLM, W3 the row-pair
+ *           layout of llmc_gemm_w3a16
+ *   group_axis 0 (groups along K; HQQ axis 1, SpQR): column k uses group g_idx[k] of ng:
+ *           scales / zeros [ng, N] fp32, s = scales[g_idx[k] * N + n]; g_idx [K] int32 required,
+ *           16-byte aligned, 0 <= g_idx[k] < ng (not checked on the device), 1 <= ng <= K;
+ *           contiguous groups pass g_idx[k] = k / group.  `group` is ignored.
+ *   group_axis 1 (groups along N; HQQ axis 0, which quantises W^T): row n uses group n / group:
+ *           scales / zeros [K, N/group] fp32, s = scales[k * (N/group) + n / group] (HQQ's
+ *           buf_scales / buf_zeros as stored); N % group == 0.  g_idx and ng are ignored.
+ *   outlier_rows [N+1] int32, outlier_cols [nnz] int32 (ascending within a row, original column
+ *           order), outlier_vals [nnz] in `dtype`: CSR of weights kept unquantised (SpQR).  Each
+ *           value REPLACES its dequantised element.  All three or none (NULL).
+ *   Bit for bit llmc_gemm_bf16 on the materialised weight.  K % 64 == 0; argument errors are
+ *   returned before any launch. */
+int llmc_gemm_w2a16_rz(const void* x, const int32_t* wq, const float* scales, const float* zeros, int sym,
+                       int group_axis, int64_t group, const int32_t* g_idx, int64_t ng,
+                       const int32_t* outlier_rows, const int32_t* outlier_cols, const void* outlier_vals,
+                       const void* bias, void* y, int64_t M, int64_t N, int64_t K, int dtype, void* stream);
+int llmc_gemm_w3a16_rz(const void* x, const int32_t* wq, const float* scales, const float* zeros, int sym,
+                       int group_axis, int64_t group, const int32_t* g_idx, int64_t ng,
+                       const int32_t* outlier_rows, const int32_t* outlier_cols, const void* outlier_vals,
+                       const void* bias, void* y, int64_t M, int64_t N, int64_t K, int dtype, void* stream);
+int llmc_gemm_w4a16_rz(const void* x, const int32_t* wq, const float* scales, const float* zeros, int sym,
+                       int group_axis, int64_t group, const int32_t* g_idx, int64_t ng,
+                       const int32_t* outlier_rows, const int32_t* outlier_cols, const void* outlier_vals,
+                       const void* bias, void* y, int64_t M, int64_t N, int64_t K, int dtype, void* stream);
+int llmc_gemm_w8a16_rz(const void* x, const int32_t* wq, const float* scales, const float* zeros, int sym,
+                       int group_axis, int64_t group, const int32_t* g_idx, int64_t ng,
+                       const int32_t* outlier_rows, const int32_t* outlier_cols, const void* outlier_vals,
+                       const void* bias, void* y, int64_t M, int64_t N, int64_t K, int dtype, void* stream);
 
 #ifdef __cplusplus
 }

@@ -98,6 +98,14 @@ SIGNATURES = {
     'llmc_gemm_w3a16_gidx': (c_int, [c_vp, c_vp, c_vp, c_vp, c_int, c_vp, c_i64, c_int, c_vp, c_vp, c_i64,
                                      c_i64, c_i64, c_int, c_vp]),
     'llmc_pack_w3_codes': (c_int, [c_vp, c_i64, c_i64, c_vp, c_vp]),
+    'llmc_gemm_w2a16_rz': (c_int, [c_vp, c_vp, c_vp, c_vp, c_int, c_int, c_i64, c_vp, c_i64, c_vp, c_vp, c_vp,
+                                   c_vp, c_vp, c_i64, c_i64, c_i64, c_int, c_vp]),
+    'llmc_gemm_w3a16_rz': (c_int, [c_vp, c_vp, c_vp, c_vp, c_int, c_int, c_i64, c_vp, c_i64, c_vp, c_vp, c_vp,
+                                   c_vp, c_vp, c_i64, c_i64, c_i64, c_int, c_vp]),
+    'llmc_gemm_w4a16_rz': (c_int, [c_vp, c_vp, c_vp, c_vp, c_int, c_int, c_i64, c_vp, c_i64, c_vp, c_vp, c_vp,
+                                   c_vp, c_vp, c_i64, c_i64, c_i64, c_int, c_vp]),
+    'llmc_gemm_w8a16_rz': (c_int, [c_vp, c_vp, c_vp, c_vp, c_int, c_int, c_i64, c_vp, c_i64, c_vp, c_vp, c_vp,
+                                   c_vp, c_vp, c_i64, c_i64, c_i64, c_int, c_vp]),
 }
 
 _lock = threading.Lock()

@@ -356,8 +356,9 @@ class BaseBlockwiseQuantization(BlockwiseOpt):
             params['w_qdq'] = functools.partial(self.w_qdq, wquantizer=self.wquantizer)
             # the packed twin of w_qdq: only a class that defines w_qdq knows what it materialises,
             # so the packer is the `w_packed` that same class defines (the base one for RTN / AWQ,
-            # GPTQ's own, act-order included).  A subclass that overrides w_qdq without a w_packed
-            # of its own (SpQR's outlier columns, HQQ) keeps the materialised path.
+            # GPTQ's own, act-order included; HQQ's and SpQR's real-valued zero-points, SpQR's
+            # outliers included).  A subclass that overrides w_qdq without a w_packed of its own
+            # keeps the materialised path.
             owner = next(c for c in type(self).__mro__ if 'w_qdq' in c.__dict__)
             if 'w_packed' in owner.__dict__:
                 params['w_qdq'].packed = functools.partial(self.w_packed, wquantizer=self.wquantizer)

@@ -61,7 +61,23 @@
 //       involution), so that one shift and one AND move the third bits of codes 16l + j and
 //       16l + j + 8 under bits 2 and 18 of u(l, j).  Exactly 3 bits per code (plus the odd-N row);
 //       llmc_pack_w3_codes writes it.
+//
+// Real-valued zero-points (kRz, HQQ and SpQR: round_zp False): the group-index form's gather with
+// fp32 qparams only; rings, consumers, epilogue, K order and tile order are unchanged.  Per element
+// the code is recovered exactly (code - 2^(b-1) on a symmetric grid), then
+// rT(__fmul_rn(__fsub_rn(code, z), s)) — quant.py:710-717 in fp32, one rounding — where the 2^23
+// formula of the integer forms would round a fractional z.  The zero-point is never shifted.
+//   kRzK  groups along K: (s, z) = qparams[g_idx[k], n] of [ng, N] (contiguous groups pass k / group)
+//   kRzN  groups along N (HQQ axis 0, which quantises W^T): (s, z) = qparams[k, n / g] of [K, N/g],
+//         HQQ's buffers as stored; with g % 32 == 0 a warp's 32 rows read one address (broadcast)
+// Outliers (SpQR), optional: CSR over rows, columns ascending in the original (K) order, values in
+// `dtype`.  A value REPLACES the dequantised element before the 16-byte store into ring B, so the
+// accumulation is llmc_gemm_bf16's on the materialised weight.  Each thread keeps a cursor into its
+// row's segment: at every step of its group it skips the columns below the step (the other
+// group's steps), then patches the step's columns in order.
 #include <stdlib.h>
+
+#include <type_traits>
 
 #include <cuda_fp8.h>
 
@@ -79,6 +95,8 @@ constexpr int kBBytes = BN * BK * 2;          // 16 KB dequantised
 constexpr int NG = 2;                         // dequant groups of four warps
 // the weight grid: integer codes, or e4m3 / e5m2 bytes (8-bit words, no zero-point)
 enum : int { kGridInt = 0, kGridE4M3 = 1, kGridE5M2 = 2 };
+// integer zero-points (the 2^23 path), or real-valued ones with groups along K / along N
+enum : int { kRzOff = 0, kRzK = 1, kRzN = 2 };
 // per weight width: INT2 / INT3 / INT4 -> 2 / 3 / 4 KB packed tile, INT8 -> 8 KB
 template <int kBits> struct Cfg {
   static constexpr int kPBytes = BN * BK * kBits / 8;
@@ -107,6 +125,17 @@ struct Params {
   float zero_default;
   int n_tiles_n, num_units, kb_total, gn;
 };
+// The real-zero forms' parameters.  A type of their own, so that Params stays within the 128 bytes
+// up to which nvcc reads a kernel's struct parameter field by field: the other forms' code is unchanged.
+struct ParamsRz : Params {
+  int code_shift;           // 2^(bit-1) on a symmetric grid, else 0
+  int group_n;              // kRzN: rows per group; the qparams are [K, N / group_n]
+  int ngn;                  // kRzN: N / group_n
+  const int32_t* o_rows;    // outliers: CSR [N + 1], or null
+  const int32_t* o_cols;    // [nnz], ascending within a row
+  const uint16_t* o_vals;   // [nnz] in `dtype`
+};
+template <int kRz> using ParamsOf = std::conditional_t<kRz == kRzOff, Params, ParamsRz>;
 
 // (a & b) | c in one LOP3
 __device__ __forceinline__ uint32_t and_or(uint32_t a, uint32_t b, uint32_t c) {
@@ -171,10 +200,16 @@ __device__ __forceinline__ uint32_t lowbit_pair(const uint32_t* w, int l, int j)
   return u;
 }
 
-template <bool kBf16, int kBits, bool kGidx, int kGrid>
+// the outlier cursor's next entry of the row: oc = its column, or INT_MAX past the row's end
+__device__ __forceinline__ void next_outlier(const int32_t* cols, int& ocur, int oend, int& oc) {
+  ++ocur;
+  oc = ocur < oend ? __ldg(cols + ocur) : INT_MAX;
+}
+
+template <bool kBf16, int kBits, bool kGidx, int kGrid, int kRz = kRzOff>
 __global__ void __launch_bounds__(Cfg<kBits>::kThreads, 1)
 w4a16_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmP,
-                  const Params p) {
+                  const ParamsOf<kRz> p) {
   using C = Cfg<kBits>;
   constexpr int DT = kBf16 ? LLMC_BF16 : LLMC_F16;
   constexpr int kLStages = C::kLStages;
@@ -292,6 +327,17 @@ w4a16_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
       int m_blk, n_blk;
       grouped_tile(u, p.num_units / p.n_tiles_n, p.n_tiles_n, p.gn, m_blk, n_blk);
       const int64_t n0 = static_cast<int64_t>(n_blk) * BN + row;
+      // real-zero forms: this row's group along N, and its cursor into the outlier CSR (oc = the
+      // column of entry ocur, INT_MAX past the row's end)
+      int nq = 0, ocur = 0, oend = 0, oc = INT_MAX;
+      if constexpr (kRz == kRzN) nq = static_cast<int>(n0 / p.group_n);
+      if constexpr (kRz != kRzOff) {
+        if (p.o_rows != nullptr && n0 < p.N) {
+          ocur = __ldg(p.o_rows + n0);
+          oend = __ldg(p.o_rows + n0 + 1);
+          oc = ocur < oend ? __ldg(p.o_cols + ocur) : INT_MAX;
+        }
+      }
       // first K step of this tile that belongs to this group: (it + kb) % NG == grp
       int kb = (grp + NG - static_cast<int>(it % NG)) % NG;
       uint32_t s_cur = 0u, z_cur = 0u;
@@ -332,13 +378,31 @@ w4a16_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
             load_lowbit_row<kBits>(pk, row, words);
           }
           const int4* gk = reinterpret_cast<const int4*>(p.g_idx + static_cast<int64_t>(kb) * BK);
+          const int k0 = kb * BK;
+          if constexpr (kRz != kRzOff) {
+            while (oc < k0) next_outlier(p.o_cols, ocur, oend, oc);   // entries of the other group's steps
+          }
 #pragma unroll
           for (int c = 0; c < 8; ++c) {              // 16-byte output chunk c = elements 8c .. 8c+7
-            const int4 ga = __ldg(gk + 2 * c), gb = __ldg(gk + 2 * c + 1);   // same for every lane
-            const int g[8] = {ga.x, ga.y, ga.z, ga.w, gb.x, gb.y, gb.z, gb.w};
             uint32_t sr[8], zr[8];
+            if constexpr (kRz == kRzN) {
+              // row k of the [K, N/g] table (K * N/g < 2^31, checked on the host); a warp's rows
+              // share n / g when g % 32 == 0
+              const int q0 = (k0 + 8 * c) * p.ngn + nq;
 #pragma unroll
-            for (int e = 0; e < 8; ++e) load_qparams(n0, g[e], sr[e], zr[e]);
+              for (int e = 0; e < 8; ++e) {
+                sr[e] = 0u; zr[e] = 0u;
+                if (n0 < p.N) {
+                  sr[e] = __ldg(reinterpret_cast<const uint32_t*>(p.scales) + (q0 + e * p.ngn));
+                  if (have_zeros) zr[e] = __ldg(reinterpret_cast<const uint32_t*>(p.zeros) + (q0 + e * p.ngn));
+                }
+              }
+            } else {
+              const int4 ga = __ldg(gk + 2 * c), gb = __ldg(gk + 2 * c + 1);   // same for every lane
+              const int g[8] = {ga.x, ga.y, ga.z, ga.w, gb.x, gb.y, gb.z, gb.w};
+#pragma unroll
+              for (int e = 0; e < 8; ++e) load_qparams(n0, g[e], sr[e], zr[e]);
+            }
             float v[8];
             if constexpr (kGrid != kGridInt) {
               float f[8];
@@ -353,8 +417,24 @@ w4a16_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
                 if constexpr (kBits == 8) q = (words[2 * c + e / 4] >> (8 * (e % 4))) & 0xFFu;
                 else if constexpr (kBits == 4) q = (words[c] >> (4 * e)) & 0xFu;
                 else q = (lowbit_pair<kBits>(words, c >> 1, e) >> (16 * (c & 1))) & 0xFFFFu;   // element 8c + e
-                const float zm = 8388608.0f + (have_zeros ? widen(zr[e]) : p.zero_default);
-                v[e] = fmul_rn(__uint_as_float(0x4B000000u | q) - zm, widen(sr[e]));
+                if constexpr (kRz != kRzOff) {
+                  // exact code, then (code - z) * s as two fp32 ops: no 2^23 offset, no FMA
+                  const float code = __int2float_rn(static_cast<int>(q) - p.code_shift);
+                  const float z = have_zeros ? __uint_as_float(zr[e]) : 0.f;
+                  v[e] = __fmul_rn(__fsub_rn(code, z), __uint_as_float(sr[e]));
+                } else {
+                  const float zm = 8388608.0f + (have_zeros ? widen(zr[e]) : p.zero_default);
+                  v[e] = fmul_rn(__uint_as_float(0x4B000000u | q) - zm, widen(sr[e]));
+                }
+              }
+              if constexpr (kRz != kRzOff) {
+#pragma unroll
+                for (int e = 0; e < 8; ++e) {          // outliers replace their element (exact: a `dtype` value)
+                  if (oc == k0 + 8 * c + e) {
+                    v[e] = widen16<DT>(__ldg(p.o_vals + ocur));
+                    next_outlier(p.o_cols, ocur, oend, oc);
+                  }
+                }
               }
             }
             const uint4 o = make_uint4(pack_pair<DT>(v[0], v[1]), pack_pair<DT>(v[2], v[3]),
@@ -506,6 +586,10 @@ w4a16_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
 
 using namespace llmc;
 
+template <int kBits, int kGrid, int kRz>
+static int launch_wNa16(const void* x, const int32_t* wq, const void* bias, void* y, int64_t M, int64_t N,
+                        int64_t K, int dtype, void* stream, const char* name, w4::ParamsOf<kRz> p);
+
 template <int kBits, int kGrid = w4::kGridInt>
 static int gemm_wNa16(const void* x, const int32_t* wq, const void* scales, const void* zeros,
                       int qparam_dtype, const void* bias, void* y, int64_t M, int64_t N, int64_t K,
@@ -531,6 +615,22 @@ static int gemm_wNa16(const void* x, const int32_t* wq, const void* scales, cons
     set_last_error("%s: K=%lld must be a multiple of 64 and pointers 16-byte aligned", name, (long long)K);
     return LLMC_EALIGN;
   }
+  Params p{};
+  p.scales = scales; p.zeros = zeros;
+  // packed half2 / bf16x2 dequant exists for INT4 only; INT8 widens native qparams to fp32
+  p.qparam_native = (qparam_dtype != LLMC_F32) ? 1 : 0;
+  p.q_transposed = q_transposed ? 1 : 0;
+  p.group = g_idx ? K : group; p.ng = static_cast<int>(ng);
+  p.g_idx = g_idx;
+  p.zero_default = static_cast<float>(1 << (kBits - 1));
+  return launch_wNa16<kBits, kGrid, w4::kRzOff>(x, wq, bias, y, M, N, K, dtype, stream, name, p);
+}
+
+// Tensor maps, tile counts and the launch of a validated call whose dequant fields `p` holds.
+template <int kBits, int kGrid, int kRz>
+static int launch_wNa16(const void* x, const int32_t* wq, const void* bias, void* y, int64_t M, int64_t N,
+                        int64_t K, int dtype, void* stream, const char* name, w4::ParamsOf<kRz> p) {
+  using namespace w4;
   using C = Cfg<kBits>;
   constexpr int wpr = C::kWordsPerRow;
   constexpr int pr = C::kPackRows;
@@ -544,15 +644,7 @@ static int gemm_wNa16(const void* x, const int32_t* wq, const void* scales, cons
   if (int rc = encode_tmap_2d(&tmP, wq, CU_TENSOR_MAP_DATA_TYPE_INT32, 4, (N + pr - 1) / pr, K * kBits / 32 * pr,
                               K * kBits / 32 * pr, BN / pr, wpr * pr, swz))
     return rc;
-  Params p{};
   p.M = M; p.N = N; p.K = K; p.out = y; p.bias = bias;
-  p.scales = scales; p.zeros = zeros;
-  // packed half2 / bf16x2 dequant exists for INT4 only; INT8 widens native qparams to fp32
-  p.qparam_native = (qparam_dtype != LLMC_F32) ? 1 : 0;
-  p.q_transposed = q_transposed ? 1 : 0;
-  p.group = g_idx ? K : group; p.ng = static_cast<int>(ng);
-  p.g_idx = g_idx;
-  p.zero_default = static_cast<float>(1 << (kBits - 1));
   p.n_tiles_n = static_cast<int>((N + BN - 1) / BN);
   const int64_t mt = (M + BM - 1) / BM;
   LLMC_CHECK_ARG(mt * p.n_tiles_n < (1ll << 31), "%s: too many tiles", name);
@@ -566,11 +658,18 @@ static int gemm_wNa16(const void* x, const int32_t* wq, const void* scales, cons
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   constexpr int smem = C::kSmemBytes;
   static_assert(smem <= 227 * 1024, "shared memory budget");
-  auto kernel = g_idx ? (dtype == LLMC_BF16 ? w4a16_gemm_kernel<true, kBits, true, kGrid>
-                                            : w4a16_gemm_kernel<false, kBits, true, kGrid>)
-                      : (dtype == LLMC_BF16 ? w4a16_gemm_kernel<true, kBits, false, kGrid>
-                                            : w4a16_gemm_kernel<false, kBits, false, kGrid>);
-  return launch_persistent(kernel, p.num_units, C::kThreads, smem, st, tmA, tmP, p);
+  if constexpr (kRz != kRzOff) {
+    // the real-zero forms always gather per element (the group-index dequant)
+    auto kernel = dtype == LLMC_BF16 ? w4a16_gemm_kernel<true, kBits, true, kGrid, kRz>
+                                     : w4a16_gemm_kernel<false, kBits, true, kGrid, kRz>;
+    return launch_persistent(kernel, p.num_units, C::kThreads, smem, st, tmA, tmP, p);
+  } else {
+    auto kernel = p.g_idx ? (dtype == LLMC_BF16 ? w4a16_gemm_kernel<true, kBits, true, kGrid>
+                                                : w4a16_gemm_kernel<false, kBits, true, kGrid>)
+                          : (dtype == LLMC_BF16 ? w4a16_gemm_kernel<true, kBits, false, kGrid>
+                                                : w4a16_gemm_kernel<false, kBits, false, kGrid>);
+    return launch_persistent(kernel, p.num_units, C::kThreads, smem, st, tmA, tmP, p);
+  }
 }
 
 extern "C" int llmc_gemm_w4a16(const void* x, const int32_t* wq, const void* scales,
@@ -728,4 +827,92 @@ extern "C" int llmc_gemm_fp8a16_gidx(const void* x, const int32_t* wq, const voi
   LLMC_CHECK_ARG(g_idx != nullptr, "gemm_fp8a16_gidx: g_idx is NULL");
   return gemm_fp8a16(x, wq, scales, zeros, qparam_dtype, bias, y, M, N, K, 0, g_idx, ng, dtype, q_transposed,
                      e5m2, stream, "gemm_fp8a16_gidx");
+}
+
+// Real-valued zero-points (HQQ, SpQR): fp32 scales / zeros, dequant rT(fmul(fsub(code, z), s)) with
+// the exact code (minus 2^(bit-1) when sym), zeros NULL => 0.  group_axis 0: column k uses group
+// g_idx[k] of ng, qparams [ng, N]; group_axis 1: rows n use group n / group, qparams [K, N/group].
+// Outliers (rows [N+1], cols [nnz], vals [nnz] in `dtype`; all three or none) replace their element.
+template <int kBits>
+static int gemm_wNa16_rz(const void* x, const int32_t* wq, const float* scales, const float* zeros, int sym,
+                         int group_axis, int64_t group, const int32_t* g_idx, int64_t ng,
+                         const int32_t* outlier_rows, const int32_t* outlier_cols, const void* outlier_vals,
+                         const void* bias, void* y, int64_t M, int64_t N, int64_t K, int dtype, void* stream,
+                         const char* name) {
+  using namespace w4;
+  LLMC_CHECK_ARG(M >= 0 && N >= 0 && K > 0, "%s: bad shape", name);
+  if (M == 0 || N == 0) return LLMC_OK;
+  LLMC_CHECK_ARG(x && wq && scales && y, "%s: null pointer", name);
+  LLMC_CHECK_ARG(dtype == LLMC_BF16 || dtype == LLMC_F16, "%s: dtype must be bf16 or fp16", name);
+  LLMC_CHECK_ARG(sym == 0 || sym == 1, "%s: sym must be 0 or 1, got %d", name, sym);
+  LLMC_CHECK_ARG(group_axis == 0 || group_axis == 1, "%s: group_axis must be 0 (K) or 1 (N), got %d", name,
+                 group_axis);
+  const int n_outlier_args = (outlier_rows != nullptr) + (outlier_cols != nullptr) + (outlier_vals != nullptr);
+  LLMC_CHECK_ARG(n_outlier_args == 0 || n_outlier_args == 3,
+                 "%s: outlier rows, cols and vals must be given together or not at all", name);
+  if (group_axis == 0) {
+    LLMC_CHECK_ARG(g_idx != nullptr, "%s: group_axis 0 needs g_idx", name);
+    LLMC_CHECK_ARG(ng >= 1 && ng <= K, "%s: ng=%lld groups for K=%lld columns", name, (long long)ng,
+                   (long long)K);
+  } else {
+    LLMC_CHECK_ARG(group > 0 && N % group == 0, "%s: group %lld must divide N=%lld", name, (long long)group,
+                   (long long)N);
+    LLMC_CHECK_ARG(K * (N / group) < (1ll << 31), "%s: qparam table [K, N/group] over 2^31 entries", name);
+  }
+  if (K % 64 != 0 || !aligned16(x) || !aligned16(wq) || !aligned16(y) || (g_idx && !aligned16(g_idx))) {
+    set_last_error("%s: K=%lld must be a multiple of 64 and pointers 16-byte aligned", name, (long long)K);
+    return LLMC_EALIGN;
+  }
+  ParamsRz p{};
+  p.scales = scales; p.zeros = zeros;
+  p.qparam_native = 0;
+  p.q_transposed = 1;
+  p.group = K;
+  p.code_shift = sym ? 1 << (kBits - 1) : 0;
+  p.o_rows = outlier_rows; p.o_cols = outlier_cols;
+  p.o_vals = static_cast<const uint16_t*>(outlier_vals);
+  if (group_axis == 0) {
+    p.ng = static_cast<int>(ng);
+    p.g_idx = g_idx;
+    return launch_wNa16<kBits, kGridInt, kRzK>(x, wq, bias, y, M, N, K, dtype, stream, name, p);
+  }
+  p.group_n = static_cast<int>(group);
+  p.ngn = static_cast<int>(N / group);
+  return launch_wNa16<kBits, kGridInt, kRzN>(x, wq, bias, y, M, N, K, dtype, stream, name, p);
+}
+
+extern "C" int llmc_gemm_w2a16_rz(const void* x, const int32_t* wq, const float* scales, const float* zeros,
+                                  int sym, int group_axis, int64_t group, const int32_t* g_idx, int64_t ng,
+                                  const int32_t* outlier_rows, const int32_t* outlier_cols,
+                                  const void* outlier_vals, const void* bias, void* y, int64_t M, int64_t N,
+                                  int64_t K, int dtype, void* stream) {
+  return gemm_wNa16_rz<2>(x, wq, scales, zeros, sym, group_axis, group, g_idx, ng, outlier_rows, outlier_cols,
+                           outlier_vals, bias, y, M, N, K, dtype, stream, "gemm_w2a16_rz");
+}
+
+extern "C" int llmc_gemm_w3a16_rz(const void* x, const int32_t* wq, const float* scales, const float* zeros,
+                                  int sym, int group_axis, int64_t group, const int32_t* g_idx, int64_t ng,
+                                  const int32_t* outlier_rows, const int32_t* outlier_cols,
+                                  const void* outlier_vals, const void* bias, void* y, int64_t M, int64_t N,
+                                  int64_t K, int dtype, void* stream) {
+  return gemm_wNa16_rz<3>(x, wq, scales, zeros, sym, group_axis, group, g_idx, ng, outlier_rows, outlier_cols,
+                           outlier_vals, bias, y, M, N, K, dtype, stream, "gemm_w3a16_rz");
+}
+
+extern "C" int llmc_gemm_w4a16_rz(const void* x, const int32_t* wq, const float* scales, const float* zeros,
+                                  int sym, int group_axis, int64_t group, const int32_t* g_idx, int64_t ng,
+                                  const int32_t* outlier_rows, const int32_t* outlier_cols,
+                                  const void* outlier_vals, const void* bias, void* y, int64_t M, int64_t N,
+                                  int64_t K, int dtype, void* stream) {
+  return gemm_wNa16_rz<4>(x, wq, scales, zeros, sym, group_axis, group, g_idx, ng, outlier_rows, outlier_cols,
+                           outlier_vals, bias, y, M, N, K, dtype, stream, "gemm_w4a16_rz");
+}
+
+extern "C" int llmc_gemm_w8a16_rz(const void* x, const int32_t* wq, const float* scales, const float* zeros,
+                                  int sym, int group_axis, int64_t group, const int32_t* g_idx, int64_t ng,
+                                  const int32_t* outlier_rows, const int32_t* outlier_cols,
+                                  const void* outlier_vals, const void* bias, void* y, int64_t M, int64_t N,
+                                  int64_t K, int dtype, void* stream) {
+  return gemm_wNa16_rz<8>(x, wq, scales, zeros, sym, group_axis, group, g_idx, ng, outlier_rows, outlier_cols,
+                           outlier_vals, bias, y, M, N, K, dtype, stream, "gemm_w8a16_rz");
 }

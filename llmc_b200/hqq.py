@@ -9,6 +9,7 @@ static fake-quant kernel through `buf_scales / buf_zeros` exactly like the refer
 import torch
 
 from .blockwise import ALGO_REGISTRY, BaseBlockwiseQuantization
+from .quant import IntegerQuantizer
 
 
 @ALGO_REGISTRY
@@ -70,3 +71,44 @@ class HQQ(BaseBlockwiseQuantization):
         if self.axis == 0:
             args['dim'] = 'ic'
         return wquantizer.fake_quant_weight_static(module.weight, args)
+
+    def w_packed(self, module, wquantizer):
+        """The packed form of exactly what `w_qdq` materialises, for EffcientFakeQuantLinear: codes from
+        the same static pass (round_zp False puts the real-valued zero-point inside the rounding), on
+        weight.T for axis 0 and transposed back to [R, C]; the fp32 buf_scales / buf_zeros as stored —
+        [C, R/group], groups along N, for axis 0; [R, C/group] for axis 1, handed over as [C/group, R]
+        with g_idx = k // group.  None (materialise) for what llmc_gemm_w*a16_rz does not serve."""
+        from .module_utils import pack_unsigned_codes
+        from .quant import OUT_CODES_I32
+        q, w = wquantizer, module.weight
+        if not (isinstance(q, IntegerQuantizer) and q.bit in (2, 3, 4, 8) and q.granularity == 'per_group'
+                and w.dim() == 2 and w.is_cuda and w.dtype in (torch.float16, torch.bfloat16)):
+            return None
+        R, C = w.shape
+        src = w.data.T if self.axis == 0 else w.data          # the tensor w_qdq quantises
+        rows, cols = src.shape
+        group = q.group_size if cols >= q.group_size else cols  # IntegerQuantizer._group_of
+        if C % 64 or cols % group:
+            return None
+        s = module.buf_scales.to(w.device)
+        if s.dtype != torch.float32 or s.numel() != rows * (cols // group):
+            return None
+        s = s.reshape(rows, cols // group)
+        zeros = module.buf_zeros
+        z = None                                             # what _static reads: zero-points, or 0
+        if torch.is_tensor(zeros) and zeros.numel() > 1:
+            z = zeros.to(device=w.device, dtype=torch.float32).reshape(s.shape)
+        elif torch.is_tensor(zeros) and zeros.numel() == 1 and (zeros.is_cuda or float(zeros) != 0.0):
+            z = zeros.to(device=w.device, dtype=torch.float32).reshape(1, 1).expand(s.shape)
+        codes = torch.empty((rows, cols), dtype=torch.int32, device=w.device)
+        q._static(src, s.reshape(-1), zeros, module.buf_qmax, module.buf_qmin, OUT_CODES_I32, codes, w.dtype,
+                  cols // group, group)
+        packed = dict(bits=q.bit, group=group, dtype=w.dtype, rz=True, sym=q.sym, outliers=None)
+        if self.axis == 0:
+            packed.update(qweight=pack_unsigned_codes(codes.t(), q.bit, signed=q.sym), scales=s.contiguous(),
+                          zeros=z.contiguous() if z is not None else None, group_axis=1, g_idx=None)
+        else:
+            g_idx = (torch.arange(C, device=w.device) // group).to(torch.int32)
+            packed.update(qweight=pack_unsigned_codes(codes, q.bit, signed=q.sym), scales=s.t().contiguous(),
+                          zeros=z.t().contiguous() if z is not None else None, group_axis=0, g_idx=g_idx)
+        return packed

@@ -99,6 +99,77 @@ def linear_forward_w4(x, wq, scales, zeros, group, bias=None, bits=4, qparams_t=
     return y.reshape(*x.shape[:-1], N)
 
 
+def linear_forward_rz(x, wq, scales, zeros, bits, sym, group_axis, group=None, g_idx=None, outliers=None,
+                      bias=None):
+    """Fake-quant forward on packed codes with REAL-VALUED zero-points (HQQ, SpQR: round_zp False),
+    csrc/gemm_w4.cu: y = x @ dequant(wq).T + bias, dequant = rT((code - zero) * scale) as two fp32
+    ops and one rounding — bit-identical to linear_forward on the weight quant.py:710-717 materialises.
+
+    wq: the packed codes of pack_unsigned_codes (bits 2 / 3 / 4 / 8).  scales / zeros: fp32 (zeros
+    None => 0); `sym` says that the codes are stored with the +2^(bits-1) offset of a symmetric grid.
+    group_axis 0: groups along K, column k in group g_idx[k] (int32 [K], required), qparams [ng, N].
+    group_axis 1: groups of `group` rows along N, qparams [K, N/group] (HQQ axis 0).
+    outliers: None or (rows int32 [N+1], cols int32 [nnz], vals [nnz] in x.dtype), the CSR of
+    outliers_to_csr; each value replaces its dequantised element."""
+    require_cuda(x, wq, scales)
+    if bits not in (2, 3, 4, 8):
+        raise ValueError(f'packed weights are 2, 3, 4 or 8 bits, not {bits}')
+    if scales.dim() != 2 or scales.dtype != torch.float32 or (zeros is not None and (
+            zeros.dtype != torch.float32 or zeros.shape != scales.shape)):
+        raise ValueError('real-zero qparams are 2-D fp32 scales (and zeros of the same shape)')
+    K = x.shape[-1]
+    if group_axis == 0:
+        N = scales.shape[1]
+        if g_idx is None or g_idx.dtype != torch.int32 or g_idx.numel() != K or not g_idx.is_cuda:
+            raise ValueError(f'group_axis 0 needs g_idx, a CUDA int32 tensor of K={K} elements')
+        ng, group = scales.shape[0], 0
+    elif group_axis == 1:
+        N = scales.shape[1] * group
+        if scales.shape[0] != K:
+            raise ValueError(f'group_axis 1 qparams are [K={K}, N/group], not {tuple(scales.shape)}')
+        ng = 0
+    else:
+        raise ValueError(f'group_axis must be 0 or 1, not {group_axis}')
+    want = ((N + 1) // 2, 3 * K // 16) if bits == 3 else (N, K * bits // 32)
+    if wq.dtype != torch.int32 or tuple(wq.shape) != want:
+        raise ValueError(f'packed weight {tuple(wq.shape)} does not match N={N}, K={K} at {bits} bits')
+    o_rows = o_cols = o_vals = None
+    nnz = 0
+    if outliers is not None:
+        o_rows, o_cols, o_vals = outliers
+        if o_rows.numel() != N + 1 or o_vals.dtype != x.dtype or o_cols.numel() != o_vals.numel():
+            raise ValueError('outliers must be a CSR (rows [N+1], cols [nnz], vals [nnz] in the activation dtype)')
+        nnz = o_cols.numel()
+        if nnz == 0:                                  # empty tensors have no storage to point at
+            o_rows = o_cols = o_vals = None
+    x2 = x.reshape(-1, K)
+    x2 = x2 if x2.is_contiguous() else x2.contiguous()
+    b = bias.to(x.dtype).contiguous() if bias is not None else None
+    y = torch.empty((x2.shape[0], N), dtype=x.dtype, device=x.device)
+    M = x2.shape[0]
+    gi = g_idx.contiguous() if g_idx is not None else None
+    with TIMER.span(f'gemm_w{bits}a16_rz', flops=2.0 * M * N * K,
+                    nbytes=2.0 * M * K + bits / 8.0 * N * K + 8.0 * scales.numel() + 6.0 * nnz + 2.0 * M * N):
+        call(f'llmc_gemm_w{bits}a16_rz', ptr(x2), ptr(wq.contiguous()), ptr(scales.contiguous()),
+             ptr(zeros.contiguous() if zeros is not None else None), int(bool(sym)), int(group_axis),
+             int(group or 0), ptr(gi), int(ng), ptr(o_rows), ptr(o_cols), ptr(o_vals), ptr(b), ptr(y), M, N, K,
+             dtype_enum(x.dtype), stream_ptr(x.device))
+    return y.reshape(*x.shape[:-1], N)
+
+
+def outliers_to_csr(mask, values):
+    """A dense outlier mask [R, C] (bool / uint8) and the weight [R, C] -> the CSR of
+    linear_forward_rz: rows int32 [R+1], cols int32 [nnz] ascending within a row, values[mask]
+    [nnz] in values' dtype.  On the mask's device."""
+    m = mask.bool()
+    idx = m.nonzero()                                 # row-major: rows, then columns, ascending
+    counts = m.sum(dim=1, dtype=torch.int64)
+    rows = torch.zeros(m.shape[0] + 1, dtype=torch.int64, device=m.device)
+    rows[1:] = counts.cumsum(0)
+    return (rows.to(torch.int32), idx[:, 1].to(torch.int32).contiguous(),
+            values[idx[:, 0], idx[:, 1]].contiguous())
+
+
 FP8_GRIDS = {torch.float8_e4m3fn: 'e4m3', torch.float8_e5m2: 'e5m2'}
 
 
@@ -379,10 +450,18 @@ class EffcientFakeQuantLinear(nn.Module):
     FP8 weights (FloatQuantizer on an e4m3 / e5m2 grid) are packed too: `qweight` then holds the
     fp8 bytes [N, K] themselves (`q_grid` 'e4m3' / 'e5m2'; 'int' for codes), with one scale per row
     or group and no zero-point, and the forward runs llmc_gemm_fp8a16 — 8 bits plus the scales per
-    weight instead of 16, bit-identical to the materialised forward (tests/test_gpu_gemm_fp8w.py)."""
+    weight instead of 16, bit-identical to the materialised forward (tests/test_gpu_gemm_fp8w.py).
 
-    # the buffers of the packed form; export_state_dict writes an FP8 module's dense `weight` instead
-    PACKED_BUFFERS = ('qweight', 'qscales', 'qzeros', 'qscales_t', 'qzeros_t', 'g_idx')
+    Real-valued zero-points (HQQ.w_packed, SpQR.w_packed; `q_rz`): fp32 qparams in the layout of
+    linear_forward_rz — [ng, N] with `g_idx` for groups along K (`q_axis` 0), [K, N/group] for HQQ's
+    groups along N (`q_axis` 1) — `q_sym` for codes stored with the symmetric offset, and SpQR's
+    outliers as a CSR over rows (`outlier_rows / outlier_cols / outlier_vals`, None without).  The
+    forward runs llmc_gemm_w{2,3,4,8}a16_rz (tests/test_gpu_gemm_rz.py)."""
+
+    # the buffers of the packed form; export_state_dict writes the dense `weight` of an FP8, 2- / 3-bit
+    # or real-zero module instead
+    PACKED_BUFFERS = ('qweight', 'qscales', 'qzeros', 'qscales_t', 'qzeros_t', 'g_idx', 'outlier_rows',
+                      'outlier_cols', 'outlier_vals')
 
     def __init__(self, weight, bias, ori_module, a_qdq, packed=None):
         super().__init__()
@@ -397,10 +476,18 @@ class EffcientFakeQuantLinear(nn.Module):
                 self.qzeros = None
             self.q_bits, self.q_group, self.q_dtype = packed['bits'], packed['group'], packed['dtype']
             self.q_grid = FP8_GRIDS.get(packed['qweight'].dtype, 'int')
-            # [K/group, N] copies for the GEMM (coalesced qparam loads); tiny next to the codes
-            self.register_buffer('qscales_t', packed['scales'].t().contiguous(), persistent=False)
-            self.register_buffer('qzeros_t', packed['zeros'].t().contiguous()
-                                 if packed['zeros'] is not None else None, persistent=False)
+            self.q_rz = packed.get('rz', False)
+            if self.q_rz:
+                # the qparams are already in the kernel's layout
+                self.q_axis, self.q_sym = packed['group_axis'], packed['sym']
+                o = packed.get('outliers')
+                for i, leaf in enumerate(('outlier_rows', 'outlier_cols', 'outlier_vals')):
+                    self.register_buffer(leaf, o[i] if o is not None else None)
+            else:
+                # [K/group, N] copies for the GEMM (coalesced qparam loads); tiny next to the codes
+                self.register_buffer('qscales_t', packed['scales'].t().contiguous(), persistent=False)
+                self.register_buffer('qzeros_t', packed['zeros'].t().contiguous()
+                                     if packed['zeros'] is not None else None, persistent=False)
             self.register_buffer('g_idx', packed.get('g_idx'))
         self.packed = packed is not None
         if bias is not None:
@@ -422,6 +509,8 @@ class EffcientFakeQuantLinear(nn.Module):
     def dequantized_weight(self):
         """rT((code - zero) * scale): the tensor the reference holds in `.weight` (elementwise, exact).
         FP8 grids: rT(fp32(byte) * scale), a zero scale read as 1, as llmc_fp8_quant's QDQ output."""
+        if self.q_rz:
+            return self._dequantized_rz()
         if self.q_grid != 'int':
             N, K = self.qweight.shape
             s = self.qscales.float().reshape(N, -1)
@@ -442,10 +531,41 @@ class EffcientFakeQuantLinear(nn.Module):
         zz = z.reshape(N, -1, 1) if torch.is_tensor(z) else z
         return ((c - zz) * s.reshape(N, -1, 1)).reshape(N, K).to(self.q_dtype)
 
+    def _rz_shape(self):
+        s = self.qscales
+        return (s.shape[1], self.g_idx.numel()) if self.q_axis == 0 else (s.shape[1] * self.q_group, s.shape[0])
+
+    def _dequantized_rz(self):
+        """rT((code - zero) * scale) as two fp32 ops, one rounding (quant.py:710-717 then .to(dtype)),
+        then the outliers overwrite their elements (SpQR's torch.where)."""
+        N, K = self._rz_shape()
+        bits = self.q_bits
+        code = unpack_unsigned_codes(self.qweight, bits, N)
+        if self.q_sym:
+            code = code - (1 << (bits - 1))
+        code = code.float()
+        if self.q_axis == 0:
+            gi = self.g_idx.long()
+            s = self.qscales[gi].t()
+            z = self.qzeros[gi].t() if self.qzeros is not None else 0.0
+        else:
+            s = self.qscales.repeat_interleave(self.q_group, dim=1).t()
+            z = self.qzeros.repeat_interleave(self.q_group, dim=1).t() if self.qzeros is not None else 0.0
+        w = ((code - z) * s).to(self.q_dtype)
+        if self.outlier_rows is not None:
+            counts = (self.outlier_rows[1:] - self.outlier_rows[:-1]).long()
+            r = torch.repeat_interleave(torch.arange(N, device=w.device), counts)
+            w[r, self.outlier_cols.long()] = self.outlier_vals
+        return w
+
     @torch.no_grad()
     def forward(self, x):
         if self.a_qdq is not None:
             x = self.a_qdq(x, self)
+        if self.packed and self.q_rz:
+            o = (self.outlier_rows, self.outlier_cols, self.outlier_vals) if self.outlier_rows is not None else None
+            return linear_forward_rz(x, self.qweight, self.qscales, self.qzeros, self.q_bits, self.q_sym, self.q_axis,
+                                     group=self.q_group, g_idx=self.g_idx, outliers=o, bias=self.bias)
         if self.packed and self.q_grid != 'int':
             return linear_forward_fp8w(x, self.qweight, self.qscales_t, self.q_group, self.bias, qparams_t=True,
                                        g_idx=self.g_idx)

@@ -152,6 +152,41 @@ class SpQR(GPTQ):
         return torch.where(mask, weight.to(self.model_dtype), y)
 
     @torch.no_grad()
+    def w_packed(self, module, wquantizer):
+        """The packed form of exactly what `w_qdq` materialises, for EffcientFakeQuantLinear: codes of
+        the static pass w_qdq runs (act-order gmap included), in the original column order; the fp32
+        statistics as [ng, R] with g_idx = invperm // group (k // group without act-order); the
+        outliers of buf_mask as a CSR with their weights in the model dtype.  None when
+        llmc_gemm_w*a16_rz does not serve the layer; it is then materialised as before."""
+        from .module_utils import outliers_to_csr, pack_unsigned_codes
+        from .quant import OUT_CODES_I32, IntegerQuantizer
+        q, w = wquantizer, module.weight.data
+        if not (isinstance(q, IntegerQuantizer) and q.bit in (2, 3, 4, 8) and q.granularity == 'per_group'
+                and w.dim() == 2 and w.is_cuda and w.is_floating_point()
+                and self.model_dtype in (torch.float16, torch.bfloat16)):
+            return None
+        R, K = w.shape
+        group = q.group_size
+        if K % 64 or K % group:
+            return None
+        ng = K // group
+        scales = module.buf_scales.to(w.device)
+        zeros = module.buf_zeros.to(w.device)
+        if scales.dtype != torch.float32 or zeros.dtype != torch.float32 or scales.numel() != R * ng:
+            return None
+        scales, zeros = scales.reshape(R, ng), zeros.reshape(R, ng)
+        gmap = (module.buf_invperm // group).to(torch.int32) if self.need_perm else None
+        codes = torch.empty((R, K), dtype=torch.int32, device=w.device)
+        q._static(w, scales.reshape(-1), zeros, module.buf_qmax, module.buf_qmin, OUT_CODES_I32, codes,
+                  self.model_dtype, ng, group, gmap=gmap)
+        g_idx = gmap if gmap is not None else (torch.arange(K, device=w.device) // group).to(torch.int32)
+        mask = module.buf_mask.to(w.device)
+        outliers = outliers_to_csr(mask, w.to(self.model_dtype)) if bool(mask.any()) else None
+        return dict(qweight=pack_unsigned_codes(codes, q.bit, signed=q.sym), scales=scales.t().contiguous(),
+                    zeros=zeros.t().contiguous(), bits=q.bit, group=group, dtype=self.model_dtype, g_idx=g_idx,
+                    rz=True, sym=q.sym, group_axis=0, outliers=outliers)
+
+    @torch.no_grad()
     def deploy(self, quant_format):
         """spqr.py:388-392."""
         if quant_format == 'real_quant':
