@@ -531,6 +531,38 @@ int llmc_gemm_w8a16_rz(const void* x, const int32_t* wq, const float* scales, co
                        const int32_t* outlier_rows, const int32_t* outlier_cols, const void* outlier_vals,
                        const void* bias, void* y, int64_t M, int64_t N, int64_t K, int dtype, void* stream);
 
+/* ------------------------------------------------------------------------------------
+ * K7  llmc_gemm_w8a8_i8 / llmc_gemm_w8a8_fp8 (csrc/gemm_w8a8.cu) — the forward of the exported
+ *   W8A8 linears (VllmRealQuantLinear and its Sgl / Lightllm / Lightx2v aliases): both operands
+ *   8-bit on the tensor cores, one scale per token and one per output channel.
+ *   x    [M, K] activation codes: int8 (i8) or e4m3 bytes (fp8), K-major, row stride K
+ *   w    [N, K] weight codes of the same type (the exported `weight`), row stride K
+ *   s_x  fp32 activation scales, s_x[m * s_x_stride]; s_w fp32 weight scales, s_w[n * s_w_stride];
+ *        a stride of 0 passes one per-tensor scale, 1 a vector
+ *   bias [N] of `dtype` or NULL; y [M, N] `dtype` (LLMC_BF16 / LLMC_F16)
+ *   Numerics, per output element, independent of M, N and the tile schedule:
+ *     acc  = sum_k x[m, k] * w[n, k]
+ *            i8:  wgmma s32.s8.s8, the exact integer sum (K <= 131056 keeps it below 2^31 for any
+ *                 int8 codes), converted with cvt.rn.f32.s32
+ *            fp8: wgmma f32.e4m3.e4m3 with a fresh fp32 dot per 128-deep K block, the blocks summed
+ *                 in ascending K order with fadd.rn into an fp32 register (Hopper's tensor core adds
+ *                 the products of one block at reduced precision; only that differs from an fp32 sum
+ *                 of exact products)
+ *     y    = rT(fmul.rn(fmul.rn(acc, s_w[n]), s_x[m]))             without a bias
+ *     y    = rT(fadd.rn(fmul.rn(fmul.rn(acc, s_w[n]), s_x[m]), bias[n]))   with one
+ *     fp32 throughout, one rounding to `dtype`.
+ *   The codes and scales are what the activation quantizer of the same config writes
+ *   (llmc_quant_dynamic / llmc_quant_static with LLMC_OUT_CODES_I8, llmc_fp8_quant out_mode 2),
+ *   widened to fp32.  K % 16 == 0 (16-byte rows; the K tail of a 128-deep block is zero-filled),
+ *   N >= 1, M == 0 is a no-op; x, w, y 16-byte aligned.  Argument errors are returned before any
+ *   launch. */
+int llmc_gemm_w8a8_i8(const void* x, const float* s_x, int64_t s_x_stride, const void* w, const float* s_w,
+                      int64_t s_w_stride, const void* bias, void* y, int64_t M, int64_t N, int64_t K,
+                      int dtype, void* stream);
+int llmc_gemm_w8a8_fp8(const void* x, const float* s_x, int64_t s_x_stride, const void* w, const float* s_w,
+                       int64_t s_w_stride, const void* bias, void* y, int64_t M, int64_t N, int64_t K,
+                       int dtype, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -106,6 +106,10 @@ SIGNATURES = {
                                    c_vp, c_vp, c_i64, c_i64, c_i64, c_int, c_vp]),
     'llmc_gemm_w8a16_rz': (c_int, [c_vp, c_vp, c_vp, c_vp, c_int, c_int, c_i64, c_vp, c_i64, c_vp, c_vp, c_vp,
                                    c_vp, c_vp, c_i64, c_i64, c_i64, c_int, c_vp]),
+    'llmc_gemm_w8a8_i8': (c_int, [c_vp, c_vp, c_i64, c_vp, c_vp, c_i64, c_vp, c_vp, c_i64, c_i64, c_i64, c_int,
+                                  c_vp]),
+    'llmc_gemm_w8a8_fp8': (c_int, [c_vp, c_vp, c_i64, c_vp, c_vp, c_i64, c_vp, c_vp, c_i64, c_i64, c_i64, c_int,
+                                   c_vp]),
 }
 
 _lock = threading.Lock()

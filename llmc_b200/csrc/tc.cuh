@@ -220,6 +220,27 @@ __device__ __forceinline__ void wgmma_m64n128k32_e4m3(float (&d)[64], uint64_t a
       : "l"(adesc), "l"(bdesc), "r"(accumulate));
 }
 
+// D[64 x 128] (+)= A[64 x 32] * B[128 x 32]^T on signed 8-bit operands with int32 accumulators,
+// issued by one warpgroup (gemm_w8a8.cu).  K-major only; fragment layout as above.  The integer
+// sum is exact (wrapping, not saturating, past int32 — the caller bounds K).
+__device__ __forceinline__ void wgmma_m64n128k32_s8(int32_t (&d)[64], uint64_t adesc, uint64_t bdesc,
+                                                    uint32_t accumulate) {
+  asm volatile(
+      "{\n"
+      ".reg .pred p;\n"
+      "setp.ne.b32 p, %66, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n128k32.s32.s8.s8 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, "
+      "%64, %65, p;\n"
+      "}\n"
+      : "+r"(d[0]), "+r"(d[1]), "+r"(d[2]), "+r"(d[3]), "+r"(d[4]), "+r"(d[5]), "+r"(d[6]), "+r"(d[7]), "+r"(d[8]), "+r"(d[9]), "+r"(d[10]), "+r"(d[11]), "+r"(d[12]), "+r"(d[13]), "+r"(d[14]), "+r"(d[15]), "+r"(d[16]), "+r"(d[17]), "+r"(d[18]), "+r"(d[19]), "+r"(d[20]), "+r"(d[21]), "+r"(d[22]), "+r"(d[23]), "+r"(d[24]), "+r"(d[25]), "+r"(d[26]), "+r"(d[27]), "+r"(d[28]), "+r"(d[29]), "+r"(d[30]), "+r"(d[31]), "+r"(d[32]), "+r"(d[33]), "+r"(d[34]), "+r"(d[35]), "+r"(d[36]), "+r"(d[37]), "+r"(d[38]), "+r"(d[39]), "+r"(d[40]), "+r"(d[41]), "+r"(d[42]), "+r"(d[43]), "+r"(d[44]), "+r"(d[45]), "+r"(d[46]), "+r"(d[47]), "+r"(d[48]), "+r"(d[49]), "+r"(d[50]), "+r"(d[51]), "+r"(d[52]), "+r"(d[53]), "+r"(d[54]), "+r"(d[55]), "+r"(d[56]), "+r"(d[57]), "+r"(d[58]), "+r"(d[59]), "+r"(d[60]), "+r"(d[61]), "+r"(d[62]), "+r"(d[63])
+      : "l"(adesc), "l"(bdesc), "r"(accumulate));
+}
+__device__ __forceinline__ void fence_acc(int32_t (&d)[64]) {
+#pragma unroll
+  for (int i = 0; i < 64; ++i) asm volatile("" : "+r"(d[i])::"memory");
+}
+
 // D[64 x 128] += A[64 x 8] * B[128 x 8]^T on tf32 operands, issued by one warpgroup.  tf32 operands
 // are read K-major only (no transpose immediates); fragment layout as above.  Always accumulates:
 // the 3xTF32 update (tf32.cu) starts from zeroed accumulators, so an exact-zero sum keeps the
@@ -244,7 +265,7 @@ __device__ __forceinline__ void wgmma_m64n128k16(float (&d)[64], uint64_t adesc,
   else wgmma_m64n128k16_f16<kTransA, kTransB>(d, adesc, bdesc, accumulate);
 }
 
-// ---- forward GEMMs (gemm.cu, gemm_w4.cu, gemm_fp8.cu) ------------------------------------------
+// ---- forward GEMMs (gemm.cu, gemm_w4.cu, gemm_fp8.cu, gemm_w8a8.cu) -----------------------------
 // L2-grouped tile order: the weights are swept in groups of `gn` n-tiles (<= ~32 MB, L2 resident,
 // see l2_group_width), all m-tiles per group, n fastest inside the group.  Activations are re-read
 // once per group from HBM, weights once; n-fastest over a 14336-row weight would instead stream

@@ -217,6 +217,59 @@ def linear_forward_fp8w(x, wq, scales, group, bias=None, qparams_t=False, g_idx=
     return y.reshape(*x.shape[:-1], N)
 
 
+def act_quantizer(act_cfg):
+    """The activation quantizer of a `quant.act` config section, as the algorithms build it
+    (blockwise.set_quant_config): FloatQuantizer for `quant_type: float-quant`, else IntegerQuantizer."""
+    from .quant import IntegerQuantizer
+    from .quant_float import FloatQuantizer
+    kw = dict(act_cfg)
+    cls = FloatQuantizer if kw.pop('quant_type', 'int-quant') == 'float-quant' else IntegerQuantizer
+    return cls(**kw)
+
+
+W8A8_ENTRY = {torch.int8: 'llmc_gemm_w8a8_i8', torch.float8_e4m3fn: 'llmc_gemm_w8a8_fp8'}
+
+
+def linear_forward_w8a8(x, w, s_w, act_cfg, input_scale=None, bias=None):
+    """The W8A8 real-quant forward (csrc/gemm_w8a8.cu): x is quantised to int8 / e4m3 codes by the
+    activation quantizer of `act_cfg` (a `quant.act` section, or the quantizer itself) exactly as the
+    fake-quant forward of that config quantises it (real_quant_act), then
+        y = rT(fp32(sum_k qx[m, k] * w[n, k]) * s_w[n] * s_x[m] (+ bias[n]))
+    on the INT8 or FP8 tensor cores, both operands 8-bit.
+
+    w [N, K] int8 (symmetric per-channel codes) or float8_e4m3fn, the exported `weight`; s_w its
+    `weight_scale`, N values (per-channel) or one (per-tensor), any float dtype (widened to fp32);
+    input_scale: None for per-token dynamic activations, the exported one-element `input_scale` for
+    per-tensor static ones.  x bf16 / fp16, K % 16 == 0."""
+    from .quant import BaseQuantizer, IntegerQuantizer
+    from .quant_float import FloatQuantizer
+    require_cuda(x, w, s_w, input_scale, bias)
+    if w.dtype not in W8A8_ENTRY:
+        raise NotImplementedError(f'W8A8 weights are int8 or float8_e4m3fn, not {w.dtype}')
+    aq = act_cfg if isinstance(act_cfg, BaseQuantizer) else act_quantizer(act_cfg)
+    want = IntegerQuantizer if w.dtype == torch.int8 else FloatQuantizer
+    if type(aq) is not want:
+        raise NotImplementedError(f'{w.dtype} weights need {want.__name__} activations, not {type(aq).__name__}')
+    K = x.shape[-1]
+    N = w.shape[0]
+    if w.dim() != 2 or w.shape[1] != K:
+        raise ValueError(f'weight shape {tuple(w.shape)} does not match K={K}')
+    sw = s_w.reshape(-1).float().contiguous()
+    if sw.numel() not in (1, N):
+        raise ValueError(f'weight_scale of {sw.numel()} values for N={N} rows')
+    x2 = x.reshape(-1, K)
+    M = x2.shape[0]
+    y = torch.empty((M, N), dtype=x.dtype, device=x.device)
+    if M == 0:
+        return y.reshape(*x.shape[:-1], N)
+    qx, sx = aq.real_quant_act(x2, input_scale)
+    b = bias.to(x.dtype).contiguous() if bias is not None else None
+    with TIMER.span('gemm_w8a8', flops=2.0 * M * N * K, nbytes=float(M * K + N * K) + 2.0 * M * N):
+        call(W8A8_ENTRY[w.dtype], ptr(qx), ptr(sx), int(sx.numel() != 1), ptr(w.contiguous()), ptr(sw),
+             int(sw.numel() != 1), ptr(b), ptr(y), M, N, K, dtype_enum(x.dtype), stream_ptr(x.device))
+    return y.reshape(*x.shape[:-1], N)
+
+
 # Counterpart of the reference's USE_FP8GEMM_TRITON_KERNEL (module_utils.py:14-20): when set,
 # LlmcFp8Linear keeps its weight in fp8 and runs block_wise_fp8_forward_func on the FP8 tensor cores.
 # Off by default: the forward then dequantises once and runs the bf16 GEMM, as it always has here.
@@ -608,7 +661,14 @@ def _cfg_get(cfg, key, default=None):
 
 class VllmRealQuantLinear(nn.Module):
     """module_utils.py:762-876 — compressed-tensors layout: `weight_packed` / `weight`,
-    `weight_scale` (fp16 when packed) or `weight_scale_inv`, `input_scale`."""
+    `weight_scale` (fp16 when packed) or `weight_scale_inv`, `input_scale`.
+
+    Extension (K7): the W8A8 exports run.  An int8 `weight` with symmetric int8 activations, or an
+    e4m3 `weight` with e4m3 activations — per-token dynamic, or per-tensor static from `input_scale`
+    — forward through linear_forward_w8a8 on the INT8 / FP8 tensor cores, the activations quantised
+    as the fake-quant forward of the same config quantises them.  `act_cfg` (the config's `act`
+    section, None for weight-only) is recorded by `new`; it is not a buffer, so the saved tensors are
+    those of the export.  Every other layout raises NotImplementedError saying why."""
 
     def __init__(self, weight, bias, scales, input_scale, need_pack, scales_name):
         super().__init__()
@@ -619,10 +679,64 @@ class VllmRealQuantLinear(nn.Module):
             self.bias = None
         self.register_buffer(scales_name, scales)
         self.register_buffer('input_scale', input_scale)
+        self.act_cfg = None
+        self._act_quantizer = None
+
+    def w8a8_unsupported(self):
+        """None when forward runs on llmc_gemm_w8a8_*, else the reason it does not."""
+        if 'weight_packed' in self._buffers:
+            return 'packed weights (weight_packed: W4A16 / W8A16 exports) have no real-quant forward'
+        if 'weight_scale_inv' in self._buffers:
+            return 'per_block FP8 exports (weight_scale_inv) have no real-quant forward'
+        if self.act_cfg is None:
+            return (f'weight-only {self.weight.dtype} exports have no real-quant forward: the W8A8 GEMM '
+                    'needs quantised activations')
+        wdt, aqt = self.weight.dtype, _cfg_get(self.act_cfg, 'quant_type', 'int-quant')
+        if wdt in (torch.bfloat16, torch.float16) and aqt == 'float-quant':
+            wdt = torch.float8_e4m3fn          # GPTQ's e4m3 codes, cast to the model dtype (see fp8_weight)
+        if wdt not in W8A8_ENTRY:
+            return f'{wdt} weights have no real-quant forward (int8 and float8_e4m3fn do)'
+        if (wdt == torch.int8) != (aqt == 'int-quant'):
+            return f'{wdt} weights with {aqt} activations have no real-quant forward'
+        static = bool(_cfg_get(self.act_cfg, 'static', False))
+        gran = _cfg_get(self.act_cfg, 'granularity')
+        if gran != ('per_tensor' if static else 'per_token'):
+            return (f'{"static" if static else "dynamic"} {gran} activations have no real-quant forward '
+                    '(per-token dynamic and per-tensor static do)')
+        if static and (self.input_scale is None or self.input_scale.numel() != 1):
+            return 'static activations need one input_scale'
+        return None
+
+    def activation_quantizer(self):
+        if self._act_quantizer is None:
+            self._act_quantizer = act_quantizer(self.act_cfg)
+        return self._act_quantizer
+
+    def fp8_weight(self):
+        """The weight as e4m3 codes.  GPTQ's deploy ends in convert_dtype, which casts an exported e4m3
+        weight to the model dtype (its values stay on the e4m3 grid, and the saved checkpoint holds
+        them so); the codes are recovered once, exactly, and kept outside the buffers.  A 16-bit weight
+        off the grid raises."""
+        w = self.weight
+        if w.dtype == torch.float8_e4m3fn:
+            return w
+        key = (w.data_ptr(), w._version)
+        if getattr(self, '_w_e4m3_key', None) != key:
+            q = w.to(torch.float8_e4m3fn)
+            if not torch.equal(q.to(w.dtype), w):
+                raise NotImplementedError(f'a {w.dtype} weight with FP8 activations must hold e4m3 grid values')
+            self._w_e4m3, self._w_e4m3_key = q, key
+        return self._w_e4m3
 
     @torch.no_grad()
     def forward(self, x):
-        raise NotImplementedError
+        reason = self.w8a8_unsupported()
+        if reason is not None:
+            raise NotImplementedError(reason)
+        static = bool(_cfg_get(self.act_cfg, 'static', False))
+        w = self.weight if self.weight.dtype == torch.int8 else self.fp8_weight()
+        return linear_forward_w8a8(x, w, self.weight_scale, self.activation_quantizer(),
+                                   self.input_scale if static else None, self.bias)
 
     @classmethod
     @torch.no_grad()
@@ -644,6 +758,7 @@ class VllmRealQuantLinear(nn.Module):
         new_module.weight_shape, new_module.weight_dtype = weight.shape, weight.dtype
         new_module.scales_shape, new_module.scales_dtype = scales.shape, scales.dtype
         new_module.zeros_shape = new_module.zeros_dtype = None
+        new_module.act_cfg = dict(act) if act is not None else None
         return new_module
 
     @classmethod

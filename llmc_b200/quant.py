@@ -588,6 +588,33 @@ class IntegerQuantizer(BaseQuantizer):
         t = self.quant_dequant(t, args['scales'], args['zeros'], args['qmax'], args['qmin'])
         return self.restore_tensor(t, org_shape).to(org_dtype)
 
+    def real_quant_act(self, act, input_scale=None):
+        """The int8 codes and fp32 scales of the W8A8 real-quant forward (llmc_gemm_w8a8_i8): the codes
+        the fake-quant forward of the same config rounds to, from the same pass, so rT(code * scale)
+        is its QDQ activation bit for bit.  -> (codes int8 [rows, K], scales fp32 [rows] or [1]).
+          input_scale None: per-token dynamic, fake_quant_act_dynamic's llmc_quant_dynamic pass with
+            codes out instead of QDQ; its `dtype` scales widened (exactly) to fp32.
+          input_scale given: per-tensor static, fake_quant_act_static's pass for its 0-dim fp32 scale
+            (x / s in fp32 rounded to the activation dtype, torch's scalar-operand path)."""
+        if self.bit != 8 or not self.sym or self.qmin != -128 or self.qmax != 127:
+            raise NotImplementedError('W8A8 real-quant activations are symmetric int8 [-128, 127] '
+                                      f'(got bit={self.bit} sym={self.sym} range=[{self.qmin}, {self.qmax}])')
+        t2d = act.reshape(-1, act.shape[-1])
+        t2d = t2d if t2d.is_contiguous() else t2d.contiguous()
+        codes = torch.empty(t2d.shape, dtype=torch.int8, device=t2d.device)
+        if input_scale is None:
+            if self.granularity != 'per_token':
+                raise NotImplementedError(f'dynamic W8A8 activations are per_token, not {self.granularity}')
+            scales, _ = self._dynamic(t2d, OUT_CODES_I8, out=codes)
+            return codes, scales.reshape(-1).float()
+        if self.granularity != 'per_tensor' or input_scale.numel() != 1:
+            raise NotImplementedError('static W8A8 activations take one per_tensor input_scale')
+        s = input_scale.reshape(1).to(device=t2d.device, dtype=torch.float32).contiguous()
+        rd = dtype_enum(t2d.dtype) if t2d.dtype != torch.float32 else -1
+        self._static(t2d, s, None, self.qmax, self.qmin, OUT_CODES_I8, codes, t2d.dtype, 0, t2d.shape[1],
+                     round_dtype=rd)
+        return codes, s
+
     # -- real quant -------------------------------------------------------------------------------
     def _code_dtype(self):
         if self.bit == 8:

@@ -190,6 +190,29 @@ class FloatQuantizer(BaseQuantizer):
         """quant.py:1083-1098."""
         return self._static(act, _zeros_to_one(args['scales']), 1).reshape(act.shape).to(act.dtype)
 
+    def real_quant_act(self, act, input_scale=None):
+        """The e4m3 bytes and fp32 scales of the W8A8 real-quant forward (llmc_gemm_w8a8_fp8): the bytes
+        the fake-quant forward of the same config rounds to, from the same llmc_fp8_quant pass, so
+        rT(fp32(byte) * scale) is its QDQ activation bit for bit.  A zero scale is returned as 1, the
+        scale the bytes were quantised with (quant.py:1062).  -> (e4m3 [rows, K], fp32 [rows] or [1]).
+          input_scale None: per-token dynamic (fake_quant_act_dynamic).
+          input_scale given: per-tensor static (fake_quant_act_static on its 0-dim scale); the caller's
+            tensor is not modified."""
+        if self.bit != 'e4m3':
+            raise NotImplementedError(f'W8A8 real-quant FP8 activations are e4m3, not {self.bit}')
+        t2d = act.reshape(-1, act.shape[-1])
+        t2d = t2d if t2d.is_contiguous() else t2d.contiguous()
+        if input_scale is None:
+            if self.granularity != 'per_token':
+                raise NotImplementedError(f'dynamic FP8 activations are per_token, not {self.granularity}')
+            out, scales = self._dynamic(t2d, 2)
+            return out, scales.reshape(-1).float()
+        if self.granularity != 'per_tensor' or input_scale.numel() != 1:
+            raise NotImplementedError('static FP8 activations take one per_tensor input_scale')
+        s = input_scale.reshape(1).to(device=t2d.device, dtype=torch.float32, copy=True)
+        _zeros_to_one(s)
+        return self._run(t2d, t2d.shape[1], 0, s, 2, 0, 1), s
+
     def _qshape(self, weight, scales):
         if self.granularity == 'per_tensor':
             return scales.view(1)
