@@ -390,7 +390,9 @@ int llmc_fp8_block_dequant(const void* w_fp8, int64_t M, int64_t N, int block, i
  *   llmc_fp8_act_quant  (csrc/fp8.cu) x [rows, K] `dtype`, K % 128 == 0: per contiguous group of 128
  *       elements s = max|x| / 448 and y = e4m3(x / s), both divisions the approximate div.full.f32
  *       the reference's kernel compiles to, the cast cvt.rn.satfinite; y [rows, K] e4m3 bytes,
- *       scales [rows, K/128] fp32.  No clamp: an all-zero group gives s = 0 and NaN codes.
+ *       scales [rows, K/128] fp32.  No clamp: an all-zero group gives s = 0 and NaN codes.  The
+ *       max (max.f32) skips NaN elements unless the whole group is NaN (s = NaN); +-inf gives
+ *       s = inf, +-0 codes for the finite elements and NaN for the infinite ones.
  *   llmc_gemm_fp8_block (csrc/gemm_fp8.cu) out[M, N] = sum over 128-deep K blocks kb, ascending,
  *       acc = fma(dot_kb * a_s[m, kb], b_s[n / 128, kb], acc), the dot on wgmma e4m3 (Hopper's
  *       reduced-precision accumulator, fresh per K block).  a [M, K], b [N, K] e4m3 (K-major),

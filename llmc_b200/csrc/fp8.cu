@@ -244,6 +244,9 @@ extern "C" int llmc_fp8_block_dequant(const void* w_fp8, int64_t M, int64_t N, i
 // instructions are issued here, so scales and codes match the reference's bit for bit on the same
 // hardware.  Reproduced quirk: unlike weight_cast_to_fp8 there is no clamp(min=1e-5), so an
 // all-zero group gets s = 0 and NaN codes (0 / 0), which fp8_gemm spreads over its output row.
+// max.f32 returns the other operand when one is NaN, so a NaN element does not reach the scale
+// (its own code is NaN) unless the whole group is NaN; an infinite element makes s = inf, the
+// group's finite codes +-0 and its infinite ones NaN.
 // Half a warp per group, 8 elements per lane: one 16-byte load (two for fp32), one 8-byte store.
 namespace llmc {
 
@@ -278,9 +281,10 @@ fp8_act_quant_kernel(const void* __restrict__ x, int64_t groups, uint8_t* __rest
 #pragma unroll
       for (int i = 0; i < 8; ++i) v[i] = 0.f;
     }
-    float mx = 0.f;
+    // seeded with an element, not 0, so that an all-NaN group keeps a NaN max like the reference's
+    float mx = fabsf(v[0]);
 #pragma unroll
-    for (int i = 0; i < 8; ++i) mx = fmaxf(mx, fabsf(v[i]));
+    for (int i = 1; i < 8; ++i) mx = fmaxf(mx, fabsf(v[i]));
     mx = warp_max(mx, 16);
     const float s = div_full(mx, 448.f);
     if (!live) continue;

@@ -22,10 +22,12 @@ def _rT(x32, dtype):
     return x32.to(dtype).float() if dtype != torch.float32 else x32
 
 
-def _fma32(a64, b64, c32):
+def fma32(a64, b64, c32):
     """fp32 fmaf(a, b, c) for fp32-representable a, b: a*b is exact in float64 (≤ 48-bit
     significands, no float64 underflow), the sum is rounded to odd in float64 and then to fp32,
-    which is a single correct rounding because float64 carries more than 24 + 1 bits."""
+    which is a single correct rounding because float64 carries more than 24 + 1 bits.  The TwoSum
+    error's sign says which way an inexact sum was rounded; it can lie far below the sum's ulp
+    (an fp32 subnormal c beside a product near 1), so it picks the direction, not its size."""
     p = a64 * b64
     c = c32.double()
     s = p + c
@@ -33,7 +35,7 @@ def _fma32(a64, b64, c32):
     err = (p - (s - bb)) + (c - bb)                     # TwoSum: p + c = s + err exactly
     odd = (s.view(torch.int64) & 1) == 1
     fix = (err != 0) & ~odd & torch.isfinite(s)
-    s = torch.where(fix, torch.nextafter(s, s + err * 2.0 ** 60), s)
+    s = torch.where(fix, torch.nextafter(s, torch.full_like(s, torch.inf).copysign(err)), s)
     return s.float()
 
 
@@ -59,7 +61,7 @@ def rmsnorm_sumsq(x):
     for i in range(it):
         for k in range(8):
             v = xp[:, i, :, k]
-            acc = _fma32(v, v, acc)
+            acc = fma32(v, v, acc)
     warp = _butterfly(acc.view(rows, WARPS, 32))
     lanes = torch.zeros(rows, 32, dtype=torch.float32, device=x.device)
     lanes[:, :WARPS] = warp

@@ -4,17 +4,28 @@ block_wise_fp8_forward_func (module_utils.py:40-45).
 
   * act_quant: s = max|x| / 448 and y = e4m3(x / s) per contiguous group of 128, with IEEE
     division.  The reference's compiled kernel (and csrc/fp8.cu) divides with the approximate
-    div.full.f32 (<= 2 ulp), so a GPU scale may differ from this one by up to 2 ulp.
-  * fp8_gemm: per 128-deep K block, ascending, d = the dot of exact products rounded once to fp32,
-    then acc = fma(fp32(d * a_s[m]), b_s[n / 128], acc).  The fma is emulated in float64 with a
-    single rounding to fp32, exact whenever d * a_s * b_s + acc is exact in float64 (always on the
-    integer grids the tests use).  The Hopper tensor core's reduced-precision dot is not modelled.
+    div.full.f32 (<= 2 ulp), so a GPU scale may differ from this one by up to 2 ulp.  The max is
+    the reference's compiled `max.f32`, which returns the other operand when one is NaN: a NaN
+    element does not reach the scale unless its whole group is NaN.  +-inf gives s = inf, so the
+    group's finite elements quantise to +-0 and its infinite ones to NaN; an all-zero group gives
+    s = 0 and NaN codes.
+  * fp8_gemm: per 128-deep K block, ascending, d = the dot of exact products rounded once to fp32
+    (NaN wherever the block's row of a or column of b holds a NaN code, as on the tensor core),
+    then acc = fma(fp32(d * a_s[m]), b_s[n / 128], acc), one correctly rounded fp32 fma.  The
+    Hopper tensor core's reduced-precision dot is not modelled: on operands whose 128-deep dots
+    are exact (w8a8_oracle.fp8_exact_operands) the kernel must match this bit for bit.
   * fp8_gemm_exact: the same sum in float64 without intermediate rounding, plus the per-element
     magnitude sum_k |a_s a_k b_s b_k| that error bounds scale with.
 """
 import torch
 
+from oracle.glue_oracle import fma32
+
 FMAX = 448.0
+
+# the order fp8_gemm promotes in, and three others that must give different bits when the
+# promotion rounds (the sanity check of a test that claims to pin the order)
+PROMOTIONS = ('a_s-then-b_s', 'b_s-then-a_s', 'a_s*b_s-fused', 'k-descending')
 
 
 def act_quant(x, block_size=128):
@@ -22,7 +33,10 @@ def act_quant(x, block_size=128):
     K = x.shape[-1]
     assert K % block_size == 0
     xs = x.float().reshape(*x.shape[:-1], K // block_size, block_size)
-    s = xs.abs().amax(-1) / torch.tensor(FMAX)
+    ax = xs.abs()
+    mx = ax.masked_fill(ax.isnan(), -1.0).amax(-1)                     # max.f32 skips NaN ...
+    mx = torch.where(mx < 0, torch.nan, mx)                             # ... unless all are NaN
+    s = mx / torch.tensor(FMAX)
     q = (xs / s[..., None]).clamp(-FMAX, FMAX).to(torch.float8_e4m3fn)   # satfinite; NaN stays NaN
     return q.reshape(x.shape), s
 
@@ -37,14 +51,30 @@ def _blocks(a, a_s, b, b_s):
     return A, B, sa, sb, kb
 
 
-def fp8_gemm(a, a_s, b, b_s):
-    """a [..., K], b [N, K] e4m3; a_s [..., K/128], b_s [ceil(N/128), K/128] -> fp32 [..., N]."""
+def _dot(Ak, Bk):
+    """[M, 128] x [N, 128] e4m3 values (float64) -> fp32 [M, N]: exact in float64 (products are
+    multiples of 2^-18 below 2^18), rounded once; NaN where either operand row holds a NaN."""
+    d = (Ak.nan_to_num(0.0) @ Bk.nan_to_num(0.0).T).float()
+    nan = Ak.isnan().any(-1)[:, None] | Bk.isnan().any(-1)[None, :]
+    return d.masked_fill(nan, torch.nan)
+
+
+def fp8_gemm(a, a_s, b, b_s, promotion='a_s-then-b_s'):
+    """a [..., K], b [N, K] e4m3; a_s [..., K/128], b_s [ceil(N/128), K/128] -> fp32 [..., N].
+    `promotion` other than the first of PROMOTIONS computes a wrong order on purpose."""
+    assert promotion in PROMOTIONS, promotion
     A, B, sa, sb, kb = _blocks(a, a_s, b, b_s)
-    acc = torch.zeros(A.shape[0], B.shape[0], dtype=torch.float32)
-    for k in range(kb):
-        d = (A[:, k] @ B[:, k].T).float()                  # exact in float64, rounded once
-        t = d * sa[:, k:k + 1]                              # mul.f32
-        acc = (t.double() * sb[:, k].double() + acc.double()).float()   # fma.rn.f32
+    acc = torch.zeros(A.shape[0], B.shape[0], dtype=torch.float32, device=A.device)
+    order = range(kb - 1, -1, -1) if promotion == 'k-descending' else range(kb)
+    for k in order:
+        d = _dot(A[:, k], B[:, k])
+        s_m, s_n = sa[:, k:k + 1], sb[:, k][None, :]
+        if promotion == 'b_s-then-a_s':
+            acc = fma32((d * s_n).double(), s_m.double(), acc)
+        elif promotion == 'a_s*b_s-fused':
+            acc = fma32(d.double(), (s_m * s_n).double(), acc)
+        else:
+            acc = fma32((d * s_m).double(), s_n.double(), acc)             # mul.rn, then fma.rn
     return acc.reshape(*a.shape[:-1], b.shape[0])
 
 
