@@ -311,6 +311,24 @@ int llmc_spqr_colblock(float* W, const float* Hinv, int64_t R, int64_t C, int64_
 int llmc_gemm_bf16(const void* x, const void* w, const void* bias, void* y, int64_t M,
                    int64_t N, int64_t K, int dtype, void* stream);
 
+/* K6 with the block glue that follows it fused into the epilogue, bit for bit llmc_gemm_bf16
+ * followed by the block_ops kernel named (no bias; checks as llmc_gemm_bf16's, plus those listed):
+ *   llmc_gemm_rope_qkv  w_qkv = [Wq; Wk; Wv] [n_q + n_k + n_v, K]: q[M, n_q], k[M, n_k], v[M, n_v]
+ *                       with llmc_rope (head_dim 128, cos / sin [seq, 128]) applied to q and k;
+ *                       row r is position r % seq.  n_q, n_k multiples of 256, n_v of 8,
+ *                       M a multiple of seq.
+ *   llmc_gemm_swiglu    w_gate_up [2 * inter, K] = gate and up interleaved in 128-row blocks
+ *                       (gate rows 0..127, up rows 0..127, gate rows 128..255, ...):
+ *                       act[M, inter] = llmc_silu_mul(gate, up); inter a multiple of 128.
+ *   llmc_gemm_residual  y[M, N] = llmc_add(res, X W^T); y may be res; N a multiple of 8. */
+int llmc_gemm_rope_qkv(const void* x, const void* w_qkv, void* q, void* k, void* v,
+                       const void* cosv, const void* sinv, int64_t M, int64_t n_q, int64_t n_k,
+                       int64_t n_v, int64_t K, int64_t seq, int dtype, void* stream);
+int llmc_gemm_swiglu(const void* x, const void* w_gate_up, void* act, int64_t M, int64_t inter,
+                     int64_t K, int dtype, void* stream);
+int llmc_gemm_residual(const void* x, const void* w, const void* res, void* y, int64_t M,
+                       int64_t N, int64_t K, int dtype, void* stream);
+
 /* ------------------------------------------------------------------------------------
  * K6  llmc_gemm_w4a16 — fake-quant forward on PACKED weights:
  *   Y[M,N] = X[M,K] · dequant(Wq)[N,K]^T (+ bias), dequant(Wq)[n,k] =

@@ -66,6 +66,10 @@ SIGNATURES = {
                                    c_int, c_int, c_int, c_int, c_vp, c_int, c_vp, c_vp, c_vp, c_vp,
                                    c_vp, c_vp, c_vp, c_i64, c_vp]),
     'llmc_gemm_bf16': (c_int, [c_vp, c_vp, c_vp, c_vp, c_i64, c_i64, c_i64, c_int, c_vp]),
+    'llmc_gemm_rope_qkv': (c_int, [c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_i64, c_i64, c_i64, c_i64,
+                                   c_i64, c_i64, c_int, c_vp]),
+    'llmc_gemm_swiglu': (c_int, [c_vp, c_vp, c_vp, c_i64, c_i64, c_i64, c_int, c_vp]),
+    'llmc_gemm_residual': (c_int, [c_vp, c_vp, c_vp, c_vp, c_i64, c_i64, c_i64, c_int, c_vp]),
     'llmc_rmsnorm': (c_int, [c_vp, c_vp, c_vp, c_i64, c_i64, c_f32, c_int, c_vp]),
     'llmc_rope': (c_int, [c_vp, c_vp, c_vp, c_i64, c_i64, c_i64, c_i64, c_int, c_vp]),
     'llmc_silu_mul': (c_int, [c_vp, c_vp, c_vp, c_i64, c_int, c_vp]),

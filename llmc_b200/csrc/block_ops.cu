@@ -92,7 +92,7 @@ silu_mul_kernel(const void* __restrict__ g, const void* __restrict__ u, void* __
     load8<DT>(u, i << 3, b);
 #pragma unroll
     for (int k = 0; k < 8; ++k) {
-      const float sg = DType<DT>::rT(a[k] / (1.0f + expf(-a[k])));       // F.silu in fp32, rounded
+      const float sg = DType<DT>::rT(silu_f32(a[k]));                      // F.silu in fp32, rounded
       o[k] = fmul_rn(sg, b[k]);                                            // store8 rounds
     }
     store8<DT>(y, i << 3, o);

@@ -269,6 +269,10 @@ __device__ __forceinline__ float fadd_rn(float a, float b) { return __fadd_rn(a,
 __device__ __forceinline__ float fsub_rn(float a, float b) { return __fsub_rn(a, b); }
 __device__ __forceinline__ float fma_rn(float a, float b, float c) { return __fmaf_rn(a, b, c); }
 
+// F.silu in fp32 (IEEE division), shared by llmc_silu_mul and the SwiGLU epilogue of the forward
+// GEMM, which must agree bit for bit.
+__device__ __forceinline__ float silu_f32(float x) { return x / (1.0f + expf(-x)); }
+
 inline bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15u) == 0; }
 
 }  // namespace llmc

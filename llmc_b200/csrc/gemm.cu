@@ -46,6 +46,27 @@ struct GemmParams {
   int gn;                   // rasterisation group: n-tiles (GEMM) / m-blocks (SYRK) per group
 };
 
+// Operands of the fused GEMM epilogues (see Epilogue).  A kernel argument of its own: grown
+// GemmParams fields change the plain GEMM's and the SYRK's register allocation.
+struct EpiParams {
+  const void* res;          // kEpiResidual: the residual [M, N], may be GemmParams::out
+  void* out_k;              // kEpiRopeQkv: k [M, n_k] and v [M, N - n_q - n_k]; q is GemmParams::out
+  void* out_v;
+  const void* cosv;         // kEpiRopeQkv: [seq, 128] rotary tables in the output dtype
+  const void* sinv;
+  int64_t n_q, n_k, seq;
+};
+
+// What the GEMM does with a finished tile.  Every fused epilogue first rounds the accumulator to
+// the output dtype, as the plain GEMM's store does, so it computes exactly what the plain GEMM
+// followed by the block_ops.cu kernel of the same name computes.
+enum Epilogue {
+  kEpiLinear,     // Y = X W^T (+ bias)
+  kEpiRopeQkv,    // W = [Wq; Wk; Wv]: q, k, v to three outputs, rope_kernel applied to q and k
+  kEpiSwiGLU,     // W = gate / up interleaved in 128-row blocks: act = silu(gate) * up
+  kEpiResidual,   // Y = res + X W^T (add_kernel)
+};
+
 struct Unit {
   int m_blk, n_blk, kb0, kb1, split;
 };
@@ -89,10 +110,123 @@ __device__ __forceinline__ Unit decode_unit(const GemmParams& p, int u) {
   return t;
 }
 
-template <bool kSyrk, bool kBf16>
+// ---- fused epilogues: this thread's part of the 64-row half tile (fragment layout at
+// tc::wgmma_m64n128k16_bf16) whose row 0 is row0 -----------------------------------------------
+__device__ __forceinline__ int64_t frag_row(int64_t row0, int i) {
+  const int tid = threadIdx.x & 127, lane = threadIdx.x & 31;
+  return row0 + (tid >> 5) * 16 + (lane >> 2) + 8 * i;
+}
+
+// rope_kernel on one head (head_dim 128) of q or k: acc holds the head's 128 columns, which go to
+// out[row][col0 + d] (ld even).  Columns d and d + 64 of a row are fragments j and j + 8 of the same
+// thread.  The position of a row is row % seq: chunks hold whole samples.
+template <int DT>
+__device__ __forceinline__ void store_rope_m64n128(const float (&acc)[64], int64_t row0, int64_t col0,
+                                                   int64_t M, const EpiParams& e, int64_t ld,
+                                                   void* out) {
+  using T = DType<DT>;
+  const int lane = threadIdx.x & 31;
+  const uint32_t* cosv = static_cast<const uint32_t*>(e.cosv);
+  const uint32_t* sinv = static_cast<const uint32_t*>(e.sinv);
+#pragma unroll
+  for (int i = 0; i < 2; ++i) {
+    const int64_t row = frag_row(row0, i);
+    if (row >= M) continue;
+    const int64_t tab = (row % e.seq) * 64 + (lane & 3);          // 32-bit pairs of [seq, 128]
+    uint16_t* o = static_cast<uint16_t*>(out) + row * ld + col0 + 2 * (lane & 3);
+#pragma unroll
+    for (int j = 0; j < 8; ++j) {
+      const uint32_t c1 = __ldg(cosv + tab + 4 * j), s1 = __ldg(sinv + tab + 4 * j);
+      const uint32_t c2 = __ldg(cosv + tab + 32 + 4 * j), s2 = __ldg(sinv + tab + 32 + 4 * j);
+      float oa[2], ob[2];
+#pragma unroll
+      for (int c = 0; c < 2; ++c) {
+        const float a = T::rT(acc[4 * j + 2 * i + c]), b = T::rT(acc[4 * (j + 8) + 2 * i + c]);
+        const float cs1 = c ? pair_hi<DT>(c1) : pair_lo<DT>(c1);
+        const float sn1 = c ? pair_hi<DT>(s1) : pair_lo<DT>(s1);
+        const float cs2 = c ? pair_hi<DT>(c2) : pair_lo<DT>(c2);
+        const float sn2 = c ? pair_hi<DT>(s2) : pair_lo<DT>(s2);
+        oa[c] = fadd_rn(T::rT(fmul_rn(a, cs1)), T::rT(fmul_rn(-b, sn1)));
+        ob[c] = fadd_rn(T::rT(fmul_rn(b, cs2)), T::rT(fmul_rn(a, sn2)));
+      }
+      *reinterpret_cast<uint32_t*>(o + 8 * j) = pack_pair<DT>(oa[0], oa[1]);
+      *reinterpret_cast<uint32_t*>(o + 8 * j + 64) = pack_pair<DT>(ob[0], ob[1]);
+    }
+  }
+}
+
+// One 64 x 256 half tile of kEpiRopeQkv: the n-tile's columns lie in one of q, k, v (n_q and n_k
+// are multiples of 256); q and k tiles are two heads each.
+template <int DT>
+__device__ __forceinline__ void store_qkv_tile(const float (&acc0)[64], const float (&acc1)[64],
+                                               int64_t row0, int64_t col0, const GemmParams& p,
+                                               const EpiParams& e) {
+  if (col0 < e.n_q) {
+    store_rope_m64n128<DT>(acc0, row0, col0, p.M, e, e.n_q, p.out);
+    store_rope_m64n128<DT>(acc1, row0, col0 + 128, p.M, e, e.n_q, p.out);
+  } else if (col0 < e.n_q + e.n_k) {
+    store_rope_m64n128<DT>(acc0, row0, col0 - e.n_q, p.M, e, e.n_k, e.out_k);
+    store_rope_m64n128<DT>(acc1, row0, col0 - e.n_q + 128, p.M, e, e.n_k, e.out_k);
+  } else {
+    const int64_t nv = p.N - e.n_q - e.n_k, c = col0 - e.n_q - e.n_k;
+    store_linear_m64n128<DT>(acc0, row0, c, p.M, nv, nv, nullptr, e.out_v);
+    store_linear_m64n128<DT>(acc1, row0, c + 128, p.M, nv, nv, nullptr, e.out_v);
+  }
+}
+
+// silu_mul_kernel on one 64 x 256 half tile of kEpiSwiGLU: gate in acc0, up in acc1, both for the
+// 128 act columns from col0 of act[M, ld].
+template <int DT>
+__device__ __forceinline__ void store_swiglu_m64n128(const float (&gate)[64], const float (&up)[64],
+                                                     int64_t row0, int64_t col0, int64_t M,
+                                                     int64_t ld, void* out) {
+  using T = DType<DT>;
+  const int lane = threadIdx.x & 31;
+#pragma unroll
+  for (int i = 0; i < 2; ++i) {
+    const int64_t row = frag_row(row0, i);
+    if (row >= M) continue;
+    uint16_t* o = static_cast<uint16_t*>(out) + row * ld + col0 + 2 * (lane & 3);
+#pragma unroll
+    for (int j = 0; j < 16; ++j) {
+      float v[2];
+#pragma unroll
+      for (int c = 0; c < 2; ++c)
+        v[c] = fmul_rn(T::rT(silu_f32(T::rT(gate[4 * j + 2 * i + c]))), T::rT(up[4 * j + 2 * i + c]));
+      *reinterpret_cast<uint32_t*>(o + 8 * j) = pack_pair<DT>(v[0], v[1]);
+    }
+  }
+}
+
+// add_kernel(res, Y) on one half tile of kEpiResidual (N even).  Each element of res is read by the
+// thread that then writes it, so res may be the output.
+template <int DT>
+__device__ __forceinline__ void store_residual_m64n128(const float (&acc)[64], int64_t row0,
+                                                       int64_t col0, const GemmParams& p,
+                                                       const void* res) {
+  using T = DType<DT>;
+  const int lane = threadIdx.x & 31;
+#pragma unroll
+  for (int j = 0; j < 16; ++j) {
+    const int64_t col = col0 + 8 * j + 2 * (lane & 3);
+    if (col >= p.N) continue;
+#pragma unroll
+    for (int i = 0; i < 2; ++i) {
+      const int64_t row = frag_row(row0, i);
+      if (row >= p.M) continue;
+      const int64_t off = row * p.ld_out + col;
+      const uint32_t r = *(static_cast<const uint32_t*>(res) + off / 2);
+      const float v0 = fadd_rn(pair_lo<DT>(r), T::rT(acc[4 * j + 2 * i]));
+      const float v1 = fadd_rn(pair_hi<DT>(r), T::rT(acc[4 * j + 2 * i + 1]));
+      *(static_cast<uint32_t*>(p.out) + off / 2) = pack_pair<DT>(v0, v1);
+    }
+  }
+}
+
+template <bool kSyrk, bool kBf16, int kEpi = kEpiLinear>
 __global__ void __launch_bounds__(kThreads, 1)
 wgmma_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
-                  const GemmParams p) {
+                  const GemmParams p, const EpiParams e) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = ring_base(smem_raw);
   const Ring<kStages> ring(smem + kStages * kStageBytes);
@@ -185,8 +319,17 @@ wgmma_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
     const int64_t col0 = static_cast<int64_t>(t.n_blk) * BN;
     if constexpr (!kSyrk) {
       constexpr int DT = kBf16 ? LLMC_BF16 : LLMC_F16;
-      store_linear_m64n128<DT>(acc0, row0, col0, p.M, p.N, p.ld_out, p.bias, p.out);
-      store_linear_m64n128<DT>(acc1, row0, col0 + 128, p.M, p.N, p.ld_out, p.bias, p.out);
+      if constexpr (kEpi == kEpiLinear) {
+        store_linear_m64n128<DT>(acc0, row0, col0, p.M, p.N, p.ld_out, p.bias, p.out);
+        store_linear_m64n128<DT>(acc1, row0, col0 + 128, p.M, p.N, p.ld_out, p.bias, p.out);
+      } else if constexpr (kEpi == kEpiRopeQkv) {
+        store_qkv_tile<DT>(acc0, acc1, row0, col0, p, e);
+      } else if constexpr (kEpi == kEpiSwiGLU) {
+        store_swiglu_m64n128<DT>(acc0, acc1, row0, col0 / 2, p.M, p.ld_out, p.out);
+      } else {
+        store_residual_m64n128<DT>(acc0, row0, col0, p, e.res);
+        store_residual_m64n128<DT>(acc1, row0, col0 + 128, p, e.res);
+      }
     } else {
       // fp32 partial slab `t.split` of the split-K sum
       float* slab = static_cast<float*>(p.out) + static_cast<int64_t>(t.split) * p.M * p.ld_out;
@@ -308,17 +451,16 @@ static SyrkPlan plan_syrk(int64_t T, int64_t C) {
   return s;
 }
 
-}  // namespace llmc
-
-using namespace llmc;
-
-extern "C" int llmc_gemm_bf16(const void* x, const void* w, const void* bias, void* y, int64_t M,
-                              int64_t N, int64_t K, int dtype, void* stream) {
+// Checks and launches the forward GEMM Y[M, N] = X[M, K] W[N, K]^T with epilogue kEpi into p.out
+// (and e's outputs; the caller checks e's pointers).  p's other fields are filled in here.
+template <int kEpi>
+static int launch_gemm(const void* x, const void* w, int64_t M, int64_t N, int64_t K, int dtype,
+                       GemmParams p, const EpiParams& e, void* stream) {
   LLMC_CHECK_ARG(M >= 0 && N >= 0 && K > 0, "gemm: bad shape");
   if (M == 0 || N == 0) return LLMC_OK;
-  LLMC_CHECK_ARG(x && w && y, "gemm: null pointer");
+  LLMC_CHECK_ARG(x && w && p.out, "gemm: null pointer");
   LLMC_CHECK_ARG(dtype == LLMC_BF16 || dtype == LLMC_F16, "gemm: dtype must be bf16 or fp16");
-  if (K % 8 != 0 || !aligned16(x) || !aligned16(w) || !aligned16(y)) {
+  if (K % 8 != 0 || !aligned16(x) || !aligned16(w) || !aligned16(p.out)) {
     set_last_error("gemm: K=%lld must be a multiple of 8 and pointers 16-byte aligned", (long long)K);
     return LLMC_EALIGN;
   }
@@ -329,9 +471,7 @@ extern "C" int llmc_gemm_bf16(const void* x, const void* w, const void* bias, vo
   if (int rc = encode_tmap_2d(&tmB, w, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, N, K, K, BN, BK,
                               CU_TENSOR_MAP_SWIZZLE_128B))
     return rc;
-  GemmParams p{};
   p.M = M; p.N = N; p.K = K;
-  p.out = y; p.bias = bias; p.ld_out = N;
   p.n_tiles_n = static_cast<int>((N + BN - 1) / BN);
   const int64_t mt = (M + BM - 1) / BM;
   LLMC_CHECK_ARG(mt * p.n_tiles_n < (1ll << 31), "gemm: too many tiles");
@@ -342,9 +482,66 @@ extern "C" int llmc_gemm_bf16(const void* x, const void* w, const void* bias, vo
   p.kb_per_split = p.kb_total;
   p.gn = l2_group_width(static_cast<int64_t>(BN) * K * 2, p.n_tiles_n);   // K > 0: one n-tile's bytes
   cudaStream_t st = static_cast<cudaStream_t>(stream);
-  return launch_persistent(dtype == LLMC_BF16 ? wgmma_gemm_kernel<false, true>
-                                              : wgmma_gemm_kernel<false, false>,
-                           p.num_units, kThreads, kSmemBytes, st, tmA, tmB, p);
+  return launch_persistent(dtype == LLMC_BF16 ? wgmma_gemm_kernel<false, true, kEpi>
+                                              : wgmma_gemm_kernel<false, false, kEpi>,
+                           p.num_units, kThreads, kSmemBytes, st, tmA, tmB, p, e);
+}
+
+}  // namespace llmc
+
+using namespace llmc;
+
+extern "C" int llmc_gemm_bf16(const void* x, const void* w, const void* bias, void* y, int64_t M,
+                              int64_t N, int64_t K, int dtype, void* stream) {
+  GemmParams p{};
+  p.out = y; p.bias = bias; p.ld_out = N;
+  return launch_gemm<kEpiLinear>(x, w, M, N, K, dtype, p, EpiParams{}, stream);
+}
+
+extern "C" int llmc_gemm_rope_qkv(const void* x, const void* w_qkv, void* q, void* k, void* v,
+                                  const void* cosv, const void* sinv, int64_t M, int64_t n_q,
+                                  int64_t n_k, int64_t n_v, int64_t K, int64_t seq, int dtype,
+                                  void* stream) {
+  LLMC_CHECK_ARG(n_q > 0 && n_k > 0 && n_v > 0 && seq > 0 && M % seq == 0,
+                 "gemm_rope_qkv: need n_q, n_k, n_v, seq > 0 and M a multiple of seq");
+  LLMC_CHECK_ARG(n_q % BN == 0 && n_k % BN == 0 && n_v % 8 == 0,
+                 "gemm_rope_qkv: n_q=%lld and n_k=%lld must be multiples of %d, n_v=%lld of 8",
+                 (long long)n_q, (long long)n_k, BN, (long long)n_v);
+  LLMC_CHECK_ARG(k && v && cosv && sinv, "gemm_rope_qkv: null pointer");
+  if (!aligned16(k) || !aligned16(v) || !aligned16(cosv) || !aligned16(sinv)) {
+    set_last_error("gemm_rope_qkv: pointers must be 16-byte aligned");
+    return LLMC_EALIGN;
+  }
+  GemmParams p{};
+  p.out = q;
+  EpiParams e{};
+  e.out_k = k; e.out_v = v; e.cosv = cosv; e.sinv = sinv;
+  e.n_q = n_q; e.n_k = n_k; e.seq = seq;
+  return launch_gemm<kEpiRopeQkv>(x, w_qkv, M, n_q + n_k + n_v, K, dtype, p, e, stream);
+}
+
+extern "C" int llmc_gemm_swiglu(const void* x, const void* w_gate_up, void* act, int64_t M,
+                                int64_t inter, int64_t K, int dtype, void* stream) {
+  LLMC_CHECK_ARG(inter > 0 && inter % 128 == 0,
+                 "gemm_swiglu: inter=%lld must be a positive multiple of 128", (long long)inter);
+  GemmParams p{};
+  p.out = act; p.ld_out = inter;
+  return launch_gemm<kEpiSwiGLU>(x, w_gate_up, M, 2 * inter, K, dtype, p, EpiParams{}, stream);
+}
+
+extern "C" int llmc_gemm_residual(const void* x, const void* w, const void* res, void* y, int64_t M,
+                                  int64_t N, int64_t K, int dtype, void* stream) {
+  LLMC_CHECK_ARG(N % 8 == 0, "gemm_residual: N=%lld must be a multiple of 8", (long long)N);
+  LLMC_CHECK_ARG(res != nullptr, "gemm_residual: null pointer");
+  if (!aligned16(res)) {
+    set_last_error("gemm_residual: pointers must be 16-byte aligned");
+    return LLMC_EALIGN;
+  }
+  GemmParams p{};
+  p.out = y; p.ld_out = N;
+  EpiParams e{};
+  e.res = res;
+  return launch_gemm<kEpiResidual>(x, w, M, N, K, dtype, p, e, stream);
 }
 
 extern "C" int64_t llmc_syrk_workspace_bytes(int64_t T, int64_t C) {
@@ -383,7 +580,7 @@ extern "C" int llmc_syrk_accum(const void* x, int64_t T, int64_t C, int dtype, f
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   int rc = launch_persistent(dtype == LLMC_BF16 ? wgmma_gemm_kernel<true, true>
                                                 : wgmma_gemm_kernel<true, false>,
-                             p.num_units, kThreads, kSmemBytes, st, tmX, tmX, p);
+                             p.num_units, kThreads, kSmemBytes, st, tmX, tmX, p, EpiParams{});
   if (rc) return rc;
   // gptq.py:283-290: H *= n/(n+b); H += (sqrt(2/(n+b)) X)^T (sqrt(2/(n+b)) X)
   const float fa = static_cast<float>(n / (n + b));

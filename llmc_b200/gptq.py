@@ -22,7 +22,8 @@ import torch.nn as nn
 from . import dist_utils
 from . import gptq_ops as ops
 from .blockwise import ALGO_REGISTRY, BaseBlockwiseQuantization
-from .module_utils import _LLMC_LINEAR_TYPES_, _TRANSFORMERS_LINEAR_TYPES_, FakeQuantLinear
+from .module_utils import (_LLMC_LINEAR_TYPES_, _TRANSFORMERS_LINEAR_TYPES_, FakeQuantLinear,
+                           linear_residual)
 
 
 def norm_into(ln, src, dst):
@@ -185,7 +186,7 @@ class GPTQ(BaseBlockwiseQuantization):
                  (not self.true_sequential and not self.quant_out)
         return (staged and not self.data_free
                 and not self.act_static and hasattr(block, 'mlp') and hasattr(block, 'self_attn')
-                and hasattr(block.self_attn, 'attend'))
+                and hasattr(block.self_attn, 'qkv_rope') and hasattr(block.mlp, 'gate_up_act'))
 
     @torch.no_grad()
     def block_opt(self, block):
@@ -240,32 +241,32 @@ class GPTQ(BaseBlockwiseQuantization):
             for i in range(0, N, chunk):
                 yield slice(i, min(i + chunk, N))
 
-        from . import block_ops
-
         x1 = torch.empty_like(X)
         for s in chunks():
             norm_into(block.input_layernorm, X[s], x1[s])
         stage(subsets[0], x1)
         att = torch.empty((N, X.shape[1], a.heads * a.head_dim), dtype=X.dtype, device=X.device)
+        w_fused = a.fused_qkv_weight(X.dtype)       # the stage's weights, once for every chunk
         for s in chunks():
-            att[s] = a.attend(a.q_proj(x1[s]), a.k_proj(x1[s]), a.v_proj(x1[s]), pos)
-        del x1
+            att[s] = a.sdpa(*a.qkv_rope(x1[s], pos, w_fused))
+        del x1, w_fused
         stage(subsets[1], att)
         h = torch.empty_like(X)
         for s in chunks():
-            block_ops.add(X[s], a.o_proj(att[s]), out=h[s])
+            linear_residual(a.o_proj, att[s], X[s], out=h[s])
         del att
         x3 = torch.empty_like(X)
         for s in chunks():
             norm_into(block.post_attention_layernorm, h[s], x3[s])
         stage(subsets[2], x3)
         act = torch.empty((N, X.shape[1], m.gate_proj.out_features), dtype=X.dtype, device=X.device)
+        w_fused = m.fused_gate_up_weight(X.dtype)
         for s in chunks():
-            m.act(m.gate_proj(x3[s]), m.up_proj(x3[s]), out=act[s])
-        del x3
+            m.gate_up_act(x3[s], out=act[s], w_gate_up=w_fused)
+        del x3, w_fused
         stage(subsets[3], act)
         for s in chunks():
-            block_ops.add(h[s], m.down_proj(act[s]), out=h[s])
+            linear_residual(m.down_proj, act[s], h[s], out=h[s])
         del act
         self.input['stacked'] = h
         self.input['data'] = list(torch.split(h, bs_list, dim=0))

@@ -37,6 +37,103 @@ def linear_forward(x, weight, bias=None):
     return y.reshape(*x.shape[:-1], N)
 
 
+# ---- the forward GEMM with the block glue that follows it in its epilogue -------------------------
+# Each computes exactly what linear_forward followed by the block_ops kernel computes; the spans are
+# 'gemm' spans like linear_forward's, with the GEMM's 2MNK flops.
+def _gemm_operands(x, w):
+    require_cuda(x, w)
+    if x.dtype != w.dtype:
+        raise TypeError(f'activation dtype {x.dtype} != weight dtype {w.dtype}')
+    x2 = x.reshape(-1, x.shape[-1])
+    return (x2 if x2.is_contiguous() else x2.contiguous()), (w if w.is_contiguous() else w.contiguous())
+
+
+def interleave_gate_up(wg, wu):
+    """The weight of llmc_gemm_swiglu: gate and up rows interleaved in blocks of 128
+    ([g 0:128, u 0:128, g 128:256, u 128:256, ...])."""
+    inter, K = wg.shape
+    assert wu.shape == wg.shape and inter % 128 == 0
+    return torch.stack([wg.reshape(-1, 128, K), wu.reshape(-1, 128, K)], dim=1).reshape(2 * inter, K)
+
+
+def gemm_rope_qkv(x, w_qkv, n_q, n_k, cos, sin):
+    """q, k, v = x [B, S, K] @ [Wq; Wk; Wv]^T with block_ops.rope_ applied to q and k (head_dim 128,
+    cos / sin [S, 128]); three contiguous [B, S, width] tensors."""
+    B, S, K = x.shape
+    x2, w = _gemm_operands(x, w_qkv)
+    n_v = w.shape[0] - n_q - n_k
+    M = x2.shape[0]
+    q, k, v = (torch.empty((B, S, n), dtype=x.dtype, device=x.device) for n in (n_q, n_k, n_v))
+    N = w.shape[0]
+    with TIMER.span('gemm', flops=2.0 * M * N * K, nbytes=2.0 * (M * K + N * K + M * N)):
+        call('llmc_gemm_rope_qkv', ptr(x2), ptr(w), ptr(q), ptr(k), ptr(v), ptr(cos.contiguous()),
+             ptr(sin.contiguous()), M, n_q, n_k, n_v, K, S, dtype_enum(x.dtype), stream_ptr(x.device))
+    return q, k, v
+
+
+def gemm_swiglu(x, w_gate_up, out=None):
+    """block_ops.silu_mul(x @ Wg^T, x @ Wu^T) for w_gate_up = interleave_gate_up(Wg, Wu), into
+    `out` (contiguous) when given."""
+    K = x.shape[-1]
+    x2, w = _gemm_operands(x, w_gate_up)
+    N, M = w.shape[0], x2.shape[0]
+    y = torch.empty((*x.shape[:-1], N // 2), dtype=x.dtype, device=x.device) if out is None else out
+    assert y.is_contiguous() and y.shape == (*x.shape[:-1], N // 2) and y.dtype == x.dtype
+    with TIMER.span('gemm', flops=2.0 * M * N * K, nbytes=2.0 * (M * K + N * K + M * N // 2)):
+        call('llmc_gemm_swiglu', ptr(x2), ptr(w), ptr(y), M, N // 2, K, dtype_enum(x.dtype),
+             stream_ptr(x.device))
+    return y
+
+
+def linear_forward_residual(x, weight, res, out):
+    """out = block_ops.add(res, x @ weight^T); out may be res."""
+    K = x.shape[-1]
+    x2, w = _gemm_operands(x, weight)
+    N, M = w.shape[0], x2.shape[0]
+    assert res.is_contiguous() and out.is_contiguous() and res.dtype == out.dtype == x.dtype
+    assert res.shape == out.shape == (*x.shape[:-1], N)
+    with TIMER.span('gemm', flops=2.0 * M * N * K, nbytes=2.0 * (M * K + N * K + 2 * M * N)):
+        call('llmc_gemm_residual', ptr(x2), ptr(w), ptr(res), ptr(out), M, N, K, dtype_enum(x.dtype),
+             stream_ptr(x.device))
+    return out
+
+
+def dense_forward_weight(layer, dtype):
+    """The dense weight W of `dtype` when `layer`'s forward on a CUDA input of `dtype` is exactly
+    linear_forward(x, W) (B200Linear's weight, FakeQuantLinear's cached tmp_weight, which this
+    materialises as the first forward would); None for any other forward: activation fake-quant, a
+    bias, a weight re-quantised every call, packed / FP8 / W8A8 deploys, hooks, a dtype mismatch."""
+    from .synth import B200Linear
+    if layer._forward_hooks or layer._forward_pre_hooks:
+        return None
+    if type(layer) is FakeQuantLinear:
+        if (layer.a_qdq is not None or layer.bias is not None or layer.dynamic_quant_weight
+                or layer.dynamic_quant_tmp_weight):
+            return None
+        if not hasattr(layer, 'tmp_weight'):
+            layer.register_buffer('tmp_weight', layer.w_qdq(layer), persistent=False)
+            layer.tmp_bias = layer.bias
+        w = layer.tmp_weight
+    elif type(layer) is B200Linear:
+        if layer.bias is not None:
+            return None
+        w = layer.weight
+    else:
+        return None
+    return w if (w.dtype == dtype and w.dim() == 2) else None
+
+
+def linear_residual(layer, x, res, out):
+    """out = res + layer(x) (block_ops.add), out may be res: in the GEMM's epilogue when the layer
+    has a dense forward weight, else the layer's forward and block_ops.add."""
+    w = dense_forward_weight(layer, x.dtype)
+    if (w is not None and x.is_cuda and w.shape[0] % 8 == 0 and res.is_contiguous()
+            and out.is_contiguous() and res.dtype == x.dtype):
+        return linear_forward_residual(x, w, res, out)
+    from . import block_ops
+    return block_ops.add(res, layer(x), out=out)
+
+
 def linear_forward_w4(x, wq, scales, zeros, group, bias=None, bits=4, qparams_t=False, g_idx=None):
     """Fake-quant forward on PACKED int4 weights (csrc/gemm_w4.cu): y = x @ dequant(wq).T + bias,
     bit-identical to linear_forward(x, rT((code - zero) * scale)) — the materialised weight of

@@ -15,7 +15,8 @@ import torch
 import torch.nn as nn
 import torch.nn.functional as F
 
-from .module_utils import _LLMC_LINEAR_TYPES_, _TRANSFORMERS_LINEAR_TYPES_, linear_forward
+from .module_utils import (_LLMC_LINEAR_TYPES_, _TRANSFORMERS_LINEAR_TYPES_, dense_forward_weight,
+                           gemm_rope_qkv, gemm_swiglu, interleave_gate_up, linear_forward)
 
 SHAPES = {
     # name: hidden, intermediate, layers, heads, kv_heads, vocab, kind, dtype
@@ -85,7 +86,45 @@ class LlamaAttention(nn.Module):
         self.v_proj = B200Linear(hidden, kv_heads * self.head_dim, bias=False)
         self.o_proj = B200Linear(heads * self.head_dim, hidden, bias=False)
 
+    def fused_qkv_weight(self, dtype):
+        """[Wq; Wk; Wv], the weight of qkv_rope's single GEMM with RoPE in its epilogue, or None
+        when the projections cannot run that way: a projection without a dense forward weight of
+        `dtype` (module_utils.dense_forward_weight), head_dim != 128, or q / k widths that are not
+        multiples of 256 (the GEMM's n-tile)."""
+        if self.head_dim != 128:
+            return None
+        ws = [dense_forward_weight(m, dtype) for m in (self.q_proj, self.k_proj, self.v_proj)]
+        if (any(w is None for w in ws) or ws[0].shape[0] % 256 or ws[1].shape[0] % 256
+                or ws[2].shape[0] % 8 or len({w.shape[1] for w in ws}) != 1):
+            return None
+        return torch.cat(ws)
+
+    def qkv_rope(self, x, position_embeddings, w_qkv=None):
+        """q, k, v of x [B, S, hidden] with RoPE applied to q and k, as the [B, heads, S, head_dim]
+        views sdpa takes.  One GEMM with RoPE in its epilogue when w_qkv = fused_qkv_weight() is
+        given or can be built here (once per call; callers that project many chunks build it once),
+        else the three projections and `attend`'s rotary path."""
+        if w_qkv is None and x.is_cuda:
+            w_qkv = self.fused_qkv_weight(x.dtype)
+        if w_qkv is not None and x.is_cuda and position_embeddings is not None:
+            B, S, _ = x.shape
+            cos, sin = position_embeddings
+            if cos.dtype == x.dtype and sin.dtype == x.dtype and cos.shape[0] >= S:
+                q, k, v = gemm_rope_qkv(x, w_qkv, self.heads * self.head_dim,
+                                        self.kv_heads * self.head_dim, cos[:S], sin[:S])
+                return self._heads(q, k, v)
+        return self._rope(self.q_proj(x), self.k_proj(x), self.v_proj(x), position_embeddings)
+
+    def _heads(self, q, k, v):
+        B, S, _ = q.shape
+        return (q.view(B, S, self.heads, self.head_dim).transpose(1, 2),
+                k.view(B, S, self.kv_heads, self.head_dim).transpose(1, 2),
+                v.view(B, S, self.kv_heads, self.head_dim).transpose(1, 2))
+
     def attend(self, q, k, v, position_embeddings):
+        return self.sdpa(*self._rope(q, k, v, position_embeddings))
+
+    def _rope(self, q, k, v, position_embeddings):
         B, S, _ = q.shape
         cos, sin = position_embeddings
         fused = (q.is_cuda and self.head_dim % 16 == 0 and q.is_contiguous() and k.is_contiguous()
@@ -94,20 +133,22 @@ class LlamaAttention(nn.Module):
             from . import block_ops
             block_ops.rope_(q, cos[:S], sin[:S], self.heads, self.head_dim)
             block_ops.rope_(k, cos[:S], sin[:S], self.kv_heads, self.head_dim)
-        q = q.view(B, S, self.heads, self.head_dim).transpose(1, 2)
-        k = k.view(B, S, self.kv_heads, self.head_dim).transpose(1, 2)
-        v = v.view(B, S, self.kv_heads, self.head_dim).transpose(1, 2)
+        q, k, v = self._heads(q, k, v)
         if not fused:
             cos, sin = cos[None, None, :S], sin[None, None, :S]
             q = q * cos + _rot_half(q) * sin
             k = k * cos + _rot_half(k) * sin
+        return q, k, v
+
+    def sdpa(self, q, k, v):
+        """Causal attention over [B, heads, S, head_dim] q, k, v; [B, S, heads * head_dim]."""
+        B, _, S, _ = q.shape
         o = F.scaled_dot_product_attention(q, k, v, is_causal=True,
                                            enable_gqa=self.kv_heads != self.heads)
         return o.transpose(1, 2).reshape(B, S, self.heads * self.head_dim)
 
     def forward(self, hidden_states, position_embeddings=None, **kw):
-        q, k, v = self.q_proj(hidden_states), self.k_proj(hidden_states), self.v_proj(hidden_states)
-        return self.o_proj(self.attend(q, k, v, position_embeddings))
+        return self.o_proj(self.sdpa(*self.qkv_rope(hidden_states, position_embeddings)))
 
 
 class LlamaMLP(nn.Module):
@@ -128,8 +169,29 @@ class LlamaMLP(nn.Module):
             return out
         return y
 
+    def fused_gate_up_weight(self, dtype):
+        """Gate and up interleaved in 128-row blocks, the weight of gate_up_act's single GEMM with
+        SiLU-mul in its epilogue, or None when the projections cannot run that way: a projection
+        without a dense forward weight of `dtype` (module_utils.dense_forward_weight), or an
+        intermediate size that is not a multiple of 128."""
+        wg = dense_forward_weight(self.gate_proj, dtype)
+        wu = dense_forward_weight(self.up_proj, dtype)
+        if wg is None or wu is None or wg.shape != wu.shape or wg.shape[0] % 128:
+            return None
+        return interleave_gate_up(wg, wu)
+
+    def gate_up_act(self, x, out=None, w_gate_up=None):
+        """act(gate_proj(x), up_proj(x)), into `out` when given.  One GEMM with SiLU-mul in its
+        epilogue when w_gate_up = fused_gate_up_weight() is given or can be built here (once per
+        call; callers that run many chunks build it once), else the two projections and `act`."""
+        if w_gate_up is None and x.is_cuda:
+            w_gate_up = self.fused_gate_up_weight(x.dtype)
+        if w_gate_up is not None and x.is_cuda and (out is None or out.is_contiguous()):
+            return gemm_swiglu(x, w_gate_up, out=out)
+        return self.act(self.gate_proj(x), self.up_proj(x), out=out)
+
     def forward(self, x):
-        return self.down_proj(self.act(self.gate_proj(x), self.up_proj(x)))
+        return self.down_proj(self.gate_up_act(x))
 
 
 class LlamaBlock(nn.Module):
