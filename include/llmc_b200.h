@@ -465,6 +465,20 @@ int llmc_gemm_w4a16_gidx(const void* x, const int32_t* wq, const void* scales, c
                          int qparam_dtype, const int32_t* g_idx, int64_t ng, int q_transposed,
                          const void* bias, void* y, int64_t M, int64_t N, int64_t K, int dtype,
                          void* stream);
+/* llmc_gemm_w4a16_awq — the same fused forward on the AutoAWQ GEMM export as stored
+ *   (AutoawqRealQuantLinear / MlcllmRealQuantLinear, module_utils.py:1004-1065):
+ *   qweight [K, N/8] int32 packed along N: nibble i of word (k, j) is column 8j + AWQ_ORDER[i],
+ *           AWQ_ORDER = {0, 2, 4, 6, 1, 3, 5, 7}
+ *   qzeros  [K/group, N/8] int32, packed the same way; scales_f16 [K/group, N] fp16 (for bf16
+ *           models too: widened in the kernel)
+ *   w[n, k] = rT(fp32(q - z) * fp32(s)) with q, z the STORED nibbles (the packer does not clamp, so a
+ *   code outside 0..15 has carried into its neighbours; the forward decodes the word as held), one
+ *   rounding; the result equals llmc_gemm_bf16 on that weight (+ bias) bit for bit.  bias [N] of
+ *   `dtype` or NULL.  K % 64 == 0, group a multiple of 64 dividing K, N % 32 == 0 (as llmc_pack_awq
+ *   requires), pointers 16-byte aligned. */
+int llmc_gemm_w4a16_awq(const void* x, const int32_t* qweight, const void* scales_f16, const int32_t* qzeros,
+                        const void* bias, void* y, int64_t M, int64_t N, int64_t K, int64_t group, int dtype,
+                        void* stream);
 int llmc_gemm_w8a16_gidx(const void* x, const int32_t* wq, const void* scales, const void* zeros,
                          int qparam_dtype, const int32_t* g_idx, int64_t ng, int q_transposed,
                          const void* bias, void* y, int64_t M, int64_t N, int64_t K, int dtype,

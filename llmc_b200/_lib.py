@@ -89,6 +89,8 @@ SIGNATURES = {
                                      c_i64, c_i64, c_int, c_vp]),
     'llmc_gemm_w8a16_gidx': (c_int, [c_vp, c_vp, c_vp, c_vp, c_int, c_vp, c_i64, c_int, c_vp, c_vp, c_i64,
                                      c_i64, c_i64, c_int, c_vp]),
+    'llmc_gemm_w4a16_awq': (c_int, [c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_i64, c_i64, c_i64, c_i64, c_int,
+                                    c_vp]),
     'llmc_gemm_fp8a16': (c_int, [c_vp, c_vp, c_vp, c_vp, c_int, c_vp, c_vp, c_i64, c_i64, c_i64, c_i64,
                                  c_int, c_int, c_vp]),
     'llmc_gemm_fp8a16_gidx': (c_int, [c_vp, c_vp, c_vp, c_vp, c_int, c_vp, c_i64, c_int, c_vp, c_vp, c_i64,

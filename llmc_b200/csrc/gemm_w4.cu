@@ -75,6 +75,23 @@
 // accumulation is llmc_gemm_bf16's on the materialised weight.  Each thread keeps a cursor into its
 // row's segment: at every step of its group it skips the columns below the step (the other
 // group's steps), then patches the step's columns in order.
+//
+// AutoAWQ layout (kLayout kPackAwq, the W4 configuration; AutoawqRealQuantLinear's export as stored):
+// qweight [K, N/8] and qzeros [K/group, N/8] int32 packed along N, nibble i of word (k, j) = column
+// 8j + AWQ_ORDER[i], AWQ_ORDER = {0, 2, 4, 6, 1, 3, 5, 7}; scales [K/group, N] fp16.  The TMA box is
+// [64 k-rows x 16 words] of qweight (4 KB, the W4 tile size), SWIZZLE_64B.  Each thread of a dequant
+// group takes one 8(n) x 8(k) block: word j = t / 8, k-rows 8 kk .. 8 kk + 7 with kk = t % 8.  It reads
+// the 8 words (row 8 kk + (r ^ kk) at read r: with the swizzle a warp's 32 reads hit 32 banks), moves
+// them back into k order with three XOR-swap stages, transposes the 8 x 8 nibble block in registers
+// (two byte-permute stages and one nibble stage), and so holds for each of its 8 columns the word of
+// 8 consecutive k codes that the contiguous W4 layout stores.  That word goes through the contiguous
+// form's decode (w4_chunk_native / w4_chunk_f32) into chunk kk of the column's row of the same
+// K-major swizzled B tile: the consumers, the epilogue and the K order are those of llmc_gemm_w4a16,
+// so the result is llmc_gemm_bf16's on rT((q - z) * s) bit for bit.  The nibbles are decoded as
+// stored (the packer's unclamped codes can carry into neighbouring nibbles; the forward reads the
+// word the checkpoint holds).  Per thread and group: one qzeros word and its 8 columns' fp16 scales
+// (16 B), prefetched one step ahead; fp16 activations take the packed half2 path (the scale is an
+// fp16 value), bf16 ones the fp32 path with the scale widened in the kernel.
 #include <stdlib.h>
 
 #include <type_traits>
@@ -97,6 +114,9 @@ constexpr int NG = 2;                         // dequant groups of four warps
 enum : int { kGridInt = 0, kGridE4M3 = 1, kGridE5M2 = 2 };
 // integer zero-points (the 2^23 path), or real-valued ones with groups along K / along N
 enum : int { kRzOff = 0, kRzK = 1, kRzN = 2 };
+// the packed layout: codes along K per weight row (LLMC_OUT_PACK_VLLM and the W3 row pairs), or
+// AutoAWQ's interleaved words along N
+enum : int { kPackK = 0, kPackAwq = 1 };
 // per weight width: INT2 / INT3 / INT4 -> 2 / 3 / 4 KB packed tile, INT8 -> 8 KB
 template <int kBits> struct Cfg {
   static constexpr int kPBytes = BN * BK * kBits / 8;
@@ -172,6 +192,70 @@ __device__ __forceinline__ void fp8x4_to_f32(uint32_t w, float* f) {
 // quant.py:1062: a zero scale dequantises with 1
 __device__ __forceinline__ float fp8_scale(float s) { return s == 0.f ? 1.f : s; }
 
+// W4: one word of 8 codes (nibble e = element e) -> the 16-byte chunk of its 8 dequantised values,
+// the arithmetic of the contiguous W4 branch of w4a16_gemm_kernel, for the AutoAWQ layout's
+// per-column qparams.  (That branch keeps its inline form: calling these there changes its
+// instruction schedule.)  Packed path: 0x6400|q = 1024+q (fp16) / 0x4300|q = 128+q (bf16), two weights per register;
+// (magic+q) - (magic+z) and * s are one HSUB2 + one HMUL2 per pair (zm2 = magic + z, s2 = s, both
+// halves; both exact in T).
+template <bool kBf16>
+__device__ __forceinline__ uint4 w4_chunk_native(uint32_t w, uint32_t zm2, uint32_t s2) {
+  constexpr uint32_t kMagic2 = kBf16 ? 0x43004300u : 0x64006400u;
+  // element pairs (0,4) (1,5) (2,6) (3,7): nibble i in the low half, nibble i+4 in the high
+  const uint32_t r04 = sub_mul2<kBf16>(and_or(w, 0x000F000Fu, kMagic2), zm2, s2);
+  const uint32_t r15 = sub_mul2<kBf16>(and_or(w >> 4, 0x000F000Fu, kMagic2), zm2, s2);
+  const uint32_t r26 = sub_mul2<kBf16>(and_or(w >> 8, 0x000F000Fu, kMagic2), zm2, s2);
+  const uint32_t r37 = sub_mul2<kBf16>(and_or(w >> 12, 0x000F000Fu, kMagic2), zm2, s2);
+  return make_uint4(__byte_perm(r04, r15, 0x5410), __byte_perm(r26, r37, 0x5410),
+                    __byte_perm(r04, r15, 0x7632), __byte_perm(r26, r37, 0x7632));
+}
+
+// fp32 path: split the word into even / odd nibbles once, then ONE byte-permute per element builds
+// the fp32 bit pattern 0x4B0000nn = 2^23 + nibble; minus zm = 2^23 + z is q - z exactly, times s
+// rounds once in fp32, then once to T.
+template <int DT>
+__device__ __forceinline__ uint4 w4_chunk_f32(uint32_t w, float zm, float s) {
+  const uint32_t ev = w & 0x0F0F0F0Fu;           // nibbles 0,2,4,6 in bytes 0..3
+  const uint32_t od = (w >> 4) & 0x0F0F0F0Fu;    // nibbles 1,3,5,7
+  float v[8];
+#pragma unroll
+  for (int j = 0; j < 4; ++j) {
+    const uint32_t be = __byte_perm(ev, 0x4B000000u, 0x7650u + j);
+    const uint32_t bo = __byte_perm(od, 0x4B000000u, 0x7650u + j);
+    v[2 * j] = fmul_rn(__uint_as_float(be) - zm, s);
+    v[2 * j + 1] = fmul_rn(__uint_as_float(bo) - zm, s);
+  }
+  return make_uint4(pack_pair<DT>(v[0], v[1]), pack_pair<DT>(v[2], v[3]),
+                    pack_pair<DT>(v[4], v[5]), pack_pair<DT>(v[6], v[7]));
+}
+
+// AutoAWQ: nibble i of a word holds column 8j + AWQ_ORDER[i], AWQ_ORDER = {0, 2, 4, 6, 1, 3, 5, 7}
+__device__ __forceinline__ constexpr int awq_column(int i) { return ((i & 3) << 1) | (i >> 2); }
+
+// Transposes the 8 x 8 nibble block w[e] nibble i -> w[i] nibble e: 4 x 4 blocks by 16-bit halves,
+// 2 x 2 blocks by bytes, then single nibbles.
+__device__ __forceinline__ void transpose_nibbles8(uint32_t* w) {
+#pragma unroll
+  for (int e = 0; e < 4; ++e) {
+    const uint32_t a = w[e], b = w[e + 4];
+    w[e] = __byte_perm(a, b, 0x5410);
+    w[e + 4] = __byte_perm(a, b, 0x7632);
+  }
+#pragma unroll
+  for (int h = 0; h < 4; ++h) {
+    const int e = (h & 1) | ((h & 2) << 1);          // 0, 1, 4, 5
+    const uint32_t a = w[e], b = w[e + 2];
+    w[e] = __byte_perm(a, b, 0x6240);
+    w[e + 2] = __byte_perm(a, b, 0x7351);
+  }
+#pragma unroll
+  for (int e = 0; e < 8; e += 2) {
+    const uint32_t a = w[e], b = w[e + 1];
+    w[e] = (a & 0x0F0F0F0Fu) | ((b << 4) & 0xF0F0F0F0u);
+    w[e + 1] = ((a >> 4) & 0x0F0F0F0Fu) | (b & 0xF0F0F0F0u);
+  }
+}
+
 // W2 / W3: a row's words of one K step in the packed tile (header: 4 words of 2-bit planes, W3 two
 // more of third bits).  W3 rows are 24 bytes apart, so the row is read as three 8-byte halves.
 template <int kBits>
@@ -206,11 +290,14 @@ __device__ __forceinline__ void next_outlier(const int32_t* cols, int& ocur, int
   oc = ocur < oend ? __ldg(cols + ocur) : INT_MAX;
 }
 
-template <bool kBf16, int kBits, bool kGidx, int kGrid, int kRz = kRzOff>
+template <bool kBf16, int kBits, bool kGidx, int kGrid, int kRz = kRzOff, int kLayout = kPackK>
 __global__ void __launch_bounds__(Cfg<kBits>::kThreads, 1)
 w4a16_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmP,
                   const ParamsOf<kRz> p) {
   using C = Cfg<kBits>;
+  constexpr bool kAwq = kLayout == kPackAwq;
+  static_assert(!kAwq || (kBits == 4 && !kGidx && kGrid == kGridInt && kRz == kRzOff),
+                "the AutoAWQ layout is a contiguous-group W4 form");
   constexpr int DT = kBf16 ? LLMC_BF16 : LLMC_F16;
   constexpr int kLStages = C::kLStages;
   constexpr int kLBytes = C::kLBytes;
@@ -244,8 +331,11 @@ w4a16_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
           uint8_t* p_dst = a_dst + kABytes;
           ring_l.expect_tx(sl, kLBytes);
           tma_load_2d(a_dst, &tmA, &ring_l.full[sl.stage], kb * BK, m_blk * BM);
-          tma_load_2d(p_dst, &tmP, &ring_l.full[sl.stage], kb * C::kWordsPerRow * C::kPackRows,
-                      n_blk * (BN / C::kPackRows));
+          if constexpr (kAwq)     // [64 k-rows x 16 words] of qweight [K, N/8]
+            tma_load_2d(p_dst, &tmP, &ring_l.full[sl.stage], n_blk * (BN / 8), kb * BK);
+          else
+            tma_load_2d(p_dst, &tmP, &ring_l.full[sl.stage], kb * C::kWordsPerRow * C::kPackRows,
+                        n_blk * (BN / C::kPackRows));
           sl.advance();
         }
       }
@@ -317,6 +407,13 @@ w4a16_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
         if (p.zeros != nullptr) z = __ldg(&reinterpret_cast<const uint32_t*>(p.zeros)[qi]);
       }
     };
+    // AutoAWQ: the qzeros word and the 8 fp16 scales (16 B) of columns n .. n + 7 in group gi
+    auto load_awq_qparams = [&](int64_t n, int gi, uint4& s8, uint32_t& zw) {
+      s8 = make_uint4(0u, 0u, 0u, 0u); zw = 0u;
+      if (n >= p.N) return;
+      s8 = __ldg(reinterpret_cast<const uint4*>(static_cast<const uint16_t*>(p.scales) + gi * p.N + n));
+      zw = __ldg(static_cast<const uint32_t*>(p.zeros) + gi * (p.N / 8) + n / 8);
+    };
     auto widen = [&](uint32_t raw) -> float {
       if (!p.qparam_native) return __uint_as_float(raw);
       return widen16<DT>(static_cast<uint16_t>(raw));
@@ -326,7 +423,8 @@ w4a16_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
     for (int u = blockIdx.x; u < p.num_units; u += gridDim.x) {
       int m_blk, n_blk;
       grouped_tile(u, p.num_units / p.n_tiles_n, p.n_tiles_n, p.gn, m_blk, n_blk);
-      const int64_t n0 = static_cast<int64_t>(n_blk) * BN + row;
+      // this thread's weight row, or with the AutoAWQ layout the first of its 8 columns
+      const int64_t n0 = static_cast<int64_t>(n_blk) * BN + (kAwq ? 8 * (row >> 3) : row);
       // real-zero forms: this row's group along N, and its cursor into the outlier CSR (oc = the
       // column of entry ocur, INT_MAX past the row's end)
       int nq = 0, ocur = 0, oend = 0, oc = INT_MAX;
@@ -341,14 +439,21 @@ w4a16_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
       // first K step of this tile that belongs to this group: (it + kb) % NG == grp
       int kb = (grp + NG - static_cast<int>(it % NG)) % NG;
       uint32_t s_cur = 0u, z_cur = 0u;
-      if (!kGidx && kb < p.kb_total) load_qparams(n0, kb / steps_per_group, s_cur, z_cur);
+      uint4 s8_cur = make_uint4(0u, 0u, 0u, 0u);     // AutoAWQ: 8 scales; z_cur is the qzeros word
+      if (!kGidx && kb < p.kb_total) {
+        if constexpr (kAwq) load_awq_qparams(n0, kb / steps_per_group, s8_cur, z_cur);
+        else load_qparams(n0, kb / steps_per_group, s_cur, z_cur);
+      }
       for (; kb < p.kb_total; kb += NG) {
         const auto sl = PipeState<kLStages>::at(it + kb);
         const auto sb = PipeState<kBStages>::at(it + kb);
         // qparams of this group's NEXT step are requested now and consumed next iteration
         uint32_t s_nxt = s_cur, z_nxt = z_cur;
-        if (!kGidx && kb + NG < p.kb_total && (kb + NG) / steps_per_group != kb / steps_per_group)
-          load_qparams(n0, (kb + NG) / steps_per_group, s_nxt, z_nxt);
+        uint4 s8_nxt = s8_cur;
+        if (!kGidx && kb + NG < p.kb_total && (kb + NG) / steps_per_group != kb / steps_per_group) {
+          if constexpr (kAwq) load_awq_qparams(n0, (kb + NG) / steps_per_group, s8_nxt, z_nxt);
+          else load_qparams(n0, (kb + NG) / steps_per_group, s_nxt, z_nxt);
+        }
         ring_l.wait_full(sl);
         ring_b.wait_empty(sb);
         const uint8_t* pk = ringL + sl.stage * kLBytes + kABytes;
@@ -356,7 +461,46 @@ w4a16_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
         const float z_c = have_zeros ? widen(z_cur) : p.zero_default;
         const float zm_cur = 8388608.0f + z_c;        // (2^23 + q) - (2^23 + z) = q - z exactly
         const float s_c = (n0 < p.N) ? widen(s_cur) : 0.f;
-        if constexpr (kGidx) {
+        if constexpr (kAwq) {
+          // this thread's 8(n) x 8(k) block (header): word j of k-rows 8 kk .. 8 kk + 7
+          const int kk = row & 7, j = row >> 3;
+          uint32_t w[8];
+#pragma unroll
+          for (int r = 0; r < 8; ++r) {
+            const int k = 8 * kk + (r ^ kk);
+            // SWIZZLE_64B: 16-byte chunk c of k-row k sits at chunk c ^ ((k >> 1) & 3)
+            w[r] = *reinterpret_cast<const uint32_t*>(pk + k * 64 + ((((j >> 2) ^ ((k >> 1) & 3)) << 4) |
+                                                                      ((j & 3) << 2)));
+          }
+          // w[r] holds k-row 8 kk + (r ^ kk): XOR-swap by the bits of kk so that w[e] holds 8 kk + e
+#pragma unroll
+          for (int b = 1; b < 8; b <<= 1) {
+            const bool f = (kk & b) != 0;
+#pragma unroll
+            for (int e = 0; e < 8; ++e) {
+              if (e & b) continue;
+              const uint32_t lo = w[e], hi = w[e | b];
+              w[e] = f ? hi : lo;
+              w[e | b] = f ? lo : hi;
+            }
+          }
+          transpose_nibbles8(w);   // w[i]: column 8j + awq_column(i), nibble e = k-row 8 kk + e
+          const uint32_t sv[4] = {s8_cur.x, s8_cur.y, s8_cur.z, s8_cur.w};
+#pragma unroll
+          for (int i = 0; i < 8; ++i) {
+            const int col = awq_column(i);
+            const uint32_t z = (z_cur >> (4 * i)) & 0xFu;                       // as stored
+            const uint32_t sh = (sv[col >> 1] >> (16 * (col & 1))) & 0xFFFFu;   // fp16 bits of the scale
+            uint4 o;
+            if constexpr (kBf16)   // an fp16 scale is no bf16 value: the fp32 path
+              o = w4_chunk_f32<DT>(w[i], __uint_as_float(0x4B000000u | z), __half2float(__ushort_as_half(
+                                                                               static_cast<unsigned short>(sh))));
+            else                   // fp16 (1024 + z) and s in both halves
+              o = w4_chunk_native<false>(w[i], (0x6400u | z) * 0x10001u, sh * 0x10001u);
+            // row 8j + col of the K-major SWIZZLE_128B B tile (row & 7 == col), chunk kk
+            *reinterpret_cast<uint4*>(bt + (8 * j + col) * 128 + ((kk ^ col) << 4)) = o;
+          }
+        } else if constexpr (kGidx) {
           // this row's packed words of the step, unswizzled (W4 / W8: word w holds elements 32/kBits * w ..;
           // W2 / W3: the words of load_lowbit_row)
           constexpr int kWords = BK * kBits / 32;
@@ -574,6 +718,7 @@ w4a16_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
         }
         s_cur = s_nxt;
         z_cur = z_nxt;
+        s8_cur = s8_nxt;
       }
       it += static_cast<uint32_t>(p.kb_total);
     }
@@ -586,7 +731,7 @@ w4a16_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
 
 using namespace llmc;
 
-template <int kBits, int kGrid, int kRz>
+template <int kBits, int kGrid, int kRz, int kLayout = w4::kPackK>
 static int launch_wNa16(const void* x, const int32_t* wq, const void* bias, void* y, int64_t M, int64_t N,
                         int64_t K, int dtype, void* stream, const char* name, w4::ParamsOf<kRz> p);
 
@@ -627,7 +772,7 @@ static int gemm_wNa16(const void* x, const int32_t* wq, const void* scales, cons
 }
 
 // Tensor maps, tile counts and the launch of a validated call whose dequant fields `p` holds.
-template <int kBits, int kGrid, int kRz>
+template <int kBits, int kGrid, int kRz, int kLayout>
 static int launch_wNa16(const void* x, const int32_t* wq, const void* bias, void* y, int64_t M, int64_t N,
                         int64_t K, int dtype, void* stream, const char* name, w4::ParamsOf<kRz> p) {
   using namespace w4;
@@ -641,9 +786,16 @@ static int launch_wNa16(const void* x, const int32_t* wq, const void* bias, void
   if (int rc = encode_tmap_2d(&tmA, x, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, M, K, K, BM, BK,
                               CU_TENSOR_MAP_SWIZZLE_128B))
     return rc;
-  if (int rc = encode_tmap_2d(&tmP, wq, CU_TENSOR_MAP_DATA_TYPE_INT32, 4, (N + pr - 1) / pr, K * kBits / 32 * pr,
-                              K * kBits / 32 * pr, BN / pr, wpr * pr, swz))
-    return rc;
+  if constexpr (kLayout == kPackAwq) {
+    // qweight [K, N/8]: 64 k-rows of 16 words (64 B) per box
+    if (int rc = encode_tmap_2d(&tmP, wq, CU_TENSOR_MAP_DATA_TYPE_INT32, 4, K, N / 8, N / 8, BK, BN / 8,
+                                CU_TENSOR_MAP_SWIZZLE_64B))
+      return rc;
+  } else {
+    if (int rc = encode_tmap_2d(&tmP, wq, CU_TENSOR_MAP_DATA_TYPE_INT32, 4, (N + pr - 1) / pr, K * kBits / 32 * pr,
+                                K * kBits / 32 * pr, BN / pr, wpr * pr, swz))
+      return rc;
+  }
   p.M = M; p.N = N; p.K = K; p.out = y; p.bias = bias;
   p.n_tiles_n = static_cast<int>((N + BN - 1) / BN);
   const int64_t mt = (M + BM - 1) / BM;
@@ -662,6 +814,10 @@ static int launch_wNa16(const void* x, const int32_t* wq, const void* bias, void
     // the real-zero forms always gather per element (the group-index dequant)
     auto kernel = dtype == LLMC_BF16 ? w4a16_gemm_kernel<true, kBits, true, kGrid, kRz>
                                      : w4a16_gemm_kernel<false, kBits, true, kGrid, kRz>;
+    return launch_persistent(kernel, p.num_units, C::kThreads, smem, st, tmA, tmP, p);
+  } else if constexpr (kLayout == kPackAwq) {
+    auto kernel = dtype == LLMC_BF16 ? w4a16_gemm_kernel<true, kBits, false, kGrid, kRzOff, kPackAwq>
+                                     : w4a16_gemm_kernel<false, kBits, false, kGrid, kRzOff, kPackAwq>;
     return launch_persistent(kernel, p.num_units, C::kThreads, smem, st, tmA, tmP, p);
   } else {
     auto kernel = p.g_idx ? (dtype == LLMC_BF16 ? w4a16_gemm_kernel<true, kBits, true, kGrid>
@@ -709,6 +865,35 @@ extern "C" int llmc_gemm_w8a16_gidx(const void* x, const int32_t* wq, const void
   LLMC_CHECK_ARG(g_idx != nullptr, "gemm_w8a16_gidx: g_idx is NULL");
   return gemm_wNa16<8>(x, wq, scales, zeros, qparam_dtype, bias, y, M, N, K, 0, g_idx, ng, dtype,
                        q_transposed, stream, "gemm_w8a16_gidx");
+}
+
+// AutoAWQ GEMM layout as stored (header): qweight [K, N/8], qzeros [K/group, N/8] int32, scales
+// [K/group, N] fp16.  N % 32 == 0: a qweight row is then a multiple of the 16 bytes a TMA row stride
+// needs (the AutoAWQ packer, llmc_pack_awq, requires it as well).
+extern "C" int llmc_gemm_w4a16_awq(const void* x, const int32_t* qweight, const void* scales_f16,
+                                   const int32_t* qzeros, const void* bias, void* y, int64_t M, int64_t N,
+                                   int64_t K, int64_t group, int dtype, void* stream) {
+  using namespace w4;
+  const char* name = "gemm_w4a16_awq";
+  LLMC_CHECK_ARG(M >= 0 && N >= 0 && K > 0, "%s: bad shape", name);
+  if (M == 0 || N == 0) return LLMC_OK;
+  LLMC_CHECK_ARG(x && qweight && scales_f16 && qzeros && y, "%s: null pointer", name);
+  LLMC_CHECK_ARG(dtype == LLMC_BF16 || dtype == LLMC_F16, "%s: dtype must be bf16 or fp16", name);
+  LLMC_CHECK_ARG(N % 32 == 0, "%s: N=%lld must be a multiple of 32", name, (long long)N);
+  LLMC_CHECK_ARG(group > 0 && K % group == 0 && group % BK == 0,
+                 "%s: group %lld must divide K=%lld and be a multiple of %d", name, (long long)group,
+                 (long long)K, BK);
+  if (K % 64 != 0 || !aligned16(x) || !aligned16(qweight) || !aligned16(scales_f16) || !aligned16(qzeros) ||
+      !aligned16(y)) {
+    set_last_error("%s: K=%lld must be a multiple of 64 and pointers 16-byte aligned", name, (long long)K);
+    return LLMC_EALIGN;
+  }
+  Params p{};
+  p.scales = scales_f16; p.zeros = qzeros;
+  p.qparam_native = dtype == LLMC_F16 ? 1 : 0;   // fp16 scales are native to fp16 activations only
+  p.q_transposed = 1;
+  p.group = group; p.ng = static_cast<int>(K / group);
+  return launch_wNa16<4, kGridInt, kRzOff, kPackAwq>(x, qweight, bias, y, M, N, K, dtype, stream, name, p);
 }
 
 // INT2 weights: wq [N, K/16] (LLMC_OUT_PACK_VLLM, zeros NULL => 2); INT3 weights: wq

@@ -196,6 +196,47 @@ def linear_forward_w4(x, wq, scales, zeros, group, bias=None, bits=4, qparams_t=
     return y.reshape(*x.shape[:-1], N)
 
 
+def linear_forward_w4a16_awq(x, qweight, scales, qzeros, group, bias=None):
+    """Real-quant forward on the AutoAWQ GEMM export as stored (csrc/gemm_w4.cu, llmc_gemm_w4a16_awq):
+    y = x @ W.T (+ bias) with W[n, k] = rT((q - z) * s), bit-identical to linear_forward on that W.
+
+    qweight [K, N/8] int32 and qzeros [K/group, N/8] int32, 8 nibbles per word along N in AutoAWQ's
+    order (nibble i = column 8j + (0, 2, 4, 6, 1, 3, 5, 7)[i]); scales [K/group, N] fp16.  q and z are
+    the nibbles as stored.  x bf16 or fp16."""
+    if x.dtype not in (torch.bfloat16, torch.float16):
+        raise ValueError(f'activations must be bf16 or fp16, not {x.dtype}')
+    if qweight.dtype != torch.int32 or qzeros.dtype != torch.int32 or scales.dtype != torch.float16:
+        raise ValueError(f'AutoAWQ tensors are int32 qweight / qzeros and fp16 scales, not '
+                         f'{qweight.dtype} / {qzeros.dtype} / {scales.dtype}')
+    K = x.shape[-1]
+    if qweight.dim() != 2 or qweight.shape[0] != K:
+        raise ValueError(f'qweight {tuple(qweight.shape)} does not match K={K}')
+    N = qweight.shape[1] * 8
+    if group <= 0 or K % group:
+        raise ValueError(f'group {group} does not divide K={K}')
+    ng = K // group
+    if tuple(scales.shape) != (ng, N) or tuple(qzeros.shape) != (ng, N // 8):
+        raise ValueError(f'scales {tuple(scales.shape)} / qzeros {tuple(qzeros.shape)} do not match '
+                         f'{ng} groups of N={N} columns')
+    if K % 64 or group % 64:
+        raise NotImplementedError(f'the AutoAWQ forward steps 64 deep along K: K={K} and group={group} '
+                                  'must be multiples of 64')
+    if N % 32:
+        raise NotImplementedError(f'the AutoAWQ forward needs N % 32 == 0 (a 16-byte qweight row), not N={N}')
+    require_cuda(x, qweight, scales, qzeros, bias)
+    x2 = x.reshape(-1, K)
+    x2 = x2 if x2.is_contiguous() else x2.contiguous()
+    b = bias.to(x.dtype).contiguous() if bias is not None else None
+    M = x2.shape[0]
+    y = torch.empty((M, N), dtype=x.dtype, device=x.device)
+    with TIMER.span('gemm_w4a16_awq', flops=2.0 * M * N * K,
+                    nbytes=2.0 * M * K + 0.5 * N * K + 2.5 * N * ng + 2.0 * M * N):
+        call('llmc_gemm_w4a16_awq', ptr(x2), ptr(qweight.contiguous()), ptr(scales.contiguous()),
+             ptr(qzeros.contiguous()), ptr(b), ptr(y), M, N, K, int(group), dtype_enum(x.dtype),
+             stream_ptr(x.device))
+    return y.reshape(*x.shape[:-1], N)
+
+
 def linear_forward_rz(x, wq, scales, zeros, bits, sym, group_axis, group=None, g_idx=None, outliers=None,
                       bias=None):
     """Fake-quant forward on packed codes with REAL-VALUED zero-points (HQQ, SpQR: round_zp False),
@@ -765,7 +806,12 @@ class VllmRealQuantLinear(nn.Module):
     — forward through linear_forward_w8a8 on the INT8 / FP8 tensor cores, the activations quantised
     as the fake-quant forward of the same config quantises them.  `act_cfg` (the config's `act`
     section, None for weight-only) is recorded by `new`; it is not a buffer, so the saved tensors are
-    those of the export.  Every other layout raises NotImplementedError saying why."""
+    those of the export.
+
+    The weight-only packed exports (W4A16 / W8A16: `weight_packed` [N, K*bits/32] of unsigned codes,
+    fp16 `weight_scale` [N, K/group]) run on llmc_gemm_w4a16 / llmc_gemm_w8a16, which read that
+    layout as stored (zeros NULL: the +2^(bits-1) storage offset).  Every other layout raises
+    NotImplementedError saying why."""
 
     def __init__(self, weight, bias, scales, input_scale, need_pack, scales_name):
         super().__init__()
@@ -779,10 +825,30 @@ class VllmRealQuantLinear(nn.Module):
         self.act_cfg = None
         self._act_quantizer = None
 
+    def packed_unsupported(self):
+        """For a `weight_packed` module: None when forward runs it on llmc_gemm_w4a16 / w8a16, else
+        the reason it does not."""
+        if self.act_cfg is not None:
+            return ('packed weights (weight_packed) with quantised activations have no real-quant forward: '
+                    'only the weight-only W4A16 / W8A16 exports run')
+        if 'weight_scale' not in self._buffers:
+            return 'packed weights (weight_packed) need a weight_scale'
+        K, words, s = self.in_features, self.weight_packed.shape[1], self.weight_scale
+        if (32 * words) % K or (32 * words) // K not in (4, 8):
+            return (f'weight_packed holds {words} words per row for in_features={K}: the packed forward '
+                    'runs 4- and 8-bit codes')
+        if s.dim() != 2 or K % s.shape[1]:
+            return f'weight_scale {tuple(s.shape)} does not split in_features={K} into groups'
+        group = K // s.shape[1]
+        if K % 64 or group % 64:
+            return (f'the packed forward steps 64 deep along K: in_features={K} and group={group} must be '
+                    'multiples of 64')
+        return None
+
     def w8a8_unsupported(self):
         """None when forward runs on llmc_gemm_w8a8_*, else the reason it does not."""
         if 'weight_packed' in self._buffers:
-            return 'packed weights (weight_packed: W4A16 / W8A16 exports) have no real-quant forward'
+            return 'packed weights (weight_packed) are W4A16 / W8A16 exports: they run on the packed GEMM'
         if 'weight_scale_inv' in self._buffers:
             return 'per_block FP8 exports (weight_scale_inv) have no real-quant forward'
         if self.act_cfg is None:
@@ -827,6 +893,14 @@ class VllmRealQuantLinear(nn.Module):
 
     @torch.no_grad()
     def forward(self, x):
+        if 'weight_packed' in self._buffers:
+            reason = self.packed_unsupported()
+            if reason is not None:
+                raise NotImplementedError(reason)
+            K = self.in_features
+            return linear_forward_w4(x, self.weight_packed, self.weight_scale, None,
+                                     K // self.weight_scale.shape[1], self.bias,
+                                     bits=32 * self.weight_packed.shape[1] // K)
         reason = self.w8a8_unsupported()
         if reason is not None:
             raise NotImplementedError(reason)
@@ -905,7 +979,10 @@ class Lightx2vRealQuantLinear(VllmRealQuantLinear):
 
 class AutoawqRealQuantLinear(nn.Module):
     """module_utils.py:936-1065 — AutoAWQ GEMM layout: qweight [C, R/8], qzeros [ng, R/8],
-    scales [ng, R] fp16."""
+    scales [ng, R] fp16.
+
+    Extension: forward runs the export as stored on llmc_gemm_w4a16_awq (linear_forward_w4a16_awq);
+    the reference's forward is not implemented."""
 
     def __init__(self, weight, bias, scales, zeros):
         super().__init__()
@@ -922,7 +999,13 @@ class AutoawqRealQuantLinear(nn.Module):
 
     @torch.no_grad()
     def forward(self, x):
-        raise NotImplementedError
+        if self.qzeros is None:
+            raise NotImplementedError('an AutoAWQ export without qzeros has no real-quant forward')
+        ng = self.scales.shape[0]
+        if self.in_features % ng:
+            raise ValueError(f'scales of {ng} groups do not split in_features={self.in_features}')
+        return linear_forward_w4a16_awq(x, self.qweight, self.scales, self.qzeros, self.in_features // ng,
+                                        self.bias)
 
     @classmethod
     @torch.no_grad()
