@@ -330,6 +330,37 @@ int llmc_gemm_residual(const void* x, const void* w, const void* res, void* y, i
                        int64_t N, int64_t K, int dtype, void* stream);
 
 /* ------------------------------------------------------------------------------------
+ * K6 grouped: a sparse-MoE layer's experts (Mixtral: w2(silu(w1 x) * w3 x) per expert) as one
+ * launch per projection, bit for bit the eager per-expert loop (gather x[tok], llmc_gemm_bf16,
+ * F.silu * up, * w[tok, slot], index_add_ into zeros).  The routing stays on the device:
+ *   xp [rows, K]      the routed rows of x gathered in expert order (rows = tokens * top_k);
+ *                     expert e owns rows [offsets[e], offsets[e+1])
+ *   offsets [E + 1]   int32 device array, offsets[0] = 0, offsets[E] = rows; read by the kernel,
+ *                     never by the host, so no call synchronises
+ *   w1, w3, w2        HOST arrays of E device pointers to each expert's weight: w1 / w3
+ *                     [inter, K], w2 [N, inter]
+ * Launches are sized by the bound ceil(rows / 128) + E m-tiles per column of n-tiles.  Each
+ * expert's weight has its own tensor map in the kernel's parameters, which caps the number of
+ * experts at LLMC_MOE_MAX_EXPERTS; more return LLMC_EINVAL.  bf16 / fp16, pointers 16-byte
+ * aligned, K a multiple of 8.
+ *   llmc_moe_gemm_swiglu  act[rows, inter] = llmc_silu_mul(xp W1_e^T, xp W3_e^T) per segment;
+ *                         inter a multiple of 128.
+ *   llmc_moe_gemm_down    y[rows, N] = rT(rT(act W2_e^T) * w_route[row]) per segment; w_route
+ *                         [rows] the routing weights in xp's row order (dtype); N a multiple of 8.
+ *   llmc_moe_combine      out[T, N] = the sum of y's rows rows[t, 0], ..., rows[t, top_k - 1]
+ *                         (int64 device array), added left to right with one rounding per add;
+ *                         N a multiple of 8. */
+#define LLMC_MOE_MAX_EXPERTS 8
+int llmc_moe_gemm_swiglu(const void* xp, const void* const* w1, const void* const* w3,
+                         const int32_t* offsets, void* act, int64_t rows, int64_t inter, int64_t K,
+                         int64_t n_experts, int dtype, void* stream);
+int llmc_moe_gemm_down(const void* act, const void* const* w2, const int32_t* offsets,
+                       const void* w_route, void* y, int64_t rows, int64_t N, int64_t inter,
+                       int64_t n_experts, int dtype, void* stream);
+int llmc_moe_combine(const void* y, const int64_t* rows, void* out, int64_t T, int64_t top_k,
+                     int64_t N, int dtype, void* stream);
+
+/* ------------------------------------------------------------------------------------
  * K6  llmc_gemm_w4a16 — fake-quant forward on PACKED weights:
  *   Y[M,N] = X[M,K] · dequant(Wq)[N,K]^T (+ bias), dequant(Wq)[n,k] =
  *   rT((code - zero) * scale) rounded to `dtype` exactly like the materialised weight of

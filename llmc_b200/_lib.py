@@ -14,6 +14,7 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, 'libllmc_b200.so')
 
 F32, F16, BF16 = 0, 1, 2
+MOE_MAX_EXPERTS = 8     # LLMC_MOE_MAX_EXPERTS
 OUT_NONE, OUT_QDQ, OUT_CODES_I8, OUT_CODES_U8, OUT_CODES_I32, OUT_PACK_VLLM = range(6)
 
 _DTYPE = {torch.float32: F32, torch.float16: F16, torch.bfloat16: BF16}
@@ -70,6 +71,11 @@ SIGNATURES = {
                                    c_i64, c_i64, c_int, c_vp]),
     'llmc_gemm_swiglu': (c_int, [c_vp, c_vp, c_vp, c_i64, c_i64, c_i64, c_int, c_vp]),
     'llmc_gemm_residual': (c_int, [c_vp, c_vp, c_vp, c_vp, c_i64, c_i64, c_i64, c_int, c_vp]),
+    'llmc_moe_gemm_swiglu': (c_int, [c_vp, c_vp, c_vp, c_vp, c_vp, c_i64, c_i64, c_i64, c_i64, c_int,
+                                     c_vp]),
+    'llmc_moe_gemm_down': (c_int, [c_vp, c_vp, c_vp, c_vp, c_vp, c_i64, c_i64, c_i64, c_i64, c_int,
+                                   c_vp]),
+    'llmc_moe_combine': (c_int, [c_vp, c_vp, c_vp, c_i64, c_i64, c_i64, c_int, c_vp]),
     'llmc_rmsnorm': (c_int, [c_vp, c_vp, c_vp, c_i64, c_i64, c_f32, c_int, c_vp]),
     'llmc_rope': (c_int, [c_vp, c_vp, c_vp, c_i64, c_i64, c_i64, c_i64, c_int, c_vp]),
     'llmc_silu_mul': (c_int, [c_vp, c_vp, c_vp, c_i64, c_int, c_vp]),

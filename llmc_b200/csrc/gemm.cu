@@ -18,6 +18,11 @@
 //      the running-mean scaling and mirrors.  Replaces GPTQ.add_batch (gptq.py:283-290), whose
 //      fp32 SGEMM on X.float() has exactly representable bf16/fp16 operands, so an fp32-
 //      accumulating tensor-core product differs only by summation order.
+//  * grouped GEMM (llmc_moe_gemm_swiglu / llmc_moe_gemm_down): one launch runs every expert of a
+//      sparse-MoE layer.  A = the routed rows gathered in expert order, expert e owning rows
+//      [offsets[e], offsets[e+1]); B = expert e's weight through its own tensor map (MoeOperands).
+//      Same main loop, tile and wgmma as the GEMM; only the unit decode, the B loads and the row
+//      bound of the store differ (see decode_moe_unit).
 #include "tc.cuh"
 
 namespace llmc {
@@ -65,10 +70,27 @@ enum Epilogue {
   kEpiRopeQkv,    // W = [Wq; Wk; Wv]: q, k, v to three outputs, rope_kernel applied to q and k
   kEpiSwiGLU,     // W = gate / up interleaved in 128-row blocks: act = silu(gate) * up
   kEpiResidual,   // Y = res + X W^T (add_kernel)
+  kEpiRouted,     // Y = rT(rT(X W^T) * w_route[row]): an expert's output times its routing weight
 };
+
+// The grouped operands: one tensor map per expert weight (AWQ rewrites the expert weights between
+// calls, so they cannot be one tensor) and the segment offsets, read from device memory so that the
+// host never learns the routing.  A kernel argument of its own, like EpiParams.
+struct MoeOperands {
+  CUtensorMap tmB[2 * LLMC_MOE_MAX_EXPERTS];   // gate/up: w1 of expert e at 2e, w3 at 2e + 1;
+                                               // down: w2 of expert e at e
+  const int32_t* offsets;                      // [E + 1] row offsets of the expert segments
+  const void* w_route;                         // kEpiRouted: [rows] routing weights (A's row order)
+  int E;
+};
+// The whole argument list of the grouped kernel fits the 4 KB kernel-parameter space: that is what
+// caps the number of experts.
+static_assert(sizeof(CUtensorMap) + sizeof(MoeOperands) + sizeof(GemmParams) <= 4096,
+              "LLMC_MOE_MAX_EXPERTS exceeds the kernel-parameter space");
 
 struct Unit {
   int m_blk, n_blk, kb0, kb1, split;
+  int e, row0, row_end;     // grouped mode: expert, first A row of the tile, end of its segment
 };
 
 template <bool kSyrk>
@@ -108,6 +130,30 @@ __device__ __forceinline__ Unit decode_unit(const GemmParams& p, int u) {
     t.kb1 = min(t.kb0 + p.kb_per_split, p.kb_total);
   }
   return t;
+}
+
+// Grouped mode: unit u is tile u - (tiles of experts < e) of expert e, in the L2-grouped order of
+// the plain GEMM within the expert; false past the last expert's tiles.  The launch bounds the
+// tile count by ceil(rows / BM) + E m-tiles per n-tile column, so it needs no host sync.
+__device__ __forceinline__ bool decode_moe_unit(const GemmParams& p, const MoeOperands& g, int u,
+                                                Unit& t) {
+  int rem = u;
+  for (int e = 0; e < g.E; ++e) {
+    const int r0 = __ldg(g.offsets + e), r1 = __ldg(g.offsets + e + 1);
+    const int m_tiles = (r1 - r0 + BM - 1) / BM;
+    if (rem < m_tiles * p.n_tiles_n) {
+      grouped_tile(rem, m_tiles, p.n_tiles_n, p.gn, t.m_blk, t.n_blk);
+      t.e = e;
+      t.row0 = r0 + t.m_blk * BM;
+      t.row_end = r1;
+      t.kb0 = 0;
+      t.kb1 = p.kb_total;
+      t.split = 0;
+      return true;
+    }
+    rem -= m_tiles * p.n_tiles_n;
+  }
+  return false;
 }
 
 // ---- fused epilogues: this thread's part of the 64-row half tile (fragment layout at
@@ -223,10 +269,39 @@ __device__ __forceinline__ void store_residual_m64n128(const float (&acc)[64], i
   }
 }
 
-template <bool kSyrk, bool kBf16, int kEpi = kEpiLinear>
-__global__ void __launch_bounds__(kThreads, 1)
-wgmma_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
-                  const GemmParams p, const EpiParams e) {
+// kEpiRouted on one half tile: the rows below row_end (the expert's segment) of Y[:, N] (N even),
+// each the GEMM's rounded output times the row's routing weight, rounded: exactly
+// `expert(x) * w[tok, slot, None]` of the eager MoE layer.
+template <int DT>
+__device__ __forceinline__ void store_routed_m64n128(const float (&acc)[64], int64_t row0,
+                                                     int64_t col0, int64_t row_end,
+                                                     const GemmParams& p, const void* w_route) {
+  using T = DType<DT>;
+  const int lane = threadIdx.x & 31;
+#pragma unroll
+  for (int i = 0; i < 2; ++i) {
+    const int64_t row = frag_row(row0, i);
+    if (row >= row_end) continue;
+    const float r = widen16<DT>(static_cast<const uint16_t*>(w_route)[row]);
+#pragma unroll
+    for (int j = 0; j < 16; ++j) {
+      const int64_t col = col0 + 8 * j + 2 * (lane & 3);
+      if (col >= p.N) continue;
+      const float v0 = fmul_rn(T::rT(acc[4 * j + 2 * i]), r);
+      const float v1 = fmul_rn(T::rT(acc[4 * j + 2 * i + 1]), r);
+      *(static_cast<uint32_t*>(p.out) + (row * p.ld_out + col) / 2) = pack_pair<DT>(v0, v1);
+    }
+  }
+}
+
+// The kernel body.  Plain mode (wgmma_gemm_kernel): B is tmB.  Grouped mode (wgmma_moe_kernel):
+// tiles come from decode_moe_unit and B from g's map of the tile's expert; for kEpiSwiGLU the
+// 256-row B stage is loaded as two 128-row boxes, w1 rows then w3 rows of the same n-block, which
+// the 128-byte swizzle lays out exactly as one box of interleave_gate_up's weight.
+template <bool kSyrk, bool kBf16, int kEpi, bool kGrouped>
+__device__ __forceinline__ void gemm_body(const CUtensorMap* tmA, const CUtensorMap* tmB,
+                                          const GemmParams& p, const EpiParams& e,
+                                          const MoeOperands* g) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = ring_base(smem_raw);
   const Ring<kStages> ring(smem + kStages * kStageBytes);
@@ -235,8 +310,12 @@ wgmma_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
   const int tid = threadIdx.x & 127;
 
   if (threadIdx.x == 0) {
-    prefetch_tmap(&tmA);
-    prefetch_tmap(&tmB);
+    prefetch_tmap(tmA);
+    if constexpr (kGrouped) {
+      for (int i = 0; i < (kEpi == kEpiSwiGLU ? 2 : 1) * g->E; ++i) prefetch_tmap(&g->tmB[i]);
+    } else {
+      prefetch_tmap(tmB);
+    }
     ring.init(1, 2);                  // empty: one arrive per consumer warpgroup
     fence_barrier_init();
   }
@@ -247,24 +326,37 @@ wgmma_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
     if (tid == 0) {
       PipeState<kStages> ps;
       for (int u = blockIdx.x; u < p.num_units; u += gridDim.x) {
-        const Unit t = decode_unit<kSyrk>(p, u);
+        Unit t;
+        if constexpr (kGrouped) {
+          if (!decode_moe_unit(p, *g, u, t)) break;
+        } else {
+          t = decode_unit<kSyrk>(p, u);
+        }
         for (int kb = t.kb0; kb < t.kb1; ++kb) {
           ring.wait_empty(ps);
           uint8_t* a_dst = smem + ps.stage * kStageBytes;
           uint8_t* b_dst = a_dst + kABytes;
           uint64_t* bar = &ring.full[ps.stage];
           ring.expect_tx(ps, kStageBytes);
-          if constexpr (!kSyrk) {
-            tma_load_2d(a_dst, &tmA, bar, kb * BK, t.m_blk * BM);
-            tma_load_2d(b_dst, &tmB, bar, kb * BK, t.n_blk * BN);
+          if constexpr (kGrouped) {
+            tma_load_2d(a_dst, tmA, bar, kb * BK, t.row0);
+            if constexpr (kEpi == kEpiSwiGLU) {
+              tma_load_2d(b_dst, &g->tmB[2 * t.e], bar, kb * BK, t.n_blk * (BN / 2));
+              tma_load_2d(b_dst + kBBytes / 2, &g->tmB[2 * t.e + 1], bar, kb * BK, t.n_blk * (BN / 2));
+            } else {
+              tma_load_2d(b_dst, &g->tmB[t.e], bar, kb * BK, t.n_blk * BN);
+            }
+          } else if constexpr (!kSyrk) {
+            tma_load_2d(a_dst, tmA, bar, kb * BK, t.m_blk * BM);
+            tma_load_2d(b_dst, tmB, bar, kb * BK, t.n_blk * BN);
           } else {
             // X[T, C]: coordinate 0 = channel, coordinate 1 = token; box = 64 ch x 64 tok
 #pragma unroll
             for (int i = 0; i < BM / 64; ++i)
-              tma_load_2d(a_dst + i * kBoxBytes, &tmA, bar, t.m_blk * BM + i * 64, kb * BK);
+              tma_load_2d(a_dst + i * kBoxBytes, tmA, bar, t.m_blk * BM + i * 64, kb * BK);
 #pragma unroll
             for (int i = 0; i < BN / 64; ++i)
-              tma_load_2d(b_dst + i * kBoxBytes, &tmA, bar, t.n_blk * BN + i * 64, kb * BK);
+              tma_load_2d(b_dst + i * kBoxBytes, tmA, bar, t.n_blk * BN + i * 64, kb * BK);
           }
           ps.advance();
         }
@@ -277,7 +369,12 @@ wgmma_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
   const int c = wg - 1;
   PipeState<kStages> ps;
   for (int u = blockIdx.x; u < p.num_units; u += gridDim.x) {
-    const Unit t = decode_unit<kSyrk>(p, u);
+    Unit t;
+    if constexpr (kGrouped) {
+      if (!decode_moe_unit(p, *g, u, t)) break;
+    } else {
+      t = decode_unit<kSyrk>(p, u);
+    }
     float acc0[64], acc1[64];                    // columns [0, 128) and [128, 256) of the tile
 #pragma unroll
     for (int i = 0; i < 64; ++i) { acc0[i] = 0.f; acc1[i] = 0.f; }
@@ -315,9 +412,19 @@ wgmma_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
     if (prev >= 0 && tid == 0) ring.release(prev);
 
     // ---- epilogue straight from the accumulator registers ----
-    const int64_t row0 = static_cast<int64_t>(t.m_blk) * BM + c * 64;
+    int64_t row0 = static_cast<int64_t>(t.m_blk) * BM + c * 64;
+    if constexpr (kGrouped) row0 = t.row0 + c * 64;
     const int64_t col0 = static_cast<int64_t>(t.n_blk) * BN;
-    if constexpr (!kSyrk) {
+    if constexpr (kGrouped) {
+      constexpr int DT = kBf16 ? LLMC_BF16 : LLMC_F16;
+      if constexpr (kEpi == kEpiSwiGLU) {
+        store_swiglu_m64n128<DT>(acc0, acc1, row0, col0 / 2, t.row_end, p.ld_out, p.out);
+      } else {
+        static_assert(kEpi == kEpiRouted, "grouped mode: kEpiSwiGLU or kEpiRouted");
+        store_routed_m64n128<DT>(acc0, row0, col0, t.row_end, p, g->w_route);
+        store_routed_m64n128<DT>(acc1, row0, col0 + 128, t.row_end, p, g->w_route);
+      }
+    } else if constexpr (!kSyrk) {
       constexpr int DT = kBf16 ? LLMC_BF16 : LLMC_F16;
       if constexpr (kEpi == kEpiLinear) {
         store_linear_m64n128<DT>(acc0, row0, col0, p.M, p.N, p.ld_out, p.bias, p.out);
@@ -338,6 +445,20 @@ wgmma_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
       store_f32_m64n128(acc1, row0, col0 + 128, p.M, p.N, p.ld_out, slab);
     }
   }
+}
+
+template <bool kSyrk, bool kBf16, int kEpi = kEpiLinear>
+__global__ void __launch_bounds__(kThreads, 1)
+wgmma_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
+                  const GemmParams p, const EpiParams e) {
+  gemm_body<kSyrk, kBf16, kEpi, false>(&tmA, &tmB, p, e, nullptr);
+}
+
+template <bool kBf16, int kEpi>
+__global__ void __launch_bounds__(kThreads, 1)
+wgmma_moe_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ MoeOperands g,
+                 const GemmParams p) {
+  gemm_body<false, kBf16, kEpi, true>(&tmA, nullptr, p, EpiParams{}, &g);
 }
 
 // ---- SYRK finalize: H = a*H + b*sum_s P_s on the upper triangle, mirrored -----------------------
@@ -487,9 +608,140 @@ static int launch_gemm(const void* x, const void* w, int64_t M, int64_t N, int64
                            p.num_units, kThreads, kSmemBytes, st, tmA, tmB, p, e);
 }
 
+// Checks and launches the grouped GEMM of kEpi over `rows` gathered rows of A [rows, K]: n_tiles
+// n-tiles of BN output columns per expert, B = w_a[e] (kEpiRouted: w2 [N, K]) or w_a[e] / w_b[e]
+// (kEpiSwiGLU: w1 / w3 [N / 2, K]).  p.out / p.ld_out are the caller's; p's other fields are
+// filled in here.
+template <int kEpi>
+static int launch_moe(const char* what, const void* a, const void* const* w_a,
+                      const void* const* w_b, const int32_t* offsets, const void* w_route,
+                      int64_t rows, int64_t N, int64_t K, int64_t E, int dtype, GemmParams p,
+                      void* stream) {
+  LLMC_CHECK_ARG(rows >= 0 && N > 0 && K > 0, "%s: bad shape", what);
+  LLMC_CHECK_ARG(E >= 1 && E <= LLMC_MOE_MAX_EXPERTS, "%s: %lld experts outside 1..%d", what,
+                 (long long)E, LLMC_MOE_MAX_EXPERTS);
+  LLMC_CHECK_ARG(rows < (1ll << 31) - BM, "%s: rows=%lld too large", what, (long long)rows);
+  if (rows == 0) return LLMC_OK;
+  LLMC_CHECK_ARG(dtype == LLMC_BF16 || dtype == LLMC_F16, "%s: dtype must be bf16 or fp16", what);
+  LLMC_CHECK_ARG(a && w_a && offsets && p.out && (kEpi != kEpiSwiGLU || w_b) &&
+                 (kEpi != kEpiRouted || w_route), "%s: null pointer", what);
+  for (int64_t e = 0; e < E; ++e)
+    LLMC_CHECK_ARG(w_a[e] && (kEpi != kEpiSwiGLU || w_b[e]), "%s: null weight of expert %lld", what,
+                   (long long)e);
+  if (K % 8 != 0 || !aligned16(a) || !aligned16(p.out)) {
+    set_last_error("%s: K=%lld must be a multiple of 8 and pointers 16-byte aligned", what,
+                   (long long)K);
+    return LLMC_EALIGN;
+  }
+  for (int64_t e = 0; e < E; ++e) {
+    if (!aligned16(w_a[e]) || (kEpi == kEpiSwiGLU && !aligned16(w_b[e]))) {
+      set_last_error("%s: weight of expert %lld not 16-byte aligned", what, (long long)e);
+      return LLMC_EALIGN;
+    }
+  }
+  CUtensorMap tmA;
+  if (int rc = encode_tmap_2d(&tmA, a, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, rows, K, K, BM, BK,
+                              CU_TENSOR_MAP_SWIZZLE_128B))
+    return rc;
+  MoeOperands g{};
+  for (int64_t e = 0; e < E; ++e) {
+    if constexpr (kEpi == kEpiSwiGLU) {
+      for (int h = 0; h < 2; ++h)
+        if (int rc = encode_tmap_2d(&g.tmB[2 * e + h], h ? w_b[e] : w_a[e],
+                                    CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, N / 2, K, K, BN / 2, BK,
+                                    CU_TENSOR_MAP_SWIZZLE_128B))
+          return rc;
+    } else {
+      if (int rc = encode_tmap_2d(&g.tmB[e], w_a[e], CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, N, K, K,
+                                  BN, BK, CU_TENSOR_MAP_SWIZZLE_128B))
+        return rc;
+    }
+  }
+  g.offsets = offsets;
+  g.w_route = w_route;
+  g.E = static_cast<int>(E);
+  p.M = rows; p.N = N; p.K = K;
+  p.n_tiles_n = static_cast<int>((N + BN - 1) / BN);
+  const int64_t units = ((rows + BM - 1) / BM + E) * p.n_tiles_n;
+  LLMC_CHECK_ARG(units < (1ll << 31), "%s: too many tiles", what);
+  p.num_units = static_cast<int>(units);
+  p.num_tiles = p.num_units;
+  p.splits = 1;
+  p.kb_total = static_cast<int>((K + BK - 1) / BK);
+  p.kb_per_split = p.kb_total;
+  p.gn = l2_group_width(static_cast<int64_t>(BN) * K * 2, p.n_tiles_n);
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  return launch_persistent(dtype == LLMC_BF16 ? wgmma_moe_kernel<true, kEpi>
+                                              : wgmma_moe_kernel<false, kEpi>,
+                           p.num_units, kThreads, kSmemBytes, st, tmA, g, p);
+}
+
+// out[t] = rT(...rT(rT(0 + y[rows[t, 0]]) + y[rows[t, 1]]) + ...): the k expert outputs of token t
+// added in the order given (ascending expert), as `zeros` + one index_add_ per expert does.
+template <int DT>
+__global__ void __launch_bounds__(256)
+moe_combine_kernel(const void* __restrict__ y, const int64_t* __restrict__ rows,
+                   void* __restrict__ out, int64_t T, int64_t k, int64_t N) {
+  const int64_t chunks = N >> 3;
+  for (int64_t i = static_cast<int64_t>(blockIdx.x) * blockDim.x + threadIdx.x; i < T * chunks;
+       i += static_cast<int64_t>(gridDim.x) * blockDim.x) {
+    const int64_t t = i / chunks, ch = i - t * chunks;
+    float acc[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
+    for (int64_t s = 0; s < k; ++s) {
+      float v[8];
+      load8<DT>(y, __ldg(rows + t * k + s) * N + ch * 8, v);
+#pragma unroll
+      for (int j = 0; j < 8; ++j) acc[j] = DType<DT>::rT(fadd_rn(acc[j], v[j]));
+    }
+    store8<DT>(out, i << 3, acc);
+  }
+}
+
 }  // namespace llmc
 
 using namespace llmc;
+
+extern "C" int llmc_moe_gemm_swiglu(const void* xp, const void* const* w1, const void* const* w3,
+                                    const int32_t* offsets, void* act, int64_t rows, int64_t inter,
+                                    int64_t K, int64_t n_experts, int dtype, void* stream) {
+  LLMC_CHECK_ARG(inter > 0 && inter % 128 == 0,
+                 "moe_gemm_swiglu: inter=%lld must be a positive multiple of 128", (long long)inter);
+  GemmParams p{};
+  p.out = act; p.ld_out = inter;
+  return launch_moe<kEpiSwiGLU>("moe_gemm_swiglu", xp, w1, w3, offsets, nullptr, rows, 2 * inter, K,
+                                n_experts, dtype, p, stream);
+}
+
+extern "C" int llmc_moe_gemm_down(const void* act, const void* const* w2, const int32_t* offsets,
+                                  const void* w_route, void* y, int64_t rows, int64_t N,
+                                  int64_t inter, int64_t n_experts, int dtype, void* stream) {
+  LLMC_CHECK_ARG(N > 0 && N % 8 == 0, "moe_gemm_down: N=%lld must be a positive multiple of 8",
+                 (long long)N);
+  GemmParams p{};
+  p.out = y; p.ld_out = N;
+  return launch_moe<kEpiRouted>("moe_gemm_down", act, w2, nullptr, offsets, w_route, rows, N, inter,
+                                n_experts, dtype, p, stream);
+}
+
+extern "C" int llmc_moe_combine(const void* y, const int64_t* rows, void* out, int64_t T,
+                                int64_t top_k, int64_t N, int dtype, void* stream) {
+  LLMC_CHECK_ARG(T >= 0 && top_k > 0 && N > 0, "moe_combine: bad shape");
+  if (T == 0) return LLMC_OK;
+  LLMC_CHECK_ARG(y && rows && out, "moe_combine: null pointer");
+  LLMC_CHECK_ARG(dtype == LLMC_BF16 || dtype == LLMC_F16, "moe_combine: dtype must be bf16 or fp16");
+  if (N % 8 != 0 || !aligned16(y) || !aligned16(out)) {
+    set_last_error("moe_combine: N=%lld must be a multiple of 8 and pointers 16-byte aligned",
+                   (long long)N);
+    return LLMC_EALIGN;
+  }
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  int64_t blocks = (T * (N >> 3) + 255) / 256;
+  if (blocks > kNumSMs * 32) blocks = kNumSMs * 32;
+#define CALL(DT) moe_combine_kernel<DT><<<(int)blocks, 256, 0, st>>>(y, rows, out, T, top_k, N); LLMC_CHECK_LAUNCH()
+  if (dtype == LLMC_BF16) { CALL(LLMC_BF16); } else { CALL(LLMC_F16); }
+#undef CALL
+  return LLMC_OK;
+}
 
 extern "C" int llmc_gemm_bf16(const void* x, const void* w, const void* bias, void* y, int64_t M,
                               int64_t N, int64_t K, int dtype, void* stream) {

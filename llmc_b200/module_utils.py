@@ -6,12 +6,13 @@ MlcllmRealQuantLinear (:1068-1084), and the type maps (:1087-1138).  Same `.new(
 factories, buffer names and `buf_*` hand-off; the forward GEMM and the packers run in
 libllmc_b200.so.
 """
+import ctypes
 from functools import partial
 
 import torch
 import torch.nn as nn
 
-from ._lib import call, dtype_enum, ptr, require_cuda, stream_ptr
+from ._lib import MOE_MAX_EXPERTS, call, dtype_enum, ptr, require_cuda, stream_ptr
 from .prof import TIMER
 
 
@@ -132,6 +133,63 @@ def linear_residual(layer, x, res, out):
         return linear_forward_residual(x, w, res, out)
     from . import block_ops
     return block_ops.add(res, layer(x), out=out)
+
+
+# ---- sparse-MoE layer as grouped expert GEMMs ------------------------------------------------------
+def moe_routing(sel, n_experts):
+    """The routing of a top-k MoE layer as device tensors whose shapes do not depend on it, so that
+    building them never synchronises with the host.  sel [T, k] holds each token's experts (distinct
+    per token).  Returns
+      perm [T*k]          the flat (token, slot) indices t*k + s sorted by expert, stably: expert e's
+                          tokens in ascending order, as torch.where(sel == e) lists them;
+      offsets [E+1]       int32 segment starts: expert e owns positions offsets[e]:offsets[e+1] of perm;
+      rows [T, k]         the positions in perm of token t's k pairs, in ascending expert order.
+    Counts come from scatter_add_, not torch.bincount, which reads its maximum back to the host."""
+    T, k = sel.shape
+    flat = sel.reshape(-1)
+    perm = torch.sort(flat, stable=True).indices
+    counts = torch.zeros(n_experts, dtype=torch.int64, device=sel.device)
+    counts.scatter_add_(0, flat, torch.ones_like(flat))
+    offsets = torch.cat([counts.new_zeros(1), counts.cumsum(0)]).to(torch.int32)
+    pos = torch.empty_like(perm).scatter_(0, perm, torch.arange(T * k, device=sel.device))
+    # a token's experts are distinct and perm is sorted by expert, so ascending position is
+    # ascending expert
+    rows = pos.view(T, k).sort(dim=1).values
+    return perm, offsets, rows
+
+
+def moe_forward(x, sel, w, experts):
+    """A Mixtral sparse-MoE layer's expert part, out[t] = sum over slots s of
+    expert_{sel[t, s]}(x[t]) * w[t, s] with expert(x) = w2(silu(w1 x) * w3 x), as three launches:
+    the grouped gate/up GEMM with SiLU-mul in its epilogue, the grouped down GEMM that scales each
+    row by its routing weight, and the combine.  x [T, H] and w [T, k] of a 16-bit dtype, sel [T, k]
+    int64, experts = one (w1, w3, w2) triple of dense weights per expert (at most
+    MOE_MAX_EXPERTS).  Bit for bit the eager loop (MixtralSparseMoe.expert_loop), with no host sync."""
+    require_cuda(x, sel, w)
+    T, K = x.shape
+    k, E = sel.shape[1], len(experts)
+    inter, N = experts[0][0].shape[0], experts[0][2].shape[0]
+    assert E <= MOE_MAX_EXPERTS and w.dtype == x.dtype
+    perm, offsets, rows = moe_routing(sel, E)
+    xp = x.index_select(0, perm // k)
+    w_route = w.reshape(-1).index_select(0, perm)
+    M = T * k
+    act = torch.empty((M, inter), dtype=x.dtype, device=x.device)
+    y = torch.empty((M, N), dtype=x.dtype, device=x.device)
+    out = torch.empty((T, N), dtype=x.dtype, device=x.device)
+    ws = [[t.contiguous() for t in e] for e in experts]
+    w1, w3, w2 = ((ctypes.c_void_p * E)(*[e[i].data_ptr() for e in ws]) for i in range(3))
+    dt, st = dtype_enum(x.dtype), stream_ptr(x.device)
+    with TIMER.span('moe_gemm_swiglu', flops=2.0 * M * 2 * inter * K,
+                    nbytes=2.0 * (M * K + E * 2 * inter * K + M * inter)):
+        call('llmc_moe_gemm_swiglu', ptr(xp), w1, w3, ptr(offsets), ptr(act), M, inter, K, E, dt, st)
+    with TIMER.span('moe_gemm_down', flops=2.0 * M * N * inter,
+                    nbytes=2.0 * (M * inter + E * N * inter + M * N + M)):
+        call('llmc_moe_gemm_down', ptr(act), w2, ptr(offsets), ptr(w_route), ptr(y), M, N, inter, E,
+             dt, st)
+    with TIMER.span('moe_combine', nbytes=2.0 * (M * N + T * N) + 8.0 * M):
+        call('llmc_moe_combine', ptr(y), ptr(rows), ptr(out), T, k, N, dt, st)
+    return out
 
 
 def linear_forward_w4(x, wq, scales, zeros, group, bias=None, bits=4, qparams_t=False, g_idx=None):

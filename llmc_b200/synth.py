@@ -15,8 +15,10 @@ import torch
 import torch.nn as nn
 import torch.nn.functional as F
 
+from ._lib import MOE_MAX_EXPERTS
 from .module_utils import (_LLMC_LINEAR_TYPES_, _TRANSFORMERS_LINEAR_TYPES_, dense_forward_weight,
-                           gemm_rope_qkv, gemm_swiglu, interleave_gate_up, linear_forward)
+                           gemm_rope_qkv, gemm_swiglu, interleave_gate_up, linear_forward,
+                           moe_forward)
 
 SHAPES = {
     # name: hidden, intermediate, layers, heads, kv_heads, vocab, kind, dtype
@@ -231,19 +233,58 @@ class MixtralSparseMoe(nn.Module):
         self.gate = nn.Linear(hidden, experts, bias=False)
         self.experts = nn.ModuleList([MixtralExpert(hidden, inter) for _ in range(experts)])
 
-    def forward(self, hidden_states):
-        B, S, H = hidden_states.shape
-        x = hidden_states.reshape(-1, H)
+    def route(self, x):
+        """The router on x [T, H]: each token's top_k experts sel [T, k] and renormalised weights
+        w [T, k] of x's dtype."""
         logits = self.gate(x)                      # module call: hooks / FakeQuantLinear see it
         w = F.softmax(logits, dim=1, dtype=torch.float)
         w, sel = torch.topk(w, self.top_k, dim=-1)
-        w = (w / w.sum(dim=-1, keepdim=True)).to(x.dtype)
+        return sel, (w / w.sum(dim=-1, keepdim=True)).to(x.dtype)
+
+    def expert_loop(self, x, sel, w):
+        """The experts one by one, each module called on exactly its routed tokens: the path for
+        experts the grouped GEMMs cannot run, and the definition moe_forward reproduces bit for bit.
+        Synchronises with the host once per expert (torch.where)."""
         out = torch.zeros_like(x)
         for e, expert in enumerate(self.experts):
             tok, slot = torch.where(sel == e)
             if tok.numel() == 0:
                 continue
             out.index_add_(0, tok, expert(x[tok]) * w[tok, slot, None])
+        return out
+
+    def grouped_weights(self, x):
+        """One (w1, w3, w2) triple of dense forward weights per expert when module_utils.moe_forward
+        computes exactly what expert_loop computes on x, else None: every expert a plain
+        MixtralExpert without hooks whose linears have a dense forward weight of x's 16-bit dtype
+        (module_utils.dense_forward_weight: no hooks, activation fake-quant, bias or packing), shapes
+        the grouped GEMMs take (inter a multiple of 128, hidden of 8), at most MOE_MAX_EXPERTS."""
+        if (not x.is_cuda or x.dtype not in (torch.bfloat16, torch.float16)
+                or len(self.experts) > MOE_MAX_EXPERTS or x.shape[1] % 8):
+            return None
+        weights = []
+        for ex in self.experts:
+            if type(ex) is not MixtralExpert or ex._forward_hooks or ex._forward_pre_hooks:
+                return None
+            ws = tuple(dense_forward_weight(m, x.dtype) for m in (ex.w1, ex.w3, ex.w2))
+            if any(t is None or t.data_ptr() % 16 for t in ws):
+                return None
+            if not weights:
+                inter, hidden = ws[0].shape
+                if inter % 128 or hidden != x.shape[1]:
+                    return None
+            if (ws[0].shape, ws[1].shape, ws[2].shape) != ((inter, hidden), (inter, hidden),
+                                                           (hidden, inter)):
+                return None
+            weights.append(ws)
+        return weights
+
+    def forward(self, hidden_states):
+        B, S, H = hidden_states.shape
+        x = hidden_states.reshape(-1, H)
+        sel, w = self.route(x)
+        weights = self.grouped_weights(x)
+        out = self.expert_loop(x, sel, w) if weights is None else moe_forward(x, sel, w, weights)
         return out.reshape(B, S, H)
 
 

@@ -1,0 +1,166 @@
+"""The Mixtral-8x7B sparse-MoE layer on the grouped expert GEMMs (module_utils.moe_forward) next to the
+per-expert loop (MixtralSparseMoe.expert_loop) it replaces.
+
+    python scripts/bench_moe.py [--reps 10] [--tokens 2048 65536] [--awq-samples 128] [--awq-rounds 3]
+                                [--out DIR]
+
+1. One MoE layer (hidden 4096, inter 14336, 8 experts, top-2, bf16) at 2048 tokens (one GPTQ
+   calibration forward at batch size 1) and 65536 tokens (the AWQ inspect batch, 128 x 512): the
+   module forward, router included, both ways.  Both paths are checked to give the same bits first;
+   after warm-up the two alternate for `reps` rounds between CUDA events, and the medians are
+   reported with the achieved TFLOP/s of the expert GEMMs (2 * tokens * top_k * 3 * hidden * inter).
+2. One AWQ run_block_loop (w4 g128, scale search + auto-clip) on a one-block Mixtral-8x7B-shaped
+   model with awq_samples x 512 calibration tokens, end to end on a host clock that ends in a device
+   synchronise: awq_rounds rounds of grouped path then loop, each run on a fresh model (the first
+   runs include the caching allocator's first allocations at this shape); every round's two runs
+   must leave the same weights.  All times are reported, the speed-up is of the medians.
+Prints, and writes to DIR/bench_moe.json, one JSON object with the card name and power limit.
+"""
+import argparse
+import copy
+import json
+import os
+import statistics
+import subprocess
+import sys
+import time
+
+import torch
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+sys.path.insert(0, ROOT)
+
+from llmc_b200 import synth  # noqa: E402
+from llmc_b200.synth import MixtralSparseMoe  # noqa: E402
+
+
+def card():
+    q = subprocess.run(['nvidia-smi', '--query-gpu=name,power.limit,clocks.max.sm', '--format=csv,noheader'],
+                       capture_output=True, text=True)
+    return q.stdout.strip() or torch.cuda.get_device_name()
+
+
+def loop_forward(moe, hs):
+    """MixtralSparseMoe.forward with the expert loop forced."""
+    B, S, H = hs.shape
+    x = hs.reshape(-1, H)
+    sel, w = moe.route(x)
+    return moe.expert_loop(x, sel, w).reshape(B, S, H)
+
+
+def timed(fn):
+    a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+    a.record()
+    fn()
+    b.record()
+    b.synchronize()
+    return a.elapsed_time(b)
+
+
+def bench_layer(res, tokens, reps):
+    s = synth.SHAPES['mixtral-8x7b']
+    H, I, E, k = s['hidden'], s['inter'], s['experts'], s['top_k']
+    g = torch.Generator(device='cuda').manual_seed(0)
+    with torch.device('meta'):
+        moe = MixtralSparseMoe(H, I, E, k)
+    moe = moe.to(torch.bfloat16).to_empty(device='cuda')
+    for p in moe.parameters():
+        p.data.normal_(0, 0.02, generator=g)
+    for T in tokens:
+        hs = torch.randn(1, T, H, device='cuda', generator=g).to(torch.bfloat16)
+        assert moe.grouped_weights(hs.view(T, H)) is not None
+        grouped, loop = moe(hs), loop_forward(moe, hs)
+        assert torch.equal(grouped.view(torch.int16), loop.view(torch.int16)), T
+        del grouped, loop
+        runs = {'grouped': lambda: moe(hs), 'loop': lambda: loop_forward(moe, hs)}
+        for fn in runs.values():
+            for _ in range(3):
+                fn()
+        torch.cuda.synchronize()
+        times = {n: [] for n in runs}
+        for _ in range(reps):
+            for n, fn in runs.items():
+                times[n].append(timed(fn))
+        med = {n: round(statistics.median(v), 3) for n, v in times.items()}
+        flops = 2.0 * T * k * 3 * H * I
+        key = f'moe_layer[T={T}]'
+        res['layer_ms'][key] = med
+        res['layer_tflops'][key] = {n: round(flops / (v * 1e-3) / 1e12, 1) for n, v in med.items()}
+        res['layer_speedup'][key] = round(med['loop'] / med['grouped'], 3)
+        print(key, med, res['layer_tflops'][key], flush=True)
+        del hs
+        torch.cuda.empty_cache()
+    del moe
+    torch.cuda.empty_cache()
+
+
+def run_awq(name, n_samples, seq_len, loop):
+    from llmc_b200.awq import Awq
+    from llmc_b200.blockwise import AttrDict
+    cfg = {'calib': {'seq_len': seq_len},
+           'quant': {'method': 'Awq',
+                     'weight': {'bit': 4, 'symmetric': True, 'granularity': 'per_group', 'group_size': 128},
+                     'special': {'trans': True, 'trans_version': 'v2', 'weight_clip': True,
+                                 'clip_sym': True}}}
+    saved = MixtralSparseMoe.forward
+    if loop:
+        MixtralSparseMoe.forward = loop_forward
+    try:
+        model = synth.SynthModel(name, n_layers=1, seed=0, device='cuda', with_head=False, init='device')
+        inp = model.first_block_input(n_samples, seq_len, bs=-1, seed=1, device='cuda')
+        c = AttrDict.wrap(copy.deepcopy(cfg))
+        algo = Awq(model, c.quant, inp, None, c)
+        torch.cuda.synchronize()
+        t0 = time.perf_counter()
+        algo.run_block_loop()
+        torch.cuda.synchronize()
+        dt = time.perf_counter() - t0
+    finally:
+        MixtralSparseMoe.forward = saved
+    state = [p.detach().clone() for p in model.get_model().layers.parameters()]
+    del algo, inp, model
+    torch.cuda.empty_cache()
+    return dt, state
+
+
+def bench_awq(res, n_samples, rounds):
+    for loop in (False, True):                     # warm-up: every kernel both paths launch
+        run_awq('tiny-mixtral', 8, 64, loop)
+    times, states = {'grouped': [], 'loop': []}, {}
+    for _ in range(rounds):                        # alternated: grouped, loop, grouped, loop, ...
+        for path in times:
+            dt, states[path] = run_awq('mixtral-8x7b', n_samples, 512, path == 'loop')
+            times[path].append(round(dt, 3))
+        assert all(torch.equal(a, b) for a, b in zip(states['grouped'], states['loop']))
+    key = f'awq_run_block_loop[mixtral-8x7b 1 block, {n_samples}x512 tokens]'
+    med = {n: statistics.median(v) for n, v in times.items()}
+    res['awq_s'][key] = times
+    res['awq_speedup'][key] = round(med['loop'] / med['grouped'], 3)
+    print(key, times, flush=True)
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument('--reps', type=int, default=10)
+    ap.add_argument('--tokens', type=int, nargs='+', default=[2048, 65536])
+    ap.add_argument('--awq-samples', type=int, default=128)
+    ap.add_argument('--awq-rounds', type=int, default=3)
+    ap.add_argument('--out', default=None)
+    args = ap.parse_args()
+    assert torch.cuda.is_available(), 'needs a CUDA device'
+    res = {'card': card(), 'reps': args.reps, 'layer_ms': {}, 'layer_tflops': {}, 'layer_speedup': {},
+           'awq_s': {}, 'awq_speedup': {}}
+    with torch.no_grad():
+        bench_layer(res, args.tokens, args.reps)
+    if args.awq_samples > 0:
+        bench_awq(res, args.awq_samples, args.awq_rounds)
+    doc = json.dumps(res)
+    print(doc)
+    if args.out:
+        os.makedirs(args.out, exist_ok=True)
+        with open(os.path.join(args.out, 'bench_moe.json'), 'w') as fh:
+            fh.write(doc + '\n')
+
+
+if __name__ == '__main__':
+    main()
