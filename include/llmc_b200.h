@@ -442,7 +442,7 @@ int llmc_fp8_block_dequant(const void* w_fp8, int64_t M, int64_t N, int block, i
  *       scales [rows, K/128] fp32.  No clamp: an all-zero group gives s = 0 and NaN codes.  The
  *       max (max.f32) skips NaN elements unless the whole group is NaN (s = NaN); +-inf gives
  *       s = inf, +-0 codes for the finite elements and NaN for the infinite ones.
- *   llmc_gemm_fp8_block (csrc/gemm_fp8.cu) out[M, N] = sum over 128-deep K blocks kb, ascending,
+ *   llmc_gemm_fp8_block (csrc/gemm_8bit.cu) out[M, N] = sum over 128-deep K blocks kb, ascending,
  *       acc = fma(dot_kb * a_s[m, kb], b_s[n / 128, kb], acc), the dot on wgmma e4m3 (Hopper's
  *       reduced-precision accumulator, fresh per K block).  a [M, K], b [N, K] e4m3 (K-major),
  *       a_s [M, K/128], b_s [ceil(N/128), K/128] fp32; K % 128 == 0, N >= 1, M == 0 is a no-op.
@@ -597,7 +597,7 @@ int llmc_gemm_w8a16_rz(const void* x, const int32_t* wq, const float* scales, co
                        const void* bias, void* y, int64_t M, int64_t N, int64_t K, int dtype, void* stream);
 
 /* ------------------------------------------------------------------------------------
- * K7  llmc_gemm_w8a8_i8 / llmc_gemm_w8a8_fp8 (csrc/gemm_w8a8.cu) — the forward of the exported
+ * K7  llmc_gemm_w8a8_i8 / llmc_gemm_w8a8_fp8 (csrc/gemm_8bit.cu) — the forward of the exported
  *   W8A8 linears (VllmRealQuantLinear and its Sgl / Lightllm / Lightx2v aliases): both operands
  *   8-bit on the tensor cores, one scale per token and one per output channel.
  *   x    [M, K] activation codes: int8 (i8) or e4m3 bytes (fp8), K-major, row stride K

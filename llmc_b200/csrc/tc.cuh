@@ -205,7 +205,7 @@ __device__ __forceinline__ void wgmma_m64n128k16_f16(float (&d)[64], uint64_t ad
 // D[64 x 128] (+)= A[64 x 32] * B[128 x 32]^T on e4m3 operands, issued by one warpgroup.  8-bit
 // operands are read K-major only (no transpose immediates); fragment layout as above.  The Hopper
 // tensor core keeps a reduced-precision fp32 accumulator for 8-bit inputs, so long K runs are
-// promoted into a full fp32 register sum by the caller (gemm_fp8.cu).
+// promoted into a full fp32 register sum by the caller (gemm_8bit.cu).
 __device__ __forceinline__ void wgmma_m64n128k32_e4m3(float (&d)[64], uint64_t adesc, uint64_t bdesc,
                                                       uint32_t accumulate) {
   asm volatile(
@@ -221,7 +221,7 @@ __device__ __forceinline__ void wgmma_m64n128k32_e4m3(float (&d)[64], uint64_t a
 }
 
 // D[64 x 128] (+)= A[64 x 32] * B[128 x 32]^T on signed 8-bit operands with int32 accumulators,
-// issued by one warpgroup (gemm_w8a8.cu).  K-major only; fragment layout as above.  The integer
+// issued by one warpgroup (gemm_8bit.cu).  K-major only; fragment layout as above.  The integer
 // sum is exact (wrapping, not saturating, past int32 — the caller bounds K).
 __device__ __forceinline__ void wgmma_m64n128k32_s8(int32_t (&d)[64], uint64_t adesc, uint64_t bdesc,
                                                     uint32_t accumulate) {
@@ -265,7 +265,7 @@ __device__ __forceinline__ void wgmma_m64n128k16(float (&d)[64], uint64_t adesc,
   else wgmma_m64n128k16_f16<kTransA, kTransB>(d, adesc, bdesc, accumulate);
 }
 
-// ---- forward GEMMs (gemm.cu, gemm_w4.cu, gemm_fp8.cu, gemm_w8a8.cu) -----------------------------
+// ---- forward GEMMs (gemm.cu, gemm_w4.cu, gemm_8bit.cu) -------------------------------------------
 // L2-grouped tile order: the weights are swept in groups of `gn` n-tiles (<= ~32 MB, L2 resident,
 // see l2_group_width), all m-tiles per group, n fastest inside the group.  Activations are re-read
 // once per group from HBM, weights once; n-fastest over a 14336-row weight would instead stream

@@ -427,7 +427,7 @@ W8A8_ENTRY = {torch.int8: 'llmc_gemm_w8a8_i8', torch.float8_e4m3fn: 'llmc_gemm_w
 
 
 def linear_forward_w8a8(x, w, s_w, act_cfg, input_scale=None, bias=None):
-    """The W8A8 real-quant forward (csrc/gemm_w8a8.cu): x is quantised to int8 / e4m3 codes by the
+    """The W8A8 real-quant forward (csrc/gemm_8bit.cu): x is quantised to int8 / e4m3 codes by the
     activation quantizer of `act_cfg` (a `quant.act` section, or the quantizer itself) exactly as the
     fake-quant forward of that config quantises it (real_quant_act), then
         y = rT(fp32(sum_k qx[m, k] * w[n, k]) * s_w[n] * s_x[m] (+ bias[n]))
@@ -474,7 +474,7 @@ USE_FP8GEMM_KERNEL = False
 
 def block_wise_fp8_forward_func(x, w, w_scale, block_size, bias):
     """module_utils.py:40-45: y = bf16(fp8_gemm(act_quant(x))) (+ bias after the rounding), as one
-    act_quant pass and one FP8 GEMM whose bf16 epilogue adds the bias (csrc/gemm_fp8.cu)."""
+    act_quant pass and one FP8 GEMM whose bf16 epilogue adds the bias (csrc/gemm_8bit.cu)."""
     from .quant_float import act_quant, gemm_fp8_block
     xq, scale = act_quant(x, block_size)
     return gemm_fp8_block(xq, scale, w, w_scale, torch.bfloat16, bias)

@@ -204,7 +204,7 @@ if 'awq' in only:
         del algo, model, inp
 
 if 'fp8' in only:
-    # The block-FP8 linear forward (act_quant + gemm_fp8_block, csrc/fp8.cu + csrc/gemm_fp8.cu) next
+    # The block-FP8 linear forward (act_quant + gemm_fp8_block, csrc/fp8.cu + csrc/gemm_8bit.cu) next
     # to the dequant-once path (llmc_fp8_block_dequant + llmc_gemm_bf16) and, where this
     # torch / cuBLAS build takes it, torch._scaled_mm with 1 x 128 / 128 x 128 block scales.
     from llmc_b200.quant_float import act_quant, gemm_fp8_block, weight_cast_to_bf16, weight_cast_to_fp8

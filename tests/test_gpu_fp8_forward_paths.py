@@ -1,5 +1,5 @@
 """GPU: the block-FP8 linear forward — llmc_fp8_act_quant (csrc/fp8.cu) feeding llmc_gemm_fp8_block
-(csrc/gemm_fp8.cu) — bit for bit against tests/fp8_gemm_oracle.py on every path, tile edge and
+(csrc/gemm_8bit.cu) — bit for bit against tests/fp8_gemm_oracle.py on every path, tile edge and
 value edge.
 
 The GEMM runs on exact-dot operands (w8a8_oracle.fp8_exact_operands): every 128-deep dot is a small
@@ -31,7 +31,7 @@ pytestmark = pytest.mark.gpu
 
 E4M3 = torch.float8_e4m3fn
 NUM_SMS = 132                           # persistent kernels run min(units, 132) CTAs
-STAGES = 6                              # gemm_fp8.cu's ring: one stage per 128-deep K block
+STAGES = 6                              # gemm_8bit.cu's ring: one stage per 128-deep K block
 ACT_PASS = NUM_SMS * 16 * 16            # act_quant: 16 groups per block, at most 132 * 16 blocks
 F32, F16, BF16 = 0, 1, 2
 LLMC_EINVAL, LLMC_EALIGN = -1, -4
@@ -112,7 +112,7 @@ def fp8_cases(M, N, K):
     kb = K // 128
     cases = {'wg1-empty' if M - (m_tiles - 1) * 128 <= 64 else 'both-wg'}
     if tiles > grid:
-        cases.add('persistent')       # a CTA carries its ring phase, barriers and d[] into more tiles
+        cases.add('persistent')       # a CTA carries its ring phase and barriers into more tiles
     if n_tiles % gn:
         cases.add('partial-group')
     elif n_tiles // gn >= 2:

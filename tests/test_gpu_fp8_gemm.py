@@ -1,5 +1,5 @@
 """GPU: the block-FP8 linear forward on the FP8 tensor cores — act_quant (csrc/fp8.cu) and
-llmc_gemm_fp8_block (csrc/gemm_fp8.cu) against the CPU oracle of tests/fp8_gemm_oracle.py.
+llmc_gemm_fp8_block (csrc/gemm_8bit.cu) against the CPU oracle of tests/fp8_gemm_oracle.py.
 
 The 128-deep dot runs in the Hopper FP8 accumulator, whose precision is below fp32, so bit-exact
 comparisons use an integer grid: small integer codes and power-of-two scales keep every partial sum

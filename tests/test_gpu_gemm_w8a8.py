@@ -1,4 +1,4 @@
-"""GPU: the W8A8 real-quant GEMM (csrc/gemm_w8a8.cu) against the CPU oracle of tests/w8a8_oracle.py.
+"""GPU: the W8A8 real-quant GEMM (csrc/gemm_8bit.cu) against the CPU oracle of tests/w8a8_oracle.py.
 
 INT8 is bit for bit on any codes: the int32 sum is exact and the epilogue is the stated fp32 one.
 FP8 is bit for bit on operands whose 128-deep partial sums are exact at any accumulator width, and
