@@ -360,6 +360,33 @@ int llmc_moe_gemm_down(const void* act, const void* const* w2, const int32_t* of
 int llmc_moe_combine(const void* y, const int64_t* rows, void* out, int64_t T, int64_t top_k,
                      int64_t N, int dtype, void* stream);
 
+/* The same two grouped projections on PACKED experts (the llmc_gemm_w4a16 / w8a16 dequant GEMM,
+ * grouped): bit for bit the per-expert loop over llmc_gemm_w{4,8}a16[_gidx] with the same operands.
+ * bits 4 or 8; each expert linear's codes wq [N_lin, K * bits / 32] int32 (LLMC_OUT_PACK_VLLM),
+ * scales / zeros in qparam_dtype (LLMC_F32 or dtype), g_idx int32 [K].  The qparam arrays are HOST
+ * arrays of E device pointers like the weights; a zeros array may be NULL (2^(bits-1), symmetric)
+ * and a g_idx array NULL (contiguous groups), but within a call either every expert linear has
+ * them or none has.  One form per call: bits, qparam dtype, layout (group < 0: qparams [ng, N_lin],
+ * else [N_lin, ng]) and ng; without g_idx ng = K / |group|.  K, |group| and (swiglu) inter
+ * multiples of 64, |group| dividing K; N a multiple of 8; no bias.  rows == 0 is a no-op; every
+ * argument error is returned before any CUDA call (misaligned xp / act / y / wq / g_idx:
+ * LLMC_EALIGN).
+ *   llmc_moe_gemm_packed_swiglu  act[rows, inter] = llmc_silu_mul(xp W1_e^T, xp W3_e^T) per segment,
+ *                                W1_e / W3_e dequantised from wq1 / wq3 [inter, K * bits / 32].
+ *   llmc_moe_gemm_packed_down    y[rows, N] = rT(rT(act W2_e^T) * w_route[row]) per segment, W2_e
+ *                                from wq2 [N, inter * bits / 32]; K = inter. */
+int llmc_moe_gemm_packed_swiglu(const void* xp, int bits, const int32_t* const* wq1,
+                                const int32_t* const* wq3, const void* const* s1, const void* const* s3,
+                                const void* const* z1, const void* const* z3, const int32_t* const* gidx1,
+                                const int32_t* const* gidx3, int qparam_dtype, int64_t group, int64_t ng,
+                                const int32_t* offsets, void* act, int64_t rows, int64_t inter, int64_t K,
+                                int64_t n_experts, int dtype, void* stream);
+int llmc_moe_gemm_packed_down(const void* act, int bits, const int32_t* const* wq2, const void* const* s2,
+                              const void* const* z2, const int32_t* const* gidx2, int qparam_dtype,
+                              int64_t group, int64_t ng, const int32_t* offsets, const void* w_route, void* y,
+                              int64_t rows, int64_t N, int64_t inter, int64_t n_experts, int dtype,
+                              void* stream);
+
 /* ------------------------------------------------------------------------------------
  * K6  llmc_gemm_w4a16 — fake-quant forward on PACKED weights:
  *   Y[M,N] = X[M,K] · dequant(Wq)[N,K]^T (+ bias), dequant(Wq)[n,k] =

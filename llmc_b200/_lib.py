@@ -76,6 +76,10 @@ SIGNATURES = {
     'llmc_moe_gemm_down': (c_int, [c_vp, c_vp, c_vp, c_vp, c_vp, c_i64, c_i64, c_i64, c_i64, c_int,
                                    c_vp]),
     'llmc_moe_combine': (c_int, [c_vp, c_vp, c_vp, c_i64, c_i64, c_i64, c_int, c_vp]),
+    'llmc_moe_gemm_packed_swiglu': (c_int, [c_vp, c_int, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_int,
+                                            c_i64, c_i64, c_vp, c_vp, c_i64, c_i64, c_i64, c_i64, c_int, c_vp]),
+    'llmc_moe_gemm_packed_down': (c_int, [c_vp, c_int, c_vp, c_vp, c_vp, c_vp, c_int, c_i64, c_i64, c_vp, c_vp,
+                                          c_vp, c_i64, c_i64, c_i64, c_i64, c_int, c_vp]),
     'llmc_rmsnorm': (c_int, [c_vp, c_vp, c_vp, c_i64, c_i64, c_f32, c_int, c_vp]),
     'llmc_rope': (c_int, [c_vp, c_vp, c_vp, c_i64, c_i64, c_i64, c_i64, c_int, c_vp]),
     'llmc_silu_mul': (c_int, [c_vp, c_vp, c_vp, c_i64, c_int, c_vp]),

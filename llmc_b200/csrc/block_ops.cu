@@ -91,10 +91,7 @@ silu_mul_kernel(const void* __restrict__ g, const void* __restrict__ u, void* __
     load8<DT>(g, i << 3, a);
     load8<DT>(u, i << 3, b);
 #pragma unroll
-    for (int k = 0; k < 8; ++k) {
-      const float sg = DType<DT>::rT(silu_f32(a[k]));                      // F.silu in fp32, rounded
-      o[k] = fmul_rn(sg, b[k]);                                            // store8 rounds
-    }
+    for (int k = 0; k < 8; ++k) o[k] = silu_mul_f32<DT, false>(a[k], b[k]);     // store8 rounds
     store8<DT>(y, i << 3, o);
   }
 }

@@ -273,6 +273,17 @@ __device__ __forceinline__ float fma_rn(float a, float b, float c) { return __fm
 // GEMM, which must agree bit for bit.
 __device__ __forceinline__ float silu_f32(float x) { return x / (1.0f + expf(-x)); }
 
+// One element of F.silu(gate) * up on DT tensors: silu in fp32 rounded to DT, the product in fp32,
+// which the caller's store rounds.  kRoundInputs: g and u are a GEMM epilogue's fp32 accumulators,
+// rounded to DT first; else they are DT values already (llmc_silu_mul).  llmc_silu_mul and every
+// SwiGLU epilogue compute it here, so they agree bit for bit.
+template <int DT, bool kRoundInputs>
+__device__ __forceinline__ float silu_mul_f32(float g, float u) {
+  using T = DType<DT>;
+  if constexpr (kRoundInputs) return fmul_rn(T::rT(silu_f32(T::rT(g))), T::rT(u));
+  else return fmul_rn(T::rT(silu_f32(g)), u);
+}
+
 inline bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15u) == 0; }
 
 }  // namespace llmc

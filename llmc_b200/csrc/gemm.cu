@@ -132,28 +132,14 @@ __device__ __forceinline__ Unit decode_unit(const GemmParams& p, int u) {
   return t;
 }
 
-// Grouped mode: unit u is tile u - (tiles of experts < e) of expert e, in the L2-grouped order of
-// the plain GEMM within the expert; false past the last expert's tiles.  The launch bounds the
-// tile count by ceil(rows / BM) + E m-tiles per n-tile column, so it needs no host sync.
+// Grouped mode: the tile of unit u (tc::moe_segment_tile); false past the last expert's tiles.
 __device__ __forceinline__ bool decode_moe_unit(const GemmParams& p, const MoeOperands& g, int u,
                                                 Unit& t) {
-  int rem = u;
-  for (int e = 0; e < g.E; ++e) {
-    const int r0 = __ldg(g.offsets + e), r1 = __ldg(g.offsets + e + 1);
-    const int m_tiles = (r1 - r0 + BM - 1) / BM;
-    if (rem < m_tiles * p.n_tiles_n) {
-      grouped_tile(rem, m_tiles, p.n_tiles_n, p.gn, t.m_blk, t.n_blk);
-      t.e = e;
-      t.row0 = r0 + t.m_blk * BM;
-      t.row_end = r1;
-      t.kb0 = 0;
-      t.kb1 = p.kb_total;
-      t.split = 0;
-      return true;
-    }
-    rem -= m_tiles * p.n_tiles_n;
-  }
-  return false;
+  t.kb0 = 0;
+  t.kb1 = p.kb_total;
+  t.split = 0;
+  return moe_segment_tile<BM>(g.offsets, g.E, u, p.n_tiles_n, p.gn, t.e, t.m_blk, t.n_blk, t.row0,
+                              t.row_end);
 }
 
 // ---- fused epilogues: this thread's part of the 64-row half tile (fragment layout at
@@ -238,7 +224,7 @@ __device__ __forceinline__ void store_swiglu_m64n128(const float (&gate)[64], co
       float v[2];
 #pragma unroll
       for (int c = 0; c < 2; ++c)
-        v[c] = fmul_rn(T::rT(silu_f32(T::rT(gate[4 * j + 2 * i + c]))), T::rT(up[4 * j + 2 * i + c]));
+        v[c] = silu_mul_f32<DT, true>(gate[4 * j + 2 * i + c], up[4 * j + 2 * i + c]);
       *reinterpret_cast<uint32_t*>(o + 8 * j) = pack_pair<DT>(v[0], v[1]);
     }
   }
@@ -265,31 +251,6 @@ __device__ __forceinline__ void store_residual_m64n128(const float (&acc)[64], i
       const float v0 = fadd_rn(pair_lo<DT>(r), T::rT(acc[4 * j + 2 * i]));
       const float v1 = fadd_rn(pair_hi<DT>(r), T::rT(acc[4 * j + 2 * i + 1]));
       *(static_cast<uint32_t*>(p.out) + off / 2) = pack_pair<DT>(v0, v1);
-    }
-  }
-}
-
-// kEpiRouted on one half tile: the rows below row_end (the expert's segment) of Y[:, N] (N even),
-// each the GEMM's rounded output times the row's routing weight, rounded: exactly
-// `expert(x) * w[tok, slot, None]` of the eager MoE layer.
-template <int DT>
-__device__ __forceinline__ void store_routed_m64n128(const float (&acc)[64], int64_t row0,
-                                                     int64_t col0, int64_t row_end,
-                                                     const GemmParams& p, const void* w_route) {
-  using T = DType<DT>;
-  const int lane = threadIdx.x & 31;
-#pragma unroll
-  for (int i = 0; i < 2; ++i) {
-    const int64_t row = frag_row(row0, i);
-    if (row >= row_end) continue;
-    const float r = widen16<DT>(static_cast<const uint16_t*>(w_route)[row]);
-#pragma unroll
-    for (int j = 0; j < 16; ++j) {
-      const int64_t col = col0 + 8 * j + 2 * (lane & 3);
-      if (col >= p.N) continue;
-      const float v0 = fmul_rn(T::rT(acc[4 * j + 2 * i]), r);
-      const float v1 = fmul_rn(T::rT(acc[4 * j + 2 * i + 1]), r);
-      *(static_cast<uint32_t*>(p.out) + (row * p.ld_out + col) / 2) = pack_pair<DT>(v0, v1);
     }
   }
 }
@@ -421,8 +382,8 @@ __device__ __forceinline__ void gemm_body(const CUtensorMap* tmA, const CUtensor
         store_swiglu_m64n128<DT>(acc0, acc1, row0, col0 / 2, t.row_end, p.ld_out, p.out);
       } else {
         static_assert(kEpi == kEpiRouted, "grouped mode: kEpiSwiGLU or kEpiRouted");
-        store_routed_m64n128<DT>(acc0, row0, col0, t.row_end, p, g->w_route);
-        store_routed_m64n128<DT>(acc1, row0, col0 + 128, t.row_end, p, g->w_route);
+        store_routed_m64n128<DT>(acc0, row0, col0, t.row_end, p.N, p.ld_out, p.out, g->w_route);
+        store_routed_m64n128<DT>(acc1, row0, col0 + 128, t.row_end, p.N, p.ld_out, p.out, g->w_route);
       }
     } else if constexpr (!kSyrk) {
       constexpr int DT = kBf16 ? LLMC_BF16 : LLMC_F16;

@@ -157,6 +157,34 @@ struct ParamsRz : Params {
 };
 template <int kRz> using ParamsOf = std::conditional_t<kRz == kRzOff, Params, ParamsRz>;
 
+// Grouped (sparse-MoE) mode: one launch runs one projection of every expert of a layer (gemm.cu's
+// grouped GEMM, on packed weights).  A = the routed rows gathered in expert order, expert e owning
+// rows [offsets[e], offsets[e+1]); tiles come from tc::moe_segment_tile.
+//   kMoeSwiGLU  the 128-row B tile is two 64-row TMA boxes: rows 0..63 are w1 rows n0 .. n0 + 63 of
+//               the tile's expert, rows 64..127 the same rows of w3.  A box is 2 KB (W4) / 4 KB (W8),
+//               a whole number of swizzle atoms, so the dequant warps' row swizzle is unchanged.  The
+//               epilogue writes act = silu(gate) * up for 64 columns (store_swiglu_m64n64).
+//   kMoeDown    128-row tiles of w2; each output row times its routing weight (store_routed_m64n128).
+enum : int { kMoeOff = 0, kMoeSwiGLU = 1, kMoeDown = 2 };
+// The grouped operands of one launch, per expert linear (gate/up: w1 of expert e at 2e, w3 at
+// 2e + 1; down: w2 of expert e at e): its packed codes' tensor map and its qparam and g_idx
+// pointers.  Every linear of a launch has one form: bits, qparam dtype and layout, zeros (all null:
+// 2^(bits-1)) and g_idx (all null: contiguous groups).  A kernel argument of its own, so that
+// Params stays within its 128 bytes.
+struct MoeW4Operands {
+  CUtensorMap tmP[2 * LLMC_MOE_MAX_EXPERTS];
+  const void* scales[2 * LLMC_MOE_MAX_EXPERTS];
+  const void* zeros[2 * LLMC_MOE_MAX_EXPERTS];
+  const int32_t* g_idx[2 * LLMC_MOE_MAX_EXPERTS];
+  const int32_t* offsets;                 // [E + 1] row offsets of the expert segments
+  const void* w_route;                    // kMoeDown: [rows] routing weights (A's row order)
+  int E;
+};
+// The whole argument list of the grouped kernel fits the 4 KB kernel-parameter space at
+// LLMC_MOE_MAX_EXPERTS experts.
+static_assert(2 * sizeof(CUtensorMap) + sizeof(Params) + sizeof(MoeW4Operands) <= 4096,
+              "LLMC_MOE_MAX_EXPERTS exceeds the kernel-parameter space");
+
 // (a & b) | c in one LOP3
 __device__ __forceinline__ uint32_t and_or(uint32_t a, uint32_t b, uint32_t c) {
   uint32_t d;
@@ -290,14 +318,48 @@ __device__ __forceinline__ void next_outlier(const int32_t* cols, int& ocur, int
   oc = ocur < oend ? __ldg(cols + ocur) : INT_MAX;
 }
 
-template <bool kBf16, int kBits, bool kGidx, int kGrid, int kRz = kRzOff, int kLayout = kPackK>
+// The grouped gate/up epilogue: acc holds gate columns 0..63 and up columns 64..127 of the tile, so
+// gate column d and up column d of a row are fragments j and j + 8 of one thread (layout at
+// tc::wgmma_m64n128k16_bf16).  act[row][col0 + d] = silu_mul_f32(rT(gate), rT(up)), rounded, for
+// the rows below row_end (the expert's segment); ld even.
+template <int DT>
+__device__ __forceinline__ void store_swiglu_m64n64(const float (&acc)[64], int64_t row0, int64_t col0,
+                                                    int64_t row_end, int64_t ld, void* out) {
+  const int tid = threadIdx.x & 127, lane = threadIdx.x & 31;
+#pragma unroll
+  for (int i = 0; i < 2; ++i) {
+    const int64_t row = row0 + (tid >> 5) * 16 + (lane >> 2) + 8 * i;
+    if (row >= row_end) continue;
+    uint16_t* o = static_cast<uint16_t*>(out) + row * ld + col0 + 2 * (lane & 3);
+#pragma unroll
+    for (int j = 0; j < 8; ++j) {
+      float v[2];
+#pragma unroll
+      for (int c = 0; c < 2; ++c)
+        v[c] = silu_mul_f32<DT, true>(acc[4 * j + 2 * i + c], acc[4 * (j + 8) + 2 * i + c]);
+      *reinterpret_cast<uint32_t*>(o + 8 * j) = pack_pair<DT>(v[0], v[1]);
+    }
+  }
+}
+
+// The last kernel argument: the grouped operands in grouped mode; in plain mode an unused null
+// pointer.  A pointer leaves the plain instantiations' code as it was without the argument (an
+// empty struct, or moving the body into a __device__ function the kernel calls, does not).
+template <int kMoe> using MoeArg = std::conditional_t<kMoe == kMoeOff, const void*, MoeW4Operands>;
+
+// Plain mode: tiles from grouped_tile, B from tmP, qparams from p.  Grouped mode (kMoe): tiles
+// from moe_segment_tile, B and the qparams of the tile's expert from `moe`; tmP is unused.
+template <bool kBf16, int kBits, bool kGidx, int kGrid, int kRz = kRzOff, int kLayout = kPackK,
+          int kMoe = kMoeOff>
 __global__ void __launch_bounds__(Cfg<kBits>::kThreads, 1)
 w4a16_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmP,
-                  const ParamsOf<kRz> p) {
+                  const ParamsOf<kRz> p, const __grid_constant__ MoeArg<kMoe> moe) {
   using C = Cfg<kBits>;
   constexpr bool kAwq = kLayout == kPackAwq;
   static_assert(!kAwq || (kBits == 4 && !kGidx && kGrid == kGridInt && kRz == kRzOff),
                 "the AutoAWQ layout is a contiguous-group W4 form");
+  static_assert(kMoe == kMoeOff || ((kBits == 4 || kBits == 8) && kGrid == kGridInt && kRz == kRzOff && !kAwq),
+                "the grouped mode runs W4 / W8 integer codes in the LLMC_OUT_PACK_VLLM layout");
   constexpr int DT = kBf16 ? LLMC_BF16 : LLMC_F16;
   constexpr int kLStages = C::kLStages;
   constexpr int kLBytes = C::kLBytes;
@@ -308,10 +370,26 @@ w4a16_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
   const Ring<kLStages> ring_l(ringB + kBStages * kBBytes);
   const Ring<kBStages> ring_b(ring_l.end());      // full: the dequantised B tile is written
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const MoeW4Operands* g = nullptr;
+  if constexpr (kMoe != kMoeOff) g = &moe;
+  // the tile of unit u (grouped mode: also its expert, first A row and segment end); false past
+  // the last expert's tiles
+  auto tile_of = [&](int u, int& e, int& m_blk, int& n_blk, int& row0, int& row_end) -> bool {
+    if constexpr (kMoe != kMoeOff) {
+      return moe_segment_tile<BM>(g->offsets, g->E, u, p.n_tiles_n, p.gn, e, m_blk, n_blk, row0, row_end);
+    } else {
+      grouped_tile(u, p.num_units / p.n_tiles_n, p.n_tiles_n, p.gn, m_blk, n_blk);
+      return true;
+    }
+  };
 
   if (threadIdx.x == 0) {
     prefetch_tmap(&tmA);
-    prefetch_tmap(&tmP);
+    if constexpr (kMoe != kMoeOff) {
+      for (int i = 0; i < (kMoe == kMoeSwiGLU ? 2 : 1) * g->E; ++i) prefetch_tmap(&g->tmP[i]);
+    } else {
+      prefetch_tmap(&tmP);
+    }
     ring_l.init(1, 2 + 4);            // empty: both consumer warpgroups + the step's dequant group
     ring_b.init(4, 2);
     fence_barrier_init();
@@ -323,19 +401,30 @@ w4a16_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
     if (lane == 0) {
       PipeState<kLStages> sl;
       for (int u = blockIdx.x; u < p.num_units; u += gridDim.x) {
-        int m_blk, n_blk;
-        grouped_tile(u, p.num_units / p.n_tiles_n, p.n_tiles_n, p.gn, m_blk, n_blk);
+        int e, m_blk, n_blk, row0, row_end;
+        if (!tile_of(u, e, m_blk, n_blk, row0, row_end)) break;
         for (int kb = 0; kb < p.kb_total; ++kb) {
           ring_l.wait_empty(sl);
           uint8_t* a_dst = ringL + sl.stage * kLBytes;
           uint8_t* p_dst = a_dst + kABytes;
           ring_l.expect_tx(sl, kLBytes);
-          tma_load_2d(a_dst, &tmA, &ring_l.full[sl.stage], kb * BK, m_blk * BM);
-          if constexpr (kAwq)     // [64 k-rows x 16 words] of qweight [K, N/8]
-            tma_load_2d(p_dst, &tmP, &ring_l.full[sl.stage], n_blk * (BN / 8), kb * BK);
-          else
-            tma_load_2d(p_dst, &tmP, &ring_l.full[sl.stage], kb * C::kWordsPerRow * C::kPackRows,
-                        n_blk * (BN / C::kPackRows));
+          if constexpr (kMoe != kMoeOff) {
+            tma_load_2d(a_dst, &tmA, &ring_l.full[sl.stage], kb * BK, row0);
+            if constexpr (kMoe == kMoeSwiGLU) {     // 64 rows of w1, then the same 64 rows of w3
+              tma_load_2d(p_dst, &g->tmP[2 * e], &ring_l.full[sl.stage], kb * C::kWordsPerRow, n_blk * (BN / 2));
+              tma_load_2d(p_dst + C::kPBytes / 2, &g->tmP[2 * e + 1], &ring_l.full[sl.stage],
+                          kb * C::kWordsPerRow, n_blk * (BN / 2));
+            } else {
+              tma_load_2d(p_dst, &g->tmP[e], &ring_l.full[sl.stage], kb * C::kWordsPerRow, n_blk * BN);
+            }
+          } else {
+            tma_load_2d(a_dst, &tmA, &ring_l.full[sl.stage], kb * BK, m_blk * BM);
+            if constexpr (kAwq)     // [64 k-rows x 16 words] of qweight [K, N/8]
+              tma_load_2d(p_dst, &tmP, &ring_l.full[sl.stage], n_blk * (BN / 8), kb * BK);
+            else
+              tma_load_2d(p_dst, &tmP, &ring_l.full[sl.stage], kb * C::kWordsPerRow * C::kPackRows,
+                          n_blk * (BN / C::kPackRows));
+          }
           sl.advance();
         }
       }
@@ -347,8 +436,8 @@ w4a16_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
     PipeState<kLStages> sl;
     PipeState<kBStages> sb;
     for (int u = blockIdx.x; u < p.num_units; u += gridDim.x) {
-      int m_blk, n_blk;
-      grouped_tile(u, p.num_units / p.n_tiles_n, p.n_tiles_n, p.gn, m_blk, n_blk);
+      int e, m_blk, n_blk, row0, row_end;
+      if (!tile_of(u, e, m_blk, n_blk, row0, row_end)) break;
       float acc[64];
 #pragma unroll
       for (int i = 0; i < 64; ++i) acc[i] = 0.f;
@@ -383,8 +472,16 @@ w4a16_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
         ring_b.release(prev_b);
       }
       // ---- epilogue from the accumulator registers ----
-      store_linear_m64n128<DT>(acc, static_cast<int64_t>(m_blk) * BM + c * 64,
-                               static_cast<int64_t>(n_blk) * BN, p.M, p.N, p.N, p.bias, p.out);
+      if constexpr (kMoe == kMoeSwiGLU) {
+        store_swiglu_m64n64<DT>(acc, static_cast<int64_t>(row0) + c * 64, static_cast<int64_t>(n_blk) * (BN / 2),
+                                row_end, p.N, p.out);
+      } else if constexpr (kMoe == kMoeDown) {
+        store_routed_m64n128<DT>(acc, static_cast<int64_t>(row0) + c * 64, static_cast<int64_t>(n_blk) * BN,
+                                 row_end, p.N, p.N, p.out, g->w_route);
+      } else {
+        store_linear_m64n128<DT>(acc, static_cast<int64_t>(m_blk) * BM + c * 64,
+                                 static_cast<int64_t>(n_blk) * BN, p.M, p.N, p.N, p.bias, p.out);
+      }
     }
   } else {
     // ===================== dequant warps (4 * NG): one weight row per thread =====================
@@ -393,6 +490,11 @@ w4a16_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
     const int grp = warp % NG;
     const int row = (warp / NG) * 32 + lane;         // 0..127 inside the group
     uint32_t it = 0;                                 // K steps issued so far (all tiles)
+    // grouped mode: the qparams and g_idx of this thread's row's expert linear in the current tile
+    // (plain mode reads p's)
+    const void* lin_s = nullptr;
+    const void* lin_z = nullptr;
+    const int32_t* lin_g = nullptr;
     // RAW bits of (scale, zero) — widening / arithmetic happens at use (widen below), so the two
     // loads stay in flight across a whole K step
     auto load_qparams = [&](int64_t n, int gi, uint32_t& s, uint32_t& z) {
@@ -400,11 +502,13 @@ w4a16_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
       if (n >= p.N) return;
       const int64_t qi = p.q_transposed ? static_cast<int64_t>(gi) * p.N + n : n * p.ng + gi;
       if (p.qparam_native) {
-        s = __ldg(&reinterpret_cast<const uint16_t*>(p.scales)[qi]);
-        if (p.zeros != nullptr) z = __ldg(&reinterpret_cast<const uint16_t*>(p.zeros)[qi]);
+        s = __ldg(&reinterpret_cast<const uint16_t*>(kMoe != kMoeOff ? lin_s : p.scales)[qi]);
+        if ((kMoe != kMoeOff ? lin_z : p.zeros) != nullptr)
+          z = __ldg(&reinterpret_cast<const uint16_t*>(kMoe != kMoeOff ? lin_z : p.zeros)[qi]);
       } else {
-        s = __ldg(&reinterpret_cast<const uint32_t*>(p.scales)[qi]);
-        if (p.zeros != nullptr) z = __ldg(&reinterpret_cast<const uint32_t*>(p.zeros)[qi]);
+        s = __ldg(&reinterpret_cast<const uint32_t*>(kMoe != kMoeOff ? lin_s : p.scales)[qi]);
+        if ((kMoe != kMoeOff ? lin_z : p.zeros) != nullptr)
+          z = __ldg(&reinterpret_cast<const uint32_t*>(kMoe != kMoeOff ? lin_z : p.zeros)[qi]);
       }
     };
     // AutoAWQ: the qzeros word and the 8 fp16 scales (16 B) of columns n .. n + 7 in group gi
@@ -418,13 +522,21 @@ w4a16_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
       if (!p.qparam_native) return __uint_as_float(raw);
       return widen16<DT>(static_cast<uint16_t>(raw));
     };
-    const bool have_zeros = p.zeros != nullptr;
+    const bool have_zeros = (kMoe != kMoeOff ? g->zeros[0] : p.zeros) != nullptr;
     const int steps_per_group = static_cast<int>(p.group / BK);
     for (int u = blockIdx.x; u < p.num_units; u += gridDim.x) {
-      int m_blk, n_blk;
-      grouped_tile(u, p.num_units / p.n_tiles_n, p.n_tiles_n, p.gn, m_blk, n_blk);
-      // this thread's weight row, or with the AutoAWQ layout the first of its 8 columns
-      const int64_t n0 = static_cast<int64_t>(n_blk) * BN + (kAwq ? 8 * (row >> 3) : row);
+      int e, m_blk, n_blk, row0, row_end;
+      if (!tile_of(u, e, m_blk, n_blk, row0, row_end)) break;
+      // this thread's weight row (of w1 / w3 for rows 0..63 / 64..127 of a gate/up tile), or with
+      // the AutoAWQ layout the first of its 8 columns
+      const int64_t n0 = kMoe == kMoeSwiGLU ? static_cast<int64_t>(n_blk) * (BN / 2) + (row & 63)
+                                            : static_cast<int64_t>(n_blk) * BN + (kAwq ? 8 * (row >> 3) : row);
+      if constexpr (kMoe != kMoeOff) {
+        const int lin = kMoe == kMoeSwiGLU ? 2 * e + (row >> 6) : e;
+        lin_s = g->scales[lin];
+        lin_z = g->zeros[lin];
+        lin_g = g->g_idx[lin];
+      }
       // real-zero forms: this row's group along N, and its cursor into the outlier CSR (oc = the
       // column of entry ocur, INT_MAX past the row's end)
       int nq = 0, ocur = 0, oend = 0, oc = INT_MAX;
@@ -521,7 +633,8 @@ w4a16_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
           } else {
             load_lowbit_row<kBits>(pk, row, words);
           }
-          const int4* gk = reinterpret_cast<const int4*>(p.g_idx + static_cast<int64_t>(kb) * BK);
+          const int4* gk = reinterpret_cast<const int4*>((kMoe != kMoeOff ? lin_g : p.g_idx) +
+                                                         static_cast<int64_t>(kb) * BK);
           const int k0 = kb * BK;
           if constexpr (kRz != kRzOff) {
             while (oc < k0) next_outlier(p.o_cols, ocur, oend, oc);   // entries of the other group's steps
@@ -814,17 +927,17 @@ static int launch_wNa16(const void* x, const int32_t* wq, const void* bias, void
     // the real-zero forms always gather per element (the group-index dequant)
     auto kernel = dtype == LLMC_BF16 ? w4a16_gemm_kernel<true, kBits, true, kGrid, kRz>
                                      : w4a16_gemm_kernel<false, kBits, true, kGrid, kRz>;
-    return launch_persistent(kernel, p.num_units, C::kThreads, smem, st, tmA, tmP, p);
+    return launch_persistent(kernel, p.num_units, C::kThreads, smem, st, tmA, tmP, p, nullptr);
   } else if constexpr (kLayout == kPackAwq) {
     auto kernel = dtype == LLMC_BF16 ? w4a16_gemm_kernel<true, kBits, false, kGrid, kRzOff, kPackAwq>
                                      : w4a16_gemm_kernel<false, kBits, false, kGrid, kRzOff, kPackAwq>;
-    return launch_persistent(kernel, p.num_units, C::kThreads, smem, st, tmA, tmP, p);
+    return launch_persistent(kernel, p.num_units, C::kThreads, smem, st, tmA, tmP, p, nullptr);
   } else {
     auto kernel = p.g_idx ? (dtype == LLMC_BF16 ? w4a16_gemm_kernel<true, kBits, true, kGrid>
                                                 : w4a16_gemm_kernel<false, kBits, true, kGrid>)
                           : (dtype == LLMC_BF16 ? w4a16_gemm_kernel<true, kBits, false, kGrid>
                                                 : w4a16_gemm_kernel<false, kBits, false, kGrid>);
-    return launch_persistent(kernel, p.num_units, C::kThreads, smem, st, tmA, tmP, p);
+    return launch_persistent(kernel, p.num_units, C::kThreads, smem, st, tmA, tmP, p, nullptr);
   }
 }
 
@@ -1100,4 +1213,158 @@ extern "C" int llmc_gemm_w8a16_rz(const void* x, const int32_t* wq, const float*
                                   int64_t K, int dtype, void* stream) {
   return gemm_wNa16_rz<8>(x, wq, scales, zeros, sym, group_axis, group, g_idx, ng, outlier_rows, outlier_cols,
                            outlier_vals, bias, y, M, N, K, dtype, stream, "gemm_w8a16_rz");
+}
+
+// ---- grouped (sparse-MoE) mode on packed experts ---------------------------------------------
+// The expert linears of one launch, in MoeW4Operands' order (gate/up: w1 of expert e at 2e, w3 at
+// 2e + 1; down: w2 of expert e at e).  A null zeros or g_idx array stands for all-null entries.
+struct MoeLinears {
+  int count;
+  const int32_t* wq[2 * LLMC_MOE_MAX_EXPERTS];
+  const void* s[2 * LLMC_MOE_MAX_EXPERTS];
+  const void* z[2 * LLMC_MOE_MAX_EXPERTS];
+  const int32_t* g[2 * LLMC_MOE_MAX_EXPERTS];
+};
+
+template <int kBits, int kMoe>
+static int launch_moe_packed(const char* name, const void* a, const MoeLinears& L, int qparam_dtype,
+                             int64_t group, int q_transposed, int64_t ng, const int32_t* offsets,
+                             const void* w_route, void* out, int64_t rows, int64_t N, int64_t K, int64_t E,
+                             int dtype, void* stream) {
+  using namespace w4;
+  using C = Cfg<kBits>;
+  constexpr CUtensorMapSwizzle swz = kBits == 4 ? CU_TENSOR_MAP_SWIZZLE_32B : CU_TENSOR_MAP_SWIZZLE_64B;
+  constexpr int box_rows = kMoe == kMoeSwiGLU ? BN / 2 : BN;
+  CUtensorMap tmA;
+  if (int rc = encode_tmap_2d(&tmA, a, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, rows, K, K, BM, BK,
+                              CU_TENSOR_MAP_SWIZZLE_128B))
+    return rc;
+  MoeW4Operands g{};
+  for (int i = 0; i < L.count; ++i) {
+    if (int rc = encode_tmap_2d(&g.tmP[i], L.wq[i], CU_TENSOR_MAP_DATA_TYPE_INT32, 4, N, K * kBits / 32,
+                                K * kBits / 32, box_rows, C::kWordsPerRow, swz))
+      return rc;
+    g.scales[i] = L.s[i]; g.zeros[i] = L.z[i]; g.g_idx[i] = L.g[i];
+  }
+  g.offsets = offsets;
+  g.w_route = w_route;
+  g.E = static_cast<int>(E);
+  const bool gidx = L.g[0] != nullptr;
+  Params p{};
+  p.M = rows; p.N = N; p.K = K; p.out = out;
+  p.qparam_native = qparam_dtype != LLMC_F32 ? 1 : 0;
+  p.q_transposed = q_transposed;
+  p.group = gidx ? K : group; p.ng = static_cast<int>(ng);
+  p.zero_default = static_cast<float>(1 << (kBits - 1));
+  p.n_tiles_n = static_cast<int>((N + box_rows - 1) / box_rows);
+  const int64_t units = ((rows + BM - 1) / BM + E) * p.n_tiles_n;
+  LLMC_CHECK_ARG(units < (1ll << 31), "%s: too many tiles", name);
+  p.num_units = static_cast<int>(units);
+  p.kb_total = static_cast<int>(K / BK);
+  p.gn = l2_group_width(static_cast<int64_t>(BN) * K * kBits / 8 + 1, p.n_tiles_n);
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  auto kernel = gidx ? (dtype == LLMC_BF16 ? w4a16_gemm_kernel<true, kBits, true, kGridInt, kRzOff, kPackK, kMoe>
+                                           : w4a16_gemm_kernel<false, kBits, true, kGridInt, kRzOff, kPackK, kMoe>)
+                     : (dtype == LLMC_BF16 ? w4a16_gemm_kernel<true, kBits, false, kGridInt, kRzOff, kPackK, kMoe>
+                                           : w4a16_gemm_kernel<false, kBits, false, kGridInt, kRzOff, kPackK, kMoe>);
+  return launch_persistent(kernel, p.num_units, C::kThreads, C::kSmemBytes, st, tmA, CUtensorMap{}, p, g);
+}
+
+// Checks and launches the grouped packed GEMM of kMoe over `rows` gathered rows of a [rows, K]
+// into out [rows, N]: N = inter (the width of w1 / w3 and of act) for gate/up, the hidden size for
+// down.  The *_b arrays are w3's (gate/up only).  Every refusal happens before any CUDA call.
+template <int kMoe>
+static int moe_packed(const char* name, const void* a, int bits, const int32_t* const* wq_a,
+                      const int32_t* const* wq_b, const void* const* s_a, const void* const* s_b,
+                      const void* const* z_a, const void* const* z_b, const int32_t* const* g_a,
+                      const int32_t* const* g_b, int qparam_dtype, int64_t group, int64_t ng,
+                      const int32_t* offsets, const void* w_route, void* out, int64_t rows, int64_t N,
+                      int64_t K, int64_t E, int dtype, void* stream) {
+  using namespace w4;
+  constexpr bool kSwiGLU = kMoe == kMoeSwiGLU;
+  LLMC_CHECK_ARG(bits == 4 || bits == 8, "%s: bits=%d must be 4 or 8", name, bits);
+  LLMC_CHECK_ARG(E >= 1 && E <= LLMC_MOE_MAX_EXPERTS, "%s: %lld experts outside 1..%d", name, (long long)E,
+                 LLMC_MOE_MAX_EXPERTS);
+  LLMC_CHECK_ARG(rows >= 0 && N > 0 && K > 0, "%s: bad shape", name);
+  LLMC_CHECK_ARG(K % BK == 0, "%s: K=%lld must be a multiple of %d", name, (long long)K, BK);
+  if (kSwiGLU)
+    LLMC_CHECK_ARG(N % 64 == 0, "%s: inter=%lld must be a multiple of 64", name, (long long)N);
+  else
+    LLMC_CHECK_ARG(N % 8 == 0, "%s: N=%lld must be a multiple of 8", name, (long long)N);
+  const int64_t ag = group < 0 ? -group : group;
+  LLMC_CHECK_ARG(ag > 0 && ag % BK == 0 && K % ag == 0,
+                 "%s: group %lld must divide K=%lld and be a multiple of %d", name, (long long)ag, (long long)K, BK);
+  LLMC_CHECK_ARG(rows < (1ll << 31) - BM, "%s: rows=%lld too large", name, (long long)rows);
+  if (rows == 0) return LLMC_OK;
+  LLMC_CHECK_ARG(dtype == LLMC_BF16 || dtype == LLMC_F16, "%s: dtype must be bf16 or fp16", name);
+  LLMC_CHECK_ARG(qparam_dtype == LLMC_F32 || qparam_dtype == dtype,
+                 "%s: qparam_dtype must be fp32 or the activation dtype", name);
+  LLMC_CHECK_ARG(a && out && offsets && wq_a && s_a && (!kSwiGLU || (wq_b && s_b)) && (kSwiGLU || w_route),
+                 "%s: null pointer", name);
+  MoeLinears L{};
+  L.count = static_cast<int>((kSwiGLU ? 2 : 1) * E);
+  for (int64_t e = 0; e < E; ++e) {
+    for (int h = 0; h < (kSwiGLU ? 2 : 1); ++h) {
+      const int i = static_cast<int>(kSwiGLU ? 2 * e + h : e);
+      L.wq[i] = h ? wq_b[e] : wq_a[e];
+      L.s[i] = h ? s_b[e] : s_a[e];
+      const void* const* z = h ? z_b : z_a;
+      const int32_t* const* gi = h ? g_b : g_a;
+      L.z[i] = z ? z[e] : nullptr;
+      L.g[i] = gi ? gi[e] : nullptr;
+      LLMC_CHECK_ARG(L.wq[i] && L.s[i], "%s: null codes or scales of expert %lld", name, (long long)e);
+    }
+  }
+  for (int i = 1; i < L.count; ++i) {
+    const long long e = kSwiGLU ? i / 2 : i;
+    LLMC_CHECK_ARG((L.z[i] == nullptr) == (L.z[0] == nullptr),
+                   "%s: zeros of expert %lld %s while expert 0's %s", name, e, L.z[i] ? "given" : "null",
+                   L.z[0] ? "are given" : "are null");
+    LLMC_CHECK_ARG((L.g[i] == nullptr) == (L.g[0] == nullptr),
+                   "%s: g_idx of expert %lld %s while expert 0's %s", name, e, L.g[i] ? "given" : "null",
+                   L.g[0] ? "is given" : "is null");
+  }
+  if (L.g[0] == nullptr)
+    LLMC_CHECK_ARG(ng == K / ag, "%s: ng=%lld, but K=%lld in groups of %lld is %lld groups", name, (long long)ng,
+                   (long long)K, (long long)ag, (long long)(K / ag));
+  else
+    LLMC_CHECK_ARG(ng >= 1 && ng <= K, "%s: ng=%lld groups for K=%lld columns", name, (long long)ng, (long long)K);
+  if (!aligned16(a) || !aligned16(out)) {
+    set_last_error("%s: activation and output pointers must be 16-byte aligned", name);
+    return LLMC_EALIGN;
+  }
+  for (int i = 0; i < L.count; ++i) {
+    if (!aligned16(L.wq[i]) || (L.g[i] && !aligned16(L.g[i]))) {
+      set_last_error("%s: codes or g_idx of expert %lld not 16-byte aligned", name,
+                     (long long)(kSwiGLU ? i / 2 : i));
+      return LLMC_EALIGN;
+    }
+  }
+  const int qt = group < 0 ? 1 : 0;
+  if (bits == 4)
+    return launch_moe_packed<4, kMoe>(name, a, L, qparam_dtype, ag, qt, ng, offsets, w_route, out, rows, N, K, E,
+                                      dtype, stream);
+  return launch_moe_packed<8, kMoe>(name, a, L, qparam_dtype, ag, qt, ng, offsets, w_route, out, rows, N, K, E,
+                                    dtype, stream);
+}
+
+extern "C" int llmc_moe_gemm_packed_swiglu(const void* xp, int bits, const int32_t* const* wq1,
+                                           const int32_t* const* wq3, const void* const* s1, const void* const* s3,
+                                           const void* const* z1, const void* const* z3, const int32_t* const* gidx1,
+                                           const int32_t* const* gidx3, int qparam_dtype, int64_t group, int64_t ng,
+                                           const int32_t* offsets, void* act, int64_t rows, int64_t inter,
+                                           int64_t K, int64_t n_experts, int dtype, void* stream) {
+  return moe_packed<w4::kMoeSwiGLU>("moe_gemm_packed_swiglu", xp, bits, wq1, wq3, s1, s3, z1, z3, gidx1, gidx3,
+                                    qparam_dtype, group, ng, offsets, nullptr, act, rows, inter, K, n_experts,
+                                    dtype, stream);
+}
+
+extern "C" int llmc_moe_gemm_packed_down(const void* act, int bits, const int32_t* const* wq2,
+                                         const void* const* s2, const void* const* z2, const int32_t* const* gidx2,
+                                         int qparam_dtype, int64_t group, int64_t ng, const int32_t* offsets,
+                                         const void* w_route, void* y, int64_t rows, int64_t N, int64_t inter,
+                                         int64_t n_experts, int dtype, void* stream) {
+  return moe_packed<w4::kMoeDown>("moe_gemm_packed_down", act, bits, wq2, nullptr, s2, nullptr, z2, nullptr,
+                                  gidx2, nullptr, qparam_dtype, group, ng, offsets, w_route, y, rows, N, inter,
+                                  n_experts, dtype, stream);
 }

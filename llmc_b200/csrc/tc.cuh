@@ -280,6 +280,32 @@ __device__ __forceinline__ void grouped_tile(int u, int m_tiles, int n_tiles, in
   n_blk = g * gn + (rem - m_blk * gsz);
 }
 
+// Grouped (sparse-MoE) mode of the forward GEMMs: A holds the routed rows in expert order, expert e
+// owning rows [offsets[e], offsets[e+1]) (int32, device memory).  Unit u is tile u - (tiles of
+// experts < e) of expert e, in grouped_tile's order within the expert, with kBM-row m-tiles; row0
+// is the tile's first A row and row_end the end of its segment.  False past the last expert's
+// tiles: the launch bounds the unit count by (ceil(rows / kBM) + E) n-tile columns, so the host
+// never reads the offsets.
+template <int kBM>
+__device__ __forceinline__ bool moe_segment_tile(const int32_t* offsets, int E, int u, int n_tiles,
+                                                 int gn, int& e_out, int& m_blk, int& n_blk,
+                                                 int& row0, int& row_end) {
+  int rem = u;
+  for (int e = 0; e < E; ++e) {
+    const int r0 = __ldg(offsets + e), r1 = __ldg(offsets + e + 1);
+    const int m_tiles = (r1 - r0 + kBM - 1) / kBM;
+    if (rem < m_tiles * n_tiles) {
+      grouped_tile(rem, m_tiles, n_tiles, gn, m_blk, n_blk);
+      e_out = e;
+      row0 = r0 + m_blk * kBM;
+      row_end = r1;
+      return true;
+    }
+    rem -= m_tiles * n_tiles;
+  }
+  return false;
+}
+
 // Stores the 16-bit pair pk (pack_pair) of columns col, col + 1 at o = &Y[row][col], the second
 // element only if `pair`: one 32-bit word when ld is even (o is then 4-byte aligned), element by
 // element otherwise.
@@ -343,6 +369,32 @@ __device__ __forceinline__ void store_linear_m64n128(const float (&acc)[64], int
       float v0 = acc[4 * j + 2 * i], v1 = acc[4 * j + 2 * i + 1];
       if (bs != nullptr) { v0 += b0; v1 += b1; }
       store_pair16(static_cast<uint16_t*>(out) + row * ld + col, pack_pair<DT>(v0, v1), pair, ld);
+    }
+  }
+}
+
+// The routed epilogue of a grouped down projection: the rows below row_end (the expert's segment)
+// of the DT matrix Y[:, N] with row stride ld (N and ld even), each the GEMM's rounded output times
+// the row's routing weight w_route[row] (DT), rounded: exactly `expert(x) * w[tok, slot, None]` of
+// the eager MoE layer.
+template <int DT>
+__device__ __forceinline__ void store_routed_m64n128(const float (&acc)[64], int64_t row0,
+                                                     int64_t col0, int64_t row_end, int64_t N,
+                                                     int64_t ld, void* out, const void* w_route) {
+  using T = DType<DT>;
+  const int lane = threadIdx.x & 31;
+#pragma unroll
+  for (int i = 0; i < 2; ++i) {
+    const int64_t row = row0 + ((threadIdx.x & 127) >> 5) * 16 + ((threadIdx.x & 31) >> 2) + 8 * i;
+    if (row >= row_end) continue;
+    const float r = widen16<DT>(static_cast<const uint16_t*>(w_route)[row]);
+#pragma unroll
+    for (int j = 0; j < 16; ++j) {
+      const int64_t col = col0 + 8 * j + 2 * (lane & 3);
+      if (col >= N) continue;
+      const float v0 = fmul_rn(T::rT(acc[4 * j + 2 * i]), r);
+      const float v1 = fmul_rn(T::rT(acc[4 * j + 2 * i + 1]), r);
+      *(static_cast<uint32_t*>(out) + (row * ld + col) / 2) = pack_pair<DT>(v0, v1);
     }
   }
 }

@@ -7,6 +7,7 @@ factories, buffer names and `buf_*` hand-off; the forward GEMM and the packers r
 libllmc_b200.so.
 """
 import ctypes
+from collections import namedtuple
 from functools import partial
 
 import torch
@@ -124,6 +125,38 @@ def dense_forward_weight(layer, dtype):
     return w if (w.dtype == dtype and w.dim() == 2) else None
 
 
+PackedOperands = namedtuple('PackedOperands', 'wq scales zeros bits group g_idx transposed')
+PackedOperands.__doc__ = """What a packed linear's forward hands to llmc_gemm_w{4,8}a16[_gidx]: codes wq [N, K*bits/32],
+scales / zeros as packed_qparams prepares them ([ng, N] when `transposed`, else [N, ng]; zeros None:
+symmetric), the group size and g_idx (int32 [K], None for contiguous groups)."""
+
+
+def packed_forward_operands(layer, dtype):
+    """The operands of `layer`'s forward on an input of `dtype` when that forward is exactly
+    linear_forward_w4 with 4- or 8-bit integer codes and nothing else, else None: a packed
+    EffcientFakeQuantLinear on the integer grid with integer zero-points (not HQQ / SpQR's real
+    ones), or a VllmRealQuantLinear weight-only W4A16 / W8A16 export it runs; no activation
+    fake-quant, bias or hooks.  The device is the caller's to check."""
+    if layer._forward_hooks or layer._forward_pre_hooks or getattr(layer, 'bias', None) is not None:
+        return None
+    if type(layer) is EffcientFakeQuantLinear:
+        if (not layer.packed or layer.q_grid != 'int' or layer.q_rz or layer.q_bits not in (4, 8)
+                or layer.a_qdq is not None):
+            return None
+        N = layer.qweight.shape[0]
+        s, z = packed_qparams(dtype, layer.qscales_t, layer.qzeros_t, N, True)
+        g = layer.g_idx.contiguous() if layer.g_idx is not None else None
+        return PackedOperands(layer.qweight.contiguous(), s, z, layer.q_bits, layer.q_group, g, True)
+    if isinstance(layer, VllmRealQuantLinear) and 'weight_packed' in layer._buffers:
+        if layer.packed_unsupported() is not None:
+            return None
+        K, wq = layer.in_features, layer.weight_packed
+        s, _ = packed_qparams(dtype, layer.weight_scale, None, wq.shape[0], False)
+        return PackedOperands(wq.contiguous(), s, None, 32 * wq.shape[1] // K, K // layer.weight_scale.shape[1],
+                              None, False)
+    return None
+
+
 def linear_residual(layer, x, res, out):
     """out = res + layer(x) (block_ops.add), out may be res: in the GEMM's epilogue when the layer
     has a dense forward weight, else the layer's forward and block_ops.add."""
@@ -163,12 +196,16 @@ def moe_forward(x, sel, w, experts):
     expert_{sel[t, s]}(x[t]) * w[t, s] with expert(x) = w2(silu(w1 x) * w3 x), as three launches:
     the grouped gate/up GEMM with SiLU-mul in its epilogue, the grouped down GEMM that scales each
     row by its routing weight, and the combine.  x [T, H] and w [T, k] of a 16-bit dtype, sel [T, k]
-    int64, experts = one (w1, w3, w2) triple of dense weights per expert (at most
-    MOE_MAX_EXPERTS).  Bit for bit the eager loop (MixtralSparseMoe.expert_loop), with no host sync."""
+    int64, experts = one (w1, w3, w2) triple per expert (at most MOE_MAX_EXPERTS): dense weights,
+    or PackedOperands of one form (packed_forward_operands; the grouped dequant GEMMs of
+    csrc/gemm_w4.cu).  Bit for bit the eager loop (MixtralSparseMoe.expert_loop), with no host
+    sync."""
     require_cuda(x, sel, w)
     T, K = x.shape
     k, E = sel.shape[1], len(experts)
-    inter, N = experts[0][0].shape[0], experts[0][2].shape[0]
+    packed = isinstance(experts[0][0], PackedOperands)
+    inter, N = ((experts[0][0].wq.shape[0], experts[0][2].wq.shape[0]) if packed
+                else (experts[0][0].shape[0], experts[0][2].shape[0]))
     assert E <= MOE_MAX_EXPERTS and w.dtype == x.dtype
     perm, offsets, rows = moe_routing(sel, E)
     xp = x.index_select(0, perm // k)
@@ -177,19 +214,66 @@ def moe_forward(x, sel, w, experts):
     act = torch.empty((M, inter), dtype=x.dtype, device=x.device)
     y = torch.empty((M, N), dtype=x.dtype, device=x.device)
     out = torch.empty((T, N), dtype=x.dtype, device=x.device)
-    ws = [[t.contiguous() for t in e] for e in experts]
-    w1, w3, w2 = ((ctypes.c_void_p * E)(*[e[i].data_ptr() for e in ws]) for i in range(3))
     dt, st = dtype_enum(x.dtype), stream_ptr(x.device)
-    with TIMER.span('moe_gemm_swiglu', flops=2.0 * M * 2 * inter * K,
-                    nbytes=2.0 * (M * K + E * 2 * inter * K + M * inter)):
-        call('llmc_moe_gemm_swiglu', ptr(xp), w1, w3, ptr(offsets), ptr(act), M, inter, K, E, dt, st)
-    with TIMER.span('moe_gemm_down', flops=2.0 * M * N * inter,
-                    nbytes=2.0 * (M * inter + E * N * inter + M * N + M)):
-        call('llmc_moe_gemm_down', ptr(act), w2, ptr(offsets), ptr(w_route), ptr(y), M, N, inter, E,
-             dt, st)
+    if packed:
+        _moe_packed_gemms(xp, experts, offsets, w_route, act, y, M, inter, N, K, E, dt, st)
+    else:
+        ws = [[t.contiguous() for t in e] for e in experts]
+        w1, w3, w2 = ((ctypes.c_void_p * E)(*[e[i].data_ptr() for e in ws]) for i in range(3))
+        with TIMER.span('moe_gemm_swiglu', flops=2.0 * M * 2 * inter * K,
+                        nbytes=2.0 * (M * K + E * 2 * inter * K + M * inter)):
+            call('llmc_moe_gemm_swiglu', ptr(xp), w1, w3, ptr(offsets), ptr(act), M, inter, K, E, dt, st)
+        with TIMER.span('moe_gemm_down', flops=2.0 * M * N * inter,
+                        nbytes=2.0 * (M * inter + E * N * inter + M * N + M)):
+            call('llmc_moe_gemm_down', ptr(act), w2, ptr(offsets), ptr(w_route), ptr(y), M, N, inter, E,
+                 dt, st)
     with TIMER.span('moe_combine', nbytes=2.0 * (M * N + T * N) + 8.0 * M):
         call('llmc_moe_combine', ptr(y), ptr(rows), ptr(out), T, k, N, dt, st)
     return out
+
+
+def packed_qparams(dtype, scales, zeros, N, qparams_t):
+    """scales / zeros as the packed GEMM takes them for activations of `dtype`: qparams already in
+    the activation dtype (RTN / AWQ / exported checkpoints) stay so and take the packed half2 / bf16x2
+    dequant path; any other (GPTQ's fp32 dynamic groups, an export's fp16 scales under bf16) become
+    fp32 and take the fp32 one — same values.  qparams_t: stored [K/group, N] (coalesced loads in the
+    kernel), else [N, K/group]; both contiguous in that shape."""
+    native = scales.dtype == dtype and (zeros is None or zeros.dtype == dtype)
+    qdt = dtype if native else torch.float32
+    shape = (-1, N) if qparams_t else (N, -1)
+    s = scales.reshape(shape).to(qdt).contiguous()
+    z = zeros.reshape(shape).to(qdt).contiguous() if zeros is not None else None
+    return s, z
+
+
+def _moe_packed_gemms(xp, experts, offsets, w_route, act, y, M, inter, N, K, E, dt, st):
+    """moe_forward's two GEMMs on PackedOperands experts: llmc_moe_gemm_packed_swiglu and
+    llmc_moe_gemm_packed_down, one form per launch."""
+    def arr(i, field):
+        ts = [getattr(e[i], field) for e in experts]
+        return None if ts[0] is None else (ctypes.c_void_p * E)(*[t.data_ptr() for t in ts])
+
+    def weight_bytes(o):                 # codes, qparams and g_idx of one expert linear
+        q = o.scales.numel() * o.scales.element_size() * (1 if o.zeros is None else 2)
+        return 4.0 * o.wq.numel() + q + (0 if o.g_idx is None else 4.0 * o.g_idx.numel())
+
+    def layout(o):
+        ng = o.scales.numel() // o.wq.shape[0]
+        return dtype_enum(o.scales.dtype), int(-o.group if o.transposed else o.group), ng
+
+    g1, g2 = experts[0][0], experts[0][2]
+    bits = g1.bits
+    qd1, grp1, ng1 = layout(g1)
+    qd2, grp2, ng2 = layout(g2)
+    with TIMER.span('moe_gemm_packed_swiglu', flops=2.0 * M * 2 * inter * K,
+                    nbytes=2.0 * (M * K + M * inter) + E * 2 * weight_bytes(g1)):
+        call('llmc_moe_gemm_packed_swiglu', ptr(xp), bits, arr(0, 'wq'), arr(1, 'wq'), arr(0, 'scales'),
+             arr(1, 'scales'), arr(0, 'zeros'), arr(1, 'zeros'), arr(0, 'g_idx'), arr(1, 'g_idx'), qd1, grp1, ng1,
+             ptr(offsets), ptr(act), M, inter, K, E, dt, st)
+    with TIMER.span('moe_gemm_packed_down', flops=2.0 * M * N * inter,
+                    nbytes=2.0 * (M * inter + M * N + M) + E * weight_bytes(g2)):
+        call('llmc_moe_gemm_packed_down', ptr(act), bits, arr(2, 'wq'), arr(2, 'scales'), arr(2, 'zeros'),
+             arr(2, 'g_idx'), qd2, grp2, ng2, ptr(offsets), ptr(w_route), ptr(y), M, N, inter, E, dt, st)
 
 
 def linear_forward_w4(x, wq, scales, zeros, group, bias=None, bits=4, qparams_t=False, g_idx=None):
@@ -223,14 +307,8 @@ def linear_forward_w4(x, wq, scales, zeros, group, bias=None, bits=4, qparams_t=
         assert wq.dtype == torch.int32 and wq.shape[1] * (32 // bits) == K, (wq.shape, K)
     x2 = x.reshape(-1, K)
     x2 = x2 if x2.is_contiguous() else x2.contiguous()
-    # qparams already in the activation dtype (RTN / AWQ / exported checkpoints) take the packed
-    # half2 / bf16x2 dequant path; fp32 qparams (GPTQ dynamic groups) the fp32 one — same values
-    native = scales.dtype == x.dtype and (zeros is None or zeros.dtype == x.dtype)
-    qdt = x.dtype if native else torch.float32
-    # qparams_t: scales / zeros already stored [K/group, N] (coalesced loads in the kernel)
-    shape = (-1, N) if qparams_t else (N, -1)
-    s = scales.reshape(shape).to(qdt).contiguous()
-    z = zeros.reshape(shape).to(qdt).contiguous() if zeros is not None else None
+    s, z = packed_qparams(x.dtype, scales, zeros, N, qparams_t)
+    qdt = s.dtype
     b = bias.to(x.dtype).contiguous() if bias is not None else None
     y = torch.empty((x2.shape[0], N), dtype=x.dtype, device=x.device)
     M = x2.shape[0]

@@ -18,7 +18,7 @@ import torch.nn.functional as F
 from ._lib import MOE_MAX_EXPERTS
 from .module_utils import (_LLMC_LINEAR_TYPES_, _TRANSFORMERS_LINEAR_TYPES_, dense_forward_weight,
                            gemm_rope_qkv, gemm_swiglu, interleave_gate_up, linear_forward,
-                           moe_forward)
+                           moe_forward, packed_forward_operands)
 
 SHAPES = {
     # name: hidden, intermediate, layers, heads, kv_heads, vocab, kind, dtype
@@ -279,12 +279,53 @@ class MixtralSparseMoe(nn.Module):
             weights.append(ws)
         return weights
 
+    def grouped_packed_operands(self, x):
+        """One (w1, w3, w2) triple of module_utils.PackedOperands per expert when moe_forward on them
+        computes exactly what expert_loop computes on x, else None: the checks of grouped_weights,
+        every expert linear packed_forward_operands' (4- / 8-bit integer codes, no hooks, activation
+        fake-quant or bias), all of one form (bits, qparam dtype and layout, zeros or not, g_idx or
+        not, groups per row), and the shapes the grouped dequant GEMMs take (hidden, inter and the
+        groups multiples of 64)."""
+        if (not x.is_cuda or x.dtype not in (torch.bfloat16, torch.float16)
+                or len(self.experts) > MOE_MAX_EXPERTS or x.shape[1] % 64):
+            return None
+        hidden = x.shape[1]
+        ops, form = [], None
+        for ex in self.experts:
+            if type(ex) is not MixtralExpert or ex._forward_hooks or ex._forward_pre_hooks:
+                return None
+            triple = tuple(packed_forward_operands(m, x.dtype) for m in (ex.w1, ex.w3, ex.w2))
+            if any(o is None for o in triple):
+                return None
+            inter = triple[0].wq.shape[0]
+            for o, (n, k) in zip(triple, ((inter, hidden), (inter, hidden), (hidden, inter))):
+                ng = o.scales.numel() // n
+                if (tuple(o.wq.shape) != (n, k * o.bits // 32) or o.wq.data_ptr() % 16
+                        or inter % 64 or o.group % 64 or k % o.group or o.scales.numel() != n * ng):
+                    return None
+                if not all(t.is_cuda for t in (o.wq, o.scales, o.zeros, o.g_idx) if t is not None):
+                    return None
+                if o.g_idx is not None and (o.g_idx.dtype != torch.int32 or o.g_idx.numel() != k
+                                            or o.g_idx.data_ptr() % 16):
+                    return None
+            f = tuple((o.bits, o.scales.dtype, o.zeros is None, o.g_idx is None, o.transposed, o.group,
+                       o.scales.numel() // o.wq.shape[0]) for o in triple)
+            if form is not None and f != form:
+                return None
+            form = f
+            if f[0] != f[1] or f[0][:5] != f[2][:5]:          # w1 / w3 one form, w2 the same but its groups
+                return None
+            ops.append(triple)
+        return ops
+
     def forward(self, hidden_states):
         B, S, H = hidden_states.shape
         x = hidden_states.reshape(-1, H)
         sel, w = self.route(x)
-        weights = self.grouped_weights(x)
-        out = self.expert_loop(x, sel, w) if weights is None else moe_forward(x, sel, w, weights)
+        experts = self.grouped_weights(x)
+        if experts is None:
+            experts = self.grouped_packed_operands(x)
+        out = self.expert_loop(x, sel, w) if experts is None else moe_forward(x, sel, w, experts)
         return out.reshape(B, S, H)
 
 

@@ -2,7 +2,7 @@
 per-expert loop (MixtralSparseMoe.expert_loop) it replaces.
 
     python scripts/bench_moe.py [--reps 10] [--tokens 2048 65536] [--awq-samples 128] [--awq-rounds 3]
-                                [--out DIR]
+                                [--packed] [--ppl-rounds 3] [--out DIR]
 
 1. One MoE layer (hidden 4096, inter 14336, 8 experts, top-2, bf16) at 2048 tokens (one GPTQ
    calibration forward at batch size 1) and 65536 tokens (the AWQ inspect batch, 128 x 512): the
@@ -14,6 +14,13 @@ per-expert loop (MixtralSparseMoe.expert_loop) it replaces.
    synchronise: awq_rounds rounds of grouped path then loop, each run on a fresh model (the first
    runs include the caching allocator's first allocations at this shape); every round's two runs
    must leave the same weights.  All times are reported, the speed-up is of the medians.
+With --packed, instead of 1. and 2.: the same layer with PACKED experts on the grouped dequant GEMMs
+(module_utils.PackedOperands, csrc/gemm_w4.cu) against the loop over their packed forwards, for W4
+g128 with bf16 qparams, W4 g128 act-order (fp32 qparams, a g_idx per linear) and W8 per-channel
+(random codes and qparams: the kernels' work does not depend on the values), at each of `tokens`,
+timed as in 1.; then the fake-quant perplexity of a one-block Mixtral-8x7B-shaped model after an RTN
+W4 g128 deploy (8 x 2048 tokens), grouped then loop for ppl_rounds alternated rounds on a host
+clock that ends in a device synchronise, with equal perplexities checked.
 Prints, and writes to DIR/bench_moe.json, one JSON object with the card name and power limit.
 """
 import argparse
@@ -94,6 +101,107 @@ def bench_layer(res, tokens, reps):
     torch.cuda.empty_cache()
 
 
+def packed_moe(form, g):
+    """The Mixtral-8x7B MoE layer (bf16) with every expert linear packed in `form`, random values."""
+    from llmc_b200.module_utils import EffcientFakeQuantLinear, pack_unsigned_codes
+    s = synth.SHAPES['mixtral-8x7b']
+    with torch.device('meta'):
+        moe = MixtralSparseMoe(s['hidden'], s['inter'], s['experts'], s['top_k'])
+    moe.gate = moe.gate.to_empty(device='cuda').to(torch.bfloat16)
+    moe.gate.weight.data.normal_(0, 0.02, generator=g)
+    for ex in moe.experts:
+        for n in ('w1', 'w3', 'w2'):
+            lin = getattr(ex, n)
+            N, K = lin.out_features, lin.in_features
+            bits, group = (8, K) if form == 'w8_channel' else (4, 128)
+            qdt = torch.float32 if form == 'w4_g128_gidx_f32' else torch.bfloat16
+            codes = torch.randint(0, 2**bits, (N, K), generator=g, device='cuda', dtype=torch.int32)
+            packed = dict(qweight=pack_unsigned_codes(codes, bits, signed=False),
+                          scales=(torch.rand(N, K // group, generator=g, device='cuda') * 0.01).to(qdt),
+                          zeros=torch.randint(0, 2**bits, (N, K // group), generator=g, device='cuda').to(qdt),
+                          bits=bits, group=group, dtype=torch.bfloat16)
+            if form == 'w4_g128_gidx_f32':
+                packed['g_idx'] = (torch.randperm(K, generator=g, device='cuda') // group).to(torch.int32)
+            del codes
+            m = EffcientFakeQuantLinear(None, None, lin, None, packed=packed)
+            m.in_features, m.out_features = K, N
+            setattr(ex, n, m)
+    return moe
+
+
+def bench_packed_layer(res, tokens, reps):
+    s = synth.SHAPES['mixtral-8x7b']
+    H, I, k = s['hidden'], s['inter'], s['top_k']
+    g = torch.Generator(device='cuda').manual_seed(0)
+    for form in ('w4_g128_native', 'w4_g128_gidx_f32', 'w8_channel'):
+        moe = packed_moe(form, g)
+        for T in tokens:
+            hs = torch.randn(1, T, H, device='cuda', generator=g).to(torch.bfloat16)
+            assert moe.grouped_packed_operands(hs.view(T, H)) is not None
+            grouped, loop = moe(hs), loop_forward(moe, hs)
+            assert torch.equal(grouped.view(torch.int16), loop.view(torch.int16)), (form, T)
+            del grouped, loop
+            runs = {'grouped': lambda: moe(hs), 'loop': lambda: loop_forward(moe, hs)}
+            for fn in runs.values():
+                for _ in range(3):
+                    fn()
+            torch.cuda.synchronize()
+            times = {n: [] for n in runs}
+            for _ in range(reps):
+                for n, fn in runs.items():
+                    times[n].append(timed(fn))
+            med = {n: round(statistics.median(v), 3) for n, v in times.items()}
+            flops = 2.0 * T * k * 3 * H * I
+            key = f'moe_layer[{form}, T={T}]'
+            res['layer_ms'][key] = med
+            res['layer_tflops'][key] = {n: round(flops / (v * 1e-3) / 1e12, 1) for n, v in med.items()}
+            res['layer_speedup'][key] = round(med['loop'] / med['grouped'], 3)
+            print(key, med, res['layer_tflops'][key], flush=True)
+            del hs
+            torch.cuda.empty_cache()
+        del moe
+        torch.cuda.empty_cache()
+
+
+def bench_packed_ppl(res, rounds):
+    from llmc_b200.blockwise import AttrDict
+    from llmc_b200.rtn import RTN
+    cfg = AttrDict.wrap({'base': {'seed': 0},
+                         'quant': {'method': 'RTN', 'weight': {'bit': 4, 'symmetric': False,
+                                                               'granularity': 'per_group', 'group_size': 128}}})
+    model = synth.SynthModel('mixtral-8x7b', n_layers=1, seed=0, device='cuda', init='device')
+    algo = RTN(model, cfg.quant, None, None, cfg)
+    algo.run_block_loop()
+    algo.deploy('fake_quant')
+    tokens = torch.randint(0, model.shape['vocab'], (1, 2048 * 8), generator=torch.Generator().manual_seed(4))
+    saved = MixtralSparseMoe.forward
+
+    def run(loop):
+        if loop:
+            MixtralSparseMoe.forward = loop_forward
+        try:
+            torch.cuda.synchronize()
+            t0 = time.perf_counter()
+            ppl = synth.perplexity(model, tokens, 2048, 1)
+            torch.cuda.synchronize()
+            return time.perf_counter() - t0, ppl
+        finally:
+            MixtralSparseMoe.forward = saved
+    run(False), run(True)                          # warm-up
+    times, ppls = {'grouped': [], 'loop': []}, {'grouped': set(), 'loop': set()}
+    for _ in range(rounds):
+        for path in times:
+            dt, ppl = run(path == 'loop')
+            times[path].append(round(dt, 3))
+            ppls[path].add(ppl)
+    assert ppls['grouped'] == ppls['loop'] and len(ppls['loop']) == 1, ppls
+    key = 'fake_quant_ppl[mixtral-8x7b 1 block, RTN w4 g128, 8x2048 tokens]'
+    med = {n: statistics.median(v) for n, v in times.items()}
+    res['ppl_s'][key] = times
+    res['ppl_speedup'][key] = round(med['loop'] / med['grouped'], 3)
+    print(key, times, flush=True)
+
+
 def run_awq(name, n_samples, seq_len, loop):
     from llmc_b200.awq import Awq
     from llmc_b200.blockwise import AttrDict
@@ -145,15 +253,24 @@ def main():
     ap.add_argument('--tokens', type=int, nargs='+', default=[2048, 65536])
     ap.add_argument('--awq-samples', type=int, default=128)
     ap.add_argument('--awq-rounds', type=int, default=3)
+    ap.add_argument('--packed', action='store_true')
+    ap.add_argument('--ppl-rounds', type=int, default=3)
     ap.add_argument('--out', default=None)
     args = ap.parse_args()
     assert torch.cuda.is_available(), 'needs a CUDA device'
-    res = {'card': card(), 'reps': args.reps, 'layer_ms': {}, 'layer_tflops': {}, 'layer_speedup': {},
-           'awq_s': {}, 'awq_speedup': {}}
-    with torch.no_grad():
-        bench_layer(res, args.tokens, args.reps)
-    if args.awq_samples > 0:
-        bench_awq(res, args.awq_samples, args.awq_rounds)
+    res = {'card': card(), 'reps': args.reps, 'layer_ms': {}, 'layer_tflops': {}, 'layer_speedup': {}}
+    if args.packed:
+        res.update(ppl_s={}, ppl_speedup={})
+        with torch.no_grad():
+            bench_packed_layer(res, args.tokens, args.reps)
+        if args.ppl_rounds > 0:
+            bench_packed_ppl(res, args.ppl_rounds)
+    else:
+        res.update(awq_s={}, awq_speedup={})
+        with torch.no_grad():
+            bench_layer(res, args.tokens, args.reps)
+        if args.awq_samples > 0:
+            bench_awq(res, args.awq_samples, args.awq_rounds)
     doc = json.dumps(res)
     print(doc)
     if args.out:
