@@ -1,4 +1,8 @@
-"""ctypes binding of libllmc_b200.so (C ABI declared in include/llmc_b200.h).
+"""ctypes binding of libllmc_b200.so.
+
+include/llmc_b200.h is the only statement of the C ABI: at import this module reads the header and
+derives from it every entry point's restype and argtypes (SIGNATURES) and the enum / #define
+constants (F32, OUT_*, MOE_MAX_EXPERTS, ...), so a signature is written once, in C.
 
 There is deliberately NO CPU / eager fallback: if the CUDA library is missing or a kernel
 reports an error the call raises.  (The oracle under oracle/ is test infrastructure and is
@@ -6,134 +10,73 @@ never imported from here.)
 """
 import ctypes
 import os
+import re
 import threading
 
 import torch
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, 'libllmc_b200.so')
-
-F32, F16, BF16 = 0, 1, 2
-MOE_MAX_EXPERTS = 8     # LLMC_MOE_MAX_EXPERTS
-OUT_NONE, OUT_QDQ, OUT_CODES_I8, OUT_CODES_U8, OUT_CODES_I32, OUT_PACK_VLLM = range(6)
-
-_DTYPE = {torch.float32: F32, torch.float16: F16, torch.bfloat16: BF16}
-
-c_i64, c_int, c_vp, c_dbl, c_f32 = (ctypes.c_int64, ctypes.c_int, ctypes.c_void_p,
-                                    ctypes.c_double, ctypes.c_float)
-
-# name -> (restype, argtypes); mirrors include/llmc_b200.h one to one.
-SIGNATURES = {
-    'llmc_b200_abi_version': (c_int, []),
-    'llmc_b200_error_string': (ctypes.c_char_p, [c_int]),
-    'llmc_b200_last_error': (ctypes.c_char_p, []),
-    'llmc_b200_launch_count': (ctypes.c_longlong, []),
-    'llmc_quant_dynamic': (c_int, [c_vp, c_i64, c_i64, c_i64, c_int, c_i64, c_int, c_int, c_int,
-                                   c_int, c_int, c_vp, c_vp, c_vp, c_int, c_vp, c_i64, c_int, c_vp]),
-    'llmc_absmean_cols': (c_int, [c_vp, c_i64, c_i64, c_int, c_vp, c_vp, c_i64, c_vp]),
-    'llmc_div_cols': (c_int, [c_vp, c_vp, c_i64, c_i64, c_int, c_vp, c_vp]),
-    'llmc_mse': (c_int, [c_vp, c_vp, c_i64, c_int, c_vp, c_vp, c_vp]),
-    'llmc_awq_clip': (c_int, [c_vp, c_i64, c_i64, c_vp, c_i64, c_int, c_i64, c_int, c_int, c_int,
-                              c_vp, c_vp, c_vp, c_i64, c_vp]),
-    'llmc_quant_static': (c_int, [c_vp, c_i64, c_i64, c_i64, c_int, c_vp, c_vp, c_int, c_int, c_i64,
-                                  c_i64, c_vp, c_int, c_int, c_int, c_int, c_vp, c_i64, c_int,
-                                  c_vp]),
-    'llmc_pack_vllm_codes': (c_int, [c_vp, c_int, c_i64, c_i64, c_int, c_vp, c_vp]),
-    'llmc_minmax_tensor': (c_int, [c_vp, c_i64, c_int, c_vp, c_vp, c_vp]),
-    'llmc_mse_range': (c_int, [c_vp, c_i64, c_i64, c_int, c_int, c_int, c_int, c_int, c_f32, c_f32, c_vp,
-                               c_vp, c_vp]),
-    'llmc_histc': (c_int, [c_vp, c_i64, c_int, c_int, c_f32, c_f32, c_vp, c_vp]),
-    'llmc_pack_awq': (c_int, [c_vp, c_i64, c_i64, c_int, c_vp, c_int, c_vp, c_i64, c_vp, c_vp,
-                              c_vp, c_vp]),
-    'llmc_tri_elems': (c_i64, [c_i64]),
-    'llmc_tri_pack': (c_int, [c_vp, c_i64, c_vp, c_vp]),
-    'llmc_tri_unpack': (c_int, [c_vp, c_i64, c_f32, c_vp, c_vp]),
-    'llmc_syrk_workspace_bytes': (c_i64, [c_i64, c_i64]),
-    'llmc_syrk_accum': (c_int, [c_vp, c_i64, c_i64, c_int, c_vp, c_dbl, c_dbl, c_vp, c_i64,
-                                c_vp]),
-    'llmc_gptq_prepare': (c_int, [c_vp, c_i64, c_vp, c_f32, c_vp, c_vp, c_i64, c_int, c_vp,
-                                  c_vp, c_vp]),
-    'llmc_chol_workspace_bytes': (c_i64, [c_i64]),
-    'llmc_chol_inv_upper': (c_int, [c_vp, c_i64, c_vp, c_i64, c_vp, c_vp]),
-    'llmc_split_tf32': (c_int, [c_vp, c_i64, c_i64, c_i64, c_vp, c_vp, c_vp]),
-    'llmc_gemm_f32x3': (c_int, [c_vp, c_vp, c_i64, c_vp, c_vp, c_i64, c_vp, c_i64, c_i64, c_i64,
-                                c_i64, c_int, c_int, c_vp]),
-    'llmc_gptq_workspace_bytes': (c_i64, [c_i64, c_i64]),
-    'llmc_gptq_colblock': (c_int, [c_vp, c_vp, c_i64, c_i64, c_i64, c_int, c_int, c_int, c_vp,
-                                   c_vp, c_vp, c_int, c_vp, c_vp, c_vp, c_vp, c_i64, c_vp]),
-    'llmc_gptq_colblock_fp8': (c_int, [c_vp, c_vp, c_i64, c_i64, c_i64, c_int, c_int, c_vp, c_vp,
-                                       c_int, c_vp, c_vp, c_vp, c_vp, c_i64, c_vp]),
-    'llmc_spqr_colblock': (c_int, [c_vp, c_vp, c_i64, c_i64, c_i64, c_int, c_int, c_int, c_int, c_int,
-                                   c_int, c_int, c_int, c_int, c_vp, c_int, c_vp, c_vp, c_vp, c_vp,
-                                   c_vp, c_vp, c_vp, c_i64, c_vp]),
-    'llmc_gemm_bf16': (c_int, [c_vp, c_vp, c_vp, c_vp, c_i64, c_i64, c_i64, c_int, c_vp]),
-    'llmc_gemm_rope_qkv': (c_int, [c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_i64, c_i64, c_i64, c_i64,
-                                   c_i64, c_i64, c_int, c_vp]),
-    'llmc_gemm_swiglu': (c_int, [c_vp, c_vp, c_vp, c_i64, c_i64, c_i64, c_int, c_vp]),
-    'llmc_gemm_residual': (c_int, [c_vp, c_vp, c_vp, c_vp, c_i64, c_i64, c_i64, c_int, c_vp]),
-    'llmc_moe_gemm_swiglu': (c_int, [c_vp, c_vp, c_vp, c_vp, c_vp, c_i64, c_i64, c_i64, c_i64, c_int,
-                                     c_vp]),
-    'llmc_moe_gemm_down': (c_int, [c_vp, c_vp, c_vp, c_vp, c_vp, c_i64, c_i64, c_i64, c_i64, c_int,
-                                   c_vp]),
-    'llmc_moe_combine': (c_int, [c_vp, c_vp, c_vp, c_i64, c_i64, c_i64, c_int, c_vp]),
-    'llmc_moe_gemm_packed_swiglu': (c_int, [c_vp, c_int, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_int,
-                                            c_i64, c_i64, c_vp, c_vp, c_i64, c_i64, c_i64, c_i64, c_int, c_vp]),
-    'llmc_moe_gemm_packed_down': (c_int, [c_vp, c_int, c_vp, c_vp, c_vp, c_vp, c_int, c_i64, c_i64, c_vp, c_vp,
-                                          c_vp, c_i64, c_i64, c_i64, c_i64, c_int, c_vp]),
-    'llmc_rmsnorm': (c_int, [c_vp, c_vp, c_vp, c_i64, c_i64, c_f32, c_int, c_vp]),
-    'llmc_rope': (c_int, [c_vp, c_vp, c_vp, c_i64, c_i64, c_i64, c_i64, c_int, c_vp]),
-    'llmc_silu_mul': (c_int, [c_vp, c_vp, c_vp, c_i64, c_int, c_vp]),
-    'llmc_add': (c_int, [c_vp, c_vp, c_vp, c_i64, c_int, c_vp]),
-    'llmc_fp8_quant': (c_int, [c_vp, c_i64, c_i64, c_int, c_i64, c_int, c_int, c_vp, c_int, c_int, c_int,
-                               c_vp, c_vp]),
-    'llmc_fp8_block_quant': (c_int, [c_vp, c_i64, c_i64, c_int, c_int, c_int, c_vp, c_int, c_vp, c_vp]),
-    'llmc_fp8_block_dequant': (c_int, [c_vp, c_i64, c_i64, c_int, c_int, c_vp, c_vp, c_vp]),
-    'llmc_fp8_act_quant': (c_int, [c_vp, c_i64, c_i64, c_int, c_vp, c_vp, c_vp]),
-    'llmc_gemm_fp8_block': (c_int, [c_vp, c_vp, c_vp, c_vp, c_vp, c_int, c_vp, c_int, c_i64, c_i64,
-                                    c_i64, c_vp]),
-    'llmc_gemm_w4a16': (c_int, [c_vp, c_vp, c_vp, c_vp, c_int, c_vp, c_vp, c_i64, c_i64, c_i64, c_i64,
-                                c_int, c_vp]),
-    'llmc_gemm_w8a16': (c_int, [c_vp, c_vp, c_vp, c_vp, c_int, c_vp, c_vp, c_i64, c_i64, c_i64, c_i64,
-                                c_int, c_vp]),
-    'llmc_gemm_w4a16_gidx': (c_int, [c_vp, c_vp, c_vp, c_vp, c_int, c_vp, c_i64, c_int, c_vp, c_vp, c_i64,
-                                     c_i64, c_i64, c_int, c_vp]),
-    'llmc_gemm_w8a16_gidx': (c_int, [c_vp, c_vp, c_vp, c_vp, c_int, c_vp, c_i64, c_int, c_vp, c_vp, c_i64,
-                                     c_i64, c_i64, c_int, c_vp]),
-    'llmc_gemm_w4a16_awq': (c_int, [c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_i64, c_i64, c_i64, c_i64, c_int,
-                                    c_vp]),
-    'llmc_gemm_fp8a16': (c_int, [c_vp, c_vp, c_vp, c_vp, c_int, c_vp, c_vp, c_i64, c_i64, c_i64, c_i64,
-                                 c_int, c_int, c_vp]),
-    'llmc_gemm_fp8a16_gidx': (c_int, [c_vp, c_vp, c_vp, c_vp, c_int, c_vp, c_i64, c_int, c_vp, c_vp, c_i64,
-                                      c_i64, c_i64, c_int, c_int, c_vp]),
-    'llmc_gemm_w2a16': (c_int, [c_vp, c_vp, c_vp, c_vp, c_int, c_vp, c_vp, c_i64, c_i64, c_i64, c_i64,
-                                c_int, c_vp]),
-    'llmc_gemm_w3a16': (c_int, [c_vp, c_vp, c_vp, c_vp, c_int, c_vp, c_vp, c_i64, c_i64, c_i64, c_i64,
-                                c_int, c_vp]),
-    'llmc_gemm_w2a16_gidx': (c_int, [c_vp, c_vp, c_vp, c_vp, c_int, c_vp, c_i64, c_int, c_vp, c_vp, c_i64,
-                                     c_i64, c_i64, c_int, c_vp]),
-    'llmc_gemm_w3a16_gidx': (c_int, [c_vp, c_vp, c_vp, c_vp, c_int, c_vp, c_i64, c_int, c_vp, c_vp, c_i64,
-                                     c_i64, c_i64, c_int, c_vp]),
-    'llmc_pack_w3_codes': (c_int, [c_vp, c_i64, c_i64, c_vp, c_vp]),
-    'llmc_gemm_w2a16_rz': (c_int, [c_vp, c_vp, c_vp, c_vp, c_int, c_int, c_i64, c_vp, c_i64, c_vp, c_vp, c_vp,
-                                   c_vp, c_vp, c_i64, c_i64, c_i64, c_int, c_vp]),
-    'llmc_gemm_w3a16_rz': (c_int, [c_vp, c_vp, c_vp, c_vp, c_int, c_int, c_i64, c_vp, c_i64, c_vp, c_vp, c_vp,
-                                   c_vp, c_vp, c_i64, c_i64, c_i64, c_int, c_vp]),
-    'llmc_gemm_w4a16_rz': (c_int, [c_vp, c_vp, c_vp, c_vp, c_int, c_int, c_i64, c_vp, c_i64, c_vp, c_vp, c_vp,
-                                   c_vp, c_vp, c_i64, c_i64, c_i64, c_int, c_vp]),
-    'llmc_gemm_w8a16_rz': (c_int, [c_vp, c_vp, c_vp, c_vp, c_int, c_int, c_i64, c_vp, c_i64, c_vp, c_vp, c_vp,
-                                   c_vp, c_vp, c_i64, c_i64, c_i64, c_int, c_vp]),
-    'llmc_gemm_w8a8_i8': (c_int, [c_vp, c_vp, c_i64, c_vp, c_vp, c_i64, c_vp, c_vp, c_i64, c_i64, c_i64, c_int,
-                                  c_vp]),
-    'llmc_gemm_w8a8_fp8': (c_int, [c_vp, c_vp, c_i64, c_vp, c_vp, c_i64, c_vp, c_vp, c_i64, c_i64, c_i64, c_int,
-                                   c_vp]),
-}
-
-_lock = threading.Lock()
-_lib = None
+HEADER_PATH = os.path.join(_HERE, '..', 'include', 'llmc_b200.h')
 
 
 class LlmcB200Error(RuntimeError):
     pass
+
+
+# every pointer binds as c_void_p, a `const char*` return value as c_char_p, these by name; any
+# other C type is an error, never a default
+_CTYPES = {'int': ctypes.c_int, 'int64_t': ctypes.c_int64, 'long long': ctypes.c_longlong,
+           'float': ctypes.c_float, 'double': ctypes.c_double}
+
+
+def _ctype(decl, proto):
+    """ctypes class of the C type `decl` ('int64_t', 'const void * const *', ...) of prototype `proto`."""
+    if '*' in decl:
+        return ctypes.c_void_p
+    if decl not in _CTYPES:
+        raise LlmcB200Error(f'llmc_b200.h: {proto}: no ctypes binding for the C type {decl!r}')
+    return _CTYPES[decl]
+
+
+def parse_header(text):
+    """(signatures, constants) of the C header `text`.  signatures: every prototype
+    `ret llmc_*(params);` (the return type on the name's line, the parameters on any number of
+    lines) as name -> (restype, [argtypes]); constants: every enum member with an explicit value
+    and every integer `#define LLMC_*`, as name -> int."""
+    text = re.sub(r'/\*.*?\*/', ' ', text, flags=re.S)
+    consts = {n: int(v, 0) for n, v in re.findall(r'^[ \t]*#[ \t]*define[ \t]+(LLMC_\w+)[ \t]+(-?\d\w*)[ \t]*$',
+                                                  text, flags=re.M)}
+    for body in re.findall(r'\benum\s*\{(.*?)\}', text, flags=re.S):
+        consts.update((n, int(v, 0)) for n, v in re.findall(r'\b(LLMC_\w+)\s*=\s*(-?\d\w*)', body))
+    sigs = {}
+    for ret, name, params in re.findall(r'^[ \t]*(\w[\w \t]*?\**)[ \t]*\b(llmc_\w+)\s*\(([^()]*)\)\s*;',
+                                        text, flags=re.M):
+        ret = ' '.join(ret.replace('*', ' *').split())
+        params = [' '.join(p.split()) for p in params.split(',')]
+        # a parameter is `type name`: drop the name unless the type is a pointer (which binds whole)
+        sigs[name] = (ctypes.c_char_p if ret == 'const char *' else _ctype(ret, name),
+                      [] if params == ['void'] else
+                      [_ctype(p if '*' in p else p.rsplit(' ', 1)[0], name) for p in params])
+    return sigs, consts
+
+
+if not os.path.exists(HEADER_PATH):
+    raise LlmcB200Error(f'{HEADER_PATH} not found: the ctypes bindings are read from this C header, '
+                        'which sits in include/ beside the llmc_b200 package')
+with open(HEADER_PATH) as _fh:
+    SIGNATURES, CONSTANTS = parse_header(_fh.read())
+
+F32, F16, BF16 = CONSTANTS['LLMC_F32'], CONSTANTS['LLMC_F16'], CONSTANTS['LLMC_BF16']
+OUT_NONE, OUT_QDQ, OUT_CODES_I8, OUT_CODES_U8, OUT_CODES_I32, OUT_PACK_VLLM, OUT_FLAG_ZP_INSIDE = (
+    CONSTANTS['LLMC_OUT_' + n] for n in ('NONE', 'QDQ', 'CODES_I8', 'CODES_U8', 'CODES_I32', 'PACK_VLLM',
+                                         'FLAG_ZP_INSIDE'))
+MOE_MAX_EXPERTS = CONSTANTS['LLMC_MOE_MAX_EXPERTS']
+
+_DTYPE = {torch.float32: F32, torch.float16: F16, torch.bfloat16: BF16}
+
+_lock = threading.Lock()
+_lib = None
 
 
 def load():

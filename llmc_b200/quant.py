@@ -13,8 +13,8 @@ import torch
 
 from . import _lib
 from .prof import TIMER
-from ._lib import (OUT_CODES_I8, OUT_CODES_I32, OUT_CODES_U8, OUT_NONE, OUT_PACK_VLLM,
-                   OUT_QDQ, call, dtype_enum, ptr, require_cuda, stream_ptr)
+from ._lib import (OUT_CODES_I8, OUT_CODES_I32, OUT_CODES_U8, OUT_FLAG_ZP_INSIDE, OUT_NONE,
+                   OUT_PACK_VLLM, OUT_QDQ, call, dtype_enum, ptr, require_cuda, stream_ptr)
 
 
 def ceil_div(a, b):
@@ -419,7 +419,7 @@ class IntegerQuantizer(BaseQuantizer):
         elif torch.is_tensor(zeros) and zeros.numel() == 1 and (zeros.is_cuda or float(zeros) != 0.0):
             z = zeros.to(device=s.device, dtype=s.dtype).reshape(1).expand(s.numel()).reshape(s.shape).contiguous()
         if not self.round_zp:
-            out_mode |= 0x100          # LLMC_OUT_FLAG_ZP_INSIDE: round(x / s + z), quant.py:702-707
+            out_mode |= OUT_FLAG_ZP_INSIDE  # round(x / s + z), quant.py:702-707
         with TIMER.span('quant_static', nbytes=float(w.element_size()) * rows * cols):
             call('llmc_quant_static', ptr(w), rows, cols, cols, dtype_enum(w.dtype), ptr(s),
                  ptr(z), dtype_enum(s.dtype), round_dtype, q_row_stride, group, ptr(gmap),

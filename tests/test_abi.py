@@ -1,5 +1,5 @@
 """CPU: libllmc_b200.so loads without a GPU and exports every symbol include/llmc_b200.h declares;
-the ctypes signature table covers the same set (no compute calls here)."""
+the ctypes signatures parsed from the header cover the same set (no compute calls here)."""
 import ctypes
 import os
 import re
@@ -31,8 +31,30 @@ def test_every_declared_symbol_is_exported(lib):
 
 
 def test_signature_table_matches_header():
+    """The loose scan above finds every `llmc_*(`; the strict parser must not skip one."""
     from llmc_b200 import _lib
     assert sorted(_lib.SIGNATURES) == _declared()
+
+
+def test_header_parser_binds_each_c_type():
+    from llmc_b200 import _lib
+    i64, vp, i32 = ctypes.c_int64, ctypes.c_void_p, ctypes.c_int
+    sig = _lib.SIGNATURES
+    assert sig['llmc_b200_error_string'] == (ctypes.c_char_p, [i32])
+    assert sig['llmc_b200_launch_count'] == (ctypes.c_longlong, [])
+    dbl, f32 = ctypes.c_double, ctypes.c_float
+    assert sig['llmc_syrk_accum'] == (i32, [vp, i64, i64, i32, vp, dbl, dbl, vp, i64, vp])
+    assert sig['llmc_mse_range'] == (i32, [vp, i64, i64, i32, i32, i32, i32, i32, f32, f32, vp, vp, vp])
+    assert sig['llmc_gemm_w4a16'] == (i32, [vp, vp, vp, vp, i32, vp, vp, i64, i64, i64, i64, i32, vp])
+    assert sig['llmc_moe_gemm_packed_swiglu'] == (i32, [vp, i32] + [vp] * 8 + [i32, i64, i64, vp, vp]
+                                                  + [i64] * 4 + [i32, vp])
+    # a prototype over two lines, enum members and defines with explicit integer values; a C type
+    # without a binding raises rather than falling back to int
+    sigs, consts = _lib.parse_header('#define LLMC_X 0x20\nenum { LLMC_A = -4, LLMC_B };\n'
+                                     'int llmc_x(const int32_t* const* a,\n           double b);\n')
+    assert sigs == {'llmc_x': (i32, [vp, dbl])} and consts == {'LLMC_X': 32, 'LLMC_A': -4}
+    with pytest.raises(_lib.LlmcB200Error, match=r'llmc_y.*unsigned'):
+        _lib.parse_header('int llmc_y(const void* x, unsigned n, void* stream);\n')
 
 
 def test_version_and_error_strings(lib):
@@ -45,11 +67,10 @@ def test_version_and_error_strings(lib):
 
 def test_argument_validation_without_gpu(lib):
     """Bad arguments are rejected before any CUDA call, so this runs on a CPU-only box."""
+    from llmc_b200 import _lib
     f = lib.llmc_quant_dynamic
-    f.restype = ctypes.c_int
-    i64, vp = ctypes.c_int64, ctypes.c_void_p
-    f.argtypes = [vp, i64, i64, i64, ctypes.c_int, i64, ctypes.c_int, ctypes.c_int, ctypes.c_int,
-                  ctypes.c_int, ctypes.c_int, vp, vp, vp, ctypes.c_int, vp, i64, ctypes.c_int, vp]
+    f.restype, f.argtypes = _lib.SIGNATURES['llmc_quant_dynamic']
+    vp = ctypes.c_void_p
     # cols not divisible by group
     rc = f(vp(16), 4, 100, 100, 1, 64, 4, 1, 0, 0, 0, None, vp(16), None, 0, None, 0, 1, None)
     assert rc == -1

@@ -12,6 +12,7 @@ import torch
 
 import fp8_gemm_oracle as fgo
 import w8a8_oracle as wo
+from llmc_b200._lib import BF16, F16, F32
 from oracle.glue_oracle import fma32
 
 GOLDEN = os.path.join(os.path.dirname(os.path.abspath(__file__)), 'golden', 'fp8_gemm_kat.pt')
@@ -229,7 +230,6 @@ def test_argument_validation_without_gpu(lib):
     def last():
         return lib.llmc_b200_last_error().decode()
 
-    F32, F16, BF16 = 0, 1, 2
     # act_quant: K % 128, null pointers, dtype; rows == 0 is a no-op
     assert lib.llmc_fp8_act_quant(p, 4, 200, BF16, p, p, null) == -1 and 'multiple of 128' in last()
     assert lib.llmc_fp8_act_quant(p, 4, 256, 7, p, p, null) == -1 and 'bad dtype' in last()

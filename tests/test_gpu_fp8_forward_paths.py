@@ -25,7 +25,7 @@ import torch
 
 import fp8_gemm_oracle as fgo
 import w8a8_oracle as wo
-from llmc_b200._lib import load, ptr, stream_ptr
+from llmc_b200._lib import BF16, F16, F32, load, ptr, stream_ptr
 
 pytestmark = pytest.mark.gpu
 
@@ -33,7 +33,6 @@ E4M3 = torch.float8_e4m3fn
 NUM_SMS = 132                           # persistent kernels run min(units, 132) CTAs
 STAGES = 6                              # gemm_8bit.cu's ring: one stage per 128-deep K block
 ACT_PASS = NUM_SMS * 16 * 16            # act_quant: 16 groups per block, at most 132 * 16 blocks
-F32, F16, BF16 = 0, 1, 2
 LLMC_EINVAL, LLMC_EALIGN = -1, -4
 INT_VIEW = {torch.float32: torch.int32, torch.bfloat16: torch.int16, torch.float16: torch.int16}
 

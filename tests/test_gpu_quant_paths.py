@@ -18,15 +18,14 @@ import math
 import pytest
 import torch
 
-from llmc_b200._lib import (BF16, F16, F32, OUT_CODES_I8, OUT_CODES_I32, OUT_CODES_U8, OUT_NONE,
-                            OUT_PACK_VLLM, OUT_QDQ, call, ptr, stream_ptr)
+from llmc_b200._lib import (BF16, F16, F32, OUT_CODES_I8, OUT_CODES_I32, OUT_CODES_U8, OUT_FLAG_ZP_INSIDE,
+                            OUT_NONE, OUT_PACK_VLLM, OUT_QDQ, call, ptr, stream_ptr)
 from oracle import quant_oracle as qo
 
 pytestmark = pytest.mark.gpu
 
 DT = {torch.float32: F32, torch.float16: F16, torch.bfloat16: BF16}
 INT_VIEW = {torch.float32: torch.int32, torch.float16: torch.int16, torch.bfloat16: torch.int16}
-ZP_INSIDE = 0x100
 SENTINEL = 0x5A5A5A5A
 
 
@@ -585,7 +584,7 @@ def stat(wv, scales, zeros, round_dtype, q_row_stride, group, gmap, bit, qmin, q
     out = _out_buf(mode, rows, cols, bit, out_dtype, ld_out)
     call('llmc_quant_static', ptr(wv), rows, cols, wv.stride(0), DT[wv.dtype], ptr(scales),
          ptr(zeros), DT[scales.dtype], round_dtype, q_row_stride, group, ptr(gmap), bit, qmin, qmax,
-         mode | (ZP_INSIDE if zp_inside else 0), ptr(out), ld_out, DT[out_dtype], stream_ptr())
+         mode | (OUT_FLAG_ZP_INSIDE if zp_inside else 0), ptr(out), ld_out, DT[out_dtype], stream_ptr())
     return out
 
 

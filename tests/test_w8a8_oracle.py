@@ -8,6 +8,7 @@ import pytest
 import torch
 
 import w8a8_oracle as wo
+from llmc_b200._lib import BF16, F16, F32
 
 E4M3 = torch.float8_e4m3fn
 
@@ -23,7 +24,6 @@ def lib():
 def test_arguments_are_checked_before_launch(lib, name):
     p, null = ctypes.c_void_p(256), ctypes.c_void_p(0)
     f = getattr(lib, name)
-    BF16, F16, F32 = 2, 1, 0
 
     def last():
         return lib.llmc_b200_last_error().decode()
