@@ -103,6 +103,41 @@ def test_mixtral_8x7b_layer_2048_tokens(dtype):
     torch.cuda.empty_cache()
 
 
+# expert counts below 8 and top_k up to E, at widths with a K tail (264), a partial 256-column
+# n-tile of the down projection (264, 320) and one gate/up n-tile (inter 128)
+EXPERTS_TOP_K = [(1, 1), (2, 1), (2, 2), (3, 2), (3, 3), (5, 3), (5, 5), (8, 3), (8, 8)]
+
+
+def _sel_random(T, E, k, seed=5):
+    """Each token's k distinct experts, in random order."""
+    g = torch.Generator().manual_seed(seed)
+    return torch.rand(T, E, generator=g).argsort(dim=1)[:, :k].cuda()
+
+
+@pytest.mark.parametrize('hidden,inter', [(264, 128), (320, 384), (4096, 128)])
+@pytest.mark.parametrize('E,k', EXPERTS_TOP_K)
+def test_expert_counts_top_k_and_widths(E, k, hidden, inter):
+    dtype = torch.bfloat16 if (E + k) % 2 else torch.float16
+    moe = _moe(hidden, inter, E, k, dtype)
+    T = 200
+    _check(moe, _x(T, hidden, dtype), _sel_random(T, E, k), _weights(T, k, dtype))
+
+
+@pytest.mark.parametrize('dtype', [torch.bfloat16, torch.float16])
+def test_zero_tokens_launch_nothing(dtype):
+    from llmc_b200._lib import load
+    hidden = 264
+    moe = _moe(hidden, 128, 3, 2, dtype)
+    x = torch.empty(0, hidden, dtype=dtype, device='cuda')
+    sel = torch.empty(0, 2, dtype=torch.int64, device='cuda')
+    torch.cuda.synchronize()
+    before = load().llmc_b200_launch_count()
+    out = moe_forward(x, sel, torch.empty(0, 2, dtype=dtype, device='cuda'), moe.grouped_weights(x))
+    torch.cuda.synchronize()
+    assert load().llmc_b200_launch_count() == before
+    assert out.shape == (0, hidden) and out.dtype == dtype
+
+
 def test_no_host_sync_on_the_grouped_path():
     s = synth.SHAPES['tiny-mixtral']
     moe = _moe(s['hidden'], s['inter'], s['experts'], s['top_k'], torch.bfloat16)

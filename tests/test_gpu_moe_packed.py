@@ -151,6 +151,44 @@ def test_partial_tiles(dtype, form):
     _check(moe, _x(T, hidden, dtype), sel, _weights(T, 2, dtype))
 
 
+# expert counts below 8 and top_k up to E, at widths with a partial 128-column n-tile of the down
+# projection (320) and inter 64: one gate/up n-tile, one k-step in the down projection
+EXPERTS_TOP_K = [(1, 1), (2, 1), (2, 2), (3, 2), (3, 3), (5, 3), (5, 5), (8, 3), (8, 8)]
+
+
+def _sel_random(T, E, k, seed=5):
+    """Each token's k distinct experts, in random order."""
+    g = torch.Generator().manual_seed(seed)
+    return torch.rand(T, E, generator=g).argsort(dim=1)[:, :k].cuda()
+
+
+@pytest.mark.parametrize('hidden,inter', [(320, 64), (320, 128), (4096, 384)])
+@pytest.mark.parametrize('E,k', EXPERTS_TOP_K)
+@pytest.mark.parametrize('form', FORMS)
+def test_expert_counts_top_k_and_widths(form, E, k, hidden, inter):
+    dtype = torch.bfloat16 if (E + k) % 2 else torch.float16
+    moe = _moe(hidden, inter, E, k, dtype, form, group=64)
+    T = 200
+    _check(moe, _x(T, hidden, dtype), _sel_random(T, E, k), _weights(T, k, dtype))
+
+
+@pytest.mark.parametrize('form', FORMS)
+def test_zero_tokens_launch_nothing(form):
+    from llmc_b200._lib import load
+    dtype, hidden = torch.bfloat16, 320
+    moe = _moe(hidden, 64, 3, 2, dtype, form, group=64)
+    x = torch.empty(0, hidden, dtype=dtype, device='cuda')
+    sel = torch.empty(0, 2, dtype=torch.int64, device='cuda')
+    ops = moe.grouped_packed_operands(x)
+    assert ops is not None
+    torch.cuda.synchronize()
+    before = load().llmc_b200_launch_count()
+    out = moe_forward(x, sel, torch.empty(0, 2, dtype=dtype, device='cuda'), ops)
+    torch.cuda.synchronize()
+    assert load().llmc_b200_launch_count() == before
+    assert out.shape == (0, hidden) and out.dtype == dtype
+
+
 @pytest.mark.parametrize('form', ['w4_g128_gidx_f32', 'vllm_w4_sym'])
 def test_no_host_sync_on_the_grouped_packed_path(form):
     s = synth.SHAPES['tiny-mixtral']
