@@ -387,6 +387,30 @@ int llmc_moe_gemm_packed_down(const void* act, int bits, const int32_t* const* w
                               int64_t rows, int64_t N, int64_t inter, int64_t n_experts, int dtype,
                               void* stream);
 
+/* The same two grouped projections on W8A8 experts (the llmc_gemm_w8a8_i8 / _fp8 GEMM, grouped): bit
+ * for bit the per-expert loop over llmc_gemm_w8a8_* with the same codes and scales, no bias.  fp8 0:
+ * int8 codes, else e4m3, for xq / actq and every expert weight alike.  s_x [rows] fp32, one scale
+ * per row of xq / actq (a per-tensor static scale repeated per row, in that row order).  Each expert
+ * linear's codes w [N_lin, K] with its own fp32 scales s_w (HOST arrays of E device pointers like
+ * the weights): N_lin values each when s_w_stride is 1, one each when it is 0.  Output bf16 / fp16
+ * (dtype).  K a multiple of 16 (int8: at most llmc_gemm_w8a8_i8's limit); N a multiple of 8.
+ * rows == 0 is a no-op; every argument error is returned before any CUDA call (misaligned xq / actq
+ * / act / y / codes: LLMC_EALIGN).
+ *   llmc_moe_gemm_w8a8_swiglu  act[rows, inter] = llmc_silu_mul(G, U) per segment, G / U the
+ *                              llmc_gemm_w8a8_* outputs of xq on w1 / w3 [inter, K] before their
+ *                              rounding; inter a multiple of 64.
+ *   llmc_moe_gemm_w8a8_down    y[rows, N] = rT(rT(S) * w_route[row]) per segment, S the
+ *                              llmc_gemm_w8a8_* output of actq on w2 [N, inter] before its rounding;
+ *                              K = inter. */
+int llmc_moe_gemm_w8a8_swiglu(const void* xq, const float* s_x, int fp8, const void* const* w1,
+                              const void* const* w3, const float* const* s_w1, const float* const* s_w3,
+                              int64_t s_w_stride, const int32_t* offsets, void* act, int64_t rows,
+                              int64_t inter, int64_t K, int64_t n_experts, int dtype, void* stream);
+int llmc_moe_gemm_w8a8_down(const void* actq, const float* s_x, int fp8, const void* const* w2,
+                            const float* const* s_w2, int64_t s_w_stride, const int32_t* offsets,
+                            const void* w_route, void* y, int64_t rows, int64_t N, int64_t inter,
+                            int64_t n_experts, int dtype, void* stream);
+
 /* ------------------------------------------------------------------------------------
  * K6  llmc_gemm_w4a16 — fake-quant forward on PACKED weights:
  *   Y[M,N] = X[M,K] · dequant(Wq)[N,K]^T (+ bias), dequant(Wq)[n,k] =

@@ -18,6 +18,8 @@
 //     INT8  wgmma m64n128k32 s32.s8.s8: the int32 sum is exact (K <= 131056 bounds it by 2^31 for
 //           any int8 codes), fp32(acc) is cvt.rn.
 //     FP8   a fresh dot per K block as in block-FP8, promoted by acc = fadd(acc, dot).
+//   Grouped W8A8 (llmc_moe_gemm_w8a8_swiglu / _down): the same GEMM over a sparse-MoE layer's routed
+//   rows, one launch per projection of every expert (MoeW8A8Operands below).
 //
 // One persistent, warp-specialised kernel template (1 CTA per SM, 3 warpgroups), the structure of
 // gemm.cu's wgmma_gemm_kernel:
@@ -89,6 +91,65 @@ struct W8A8Params {
 template <Mode kMode>
 using Params = std::conditional_t<kMode == kBlockFp8, Fp8GemmParams, W8A8Params>;
 
+// Grouped (sparse-MoE) mode of the W8A8 GEMM: one launch runs one projection of every expert of a
+// layer (gemm.cu's and gemm_w4.cu's grouped GEMMs, on 8-bit codes).  A = the routed rows quantised
+// in expert order, expert e owning rows [offsets[e], offsets[e+1]); tiles come from
+// tc::moe_segment_tile; s_x is one fp32 scale per A row (stride 1).
+//   kMoeSwiGLU  the 128-row B stage is two 64-row TMA boxes: w1 rows n0 .. n0 + 63 of the tile's
+//               expert, then the same rows of w3.  A box is 64 x 128 bytes, a whole number of
+//               128-byte swizzle atoms, so the stage is byte for byte the plain kernel's.  The
+//               epilogue writes act = silu(gate) * up for 64 columns (tc::store_swiglu_m64n64).
+//   kMoeDown    128-row tiles of w2; each output row times its routing weight (tc::store_routed_m64n128).
+// Both scale the accumulator as the plain W8A8 epilogue does first (scale_moe_w8a8).
+enum : int { kMoeOff = 0, kMoeSwiGLU = 1, kMoeDown = 2 };
+// The grouped operands of one launch, per expert linear (gate/up: w1 of expert e at 2e, w3 at
+// 2e + 1; down: w2 of expert e at e): its codes' tensor map and its weight scales (N values, or one
+// when W8A8Params::s_w_stride is 0).  A kernel argument of its own, after Params.
+struct MoeW8A8Operands {
+  CUtensorMap tmB[2 * LLMC_MOE_MAX_EXPERTS];
+  const float* s_w[2 * LLMC_MOE_MAX_EXPERTS];
+  const int32_t* offsets;                 // [E + 1] row offsets of the expert segments
+  const void* w_route;                    // kMoeDown: [rows] routing weights (A's row order)
+  int E;
+};
+// The whole argument list of the grouped kernel fits the 4 KB kernel-parameter space at
+// LLMC_MOE_MAX_EXPERTS experts.
+static_assert(2 * sizeof(CUtensorMap) + sizeof(W8A8Params) + sizeof(MoeW8A8Operands) <= 4096,
+              "LLMC_MOE_MAX_EXPERTS exceeds the kernel-parameter space");
+
+// The last kernel argument: the grouped operands in grouped mode; in plain mode an unused null
+// pointer, which leaves the plain instantiations' code as it was without the argument.
+template <int kMoe> using MoeArg = std::conditional_t<kMoe == kMoeOff, const void*, MoeW8A8Operands>;
+
+// Grouped mode: acc = fmul(fmul(acc, s_w[col]), s_x[row]) over this thread's part of an m64n128
+// fragment (layout at wgmma_m64n128k16_bf16) whose first row is A row row0 — the plain W8A8
+// epilogue's scaling, before the shared grouped stores round.  kSwiGLU: fragments j < 8 are w1
+// column col0 + 8 j + ... (scales sw_a), fragments j >= 8 the same columns of w3 (sw_b); else
+// fragment j is w2 column col0 + 8 j + ... (sw_a).  Rows past p.M and columns past p.N read the
+// last row's / column's scale; their results are never stored.
+template <bool kSwiGLU>
+__device__ __forceinline__ void scale_moe_w8a8(float (&acc)[64], int64_t row0, int64_t col0, const W8A8Params& p,
+                                               const float* sw_a, const float* sw_b) {
+  const int tid = threadIdx.x & 127, lane = threadIdx.x & 31;
+  const int64_t r_lo = row0 + (tid >> 5) * 16 + (lane >> 2);
+  const float sx0 = __ldg(p.s_x + min(r_lo, p.M - 1));
+  const float sx1 = __ldg(p.s_x + min(r_lo + 8, p.M - 1));
+#pragma unroll
+  for (int j = 0; j < 16; ++j) {
+    const float* sw = (kSwiGLU && j >= 8) ? sw_b : sw_a;
+    const int64_t col = col0 + 8 * (kSwiGLU ? (j & 7) : j) + 2 * (lane & 3);
+#pragma unroll
+    for (int e = 0; e < 2; ++e) {
+      const float s = __ldg(sw + min(col + e, p.N - 1) * p.s_w_stride);
+#pragma unroll
+      for (int i = 0; i < 2; ++i) {
+        const int x = 4 * j + 2 * i + e;
+        acc[x] = fmul_rn(fmul_rn(acc[x], s), i ? sx1 : sx0);
+      }
+    }
+  }
+}
+
 // Y = rT(fmul(fmul(acc, s_w[n]), s_x[m]) (+ bias[n])) for this thread's part of an m64n128
 // fragment (layout at wgmma_m64n128k16_bf16) whose element (0, 0) is Y[row0][col0].
 template <int DT>
@@ -150,11 +211,24 @@ __device__ __forceinline__ void store_bf16_bias_m64n128(const float (&acc)[64], 
 }
 
 // DT is the output dtype: fp32 / bf16 for kBlockFp8, bf16 / fp16 for the W8A8 modes.
-template <Mode kMode, int DT>
+// Plain mode: tiles from grouped_tile, B from tmB.  Grouped mode (kMoe, W8A8 only): tiles from
+// moe_segment_tile, B and the weight scales of the tile's expert from `moe`; tmB is unused.
+template <Mode kMode, int DT, int kMoe = kMoeOff>
 __global__ void __launch_bounds__(kThreads, 1)
 gemm_8bit_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
-                 const Params<kMode> p) {
+                 const Params<kMode> p, const __grid_constant__ MoeArg<kMoe> moe) {
+  static_assert(kMoe == kMoeOff || kMode != kBlockFp8, "the grouped mode runs the W8A8 GEMM");
   constexpr bool kInt8 = kMode == kW8A8Int8;
+  // the tile of unit u (grouped mode: also its expert, first A row and segment end); false past
+  // the last expert's tiles
+  auto tile_of = [&](int u, int& e, int& m_blk, int& n_blk, int& row0, int& row_end) -> bool {
+    if constexpr (kMoe != kMoeOff) {
+      return moe_segment_tile<kBM>(moe.offsets, moe.E, u, p.n_tiles, p.gn, e, m_blk, n_blk, row0, row_end);
+    } else {
+      grouped_tile(u, p.m_tiles, p.n_tiles, p.gn, m_blk, n_blk);
+      return true;
+    }
+  };
   extern __shared__ uint8_t smem_raw[];
   // The ring is reached only through TMA and wgmma descriptors, so the generic address costs
   // nothing here.  tc::ring_base and tc::Ring's init, waits and release are not used: with either,
@@ -171,7 +245,11 @@ gemm_8bit_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
 
   if (threadIdx.x == 0) {
     prefetch_tmap(&tmA);
-    prefetch_tmap(&tmB);
+    if constexpr (kMoe != kMoeOff) {
+      for (int i = 0; i < (kMoe == kMoeSwiGLU ? 2 : 1) * moe.E; ++i) prefetch_tmap(&moe.tmB[i]);
+    } else {
+      prefetch_tmap(&tmB);
+    }
     for (int s = 0; s < kStages; ++s) {
       mbar_init(&full_bar[s], 1);
       mbar_init(&empty_bar[s], 2);    // one arrive per consumer warpgroup
@@ -185,14 +263,24 @@ gemm_8bit_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
     if (tid == 0) {
       PipeState<kStages> ps;
       for (int u = blockIdx.x; u < p.num_tiles; u += gridDim.x) {
-        int m_blk, n_blk;
-        grouped_tile(u, p.m_tiles, p.n_tiles, p.gn, m_blk, n_blk);
+        int e, m_blk, n_blk, row0, row_end;
+        if (!tile_of(u, e, m_blk, n_blk, row0, row_end)) break;
         for (int kb = 0; kb < p.kb_total; ++kb) {
           mbar_wait(&empty_bar[ps.stage], ps.phase ^ 1);
           uint8_t* a_dst = smem + ps.stage * kStageBytes;
           mbar_expect_tx(&full_bar[ps.stage], kStageBytes);
-          tma_load_2d(a_dst, &tmA, &full_bar[ps.stage], kb * kBK, m_blk * kBM);
-          tma_load_2d(a_dst + kTileBytes, &tmB, &full_bar[ps.stage], kb * kBK, n_blk * kBN);
+          if constexpr (kMoe == kMoeSwiGLU) {          // 64 rows of w1, then the same 64 rows of w3
+            tma_load_2d(a_dst, &tmA, &full_bar[ps.stage], kb * kBK, row0);
+            tma_load_2d(a_dst + kTileBytes, &moe.tmB[2 * e], &full_bar[ps.stage], kb * kBK, n_blk * (kBN / 2));
+            tma_load_2d(a_dst + kTileBytes + kTileBytes / 2, &moe.tmB[2 * e + 1], &full_bar[ps.stage], kb * kBK,
+                        n_blk * (kBN / 2));
+          } else if constexpr (kMoe == kMoeDown) {
+            tma_load_2d(a_dst, &tmA, &full_bar[ps.stage], kb * kBK, row0);
+            tma_load_2d(a_dst + kTileBytes, &moe.tmB[e], &full_bar[ps.stage], kb * kBK, n_blk * kBN);
+          } else {
+            tma_load_2d(a_dst, &tmA, &full_bar[ps.stage], kb * kBK, m_blk * kBM);
+            tma_load_2d(a_dst + kTileBytes, &tmB, &full_bar[ps.stage], kb * kBK, n_blk * kBN);
+          }
           ps.advance();
         }
       }
@@ -205,8 +293,8 @@ gemm_8bit_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
   const int lane = tid & 31;
   PipeState<kStages> ps;
   for (int u = blockIdx.x; u < p.num_tiles; u += gridDim.x) {
-    int m_blk, n_blk;
-    grouped_tile(u, p.m_tiles, p.n_tiles, p.gn, m_blk, n_blk);
+    int e, m_blk, n_blk, row0, row_end;
+    if (!tile_of(u, e, m_blk, n_blk, row0, row_end)) break;
     // block-FP8: this thread's first fragment row (layout at wgmma_m64n128k16_bf16) and the scales
     // of its two rows; rows past M read the scale of row M - 1 — their results are never stored
     int64_t r_lo = 0;
@@ -281,14 +369,22 @@ gemm_8bit_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
     }
 
     // ---- epilogue straight from the registers ----
-    const int64_t row0 = static_cast<int64_t>(m_blk) * kBM + c * 64;
+    const int64_t r0 = static_cast<int64_t>(m_blk) * kBM + c * 64;
     const int64_t col0 = static_cast<int64_t>(n_blk) * kBN;
-    if constexpr (kMode != kBlockFp8) {
-      store_w8a8_m64n128<DT>(acc, row0, col0, p);
+    if constexpr (kMoe == kMoeSwiGLU) {
+      const int64_t rg = static_cast<int64_t>(row0) + c * 64, cg = static_cast<int64_t>(n_blk) * (kBN / 2);
+      scale_moe_w8a8<true>(acc, rg, cg, p, moe.s_w[2 * e], moe.s_w[2 * e + 1]);
+      store_swiglu_m64n64<DT>(acc, rg, cg, row_end, p.N, p.out);
+    } else if constexpr (kMoe == kMoeDown) {
+      const int64_t rg = static_cast<int64_t>(row0) + c * 64;
+      scale_moe_w8a8<false>(acc, rg, col0, p, moe.s_w[e], nullptr);
+      store_routed_m64n128<DT>(acc, rg, col0, row_end, p.N, p.N, p.out, moe.w_route);
+    } else if constexpr (kMode != kBlockFp8) {
+      store_w8a8_m64n128<DT>(acc, r0, col0, p);
     } else if constexpr (DT == LLMC_F32) {
-      store_f32_m64n128(acc, row0, col0, p.M, p.N, p.N, static_cast<float*>(p.out));
+      store_f32_m64n128(acc, r0, col0, p.M, p.N, p.N, static_cast<float*>(p.out));
     } else if (p.bias == nullptr) {
-      store_linear_m64n128<LLMC_BF16>(acc, row0, col0, p.M, p.N, p.N, nullptr, p.out);
+      store_linear_m64n128<LLMC_BF16>(acc, r0, col0, p.M, p.N, p.N, nullptr, p.out);
     } else {
       store_bf16_bias_m64n128(acc, r_lo, col0, p);
     }
@@ -317,7 +413,7 @@ int launch_gemm_8bit(const void* a, const void* b, int64_t M, int64_t N, int64_t
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   return launch_persistent(dt == LLMC_BF16 ? gemm_8bit_kernel<kMode, LLMC_BF16>
                                            : gemm_8bit_kernel<kMode, kOtherDt>,
-                           p.num_tiles, kThreads, kSmemBytes, st, tmA, tmB, p);
+                           p.num_tiles, kThreads, kSmemBytes, st, tmA, tmB, p, static_cast<const void*>(nullptr));
 }
 
 template <bool kFp8>
@@ -347,6 +443,84 @@ int gemm_w8a8(const char* what, const void* x, const float* s_x, int64_t s_x_str
   p.bias = bias; p.out = y;
   const int kb_total = static_cast<int>((K + kBK - 1) / kBK);   // TMA zero-fills the K tail
   return launch_gemm_8bit<kFp8 ? kW8A8Fp8 : kW8A8Int8>(x, w, M, N, K, kb_total, dtype, p, stream);
+}
+
+// Checks and launches the grouped W8A8 GEMM of kMoe over `rows` quantised rows a [rows, K] into
+// out [rows, N]: N = inter (the width of w1 / w3 and of act) for gate/up, the hidden size for down.
+// w_b / s_b are w3's (gate/up only).  Every refusal happens before any CUDA call.
+template <int kMoe>
+int moe_w8a8(const char* what, const void* a, const float* s_x, int fp8, const void* const* w_a,
+             const void* const* w_b, const float* const* s_a, const float* const* s_b, int64_t s_w_stride,
+             const int32_t* offsets, const void* w_route, void* out, int64_t rows, int64_t N, int64_t K,
+             int64_t E, int dtype, void* stream) {
+  constexpr bool kSwiGLU = kMoe == kMoeSwiGLU;
+  LLMC_CHECK_ARG(E >= 1 && E <= LLMC_MOE_MAX_EXPERTS, "%s: %lld experts outside 1..%d", what, (long long)E,
+                 LLMC_MOE_MAX_EXPERTS);
+  LLMC_CHECK_ARG(rows >= 0 && N > 0 && K > 0, "%s: bad shape rows=%lld N=%lld K=%lld", what, (long long)rows,
+                 (long long)N, (long long)K);
+  LLMC_CHECK_ARG(K % 16 == 0, "%s: K=%lld must be a multiple of 16", what, (long long)K);
+  if (kSwiGLU)
+    LLMC_CHECK_ARG(N % 64 == 0, "%s: inter=%lld must be a multiple of 64", what, (long long)N);
+  else
+    LLMC_CHECK_ARG(N % 8 == 0, "%s: N=%lld must be a multiple of 8", what, (long long)N);
+  LLMC_CHECK_ARG(fp8 || K <= kMaxKInt8, "%s: K=%lld > %lld overflows the int32 sum", what, (long long)K,
+                 (long long)kMaxKInt8);
+  LLMC_CHECK_ARG(s_w_stride == 0 || s_w_stride == 1, "%s: s_w_stride %lld must be 0 or 1", what,
+                 (long long)s_w_stride);
+  LLMC_CHECK_ARG(dtype == LLMC_BF16 || dtype == LLMC_F16, "%s: dtype %d must be bf16 or fp16", what, dtype);
+  LLMC_CHECK_ARG(rows < (1ll << 31) - kBM, "%s: rows=%lld too large", what, (long long)rows);
+  if (rows == 0) return LLMC_OK;
+  LLMC_CHECK_ARG(a && s_x && out && offsets && w_a && s_a && (!kSwiGLU || (w_b && s_b)) && (kSwiGLU || w_route),
+                 "%s: null pointer", what);
+  for (int64_t e = 0; e < E; ++e)
+    LLMC_CHECK_ARG(w_a[e] && s_a[e] && (!kSwiGLU || (w_b[e] && s_b[e])),
+                   "%s: null codes or scales of expert %lld", what, (long long)e);
+  if (!aligned16(a) || !aligned16(out)) {
+    set_last_error("%s: activation and output pointers must be 16-byte aligned", what);
+    return LLMC_EALIGN;
+  }
+  for (int64_t e = 0; e < E; ++e) {
+    if (!aligned16(w_a[e]) || (kSwiGLU && !aligned16(w_b[e]))) {
+      set_last_error("%s: codes of expert %lld not 16-byte aligned", what, (long long)e);
+      return LLMC_EALIGN;
+    }
+  }
+  const int n_tiles = static_cast<int>(kSwiGLU ? N / (kBN / 2) : (N + kBN - 1) / kBN);
+  const int64_t units = ((rows + kBM - 1) / kBM + E) * n_tiles;
+  LLMC_CHECK_ARG(units < (1ll << 31), "%s: too many tiles", what);
+
+  CUtensorMap tmA;
+  if (int rc = encode_tmap_2d(&tmA, a, CU_TENSOR_MAP_DATA_TYPE_UINT8, 1, rows, K, K, kBM, kBK,
+                              CU_TENSOR_MAP_SWIZZLE_128B))
+    return rc;
+  MoeW8A8Operands g{};
+  constexpr uint32_t box_rows = kSwiGLU ? kBN / 2 : kBN;
+  for (int64_t e = 0; e < E; ++e) {
+    for (int h = 0; h < (kSwiGLU ? 2 : 1); ++h) {
+      const int i = static_cast<int>(kSwiGLU ? 2 * e + h : e);
+      if (int rc = encode_tmap_2d(&g.tmB[i], h ? w_b[e] : w_a[e], CU_TENSOR_MAP_DATA_TYPE_UINT8, 1, N, K, K,
+                                  box_rows, kBK, CU_TENSOR_MAP_SWIZZLE_128B))
+        return rc;
+      g.s_w[i] = h ? s_b[e] : s_a[e];
+    }
+  }
+  g.offsets = offsets;
+  g.w_route = w_route;
+  g.E = static_cast<int>(E);
+  W8A8Params p{};
+  p.s_x = s_x; p.s_x_stride = 1; p.s_w_stride = s_w_stride;
+  p.out = out;
+  p.M = rows; p.N = N;
+  p.kb_total = static_cast<int>((K + kBK - 1) / kBK);   // TMA zero-fills the K tail
+  p.n_tiles = n_tiles;
+  p.num_tiles = static_cast<int>(units);
+  p.gn = l2_group_width(static_cast<int64_t>(kBN) * K, n_tiles);   // one n-tile's weight bytes
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  auto kernel = fp8 ? (dtype == LLMC_BF16 ? gemm_8bit_kernel<kW8A8Fp8, LLMC_BF16, kMoe>
+                                          : gemm_8bit_kernel<kW8A8Fp8, LLMC_F16, kMoe>)
+                    : (dtype == LLMC_BF16 ? gemm_8bit_kernel<kW8A8Int8, LLMC_BF16, kMoe>
+                                          : gemm_8bit_kernel<kW8A8Int8, LLMC_F16, kMoe>);
+  return launch_persistent(kernel, p.num_tiles, kThreads, kSmemBytes, st, tmA, CUtensorMap{}, p, g);
 }
 
 }  // namespace
@@ -393,4 +567,21 @@ extern "C" int llmc_gemm_w8a8_fp8(const void* x, const float* s_x, int64_t s_x_s
                                   int64_t N, int64_t K, int dtype, void* stream) {
   return gemm_w8a8<true>("gemm_w8a8_fp8", x, s_x, s_x_stride, w, s_w, s_w_stride, bias, y, M, N, K, dtype,
                          stream);
+}
+
+extern "C" int llmc_moe_gemm_w8a8_swiglu(const void* xq, const float* s_x, int fp8, const void* const* w1,
+                                         const void* const* w3, const float* const* s_w1,
+                                         const float* const* s_w3, int64_t s_w_stride, const int32_t* offsets,
+                                         void* act, int64_t rows, int64_t inter, int64_t K, int64_t n_experts,
+                                         int dtype, void* stream) {
+  return moe_w8a8<kMoeSwiGLU>("moe_gemm_w8a8_swiglu", xq, s_x, fp8, w1, w3, s_w1, s_w3, s_w_stride, offsets,
+                              nullptr, act, rows, inter, K, n_experts, dtype, stream);
+}
+
+extern "C" int llmc_moe_gemm_w8a8_down(const void* actq, const float* s_x, int fp8, const void* const* w2,
+                                       const float* const* s_w2, int64_t s_w_stride, const int32_t* offsets,
+                                       const void* w_route, void* y, int64_t rows, int64_t N, int64_t inter,
+                                       int64_t n_experts, int dtype, void* stream) {
+  return moe_w8a8<kMoeDown>("moe_gemm_w8a8_down", actq, s_x, fp8, w2, nullptr, s_w2, nullptr, s_w_stride,
+                            offsets, w_route, y, rows, N, inter, n_experts, dtype, stream);
 }

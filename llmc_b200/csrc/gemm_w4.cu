@@ -318,30 +318,6 @@ __device__ __forceinline__ void next_outlier(const int32_t* cols, int& ocur, int
   oc = ocur < oend ? __ldg(cols + ocur) : INT_MAX;
 }
 
-// The grouped gate/up epilogue: acc holds gate columns 0..63 and up columns 64..127 of the tile, so
-// gate column d and up column d of a row are fragments j and j + 8 of one thread (layout at
-// tc::wgmma_m64n128k16_bf16).  act[row][col0 + d] = silu_mul_f32(rT(gate), rT(up)), rounded, for
-// the rows below row_end (the expert's segment); ld even.
-template <int DT>
-__device__ __forceinline__ void store_swiglu_m64n64(const float (&acc)[64], int64_t row0, int64_t col0,
-                                                    int64_t row_end, int64_t ld, void* out) {
-  const int tid = threadIdx.x & 127, lane = threadIdx.x & 31;
-#pragma unroll
-  for (int i = 0; i < 2; ++i) {
-    const int64_t row = row0 + (tid >> 5) * 16 + (lane >> 2) + 8 * i;
-    if (row >= row_end) continue;
-    uint16_t* o = static_cast<uint16_t*>(out) + row * ld + col0 + 2 * (lane & 3);
-#pragma unroll
-    for (int j = 0; j < 8; ++j) {
-      float v[2];
-#pragma unroll
-      for (int c = 0; c < 2; ++c)
-        v[c] = silu_mul_f32<DT, true>(acc[4 * j + 2 * i + c], acc[4 * (j + 8) + 2 * i + c]);
-      *reinterpret_cast<uint32_t*>(o + 8 * j) = pack_pair<DT>(v[0], v[1]);
-    }
-  }
-}
-
 // The last kernel argument: the grouped operands in grouped mode; in plain mode an unused null
 // pointer.  A pointer leaves the plain instantiations' code as it was without the argument (an
 // empty struct, or moving the body into a __device__ function the kernel calls, does not).

@@ -157,6 +157,28 @@ def packed_forward_operands(layer, dtype):
     return None
 
 
+W8A8Operands = namedtuple('W8A8Operands', 'w s_w aq input_scale act_cfg')
+W8A8Operands.__doc__ = """What a W8A8 export's forward hands to llmc_gemm_w8a8_*: codes w [N, K] (int8, or e4m3 with
+fp8_weight's recovery), weight scales s_w fp32 (N values, or one), the activation quantizer aq, the
+static input_scale (None: per-token dynamic) and the act config they come from."""
+
+
+def w8a8_forward_operands(layer):
+    """The operands of `layer`'s forward when that forward is exactly linear_forward_w8a8 and nothing
+    else, else None: a VllmRealQuantLinear W8A8 export it runs (w8a8_unsupported() is None) without a
+    bias or hooks.  The device is the caller's to check."""
+    if (not isinstance(layer, VllmRealQuantLinear) or layer._forward_hooks or layer._forward_pre_hooks
+            or layer.bias is not None or layer.w8a8_unsupported() is not None):
+        return None
+    try:
+        w = layer.weight if layer.weight.dtype == torch.int8 else layer.fp8_weight()
+    except NotImplementedError:                   # off the e4m3 grid: the forward raises it
+        return None
+    static = bool(_cfg_get(layer.act_cfg, 'static', False))
+    return W8A8Operands(w.contiguous(), layer.weight_scale.reshape(-1).float().contiguous(),
+                        layer.activation_quantizer(), layer.input_scale if static else None, layer.act_cfg)
+
+
 def linear_residual(layer, x, res, out):
     """out = res + layer(x) (block_ops.add), out may be res: in the GEMM's epilogue when the layer
     has a dense forward weight, else the layer's forward and block_ops.add."""
@@ -197,14 +219,17 @@ def moe_forward(x, sel, w, experts):
     the grouped gate/up GEMM with SiLU-mul in its epilogue, the grouped down GEMM that scales each
     row by its routing weight, and the combine.  x [T, H] and w [T, k] of a 16-bit dtype, sel [T, k]
     int64, experts = one (w1, w3, w2) triple per expert (at most MOE_MAX_EXPERTS): dense weights,
-    or PackedOperands of one form (packed_forward_operands; the grouped dequant GEMMs of
-    csrc/gemm_w4.cu).  Bit for bit the eager loop (MixtralSparseMoe.expert_loop), with no host
-    sync."""
+    PackedOperands of one form (packed_forward_operands; the grouped dequant GEMMs of
+    csrc/gemm_w4.cu) or W8A8Operands of one form (w8a8_forward_operands; the grouped W8A8 GEMMs of
+    csrc/gemm_8bit.cu, each fed by one activation-quantiser pass).  Bit for bit the eager loop
+    (MixtralSparseMoe.expert_loop), with no host sync."""
     require_cuda(x, sel, w)
     T, K = x.shape
     k, E = sel.shape[1], len(experts)
     packed = isinstance(experts[0][0], PackedOperands)
+    w8a8 = isinstance(experts[0][0], W8A8Operands)
     inter, N = ((experts[0][0].wq.shape[0], experts[0][2].wq.shape[0]) if packed
+                else (experts[0][0].w.shape[0], experts[0][2].w.shape[0]) if w8a8
                 else (experts[0][0].shape[0], experts[0][2].shape[0]))
     assert E <= MOE_MAX_EXPERTS and w.dtype == x.dtype
     perm, offsets, rows = moe_routing(sel, E)
@@ -217,6 +242,9 @@ def moe_forward(x, sel, w, experts):
     dt, st = dtype_enum(x.dtype), stream_ptr(x.device)
     if packed:
         _moe_packed_gemms(xp, experts, offsets, w_route, act, y, M, inter, N, K, E, dt, st)
+    elif w8a8:
+        _moe_w8a8_gemms(xp, experts, sel.reshape(-1).index_select(0, perm), offsets, w_route, act, y, M, inter,
+                        N, K, E, dt, st)
     else:
         ws = [[t.contiguous() for t in e] for e in experts]
         w1, w3, w2 = ((ctypes.c_void_p * E)(*[e[i].data_ptr() for e in ws]) for i in range(3))
@@ -274,6 +302,39 @@ def _moe_packed_gemms(xp, experts, offsets, w_route, act, y, M, inter, N, K, E, 
                     nbytes=2.0 * (M * inter + M * N + M) + E * weight_bytes(g2)):
         call('llmc_moe_gemm_packed_down', ptr(act), bits, arr(2, 'wq'), arr(2, 'scales'), arr(2, 'zeros'),
              arr(2, 'g_idx'), qd2, grp2, ng2, ptr(offsets), ptr(w_route), ptr(y), M, N, inter, E, dt, st)
+
+
+def _moe_w8a8_gemms(xp, experts, expert_of_row, offsets, w_route, act, y, M, inter, N, K, E, dt, st):
+    """moe_forward's two GEMMs on W8A8Operands experts: xp quantised once by w1's activation quantizer,
+    llmc_moe_gemm_w8a8_swiglu, act quantised once by w2's, llmc_moe_gemm_w8a8_down.  Per-token dynamic
+    activations take the quantiser's per-token pass over all rows (each row's codes and scale depend
+    on that row alone); static ones its per-tensor pass with one scale per row, the input_scale of the
+    row's expert (expert_of_row [M]: the expert of each of xp's rows), gathered on the device."""
+    if M == 0:
+        return
+    o1 = experts[0][0]
+    fp8 = int(o1.w.dtype == torch.float8_e4m3fn)
+    stride = int(o1.s_w.numel() != 1)
+
+    def arr(i, field):
+        return (ctypes.c_void_p * E)(*[getattr(e[i], field).data_ptr() for e in experts])
+
+    def quantise(a, i):
+        if experts[0][i].input_scale is None:
+            return experts[0][i].aq.real_quant_act(a)
+        table = torch.cat([e[i].input_scale.reshape(-1) for e in experts])
+        return experts[0][i].aq.real_quant_act(a, table.index_select(0, expert_of_row))
+
+    xq, sx = quantise(xp, 0)
+    with TIMER.span('moe_gemm_w8a8_swiglu', flops=2.0 * M * 2 * inter * K,
+                    nbytes=float(M * K + E * 2 * inter * K) + 2.0 * M * inter):
+        call('llmc_moe_gemm_w8a8_swiglu', ptr(xq), ptr(sx), fp8, arr(0, 'w'), arr(1, 'w'), arr(0, 's_w'),
+             arr(1, 's_w'), stride, ptr(offsets), ptr(act), M, inter, K, E, dt, st)
+    aq, sa = quantise(act, 2)
+    with TIMER.span('moe_gemm_w8a8_down', flops=2.0 * M * N * inter,
+                    nbytes=float(M * inter + E * N * inter) + 2.0 * (M * N + M)):
+        call('llmc_moe_gemm_w8a8_down', ptr(aq), ptr(sa), fp8, arr(2, 'w'), arr(2, 's_w'), stride, ptr(offsets),
+             ptr(w_route), ptr(y), M, N, inter, E, dt, st)
 
 
 def linear_forward_w4(x, wq, scales, zeros, group, bias=None, bits=4, qparams_t=False, g_idx=None):

@@ -595,7 +595,9 @@ class IntegerQuantizer(BaseQuantizer):
           input_scale None: per-token dynamic, fake_quant_act_dynamic's llmc_quant_dynamic pass with
             codes out instead of QDQ; its `dtype` scales widened (exactly) to fp32.
           input_scale given: per-tensor static, fake_quant_act_static's pass for its 0-dim fp32 scale
-            (x / s in fp32 rounded to the activation dtype, torch's scalar-operand path)."""
+            (x / s in fp32 rounded to the activation dtype, torch's scalar-operand path).  One value,
+            or one per row (a grouped MoE layer's rows each under their expert's input_scale): the
+            same pass and arithmetic, row r under scale r; -> scales fp32 [1] or [rows]."""
         if self.bit != 8 or not self.sym or self.qmin != -128 or self.qmax != 127:
             raise NotImplementedError('W8A8 real-quant activations are symmetric int8 [-128, 127] '
                                       f'(got bit={self.bit} sym={self.sym} range=[{self.qmin}, {self.qmax}])')
@@ -607,12 +609,12 @@ class IntegerQuantizer(BaseQuantizer):
                 raise NotImplementedError(f'dynamic W8A8 activations are per_token, not {self.granularity}')
             scales, _ = self._dynamic(t2d, OUT_CODES_I8, out=codes)
             return codes, scales.reshape(-1).float()
-        if self.granularity != 'per_tensor' or input_scale.numel() != 1:
-            raise NotImplementedError('static W8A8 activations take one per_tensor input_scale')
-        s = input_scale.reshape(1).to(device=t2d.device, dtype=torch.float32).contiguous()
+        if self.granularity != 'per_tensor' or input_scale.numel() not in (1, t2d.shape[0]):
+            raise NotImplementedError('static W8A8 activations take one per_tensor input_scale (or one per row)')
+        s = input_scale.reshape(-1).to(device=t2d.device, dtype=torch.float32).contiguous()
         rd = dtype_enum(t2d.dtype) if t2d.dtype != torch.float32 else -1
-        self._static(t2d, s, None, self.qmax, self.qmin, OUT_CODES_I8, codes, t2d.dtype, 0, t2d.shape[1],
-                     round_dtype=rd)
+        self._static(t2d, s, None, self.qmax, self.qmin, OUT_CODES_I8, codes, t2d.dtype, int(s.numel() != 1),
+                     t2d.shape[1], round_dtype=rd)
         return codes, s
 
     # -- real quant -------------------------------------------------------------------------------

@@ -197,7 +197,9 @@ class FloatQuantizer(BaseQuantizer):
         scale the bytes were quantised with (quant.py:1062).  -> (e4m3 [rows, K], fp32 [rows] or [1]).
           input_scale None: per-token dynamic (fake_quant_act_dynamic).
           input_scale given: per-tensor static (fake_quant_act_static on its 0-dim scale); the caller's
-            tensor is not modified."""
+            tensor is not modified.  One value, or one per row (a grouped MoE layer's rows each under
+            their expert's input_scale): the same pass and arithmetic, row r under scale r; -> scales
+            fp32 [1] or [rows]."""
         if self.bit != 'e4m3':
             raise NotImplementedError(f'W8A8 real-quant FP8 activations are e4m3, not {self.bit}')
         t2d = act.reshape(-1, act.shape[-1])
@@ -207,11 +209,11 @@ class FloatQuantizer(BaseQuantizer):
                 raise NotImplementedError(f'dynamic FP8 activations are per_token, not {self.granularity}')
             out, scales = self._dynamic(t2d, 2)
             return out, scales.reshape(-1).float()
-        if self.granularity != 'per_tensor' or input_scale.numel() != 1:
-            raise NotImplementedError('static FP8 activations take one per_tensor input_scale')
-        s = input_scale.reshape(1).to(device=t2d.device, dtype=torch.float32, copy=True)
+        if self.granularity != 'per_tensor' or input_scale.numel() not in (1, t2d.shape[0]):
+            raise NotImplementedError('static FP8 activations take one per_tensor input_scale (or one per row)')
+        s = input_scale.reshape(-1).to(device=t2d.device, dtype=torch.float32, copy=True)
         _zeros_to_one(s)
-        return self._run(t2d, t2d.shape[1], 0, s, 2, 0, 1), s
+        return self._run(t2d, t2d.shape[1], 0, s, 2, int(s.numel() != 1), 1), s
 
     def _qshape(self, weight, scales):
         if self.granularity == 'per_tensor':

@@ -18,7 +18,7 @@ import torch.nn.functional as F
 from ._lib import MOE_MAX_EXPERTS
 from .module_utils import (_LLMC_LINEAR_TYPES_, _TRANSFORMERS_LINEAR_TYPES_, dense_forward_weight,
                            gemm_rope_qkv, gemm_swiglu, interleave_gate_up, linear_forward,
-                           moe_forward, packed_forward_operands)
+                           moe_forward, packed_forward_operands, w8a8_forward_operands)
 
 SHAPES = {
     # name: hidden, intermediate, layers, heads, kv_heads, vocab, kind, dtype
@@ -221,6 +221,23 @@ class MixtralExpert(nn.Module):
         return self.w2(F.silu(self.w1(x)) * self.w3(x))
 
 
+# the largest K of llmc_gemm_w8a8_i8 (csrc/gemm_8bit.cu kMaxKInt8): its int32 sum is exact below it
+W8A8_MAX_K_INT8 = ((1 << 17) - 1) // 16 * 16
+
+
+def _same_input_scale(a, b):
+    """Whether the static input scales of linears a and b hold one value.  Read once per pair of
+    buffer versions and cached on a, keyed by both buffers' (data_ptr, _version) as fp8_weight keys
+    its codes, so that later forwards do not synchronise."""
+    sa, sb = a.input_scale, b.input_scale
+    key = (sa.data_ptr(), sa._version, sb.data_ptr(), sb._version)
+    cached = getattr(a, '_same_input_scale', None)
+    if cached is None or cached[0] != key:
+        cached = (key, sa.numel() == sb.numel() and torch.equal(sa.reshape(-1).float(), sb.reshape(-1).float()))
+        a._same_input_scale = cached
+    return cached[1]
+
+
 class MixtralSparseMoe(nn.Module):
     """Per-expert nn.Linear layout the reference's wrapper expects (models/mixtral.py:43-86:
     block_sparse_moe.gate / experts[i].w1|w2|w3); the installed transformers 5.x fuses the experts,
@@ -318,6 +335,43 @@ class MixtralSparseMoe(nn.Module):
             ops.append(triple)
         return ops
 
+    def grouped_w8a8_operands(self, x):
+        """One (w1, w3, w2) triple of module_utils.W8A8Operands per expert when moe_forward on them
+        computes exactly what expert_loop computes on x, else None: every expert a plain MixtralExpert
+        without hooks, every linear w8a8_forward_operands' (a W8A8 export without bias or hooks), all
+        of one form (int8 or e4m3 codes, dynamic or static activations of one act config, per-channel
+        or per-tensor weight scales), the shapes the grouped W8A8 GEMMs take (hidden and inter
+        multiples of 16, inter of 64), at most MOE_MAX_EXPERTS.  Static activations also need
+        w1.input_scale == w3.input_scale in every expert: the gate/up launch quantises each row once,
+        where the loop quantises it for w1 and for w3 apart."""
+        if (not x.is_cuda or x.dtype not in (torch.bfloat16, torch.float16)
+                or len(self.experts) > MOE_MAX_EXPERTS or x.shape[1] % 16):
+            return None
+        hidden = x.shape[1]
+        ops, form = [], None
+        for ex in self.experts:
+            if type(ex) is not MixtralExpert or ex._forward_hooks or ex._forward_pre_hooks:
+                return None
+            triple = tuple(w8a8_forward_operands(m) for m in (ex.w1, ex.w3, ex.w2))
+            if any(o is None for o in triple):
+                return None
+            inter = triple[0].w.shape[0]
+            if inter % 64 or (triple[0].w.dtype == torch.int8 and max(hidden, inter) > W8A8_MAX_K_INT8):
+                return None
+            for o, (n, k) in zip(triple, ((inter, hidden), (inter, hidden), (hidden, inter))):
+                if (tuple(o.w.shape) != (n, k) or o.w.data_ptr() % 16 or o.s_w.numel() not in (1, n)
+                        or not (o.w.is_cuda and o.s_w.is_cuda)
+                        or (o.input_scale is not None and not o.input_scale.is_cuda)):
+                    return None
+            f = [(o.w.dtype, o.input_scale is None, o.s_w.numel() == 1, o.act_cfg) for o in triple]
+            if f[0] != f[1] or f[0] != f[2] or (form is not None and f[0] != form):
+                return None
+            form = f[0]
+            if triple[0].input_scale is not None and not _same_input_scale(ex.w1, ex.w3):
+                return None
+            ops.append(triple)
+        return ops
+
     def forward(self, hidden_states):
         B, S, H = hidden_states.shape
         x = hidden_states.reshape(-1, H)
@@ -325,6 +379,8 @@ class MixtralSparseMoe(nn.Module):
         experts = self.grouped_weights(x)
         if experts is None:
             experts = self.grouped_packed_operands(x)
+        if experts is None:
+            experts = self.grouped_w8a8_operands(x)
         out = self.expert_loop(x, sel, w) if experts is None else moe_forward(x, sel, w, experts)
         return out.reshape(B, S, H)
 

@@ -2,7 +2,7 @@
 per-expert loop (MixtralSparseMoe.expert_loop) it replaces.
 
     python scripts/bench_moe.py [--reps 10] [--tokens 2048 65536] [--awq-samples 128] [--awq-rounds 3]
-                                [--packed] [--ppl-rounds 3] [--out DIR]
+                                [--packed] [--ppl-rounds 3] [--w8a8] [--out DIR]
 
 1. One MoE layer (hidden 4096, inter 14336, 8 experts, top-2, bf16) at 2048 tokens (one GPTQ
    calibration forward at batch size 1) and 65536 tokens (the AWQ inspect batch, 128 x 512): the
@@ -21,6 +21,12 @@ g128 with bf16 qparams, W4 g128 act-order (fp32 qparams, a g_idx per linear) and
 timed as in 1.; then the fake-quant perplexity of a one-block Mixtral-8x7B-shaped model after an RTN
 W4 g128 deploy (8 x 2048 tokens), grouped then loop for ppl_rounds alternated rounds on a host
 clock that ends in a device synchronise, with equal perplexities checked.
+With --w8a8, instead: the same layer with W8A8 experts (exported VllmRealQuantLinear int8 / e4m3
+linears) on the grouped W8A8 GEMMs (module_utils.W8A8Operands, csrc/gemm_8bit.cu) against the loop
+over their real-quant forwards, for e4m3 per-tensor weights with static per-tensor activations
+(configs/rtn_fp8_static_mixtral.yml), e4m3 per-channel with per-token dynamic activations and int8
+per-channel with per-token dynamic activations (random codes and scales), at each of `tokens`, timed
+as in 1.
 Prints, and writes to DIR/bench_moe.json, one JSON object with the card name and power limit.
 """
 import argparse
@@ -64,6 +70,29 @@ def timed(fn):
     return a.elapsed_time(b)
 
 
+def compare_and_time(res, key, moe, hs, flops, reps):
+    """The module forward (grouped) and loop_forward on hs: the same bits first, then after warm-up
+    `reps` alternated rounds between CUDA events; records the medians, the TFLOP/s of `flops` and the
+    speed-up under `key`."""
+    grouped, loop = moe(hs), loop_forward(moe, hs)
+    assert torch.equal(grouped.view(torch.int16), loop.view(torch.int16)), key
+    del grouped, loop
+    runs = {'grouped': lambda: moe(hs), 'loop': lambda: loop_forward(moe, hs)}
+    for fn in runs.values():
+        for _ in range(3):
+            fn()
+    torch.cuda.synchronize()
+    times = {n: [] for n in runs}
+    for _ in range(reps):
+        for n, fn in runs.items():
+            times[n].append(timed(fn))
+    med = {n: round(statistics.median(v), 3) for n, v in times.items()}
+    res['layer_ms'][key] = med
+    res['layer_tflops'][key] = {n: round(flops / (v * 1e-3) / 1e12, 1) for n, v in med.items()}
+    res['layer_speedup'][key] = round(med['loop'] / med['grouped'], 3)
+    print(key, med, res['layer_tflops'][key], flush=True)
+
+
 def bench_layer(res, tokens, reps):
     s = synth.SHAPES['mixtral-8x7b']
     H, I, E, k = s['hidden'], s['inter'], s['experts'], s['top_k']
@@ -76,25 +105,7 @@ def bench_layer(res, tokens, reps):
     for T in tokens:
         hs = torch.randn(1, T, H, device='cuda', generator=g).to(torch.bfloat16)
         assert moe.grouped_weights(hs.view(T, H)) is not None
-        grouped, loop = moe(hs), loop_forward(moe, hs)
-        assert torch.equal(grouped.view(torch.int16), loop.view(torch.int16)), T
-        del grouped, loop
-        runs = {'grouped': lambda: moe(hs), 'loop': lambda: loop_forward(moe, hs)}
-        for fn in runs.values():
-            for _ in range(3):
-                fn()
-        torch.cuda.synchronize()
-        times = {n: [] for n in runs}
-        for _ in range(reps):
-            for n, fn in runs.items():
-                times[n].append(timed(fn))
-        med = {n: round(statistics.median(v), 3) for n, v in times.items()}
-        flops = 2.0 * T * k * 3 * H * I
-        key = f'moe_layer[T={T}]'
-        res['layer_ms'][key] = med
-        res['layer_tflops'][key] = {n: round(flops / (v * 1e-3) / 1e12, 1) for n, v in med.items()}
-        res['layer_speedup'][key] = round(med['loop'] / med['grouped'], 3)
-        print(key, med, res['layer_tflops'][key], flush=True)
+        compare_and_time(res, f'moe_layer[T={T}]', moe, hs, 2.0 * T * k * 3 * H * I, reps)
         del hs
         torch.cuda.empty_cache()
     del moe
@@ -138,25 +149,61 @@ def bench_packed_layer(res, tokens, reps):
         for T in tokens:
             hs = torch.randn(1, T, H, device='cuda', generator=g).to(torch.bfloat16)
             assert moe.grouped_packed_operands(hs.view(T, H)) is not None
-            grouped, loop = moe(hs), loop_forward(moe, hs)
-            assert torch.equal(grouped.view(torch.int16), loop.view(torch.int16)), (form, T)
-            del grouped, loop
-            runs = {'grouped': lambda: moe(hs), 'loop': lambda: loop_forward(moe, hs)}
-            for fn in runs.values():
-                for _ in range(3):
-                    fn()
-            torch.cuda.synchronize()
-            times = {n: [] for n in runs}
-            for _ in range(reps):
-                for n, fn in runs.items():
-                    times[n].append(timed(fn))
-            med = {n: round(statistics.median(v), 3) for n, v in times.items()}
-            flops = 2.0 * T * k * 3 * H * I
-            key = f'moe_layer[{form}, T={T}]'
-            res['layer_ms'][key] = med
-            res['layer_tflops'][key] = {n: round(flops / (v * 1e-3) / 1e12, 1) for n, v in med.items()}
-            res['layer_speedup'][key] = round(med['loop'] / med['grouped'], 3)
-            print(key, med, res['layer_tflops'][key], flush=True)
+            compare_and_time(res, f'moe_layer[{form}, T={T}]', moe, hs, 2.0 * T * k * 3 * H * I, reps)
+            del hs
+            torch.cuda.empty_cache()
+        del moe
+        torch.cuda.empty_cache()
+
+
+# form: (codes, static input scales, per-channel weight scales)
+W8A8_FORMS = {'e4m3_tensor_static': ('e4m3', True, False), 'e4m3_channel_dynamic': ('e4m3', False, True),
+              'int8_channel_dynamic': ('int8', False, True)}
+
+
+def w8a8_moe(form, g):
+    """The Mixtral-8x7B MoE layer (bf16) with every expert linear a W8A8 export (VllmRealQuantLinear) of
+    `form`, random codes and scales; static input scales differ per expert, w1's and w3's alike."""
+    from llmc_b200.module_utils import VllmRealQuantLinear
+    kind, static, per_channel = W8A8_FORMS[form]
+    act = ({'bit': 8, 'symmetric': True} if kind == 'int8' else
+           {'quant_type': 'float-quant', 'bit': 'e4m3', 'symmetric': True, 'use_qtorch': True})
+    act.update({'granularity': 'per_tensor', 'static': True, 'calib_algo': 'static_minmax'} if static
+               else {'granularity': 'per_token'})
+    s = synth.SHAPES['mixtral-8x7b']
+    with torch.device('meta'):
+        moe = MixtralSparseMoe(s['hidden'], s['inter'], s['experts'], s['top_k'])
+    moe.gate = moe.gate.to_empty(device='cuda').to(torch.bfloat16)
+    moe.gate.weight.data.normal_(0, 0.02, generator=g)
+    for ex in moe.experts:
+        in_scale = torch.rand(1, generator=g, device='cuda') * 0.01 + 0.005
+        for n in ('w1', 'w3', 'w2'):
+            lin = getattr(ex, n)
+            N, K = lin.out_features, lin.in_features
+            if kind == 'int8':
+                w = torch.randint(-127, 128, (N, K), generator=g, device='cuda', dtype=torch.int8)
+                sw = torch.rand(N if per_channel else 1, 1, generator=g, device='cuda') * 2e-4 + 5e-5
+            else:
+                w = torch.randn(N, K, generator=g, device='cuda').to(torch.float8_e4m3fn)
+                sw = torch.rand(N if per_channel else 1, 1, generator=g, device='cuda') * 0.01 + 0.002
+            if n == 'w2':
+                in_scale = torch.rand(1, generator=g, device='cuda') * 0.01 + 0.005
+            m = VllmRealQuantLinear(w, None, sw, in_scale.clone() if static else None, False, 'weight_scale')
+            m.in_features, m.out_features, m.act_cfg = K, N, dict(act)
+            setattr(ex, n, m)
+    return moe
+
+
+def bench_w8a8_layer(res, tokens, reps):
+    s = synth.SHAPES['mixtral-8x7b']
+    H, I, k = s['hidden'], s['inter'], s['top_k']
+    g = torch.Generator(device='cuda').manual_seed(0)
+    for form in W8A8_FORMS:
+        moe = w8a8_moe(form, g)
+        for T in tokens:
+            hs = torch.randn(1, T, H, device='cuda', generator=g).to(torch.bfloat16)
+            assert moe.grouped_w8a8_operands(hs.view(T, H)) is not None
+            compare_and_time(res, f'moe_layer[{form}, T={T}]', moe, hs, 2.0 * T * k * 3 * H * I, reps)
             del hs
             torch.cuda.empty_cache()
         del moe
@@ -254,12 +301,16 @@ def main():
     ap.add_argument('--awq-samples', type=int, default=128)
     ap.add_argument('--awq-rounds', type=int, default=3)
     ap.add_argument('--packed', action='store_true')
+    ap.add_argument('--w8a8', action='store_true')
     ap.add_argument('--ppl-rounds', type=int, default=3)
     ap.add_argument('--out', default=None)
     args = ap.parse_args()
     assert torch.cuda.is_available(), 'needs a CUDA device'
     res = {'card': card(), 'reps': args.reps, 'layer_ms': {}, 'layer_tflops': {}, 'layer_speedup': {}}
-    if args.packed:
+    if args.w8a8:
+        with torch.no_grad():
+            bench_w8a8_layer(res, args.tokens, args.reps)
+    elif args.packed:
         res.update(ppl_s={}, ppl_speedup={})
         with torch.no_grad():
             bench_packed_layer(res, args.tokens, args.reps)
