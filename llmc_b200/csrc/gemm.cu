@@ -22,7 +22,7 @@
 //      sparse-MoE layer.  A = the routed rows gathered in expert order, expert e owning rows
 //      [offsets[e], offsets[e+1]); B = expert e's weight through its own tensor map (MoeOperands).
 //      Same main loop, tile and wgmma as the GEMM; only the unit decode, the B loads and the row
-//      bound of the store differ (see decode_moe_unit).
+//      bound of the store differ (see decode_moe_unit and tc::moe_load_b).
 #include "tc.cuh"
 
 namespace llmc {
@@ -70,18 +70,14 @@ enum Epilogue {
   kEpiRopeQkv,    // W = [Wq; Wk; Wv]: q, k, v to three outputs, rope_kernel applied to q and k
   kEpiSwiGLU,     // W = gate / up interleaved in 128-row blocks: act = silu(gate) * up
   kEpiResidual,   // Y = res + X W^T (add_kernel)
-  kEpiRouted,     // Y = rT(rT(X W^T) * w_route[row]): an expert's output times its routing weight
 };
 
 // The grouped operands: one tensor map per expert weight (AWQ rewrites the expert weights between
 // calls, so they cannot be one tensor) and the segment offsets, read from device memory so that the
 // host never learns the routing.  A kernel argument of its own, like EpiParams.
 struct MoeOperands {
-  CUtensorMap tmB[2 * LLMC_MOE_MAX_EXPERTS];   // gate/up: w1 of expert e at 2e, w3 at 2e + 1;
-                                               // down: w2 of expert e at e
-  const int32_t* offsets;                      // [E + 1] row offsets of the expert segments
-  const void* w_route;                         // kEpiRouted: [rows] routing weights (A's row order)
-  int E;
+  CUtensorMap tmB[2 * LLMC_MOE_MAX_EXPERTS];   // one per expert linear (tc::moe_load_b)
+  MoeSegments seg;
 };
 // The whole argument list of the grouped kernel fits the 4 KB kernel-parameter space: that is what
 // caps the number of experts.
@@ -138,8 +134,7 @@ __device__ __forceinline__ bool decode_moe_unit(const GemmParams& p, const MoeOp
   t.kb0 = 0;
   t.kb1 = p.kb_total;
   t.split = 0;
-  return moe_segment_tile<BM>(g.offsets, g.E, u, p.n_tiles_n, p.gn, t.e, t.m_blk, t.n_blk, t.row0,
-                              t.row_end);
+  return moe_segment_tile<BM>(g.seg, u, p.n_tiles_n, p.gn, t.e, t.m_blk, t.n_blk, t.row0, t.row_end);
 }
 
 // ---- fused epilogues: this thread's part of the 64-row half tile (fragment layout at
@@ -255,11 +250,12 @@ __device__ __forceinline__ void store_residual_m64n128(const float (&acc)[64], i
   }
 }
 
-// The kernel body.  Plain mode (wgmma_gemm_kernel): B is tmB.  Grouped mode (wgmma_moe_kernel):
-// tiles come from decode_moe_unit and B from g's map of the tile's expert; for kEpiSwiGLU the
-// 256-row B stage is loaded as two 128-row boxes, w1 rows then w3 rows of the same n-block, which
-// the 128-byte swizzle lays out exactly as one box of interleave_gate_up's weight.
-template <bool kSyrk, bool kBf16, int kEpi, bool kGrouped>
+// The kernel body.  Plain mode (wgmma_gemm_kernel, kMoe == kMoeOff): B is tmB, the epilogue kEpi.
+// Grouped mode (wgmma_moe_kernel): tiles come from decode_moe_unit and B from g's maps of the
+// tile's expert; for kMoeSwiGLU the 256-row B stage is two 128-row boxes, w1 rows then w3 rows of
+// the same n-block, which the 128-byte swizzle lays out exactly as one box of interleave_gate_up's
+// weight, so the epilogue is kEpiSwiGLU's.
+template <bool kSyrk, bool kBf16, int kEpi, int kMoe>
 __device__ __forceinline__ void gemm_body(const CUtensorMap* tmA, const CUtensorMap* tmB,
                                           const GemmParams& p, const EpiParams& e,
                                           const MoeOperands* g) {
@@ -272,8 +268,8 @@ __device__ __forceinline__ void gemm_body(const CUtensorMap* tmA, const CUtensor
 
   if (threadIdx.x == 0) {
     prefetch_tmap(tmA);
-    if constexpr (kGrouped) {
-      for (int i = 0; i < (kEpi == kEpiSwiGLU ? 2 : 1) * g->E; ++i) prefetch_tmap(&g->tmB[i]);
+    if constexpr (kMoe != kMoeOff) {
+      prefetch_moe_tmaps<kMoe>(g->tmB, g->seg);
     } else {
       prefetch_tmap(tmB);
     }
@@ -288,7 +284,7 @@ __device__ __forceinline__ void gemm_body(const CUtensorMap* tmA, const CUtensor
       PipeState<kStages> ps;
       for (int u = blockIdx.x; u < p.num_units; u += gridDim.x) {
         Unit t;
-        if constexpr (kGrouped) {
+        if constexpr (kMoe != kMoeOff) {
           if (!decode_moe_unit(p, *g, u, t)) break;
         } else {
           t = decode_unit<kSyrk>(p, u);
@@ -299,14 +295,9 @@ __device__ __forceinline__ void gemm_body(const CUtensorMap* tmA, const CUtensor
           uint8_t* b_dst = a_dst + kABytes;
           uint64_t* bar = &ring.full[ps.stage];
           ring.expect_tx(ps, kStageBytes);
-          if constexpr (kGrouped) {
+          if constexpr (kMoe != kMoeOff) {
             tma_load_2d(a_dst, tmA, bar, kb * BK, t.row0);
-            if constexpr (kEpi == kEpiSwiGLU) {
-              tma_load_2d(b_dst, &g->tmB[2 * t.e], bar, kb * BK, t.n_blk * (BN / 2));
-              tma_load_2d(b_dst + kBBytes / 2, &g->tmB[2 * t.e + 1], bar, kb * BK, t.n_blk * (BN / 2));
-            } else {
-              tma_load_2d(b_dst, &g->tmB[t.e], bar, kb * BK, t.n_blk * BN);
-            }
+            moe_load_b<kMoe>(b_dst, g->tmB, bar, t.e, kb * BK, t.n_blk, BN, kBBytes / 2);
           } else if constexpr (!kSyrk) {
             tma_load_2d(a_dst, tmA, bar, kb * BK, t.m_blk * BM);
             tma_load_2d(b_dst, tmB, bar, kb * BK, t.n_blk * BN);
@@ -331,7 +322,7 @@ __device__ __forceinline__ void gemm_body(const CUtensorMap* tmA, const CUtensor
   PipeState<kStages> ps;
   for (int u = blockIdx.x; u < p.num_units; u += gridDim.x) {
     Unit t;
-    if constexpr (kGrouped) {
+    if constexpr (kMoe != kMoeOff) {
       if (!decode_moe_unit(p, *g, u, t)) break;
     } else {
       t = decode_unit<kSyrk>(p, u);
@@ -374,16 +365,15 @@ __device__ __forceinline__ void gemm_body(const CUtensorMap* tmA, const CUtensor
 
     // ---- epilogue straight from the accumulator registers ----
     int64_t row0 = static_cast<int64_t>(t.m_blk) * BM + c * 64;
-    if constexpr (kGrouped) row0 = t.row0 + c * 64;
+    if constexpr (kMoe != kMoeOff) row0 = t.row0 + c * 64;
     const int64_t col0 = static_cast<int64_t>(t.n_blk) * BN;
-    if constexpr (kGrouped) {
+    if constexpr (kMoe != kMoeOff) {
       constexpr int DT = kBf16 ? LLMC_BF16 : LLMC_F16;
-      if constexpr (kEpi == kEpiSwiGLU) {
+      if constexpr (kMoe == kMoeSwiGLU) {
         store_swiglu_m64n128<DT>(acc0, acc1, row0, col0 / 2, t.row_end, p.ld_out, p.out);
       } else {
-        static_assert(kEpi == kEpiRouted, "grouped mode: kEpiSwiGLU or kEpiRouted");
-        store_routed_m64n128<DT>(acc0, row0, col0, t.row_end, p.N, p.ld_out, p.out, g->w_route);
-        store_routed_m64n128<DT>(acc1, row0, col0 + 128, t.row_end, p.N, p.ld_out, p.out, g->w_route);
+        store_routed_m64n128<DT>(acc0, row0, col0, t.row_end, p.N, p.ld_out, p.out, g->seg.w_route);
+        store_routed_m64n128<DT>(acc1, row0, col0 + 128, t.row_end, p.N, p.ld_out, p.out, g->seg.w_route);
       }
     } else if constexpr (!kSyrk) {
       constexpr int DT = kBf16 ? LLMC_BF16 : LLMC_F16;
@@ -412,14 +402,14 @@ template <bool kSyrk, bool kBf16, int kEpi = kEpiLinear>
 __global__ void __launch_bounds__(kThreads, 1)
 wgmma_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                   const GemmParams p, const EpiParams e) {
-  gemm_body<kSyrk, kBf16, kEpi, false>(&tmA, &tmB, p, e, nullptr);
+  gemm_body<kSyrk, kBf16, kEpi, kMoeOff>(&tmA, &tmB, p, e, nullptr);
 }
 
-template <bool kBf16, int kEpi>
+template <bool kBf16, int kMoe>
 __global__ void __launch_bounds__(kThreads, 1)
 wgmma_moe_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ MoeOperands g,
                  const GemmParams p) {
-  gemm_body<false, kBf16, kEpi, true>(&tmA, nullptr, p, EpiParams{}, &g);
+  gemm_body<false, kBf16, kEpiLinear, kMoe>(&tmA, nullptr, p, EpiParams{}, &g);
 }
 
 // ---- SYRK finalize: H = a*H + b*sum_s P_s on the upper triangle, mirrored -----------------------
@@ -569,71 +559,39 @@ static int launch_gemm(const void* x, const void* w, int64_t M, int64_t N, int64
                            p.num_units, kThreads, kSmemBytes, st, tmA, tmB, p, e);
 }
 
-// Checks and launches the grouped GEMM of kEpi over `rows` gathered rows of A [rows, K]: n_tiles
-// n-tiles of BN output columns per expert, B = w_a[e] (kEpiRouted: w2 [N, K]) or w_a[e] / w_b[e]
-// (kEpiSwiGLU: w1 / w3 [N / 2, K]).  p.out / p.ld_out are the caller's; p's other fields are
-// filled in here.
-template <int kEpi>
-static int launch_moe(const char* what, const void* a, const void* const* w_a,
-                      const void* const* w_b, const int32_t* offsets, const void* w_route,
-                      int64_t rows, int64_t N, int64_t K, int64_t E, int dtype, GemmParams p,
-                      void* stream) {
-  LLMC_CHECK_ARG(rows >= 0 && N > 0 && K > 0, "%s: bad shape", what);
-  LLMC_CHECK_ARG(E >= 1 && E <= LLMC_MOE_MAX_EXPERTS, "%s: %lld experts outside 1..%d", what,
-                 (long long)E, LLMC_MOE_MAX_EXPERTS);
-  LLMC_CHECK_ARG(rows < (1ll << 31) - BM, "%s: rows=%lld too large", what, (long long)rows);
-  if (rows == 0) return LLMC_OK;
-  LLMC_CHECK_ARG(dtype == LLMC_BF16 || dtype == LLMC_F16, "%s: dtype must be bf16 or fp16", what);
-  LLMC_CHECK_ARG(a && w_a && offsets && p.out && (kEpi != kEpiSwiGLU || w_b) &&
-                 (kEpi != kEpiRouted || w_route), "%s: null pointer", what);
-  for (int64_t e = 0; e < E; ++e)
-    LLMC_CHECK_ARG(w_a[e] && (kEpi != kEpiSwiGLU || w_b[e]), "%s: null weight of expert %lld", what,
-                   (long long)e);
-  if (K % 8 != 0 || !aligned16(a) || !aligned16(p.out)) {
-    set_last_error("%s: K=%lld must be a multiple of 8 and pointers 16-byte aligned", what,
-                   (long long)K);
+// Checks and launches the grouped GEMM over m.rows gathered rows: n-tiles of BN output columns per
+// expert, each expert's B one tensor map (kMoeSwiGLU: BN / 2 rows of w1, then of w3).
+template <int kMoe>
+static int launch_moe(const MoeLaunch<kMoe>& m, void* stream) {
+  int n_tiles, units;
+  if (int rc = m.check_values(BM, BN)) return rc;
+  if (m.K % 8 != 0) {
+    set_last_error("%s: K=%lld must be a multiple of 8", m.what, (long long)m.K);
     return LLMC_EALIGN;
   }
-  for (int64_t e = 0; e < E; ++e) {
-    if (!aligned16(w_a[e]) || (kEpi == kEpiSwiGLU && !aligned16(w_b[e]))) {
-      set_last_error("%s: weight of expert %lld not 16-byte aligned", what, (long long)e);
-      return LLMC_EALIGN;
-    }
-  }
+  if (int rc = m.plan(BM, BN, n_tiles, units)) return rc;
+  if (m.rows == 0) return LLMC_OK;
+  if (int rc = m.check_pointers()) return rc;
   CUtensorMap tmA;
-  if (int rc = encode_tmap_2d(&tmA, a, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, rows, K, K, BM, BK,
+  if (int rc = encode_tmap_2d(&tmA, m.a, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, m.rows, m.K, m.K, BM, BK,
                               CU_TENSOR_MAP_SWIZZLE_128B))
     return rc;
   MoeOperands g{};
-  for (int64_t e = 0; e < E; ++e) {
-    if constexpr (kEpi == kEpiSwiGLU) {
-      for (int h = 0; h < 2; ++h)
-        if (int rc = encode_tmap_2d(&g.tmB[2 * e + h], h ? w_b[e] : w_a[e],
-                                    CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, N / 2, K, K, BN / 2, BK,
-                                    CU_TENSOR_MAP_SWIZZLE_128B))
-          return rc;
-    } else {
-      if (int rc = encode_tmap_2d(&g.tmB[e], w_a[e], CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, N, K, K,
-                                  BN, BK, CU_TENSOR_MAP_SWIZZLE_128B))
-        return rc;
-    }
-  }
-  g.offsets = offsets;
-  g.w_route = w_route;
-  g.E = static_cast<int>(E);
-  p.M = rows; p.N = N; p.K = K;
-  p.n_tiles_n = static_cast<int>((N + BN - 1) / BN);
-  const int64_t units = ((rows + BM - 1) / BM + E) * p.n_tiles_n;
-  LLMC_CHECK_ARG(units < (1ll << 31), "%s: too many tiles", what);
-  p.num_units = static_cast<int>(units);
+  if (int rc = m.encode_tmaps(g.tmB, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, m.K, BN, BK, CU_TENSOR_MAP_SWIZZLE_128B))
+    return rc;
+  g.seg = m.segments();
+  GemmParams p{};
+  p.out = m.out; p.ld_out = m.N;
+  p.M = m.rows; p.N = kMoe == kMoeSwiGLU ? 2 * m.N : m.N; p.K = m.K;   // gate/up: w1 and w3 columns
+  p.n_tiles_n = n_tiles;
+  p.num_units = units;
   p.num_tiles = p.num_units;
   p.splits = 1;
-  p.kb_total = static_cast<int>((K + BK - 1) / BK);
+  p.kb_total = static_cast<int>((m.K + BK - 1) / BK);
   p.kb_per_split = p.kb_total;
-  p.gn = l2_group_width(static_cast<int64_t>(BN) * K * 2, p.n_tiles_n);
+  p.gn = l2_group_width(static_cast<int64_t>(BN) * m.K * 2, p.n_tiles_n);
   cudaStream_t st = static_cast<cudaStream_t>(stream);
-  return launch_persistent(dtype == LLMC_BF16 ? wgmma_moe_kernel<true, kEpi>
-                                              : wgmma_moe_kernel<false, kEpi>,
+  return launch_persistent(m.dtype == LLMC_BF16 ? wgmma_moe_kernel<true, kMoe> : wgmma_moe_kernel<false, kMoe>,
                            p.num_units, kThreads, kSmemBytes, st, tmA, g, p);
 }
 
@@ -665,23 +623,15 @@ using namespace llmc;
 extern "C" int llmc_moe_gemm_swiglu(const void* xp, const void* const* w1, const void* const* w3,
                                     const int32_t* offsets, void* act, int64_t rows, int64_t inter,
                                     int64_t K, int64_t n_experts, int dtype, void* stream) {
-  LLMC_CHECK_ARG(inter > 0 && inter % 128 == 0,
-                 "moe_gemm_swiglu: inter=%lld must be a positive multiple of 128", (long long)inter);
-  GemmParams p{};
-  p.out = act; p.ld_out = inter;
-  return launch_moe<kEpiSwiGLU>("moe_gemm_swiglu", xp, w1, w3, offsets, nullptr, rows, 2 * inter, K,
-                                n_experts, dtype, p, stream);
+  return launch_moe<kMoeSwiGLU>({"moe_gemm_swiglu", xp, act, w1, w3, offsets, nullptr, rows, inter, K, n_experts,
+                                 dtype, "weight"}, stream);
 }
 
 extern "C" int llmc_moe_gemm_down(const void* act, const void* const* w2, const int32_t* offsets,
                                   const void* w_route, void* y, int64_t rows, int64_t N,
                                   int64_t inter, int64_t n_experts, int dtype, void* stream) {
-  LLMC_CHECK_ARG(N > 0 && N % 8 == 0, "moe_gemm_down: N=%lld must be a positive multiple of 8",
-                 (long long)N);
-  GemmParams p{};
-  p.out = y; p.ld_out = N;
-  return launch_moe<kEpiRouted>("moe_gemm_down", act, w2, nullptr, offsets, w_route, rows, N, inter,
-                                n_experts, dtype, p, stream);
+  return launch_moe<kMoeDown>({"moe_gemm_down", act, y, w2, nullptr, offsets, w_route, rows, N, inter, n_experts,
+                               dtype, "weight"}, stream);
 }
 
 extern "C" int llmc_moe_combine(const void* y, const int64_t* rows, void* out, int64_t T,

@@ -91,35 +91,23 @@ struct W8A8Params {
 template <Mode kMode>
 using Params = std::conditional_t<kMode == kBlockFp8, Fp8GemmParams, W8A8Params>;
 
-// Grouped (sparse-MoE) mode of the W8A8 GEMM: one launch runs one projection of every expert of a
-// layer (gemm.cu's and gemm_w4.cu's grouped GEMMs, on 8-bit codes).  A = the routed rows quantised
-// in expert order, expert e owning rows [offsets[e], offsets[e+1]); tiles come from
-// tc::moe_segment_tile; s_x is one fp32 scale per A row (stride 1).
-//   kMoeSwiGLU  the 128-row B stage is two 64-row TMA boxes: w1 rows n0 .. n0 + 63 of the tile's
-//               expert, then the same rows of w3.  A box is 64 x 128 bytes, a whole number of
-//               128-byte swizzle atoms, so the stage is byte for byte the plain kernel's.  The
-//               epilogue writes act = silu(gate) * up for 64 columns (tc::store_swiglu_m64n64).
-//   kMoeDown    128-row tiles of w2; each output row times its routing weight (tc::store_routed_m64n128).
-// Both scale the accumulator as the plain W8A8 epilogue does first (scale_moe_w8a8).
-enum : int { kMoeOff = 0, kMoeSwiGLU = 1, kMoeDown = 2 };
-// The grouped operands of one launch, per expert linear (gate/up: w1 of expert e at 2e, w3 at
-// 2e + 1; down: w2 of expert e at e): its codes' tensor map and its weight scales (N values, or one
-// when W8A8Params::s_w_stride is 0).  A kernel argument of its own, after Params.
+// Grouped (sparse-MoE) mode of the W8A8 GEMM (tc::MoeMode, on 8-bit codes): A = the routed rows
+// quantised in expert order, s_x one fp32 scale per A row (stride 1).  The gate/up B stage is two
+// 64 x 128-byte boxes, whole 128-byte swizzle atoms, so the stage is byte for byte the plain
+// kernel's; the epilogue writes act = silu(gate) * up for 64 columns (tc::store_swiglu_m64n64).
+// Both projections scale the accumulator as the plain W8A8 epilogue does first (scale_moe_w8a8).
+// The grouped operands of one launch, per expert linear (tc::moe_load_b's order): its codes' tensor
+// map and its weight scales (N values, or one when W8A8Params::s_w_stride is 0).  A kernel argument
+// of its own, after Params.
 struct MoeW8A8Operands {
   CUtensorMap tmB[2 * LLMC_MOE_MAX_EXPERTS];
   const float* s_w[2 * LLMC_MOE_MAX_EXPERTS];
-  const int32_t* offsets;                 // [E + 1] row offsets of the expert segments
-  const void* w_route;                    // kMoeDown: [rows] routing weights (A's row order)
-  int E;
+  MoeSegments seg;
 };
 // The whole argument list of the grouped kernel fits the 4 KB kernel-parameter space at
 // LLMC_MOE_MAX_EXPERTS experts.
 static_assert(2 * sizeof(CUtensorMap) + sizeof(W8A8Params) + sizeof(MoeW8A8Operands) <= 4096,
               "LLMC_MOE_MAX_EXPERTS exceeds the kernel-parameter space");
-
-// The last kernel argument: the grouped operands in grouped mode; in plain mode an unused null
-// pointer, which leaves the plain instantiations' code as it was without the argument.
-template <int kMoe> using MoeArg = std::conditional_t<kMoe == kMoeOff, const void*, MoeW8A8Operands>;
 
 // Grouped mode: acc = fmul(fmul(acc, s_w[col]), s_x[row]) over this thread's part of an m64n128
 // fragment (layout at wgmma_m64n128k16_bf16) whose first row is A row row0 — the plain W8A8
@@ -216,14 +204,14 @@ __device__ __forceinline__ void store_bf16_bias_m64n128(const float (&acc)[64], 
 template <Mode kMode, int DT, int kMoe = kMoeOff>
 __global__ void __launch_bounds__(kThreads, 1)
 gemm_8bit_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
-                 const Params<kMode> p, const __grid_constant__ MoeArg<kMoe> moe) {
+                 const Params<kMode> p, const __grid_constant__ MoeArg<kMoe, MoeW8A8Operands> moe) {
   static_assert(kMoe == kMoeOff || kMode != kBlockFp8, "the grouped mode runs the W8A8 GEMM");
   constexpr bool kInt8 = kMode == kW8A8Int8;
   // the tile of unit u (grouped mode: also its expert, first A row and segment end); false past
   // the last expert's tiles
   auto tile_of = [&](int u, int& e, int& m_blk, int& n_blk, int& row0, int& row_end) -> bool {
     if constexpr (kMoe != kMoeOff) {
-      return moe_segment_tile<kBM>(moe.offsets, moe.E, u, p.n_tiles, p.gn, e, m_blk, n_blk, row0, row_end);
+      return moe_segment_tile<kBM>(moe.seg, u, p.n_tiles, p.gn, e, m_blk, n_blk, row0, row_end);
     } else {
       grouped_tile(u, p.m_tiles, p.n_tiles, p.gn, m_blk, n_blk);
       return true;
@@ -246,7 +234,7 @@ gemm_8bit_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
   if (threadIdx.x == 0) {
     prefetch_tmap(&tmA);
     if constexpr (kMoe != kMoeOff) {
-      for (int i = 0; i < (kMoe == kMoeSwiGLU ? 2 : 1) * moe.E; ++i) prefetch_tmap(&moe.tmB[i]);
+      prefetch_moe_tmaps<kMoe>(moe.tmB, moe.seg);
     } else {
       prefetch_tmap(&tmB);
     }
@@ -269,14 +257,9 @@ gemm_8bit_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
           mbar_wait(&empty_bar[ps.stage], ps.phase ^ 1);
           uint8_t* a_dst = smem + ps.stage * kStageBytes;
           mbar_expect_tx(&full_bar[ps.stage], kStageBytes);
-          if constexpr (kMoe == kMoeSwiGLU) {          // 64 rows of w1, then the same 64 rows of w3
+          if constexpr (kMoe != kMoeOff) {
             tma_load_2d(a_dst, &tmA, &full_bar[ps.stage], kb * kBK, row0);
-            tma_load_2d(a_dst + kTileBytes, &moe.tmB[2 * e], &full_bar[ps.stage], kb * kBK, n_blk * (kBN / 2));
-            tma_load_2d(a_dst + kTileBytes + kTileBytes / 2, &moe.tmB[2 * e + 1], &full_bar[ps.stage], kb * kBK,
-                        n_blk * (kBN / 2));
-          } else if constexpr (kMoe == kMoeDown) {
-            tma_load_2d(a_dst, &tmA, &full_bar[ps.stage], kb * kBK, row0);
-            tma_load_2d(a_dst + kTileBytes, &moe.tmB[e], &full_bar[ps.stage], kb * kBK, n_blk * kBN);
+            moe_load_b<kMoe>(a_dst + kTileBytes, moe.tmB, &full_bar[ps.stage], e, kb * kBK, n_blk, kBN, kTileBytes / 2);
           } else {
             tma_load_2d(a_dst, &tmA, &full_bar[ps.stage], kb * kBK, m_blk * kBM);
             tma_load_2d(a_dst + kTileBytes, &tmB, &full_bar[ps.stage], kb * kBK, n_blk * kBN);
@@ -378,7 +361,7 @@ gemm_8bit_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
     } else if constexpr (kMoe == kMoeDown) {
       const int64_t rg = static_cast<int64_t>(row0) + c * 64;
       scale_moe_w8a8<false>(acc, rg, col0, p, moe.s_w[e], nullptr);
-      store_routed_m64n128<DT>(acc, rg, col0, row_end, p.N, p.N, p.out, moe.w_route);
+      store_routed_m64n128<DT>(acc, rg, col0, row_end, p.N, p.N, p.out, moe.seg.w_route);
     } else if constexpr (kMode != kBlockFp8) {
       store_w8a8_m64n128<DT>(acc, r0, col0, p);
     } else if constexpr (DT == LLMC_F32) {
@@ -445,81 +428,47 @@ int gemm_w8a8(const char* what, const void* x, const float* s_x, int64_t s_x_str
   return launch_gemm_8bit<kFp8 ? kW8A8Fp8 : kW8A8Int8>(x, w, M, N, K, kb_total, dtype, p, stream);
 }
 
-// Checks and launches the grouped W8A8 GEMM of kMoe over `rows` quantised rows a [rows, K] into
-// out [rows, N]: N = inter (the width of w1 / w3 and of act) for gate/up, the hidden size for down.
-// w_b / s_b are w3's (gate/up only).  Every refusal happens before any CUDA call.
+// Checks and launches the grouped W8A8 GEMM over m.rows quantised rows, s_x one scale per row;
+// s_a / s_b the per-expert weight scales of w_a / w_b.
 template <int kMoe>
-int moe_w8a8(const char* what, const void* a, const float* s_x, int fp8, const void* const* w_a,
-             const void* const* w_b, const float* const* s_a, const float* const* s_b, int64_t s_w_stride,
-             const int32_t* offsets, const void* w_route, void* out, int64_t rows, int64_t N, int64_t K,
-             int64_t E, int dtype, void* stream) {
-  constexpr bool kSwiGLU = kMoe == kMoeSwiGLU;
-  LLMC_CHECK_ARG(E >= 1 && E <= LLMC_MOE_MAX_EXPERTS, "%s: %lld experts outside 1..%d", what, (long long)E,
-                 LLMC_MOE_MAX_EXPERTS);
-  LLMC_CHECK_ARG(rows >= 0 && N > 0 && K > 0, "%s: bad shape rows=%lld N=%lld K=%lld", what, (long long)rows,
-                 (long long)N, (long long)K);
-  LLMC_CHECK_ARG(K % 16 == 0, "%s: K=%lld must be a multiple of 16", what, (long long)K);
-  if (kSwiGLU)
-    LLMC_CHECK_ARG(N % 64 == 0, "%s: inter=%lld must be a multiple of 64", what, (long long)N);
-  else
-    LLMC_CHECK_ARG(N % 8 == 0, "%s: N=%lld must be a multiple of 8", what, (long long)N);
-  LLMC_CHECK_ARG(fp8 || K <= kMaxKInt8, "%s: K=%lld > %lld overflows the int32 sum", what, (long long)K,
+int moe_w8a8(const MoeLaunch<kMoe>& m, const float* s_x, int fp8, const float* const* s_a, const float* const* s_b,
+             int64_t s_w_stride, void* stream) {
+  int n_tiles, units;
+  if (int rc = m.check_values(kBM, kBN)) return rc;
+  LLMC_CHECK_ARG(m.K % 16 == 0, "%s: K=%lld must be a multiple of 16", m.what, (long long)m.K);
+  LLMC_CHECK_ARG(fp8 || m.K <= kMaxKInt8, "%s: K=%lld > %lld overflows the int32 sum", m.what, (long long)m.K,
                  (long long)kMaxKInt8);
-  LLMC_CHECK_ARG(s_w_stride == 0 || s_w_stride == 1, "%s: s_w_stride %lld must be 0 or 1", what,
+  LLMC_CHECK_ARG(s_w_stride == 0 || s_w_stride == 1, "%s: s_w_stride %lld must be 0 or 1", m.what,
                  (long long)s_w_stride);
-  LLMC_CHECK_ARG(dtype == LLMC_BF16 || dtype == LLMC_F16, "%s: dtype %d must be bf16 or fp16", what, dtype);
-  LLMC_CHECK_ARG(rows < (1ll << 31) - kBM, "%s: rows=%lld too large", what, (long long)rows);
-  if (rows == 0) return LLMC_OK;
-  LLMC_CHECK_ARG(a && s_x && out && offsets && w_a && s_a && (!kSwiGLU || (w_b && s_b)) && (kSwiGLU || w_route),
-                 "%s: null pointer", what);
-  for (int64_t e = 0; e < E; ++e)
-    LLMC_CHECK_ARG(w_a[e] && s_a[e] && (!kSwiGLU || (w_b[e] && s_b[e])),
-                   "%s: null codes or scales of expert %lld", what, (long long)e);
-  if (!aligned16(a) || !aligned16(out)) {
-    set_last_error("%s: activation and output pointers must be 16-byte aligned", what);
-    return LLMC_EALIGN;
+  if (int rc = m.plan(kBM, kBN, n_tiles, units)) return rc;
+  if (m.rows == 0) return LLMC_OK;
+  if (int rc = m.check_pointers()) return rc;
+  LLMC_CHECK_ARG(s_x && s_a && (!m.kSwiGLU || s_b), "%s: null pointer", m.what);
+  MoeW8A8Operands g{};
+  for (int i = 0; i < m.linears(); ++i) {
+    g.s_w[i] = m.linear(s_a, s_b, i);
+    LLMC_CHECK_ARG(g.s_w[i], "%s: null codes or scales of expert %d", m.what, m.expert_of(i));
   }
-  for (int64_t e = 0; e < E; ++e) {
-    if (!aligned16(w_a[e]) || (kSwiGLU && !aligned16(w_b[e]))) {
-      set_last_error("%s: codes of expert %lld not 16-byte aligned", what, (long long)e);
-      return LLMC_EALIGN;
-    }
-  }
-  const int n_tiles = static_cast<int>(kSwiGLU ? N / (kBN / 2) : (N + kBN - 1) / kBN);
-  const int64_t units = ((rows + kBM - 1) / kBM + E) * n_tiles;
-  LLMC_CHECK_ARG(units < (1ll << 31), "%s: too many tiles", what);
-
   CUtensorMap tmA;
-  if (int rc = encode_tmap_2d(&tmA, a, CU_TENSOR_MAP_DATA_TYPE_UINT8, 1, rows, K, K, kBM, kBK,
+  if (int rc = encode_tmap_2d(&tmA, m.a, CU_TENSOR_MAP_DATA_TYPE_UINT8, 1, m.rows, m.K, m.K, kBM, kBK,
                               CU_TENSOR_MAP_SWIZZLE_128B))
     return rc;
-  MoeW8A8Operands g{};
-  constexpr uint32_t box_rows = kSwiGLU ? kBN / 2 : kBN;
-  for (int64_t e = 0; e < E; ++e) {
-    for (int h = 0; h < (kSwiGLU ? 2 : 1); ++h) {
-      const int i = static_cast<int>(kSwiGLU ? 2 * e + h : e);
-      if (int rc = encode_tmap_2d(&g.tmB[i], h ? w_b[e] : w_a[e], CU_TENSOR_MAP_DATA_TYPE_UINT8, 1, N, K, K,
-                                  box_rows, kBK, CU_TENSOR_MAP_SWIZZLE_128B))
-        return rc;
-      g.s_w[i] = h ? s_b[e] : s_a[e];
-    }
-  }
-  g.offsets = offsets;
-  g.w_route = w_route;
-  g.E = static_cast<int>(E);
+  if (int rc = m.encode_tmaps(g.tmB, CU_TENSOR_MAP_DATA_TYPE_UINT8, 1, m.K, kBN, kBK, CU_TENSOR_MAP_SWIZZLE_128B))
+    return rc;
+  g.seg = m.segments();
   W8A8Params p{};
   p.s_x = s_x; p.s_x_stride = 1; p.s_w_stride = s_w_stride;
-  p.out = out;
-  p.M = rows; p.N = N;
-  p.kb_total = static_cast<int>((K + kBK - 1) / kBK);   // TMA zero-fills the K tail
+  p.out = m.out;
+  p.M = m.rows; p.N = m.N;
+  p.kb_total = static_cast<int>((m.K + kBK - 1) / kBK);   // TMA zero-fills the K tail
   p.n_tiles = n_tiles;
-  p.num_tiles = static_cast<int>(units);
-  p.gn = l2_group_width(static_cast<int64_t>(kBN) * K, n_tiles);   // one n-tile's weight bytes
+  p.num_tiles = units;
+  p.gn = l2_group_width(static_cast<int64_t>(kBN) * m.K, n_tiles);   // one n-tile's weight bytes
   cudaStream_t st = static_cast<cudaStream_t>(stream);
-  auto kernel = fp8 ? (dtype == LLMC_BF16 ? gemm_8bit_kernel<kW8A8Fp8, LLMC_BF16, kMoe>
-                                          : gemm_8bit_kernel<kW8A8Fp8, LLMC_F16, kMoe>)
-                    : (dtype == LLMC_BF16 ? gemm_8bit_kernel<kW8A8Int8, LLMC_BF16, kMoe>
-                                          : gemm_8bit_kernel<kW8A8Int8, LLMC_F16, kMoe>);
+  auto kernel = fp8 ? (m.dtype == LLMC_BF16 ? gemm_8bit_kernel<kW8A8Fp8, LLMC_BF16, kMoe>
+                                            : gemm_8bit_kernel<kW8A8Fp8, LLMC_F16, kMoe>)
+                    : (m.dtype == LLMC_BF16 ? gemm_8bit_kernel<kW8A8Int8, LLMC_BF16, kMoe>
+                                            : gemm_8bit_kernel<kW8A8Int8, LLMC_F16, kMoe>);
   return launch_persistent(kernel, p.num_tiles, kThreads, kSmemBytes, st, tmA, CUtensorMap{}, p, g);
 }
 
@@ -574,14 +523,14 @@ extern "C" int llmc_moe_gemm_w8a8_swiglu(const void* xq, const float* s_x, int f
                                          const float* const* s_w3, int64_t s_w_stride, const int32_t* offsets,
                                          void* act, int64_t rows, int64_t inter, int64_t K, int64_t n_experts,
                                          int dtype, void* stream) {
-  return moe_w8a8<kMoeSwiGLU>("moe_gemm_w8a8_swiglu", xq, s_x, fp8, w1, w3, s_w1, s_w3, s_w_stride, offsets,
-                              nullptr, act, rows, inter, K, n_experts, dtype, stream);
+  return moe_w8a8<kMoeSwiGLU>({"moe_gemm_w8a8_swiglu", xq, act, w1, w3, offsets, nullptr, rows, inter, K, n_experts,
+                               dtype, "codes or scales"}, s_x, fp8, s_w1, s_w3, s_w_stride, stream);
 }
 
 extern "C" int llmc_moe_gemm_w8a8_down(const void* actq, const float* s_x, int fp8, const void* const* w2,
                                        const float* const* s_w2, int64_t s_w_stride, const int32_t* offsets,
                                        const void* w_route, void* y, int64_t rows, int64_t N, int64_t inter,
                                        int64_t n_experts, int dtype, void* stream) {
-  return moe_w8a8<kMoeDown>("moe_gemm_w8a8_down", actq, s_x, fp8, w2, nullptr, s_w2, nullptr, s_w_stride,
-                            offsets, w_route, y, rows, N, inter, n_experts, dtype, stream);
+  return moe_w8a8<kMoeDown>({"moe_gemm_w8a8_down", actq, y, w2, nullptr, offsets, w_route, rows, N, inter, n_experts,
+                             dtype, "codes or scales"}, s_x, fp8, s_w2, nullptr, s_w_stride, stream);
 }

@@ -157,28 +157,20 @@ struct ParamsRz : Params {
 };
 template <int kRz> using ParamsOf = std::conditional_t<kRz == kRzOff, Params, ParamsRz>;
 
-// Grouped (sparse-MoE) mode: one launch runs one projection of every expert of a layer (gemm.cu's
-// grouped GEMM, on packed weights).  A = the routed rows gathered in expert order, expert e owning
-// rows [offsets[e], offsets[e+1]); tiles come from tc::moe_segment_tile.
-//   kMoeSwiGLU  the 128-row B tile is two 64-row TMA boxes: rows 0..63 are w1 rows n0 .. n0 + 63 of
-//               the tile's expert, rows 64..127 the same rows of w3.  A box is 2 KB (W4) / 4 KB (W8),
-//               a whole number of swizzle atoms, so the dequant warps' row swizzle is unchanged.  The
-//               epilogue writes act = silu(gate) * up for 64 columns (store_swiglu_m64n64).
-//   kMoeDown    128-row tiles of w2; each output row times its routing weight (store_routed_m64n128).
-enum : int { kMoeOff = 0, kMoeSwiGLU = 1, kMoeDown = 2 };
-// The grouped operands of one launch, per expert linear (gate/up: w1 of expert e at 2e, w3 at
-// 2e + 1; down: w2 of expert e at e): its packed codes' tensor map and its qparam and g_idx
-// pointers.  Every linear of a launch has one form: bits, qparam dtype and layout, zeros (all null:
-// 2^(bits-1)) and g_idx (all null: contiguous groups).  A kernel argument of its own, so that
-// Params stays within its 128 bytes.
+// Grouped (sparse-MoE) mode (tc::MoeMode, on packed weights): the gate/up B tile is two 64-row
+// boxes of 2 KB (W4) / 4 KB (W8), whole swizzle atoms, so the dequant warps' row swizzle is
+// unchanged; rows 0..63 of the tile are w1's, 64..127 w3's.  The epilogue writes act =
+// silu(gate) * up for 64 columns (store_swiglu_m64n64).
+// The grouped operands of one launch, per expert linear (tc::moe_load_b's order): its packed
+// codes' tensor map and its qparam and g_idx pointers.  Every linear of a launch has one form:
+// bits, qparam dtype and layout, zeros (all null: 2^(bits-1)) and g_idx (all null: contiguous
+// groups).  A kernel argument of its own, so that Params stays within its 128 bytes.
 struct MoeW4Operands {
   CUtensorMap tmP[2 * LLMC_MOE_MAX_EXPERTS];
   const void* scales[2 * LLMC_MOE_MAX_EXPERTS];
   const void* zeros[2 * LLMC_MOE_MAX_EXPERTS];
   const int32_t* g_idx[2 * LLMC_MOE_MAX_EXPERTS];
-  const int32_t* offsets;                 // [E + 1] row offsets of the expert segments
-  const void* w_route;                    // kMoeDown: [rows] routing weights (A's row order)
-  int E;
+  MoeSegments seg;
 };
 // The whole argument list of the grouped kernel fits the 4 KB kernel-parameter space at
 // LLMC_MOE_MAX_EXPERTS experts.
@@ -318,18 +310,13 @@ __device__ __forceinline__ void next_outlier(const int32_t* cols, int& ocur, int
   oc = ocur < oend ? __ldg(cols + ocur) : INT_MAX;
 }
 
-// The last kernel argument: the grouped operands in grouped mode; in plain mode an unused null
-// pointer.  A pointer leaves the plain instantiations' code as it was without the argument (an
-// empty struct, or moving the body into a __device__ function the kernel calls, does not).
-template <int kMoe> using MoeArg = std::conditional_t<kMoe == kMoeOff, const void*, MoeW4Operands>;
-
 // Plain mode: tiles from grouped_tile, B from tmP, qparams from p.  Grouped mode (kMoe): tiles
 // from moe_segment_tile, B and the qparams of the tile's expert from `moe`; tmP is unused.
 template <bool kBf16, int kBits, bool kGidx, int kGrid, int kRz = kRzOff, int kLayout = kPackK,
           int kMoe = kMoeOff>
 __global__ void __launch_bounds__(Cfg<kBits>::kThreads, 1)
 w4a16_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmP,
-                  const ParamsOf<kRz> p, const __grid_constant__ MoeArg<kMoe> moe) {
+                  const ParamsOf<kRz> p, const __grid_constant__ MoeArg<kMoe, MoeW4Operands> moe) {
   using C = Cfg<kBits>;
   constexpr bool kAwq = kLayout == kPackAwq;
   static_assert(!kAwq || (kBits == 4 && !kGidx && kGrid == kGridInt && kRz == kRzOff),
@@ -352,7 +339,7 @@ w4a16_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
   // the last expert's tiles
   auto tile_of = [&](int u, int& e, int& m_blk, int& n_blk, int& row0, int& row_end) -> bool {
     if constexpr (kMoe != kMoeOff) {
-      return moe_segment_tile<BM>(g->offsets, g->E, u, p.n_tiles_n, p.gn, e, m_blk, n_blk, row0, row_end);
+      return moe_segment_tile<BM>(g->seg, u, p.n_tiles_n, p.gn, e, m_blk, n_blk, row0, row_end);
     } else {
       grouped_tile(u, p.num_units / p.n_tiles_n, p.n_tiles_n, p.gn, m_blk, n_blk);
       return true;
@@ -362,7 +349,7 @@ w4a16_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
   if (threadIdx.x == 0) {
     prefetch_tmap(&tmA);
     if constexpr (kMoe != kMoeOff) {
-      for (int i = 0; i < (kMoe == kMoeSwiGLU ? 2 : 1) * g->E; ++i) prefetch_tmap(&g->tmP[i]);
+      prefetch_moe_tmaps<kMoe>(g->tmP, g->seg);
     } else {
       prefetch_tmap(&tmP);
     }
@@ -386,13 +373,8 @@ w4a16_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
           ring_l.expect_tx(sl, kLBytes);
           if constexpr (kMoe != kMoeOff) {
             tma_load_2d(a_dst, &tmA, &ring_l.full[sl.stage], kb * BK, row0);
-            if constexpr (kMoe == kMoeSwiGLU) {     // 64 rows of w1, then the same 64 rows of w3
-              tma_load_2d(p_dst, &g->tmP[2 * e], &ring_l.full[sl.stage], kb * C::kWordsPerRow, n_blk * (BN / 2));
-              tma_load_2d(p_dst + C::kPBytes / 2, &g->tmP[2 * e + 1], &ring_l.full[sl.stage],
-                          kb * C::kWordsPerRow, n_blk * (BN / 2));
-            } else {
-              tma_load_2d(p_dst, &g->tmP[e], &ring_l.full[sl.stage], kb * C::kWordsPerRow, n_blk * BN);
-            }
+            moe_load_b<kMoe>(p_dst, g->tmP, &ring_l.full[sl.stage], e, kb * C::kWordsPerRow, n_blk, BN,
+                             C::kPBytes / 2);
           } else {
             tma_load_2d(a_dst, &tmA, &ring_l.full[sl.stage], kb * BK, m_blk * BM);
             if constexpr (kAwq)     // [64 k-rows x 16 words] of qweight [K, N/8]
@@ -453,7 +435,7 @@ w4a16_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
                                 row_end, p.N, p.out);
       } else if constexpr (kMoe == kMoeDown) {
         store_routed_m64n128<DT>(acc, static_cast<int64_t>(row0) + c * 64, static_cast<int64_t>(n_blk) * BN,
-                                 row_end, p.N, p.N, p.out, g->w_route);
+                                 row_end, p.N, p.N, p.out, g->seg.w_route);
       } else {
         store_linear_m64n128<DT>(acc, static_cast<int64_t>(m_blk) * BM + c * 64,
                                  static_cast<int64_t>(n_blk) * BN, p.M, p.N, p.N, p.bias, p.out);
@@ -1192,137 +1174,96 @@ extern "C" int llmc_gemm_w8a16_rz(const void* x, const int32_t* wq, const float*
 }
 
 // ---- grouped (sparse-MoE) mode on packed experts ---------------------------------------------
-// The expert linears of one launch, in MoeW4Operands' order (gate/up: w1 of expert e at 2e, w3 at
-// 2e + 1; down: w2 of expert e at e).  A null zeros or g_idx array stands for all-null entries.
-struct MoeLinears {
-  int count;
-  const int32_t* wq[2 * LLMC_MOE_MAX_EXPERTS];
-  const void* s[2 * LLMC_MOE_MAX_EXPERTS];
-  const void* z[2 * LLMC_MOE_MAX_EXPERTS];
-  const int32_t* g[2 * LLMC_MOE_MAX_EXPERTS];
-};
-
+// g: the checked qparam and g_idx pointers of every expert linear; its maps and segments are set here.
 template <int kBits, int kMoe>
-static int launch_moe_packed(const char* name, const void* a, const MoeLinears& L, int qparam_dtype,
-                             int64_t group, int q_transposed, int64_t ng, const int32_t* offsets,
-                             const void* w_route, void* out, int64_t rows, int64_t N, int64_t K, int64_t E,
-                             int dtype, void* stream) {
+static int launch_moe_packed(const MoeLaunch<kMoe>& m, w4::MoeW4Operands& g, int qparam_dtype, int64_t group,
+                             int q_transposed, int64_t ng, int n_tiles, int units, void* stream) {
   using namespace w4;
   using C = Cfg<kBits>;
   constexpr CUtensorMapSwizzle swz = kBits == 4 ? CU_TENSOR_MAP_SWIZZLE_32B : CU_TENSOR_MAP_SWIZZLE_64B;
-  constexpr int box_rows = kMoe == kMoeSwiGLU ? BN / 2 : BN;
   CUtensorMap tmA;
-  if (int rc = encode_tmap_2d(&tmA, a, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, rows, K, K, BM, BK,
+  if (int rc = encode_tmap_2d(&tmA, m.a, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, m.rows, m.K, m.K, BM, BK,
                               CU_TENSOR_MAP_SWIZZLE_128B))
     return rc;
-  MoeW4Operands g{};
-  for (int i = 0; i < L.count; ++i) {
-    if (int rc = encode_tmap_2d(&g.tmP[i], L.wq[i], CU_TENSOR_MAP_DATA_TYPE_INT32, 4, N, K * kBits / 32,
-                                K * kBits / 32, box_rows, C::kWordsPerRow, swz))
-      return rc;
-    g.scales[i] = L.s[i]; g.zeros[i] = L.z[i]; g.g_idx[i] = L.g[i];
-  }
-  g.offsets = offsets;
-  g.w_route = w_route;
-  g.E = static_cast<int>(E);
-  const bool gidx = L.g[0] != nullptr;
+  if (int rc = m.encode_tmaps(g.tmP, CU_TENSOR_MAP_DATA_TYPE_INT32, 4, m.K * kBits / 32, BN, C::kWordsPerRow, swz))
+    return rc;
+  g.seg = m.segments();
+  const bool gidx = g.g_idx[0] != nullptr;
   Params p{};
-  p.M = rows; p.N = N; p.K = K; p.out = out;
+  p.M = m.rows; p.N = m.N; p.K = m.K; p.out = m.out;
   p.qparam_native = qparam_dtype != LLMC_F32 ? 1 : 0;
   p.q_transposed = q_transposed;
-  p.group = gidx ? K : group; p.ng = static_cast<int>(ng);
+  p.group = gidx ? m.K : group; p.ng = static_cast<int>(ng);
   p.zero_default = static_cast<float>(1 << (kBits - 1));
-  p.n_tiles_n = static_cast<int>((N + box_rows - 1) / box_rows);
-  const int64_t units = ((rows + BM - 1) / BM + E) * p.n_tiles_n;
-  LLMC_CHECK_ARG(units < (1ll << 31), "%s: too many tiles", name);
-  p.num_units = static_cast<int>(units);
-  p.kb_total = static_cast<int>(K / BK);
-  p.gn = l2_group_width(static_cast<int64_t>(BN) * K * kBits / 8 + 1, p.n_tiles_n);
+  p.n_tiles_n = n_tiles;
+  p.num_units = units;
+  p.kb_total = static_cast<int>(m.K / BK);
+  p.gn = l2_group_width(static_cast<int64_t>(BN) * m.K * kBits / 8 + 1, p.n_tiles_n);
   cudaStream_t st = static_cast<cudaStream_t>(stream);
-  auto kernel = gidx ? (dtype == LLMC_BF16 ? w4a16_gemm_kernel<true, kBits, true, kGridInt, kRzOff, kPackK, kMoe>
-                                           : w4a16_gemm_kernel<false, kBits, true, kGridInt, kRzOff, kPackK, kMoe>)
-                     : (dtype == LLMC_BF16 ? w4a16_gemm_kernel<true, kBits, false, kGridInt, kRzOff, kPackK, kMoe>
-                                           : w4a16_gemm_kernel<false, kBits, false, kGridInt, kRzOff, kPackK, kMoe>);
+  const bool bf16 = m.dtype == LLMC_BF16;
+  auto kernel = gidx ? (bf16 ? w4a16_gemm_kernel<true, kBits, true, kGridInt, kRzOff, kPackK, kMoe>
+                             : w4a16_gemm_kernel<false, kBits, true, kGridInt, kRzOff, kPackK, kMoe>)
+                     : (bf16 ? w4a16_gemm_kernel<true, kBits, false, kGridInt, kRzOff, kPackK, kMoe>
+                             : w4a16_gemm_kernel<false, kBits, false, kGridInt, kRzOff, kPackK, kMoe>);
   return launch_persistent(kernel, p.num_units, C::kThreads, C::kSmemBytes, st, tmA, CUtensorMap{}, p, g);
 }
 
-// Checks and launches the grouped packed GEMM of kMoe over `rows` gathered rows of a [rows, K]
-// into out [rows, N]: N = inter (the width of w1 / w3 and of act) for gate/up, the hidden size for
-// down.  The *_b arrays are w3's (gate/up only).  Every refusal happens before any CUDA call.
+// Checks and launches the grouped packed GEMM over m.rows gathered rows (the codes are m's
+// weights); the *_a / *_b arrays are the qparams and g_idx of w_a / w_b.
 template <int kMoe>
-static int moe_packed(const char* name, const void* a, int bits, const int32_t* const* wq_a,
-                      const int32_t* const* wq_b, const void* const* s_a, const void* const* s_b,
+static int moe_packed(const MoeLaunch<kMoe>& m, int bits, const void* const* s_a, const void* const* s_b,
                       const void* const* z_a, const void* const* z_b, const int32_t* const* g_a,
-                      const int32_t* const* g_b, int qparam_dtype, int64_t group, int64_t ng,
-                      const int32_t* offsets, const void* w_route, void* out, int64_t rows, int64_t N,
-                      int64_t K, int64_t E, int dtype, void* stream) {
+                      const int32_t* const* g_b, int qparam_dtype, int64_t group, int64_t ng, void* stream) {
   using namespace w4;
-  constexpr bool kSwiGLU = kMoe == kMoeSwiGLU;
+  const char* name = m.what;
+  int n_tiles, units;
+  if (int rc = m.check_values(BM, BN)) return rc;
   LLMC_CHECK_ARG(bits == 4 || bits == 8, "%s: bits=%d must be 4 or 8", name, bits);
-  LLMC_CHECK_ARG(E >= 1 && E <= LLMC_MOE_MAX_EXPERTS, "%s: %lld experts outside 1..%d", name, (long long)E,
-                 LLMC_MOE_MAX_EXPERTS);
-  LLMC_CHECK_ARG(rows >= 0 && N > 0 && K > 0, "%s: bad shape", name);
-  LLMC_CHECK_ARG(K % BK == 0, "%s: K=%lld must be a multiple of %d", name, (long long)K, BK);
-  if (kSwiGLU)
-    LLMC_CHECK_ARG(N % 64 == 0, "%s: inter=%lld must be a multiple of 64", name, (long long)N);
-  else
-    LLMC_CHECK_ARG(N % 8 == 0, "%s: N=%lld must be a multiple of 8", name, (long long)N);
+  LLMC_CHECK_ARG(m.K % BK == 0, "%s: K=%lld must be a multiple of %d", name, (long long)m.K, BK);
   const int64_t ag = group < 0 ? -group : group;
-  LLMC_CHECK_ARG(ag > 0 && ag % BK == 0 && K % ag == 0,
-                 "%s: group %lld must divide K=%lld and be a multiple of %d", name, (long long)ag, (long long)K, BK);
-  LLMC_CHECK_ARG(rows < (1ll << 31) - BM, "%s: rows=%lld too large", name, (long long)rows);
-  if (rows == 0) return LLMC_OK;
-  LLMC_CHECK_ARG(dtype == LLMC_BF16 || dtype == LLMC_F16, "%s: dtype must be bf16 or fp16", name);
-  LLMC_CHECK_ARG(qparam_dtype == LLMC_F32 || qparam_dtype == dtype,
+  LLMC_CHECK_ARG(ag > 0 && ag % BK == 0 && m.K % ag == 0, "%s: group %lld must divide K=%lld and be a multiple of %d",
+                 name, (long long)ag, (long long)m.K, BK);
+  LLMC_CHECK_ARG(qparam_dtype == LLMC_F32 || qparam_dtype == m.dtype,
                  "%s: qparam_dtype must be fp32 or the activation dtype", name);
-  LLMC_CHECK_ARG(a && out && offsets && wq_a && s_a && (!kSwiGLU || (wq_b && s_b)) && (kSwiGLU || w_route),
-                 "%s: null pointer", name);
-  MoeLinears L{};
-  L.count = static_cast<int>((kSwiGLU ? 2 : 1) * E);
-  for (int64_t e = 0; e < E; ++e) {
-    for (int h = 0; h < (kSwiGLU ? 2 : 1); ++h) {
-      const int i = static_cast<int>(kSwiGLU ? 2 * e + h : e);
-      L.wq[i] = h ? wq_b[e] : wq_a[e];
-      L.s[i] = h ? s_b[e] : s_a[e];
-      const void* const* z = h ? z_b : z_a;
-      const int32_t* const* gi = h ? g_b : g_a;
-      L.z[i] = z ? z[e] : nullptr;
-      L.g[i] = gi ? gi[e] : nullptr;
-      LLMC_CHECK_ARG(L.wq[i] && L.s[i], "%s: null codes or scales of expert %lld", name, (long long)e);
-    }
+  if (int rc = m.plan(BM, BN, n_tiles, units)) return rc;
+  if (m.rows == 0) return LLMC_OK;
+  if (int rc = m.check_pointers()) return rc;
+  LLMC_CHECK_ARG(s_a && (!m.kSwiGLU || s_b), "%s: null pointer", name);
+  MoeW4Operands g{};
+  const void** z = g.zeros;
+  const int32_t** gi = g.g_idx;
+  for (int i = 0; i < m.linears(); ++i) {
+    g.scales[i] = m.linear(s_a, s_b, i);
+    z[i] = m.linear(z_a, z_b, i);
+    gi[i] = m.linear(g_a, g_b, i);
+    LLMC_CHECK_ARG(g.scales[i], "%s: null codes or scales of expert %d", name, m.expert_of(i));
   }
-  for (int i = 1; i < L.count; ++i) {
-    const long long e = kSwiGLU ? i / 2 : i;
-    LLMC_CHECK_ARG((L.z[i] == nullptr) == (L.z[0] == nullptr),
-                   "%s: zeros of expert %lld %s while expert 0's %s", name, e, L.z[i] ? "given" : "null",
-                   L.z[0] ? "are given" : "are null");
-    LLMC_CHECK_ARG((L.g[i] == nullptr) == (L.g[0] == nullptr),
-                   "%s: g_idx of expert %lld %s while expert 0's %s", name, e, L.g[i] ? "given" : "null",
-                   L.g[0] ? "is given" : "is null");
+  for (int i = 1; i < m.linears(); ++i) {
+    const int e = m.expert_of(i);
+    LLMC_CHECK_ARG((z[i] == nullptr) == (z[0] == nullptr), "%s: zeros of expert %d %s while expert 0's %s", name, e,
+                   z[i] ? "given" : "null", z[0] ? "are given" : "are null");
+    LLMC_CHECK_ARG((gi[i] == nullptr) == (gi[0] == nullptr), "%s: g_idx of expert %d %s while expert 0's %s", name,
+                   e, gi[i] ? "given" : "null", gi[0] ? "is given" : "is null");
   }
-  if (L.g[0] == nullptr)
-    LLMC_CHECK_ARG(ng == K / ag, "%s: ng=%lld, but K=%lld in groups of %lld is %lld groups", name, (long long)ng,
-                   (long long)K, (long long)ag, (long long)(K / ag));
+  if (gi[0] == nullptr)
+    LLMC_CHECK_ARG(ng == m.K / ag, "%s: ng=%lld, but K=%lld in groups of %lld is %lld groups", name, (long long)ng,
+                   (long long)m.K, (long long)ag, (long long)(m.K / ag));
   else
-    LLMC_CHECK_ARG(ng >= 1 && ng <= K, "%s: ng=%lld groups for K=%lld columns", name, (long long)ng, (long long)K);
-  if (!aligned16(a) || !aligned16(out)) {
-    set_last_error("%s: activation and output pointers must be 16-byte aligned", name);
-    return LLMC_EALIGN;
-  }
-  for (int i = 0; i < L.count; ++i) {
-    if (!aligned16(L.wq[i]) || (L.g[i] && !aligned16(L.g[i]))) {
-      set_last_error("%s: codes or g_idx of expert %lld not 16-byte aligned", name,
-                     (long long)(kSwiGLU ? i / 2 : i));
+    LLMC_CHECK_ARG(ng >= 1 && ng <= m.K, "%s: ng=%lld groups for K=%lld columns", name, (long long)ng,
+                   (long long)m.K);
+  for (int i = 0; i < m.linears(); ++i) {
+    if (gi[i] && !aligned16(gi[i])) {
+      set_last_error("%s: g_idx of expert %d not 16-byte aligned", name, m.expert_of(i));
       return LLMC_EALIGN;
     }
   }
   const int qt = group < 0 ? 1 : 0;
-  if (bits == 4)
-    return launch_moe_packed<4, kMoe>(name, a, L, qparam_dtype, ag, qt, ng, offsets, w_route, out, rows, N, K, E,
-                                      dtype, stream);
-  return launch_moe_packed<8, kMoe>(name, a, L, qparam_dtype, ag, qt, ng, offsets, w_route, out, rows, N, K, E,
-                                    dtype, stream);
+  if (bits == 4) return launch_moe_packed<4>(m, g, qparam_dtype, ag, qt, ng, n_tiles, units, stream);
+  return launch_moe_packed<8>(m, g, qparam_dtype, ag, qt, ng, n_tiles, units, stream);
 }
+
+// The packed codes arrays, as MoeLaunch's untyped per-expert weight arrays.
+static const void* const* codes(const int32_t* const* wq) { return reinterpret_cast<const void* const*>(wq); }
 
 extern "C" int llmc_moe_gemm_packed_swiglu(const void* xp, int bits, const int32_t* const* wq1,
                                            const int32_t* const* wq3, const void* const* s1, const void* const* s3,
@@ -1330,9 +1271,9 @@ extern "C" int llmc_moe_gemm_packed_swiglu(const void* xp, int bits, const int32
                                            const int32_t* const* gidx3, int qparam_dtype, int64_t group, int64_t ng,
                                            const int32_t* offsets, void* act, int64_t rows, int64_t inter,
                                            int64_t K, int64_t n_experts, int dtype, void* stream) {
-  return moe_packed<w4::kMoeSwiGLU>("moe_gemm_packed_swiglu", xp, bits, wq1, wq3, s1, s3, z1, z3, gidx1, gidx3,
-                                    qparam_dtype, group, ng, offsets, nullptr, act, rows, inter, K, n_experts,
-                                    dtype, stream);
+  return moe_packed<kMoeSwiGLU>({"moe_gemm_packed_swiglu", xp, act, codes(wq1), codes(wq3), offsets, nullptr, rows,
+                                 inter, K, n_experts, dtype, "codes or scales"},
+                                bits, s1, s3, z1, z3, gidx1, gidx3, qparam_dtype, group, ng, stream);
 }
 
 extern "C" int llmc_moe_gemm_packed_down(const void* act, int bits, const int32_t* const* wq2,
@@ -1340,7 +1281,7 @@ extern "C" int llmc_moe_gemm_packed_down(const void* act, int bits, const int32_
                                          int qparam_dtype, int64_t group, int64_t ng, const int32_t* offsets,
                                          const void* w_route, void* y, int64_t rows, int64_t N, int64_t inter,
                                          int64_t n_experts, int dtype, void* stream) {
-  return moe_packed<w4::kMoeDown>("moe_gemm_packed_down", act, bits, wq2, nullptr, s2, nullptr, z2, nullptr,
-                                  gidx2, nullptr, qparam_dtype, group, ng, offsets, w_route, y, rows, N, inter,
-                                  n_experts, dtype, stream);
+  return moe_packed<kMoeDown>({"moe_gemm_packed_down", act, y, codes(wq2), nullptr, offsets, w_route, rows, N, inter,
+                               n_experts, dtype, "codes or scales"},
+                              bits, s2, nullptr, z2, nullptr, gidx2, nullptr, qparam_dtype, group, ng, stream);
 }

@@ -5,6 +5,8 @@
 
 #include <cuda.h>  // CUtensorMap (types only; the driver entry point is resolved at run time)
 
+#include <type_traits>
+
 #include "common.cuh"
 
 namespace llmc {
@@ -280,19 +282,61 @@ __device__ __forceinline__ void grouped_tile(int u, int m_tiles, int n_tiles, in
   n_blk = g * gn + (rem - m_blk * gsz);
 }
 
-// Grouped (sparse-MoE) mode of the forward GEMMs: A holds the routed rows in expert order, expert e
-// owning rows [offsets[e], offsets[e+1]) (int32, device memory).  Unit u is tile u - (tiles of
-// experts < e) of expert e, in grouped_tile's order within the expert, with kBM-row m-tiles; row0
-// is the tile's first A row and row_end the end of its segment.  False past the last expert's
-// tiles: the launch bounds the unit count by (ceil(rows / kBM) + E) n-tile columns, so the host
-// never reads the offsets.
+// Grouped (sparse-MoE) mode of the forward GEMMs (gemm.cu, gemm_w4.cu, gemm_8bit.cu): one launch
+// runs one projection of every expert of a layer (DESIGN.md §4).  kMoeSwiGLU: gate/up, the B tile
+// is w1 rows then the same w3 rows (moe_load_b), the epilogue writes silu(gate) * up; kMoeDown: w2,
+// each output row times its routing weight.  kMoeOff: the plain GEMM.
+enum MoeMode : int { kMoeOff, kMoeSwiGLU, kMoeDown };
+
+// The segments of a grouped launch, the last member of each kernel's grouped operands.  A holds the
+// routed rows in expert order, expert e owning rows [offsets[e], offsets[e+1]).
+struct MoeSegments {
+  const int32_t* offsets;   // [E + 1] int32, device memory: read by the kernel, never by the host
+  const void* w_route;      // kMoeDown: [rows] routing weights in A's row order
+  int E;
+};
+
+// The last kernel argument of a GEMM with a grouped mode: its grouped operands in grouped mode; in
+// plain mode an unused null pointer, which leaves the plain instantiations' code as it was without
+// the argument (an empty struct, or the body in a __device__ function the kernel calls, does not).
+template <int kMoe, class Operands>
+using MoeArg = std::conditional_t<kMoe == kMoeOff, const void*, Operands>;
+
+// Prefetches the expert tensor maps of a grouped launch: one per expert linear (moe_load_b).  The
+// bound is read through s after each prefetch (a memory clobber), which keeps the loop as the
+// kernels had it inline; an E passed by value lets ptxas unroll it.
+template <int kMoe>
+__device__ __forceinline__ void prefetch_moe_tmaps(const CUtensorMap* maps, const MoeSegments& s) {
+  for (int i = 0; i < (kMoe == kMoeSwiGLU ? 2 : 1) * s.E; ++i) prefetch_tmap(&maps[i]);
+}
+
+// Loads the tile_rows-row B tile of n-tile n_blk of expert e, K coordinate k, into dst.  The maps
+// are one per expert linear: gate/up w1 of expert e at 2e and w3 at 2e + 1, down w2 at e.
+// kMoeSwiGLU: rows n_blk * tile_rows / 2 .. of w1 into dst, the same rows of w3 into
+// dst + half_bytes; a half box is a whole number of swizzle atoms, so the tile holds gate columns
+// then up columns.  kMoeDown: rows n_blk * tile_rows .. of w2.
+template <int kMoe>
+__device__ __forceinline__ void moe_load_b(uint8_t* dst, const CUtensorMap* maps, uint64_t* bar, int e,
+                                           int32_t k, int n_blk, int tile_rows, int half_bytes) {
+  if constexpr (kMoe == kMoeSwiGLU) {
+    tma_load_2d(dst, &maps[2 * e], bar, k, n_blk * (tile_rows / 2));
+    tma_load_2d(dst + half_bytes, &maps[2 * e + 1], bar, k, n_blk * (tile_rows / 2));
+  } else {
+    tma_load_2d(dst, &maps[e], bar, k, n_blk * tile_rows);
+  }
+}
+
+// Unit u of a grouped launch is tile u - (tiles of experts < e) of expert e, in grouped_tile's
+// order within the expert, with kBM-row m-tiles; row0 is the tile's first A row and row_end the end
+// of its segment.  False past the last expert's tiles: the launch bounds the unit count by
+// (ceil(rows / kBM) + E) n-tile columns (MoeLaunch::plan), so the host never reads the offsets.
 template <int kBM>
-__device__ __forceinline__ bool moe_segment_tile(const int32_t* offsets, int E, int u, int n_tiles,
-                                                 int gn, int& e_out, int& m_blk, int& n_blk,
-                                                 int& row0, int& row_end) {
+__device__ __forceinline__ bool moe_segment_tile(const MoeSegments& s, int u, int n_tiles, int gn,
+                                                 int& e_out, int& m_blk, int& n_blk, int& row0,
+                                                 int& row_end) {
   int rem = u;
-  for (int e = 0; e < E; ++e) {
-    const int r0 = __ldg(offsets + e), r1 = __ldg(offsets + e + 1);
+  for (int e = 0; e < s.E; ++e) {
+    const int r0 = __ldg(s.offsets + e), r1 = __ldg(s.offsets + e + 1);
     const int m_tiles = (r1 - r0 + kBM - 1) / kBM;
     if (rem < m_tiles * n_tiles) {
       grouped_tile(rem, m_tiles, n_tiles, gn, m_blk, n_blk);
@@ -441,6 +485,89 @@ inline int l2_group_width(int64_t divisor, int n_tiles) {
   if (gn > n_tiles) gn = n_tiles;
   return static_cast<int>(gn);
 }
+
+// A grouped (sparse-MoE) launch of mode kMoe (tc::moe_segment_tile): the arguments every grouped
+// entry point has, and what follows from them alone.  Checks that read only scalars come before the
+// rows == 0 return (check_values, plan), checks that read a pointer after it (check_pointers), and
+// every refusal before any CUDA call.
+template <int kMoe>
+struct MoeLaunch {
+  static constexpr bool kSwiGLU = kMoe == tc::kMoeSwiGLU;
+  const char* what;
+  const void* a;                  // [rows, K]: the routed rows in expert order
+  void* out;                      // [rows, N]
+  const void* const* w_a;         // HOST arrays of E device pointers, one per expert, to its weight
+  const void* const* w_b;         //   or codes: w1 / w3 [N, K] for gate/up, w2 [N, K] (no w_b) for down
+  const int32_t* offsets;
+  const void* w_route;            // down: [rows] routing weights in A's row order
+  int64_t rows, N, K, E;          // N: act's width (inter) for gate/up, the hidden size for down
+  int dtype;                      // the 16-bit dtype of the GEMM's output
+  const char* noun;               // an expert's weight in the null-entry error
+
+  int linears() const { return static_cast<int>((kSwiGLU ? 2 : 1) * E); }
+  static int expert_of(int i) { return kSwiGLU ? i / 2 : i; }
+  // Expert linear i, from per-expert arrays x_a and (gate/up) x_b: w1 of expert e at 2e, w3 at
+  // 2e + 1; down: w2 of expert e at e.  Null when its array is.
+  template <class T>
+  static T linear(const T* x_a, const T* x_b, int i) {
+    const T* x = kSwiGLU && (i & 1) ? x_b : x_a;
+    return x ? x[expert_of(i)] : nullptr;
+  }
+  tc::MoeSegments segments() const { return {offsets, w_route, static_cast<int>(E)}; }
+
+  // bm x bn: the kernel's output tile; a gate/up tile holds bn / 2 columns of w1 and of w3.
+  int check_values(int64_t bm, int64_t bn) const {
+    LLMC_CHECK_ARG(E >= 1 && E <= LLMC_MOE_MAX_EXPERTS, "%s: %lld experts outside 1..%d", what, (long long)E,
+                   LLMC_MOE_MAX_EXPERTS);
+    LLMC_CHECK_ARG(rows >= 0 && N > 0 && K > 0, "%s: bad shape rows=%lld N=%lld K=%lld", what, (long long)rows,
+                   (long long)N, (long long)K);
+    LLMC_CHECK_ARG(rows < (1ll << 31) - bm, "%s: rows=%lld too large", what, (long long)rows);
+    if (kSwiGLU)
+      LLMC_CHECK_ARG(N % (bn / 2) == 0, "%s: inter=%lld must be a multiple of %lld", what, (long long)N,
+                     (long long)(bn / 2));
+    else
+      LLMC_CHECK_ARG(N % 8 == 0, "%s: N=%lld must be a multiple of 8", what, (long long)N);
+    LLMC_CHECK_ARG(dtype == LLMC_BF16 || dtype == LLMC_F16, "%s: dtype must be bf16 or fp16", what);
+    return LLMC_OK;
+  }
+  // n_tiles n-tiles per expert, and the unit count (ceil(rows / bm) + E) * n_tiles, which bounds
+  // the tiles of every segmentation of the rows.
+  int plan(int64_t bm, int64_t bn, int& n_tiles, int& units) const {
+    const int64_t nt = kSwiGLU ? N / (bn / 2) : (N + bn - 1) / bn;
+    const int64_t m_cols = (rows + bm - 1) / bm + E;
+    LLMC_CHECK_ARG(nt < (1ll << 31) && m_cols * nt < (1ll << 31), "%s: too many tiles", what);
+    n_tiles = static_cast<int>(nt);
+    units = static_cast<int>(m_cols * nt);
+    return LLMC_OK;
+  }
+  int check_pointers() const {
+    LLMC_CHECK_ARG(a && out && offsets && w_a && (kSwiGLU ? w_b != nullptr : w_route != nullptr),
+                   "%s: null pointer", what);
+    for (int i = 0; i < linears(); ++i)
+      LLMC_CHECK_ARG(linear(w_a, w_b, i), "%s: null %s of expert %d", what, noun, expert_of(i));
+    if (!aligned16(a) || !aligned16(out)) {
+      set_last_error("%s: activation and output pointers must be 16-byte aligned", what);
+      return LLMC_EALIGN;
+    }
+    for (int i = 0; i < linears(); ++i) {
+      if (!aligned16(linear(w_a, w_b, i))) {
+        set_last_error("%s: weight of expert %d not 16-byte aligned", what, expert_of(i));
+        return LLMC_EALIGN;
+      }
+    }
+    return LLMC_OK;
+  }
+  // The tensor map of every expert linear's [N, cols] weight (row stride cols), in linear()'s
+  // order; boxes of box_cols x (bn / 2) rows for gate/up (tc::moe_load_b), bn rows for down.
+  int encode_tmaps(CUtensorMap* maps, CUtensorMapDataType dt, uint32_t elem_bytes, uint64_t cols, int64_t bn,
+                   uint32_t box_cols, CUtensorMapSwizzle swizzle) const {
+    for (int i = 0; i < linears(); ++i)
+      if (int rc = encode_tmap_2d(&maps[i], linear(w_a, w_b, i), dt, elem_bytes, N, cols, cols,
+                                  static_cast<uint32_t>(kSwiGLU ? bn / 2 : bn), box_cols, swizzle))
+        return rc;
+    return LLMC_OK;
+  }
+};
 
 // tf32.cu: 3xTF32 rank-K updates (see there) and the tf32 split hi = tf32(x), lo = tf32(x - hi).
 // tf32_split(x) is that split of one element (.x = hi, .y = lo), tf32 rounding to nearest with

@@ -224,14 +224,13 @@ def moe_forward(x, sel, w, experts):
     csrc/gemm_8bit.cu, each fed by one activation-quantiser pass).  Bit for bit the eager loop
     (MixtralSparseMoe.expert_loop), with no host sync."""
     require_cuda(x, sel, w)
-    T, K = x.shape
-    k, E = sel.shape[1], len(experts)
-    packed = isinstance(experts[0][0], PackedOperands)
-    w8a8 = isinstance(experts[0][0], W8A8Operands)
-    inter, N = ((experts[0][0].wq.shape[0], experts[0][2].wq.shape[0]) if packed
-                else (experts[0][0].w.shape[0], experts[0][2].w.shape[0]) if w8a8
-                else (experts[0][0].shape[0], experts[0][2].shape[0]))
+    T, k, E = x.shape[0], sel.shape[1], len(experts)
     assert E <= MOE_MAX_EXPERTS and w.dtype == x.dtype
+    o1, o2 = experts[0][0], experts[0][2]
+    gemms = (_moe_packed_gemms if isinstance(o1, PackedOperands)
+             else _moe_w8a8_gemms if isinstance(o1, W8A8Operands) else _moe_dense_gemms)
+    # one row per output feature: the dense weight, or the codes heading both operand tuples
+    inter, N = ((o if isinstance(o, torch.Tensor) else o[0]).shape[0] for o in (o1, o2))
     perm, offsets, rows = moe_routing(sel, E)
     xp = x.index_select(0, perm // k)
     w_route = w.reshape(-1).index_select(0, perm)
@@ -239,24 +238,9 @@ def moe_forward(x, sel, w, experts):
     act = torch.empty((M, inter), dtype=x.dtype, device=x.device)
     y = torch.empty((M, N), dtype=x.dtype, device=x.device)
     out = torch.empty((T, N), dtype=x.dtype, device=x.device)
-    dt, st = dtype_enum(x.dtype), stream_ptr(x.device)
-    if packed:
-        _moe_packed_gemms(xp, experts, offsets, w_route, act, y, M, inter, N, K, E, dt, st)
-    elif w8a8:
-        _moe_w8a8_gemms(xp, experts, sel.reshape(-1).index_select(0, perm), offsets, w_route, act, y, M, inter,
-                        N, K, E, dt, st)
-    else:
-        ws = [[t.contiguous() for t in e] for e in experts]
-        w1, w3, w2 = ((ctypes.c_void_p * E)(*[e[i].data_ptr() for e in ws]) for i in range(3))
-        with TIMER.span('moe_gemm_swiglu', flops=2.0 * M * 2 * inter * K,
-                        nbytes=2.0 * (M * K + E * 2 * inter * K + M * inter)):
-            call('llmc_moe_gemm_swiglu', ptr(xp), w1, w3, ptr(offsets), ptr(act), M, inter, K, E, dt, st)
-        with TIMER.span('moe_gemm_down', flops=2.0 * M * N * inter,
-                        nbytes=2.0 * (M * inter + E * N * inter + M * N + M)):
-            call('llmc_moe_gemm_down', ptr(act), w2, ptr(offsets), ptr(w_route), ptr(y), M, N, inter, E,
-                 dt, st)
+    gemms(xp, experts, sel, perm, offsets, w_route, act, y)
     with TIMER.span('moe_combine', nbytes=2.0 * (M * N + T * N) + 8.0 * M):
-        call('llmc_moe_combine', ptr(y), ptr(rows), ptr(out), T, k, N, dt, st)
+        call('llmc_moe_combine', ptr(y), ptr(rows), ptr(out), T, k, N, dtype_enum(x.dtype), stream_ptr(x.device))
     return out
 
 
@@ -274,12 +258,38 @@ def packed_qparams(dtype, scales, zeros, N, qparams_t):
     return s, z
 
 
-def _moe_packed_gemms(xp, experts, offsets, w_route, act, y, M, inter, N, K, E, dt, st):
-    """moe_forward's two GEMMs on PackedOperands experts: llmc_moe_gemm_packed_swiglu and
-    llmc_moe_gemm_packed_down, one form per launch."""
-    def arr(i, field):
-        ts = [getattr(e[i], field) for e in experts]
-        return None if ts[0] is None else (ctypes.c_void_p * E)(*[t.data_ptr() for t in ts])
+# moe_forward's GEMM pair, one per operand type.  Each takes the routed rows xp [M, K] (expert e's at
+# offsets[e]:offsets[e+1]), the experts' (w1, w3, w2) operands, sel [T, k] and perm (moe_routing),
+# the routing weights w_route [M] in xp's row order, and fills act [M, inter] and y [M, N].
+def _moe_shapes(xp, experts, act, y):
+    """M, K, inter, N, E, the dtype enum and the stream of a GEMM pair's launches."""
+    return (*xp.shape, act.shape[1], y.shape[1], len(experts), dtype_enum(xp.dtype), stream_ptr(xp.device))
+
+
+def _expert_ptrs(experts, i, field=None):
+    """A HOST array of the experts' device pointers to operand i (or to its `field`); None when expert
+    0's is None (the entry point's "none of them")."""
+    ts = [e[i] if field is None else getattr(e[i], field) for e in experts]
+    return None if ts[0] is None else (ctypes.c_void_p * len(ts))(*[t.data_ptr() for t in ts])
+
+
+def _moe_dense_gemms(xp, experts, sel, perm, offsets, w_route, act, y):
+    """Dense weights: llmc_moe_gemm_swiglu and llmc_moe_gemm_down."""
+    M, K, inter, N, E, dt, st = _moe_shapes(xp, experts, act, y)
+    ws = [[t.contiguous() for t in e] for e in experts]
+    w1, w3, w2 = (_expert_ptrs(ws, i) for i in range(3))
+    with TIMER.span('moe_gemm_swiglu', flops=2.0 * M * 2 * inter * K,
+                    nbytes=2.0 * (M * K + E * 2 * inter * K + M * inter)):
+        call('llmc_moe_gemm_swiglu', ptr(xp), w1, w3, ptr(offsets), ptr(act), M, inter, K, E, dt, st)
+    with TIMER.span('moe_gemm_down', flops=2.0 * M * N * inter,
+                    nbytes=2.0 * (M * inter + E * N * inter + M * N + M)):
+        call('llmc_moe_gemm_down', ptr(act), w2, ptr(offsets), ptr(w_route), ptr(y), M, N, inter, E, dt, st)
+
+
+def _moe_packed_gemms(xp, experts, sel, perm, offsets, w_route, act, y):
+    """PackedOperands: llmc_moe_gemm_packed_swiglu and llmc_moe_gemm_packed_down, one form per launch."""
+    M, K, inter, N, E, dt, st = _moe_shapes(xp, experts, act, y)
+    arr = partial(_expert_ptrs, experts)
 
     def weight_bytes(o):                 # codes, qparams and g_idx of one expert linear
         q = o.scales.numel() * o.scales.element_size() * (1 if o.zeros is None else 2)
@@ -304,20 +314,20 @@ def _moe_packed_gemms(xp, experts, offsets, w_route, act, y, M, inter, N, K, E, 
              arr(2, 'g_idx'), qd2, grp2, ng2, ptr(offsets), ptr(w_route), ptr(y), M, N, inter, E, dt, st)
 
 
-def _moe_w8a8_gemms(xp, experts, expert_of_row, offsets, w_route, act, y, M, inter, N, K, E, dt, st):
-    """moe_forward's two GEMMs on W8A8Operands experts: xp quantised once by w1's activation quantizer,
-    llmc_moe_gemm_w8a8_swiglu, act quantised once by w2's, llmc_moe_gemm_w8a8_down.  Per-token dynamic
-    activations take the quantiser's per-token pass over all rows (each row's codes and scale depend
-    on that row alone); static ones its per-tensor pass with one scale per row, the input_scale of the
-    row's expert (expert_of_row [M]: the expert of each of xp's rows), gathered on the device."""
+def _moe_w8a8_gemms(xp, experts, sel, perm, offsets, w_route, act, y):
+    """W8A8Operands: xp quantised once by w1's activation quantizer, llmc_moe_gemm_w8a8_swiglu, act
+    quantised once by w2's, llmc_moe_gemm_w8a8_down.  Per-token dynamic activations take the
+    quantiser's per-token pass over all rows (each row's codes and scale depend on that row alone);
+    static ones its per-tensor pass with one scale per row, the input_scale of the row's expert,
+    gathered on the device."""
+    M, K, inter, N, E, dt, st = _moe_shapes(xp, experts, act, y)
+    expert_of_row = sel.reshape(-1).index_select(0, perm)
     if M == 0:
         return
     o1 = experts[0][0]
     fp8 = int(o1.w.dtype == torch.float8_e4m3fn)
     stride = int(o1.s_w.numel() != 1)
-
-    def arr(i, field):
-        return (ctypes.c_void_p * E)(*[getattr(e[i], field).data_ptr() for e in experts])
+    arr = partial(_expert_ptrs, experts)
 
     def quantise(a, i):
         if experts[0][i].input_scale is None:

@@ -66,6 +66,9 @@ def test_dtypes(lib):
     assert _swiglu(lib, dtype=_lib.F32, qdt=_lib.F32) == -1 and 'dtype must be bf16 or fp16' in _last(lib)
     assert _down(lib, dtype=_lib.F32) == -1 and 'dtype must be bf16 or fp16' in _last(lib)
     assert _swiglu(lib, qdt=_lib.F16) == -1 and 'qparam_dtype' in _last(lib)
+    # scalar arguments are refused before the rows == 0 return
+    assert _swiglu(lib, rows=0, dtype=_lib.F32, qdt=_lib.F32) == -1 and 'dtype must be bf16 or fp16' in _last(lib)
+    assert _swiglu(lib, rows=0, qdt=_lib.F16) == -1 and 'qparam_dtype' in _last(lib)
 
 
 def test_null_arrays_and_entries_name_the_expert(lib):

@@ -121,8 +121,10 @@ def test_moe_argument_validation_without_gpu():
     w3[2] = None
     assert swiglu(p, w, w3, p, p, 256, 512, 256, 4, _lib.BF16, null) == -1
     assert 'null weight of expert 2' in last()
-    # fp32 is not a GEMM dtype
+    # fp32 is not a GEMM dtype, refused before the rows == 0 return like every scalar argument
     assert swiglu(p, w, w, p, p, 256, 512, 256, 4, _lib.F32, null) == -1
+    assert swiglu(null, w, w, null, null, 0, 512, 256, 4, _lib.F32, null) == -1
+    assert 'dtype must be bf16 or fp16' in last()
     # combine: N not a multiple of 8, top_k 0, dtype
     assert combine(p, p, p, 16, 2, 100, _lib.BF16, null) == -4
     assert combine(p, p, p, 16, 0, 128, _lib.BF16, null) == -1
