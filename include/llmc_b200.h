@@ -386,6 +386,24 @@ int llmc_moe_gemm_packed_down(const void* act, int bits, const int32_t* const* w
                               int64_t group, int64_t ng, const int32_t* offsets, const void* w_route, void* y,
                               int64_t rows, int64_t N, int64_t inter, int64_t n_experts, int dtype,
                               void* stream);
+/* The same pair on FP8 experts (the llmc_gemm_fp8a16 dequant GEMM, grouped): bit for bit the
+ * per-expert loop over llmc_gemm_fp8a16[_gidx] with the same operands.  e5m2 1: e5m2 bytes, 0:
+ * e4m3, for every expert linear alike.  Each expert linear's wq is its fp8 bytes [N_lin, K] viewed
+ * as int32 [N_lin, K/4]; dequant = rT(fmul_rn(fp32(byte), s)), s = 1 where the scale is 0.  No
+ * zero-point arguments; otherwise the operands, layouts and rules of the packed pair above (scales
+ * and g_idx HOST arrays of E device pointers, one form per call, rows == 0 a no-op, every argument
+ * error before any CUDA call, misalignment LLMC_EALIGN).
+ *   llmc_moe_gemm_fp8a16_swiglu  act[rows, inter] = llmc_silu_mul(xp W1_e^T, xp W3_e^T) per segment.
+ *   llmc_moe_gemm_fp8a16_down    y[rows, N] = rT(rT(act W2_e^T) * w_route[row]) per segment; K = inter. */
+int llmc_moe_gemm_fp8a16_swiglu(const void* xp, int e5m2, const int32_t* const* wq1, const int32_t* const* wq3,
+                                const void* const* s1, const void* const* s3, const int32_t* const* gidx1,
+                                const int32_t* const* gidx3, int qparam_dtype, int64_t group, int64_t ng,
+                                const int32_t* offsets, void* act, int64_t rows, int64_t inter, int64_t K,
+                                int64_t n_experts, int dtype, void* stream);
+int llmc_moe_gemm_fp8a16_down(const void* act, int e5m2, const int32_t* const* wq2, const void* const* s2,
+                              const int32_t* const* gidx2, int qparam_dtype, int64_t group, int64_t ng,
+                              const int32_t* offsets, const void* w_route, void* y, int64_t rows, int64_t N,
+                              int64_t inter, int64_t n_experts, int dtype, void* stream);
 
 /* The same two grouped projections on W8A8 experts (the llmc_gemm_w8a8_i8 / _fp8 GEMM, grouped): bit
  * for bit the per-expert loop over llmc_gemm_w8a8_* with the same codes and scales, no bias.  fp8 0:

@@ -20,6 +20,21 @@ from .quant import IntegerQuantizer
 from .registry import ALGO_REGISTRY  # noqa: F401  (re-exported for algorithm modules)
 
 
+def _same_act_scale(a, b):
+    """Whether linears a and b hold one static activation scale (buf_act_scales_0).  Read once per
+    pair of buffer versions and cached on a, as synth._same_input_scale does, so that later forwards
+    do not synchronise."""
+    sa, sb = a.buf_act_scales_0, b.buf_act_scales_0
+    if sa is sb:
+        return True
+    key = (sa.data_ptr(), sa._version, sb.data_ptr(), sb._version)
+    cached = getattr(a, '_same_act_scale', None)
+    if cached is None or cached[0] != key:
+        cached = (key, sa.numel() == sb.numel() and torch.equal(sa.reshape(-1).float(), sb.reshape(-1).float()))
+        a._same_act_scale = cached
+    return cached[1]
+
+
 class AttrDict(dict):
     """The 10-line stand-in for easydict (not installed): cfg.quant.weight.bit style access."""
 
@@ -301,6 +316,47 @@ class BaseBlockwiseQuantization(BlockwiseOpt):
             return aquantizer.fake_quant_act_static(act, args)
         return aquantizer.fake_quant_act_dynamic(act)
 
+    def a_qdq_routed(self, linears, aquantizer):
+        """The routed twin of a_qdq, for a grouped MoE layer (module_utils.moe_forward): linears[e] are
+        the linears of expert e that take the same rows (w1 and w3, or w2).  Returns f(act,
+        expert_of_row) that gives, in one pass over the routed rows act [M, K] (expert_of_row [M] on
+        the device), what a_qdq(rows of e, m) gives every m in linears[e], bit for bit; or None when
+        one pass cannot:
+          dynamic, per_token / per_channel / per_group: every row's qparams come from that row alone,
+            so fake_quant_act_dynamic over all rows;
+          static, per_tensor, symmetric: the quantiser's static pass with one scale per row, the
+            buf_act_scales_0 of the row's expert gathered on the device (0-dim scales only, whose
+            arithmetic that pass restates).  qmin / qmax are the quantiser's own, the values
+            register_act_qparams stores.  The linears of one expert must hold one scale (read once
+            per buffer version, then cached), since each quantises the same rows.
+        Refused: per_tensor dynamic activations (the scale depends on the expert's whole segment),
+        asymmetric static ones and every other form."""
+        from .quant_float import FloatQuantizer
+        q = aquantizer
+        if type(q) not in (IntegerQuantizer, FloatQuantizer):
+            return None
+        if not self.act_static:
+            if q.granularity not in ('per_token', 'per_channel', 'per_group'):
+                return None
+            if type(q) is IntegerQuantizer and (q.calib_algo not in ('minmax', 'learnable') or not q.round_zp):
+                return None
+            return lambda act, expert_of_row: q.fake_quant_act_dynamic(act)
+        if q.granularity != 'per_tensor' or not q.sym:
+            return None
+        for ms in linears:
+            for m in ms:
+                sc = getattr(m, 'buf_act_scales_0', None)
+                if sc is None or sc.dim() != 0 or not sc.is_cuda or not sc.is_floating_point():
+                    return None
+            if not all(_same_act_scale(ms[0], m) for m in ms[1:]):
+                return None
+        first = [ms[0] for ms in linears]
+
+        def qdq(act, expert_of_row):
+            table = torch.stack([m.buf_act_scales_0.float() for m in first])
+            return q.fake_quant_act_static_rows(act, table.index_select(0, expert_of_row))
+        return qdq
+
     def w_packed(self, module, wquantizer):
         """K6 hand-off for EffcientFakeQuantLinear: the packed form of exactly what `w_qdq` would
         materialise, or None when this layer / quantizer is not a plain INT2 / INT3 / INT4 / INT8 group or
@@ -362,6 +418,11 @@ class BaseBlockwiseQuantization(BlockwiseOpt):
             owner = next(c for c in type(self).__mro__ if 'w_qdq' in c.__dict__)
             if 'w_packed' in owner.__dict__:
                 params['w_qdq'].packed = functools.partial(self.w_packed, wquantizer=self.wquantizer)
+            # the routed twin of a_qdq (a grouped MoE layer's activations in one pass), by the same
+            # rule: only the class that defines a_qdq knows what it computes
+            owner = next(c for c in type(self).__mro__ if 'a_qdq' in c.__dict__)
+            if params['a_qdq'] is not None and 'a_qdq_routed' in owner.__dict__:
+                params['a_qdq'].routed = functools.partial(self.a_qdq_routed, aquantizer=self.aquantizer)
         elif mode in _REALQUANT_LINEAR_MAP_:
             params['w_q'] = functools.partial(self.w_q, wquantizer=self.wquantizer)
             params['quant_config'] = self.quant_config

@@ -160,7 +160,8 @@ template <int kRz> using ParamsOf = std::conditional_t<kRz == kRzOff, Params, Pa
 // Grouped (sparse-MoE) mode (tc::MoeMode, on packed weights): the gate/up B tile is two 64-row
 // boxes of 2 KB (W4) / 4 KB (W8), whole swizzle atoms, so the dequant warps' row swizzle is
 // unchanged; rows 0..63 of the tile are w1's, 64..127 w3's.  The epilogue writes act =
-// silu(gate) * up for 64 columns (store_swiglu_m64n64).
+// silu(gate) * up for 64 columns (store_swiglu_m64n64).  FP8 grids run in it as in plain mode: the
+// W8 configuration on the bytes viewed as words, with no zero-point.
 // The grouped operands of one launch, per expert linear (tc::moe_load_b's order): its packed
 // codes' tensor map and its qparam and g_idx pointers.  Every linear of a launch has one form:
 // bits, qparam dtype and layout, zeros (all null: 2^(bits-1)) and g_idx (all null: contiguous
@@ -321,8 +322,9 @@ w4a16_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
   constexpr bool kAwq = kLayout == kPackAwq;
   static_assert(!kAwq || (kBits == 4 && !kGidx && kGrid == kGridInt && kRz == kRzOff),
                 "the AutoAWQ layout is a contiguous-group W4 form");
-  static_assert(kMoe == kMoeOff || ((kBits == 4 || kBits == 8) && kGrid == kGridInt && kRz == kRzOff && !kAwq),
-                "the grouped mode runs W4 / W8 integer codes in the LLMC_OUT_PACK_VLLM layout");
+  static_assert(kMoe == kMoeOff || ((kBits == 4 || kBits == 8) && (kGrid == kGridInt || kBits == 8) &&
+                                    kRz == kRzOff && !kAwq),
+                "the grouped mode runs W4 / W8 integer codes or fp8 bytes in the LLMC_OUT_PACK_VLLM layout");
   constexpr int DT = kBf16 ? LLMC_BF16 : LLMC_F16;
   constexpr int kLStages = C::kLStages;
   constexpr int kLBytes = C::kLBytes;
@@ -1175,7 +1177,7 @@ extern "C" int llmc_gemm_w8a16_rz(const void* x, const int32_t* wq, const float*
 
 // ---- grouped (sparse-MoE) mode on packed experts ---------------------------------------------
 // g: the checked qparam and g_idx pointers of every expert linear; its maps and segments are set here.
-template <int kBits, int kMoe>
+template <int kBits, int kGrid, int kMoe>
 static int launch_moe_packed(const MoeLaunch<kMoe>& m, w4::MoeW4Operands& g, int qparam_dtype, int64_t group,
                              int q_transposed, int64_t ng, int n_tiles, int units, void* stream) {
   using namespace w4;
@@ -1201,17 +1203,18 @@ static int launch_moe_packed(const MoeLaunch<kMoe>& m, w4::MoeW4Operands& g, int
   p.gn = l2_group_width(static_cast<int64_t>(BN) * m.K * kBits / 8 + 1, p.n_tiles_n);
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   const bool bf16 = m.dtype == LLMC_BF16;
-  auto kernel = gidx ? (bf16 ? w4a16_gemm_kernel<true, kBits, true, kGridInt, kRzOff, kPackK, kMoe>
-                             : w4a16_gemm_kernel<false, kBits, true, kGridInt, kRzOff, kPackK, kMoe>)
-                     : (bf16 ? w4a16_gemm_kernel<true, kBits, false, kGridInt, kRzOff, kPackK, kMoe>
-                             : w4a16_gemm_kernel<false, kBits, false, kGridInt, kRzOff, kPackK, kMoe>);
+  auto kernel = gidx ? (bf16 ? w4a16_gemm_kernel<true, kBits, true, kGrid, kRzOff, kPackK, kMoe>
+                             : w4a16_gemm_kernel<false, kBits, true, kGrid, kRzOff, kPackK, kMoe>)
+                     : (bf16 ? w4a16_gemm_kernel<true, kBits, false, kGrid, kRzOff, kPackK, kMoe>
+                             : w4a16_gemm_kernel<false, kBits, false, kGrid, kRzOff, kPackK, kMoe>);
   return launch_persistent(kernel, p.num_units, C::kThreads, C::kSmemBytes, st, tmA, CUtensorMap{}, p, g);
 }
 
 // Checks and launches the grouped packed GEMM over m.rows gathered rows (the codes are m's
-// weights); the *_a / *_b arrays are the qparams and g_idx of w_a / w_b.
+// weights); the *_a / *_b arrays are the qparams and g_idx of w_a / w_b.  grid: integer codes of
+// `bits` (4 or 8) with optional zeros, or fp8 bytes (kGridE4M3 / kGridE5M2, bits 8, no zeros).
 template <int kMoe>
-static int moe_packed(const MoeLaunch<kMoe>& m, int bits, const void* const* s_a, const void* const* s_b,
+static int moe_packed(const MoeLaunch<kMoe>& m, int bits, int grid, const void* const* s_a, const void* const* s_b,
                       const void* const* z_a, const void* const* z_b, const int32_t* const* g_a,
                       const int32_t* const* g_b, int qparam_dtype, int64_t group, int64_t ng, void* stream) {
   using namespace w4;
@@ -1258,8 +1261,10 @@ static int moe_packed(const MoeLaunch<kMoe>& m, int bits, const void* const* s_a
     }
   }
   const int qt = group < 0 ? 1 : 0;
-  if (bits == 4) return launch_moe_packed<4>(m, g, qparam_dtype, ag, qt, ng, n_tiles, units, stream);
-  return launch_moe_packed<8>(m, g, qparam_dtype, ag, qt, ng, n_tiles, units, stream);
+  if (grid == kGridE4M3) return launch_moe_packed<8, kGridE4M3>(m, g, qparam_dtype, ag, qt, ng, n_tiles, units, stream);
+  if (grid == kGridE5M2) return launch_moe_packed<8, kGridE5M2>(m, g, qparam_dtype, ag, qt, ng, n_tiles, units, stream);
+  if (bits == 4) return launch_moe_packed<4, kGridInt>(m, g, qparam_dtype, ag, qt, ng, n_tiles, units, stream);
+  return launch_moe_packed<8, kGridInt>(m, g, qparam_dtype, ag, qt, ng, n_tiles, units, stream);
 }
 
 // The packed codes arrays, as MoeLaunch's untyped per-expert weight arrays.
@@ -1273,7 +1278,7 @@ extern "C" int llmc_moe_gemm_packed_swiglu(const void* xp, int bits, const int32
                                            int64_t K, int64_t n_experts, int dtype, void* stream) {
   return moe_packed<kMoeSwiGLU>({"moe_gemm_packed_swiglu", xp, act, codes(wq1), codes(wq3), offsets, nullptr, rows,
                                  inter, K, n_experts, dtype, "codes or scales"},
-                                bits, s1, s3, z1, z3, gidx1, gidx3, qparam_dtype, group, ng, stream);
+                                bits, w4::kGridInt, s1, s3, z1, z3, gidx1, gidx3, qparam_dtype, group, ng, stream);
 }
 
 extern "C" int llmc_moe_gemm_packed_down(const void* act, int bits, const int32_t* const* wq2,
@@ -1283,5 +1288,37 @@ extern "C" int llmc_moe_gemm_packed_down(const void* act, int bits, const int32_
                                          int64_t n_experts, int dtype, void* stream) {
   return moe_packed<kMoeDown>({"moe_gemm_packed_down", act, y, codes(wq2), nullptr, offsets, w_route, rows, N, inter,
                                n_experts, dtype, "codes or scales"},
-                              bits, s2, nullptr, z2, nullptr, gidx2, nullptr, qparam_dtype, group, ng, stream);
+                              bits, w4::kGridInt, s2, nullptr, z2, nullptr, gidx2, nullptr, qparam_dtype, group, ng,
+                              stream);
+}
+
+// FP8 experts: the fp8 bytes [N_lin, K] of each expert linear viewed as int32 [N_lin, K/4], as
+// llmc_gemm_fp8a16; no zero-points.  e5m2 is checked with the other scalars, before rows == 0.
+static int fp8_grid(int e5m2) { return e5m2 == 1 ? w4::kGridE5M2 : w4::kGridE4M3; }
+
+extern "C" int llmc_moe_gemm_fp8a16_swiglu(const void* xp, int e5m2, const int32_t* const* wq1,
+                                           const int32_t* const* wq3, const void* const* s1, const void* const* s3,
+                                           const int32_t* const* gidx1, const int32_t* const* gidx3,
+                                           int qparam_dtype, int64_t group, int64_t ng, const int32_t* offsets,
+                                           void* act, int64_t rows, int64_t inter, int64_t K, int64_t n_experts,
+                                           int dtype, void* stream) {
+  const char* name = "moe_gemm_fp8a16_swiglu";
+  LLMC_CHECK_ARG(e5m2 == 0 || e5m2 == 1, "%s: e5m2 must be 0 (e4m3) or 1 (e5m2), got %d", name, e5m2);
+  return moe_packed<kMoeSwiGLU>({name, xp, act, codes(wq1), codes(wq3), offsets, nullptr, rows, inter, K, n_experts,
+                                 dtype, "codes or scales"},
+                                8, fp8_grid(e5m2), s1, s3, nullptr, nullptr, gidx1, gidx3, qparam_dtype, group, ng,
+                                stream);
+}
+
+extern "C" int llmc_moe_gemm_fp8a16_down(const void* act, int e5m2, const int32_t* const* wq2,
+                                         const void* const* s2, const int32_t* const* gidx2, int qparam_dtype,
+                                         int64_t group, int64_t ng, const int32_t* offsets, const void* w_route,
+                                         void* y, int64_t rows, int64_t N, int64_t inter, int64_t n_experts,
+                                         int dtype, void* stream) {
+  const char* name = "moe_gemm_fp8a16_down";
+  LLMC_CHECK_ARG(e5m2 == 0 || e5m2 == 1, "%s: e5m2 must be 0 (e4m3) or 1 (e5m2), got %d", name, e5m2);
+  return moe_packed<kMoeDown>({name, act, y, codes(wq2), nullptr, offsets, w_route, rows, N, inter, n_experts, dtype,
+                               "codes or scales"},
+                              8, fp8_grid(e5m2), s2, nullptr, nullptr, nullptr, gidx2, nullptr, qparam_dtype, group,
+                              ng, stream);
 }

@@ -105,12 +105,19 @@ def dense_forward_weight(layer, dtype):
     linear_forward(x, W) (B200Linear's weight, FakeQuantLinear's cached tmp_weight, which this
     materialises as the first forward would); None for any other forward: activation fake-quant, a
     bias, a weight re-quantised every call, packed / FP8 / W8A8 deploys, hooks, a dtype mismatch."""
+    if getattr(layer, 'a_qdq', None) is not None:
+        return None
+    return _dense_weight(layer, dtype)
+
+
+def _dense_weight(layer, dtype):
+    """dense_forward_weight's weight of a B200Linear or FakeQuantLinear whatever its a_qdq: the
+    linear_forward that follows the activation fake-quant."""
     from .synth import B200Linear
     if layer._forward_hooks or layer._forward_pre_hooks:
         return None
     if type(layer) is FakeQuantLinear:
-        if (layer.a_qdq is not None or layer.bias is not None or layer.dynamic_quant_weight
-                or layer.dynamic_quant_tmp_weight):
+        if layer.bias is not None or layer.dynamic_quant_weight or layer.dynamic_quant_tmp_weight:
             return None
         if not hasattr(layer, 'tmp_weight'):
             layer.register_buffer('tmp_weight', layer.w_qdq(layer), persistent=False)
@@ -140,13 +147,7 @@ def packed_forward_operands(layer, dtype):
     if layer._forward_hooks or layer._forward_pre_hooks or getattr(layer, 'bias', None) is not None:
         return None
     if type(layer) is EffcientFakeQuantLinear:
-        if (not layer.packed or layer.q_grid != 'int' or layer.q_rz or layer.q_bits not in (4, 8)
-                or layer.a_qdq is not None):
-            return None
-        N = layer.qweight.shape[0]
-        s, z = packed_qparams(dtype, layer.qscales_t, layer.qzeros_t, N, True)
-        g = layer.g_idx.contiguous() if layer.g_idx is not None else None
-        return PackedOperands(layer.qweight.contiguous(), s, z, layer.q_bits, layer.q_group, g, True)
+        return _packed_int_operands(layer, dtype) if layer.a_qdq is None else None
     if isinstance(layer, VllmRealQuantLinear) and 'weight_packed' in layer._buffers:
         if layer.packed_unsupported() is not None:
             return None
@@ -155,6 +156,48 @@ def packed_forward_operands(layer, dtype):
         return PackedOperands(wq.contiguous(), s, None, 32 * wq.shape[1] // K, K // layer.weight_scale.shape[1],
                               None, False)
     return None
+
+
+def _packed_int_operands(layer, dtype):
+    """The PackedOperands of an EffcientFakeQuantLinear on 4- / 8-bit integer codes with integer
+    zero-points, whatever its a_qdq; else None."""
+    if not layer.packed or layer.q_grid != 'int' or layer.q_rz or layer.q_bits not in (4, 8):
+        return None
+    N = layer.qweight.shape[0]
+    s, z = packed_qparams(dtype, layer.qscales_t, layer.qzeros_t, N, True)
+    g = layer.g_idx.contiguous() if layer.g_idx is not None else None
+    return PackedOperands(layer.qweight.contiguous(), s, z, layer.q_bits, layer.q_group, g, True)
+
+
+Fp8Operands = namedtuple('Fp8Operands', 'wq scales zeros bits group g_idx transposed e5m2')
+Fp8Operands.__doc__ = """What an FP8-grid EffcientFakeQuantLinear's forward hands to llmc_gemm_fp8a16[_gidx]: its
+fp8 bytes [N, K] viewed as int32 wq [N, K/4], scales [ng, N] in the activation dtype or fp32
+(`transposed`), the group size, g_idx (None: contiguous groups) and e5m2 (0: e4m3).  zeros (None)
+and bits (8) make it read like PackedOperands."""
+
+
+def fake_quant_forward_operands(layer, dtype):
+    """(weight operands, a_qdq) of a fake-quant linear whose forward on an input x of `dtype` is
+    exactly a_qdq(x, layer) (when a_qdq is not None) followed by one GEMM on those operands, else
+    None: a FakeQuantLinear's dense tmp_weight (_dense_weight), a packed INT4 / INT8
+    EffcientFakeQuantLinear's PackedOperands, or an FP8-grid one's Fp8Operands (linear_forward_fp8w);
+    no bias or hooks.  The device is the caller's to check."""
+    if layer._forward_hooks or layer._forward_pre_hooks or getattr(layer, 'bias', None) is not None:
+        return None
+    if type(layer) is FakeQuantLinear:
+        w = _dense_weight(layer, dtype)
+    elif type(layer) is EffcientFakeQuantLinear and layer.packed and not layer.q_rz and layer.q_grid != 'int':
+        N = layer.qweight.shape[0]
+        qdt = dtype if layer.qscales_t.dtype == dtype else torch.float32
+        s = layer.qscales_t.reshape(-1, N).to(qdt).contiguous()
+        g = layer.g_idx.contiguous() if layer.g_idx is not None else None
+        w = Fp8Operands(layer.qweight.contiguous().view(torch.int32), s, None, 8, layer.q_group, g, True,
+                        int(layer.qweight.dtype == torch.float8_e5m2))
+    elif type(layer) is EffcientFakeQuantLinear:
+        w = _packed_int_operands(layer, dtype)
+    else:
+        return None
+    return None if w is None else (w, layer.a_qdq)
 
 
 W8A8Operands = namedtuple('W8A8Operands', 'w s_w aq input_scale act_cfg')
@@ -213,21 +256,25 @@ def moe_routing(sel, n_experts):
     return perm, offsets, rows
 
 
-def moe_forward(x, sel, w, experts):
+def moe_forward(x, sel, w, experts, a_qdq=None):
     """A Mixtral sparse-MoE layer's expert part, out[t] = sum over slots s of
     expert_{sel[t, s]}(x[t]) * w[t, s] with expert(x) = w2(silu(w1 x) * w3 x), as three launches:
     the grouped gate/up GEMM with SiLU-mul in its epilogue, the grouped down GEMM that scales each
     row by its routing weight, and the combine.  x [T, H] and w [T, k] of a 16-bit dtype, sel [T, k]
     int64, experts = one (w1, w3, w2) triple per expert (at most MOE_MAX_EXPERTS): dense weights,
     PackedOperands of one form (packed_forward_operands; the grouped dequant GEMMs of
-    csrc/gemm_w4.cu) or W8A8Operands of one form (w8a8_forward_operands; the grouped W8A8 GEMMs of
-    csrc/gemm_8bit.cu, each fed by one activation-quantiser pass).  Bit for bit the eager loop
-    (MixtralSparseMoe.expert_loop), with no host sync."""
+    csrc/gemm_w4.cu), Fp8Operands of one form (fake_quant_forward_operands; the same GEMMs on fp8
+    bytes) or W8A8Operands of one form (w8a8_forward_operands; the grouped W8A8 GEMMs of
+    csrc/gemm_8bit.cu, each fed by one activation-quantiser pass).  a_qdq: None, or the activation
+    fake-quant of the experts' linears as a pair of routed twins (blockwise.a_qdq_routed), applied
+    to the routed rows before gate/up and to act before the down projection.  Bit for bit the eager
+    loop (MixtralSparseMoe.expert_loop), with no host sync."""
     require_cuda(x, sel, w)
     T, k, E = x.shape[0], sel.shape[1], len(experts)
     assert E <= MOE_MAX_EXPERTS and w.dtype == x.dtype
     o1, o2 = experts[0][0], experts[0][2]
     gemms = (_moe_packed_gemms if isinstance(o1, PackedOperands)
+             else _moe_fp8_gemms if isinstance(o1, Fp8Operands)
              else _moe_w8a8_gemms if isinstance(o1, W8A8Operands) else _moe_dense_gemms)
     # one row per output feature: the dense weight, or the codes heading both operand tuples
     inter, N = ((o if isinstance(o, torch.Tensor) else o[0]).shape[0] for o in (o1, o2))
@@ -238,7 +285,12 @@ def moe_forward(x, sel, w, experts):
     act = torch.empty((M, inter), dtype=x.dtype, device=x.device)
     y = torch.empty((M, N), dtype=x.dtype, device=x.device)
     out = torch.empty((T, N), dtype=x.dtype, device=x.device)
-    gemms(xp, experts, sel, perm, offsets, w_route, act, y)
+    qdq_act = None
+    if a_qdq is not None and M > 0:
+        expert_of_row = sel.reshape(-1).index_select(0, perm)
+        xp = a_qdq[0](xp, expert_of_row)
+        qdq_act = partial(a_qdq[1], expert_of_row=expert_of_row)
+    gemms(xp, experts, sel, perm, offsets, w_route, act, y, qdq_act)
     with TIMER.span('moe_combine', nbytes=2.0 * (M * N + T * N) + 8.0 * M):
         call('llmc_moe_combine', ptr(y), ptr(rows), ptr(out), T, k, N, dtype_enum(x.dtype), stream_ptr(x.device))
     return out
@@ -260,7 +312,8 @@ def packed_qparams(dtype, scales, zeros, N, qparams_t):
 
 # moe_forward's GEMM pair, one per operand type.  Each takes the routed rows xp [M, K] (expert e's at
 # offsets[e]:offsets[e+1]), the experts' (w1, w3, w2) operands, sel [T, k] and perm (moe_routing),
-# the routing weights w_route [M] in xp's row order, and fills act [M, inter] and y [M, N].
+# the routing weights w_route [M] in xp's row order, and fills act [M, inter] and y [M, N].  The
+# down projection reads mid(act) when mid (a function of act alone) is given, else act.
 def _moe_shapes(xp, experts, act, y):
     """M, K, inter, N, E, the dtype enum and the stream of a GEMM pair's launches."""
     return (*xp.shape, act.shape[1], y.shape[1], len(experts), dtype_enum(xp.dtype), stream_ptr(xp.device))
@@ -273,7 +326,11 @@ def _expert_ptrs(experts, i, field=None):
     return None if ts[0] is None else (ctypes.c_void_p * len(ts))(*[t.data_ptr() for t in ts])
 
 
-def _moe_dense_gemms(xp, experts, sel, perm, offsets, w_route, act, y):
+def _down_input(act, mid):
+    return act if mid is None else mid(act)
+
+
+def _moe_dense_gemms(xp, experts, sel, perm, offsets, w_route, act, y, mid=None):
     """Dense weights: llmc_moe_gemm_swiglu and llmc_moe_gemm_down."""
     M, K, inter, N, E, dt, st = _moe_shapes(xp, experts, act, y)
     ws = [[t.contiguous() for t in e] for e in experts]
@@ -281,12 +338,13 @@ def _moe_dense_gemms(xp, experts, sel, perm, offsets, w_route, act, y):
     with TIMER.span('moe_gemm_swiglu', flops=2.0 * M * 2 * inter * K,
                     nbytes=2.0 * (M * K + E * 2 * inter * K + M * inter)):
         call('llmc_moe_gemm_swiglu', ptr(xp), w1, w3, ptr(offsets), ptr(act), M, inter, K, E, dt, st)
+    a2 = _down_input(act, mid)
     with TIMER.span('moe_gemm_down', flops=2.0 * M * N * inter,
                     nbytes=2.0 * (M * inter + E * N * inter + M * N + M)):
-        call('llmc_moe_gemm_down', ptr(act), w2, ptr(offsets), ptr(w_route), ptr(y), M, N, inter, E, dt, st)
+        call('llmc_moe_gemm_down', ptr(a2), w2, ptr(offsets), ptr(w_route), ptr(y), M, N, inter, E, dt, st)
 
 
-def _moe_packed_gemms(xp, experts, sel, perm, offsets, w_route, act, y):
+def _moe_packed_gemms(xp, experts, sel, perm, offsets, w_route, act, y, mid=None):
     """PackedOperands: llmc_moe_gemm_packed_swiglu and llmc_moe_gemm_packed_down, one form per launch."""
     M, K, inter, N, E, dt, st = _moe_shapes(xp, experts, act, y)
     arr = partial(_expert_ptrs, experts)
@@ -308,18 +366,48 @@ def _moe_packed_gemms(xp, experts, sel, perm, offsets, w_route, act, y):
         call('llmc_moe_gemm_packed_swiglu', ptr(xp), bits, arr(0, 'wq'), arr(1, 'wq'), arr(0, 'scales'),
              arr(1, 'scales'), arr(0, 'zeros'), arr(1, 'zeros'), arr(0, 'g_idx'), arr(1, 'g_idx'), qd1, grp1, ng1,
              ptr(offsets), ptr(act), M, inter, K, E, dt, st)
+    a2 = _down_input(act, mid)
     with TIMER.span('moe_gemm_packed_down', flops=2.0 * M * N * inter,
                     nbytes=2.0 * (M * inter + M * N + M) + E * weight_bytes(g2)):
-        call('llmc_moe_gemm_packed_down', ptr(act), bits, arr(2, 'wq'), arr(2, 'scales'), arr(2, 'zeros'),
+        call('llmc_moe_gemm_packed_down', ptr(a2), bits, arr(2, 'wq'), arr(2, 'scales'), arr(2, 'zeros'),
              arr(2, 'g_idx'), qd2, grp2, ng2, ptr(offsets), ptr(w_route), ptr(y), M, N, inter, E, dt, st)
 
 
-def _moe_w8a8_gemms(xp, experts, sel, perm, offsets, w_route, act, y):
+def _moe_fp8_gemms(xp, experts, sel, perm, offsets, w_route, act, y, mid=None):
+    """Fp8Operands: llmc_moe_gemm_fp8a16_swiglu and llmc_moe_gemm_fp8a16_down, one form per launch."""
+    M, K, inter, N, E, dt, st = _moe_shapes(xp, experts, act, y)
+    arr = partial(_expert_ptrs, experts)
+
+    def weight_bytes(o):                 # bytes, scales and g_idx of one expert linear
+        return 4.0 * o.wq.numel() + o.scales.numel() * o.scales.element_size() + (
+            0 if o.g_idx is None else 4.0 * o.g_idx.numel())
+
+    def layout(o):
+        ng = o.scales.numel() // o.wq.shape[0]
+        return dtype_enum(o.scales.dtype), int(-o.group if o.transposed else o.group), ng
+
+    g1, g2 = experts[0][0], experts[0][2]
+    qd1, grp1, ng1 = layout(g1)
+    qd2, grp2, ng2 = layout(g2)
+    with TIMER.span('moe_gemm_fp8a16_swiglu', flops=2.0 * M * 2 * inter * K,
+                    nbytes=2.0 * (M * K + M * inter) + E * 2 * weight_bytes(g1)):
+        call('llmc_moe_gemm_fp8a16_swiglu', ptr(xp), g1.e5m2, arr(0, 'wq'), arr(1, 'wq'), arr(0, 'scales'),
+             arr(1, 'scales'), arr(0, 'g_idx'), arr(1, 'g_idx'), qd1, grp1, ng1, ptr(offsets), ptr(act), M, inter, K,
+             E, dt, st)
+    a2 = _down_input(act, mid)
+    with TIMER.span('moe_gemm_fp8a16_down', flops=2.0 * M * N * inter,
+                    nbytes=2.0 * (M * inter + M * N + M) + E * weight_bytes(g2)):
+        call('llmc_moe_gemm_fp8a16_down', ptr(a2), g2.e5m2, arr(2, 'wq'), arr(2, 'scales'),
+             arr(2, 'g_idx'), qd2, grp2, ng2, ptr(offsets), ptr(w_route), ptr(y), M, N, inter, E, dt, st)
+
+
+def _moe_w8a8_gemms(xp, experts, sel, perm, offsets, w_route, act, y, mid=None):
     """W8A8Operands: xp quantised once by w1's activation quantizer, llmc_moe_gemm_w8a8_swiglu, act
     quantised once by w2's, llmc_moe_gemm_w8a8_down.  Per-token dynamic activations take the
     quantiser's per-token pass over all rows (each row's codes and scale depend on that row alone);
     static ones its per-tensor pass with one scale per row, the input_scale of the row's expert,
-    gathered on the device."""
+    gathered on the device.  Its activations are quantised here, so mid is None."""
+    assert mid is None
     M, K, inter, N, E, dt, st = _moe_shapes(xp, experts, act, y)
     expert_of_row = sel.reshape(-1).index_select(0, perm)
     if M == 0:

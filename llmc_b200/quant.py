@@ -588,6 +588,21 @@ class IntegerQuantizer(BaseQuantizer):
         t = self.quant_dequant(t, args['scales'], args['zeros'], args['qmax'], args['qmin'])
         return self.restore_tensor(t, org_shape).to(org_dtype)
 
+    def fake_quant_act_static_rows(self, act, scales):
+        """fake_quant_act_static of a per_tensor symmetric quantizer on a 0-dim scale, with one scale
+        per row of act instead (a grouped MoE layer's rows each under their expert's scale): the same
+        pass and arithmetic, _elementwise's fp32-scalar path (x / s in fp32 rounded to act's dtype)
+        with row stride 1 instead of 0, so row r is bit for bit what the 0-dim scales[r] gives it.
+        The zero-point of a symmetric grid is 0, which the kernel also reads for a null one."""
+        t2d = act.reshape(-1, act.shape[-1])
+        t2d = t2d if t2d.is_contiguous() else t2d.contiguous()
+        ct = t2d.dtype
+        rd = dtype_enum(ct) if ct != torch.float32 else -1
+        s = scales.reshape(-1).to(device=t2d.device, dtype=torch.float32).contiguous()
+        out = torch.empty(t2d.shape, dtype=ct, device=t2d.device)
+        self._static(t2d, s, None, self.qmax, self.qmin, OUT_QDQ, out, ct, 1, t2d.shape[1], round_dtype=rd)
+        return out.reshape(act.shape)
+
     def real_quant_act(self, act, input_scale=None):
         """The int8 codes and fp32 scales of the W8A8 real-quant forward (llmc_gemm_w8a8_i8): the codes
         the fake-quant forward of the same config rounds to, from the same pass, so rT(code * scale)

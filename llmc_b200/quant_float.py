@@ -190,6 +190,18 @@ class FloatQuantizer(BaseQuantizer):
         """quant.py:1083-1098."""
         return self._static(act, _zeros_to_one(args['scales']), 1).reshape(act.shape).to(act.dtype)
 
+    def fake_quant_act_static_rows(self, act, scales):
+        """fake_quant_act_static on a 0-dim scale, with one scale per row of act instead (a grouped MoE
+        layer's rows each under their expert's scale): the same llmc_fp8_quant pass in QDQ mode with
+        fp32 scales and row stride 1, as real_quant_act runs it for bytes, so row r is bit for bit what
+        the 0-dim scales[r] gives it.  Zero scales read as 1 (quant.py:1062) on a copy: the caller's
+        tensor is not modified."""
+        t2d = act.reshape(-1, act.shape[-1])
+        t2d = t2d if t2d.is_contiguous() else t2d.contiguous()
+        s = scales.reshape(-1).to(device=t2d.device, dtype=torch.float32, copy=True)
+        _zeros_to_one(s)
+        return self._run(t2d, t2d.shape[1], 0, s, 1, 1, 1).reshape(act.shape)
+
     def real_quant_act(self, act, input_scale=None):
         """The e4m3 bytes and fp32 scales of the W8A8 real-quant forward (llmc_gemm_w8a8_fp8): the bytes
         the fake-quant forward of the same config rounds to, from the same llmc_fp8_quant pass, so

@@ -10,6 +10,7 @@ and exported state-dict keys line up.
 """
 import math
 from collections import OrderedDict
+from functools import partial
 
 import torch
 import torch.nn as nn
@@ -18,7 +19,8 @@ import torch.nn.functional as F
 from ._lib import MOE_MAX_EXPERTS
 from .module_utils import (_LLMC_LINEAR_TYPES_, _TRANSFORMERS_LINEAR_TYPES_, dense_forward_weight,
                            gemm_rope_qkv, gemm_swiglu, interleave_gate_up, linear_forward,
-                           moe_forward, packed_forward_operands, w8a8_forward_operands)
+                           Fp8Operands, fake_quant_forward_operands, moe_forward, packed_forward_operands,
+                           w8a8_forward_operands)
 
 SHAPES = {
     # name: hidden, intermediate, layers, heads, kv_heads, vocab, kind, dtype
@@ -238,6 +240,42 @@ def _same_input_scale(a, b):
     return cached[1]
 
 
+def _dense_triple_form(ws, hidden):
+    """The form (inter) of one expert's dense (w1, w3, w2) forward weights when the grouped bf16
+    GEMMs take them for hidden size `hidden`, else None: none missing, 16-byte aligned, inter a
+    multiple of 128, shapes [inter, hidden] / [inter, hidden] / [hidden, inter]."""
+    if any(t is None or t.data_ptr() % 16 for t in ws):
+        return None
+    inter = ws[0].shape[0]
+    ok = inter % 128 == 0 and (ws[0].shape, ws[1].shape, ws[2].shape) == (
+        (inter, hidden), (inter, hidden), (hidden, inter))
+    return inter if ok else None
+
+
+def _packed_triple_form(triple, hidden):
+    """The form of one expert's (w1, w3, w2) PackedOperands / Fp8Operands when the grouped dequant
+    GEMMs take it for hidden size `hidden`, else None: codes of the right shape, 16-byte aligned,
+    inter and the groups multiples of 64, CUDA tensors, int32 g_idx of K entries, and w1 / w3 of one
+    form, w2 the same but its groups.  The form is per linear: (grid, bits, qparam dtype, zeros or
+    not, g_idx or not, layout, group, groups per row), then inter."""
+    inter = triple[0].wq.shape[0]
+    for o, (n, k) in zip(triple, ((inter, hidden), (inter, hidden), (hidden, inter))):
+        ng = o.scales.numel() // n
+        if (tuple(o.wq.shape) != (n, k * o.bits // 32) or o.wq.data_ptr() % 16
+                or inter % 64 or o.group % 64 or k % o.group or o.scales.numel() != n * ng):
+            return None
+        if not all(t.is_cuda for t in (o.wq, o.scales, o.zeros, o.g_idx) if t is not None):
+            return None
+        if o.g_idx is not None and (o.g_idx.dtype != torch.int32 or o.g_idx.numel() != k
+                                    or o.g_idx.data_ptr() % 16):
+            return None
+    f = tuple((getattr(o, 'e5m2', None), o.bits, o.scales.dtype, o.zeros is None, o.g_idx is None, o.transposed,
+               o.group, o.scales.numel() // o.wq.shape[0]) for o in triple)
+    if f[0] != f[1] or f[0][:6] != f[2][:6]:          # w1 / w3 one form, w2 the same but its groups
+        return None
+    return f + (inter,)
+
+
 class MixtralSparseMoe(nn.Module):
     """Per-expert nn.Linear layout the reference's wrapper expects (models/mixtral.py:43-86:
     block_sparse_moe.gate / experts[i].w1|w2|w3); the installed transformers 5.x fuses the experts,
@@ -279,20 +317,15 @@ class MixtralSparseMoe(nn.Module):
         if (not x.is_cuda or x.dtype not in (torch.bfloat16, torch.float16)
                 or len(self.experts) > MOE_MAX_EXPERTS or x.shape[1] % 8):
             return None
-        weights = []
+        weights, form = [], None
         for ex in self.experts:
             if type(ex) is not MixtralExpert or ex._forward_hooks or ex._forward_pre_hooks:
                 return None
             ws = tuple(dense_forward_weight(m, x.dtype) for m in (ex.w1, ex.w3, ex.w2))
-            if any(t is None or t.data_ptr() % 16 for t in ws):
+            f = _dense_triple_form(ws, x.shape[1])
+            if f is None or (form is not None and f != form):
                 return None
-            if not weights:
-                inter, hidden = ws[0].shape
-                if inter % 128 or hidden != x.shape[1]:
-                    return None
-            if (ws[0].shape, ws[1].shape, ws[2].shape) != ((inter, hidden), (inter, hidden),
-                                                           (hidden, inter)):
-                return None
+            form = f
             weights.append(ws)
         return weights
 
@@ -314,24 +347,10 @@ class MixtralSparseMoe(nn.Module):
             triple = tuple(packed_forward_operands(m, x.dtype) for m in (ex.w1, ex.w3, ex.w2))
             if any(o is None for o in triple):
                 return None
-            inter = triple[0].wq.shape[0]
-            for o, (n, k) in zip(triple, ((inter, hidden), (inter, hidden), (hidden, inter))):
-                ng = o.scales.numel() // n
-                if (tuple(o.wq.shape) != (n, k * o.bits // 32) or o.wq.data_ptr() % 16
-                        or inter % 64 or o.group % 64 or k % o.group or o.scales.numel() != n * ng):
-                    return None
-                if not all(t.is_cuda for t in (o.wq, o.scales, o.zeros, o.g_idx) if t is not None):
-                    return None
-                if o.g_idx is not None and (o.g_idx.dtype != torch.int32 or o.g_idx.numel() != k
-                                            or o.g_idx.data_ptr() % 16):
-                    return None
-            f = tuple((o.bits, o.scales.dtype, o.zeros is None, o.g_idx is None, o.transposed, o.group,
-                       o.scales.numel() // o.wq.shape[0]) for o in triple)
-            if form is not None and f != form:
+            f = _packed_triple_form(triple, hidden)
+            if f is None or (form is not None and f != form):
                 return None
             form = f
-            if f[0] != f[1] or f[0][:5] != f[2][:5]:          # w1 / w3 one form, w2 the same but its groups
-                return None
             ops.append(triple)
         return ops
 
@@ -372,16 +391,71 @@ class MixtralSparseMoe(nn.Module):
             ops.append(triple)
         return ops
 
+    def grouped_fake_quant_operands(self, x):
+        """(experts, a_qdq) for module_utils.moe_forward when it computes exactly what expert_loop
+        computes on x, else None: the fake-quant forms the other selectors leave to the loop.  Every
+        expert a plain MixtralExpert without hooks; every linear's forward a_qdq then one GEMM
+        (module_utils.fake_quant_forward_operands: FakeQuantLinear's dense tmp_weight, packed INT4 /
+        INT8 or FP8-grid EffcientFakeQuantLinear, no bias or hooks), of one weight form with the
+        shapes its grouped GEMMs take, at most MOE_MAX_EXPERTS; and either
+          no activation fake-quant on any linear (FP8 weights only: the other two have their own
+          selectors), or
+          one a_qdq on all of them, the same bound method and arguments, whose class gives it a
+          routed twin (`a_qdq.routed`, blockwise.a_qdq_routed) that accepts the layer: one pass
+          over the routed rows before gate/up for every expert's w1 and w3, one over act before the
+          down projection for every w2.
+        a_qdq is then None, or the pair of those passes."""
+        if (not x.is_cuda or x.dtype not in (torch.bfloat16, torch.float16)
+                or len(self.experts) > MOE_MAX_EXPERTS or x.shape[1] % 8):
+            return None
+        hidden = x.shape[1]
+        ops, qdqs, form = [], [], None
+        for ex in self.experts:
+            if type(ex) is not MixtralExpert or ex._forward_hooks or ex._forward_pre_hooks:
+                return None
+            got = tuple(fake_quant_forward_operands(m, x.dtype) for m in (ex.w1, ex.w3, ex.w2))
+            if any(g is None for g in got):
+                return None
+            triple = tuple(g[0] for g in got)
+            kind = torch.Tensor if isinstance(triple[0], torch.Tensor) else type(triple[0])
+            if any(not isinstance(o, kind) for o in triple) or (kind is not torch.Tensor and hidden % 64):
+                return None
+            f = _dense_triple_form(triple, hidden) if kind is torch.Tensor else _packed_triple_form(triple, hidden)
+            if f is None or (form is not None and (kind, f) != form):
+                return None
+            form = (kind, f)
+            ops.append(triple)
+            qdqs.extend(g[1] for g in got)
+        a0 = qdqs[0]
+        if a0 is None:
+            return (ops, None) if form[0] is Fp8Operands and all(a is None for a in qdqs) else None
+        routed = getattr(a0, 'routed', None)
+        if routed is None or not all(isinstance(a, partial) and a.func == a0.func and a.args == a0.args
+                                     and a.keywords == a0.keywords for a in qdqs):
+            return None
+        qdq_in = routed([(ex.w1, ex.w3) for ex in self.experts])
+        qdq_act = routed([(ex.w2,) for ex in self.experts])
+        if qdq_in is None or qdq_act is None:
+            return None
+        return ops, (qdq_in, qdq_act)
+
     def forward(self, hidden_states):
         B, S, H = hidden_states.shape
         x = hidden_states.reshape(-1, H)
         sel, w = self.route(x)
-        experts = self.grouped_weights(x)
+        experts, a_qdq = self.grouped_weights(x), None
         if experts is None:
             experts = self.grouped_packed_operands(x)
         if experts is None:
             experts = self.grouped_w8a8_operands(x)
-        out = self.expert_loop(x, sel, w) if experts is None else moe_forward(x, sel, w, experts)
+        if experts is None:
+            experts, a_qdq = self.grouped_fake_quant_operands(x) or (None, None)
+        if experts is None:
+            out = self.expert_loop(x, sel, w)
+        elif a_qdq is None:
+            out = moe_forward(x, sel, w, experts)
+        else:
+            out = moe_forward(x, sel, w, experts, a_qdq)
         return out.reshape(B, S, H)
 
 

@@ -2,7 +2,7 @@
 per-expert loop (MixtralSparseMoe.expert_loop) it replaces.
 
     python scripts/bench_moe.py [--reps 10] [--tokens 2048 65536] [--awq-samples 128] [--awq-rounds 3]
-                                [--packed] [--ppl-rounds 3] [--w8a8] [--out DIR]
+                                [--packed] [--ppl-rounds 3] [--w8a8] [--fake-quant] [--out DIR]
 
 1. One MoE layer (hidden 4096, inter 14336, 8 experts, top-2, bf16) at 2048 tokens (one GPTQ
    calibration forward at batch size 1) and 65536 tokens (the AWQ inspect batch, 128 x 512): the
@@ -27,6 +27,15 @@ over their real-quant forwards, for e4m3 per-tensor weights with static per-tens
 (configs/rtn_fp8_static_mixtral.yml), e4m3 per-channel with per-token dynamic activations and int8
 per-channel with per-token dynamic activations (random codes and scales), at each of `tokens`, timed
 as in 1.
+With --fake-quant, instead: the same layer with fake-quant experts under activation fake-quant
+(module_utils.fake_quant_forward_operands, the routed twin of blockwise's a_qdq) against the loop over
+their fake-quant forwards, for e4m3 per-tensor weights with static e4m3 activations
+(configs/rtn_fp8_static_mixtral.yml), e4m3 per-channel weights with per-token e4m3 activations and
+int8 per-channel weights with per-token int8 activations, weights quantised from random ones, static
+scales random per expert; at each of `tokens`, timed as in 1.  Then the fake-quant perplexity of a
+one-block Mixtral-8x7B-shaped model under configs/rtn_fp8_static_mixtral.yml (RTN with static
+calibration on 16 x 512 tokens, then 8 x 2048 eval tokens), grouped then loop for ppl_rounds
+alternated rounds as with --packed, with equal perplexities checked.
 Prints, and writes to DIR/bench_moe.json, one JSON object with the card name and power limit.
 """
 import argparse
@@ -210,6 +219,117 @@ def bench_w8a8_layer(res, tokens, reps):
         torch.cuda.empty_cache()
 
 
+# form: (weight quantizer, activation quantizer, static activations)
+FAKE_QUANT_FORMS = {
+    'e4m3_tensor_w_e4m3_static_a': ({'quant_type': 'float-quant', 'bit': 'e4m3', 'granularity': 'per_tensor'},
+                                    {'quant_type': 'float-quant', 'bit': 'e4m3', 'granularity': 'per_tensor',
+                                     'calib_algo': 'static_minmax'}, True),
+    'e4m3_channel_w_e4m3_token_a': ({'quant_type': 'float-quant', 'bit': 'e4m3', 'granularity': 'per_channel'},
+                                    {'quant_type': 'float-quant', 'bit': 'e4m3', 'granularity': 'per_token'}, False),
+    'int8_channel_w_int8_token_a': ({'bit': 8, 'granularity': 'per_channel'},
+                                    {'bit': 8, 'granularity': 'per_token'}, False),
+}
+
+
+def fake_quant_moe(form, g):
+    """The Mixtral-8x7B MoE layer (bf16) with every expert linear replaced as a fake-quant deploy
+    replaces it (EffcientFakeQuantLinear.new with blockwise's w_qdq / a_qdq), weights quantised from
+    random ones; static activation scales random per expert, w1's and w3's one tensor."""
+    from llmc_b200.blockwise import BaseBlockwiseQuantization
+    from llmc_b200.module_utils import EffcientFakeQuantLinear, act_quantizer
+    wcfg, acfg, static = FAKE_QUANT_FORMS[form]
+    fp8 = {'symmetric': True, 'use_qtorch': True}
+    wq = act_quantizer({**fp8, **wcfg} if 'quant_type' in wcfg else {'symmetric': True, **wcfg})
+    aq = act_quantizer({**fp8, **acfg} if 'quant_type' in acfg else {'symmetric': True, **acfg})
+    algo = object.__new__(BaseBlockwiseQuantization)
+    algo.wquantizer, algo.aquantizer, algo.act_static = wq, aq, static
+    params = algo.get_replacement_params('fake_quant')
+    s = synth.SHAPES['mixtral-8x7b']
+    with torch.device('meta'):
+        moe = MixtralSparseMoe(s['hidden'], s['inter'], s['experts'], s['top_k'])
+    moe = moe.to(torch.bfloat16).to_empty(device='cuda')
+    for p in moe.parameters():
+        p.data.normal_(0, 0.02, generator=g)
+    for ex in moe.experts:
+        s_in = torch.rand((), generator=g, device='cuda') * 0.02 + 0.01
+        for n in ('w1', 'w3', 'w2'):
+            m = EffcientFakeQuantLinear.new(getattr(ex, n), params['w_qdq'], params['a_qdq'])
+            if static:
+                sc = s_in if n != 'w2' else torch.rand((), generator=g, device='cuda') * 0.004 + 1e-3
+                m.register_buffer('buf_act_scales_0', sc)
+                m.register_buffer('buf_act_zeros_0', torch.tensor(0.0, device='cuda'))
+                m.register_buffer('buf_act_qmin_0', aq.qmin.to('cuda'))
+                m.register_buffer('buf_act_qmax_0', aq.qmax.to('cuda'))
+            setattr(ex, n, m)
+    return moe
+
+
+def bench_fake_quant_layer(res, tokens, reps):
+    s = synth.SHAPES['mixtral-8x7b']
+    H, I, k = s['hidden'], s['inter'], s['top_k']
+    g = torch.Generator(device='cuda').manual_seed(0)
+    for form in FAKE_QUANT_FORMS:
+        moe = fake_quant_moe(form, g)
+        for T in tokens:
+            hs = torch.randn(1, T, H, device='cuda', generator=g).to(torch.bfloat16)
+            assert moe.grouped_fake_quant_operands(hs.view(T, H)) is not None
+            compare_and_time(res, f'moe_layer[{form}, T={T}]', moe, hs, 2.0 * T * k * 3 * H * I, reps)
+            del hs
+            torch.cuda.empty_cache()
+        del moe
+        torch.cuda.empty_cache()
+
+
+def time_ppl(res, key, model, tokens, seq_len, rounds):
+    """Perplexity of `model` on `tokens`, grouped then loop for `rounds` alternated rounds after one
+    warm-up each, on a host clock that ends in a device synchronise; equal perplexities checked."""
+    saved = MixtralSparseMoe.forward
+
+    def run(loop):
+        if loop:
+            MixtralSparseMoe.forward = loop_forward
+        try:
+            torch.cuda.synchronize()
+            t0 = time.perf_counter()
+            ppl = synth.perplexity(model, tokens, seq_len, 1)
+            torch.cuda.synchronize()
+            return time.perf_counter() - t0, ppl
+        finally:
+            MixtralSparseMoe.forward = saved
+    run(False), run(True)                          # warm-up
+    times, ppls = {'grouped': [], 'loop': []}, {'grouped': set(), 'loop': set()}
+    for _ in range(rounds):
+        for path in times:
+            dt, ppl = run(path == 'loop')
+            times[path].append(round(dt, 3))
+            ppls[path].add(ppl)
+    assert ppls['grouped'] == ppls['loop'] and len(ppls['loop']) == 1, ppls
+    med = {n: statistics.median(v) for n, v in times.items()}
+    res['ppl_s'][key] = times
+    res['ppl_speedup'][key] = round(med['loop'] / med['grouped'], 3)
+    print(key, times, flush=True)
+
+
+def bench_fake_quant_ppl(res, rounds):
+    import yaml
+    from llmc_b200.blockwise import AttrDict
+    from llmc_b200.rtn import RTN
+    with open(os.path.join(ROOT, 'configs', 'rtn_fp8_static_mixtral.yml')) as fh:
+        cfg = AttrDict.wrap(yaml.safe_load(fh))
+    model = synth.SynthModel('mixtral-8x7b', n_layers=1, seed=0, device='cuda', init='device')
+    c = cfg.calib
+    inp = model.first_block_input(c.n_samples, c.seq_len, bs=c.bs, seed=1, device='cuda')
+    algo = RTN(model, cfg.quant, inp, None, cfg)
+    algo.run_block_loop()
+    algo.deploy('fake_quant')
+    del inp
+    x = torch.zeros(1, model.shape['hidden'], dtype=model.shape['dtype'], device='cuda')
+    assert all(blk.block_sparse_moe.grouped_fake_quant_operands(x) is not None for blk in model.get_blocks())
+    tokens = torch.randint(0, model.shape['vocab'], (1, 2048 * 8), generator=torch.Generator().manual_seed(4))
+    time_ppl(res, 'fake_quant_ppl[mixtral-8x7b 1 block, rtn_fp8_static_mixtral.yml, 8x2048 tokens]', model,
+             tokens, 2048, rounds)
+
+
 def bench_packed_ppl(res, rounds):
     from llmc_b200.blockwise import AttrDict
     from llmc_b200.rtn import RTN
@@ -302,12 +422,19 @@ def main():
     ap.add_argument('--awq-rounds', type=int, default=3)
     ap.add_argument('--packed', action='store_true')
     ap.add_argument('--w8a8', action='store_true')
+    ap.add_argument('--fake-quant', action='store_true')
     ap.add_argument('--ppl-rounds', type=int, default=3)
     ap.add_argument('--out', default=None)
     args = ap.parse_args()
     assert torch.cuda.is_available(), 'needs a CUDA device'
     res = {'card': card(), 'reps': args.reps, 'layer_ms': {}, 'layer_tflops': {}, 'layer_speedup': {}}
-    if args.w8a8:
+    if args.fake_quant:
+        res.update(ppl_s={}, ppl_speedup={})
+        with torch.no_grad():
+            bench_fake_quant_layer(res, args.tokens, args.reps)
+        if args.ppl_rounds > 0:
+            bench_fake_quant_ppl(res, args.ppl_rounds)
+    elif args.w8a8:
         with torch.no_grad():
             bench_w8a8_layer(res, args.tokens, args.reps)
     elif args.packed:
