@@ -341,16 +341,24 @@ int llmc_gemm_residual(const void* x, const void* w, const void* res, void* y, i
  *                     [inter, K], w2 [N, inter]
  * Launches are sized by the bound ceil(rows / 128) + E m-tiles per column of n-tiles.  Each
  * expert's weight has its own tensor map in the kernel's parameters, which caps the number of
- * experts at LLMC_MOE_MAX_EXPERTS; more return LLMC_EINVAL.  bf16 / fp16, pointers 16-byte
- * aligned, K a multiple of 8.
+ * experts at LLMC_MOE_MAX_EXPERTS; more return LLMC_EINVAL.  At 64 experts the largest argument
+ * list is about 20 KB, past the 4 KB kernel-parameter limit of older toolkits: the library needs
+ * CUDA 12.1 or later and a driver of R530 or later (32,764 parameter bytes on Volta and newer).
+ * bf16 / fp16, pointers 16-byte aligned, K a multiple of 8.
  *   llmc_moe_gemm_swiglu  act[rows, inter] = llmc_silu_mul(xp W1_e^T, xp W3_e^T) per segment;
  *                         inter a multiple of 128.
  *   llmc_moe_gemm_down    y[rows, N] = rT(rT(act W2_e^T) * w_route[row]) per segment; w_route
  *                         [rows] the routing weights in xp's row order (dtype); N a multiple of 8.
  *   llmc_moe_combine      out[T, N] = the sum of y's rows rows[t, 0], ..., rows[t, top_k - 1]
  *                         (int64 device array), added left to right with one rounding per add;
- *                         N a multiple of 8. */
-#define LLMC_MOE_MAX_EXPERTS 8
+ *                         N a multiple of 8.
+ *   llmc_moe_combine_shared  out[t] = rT(routed[t] + rT(rT(sigmoid(g[t])) * s[t])): routed[t] the
+ *                         sum llmc_moe_combine writes, g [T] the shared expert's gate logit (one per
+ *                         token, dtype), s [T, N] the shared expert's output; the roundings of
+ *                         Qwen2-MoE's block (index_add_ into zeros, F.sigmoid(gate(x)) * shared, the
+ *                         add).  top_k > 0, N a multiple of 8, pointers 16-byte aligned; scalar checks,
+ *                         then the T == 0 no-op, then pointer checks, all before any CUDA call. */
+#define LLMC_MOE_MAX_EXPERTS 64
 int llmc_moe_gemm_swiglu(const void* xp, const void* const* w1, const void* const* w3,
                          const int32_t* offsets, void* act, int64_t rows, int64_t inter, int64_t K,
                          int64_t n_experts, int dtype, void* stream);
@@ -359,6 +367,9 @@ int llmc_moe_gemm_down(const void* act, const void* const* w2, const int32_t* of
                        int64_t n_experts, int dtype, void* stream);
 int llmc_moe_combine(const void* y, const int64_t* rows, void* out, int64_t T, int64_t top_k,
                      int64_t N, int dtype, void* stream);
+int llmc_moe_combine_shared(const void* y, const int64_t* rows, const void* gate_logit,
+                            const void* shared, void* out, int64_t T, int64_t top_k, int64_t N,
+                            int dtype, void* stream);
 
 /* The same two grouped projections on PACKED experts (the llmc_gemm_w4a16 / w8a16 dequant GEMM,
  * grouped): bit for bit the per-expert loop over llmc_gemm_w{4,8}a16[_gidx] with the same operands.

@@ -272,6 +272,8 @@ __device__ __forceinline__ float fma_rn(float a, float b, float c) { return __fm
 // F.silu in fp32 (IEEE division), shared by llmc_silu_mul and the SwiGLU epilogue of the forward
 // GEMM, which must agree bit for bit.
 __device__ __forceinline__ float silu_f32(float x) { return x / (1.0f + expf(-x)); }
+// F.sigmoid in fp32 (torch's sigmoid kernel: 1 / (1 + exp(-x)), IEEE division).
+__device__ __forceinline__ float sigmoid_f32(float x) { return 1.0f / (1.0f + expf(-x)); }
 
 // One element of F.silu(gate) * up on DT tensors: silu in fp32 rounded to DT, the product in fp32,
 // which the caller's store rounds.  kRoundInputs: g and u are a GEMM epilogue's fp32 accumulators,

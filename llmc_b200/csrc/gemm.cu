@@ -79,9 +79,9 @@ struct MoeOperands {
   CUtensorMap tmB[2 * LLMC_MOE_MAX_EXPERTS];   // one per expert linear (tc::moe_load_b)
   MoeSegments seg;
 };
-// The whole argument list of the grouped kernel fits the 4 KB kernel-parameter space: that is what
-// caps the number of experts.
-static_assert(sizeof(CUtensorMap) + sizeof(MoeOperands) + sizeof(GemmParams) <= 4096,
+// The whole argument list of the grouped kernel fits the 32,764-byte kernel-parameter space of
+// CUDA 12.1+ (driver R530+): that is what caps the number of experts.
+static_assert(sizeof(CUtensorMap) + sizeof(MoeOperands) + sizeof(GemmParams) <= 32764,
               "LLMC_MOE_MAX_EXPERTS exceeds the kernel-parameter space");
 
 struct Unit {
@@ -597,10 +597,14 @@ static int launch_moe(const MoeLaunch<kMoe>& m, void* stream) {
 
 // out[t] = rT(...rT(rT(0 + y[rows[t, 0]]) + y[rows[t, 1]]) + ...): the k expert outputs of token t
 // added in the order given (ascending expert), as `zeros` + one index_add_ per expert does.
-template <int DT>
+// kShared (Qwen2-MoE's gated shared expert): then out[t] = rT(out[t] + rT(rT(sigmoid(g[t])) * s[t])),
+// the roundings of F.sigmoid(gate(x)) * shared_expert(x) and the add that follows.
+template <int DT, bool kShared>
 __global__ void __launch_bounds__(256)
 moe_combine_kernel(const void* __restrict__ y, const int64_t* __restrict__ rows,
+                   const void* __restrict__ g, const void* __restrict__ sh,
                    void* __restrict__ out, int64_t T, int64_t k, int64_t N) {
+  using D = DType<DT>;
   const int64_t chunks = N >> 3;
   for (int64_t i = static_cast<int64_t>(blockIdx.x) * blockDim.x + threadIdx.x; i < T * chunks;
        i += static_cast<int64_t>(gridDim.x) * blockDim.x) {
@@ -610,10 +614,32 @@ moe_combine_kernel(const void* __restrict__ y, const int64_t* __restrict__ rows,
       float v[8];
       load8<DT>(y, __ldg(rows + t * k + s) * N + ch * 8, v);
 #pragma unroll
-      for (int j = 0; j < 8; ++j) acc[j] = DType<DT>::rT(fadd_rn(acc[j], v[j]));
+      for (int j = 0; j < 8; ++j) acc[j] = D::rT(fadd_rn(acc[j], v[j]));
+    }
+    if constexpr (kShared) {
+      const float sg = D::rT(sigmoid_f32(D::load(g, t)));
+      float v[8];
+      load8<DT>(sh, i << 3, v);
+#pragma unroll
+      for (int j = 0; j < 8; ++j) acc[j] = D::rT(fadd_rn(acc[j], D::rT(fmul_rn(sg, v[j]))));
     }
     store8<DT>(out, i << 3, acc);
   }
+}
+
+// The launch behind llmc_moe_combine and llmc_moe_combine_shared (g, sh unused by the former), on
+// arguments its caller has checked: T > 0, N a multiple of 8.
+template <bool kShared>
+static int launch_moe_combine(const void* y, const int64_t* rows, const void* g, const void* sh, void* out,
+                              int64_t T, int64_t top_k, int64_t N, int dtype, void* stream) {
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  int64_t blocks = (T * (N >> 3) + 255) / 256;
+  if (blocks > kNumSMs * 32) blocks = kNumSMs * 32;
+#define CALL(DT) moe_combine_kernel<DT, kShared><<<(int)blocks, 256, 0, st>>>(y, rows, g, sh, out, T, top_k, N); \
+  LLMC_CHECK_LAUNCH()
+  if (dtype == LLMC_BF16) { CALL(LLMC_BF16); } else { CALL(LLMC_F16); }
+#undef CALL
+  return LLMC_OK;
 }
 
 }  // namespace llmc
@@ -645,13 +671,26 @@ extern "C" int llmc_moe_combine(const void* y, const int64_t* rows, void* out, i
                    (long long)N);
     return LLMC_EALIGN;
   }
-  cudaStream_t st = static_cast<cudaStream_t>(stream);
-  int64_t blocks = (T * (N >> 3) + 255) / 256;
-  if (blocks > kNumSMs * 32) blocks = kNumSMs * 32;
-#define CALL(DT) moe_combine_kernel<DT><<<(int)blocks, 256, 0, st>>>(y, rows, out, T, top_k, N); LLMC_CHECK_LAUNCH()
-  if (dtype == LLMC_BF16) { CALL(LLMC_BF16); } else { CALL(LLMC_F16); }
-#undef CALL
-  return LLMC_OK;
+  return launch_moe_combine<false>(y, rows, nullptr, nullptr, out, T, top_k, N, dtype, stream);
+}
+
+extern "C" int llmc_moe_combine_shared(const void* y, const int64_t* rows, const void* gate_logit,
+                                       const void* shared, void* out, int64_t T, int64_t top_k, int64_t N,
+                                       int dtype, void* stream) {
+  LLMC_CHECK_ARG(T >= 0 && top_k > 0 && N > 0, "moe_combine_shared: bad shape T=%lld top_k=%lld N=%lld",
+                 (long long)T, (long long)top_k, (long long)N);
+  LLMC_CHECK_ARG(dtype == LLMC_BF16 || dtype == LLMC_F16, "moe_combine_shared: dtype must be bf16 or fp16");
+  if (N % 8 != 0) {
+    set_last_error("moe_combine_shared: N=%lld must be a multiple of 8", (long long)N);
+    return LLMC_EALIGN;
+  }
+  if (T == 0) return LLMC_OK;
+  LLMC_CHECK_ARG(y && rows && gate_logit && shared && out, "moe_combine_shared: null pointer");
+  if (!aligned16(y) || !aligned16(shared) || !aligned16(out)) {
+    set_last_error("moe_combine_shared: y, shared and out must be 16-byte aligned");
+    return LLMC_EALIGN;
+  }
+  return launch_moe_combine<true>(y, rows, gate_logit, shared, out, T, top_k, N, dtype, stream);
 }
 
 extern "C" int llmc_gemm_bf16(const void* x, const void* w, const void* bias, void* y, int64_t M,

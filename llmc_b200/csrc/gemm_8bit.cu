@@ -104,9 +104,9 @@ struct MoeW8A8Operands {
   const float* s_w[2 * LLMC_MOE_MAX_EXPERTS];
   MoeSegments seg;
 };
-// The whole argument list of the grouped kernel fits the 4 KB kernel-parameter space at
-// LLMC_MOE_MAX_EXPERTS experts.
-static_assert(2 * sizeof(CUtensorMap) + sizeof(W8A8Params) + sizeof(MoeW8A8Operands) <= 4096,
+// The whole argument list of the grouped kernel fits the 32,764-byte kernel-parameter space of
+// CUDA 12.1+ (driver R530+) at LLMC_MOE_MAX_EXPERTS experts.
+static_assert(2 * sizeof(CUtensorMap) + sizeof(W8A8Params) + sizeof(MoeW8A8Operands) <= 32764,
               "LLMC_MOE_MAX_EXPERTS exceeds the kernel-parameter space");
 
 // Grouped mode: acc = fmul(fmul(acc, s_w[col]), s_x[row]) over this thread's part of an m64n128

@@ -173,9 +173,9 @@ struct MoeW4Operands {
   const int32_t* g_idx[2 * LLMC_MOE_MAX_EXPERTS];
   MoeSegments seg;
 };
-// The whole argument list of the grouped kernel fits the 4 KB kernel-parameter space at
-// LLMC_MOE_MAX_EXPERTS experts.
-static_assert(2 * sizeof(CUtensorMap) + sizeof(Params) + sizeof(MoeW4Operands) <= 4096,
+// The whole argument list of the grouped kernel fits the 32,764-byte kernel-parameter space of
+// CUDA 12.1+ (driver R530+) at LLMC_MOE_MAX_EXPERTS experts.
+static_assert(2 * sizeof(CUtensorMap) + sizeof(Params) + sizeof(MoeW4Operands) <= 32764,
               "LLMC_MOE_MAX_EXPERTS exceeds the kernel-parameter space");
 
 // (a & b) | c in one LOP3

@@ -256,8 +256,8 @@ def moe_routing(sel, n_experts):
     return perm, offsets, rows
 
 
-def moe_forward(x, sel, w, experts, a_qdq=None):
-    """A Mixtral sparse-MoE layer's expert part, out[t] = sum over slots s of
+def moe_forward(x, sel, w, experts, a_qdq=None, shared=None):
+    """A sparse-MoE layer's expert part, out[t] = sum over slots s of
     expert_{sel[t, s]}(x[t]) * w[t, s] with expert(x) = w2(silu(w1 x) * w3 x), as three launches:
     the grouped gate/up GEMM with SiLU-mul in its epilogue, the grouped down GEMM that scales each
     row by its routing weight, and the combine.  x [T, H] and w [T, k] of a 16-bit dtype, sel [T, k]
@@ -267,8 +267,10 @@ def moe_forward(x, sel, w, experts, a_qdq=None):
     bytes) or W8A8Operands of one form (w8a8_forward_operands; the grouped W8A8 GEMMs of
     csrc/gemm_8bit.cu, each fed by one activation-quantiser pass).  a_qdq: None, or the activation
     fake-quant of the experts' linears as a pair of routed twins (blockwise.a_qdq_routed), applied
-    to the routed rows before gate/up and to act before the down projection.  Bit for bit the eager
-    loop (MixtralSparseMoe.expert_loop), with no host sync."""
+    to the routed rows before gate/up and to act before the down projection.  shared: None, or
+    (gate_logit [T, 1], s [T, H]) of a gated shared expert (Qwen2-MoE), added by the combine as
+    out[t] + sigmoid(gate_logit[t]) * s[t] (llmc_moe_combine_shared).  Bit for bit the eager loop
+    (SparseMoe.expert_loop, then the shared expert's add), with no host sync."""
     require_cuda(x, sel, w)
     T, k, E = x.shape[0], sel.shape[1], len(experts)
     assert E <= MOE_MAX_EXPERTS and w.dtype == x.dtype
@@ -291,8 +293,27 @@ def moe_forward(x, sel, w, experts, a_qdq=None):
         xp = a_qdq[0](xp, expert_of_row)
         qdq_act = partial(a_qdq[1], expert_of_row=expert_of_row)
     gemms(xp, experts, sel, perm, offsets, w_route, act, y, qdq_act)
-    with TIMER.span('moe_combine', nbytes=2.0 * (M * N + T * N) + 8.0 * M):
-        call('llmc_moe_combine', ptr(y), ptr(rows), ptr(out), T, k, N, dtype_enum(x.dtype), stream_ptr(x.device))
+    if shared is None:
+        with TIMER.span('moe_combine', nbytes=2.0 * (M * N + T * N) + 8.0 * M):
+            call('llmc_moe_combine', ptr(y), ptr(rows), ptr(out), T, k, N, dtype_enum(x.dtype), stream_ptr(x.device))
+    else:
+        moe_combine_shared(y, rows, shared[0], shared[1], out)
+    return out
+
+
+def moe_combine_shared(y, rows, gate_logit, s, out):
+    """out [T, N] = rT(routed[t] + rT(rT(sigmoid(gate_logit[t])) * s[t])), routed[t] the sum of y's
+    rows rows[t, :] in that order (llmc_moe_combine): a Qwen2-MoE layer's routed experts plus its
+    gated shared expert.  y [M, N], rows [T, k] int64, gate_logit [T, 1] and s [T, N] of y's dtype."""
+    require_cuda(y, rows, gate_logit, s, out)
+    T, k = rows.shape
+    N = y.shape[1]
+    g, s = gate_logit.contiguous(), s.contiguous()
+    assert g.numel() == T and s.shape == (T, N) and out.shape == (T, N)
+    assert g.dtype == s.dtype == out.dtype == y.dtype and out.is_contiguous()
+    with TIMER.span('moe_combine_shared', nbytes=2.0 * (y.shape[0] * N + 2 * T * N + T) + 8.0 * T * k):
+        call('llmc_moe_combine_shared', ptr(y), ptr(rows), ptr(g), ptr(s), ptr(out), T, k, N,
+             dtype_enum(y.dtype), stream_ptr(y.device))
     return out
 
 

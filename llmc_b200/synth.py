@@ -36,6 +36,14 @@ SHAPES = {
                          kind='mixtral', dtype=torch.bfloat16, experts=8, top_k=2),
     'tiny-mixtral': dict(hidden=256, inter=512, layers=2, heads=4, kv_heads=2, vocab=512,
                          kind='mixtral', dtype=torch.bfloat16, experts=4, top_k=2),
+    # Qwen1.5-MoE-A2.7B: transformers' Qwen2MoeConfig defaults (every layer sparse, q/k/v with bias);
+    # inter is the dense intermediate size the config states, moe_inter / shared_inter the experts'
+    'qwen1.5-moe-a2.7b': dict(hidden=2048, inter=5632, layers=24, heads=16, kv_heads=16, vocab=151936,
+                              kind='qwen2moe', dtype=torch.bfloat16, experts=60, top_k=4, moe_inter=1408,
+                              shared_inter=5632, rope_theta=1000000.0, rms_eps=1e-6),
+    'tiny-qwen-moe': dict(hidden=256, inter=512, layers=2, heads=4, kv_heads=4, vocab=512,
+                          kind='qwen2moe', dtype=torch.bfloat16, experts=12, top_k=4, moe_inter=128,
+                          shared_inter=256, rope_theta=1000000.0, rms_eps=1e-6),
     'tiny-llama': dict(hidden=256, inter=512, layers=2, heads=4, kv_heads=2, vocab=512,
                        kind='llama', dtype=torch.bfloat16),
     'tiny-opt': dict(hidden=128, inter=512, layers=2, heads=4, kv_heads=4, vocab=512,
@@ -82,12 +90,14 @@ def _rot_half(x):
 
 
 class LlamaAttention(nn.Module):
-    def __init__(self, hidden, heads, kv_heads):
+    """qkv_bias (Qwen2): q / k / v carry a bias, added in the GEMM's bias epilogue (B200Linear)."""
+
+    def __init__(self, hidden, heads, kv_heads, qkv_bias=False):
         super().__init__()
         self.heads, self.kv_heads, self.head_dim = heads, kv_heads, hidden // heads
-        self.q_proj = B200Linear(hidden, heads * self.head_dim, bias=False)
-        self.k_proj = B200Linear(hidden, kv_heads * self.head_dim, bias=False)
-        self.v_proj = B200Linear(hidden, kv_heads * self.head_dim, bias=False)
+        self.q_proj = B200Linear(hidden, heads * self.head_dim, bias=qkv_bias)
+        self.k_proj = B200Linear(hidden, kv_heads * self.head_dim, bias=qkv_bias)
+        self.v_proj = B200Linear(hidden, kv_heads * self.head_dim, bias=qkv_bias)
         self.o_proj = B200Linear(heads * self.head_dim, hidden, bias=False)
 
     def fused_qkv_weight(self, dtype):
@@ -276,25 +286,39 @@ def _packed_triple_form(triple, hidden):
     return f + (inter,)
 
 
-class MixtralSparseMoe(nn.Module):
-    """Per-expert nn.Linear layout the reference's wrapper expects (models/mixtral.py:43-86:
-    block_sparse_moe.gate / experts[i].w1|w2|w3); the installed transformers 5.x fuses the experts,
-    so the shape model is restated here (SURVEY.md §7.3 item 8).  Hooks on an expert only ever see
-    the tokens routed to it (Appendix E-11)."""
+class SparseMoe(nn.Module):
+    """A sparse-MoE layer with per-expert nn.Linear experts, as the reference's wrappers expect them;
+    the installed transformers 5.x fuses the experts, so the shape models are restated here (SURVEY.md
+    §7.3 item 8).  A subclass names its expert class and the attribute names of an expert's (gate,
+    up, down) linears; the router, the per-expert loop and the grouped-path selectors are written
+    once here.  Hooks on an expert only ever see the tokens routed to it (Appendix E-11)."""
 
-    def __init__(self, hidden, inter, experts, top_k):
+    expert_cls = None
+    linear_names = None                       # an expert's (gate, up, down) linears
+    norm_topk_prob = True
+
+    def __init__(self, hidden, experts, top_k, make_expert):
         super().__init__()
         self.top_k = top_k
         self.gate = nn.Linear(hidden, experts, bias=False)
-        self.experts = nn.ModuleList([MixtralExpert(hidden, inter) for _ in range(experts)])
+        self.experts = nn.ModuleList([make_expert() for _ in range(experts)])
+
+    def expert_linears(self, ex):
+        """Expert ex's (gate, up, down) linears: Mixtral's (w1, w3, w2)."""
+        return tuple(getattr(ex, n) for n in self.linear_names)
+
+    def _plain(self, ex):
+        return type(ex) is self.expert_cls and not ex._forward_hooks and not ex._forward_pre_hooks
 
     def route(self, x):
-        """The router on x [T, H]: each token's top_k experts sel [T, k] and renormalised weights
-        w [T, k] of x's dtype."""
+        """The router on x [T, H]: each token's top_k experts sel [T, k] and weights w [T, k] of x's
+        dtype: softmax in fp32, top-k, renormalised when norm_topk_prob."""
         logits = self.gate(x)                      # module call: hooks / FakeQuantLinear see it
         w = F.softmax(logits, dim=1, dtype=torch.float)
         w, sel = torch.topk(w, self.top_k, dim=-1)
-        return sel, (w / w.sum(dim=-1, keepdim=True)).to(x.dtype)
+        if self.norm_topk_prob:
+            w = w / w.sum(dim=-1, keepdim=True)
+        return sel, w.to(x.dtype)
 
     def expert_loop(self, x, sel, w):
         """The experts one by one, each module called on exactly its routed tokens: the path for
@@ -309,19 +333,20 @@ class MixtralSparseMoe(nn.Module):
         return out
 
     def grouped_weights(self, x):
-        """One (w1, w3, w2) triple of dense forward weights per expert when module_utils.moe_forward
-        computes exactly what expert_loop computes on x, else None: every expert a plain
-        MixtralExpert without hooks whose linears have a dense forward weight of x's 16-bit dtype
-        (module_utils.dense_forward_weight: no hooks, activation fake-quant, bias or packing), shapes
-        the grouped GEMMs take (inter a multiple of 128, hidden of 8), at most MOE_MAX_EXPERTS."""
+        """One (gate, up, down) triple of dense forward weights per expert when
+        module_utils.moe_forward computes exactly what expert_loop computes on x, else None: every
+        expert a plain expert_cls without hooks whose linears have a dense forward weight of x's
+        16-bit dtype (module_utils.dense_forward_weight: no hooks, activation fake-quant, bias or
+        packing), shapes the grouped GEMMs take (inter a multiple of 128, hidden of 8), at most
+        MOE_MAX_EXPERTS."""
         if (not x.is_cuda or x.dtype not in (torch.bfloat16, torch.float16)
                 or len(self.experts) > MOE_MAX_EXPERTS or x.shape[1] % 8):
             return None
         weights, form = [], None
         for ex in self.experts:
-            if type(ex) is not MixtralExpert or ex._forward_hooks or ex._forward_pre_hooks:
+            if not self._plain(ex):
                 return None
-            ws = tuple(dense_forward_weight(m, x.dtype) for m in (ex.w1, ex.w3, ex.w2))
+            ws = tuple(dense_forward_weight(m, x.dtype) for m in self.expert_linears(ex))
             f = _dense_triple_form(ws, x.shape[1])
             if f is None or (form is not None and f != form):
                 return None
@@ -330,21 +355,21 @@ class MixtralSparseMoe(nn.Module):
         return weights
 
     def grouped_packed_operands(self, x):
-        """One (w1, w3, w2) triple of module_utils.PackedOperands per expert when moe_forward on them
-        computes exactly what expert_loop computes on x, else None: the checks of grouped_weights,
-        every expert linear packed_forward_operands' (4- / 8-bit integer codes, no hooks, activation
-        fake-quant or bias), all of one form (bits, qparam dtype and layout, zeros or not, g_idx or
-        not, groups per row), and the shapes the grouped dequant GEMMs take (hidden, inter and the
-        groups multiples of 64)."""
+        """One (gate, up, down) triple of module_utils.PackedOperands per expert when moe_forward on
+        them computes exactly what expert_loop computes on x, else None: the checks of
+        grouped_weights, every expert linear packed_forward_operands' (4- / 8-bit integer codes, no
+        hooks, activation fake-quant or bias), all of one form (bits, qparam dtype and layout, zeros
+        or not, g_idx or not, groups per row), and the shapes the grouped dequant GEMMs take (hidden,
+        inter and the groups multiples of 64)."""
         if (not x.is_cuda or x.dtype not in (torch.bfloat16, torch.float16)
                 or len(self.experts) > MOE_MAX_EXPERTS or x.shape[1] % 64):
             return None
         hidden = x.shape[1]
         ops, form = [], None
         for ex in self.experts:
-            if type(ex) is not MixtralExpert or ex._forward_hooks or ex._forward_pre_hooks:
+            if not self._plain(ex):
                 return None
-            triple = tuple(packed_forward_operands(m, x.dtype) for m in (ex.w1, ex.w3, ex.w2))
+            triple = tuple(packed_forward_operands(m, x.dtype) for m in self.expert_linears(ex))
             if any(o is None for o in triple):
                 return None
             f = _packed_triple_form(triple, hidden)
@@ -355,23 +380,24 @@ class MixtralSparseMoe(nn.Module):
         return ops
 
     def grouped_w8a8_operands(self, x):
-        """One (w1, w3, w2) triple of module_utils.W8A8Operands per expert when moe_forward on them
-        computes exactly what expert_loop computes on x, else None: every expert a plain MixtralExpert
-        without hooks, every linear w8a8_forward_operands' (a W8A8 export without bias or hooks), all
-        of one form (int8 or e4m3 codes, dynamic or static activations of one act config, per-channel
-        or per-tensor weight scales), the shapes the grouped W8A8 GEMMs take (hidden and inter
-        multiples of 16, inter of 64), at most MOE_MAX_EXPERTS.  Static activations also need
-        w1.input_scale == w3.input_scale in every expert: the gate/up launch quantises each row once,
-        where the loop quantises it for w1 and for w3 apart."""
+        """One (gate, up, down) triple of module_utils.W8A8Operands per expert when moe_forward on
+        them computes exactly what expert_loop computes on x, else None: every expert a plain
+        expert_cls without hooks, every linear w8a8_forward_operands' (a W8A8 export without bias or
+        hooks), all of one form (int8 or e4m3 codes, dynamic or static activations of one act config,
+        per-channel or per-tensor weight scales), the shapes the grouped W8A8 GEMMs take (hidden and
+        inter multiples of 16, inter of 64), at most MOE_MAX_EXPERTS.  Static activations also need
+        gate.input_scale == up.input_scale in every expert: the gate/up launch quantises each row
+        once, where the loop quantises it for gate and for up apart."""
         if (not x.is_cuda or x.dtype not in (torch.bfloat16, torch.float16)
                 or len(self.experts) > MOE_MAX_EXPERTS or x.shape[1] % 16):
             return None
         hidden = x.shape[1]
         ops, form = [], None
         for ex in self.experts:
-            if type(ex) is not MixtralExpert or ex._forward_hooks or ex._forward_pre_hooks:
+            if not self._plain(ex):
                 return None
-            triple = tuple(w8a8_forward_operands(m) for m in (ex.w1, ex.w3, ex.w2))
+            lin = self.expert_linears(ex)
+            triple = tuple(w8a8_forward_operands(m) for m in lin)
             if any(o is None for o in triple):
                 return None
             inter = triple[0].w.shape[0]
@@ -386,7 +412,7 @@ class MixtralSparseMoe(nn.Module):
             if f[0] != f[1] or f[0] != f[2] or (form is not None and f[0] != form):
                 return None
             form = f[0]
-            if triple[0].input_scale is not None and not _same_input_scale(ex.w1, ex.w3):
+            if triple[0].input_scale is not None and not _same_input_scale(lin[0], lin[1]):
                 return None
             ops.append(triple)
         return ops
@@ -394,7 +420,7 @@ class MixtralSparseMoe(nn.Module):
     def grouped_fake_quant_operands(self, x):
         """(experts, a_qdq) for module_utils.moe_forward when it computes exactly what expert_loop
         computes on x, else None: the fake-quant forms the other selectors leave to the loop.  Every
-        expert a plain MixtralExpert without hooks; every linear's forward a_qdq then one GEMM
+        expert a plain expert_cls without hooks; every linear's forward a_qdq then one GEMM
         (module_utils.fake_quant_forward_operands: FakeQuantLinear's dense tmp_weight, packed INT4 /
         INT8 or FP8-grid EffcientFakeQuantLinear, no bias or hooks), of one weight form with the
         shapes its grouped GEMMs take, at most MOE_MAX_EXPERTS; and either
@@ -402,8 +428,8 @@ class MixtralSparseMoe(nn.Module):
           selectors), or
           one a_qdq on all of them, the same bound method and arguments, whose class gives it a
           routed twin (`a_qdq.routed`, blockwise.a_qdq_routed) that accepts the layer: one pass
-          over the routed rows before gate/up for every expert's w1 and w3, one over act before the
-          down projection for every w2.
+          over the routed rows before gate/up for every expert's gate and up linears, one over act
+          before the down projection for every down linear.
         a_qdq is then None, or the pair of those passes."""
         if (not x.is_cuda or x.dtype not in (torch.bfloat16, torch.float16)
                 or len(self.experts) > MOE_MAX_EXPERTS or x.shape[1] % 8):
@@ -411,9 +437,9 @@ class MixtralSparseMoe(nn.Module):
         hidden = x.shape[1]
         ops, qdqs, form = [], [], None
         for ex in self.experts:
-            if type(ex) is not MixtralExpert or ex._forward_hooks or ex._forward_pre_hooks:
+            if not self._plain(ex):
                 return None
-            got = tuple(fake_quant_forward_operands(m, x.dtype) for m in (ex.w1, ex.w3, ex.w2))
+            got = tuple(fake_quant_forward_operands(m, x.dtype) for m in self.expert_linears(ex))
             if any(g is None for g in got):
                 return None
             triple = tuple(g[0] for g in got)
@@ -433,16 +459,16 @@ class MixtralSparseMoe(nn.Module):
         if routed is None or not all(isinstance(a, partial) and a.func == a0.func and a.args == a0.args
                                      and a.keywords == a0.keywords for a in qdqs):
             return None
-        qdq_in = routed([(ex.w1, ex.w3) for ex in self.experts])
-        qdq_act = routed([(ex.w2,) for ex in self.experts])
+        lins = [self.expert_linears(ex) for ex in self.experts]
+        qdq_in = routed([lin[:2] for lin in lins])
+        qdq_act = routed([lin[2:] for lin in lins])
         if qdq_in is None or qdq_act is None:
             return None
         return ops, (qdq_in, qdq_act)
 
-    def forward(self, hidden_states):
-        B, S, H = hidden_states.shape
-        x = hidden_states.reshape(-1, H)
-        sel, w = self.route(x)
+    def grouped_operands(self, x):
+        """(experts, a_qdq) of the first selector that accepts x, else (None, None): the grouped
+        path's operands, or the per-expert loop."""
         experts, a_qdq = self.grouped_weights(x), None
         if experts is None:
             experts = self.grouped_packed_operands(x)
@@ -450,12 +476,71 @@ class MixtralSparseMoe(nn.Module):
             experts = self.grouped_w8a8_operands(x)
         if experts is None:
             experts, a_qdq = self.grouped_fake_quant_operands(x) or (None, None)
+        return experts, a_qdq
+
+
+class MixtralSparseMoe(SparseMoe):
+    """Mixtral's block_sparse_moe: gate / experts[i].w1|w2|w3 (models/mixtral.py:43-86), top-k
+    weights renormalised."""
+
+    expert_cls = MixtralExpert
+    linear_names = ('w1', 'w3', 'w2')
+
+    def __init__(self, hidden, inter, experts, top_k):
+        super().__init__(hidden, experts, top_k, partial(MixtralExpert, hidden, inter))
+
+    def forward(self, hidden_states):
+        B, S, H = hidden_states.shape
+        x = hidden_states.reshape(-1, H)
+        sel, w = self.route(x)
+        experts, a_qdq = self.grouped_operands(x)
         if experts is None:
             out = self.expert_loop(x, sel, w)
         elif a_qdq is None:
             out = moe_forward(x, sel, w, experts)
         else:
             out = moe_forward(x, sel, w, experts, a_qdq)
+        return out.reshape(B, S, H)
+
+
+class Qwen2MoeSparseMoe(SparseMoe):
+    """Qwen2-MoE's mlp (models/qwen2moe.py:51-116): gate / experts[i].gate_proj|up_proj|down_proj,
+    a shared expert (shared_expert.gate_proj|up_proj|down_proj) and its gate shared_expert_gate
+    (Linear(hidden, 1)).  Top-k weights are not renormalised (norm_topk_prob False).  The block's
+    output is transformers' Qwen2MoeSparseMoeBlock.forward (modeling_qwen2_moe.py):
+      routed = index_add_ of each expert's rows * weight into zeros, expert by expert;
+      shared = F.sigmoid(shared_expert_gate(x)) * shared_expert(x);
+      out = routed + shared,
+    each op rounding to the activation dtype once (shared_loop restates it)."""
+
+    expert_cls = LlamaMLP
+    linear_names = ('gate_proj', 'up_proj', 'down_proj')
+    norm_topk_prob = False
+
+    def __init__(self, hidden, inter, shared_inter, experts, top_k):
+        super().__init__(hidden, experts, top_k, partial(LlamaMLP, hidden, inter))
+        self.shared_expert = LlamaMLP(hidden, shared_inter)
+        self.shared_expert_gate = B200Linear(hidden, 1, bias=False)
+
+    def shared(self, x):
+        """(shared_expert_gate(x) [T, 1], shared_expert(x) [T, H]) through the modules' own forwards:
+        the shared expert's gate/up on the fused SwiGLU GEMM when its weights allow."""
+        return self.shared_expert_gate(x), self.shared_expert(x)
+
+    def shared_loop(self, x, sel, w):
+        """The definition: expert_loop's routed sum plus F.sigmoid(gate logit) * shared expert."""
+        g, s = self.shared(x)
+        return self.expert_loop(x, sel, w) + F.sigmoid(g) * s
+
+    def forward(self, hidden_states):
+        B, S, H = hidden_states.shape
+        x = hidden_states.reshape(-1, H)
+        sel, w = self.route(x)
+        experts, a_qdq = self.grouped_operands(x)
+        if experts is None:
+            out = self.shared_loop(x, sel, w)
+        else:
+            out = moe_forward(x, sel, w, experts, a_qdq, self.shared(x))
         return out.reshape(B, S, H)
 
 
@@ -471,6 +556,23 @@ class MixtralBlock(nn.Module):
         h = hidden_states + self.self_attn(self.input_layernorm(hidden_states),
                                            position_embeddings=position_embeddings)
         return h + self.block_sparse_moe(self.post_attention_layernorm(h))
+
+
+class Qwen2MoeBlock(nn.Module):
+    """transformers' Qwen2MoeDecoderLayer with every layer sparse: attention with q/k/v bias, then
+    the sparse-MoE mlp with its shared expert."""
+
+    def __init__(self, hidden, heads, kv_heads, moe_inter, shared_inter, experts, top_k, eps):
+        super().__init__()
+        self.self_attn = LlamaAttention(hidden, heads, kv_heads, qkv_bias=True)
+        self.mlp = Qwen2MoeSparseMoe(hidden, moe_inter, shared_inter, experts, top_k)
+        self.input_layernorm = RMSNorm(hidden, eps)
+        self.post_attention_layernorm = RMSNorm(hidden, eps)
+
+    def forward(self, hidden_states, position_embeddings=None, **kw):
+        h = hidden_states + self.self_attn(self.input_layernorm(hidden_states),
+                                           position_embeddings=position_embeddings)
+        return h + self.mlp(self.post_attention_layernorm(h))
 
 
 class OPTAttention(nn.Module):
@@ -518,6 +620,10 @@ class _Decoder(nn.Module):
             blocks = [MixtralBlock(s['hidden'], s['inter'], s['heads'], s['kv_heads'], s['experts'],
                                    s['top_k']) for _ in range(n_layers)]
             self.norm = RMSNorm(s['hidden'])
+        elif s['kind'] == 'qwen2moe':
+            blocks = [Qwen2MoeBlock(s['hidden'], s['heads'], s['kv_heads'], s['moe_inter'], s['shared_inter'],
+                                    s['experts'], s['top_k'], s['rms_eps']) for _ in range(n_layers)]
+            self.norm = RMSNorm(s['hidden'], s['rms_eps'])
         else:
             blocks = [OPTBlock(s['hidden'], s['inter'], s['heads']) for _ in range(n_layers)]
             self.norm = nn.LayerNorm(s['hidden'])
@@ -604,7 +710,7 @@ class SynthModel:
         """The architecture part of the config.json `save_pretrained` would write for this shape."""
         s = self.shape
         arch = {'llama': ('LlamaForCausalLM', 'llama'), 'mixtral': ('MixtralForCausalLM', 'mixtral'),
-                'opt': ('OPTForCausalLM', 'opt')}[self.kind]
+                'qwen2moe': ('Qwen2MoeForCausalLM', 'qwen2_moe'), 'opt': ('OPTForCausalLM', 'opt')}[self.kind]
         doc = {'architectures': [arch[0]], 'model_type': arch[1], 'hidden_size': s['hidden'],
                'num_hidden_layers': len(self.model.layers), 'num_attention_heads': s['heads'],
                'vocab_size': s['vocab'], 'torch_dtype': str(self.torch_dtype).replace('torch.', '')}
@@ -614,6 +720,11 @@ class SynthModel:
             doc.update({'intermediate_size': s['inter'], 'num_key_value_heads': s['kv_heads']})
         if self.kind == 'mixtral':
             doc.update({'num_local_experts': s['experts'], 'num_experts_per_tok': s['top_k']})
+        if self.kind == 'qwen2moe':
+            doc.update({'num_experts': s['experts'], 'num_experts_per_tok': s['top_k'],
+                        'moe_intermediate_size': s['moe_inter'], 'shared_expert_intermediate_size': s['shared_inter'],
+                        'norm_topk_prob': False, 'qkv_bias': True, 'rms_norm_eps': s['rms_eps'],
+                        'rope_theta': s['rope_theta']})
         return doc
 
     # ---- structure (base_model.py:346-351, llama.py:52-91, opt.py:60-100) -----------------------
@@ -628,6 +739,8 @@ class SynthModel:
     def get_extra_modules(self, block):
         if self.kind == 'mixtral':                         # models/mixtral.py:38-41
             return {'block_sparse_moe': block.block_sparse_moe}
+        if self.kind == 'qwen2moe':                        # models/qwen2moe.py:28-31
+            return {'mlp': block.mlp}
         return {}
 
     def get_subsets_in_block(self, block):
@@ -650,6 +763,8 @@ class SynthModel:
                        prev_op=[moe.experts[i].w3], input=[f'block_sparse_moe.experts.{i}.w2'],
                        inspect=moe.experts[i].w2, has_kwargs=False, is_mlp=True) for i in range(ne)],
             ]
+        if self.kind == 'qwen2moe':
+            return self._qwen2moe_subsets(block)
         if self.kind == 'llama':
             a, m = block.self_attn, block.mlp
             return [
@@ -679,6 +794,37 @@ class SynthModel:
                  inspect=block.fc2, has_kwargs=False, is_mlp=True),
         ]
 
+    @staticmethod
+    def _qwen2moe_subsets(block):
+        """models/qwen2moe.py:51-116, its sparse branch (every layer here is sparse)."""
+        a, moe = block.self_attn, block.mlp
+        ne = len(moe.experts)
+        first = OrderedDict([(f'mlp.experts.{i}.gate_proj', moe.experts[i].gate_proj) for i in range(ne)])  # :81-82
+        first.update((f'mlp.experts.{i}.up_proj', moe.experts[i].up_proj) for i in range(ne))              # :83-84
+        first['mlp.shared_expert.gate_proj'] = moe.shared_expert.gate_proj                                 # :85
+        first['mlp.shared_expert.up_proj'] = moe.shared_expert.up_proj                                     # :86
+        first['mlp.gate'] = moe.gate                                                                       # :87
+        first['mlp.shared_expert_gate'] = moe.shared_expert_gate                                           # :88
+        return [
+            dict(layers=OrderedDict([('self_attn.q_proj', a.q_proj), ('self_attn.k_proj', a.k_proj),   # :53-65
+                                     ('self_attn.v_proj', a.v_proj)]),
+                 prev_op=[block.input_layernorm], input=['self_attn.q_proj'], inspect=a, has_kwargs=True),
+            dict(layers=OrderedDict([('self_attn.o_proj', a.o_proj)]), prev_op=[a.v_proj],            # :67-75
+                 input=['self_attn.o_proj'], inspect=a.o_proj, has_kwargs=False),
+            dict(layers=first, prev_op=[block.post_attention_layernorm], input=['mlp'], inspect=moe,  # :78-96
+                 has_kwargs=False, is_mlp=True),
+            *[dict(layers=OrderedDict([(f'mlp.experts.{i}.down_proj', moe.experts[i].down_proj)]),   # :97-107
+                   prev_op=[moe.experts[i].up_proj], input=[f'mlp.experts.{i}.down_proj'],
+                   inspect=moe.experts[i].down_proj, has_kwargs=False, is_mlp=True) for i in range(ne)],
+            dict(layers=OrderedDict([('mlp.shared_expert.down_proj', moe.shared_expert.down_proj)]),  # :108-116
+                 prev_op=[moe.shared_expert.up_proj], input=['mlp.shared_expert.down_proj'],
+                 inspect=moe.shared_expert.down_proj, has_kwargs=False),
+        ]
+
+    def _rope(self, seq_len, device):
+        hd = self.shape['hidden'] // self.shape['heads']
+        return rope_cos_sin(seq_len, hd, device, self.torch_dtype, theta=self.shape.get('rope_theta', 500000.0))
+
     # ---- first block input (base_model.py:264-321 Catcher), synthetic tokens ----------------------
     @torch.no_grad()
     def first_block_input(self, n_samples, seq_len, bs=1, seed=1, device='cuda', ids=None):
@@ -691,9 +837,8 @@ class SynthModel:
         data, kwargs = [], []
         step = n_samples if bs == -1 else bs
         kw = {}
-        if self.kind in ('llama', 'mixtral'):
-            hd = self.shape['hidden'] // self.shape['heads']
-            kw['position_embeddings'] = rope_cos_sin(seq_len, hd, device, self.torch_dtype)
+        if self.kind in ('llama', 'mixtral', 'qwen2moe'):
+            kw['position_embeddings'] = self._rope(seq_len, device)
         for i in range(0, n_samples, step):
             x = emb(ids[i:i + step].to(emb.weight.device)).to(device)
             if self.kind == 'opt':
@@ -752,9 +897,8 @@ class SynthModel:
         m = self.model
         x = m.embed_tokens(ids.to(m.embed_tokens.weight.device)).to(device)
         kw = {}
-        if self.kind in ('llama', 'mixtral'):
-            hd = self.shape['hidden'] // self.shape['heads']
-            kw['position_embeddings'] = rope_cos_sin(ids.shape[1], hd, device, self.torch_dtype)
+        if self.kind in ('llama', 'mixtral', 'qwen2moe'):
+            kw['position_embeddings'] = self._rope(ids.shape[1], device)
         for b in m.layers:
             x = b(x, **kw)
         x = m.norm(x)
