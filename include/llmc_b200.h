@@ -329,6 +329,27 @@ int llmc_gemm_swiglu(const void* x, const void* w_gate_up, void* act, int64_t M,
 int llmc_gemm_residual(const void* x, const void* w, const void* res, void* y, int64_t M,
                        int64_t N, int64_t K, int dtype, void* stream);
 
+/* K6 with the projections of DeepSeek-V2's multi-head latent attention (MLA, no q LoRA) in its
+ * epilogue: heads of 192 = nope 128 | pe 64 for q and k, 128 for v, a 64-wide rotary slice.  Both
+ * write into the buffers SDPA then reads as [B, S, H, D] views: q [M, H * 192], k [M, H * 192],
+ * v [M, H * 128].  Bit for bit llmc_gemm_bf16 followed by the torch glue of DeepseekV2Attention
+ * (split, apply_rotary_emb, broadcast of k_pe, cat).  Checks as llmc_gemm_bf16's, plus those listed.
+ *   llmc_gemm_mla_qkv   w_qkva = [W_q; W_kv_a] [H * 192 + kv_lora + 64, K]: q as q_proj lays it
+ *                       out with each head's pe slice rotated; latent [M, kv_lora] the first kv_lora
+ *                       columns of kv_a_proj_with_mqa; its last 64 columns (k_pe) rotated and written
+ *                       to the pe slot of every head of k.  The rotation (apply_rotary_emb) takes
+ *                       interleaved pairs (a, b) = rT(acc) and stores rT(a c - b s), rT(a s + b c) in
+ *                       fp32, one rounding per operation; cos / sin fp32 [seq, 32]; row r is position
+ *                       r % seq.  H a multiple of 4 (q a whole number of 256-wide n-tiles), kv_lora of
+ *                       64, M a multiple of seq.
+ *   llmc_gemm_mla_kv_b  w_kv_b [H * 256, K] (kv_b_proj): each head's first 128 columns to k's nope
+ *                       slot (columns h * 192 .. h * 192 + 127), its last 128 to v. */
+int llmc_gemm_mla_qkv(const void* x, const void* w_qkva, void* q, void* k, void* latent,
+                      const float* cosv, const float* sinv, int64_t M, int64_t heads, int64_t kv_lora,
+                      int64_t K, int64_t seq, int dtype, void* stream);
+int llmc_gemm_mla_kv_b(const void* x, const void* w_kv_b, void* k, void* v, int64_t M, int64_t heads,
+                       int64_t K, int dtype, void* stream);
+
 /* ------------------------------------------------------------------------------------
  * K6 grouped: a sparse-MoE layer's experts (Mixtral: w2(silu(w1 x) * w3 x) per expert) as one
  * launch per projection, bit for bit the eager per-expert loop (gather x[tok], llmc_gemm_bf16,
@@ -357,7 +378,14 @@ int llmc_gemm_residual(const void* x, const void* w, const void* res, void* y, i
  *                         token, dtype), s [T, N] the shared expert's output; the roundings of
  *                         Qwen2-MoE's block (index_add_ into zeros, F.sigmoid(gate(x)) * shared, the
  *                         add).  top_k > 0, N a multiple of 8, pointers 16-byte aligned; scalar checks,
- *                         then the T == 0 no-op, then pointer checks, all before any CUDA call. */
+ *                         then the T == 0 no-op, then pointer checks, all before any CUDA call.
+ *   llmc_moe_combine_weighted  out[t] = rT(acc + s[t]), acc = rT(...rT(rT(y[r0] w[r0]) + rT(y[r1]
+ *                         w[r1]))...) over r = rows[t, 0], ..., rows[t, top_k - 1]: w fp32 [rows] the
+ *                         routing weights in y's row order, s [T, N] the shared experts' output; the
+ *                         roundings of DeepSeek-V2's block (expert(x) * w in fp32 rounded once,
+ *                         index_add_ into zeros, + shared_experts(x)).  y holds the experts' unscaled
+ *                         outputs: llmc_moe_gemm_down with unit routing weights of the dtype, for which
+ *                         rT(rT(acc) * 1) = rT(acc).  Checks as llmc_moe_combine_shared's. */
 #define LLMC_MOE_MAX_EXPERTS 64
 int llmc_moe_gemm_swiglu(const void* xp, const void* const* w1, const void* const* w3,
                          const int32_t* offsets, void* act, int64_t rows, int64_t inter, int64_t K,
@@ -370,6 +398,8 @@ int llmc_moe_combine(const void* y, const int64_t* rows, void* out, int64_t T, i
 int llmc_moe_combine_shared(const void* y, const int64_t* rows, const void* gate_logit,
                             const void* shared, void* out, int64_t T, int64_t top_k, int64_t N,
                             int dtype, void* stream);
+int llmc_moe_combine_weighted(const void* y, const int64_t* rows, const float* w, const void* shared,
+                              void* out, int64_t T, int64_t top_k, int64_t N, int dtype, void* stream);
 
 /* The same two grouped projections on PACKED experts (the llmc_gemm_w4a16 / w8a16 dequant GEMM,
  * grouped): bit for bit the per-expert loop over llmc_gemm_w{4,8}a16[_gidx] with the same operands.

@@ -56,10 +56,10 @@ struct GemmParams {
 struct EpiParams {
   const void* res;          // kEpiResidual: the residual [M, N], may be GemmParams::out
   void* out_k;              // kEpiRopeQkv: k [M, n_k] and v [M, N - n_q - n_k]; q is GemmParams::out
-  void* out_v;
+  void* out_v;              // kEpiMlaQkv: k [M, n_q] and the latent [M, n_k]; kEpiMlaKvB: v [M, n_k]
   const void* cosv;         // kEpiRopeQkv: [seq, 128] rotary tables in the output dtype
-  const void* sinv;
-  int64_t n_q, n_k, seq;
+  const void* sinv;         // kEpiMlaQkv: [seq, 32] fp32
+  int64_t n_q, n_k, seq;    // kEpiMlaQkv: n_q = H * 192, n_k = kv_lora; kEpiMlaKvB: H * 192, H * 128
 };
 
 // What the GEMM does with a finished tile.  Every fused epilogue first rounds the accumulator to
@@ -70,6 +70,9 @@ enum Epilogue {
   kEpiRopeQkv,    // W = [Wq; Wk; Wv]: q, k, v to three outputs, rope_kernel applied to q and k
   kEpiSwiGLU,     // W = gate / up interleaved in 128-row blocks: act = silu(gate) * up
   kEpiResidual,   // Y = res + X W^T (add_kernel)
+  kEpiMlaQkv,     // W = [Wq; Wkv_a] of MLA: q with each head's pe slice rotated, the latent, and
+                  // the rotated k_pe into every head's pe slot of k (store_mla_tile)
+  kEpiMlaKvB,     // W = Wkv_b of MLA, one head per n-tile: k_nope into k's nope slots, v apart
 };
 
 // The grouped operands: one tensor map per expert weight (AWQ rewrites the expert weights between
@@ -250,6 +253,74 @@ __device__ __forceinline__ void store_residual_m64n128(const float (&acc)[64], i
   }
 }
 
+// One 64-column chunk of a half tile, fragments jb .. jb + 7 of acc, to out[row][col0 + d] (ld
+// even), rounded once as the plain GEMM's store rounds.  kRope: MLA's apply_rotary_emb on the chunk
+// (rope dim 64): interleaved pairs (2p, 2p + 1) are (a, b) = rT(acc), and the stored pair is
+// (a c - b s, a s + b c) in fp32, one rounding per operation as torch's complex64 product takes it,
+// with (c, s) = (cos, sin)[row % seq][p] of the fp32 [seq, 32] tables.  A pair is fragments
+// 4j + 2i and 4j + 2i + 1 of one thread.  n_out > 1 writes the same values at col0 + h * ld_h for
+// h < n_out (k_pe, which every head shares).
+template <int DT, bool kRope>
+__device__ __forceinline__ void store_mla_chunk(const float (&acc)[64], int jb, int64_t row0, int64_t col0,
+                                                int64_t M, const EpiParams& e, int64_t ld, void* out,
+                                                int64_t n_out, int64_t ld_h) {
+  using T = DType<DT>;
+  const int lane = threadIdx.x & 31;
+  const float* cosv = static_cast<const float*>(e.cosv);
+  const float* sinv = static_cast<const float*>(e.sinv);
+#pragma unroll
+  for (int i = 0; i < 2; ++i) {
+    const int64_t row = frag_row(row0, i);
+    if (row >= M) continue;
+    const int64_t tab = (row % e.seq) * 32 + (lane & 3);
+    uint32_t v[8];
+#pragma unroll
+    for (int j = 0; j < 8; ++j) {
+      const float a = acc[4 * (jb + j) + 2 * i], b = acc[4 * (jb + j) + 2 * i + 1];
+      if constexpr (kRope) {
+        const float ra = T::rT(a), rb = T::rT(b);
+        const float cs = __ldg(cosv + tab + 4 * j), sn = __ldg(sinv + tab + 4 * j);
+        v[j] = pack_pair<DT>(fadd_rn(fmul_rn(ra, cs), -fmul_rn(rb, sn)),
+                             fadd_rn(fmul_rn(ra, sn), fmul_rn(rb, cs)));
+      } else {
+        v[j] = pack_pair<DT>(a, b);
+      }
+    }
+    for (int64_t h = 0; h < n_out; ++h) {
+      uint16_t* o = static_cast<uint16_t*>(out) + row * ld + col0 + h * ld_h + 2 * (lane & 3);
+#pragma unroll
+      for (int j = 0; j < 8; ++j) *reinterpret_cast<uint32_t*>(o + 8 * j) = v[j];
+    }
+  }
+}
+
+// One 64-column chunk of kEpiMlaQkv starting at column gc of [q | latent | k_pe]: q's chunks are
+// nope, nope, pe per 192-wide head; the latent is n_k columns; k_pe goes to the pe slot (columns
+// 128 .. 191) of each of the n_q / 192 heads of k.  Chunks past N (the tile's tail) are skipped.
+template <int DT>
+__device__ __forceinline__ void store_mla_qkv_chunk(const float (&acc)[64], int jb, int64_t row0, int64_t gc,
+                                                    const GemmParams& p, const EpiParams& e) {
+  if (gc < e.n_q) {
+    if ((gc >> 6) % 3 == 2)
+      store_mla_chunk<DT, true>(acc, jb, row0, gc, p.M, e, e.n_q, p.out, 1, 0);
+    else
+      store_mla_chunk<DT, false>(acc, jb, row0, gc, p.M, e, e.n_q, p.out, 1, 0);
+  } else if (gc - e.n_q < e.n_k) {
+    store_mla_chunk<DT, false>(acc, jb, row0, gc - e.n_q, p.M, e, e.n_k, e.out_v, 1, 0);
+  } else if (gc - e.n_q == e.n_k) {
+    store_mla_chunk<DT, true>(acc, jb, row0, 128, p.M, e, e.n_q, e.out_k, e.n_q / 192, 192);
+  }
+}
+
+template <int DT>
+__device__ __forceinline__ void store_mla_tile(const float (&acc0)[64], const float (&acc1)[64], int64_t row0,
+                                               int64_t col0, const GemmParams& p, const EpiParams& e) {
+  store_mla_qkv_chunk<DT>(acc0, 0, row0, col0, p, e);
+  store_mla_qkv_chunk<DT>(acc0, 8, row0, col0 + 64, p, e);
+  store_mla_qkv_chunk<DT>(acc1, 0, row0, col0 + 128, p, e);
+  store_mla_qkv_chunk<DT>(acc1, 8, row0, col0 + 192, p, e);
+}
+
 // The kernel body.  Plain mode (wgmma_gemm_kernel, kMoe == kMoeOff): B is tmB, the epilogue kEpi.
 // Grouped mode (wgmma_moe_kernel): tiles come from decode_moe_unit and B from g's maps of the
 // tile's expert; for kMoeSwiGLU the 256-row B stage is two 128-row boxes, w1 rows then w3 rows of
@@ -384,6 +455,12 @@ __device__ __forceinline__ void gemm_body(const CUtensorMap* tmA, const CUtensor
         store_qkv_tile<DT>(acc0, acc1, row0, col0, p, e);
       } else if constexpr (kEpi == kEpiSwiGLU) {
         store_swiglu_m64n128<DT>(acc0, acc1, row0, col0 / 2, p.M, p.ld_out, p.out);
+      } else if constexpr (kEpi == kEpiMlaQkv) {
+        store_mla_tile<DT>(acc0, acc1, row0, col0, p, e);
+      } else if constexpr (kEpi == kEpiMlaKvB) {
+        // n-tile h is head h: its k_nope (128) and v (128) columns
+        store_linear_m64n128<DT>(acc0, row0, t.n_blk * 192, p.M, e.n_q, e.n_q, nullptr, p.out);
+        store_linear_m64n128<DT>(acc1, row0, t.n_blk * 128, p.M, e.n_k, e.n_k, nullptr, e.out_v);
       } else {
         store_residual_m64n128<DT>(acc0, row0, col0, p, e.res);
         store_residual_m64n128<DT>(acc1, row0, col0 + 128, p, e.res);
@@ -597,9 +674,13 @@ static int launch_moe(const MoeLaunch<kMoe>& m, void* stream) {
 
 // out[t] = rT(...rT(rT(0 + y[rows[t, 0]]) + y[rows[t, 1]]) + ...): the k expert outputs of token t
 // added in the order given (ascending expert), as `zeros` + one index_add_ per expert does.
-// kShared (Qwen2-MoE's gated shared expert): then out[t] = rT(out[t] + rT(rT(sigmoid(g[t])) * s[t])),
+// kCombineGated (Qwen2-MoE's gated shared expert): then out[t] = rT(out[t] + rT(rT(sigmoid(g[t])) * s[t])),
 // the roundings of F.sigmoid(gate(x)) * shared_expert(x) and the add that follows.
-template <int DT, bool kShared>
+// kCombineWeighted (DeepSeek-V2's fp32 routing weights and ungated shared experts): each term is
+// rT(y[r] * w[r]) with w fp32 [rows] in y's row order (g), then out[t] = rT(out[t] + s[t]).
+enum CombineMode { kCombinePlain, kCombineGated, kCombineWeighted };
+
+template <int DT, int kMode>
 __global__ void __launch_bounds__(256)
 moe_combine_kernel(const void* __restrict__ y, const int64_t* __restrict__ rows,
                    const void* __restrict__ g, const void* __restrict__ sh,
@@ -612,30 +693,42 @@ moe_combine_kernel(const void* __restrict__ y, const int64_t* __restrict__ rows,
     float acc[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
     for (int64_t s = 0; s < k; ++s) {
       float v[8];
-      load8<DT>(y, __ldg(rows + t * k + s) * N + ch * 8, v);
+      const int64_t r = __ldg(rows + t * k + s);
+      load8<DT>(y, r * N + ch * 8, v);
+      if constexpr (kMode == kCombineWeighted) {
+        const float w = __ldg(static_cast<const float*>(g) + r);
 #pragma unroll
-      for (int j = 0; j < 8; ++j) acc[j] = D::rT(fadd_rn(acc[j], v[j]));
+        for (int j = 0; j < 8; ++j) acc[j] = D::rT(fadd_rn(acc[j], D::rT(fmul_rn(v[j], w))));
+      } else {
+#pragma unroll
+        for (int j = 0; j < 8; ++j) acc[j] = D::rT(fadd_rn(acc[j], v[j]));
+      }
     }
-    if constexpr (kShared) {
+    if constexpr (kMode == kCombineGated) {
       const float sg = D::rT(sigmoid_f32(D::load(g, t)));
       float v[8];
       load8<DT>(sh, i << 3, v);
 #pragma unroll
       for (int j = 0; j < 8; ++j) acc[j] = D::rT(fadd_rn(acc[j], D::rT(fmul_rn(sg, v[j]))));
+    } else if constexpr (kMode == kCombineWeighted) {
+      float v[8];
+      load8<DT>(sh, i << 3, v);
+#pragma unroll
+      for (int j = 0; j < 8; ++j) acc[j] = D::rT(fadd_rn(acc[j], v[j]));
     }
     store8<DT>(out, i << 3, acc);
   }
 }
 
-// The launch behind llmc_moe_combine and llmc_moe_combine_shared (g, sh unused by the former), on
+// The launch behind the llmc_moe_combine* entry points (g, sh unused by llmc_moe_combine), on
 // arguments its caller has checked: T > 0, N a multiple of 8.
-template <bool kShared>
+template <int kMode>
 static int launch_moe_combine(const void* y, const int64_t* rows, const void* g, const void* sh, void* out,
                               int64_t T, int64_t top_k, int64_t N, int dtype, void* stream) {
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   int64_t blocks = (T * (N >> 3) + 255) / 256;
   if (blocks > kNumSMs * 32) blocks = kNumSMs * 32;
-#define CALL(DT) moe_combine_kernel<DT, kShared><<<(int)blocks, 256, 0, st>>>(y, rows, g, sh, out, T, top_k, N); \
+#define CALL(DT) moe_combine_kernel<DT, kMode><<<(int)blocks, 256, 0, st>>>(y, rows, g, sh, out, T, top_k, N); \
   LLMC_CHECK_LAUNCH()
   if (dtype == LLMC_BF16) { CALL(LLMC_BF16); } else { CALL(LLMC_F16); }
 #undef CALL
@@ -671,7 +764,7 @@ extern "C" int llmc_moe_combine(const void* y, const int64_t* rows, void* out, i
                    (long long)N);
     return LLMC_EALIGN;
   }
-  return launch_moe_combine<false>(y, rows, nullptr, nullptr, out, T, top_k, N, dtype, stream);
+  return launch_moe_combine<kCombinePlain>(y, rows, nullptr, nullptr, out, T, top_k, N, dtype, stream);
 }
 
 extern "C" int llmc_moe_combine_shared(const void* y, const int64_t* rows, const void* gate_logit,
@@ -690,7 +783,26 @@ extern "C" int llmc_moe_combine_shared(const void* y, const int64_t* rows, const
     set_last_error("moe_combine_shared: y, shared and out must be 16-byte aligned");
     return LLMC_EALIGN;
   }
-  return launch_moe_combine<true>(y, rows, gate_logit, shared, out, T, top_k, N, dtype, stream);
+  return launch_moe_combine<kCombineGated>(y, rows, gate_logit, shared, out, T, top_k, N, dtype, stream);
+}
+
+extern "C" int llmc_moe_combine_weighted(const void* y, const int64_t* rows, const float* w, const void* shared,
+                                         void* out, int64_t T, int64_t top_k, int64_t N, int dtype,
+                                         void* stream) {
+  LLMC_CHECK_ARG(T >= 0 && top_k > 0 && N > 0, "moe_combine_weighted: bad shape T=%lld top_k=%lld N=%lld",
+                 (long long)T, (long long)top_k, (long long)N);
+  LLMC_CHECK_ARG(dtype == LLMC_BF16 || dtype == LLMC_F16, "moe_combine_weighted: dtype must be bf16 or fp16");
+  if (N % 8 != 0) {
+    set_last_error("moe_combine_weighted: N=%lld must be a multiple of 8", (long long)N);
+    return LLMC_EALIGN;
+  }
+  if (T == 0) return LLMC_OK;
+  LLMC_CHECK_ARG(y && rows && w && shared && out, "moe_combine_weighted: null pointer");
+  if (!aligned16(y) || !aligned16(shared) || !aligned16(out)) {
+    set_last_error("moe_combine_weighted: y, shared and out must be 16-byte aligned");
+    return LLMC_EALIGN;
+  }
+  return launch_moe_combine<kCombineWeighted>(y, rows, w, shared, out, T, top_k, N, dtype, stream);
 }
 
 extern "C" int llmc_gemm_bf16(const void* x, const void* w, const void* bias, void* y, int64_t M,
@@ -744,6 +856,42 @@ extern "C" int llmc_gemm_residual(const void* x, const void* w, const void* res,
   EpiParams e{};
   e.res = res;
   return launch_gemm<kEpiResidual>(x, w, M, N, K, dtype, p, e, stream);
+}
+
+extern "C" int llmc_gemm_mla_qkv(const void* x, const void* w_qkva, void* q, void* k, void* latent,
+                                 const float* cosv, const float* sinv, int64_t M, int64_t heads,
+                                 int64_t kv_lora, int64_t K, int64_t seq, int dtype, void* stream) {
+  LLMC_CHECK_ARG(heads > 0 && heads % 4 == 0, "gemm_mla_qkv: heads=%lld must be a positive multiple of 4",
+                 (long long)heads);
+  LLMC_CHECK_ARG(kv_lora > 0 && kv_lora % 64 == 0, "gemm_mla_qkv: kv_lora=%lld must be a positive multiple of 64",
+                 (long long)kv_lora);
+  LLMC_CHECK_ARG(seq > 0 && M % seq == 0, "gemm_mla_qkv: need seq > 0 and M a multiple of seq");
+  LLMC_CHECK_ARG(k && latent && cosv && sinv, "gemm_mla_qkv: null pointer");
+  if (!aligned16(k) || !aligned16(latent) || !aligned16(cosv) || !aligned16(sinv)) {
+    set_last_error("gemm_mla_qkv: pointers must be 16-byte aligned");
+    return LLMC_EALIGN;
+  }
+  GemmParams p{};
+  p.out = q;
+  EpiParams e{};
+  e.out_k = k; e.out_v = latent; e.cosv = cosv; e.sinv = sinv;
+  e.n_q = heads * 192; e.n_k = kv_lora; e.seq = seq;
+  return launch_gemm<kEpiMlaQkv>(x, w_qkva, M, e.n_q + kv_lora + 64, K, dtype, p, e, stream);
+}
+
+extern "C" int llmc_gemm_mla_kv_b(const void* x, const void* w_kv_b, void* k, void* v, int64_t M,
+                                  int64_t heads, int64_t K, int dtype, void* stream) {
+  LLMC_CHECK_ARG(heads > 0, "gemm_mla_kv_b: heads=%lld must be positive", (long long)heads);
+  LLMC_CHECK_ARG(v != nullptr, "gemm_mla_kv_b: null pointer");
+  if (!aligned16(v)) {
+    set_last_error("gemm_mla_kv_b: pointers must be 16-byte aligned");
+    return LLMC_EALIGN;
+  }
+  GemmParams p{};
+  p.out = k;
+  EpiParams e{};
+  e.out_v = v; e.n_q = heads * 192; e.n_k = heads * 128;
+  return launch_gemm<kEpiMlaKvB>(x, w_kv_b, M, heads * 256, K, dtype, p, e, stream);
 }
 
 extern "C" int64_t llmc_syrk_workspace_bytes(int64_t T, int64_t C) {

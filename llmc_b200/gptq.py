@@ -143,6 +143,8 @@ class GPTQ(BaseBlockwiseQuantization):
                 for n in names:
                     leader[n] = src
         for name, layer in named_layers.items():
+            if not isinstance(layer, tuple(_LLMC_LINEAR_TYPES_ + _TRANSFORMERS_LINEAR_TYPES_)):
+                continue        # a non-linear subset member (DeepseekV2Gate): no Hessian (gptq.py:246-251)
             self.layers_cache[name] = {}
             lead = leader.get(name, name)
             if lead == name or lead not in self.layers_cache:

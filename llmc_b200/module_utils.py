@@ -73,6 +73,37 @@ def gemm_rope_qkv(x, w_qkv, n_q, n_k, cos, sin):
     return q, k, v
 
 
+def gemm_mla_qkv(x, w_qkva, heads, kv_lora, cos, sin):
+    """MLA's first projections, x [B, S, K] @ [W_q; W_kv_a]^T in one GEMM (llmc_gemm_mla_qkv): q
+    [B, S, heads * 192] with each head's pe slice rotated, k [B, S, heads * 192] with the rotated
+    k_pe in every head's pe slot (its nope slots are gemm_mla_kv_b's to fill) and the latent
+    [B, S, kv_lora].  cos / sin fp32 [S, 32]."""
+    B, S, K = x.shape
+    x2, w = _gemm_operands(x, w_qkva)
+    M, N = x2.shape[0], w.shape[0]
+    assert N == heads * 192 + kv_lora + 64 and cos.dtype == sin.dtype == torch.float32
+    q, k = (torch.empty((B, S, heads * 192), dtype=x.dtype, device=x.device) for _ in range(2))
+    latent = torch.empty((B, S, kv_lora), dtype=x.dtype, device=x.device)
+    with TIMER.span('gemm', flops=2.0 * M * N * K, nbytes=2.0 * (M * K + N * K + M * (N + (heads - 1) * 64))):
+        call('llmc_gemm_mla_qkv', ptr(x2), ptr(w), ptr(q), ptr(k), ptr(latent), ptr(cos.contiguous()),
+             ptr(sin.contiguous()), M, heads, kv_lora, K, S, dtype_enum(x.dtype), stream_ptr(x.device))
+    return q, k, latent
+
+
+def gemm_mla_kv_b(latent, w_kv_b, k, heads):
+    """MLA's kv_b_proj on the normed latent [B, S, kv_lora] (llmc_gemm_mla_kv_b): each head's k_nope
+    into the nope slots of gemm_mla_qkv's k, in place; returns v [B, S, heads * 128]."""
+    B, S, K = latent.shape
+    x2, w = _gemm_operands(latent, w_kv_b)
+    M, N = x2.shape[0], w.shape[0]
+    assert N == heads * 256 and k.shape == (B, S, heads * 192) and k.is_contiguous() and k.dtype == latent.dtype
+    v = torch.empty((B, S, heads * 128), dtype=latent.dtype, device=latent.device)
+    with TIMER.span('gemm', flops=2.0 * M * N * K, nbytes=2.0 * (M * K + N * K + M * N)):
+        call('llmc_gemm_mla_kv_b', ptr(x2), ptr(w), ptr(k), ptr(v), M, heads, K, dtype_enum(latent.dtype),
+             stream_ptr(latent.device))
+    return v
+
+
 def gemm_swiglu(x, w_gate_up, out=None):
     """block_ops.silu_mul(x @ Wg^T, x @ Wu^T) for w_gate_up = interleave_gate_up(Wg, Wu), into
     `out` (contiguous) when given."""
@@ -269,11 +300,15 @@ def moe_forward(x, sel, w, experts, a_qdq=None, shared=None):
     fake-quant of the experts' linears as a pair of routed twins (blockwise.a_qdq_routed), applied
     to the routed rows before gate/up and to act before the down projection.  shared: None, or
     (gate_logit [T, 1], s [T, H]) of a gated shared expert (Qwen2-MoE), added by the combine as
-    out[t] + sigmoid(gate_logit[t]) * s[t] (llmc_moe_combine_shared).  Bit for bit the eager loop
+    out[t] + sigmoid(gate_logit[t]) * s[t] (llmc_moe_combine_shared).  fp32 w (DeepSeek-V2): the down
+    GEMM runs with unit routing weights of x's dtype (rT(rT(acc) * 1) = rT(acc)), and shared, the
+    ungated shared experts' output s [T, H], is required: the combine takes each term as
+    rT(y * w) in fp32 and adds s (llmc_moe_combine_weighted).  Bit for bit the eager loop
     (SparseMoe.expert_loop, then the shared expert's add), with no host sync."""
     require_cuda(x, sel, w)
     T, k, E = x.shape[0], sel.shape[1], len(experts)
-    assert E <= MOE_MAX_EXPERTS and w.dtype == x.dtype
+    weighted = w.dtype == torch.float32
+    assert E <= MOE_MAX_EXPERTS and (w.dtype == x.dtype or (weighted and shared is not None))
     o1, o2 = experts[0][0], experts[0][2]
     gemms = (_moe_packed_gemms if isinstance(o1, PackedOperands)
              else _moe_fp8_gemms if isinstance(o1, Fp8Operands)
@@ -284,6 +319,9 @@ def moe_forward(x, sel, w, experts, a_qdq=None, shared=None):
     xp = x.index_select(0, perm // k)
     w_route = w.reshape(-1).index_select(0, perm)
     M = T * k
+    w_rows = None
+    if weighted:
+        w_rows, w_route = w_route, torch.ones(M, dtype=x.dtype, device=x.device)
     act = torch.empty((M, inter), dtype=x.dtype, device=x.device)
     y = torch.empty((M, N), dtype=x.dtype, device=x.device)
     out = torch.empty((T, N), dtype=x.dtype, device=x.device)
@@ -293,11 +331,30 @@ def moe_forward(x, sel, w, experts, a_qdq=None, shared=None):
         xp = a_qdq[0](xp, expert_of_row)
         qdq_act = partial(a_qdq[1], expert_of_row=expert_of_row)
     gemms(xp, experts, sel, perm, offsets, w_route, act, y, qdq_act)
-    if shared is None:
+    if weighted:
+        moe_combine_weighted(y, rows, w_rows, shared, out)
+    elif shared is None:
         with TIMER.span('moe_combine', nbytes=2.0 * (M * N + T * N) + 8.0 * M):
             call('llmc_moe_combine', ptr(y), ptr(rows), ptr(out), T, k, N, dtype_enum(x.dtype), stream_ptr(x.device))
     else:
         moe_combine_shared(y, rows, shared[0], shared[1], out)
+    return out
+
+
+def moe_combine_weighted(y, rows, w, s, out):
+    """out [T, N] = rT(acc + s[t]), acc = rT(...rT(rT(y[r0] * w[r0]) + rT(y[r1] * w[r1]))...) over
+    r = rows[t, :] in that order: a DeepSeek-V2 layer's routed experts, each scaled by its fp32
+    routing weight and rounded once, plus its ungated shared experts.  y [M, N], rows [T, k] int64,
+    w fp32 [M] in y's row order, s [T, N] of y's dtype."""
+    require_cuda(y, rows, w, s, out)
+    T, k = rows.shape
+    N = y.shape[1]
+    w, s = w.contiguous(), s.contiguous()
+    assert w.dtype == torch.float32 and w.numel() == y.shape[0] and s.shape == (T, N) and out.shape == (T, N)
+    assert s.dtype == out.dtype == y.dtype and out.is_contiguous()
+    with TIMER.span('moe_combine_weighted', nbytes=2.0 * (y.shape[0] * N + 2 * T * N) + 12.0 * T * k):
+        call('llmc_moe_combine_weighted', ptr(y), ptr(rows), ptr(w), ptr(s), ptr(out), T, k, N,
+             dtype_enum(y.dtype), stream_ptr(y.device))
     return out
 
 

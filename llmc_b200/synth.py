@@ -18,7 +18,8 @@ import torch.nn.functional as F
 
 from ._lib import MOE_MAX_EXPERTS
 from .module_utils import (_LLMC_LINEAR_TYPES_, _TRANSFORMERS_LINEAR_TYPES_, dense_forward_weight,
-                           gemm_rope_qkv, gemm_swiglu, interleave_gate_up, linear_forward,
+                           gemm_mla_kv_b, gemm_mla_qkv, gemm_rope_qkv, gemm_swiglu, interleave_gate_up,
+                           linear_forward,
                            Fp8Operands, fake_quant_forward_operands, moe_forward, packed_forward_operands,
                            w8a8_forward_operands)
 
@@ -44,6 +45,16 @@ SHAPES = {
     'tiny-qwen-moe': dict(hidden=256, inter=512, layers=2, heads=4, kv_heads=4, vocab=512,
                           kind='qwen2moe', dtype=torch.bfloat16, experts=12, top_k=4, moe_inter=128,
                           shared_inter=256, rope_theta=1000000.0, rms_eps=1e-6),
+    # DeepSeek-V2-Lite (the published config.json; its yarn rope scaling is not built: default rope):
+    # MLA without q LoRA, layer 0 dense (inter), the others 64 routed experts top-6 + 2 shared
+    'deepseek-v2-lite': dict(hidden=2048, inter=10944, layers=27, heads=16, kv_heads=16, vocab=102400,
+                             kind='deepseek_v2', dtype=torch.bfloat16, experts=64, top_k=6, moe_inter=1408,
+                             shared_experts=2, first_k_dense=1, kv_lora=512, rope_dim=64, nope_dim=128,
+                             v_dim=128, rope_theta=10000.0, routed_scale=1.0, rms_eps=1e-6),
+    'tiny-deepseek-v2': dict(hidden=256, inter=512, layers=2, heads=4, kv_heads=4, vocab=512,
+                             kind='deepseek_v2', dtype=torch.bfloat16, experts=12, top_k=6, moe_inter=128,
+                             shared_experts=2, first_k_dense=1, kv_lora=128, rope_dim=64, nope_dim=128,
+                             v_dim=128, rope_theta=10000.0, routed_scale=1.5, rms_eps=1e-6),
     'tiny-llama': dict(hidden=256, inter=512, layers=2, heads=4, kv_heads=2, vocab=512,
                        kind='llama', dtype=torch.bfloat16),
     'tiny-opt': dict(hidden=128, inter=512, layers=2, heads=4, kv_heads=4, vocab=512,
@@ -575,6 +586,193 @@ class Qwen2MoeBlock(nn.Module):
         return h + self.mlp(self.post_attention_layernorm(h))
 
 
+def mla_rope_cos_sin(seq_len, rope_dim, device, theta):
+    """DeepSeek-V2's default rotary tables as fp32 (cos, sin) [seq_len, rope_dim / 2]: the real and
+    imaginary parts of transformers' freqs_cis (torch.polar of position * inv_freq), computed on the
+    CPU so that every device sees the same bits."""
+    inv = 1.0 / (theta ** (torch.arange(0, rope_dim, 2, dtype=torch.int64).float() / rope_dim))
+    freqs = torch.outer(torch.arange(seq_len).float(), inv)
+    fc = torch.polar(torch.ones_like(freqs), freqs)
+    return fc.real.contiguous().to(device), fc.imag.contiguous().to(device)
+
+
+def mla_rotate(t, cos, sin):
+    """apply_rotary_emb of modeling_deepseek_v2 on t [..., S, (H,) 64] (the position axis is the one
+    cos [S, 32] lines up with): interleaved pairs (a, b) become (a c - b s, a s + b c) in fp32, one
+    rounding per operation as torch's complex64 product takes them, then t's dtype."""
+    a, b = t[..., 0::2].float(), t[..., 1::2].float()
+    if t.dim() == 4:                                     # [B, S, H, 64]: one table row per S
+        cos, sin = cos[:, None], sin[:, None]
+    return torch.stack((a * cos - b * sin, a * sin + b * cos), dim=-1).flatten(-2).to(t.dtype)
+
+
+class DeepseekV2Attention(nn.Module):
+    """transformers' DeepseekV2Attention without q LoRA (DeepSeek-V2-Lite): q_proj, then MLA's
+    compressed kv (kv_a_proj_with_mqa -> latent | k_pe, kv_a_layernorm, kv_b_proj -> k_nope | v),
+    rotary on q's and k's pe slices (mla_rotate), k_pe shared by every head, causal SDPA at scale
+    qk_head_dim ** -0.5, o_proj.  q, k and v are built in buffers [B, S, H * 192], [B, S, H * 192] and
+    [B, S, H * 128] that SDPA reads as [B, S, H, D] views.  No qkv_rope: MLA blocks take GPTQ's
+    generic hook schedule, not the Llama staged pass."""
+
+    def __init__(self, hidden, heads, kv_lora, rope_dim=64, nope_dim=128, v_dim=128, eps=1e-6,
+                 q_lora_rank=None):
+        super().__init__()
+        if q_lora_rank is not None:
+            raise NotImplementedError(
+                'DeepseekV2Attention: q_lora_rank models (q_a_proj / q_b_proj, DeepSeek-V2 236B) are not '
+                'built; only DeepSeek-V2-Lite\'s q_proj form is')
+        self.heads, self.kv_lora = heads, kv_lora
+        self.rope_dim, self.nope_dim, self.v_dim = rope_dim, nope_dim, v_dim
+        self.qk_dim = nope_dim + rope_dim
+        self.q_proj = B200Linear(hidden, heads * self.qk_dim, bias=False)
+        self.kv_a_proj_with_mqa = B200Linear(hidden, kv_lora + rope_dim, bias=False)
+        self.kv_a_layernorm = RMSNorm(kv_lora, eps)
+        self.kv_b_proj = B200Linear(kv_lora, heads * (nope_dim + v_dim), bias=False)
+        self.o_proj = B200Linear(heads * v_dim, hidden, bias=False)
+        self.scaling = self.qk_dim ** (-0.5)
+
+    def fused_weights(self, dtype):
+        """([W_q; W_kv_a], W_kv_b) for the two MLA GEMMs (llmc_gemm_mla_qkv / _kv_b), or None when
+        the projections cannot run that way: a projection without a dense forward weight of `dtype`
+        (module_utils.dense_forward_weight: no hooks, fake-quant activations, bias or packing), head
+        dims other than 128 / 64 / 128, heads not a multiple of 4 or kv_lora not of 64."""
+        if ((self.nope_dim, self.rope_dim, self.v_dim) != (128, 64, 128) or self.heads % 4
+                or self.kv_lora % 64):
+            return None
+        ws = [dense_forward_weight(m, dtype) for m in (self.q_proj, self.kv_a_proj_with_mqa, self.kv_b_proj)]
+        if any(w is None for w in ws) or ws[0].shape[1] != ws[1].shape[1]:
+            return None
+        return torch.cat(ws[:2]), ws[2]
+
+    def qkv(self, x, position_embeddings):
+        """The q, k, v buffers of x [B, S, hidden]: the two fused GEMMs when fused_weights allows,
+        else the module calls (hooks and fake-quant linears see their inputs) and the torch glue."""
+        B, S, _ = x.shape
+        cos, sin = position_embeddings
+        cos, sin = cos[:S], sin[:S]
+        w = self.fused_weights(x.dtype) if x.is_cuda else None
+        if w is not None and cos.dtype == torch.float32 and sin.dtype == torch.float32 and cos.is_cuda:
+            q, k, latent = gemm_mla_qkv(x, w[0], self.heads, self.kv_lora, cos, sin)
+            v = gemm_mla_kv_b(self.kv_a_layernorm(latent), w[1], k, self.heads)
+            return q, k, v
+        H, dn = self.heads, self.nope_dim
+        q = self.q_proj(x).contiguous()
+        qh = q.view(B, S, H, self.qk_dim)
+        qh[..., dn:] = mla_rotate(qh[..., dn:], cos, sin)
+        ckv = self.kv_a_proj_with_mqa(x)
+        latent = ckv[..., :self.kv_lora].contiguous()
+        kv = self.kv_b_proj(self.kv_a_layernorm(latent)).view(B, S, H, dn + self.v_dim)
+        k = torch.empty_like(q)
+        kh = k.view(B, S, H, self.qk_dim)
+        kh[..., :dn] = kv[..., :dn]
+        kh[..., dn:] = mla_rotate(ckv[..., self.kv_lora:], cos, sin)[:, :, None, :]
+        v = kv[..., dn:].reshape(B, S, H * self.v_dim)
+        return q, k, v
+
+    def sdpa(self, q, k, v):
+        """Causal attention of the q, k, v buffers; [B, S, H * v_dim]."""
+        B, S, _ = q.shape
+        H = self.heads
+        o = F.scaled_dot_product_attention(q.view(B, S, H, -1).transpose(1, 2), k.view(B, S, H, -1).transpose(1, 2),
+                                           v.view(B, S, H, -1).transpose(1, 2), is_causal=True, scale=self.scaling)
+        return o.transpose(1, 2).reshape(B, S, H * self.v_dim)
+
+    def forward(self, hidden_states, position_embeddings=None, **kw):
+        return self.o_proj(self.sdpa(*self.qkv(hidden_states, position_embeddings)))
+
+
+class DeepseekV2Gate(nn.Module):
+    """The remote-code MoEGate as the reference's DeepseekV2 wrapper meets it: its own module with a
+    weight [experts, hidden] and no nn.Linear base, so it is a member of the MoE subset (AWQ scales
+    it and searches over it) but not a block linear (no deploy replaces it, GPTQ skips it).  Called
+    as a module, so hooks see x; the logits are F.linear in fp32."""
+
+    def __init__(self, hidden, experts):
+        super().__init__()
+        self.in_features, self.out_features = hidden, experts
+        self.weight = nn.Parameter(torch.empty(experts, hidden))
+
+    def forward(self, x):
+        return F.linear(x.float(), self.weight.float())
+
+
+class DeepseekV2SparseMoe(SparseMoe):
+    """DeepSeek-V2's mlp (models/deepseekv2.py): gate (DeepseekV2Gate) / experts[i].gate_proj|up_proj|
+    down_proj and shared_experts (one SwiGLU MLP of n_shared * moe_inter).  The router is greedy
+    top-k of the fp32 softmax, not renormalised, times routed_scaling_factor, all in fp32; the
+    weights stay fp32.  The output is transformers' DeepseekV2Moe.forward (shared_loop restates it):
+      routed = zeros, then per expert in ascending order index_add_(tok, (expert(x[tok]) * w).to(dtype)),
+               the product bf16 x fp32 computed in fp32 and rounded once;
+      out = routed + shared_experts(x)."""
+
+    expert_cls = LlamaMLP
+    linear_names = ('gate_proj', 'up_proj', 'down_proj')
+
+    def __init__(self, hidden, inter, experts, top_k, n_shared, routed_scale, topk_method='greedy'):
+        if topk_method != 'greedy':
+            raise NotImplementedError(
+                f'DeepseekV2SparseMoe: topk_method {topk_method!r} (DeepSeek-V2 236B\'s group-limited '
+                'routing) is not built; only greedy top-k is')
+        super().__init__(hidden, experts, top_k, partial(LlamaMLP, hidden, inter))
+        self.gate = DeepseekV2Gate(hidden, experts)
+        self.shared_experts = LlamaMLP(hidden, inter * n_shared)
+        self.routed_scaling_factor = routed_scale
+
+    def route(self, x):
+        """sel [T, k] and fp32 weights w [T, k]: softmax of the fp32 logits, greedy top-k (unsorted),
+        times routed_scaling_factor."""
+        scores = self.gate(x).softmax(dim=-1, dtype=torch.float32)
+        w, sel = torch.topk(scores, self.top_k, dim=-1, sorted=False)
+        return sel, w * self.routed_scaling_factor
+
+    def expert_loop(self, x, sel, w):
+        """DeepseekV2Experts.forward on per-expert modules: one rounding of expert(x) * w (fp32)."""
+        out = torch.zeros_like(x)
+        for e, expert in enumerate(self.experts):
+            tok, slot = torch.where(sel == e)
+            if tok.numel() == 0:
+                continue
+            out.index_add_(0, tok, (expert(x[tok]) * w[tok, slot, None]).to(x.dtype))
+        return out
+
+    def shared_loop(self, x, sel, w):
+        """The definition: expert_loop's routed sum plus the shared experts."""
+        return self.expert_loop(x, sel, w) + self.shared_experts(x)
+
+    def forward(self, hidden_states):
+        B, S, H = hidden_states.shape
+        x = hidden_states.reshape(-1, H)
+        sel, w = self.route(x)
+        experts, a_qdq = self.grouped_operands(x)
+        if experts is None:
+            out = self.shared_loop(x, sel, w)
+        else:
+            out = moe_forward(x, sel, w, experts, a_qdq, self.shared_experts(x))
+        return out.reshape(B, S, H)
+
+
+class DeepseekV2Block(nn.Module):
+    """transformers' DeepseekV2DecoderLayer: MLA attention, then a dense SwiGLU MLP (layers before
+    first_k_dense_replace) or the sparse MoE with its shared experts."""
+
+    def __init__(self, s, layer_idx):
+        super().__init__()
+        self.self_attn = DeepseekV2Attention(s['hidden'], s['heads'], s['kv_lora'], s['rope_dim'], s['nope_dim'],
+                                             s['v_dim'], s['rms_eps'], s.get('q_lora_rank'))
+        if layer_idx >= s['first_k_dense']:
+            self.mlp = DeepseekV2SparseMoe(s['hidden'], s['moe_inter'], s['experts'], s['top_k'],
+                                           s['shared_experts'], s['routed_scale'], s.get('topk_method', 'greedy'))
+        else:
+            self.mlp = LlamaMLP(s['hidden'], s['inter'])
+        self.input_layernorm = RMSNorm(s['hidden'], s['rms_eps'])
+        self.post_attention_layernorm = RMSNorm(s['hidden'], s['rms_eps'])
+
+    def forward(self, hidden_states, position_embeddings=None, **kw):
+        h = hidden_states + self.self_attn(self.input_layernorm(hidden_states),
+                                           position_embeddings=position_embeddings)
+        return h + self.mlp(self.post_attention_layernorm(h))
+
+
 class OPTAttention(nn.Module):
     def __init__(self, hidden, heads):
         super().__init__()
@@ -623,6 +821,9 @@ class _Decoder(nn.Module):
         elif s['kind'] == 'qwen2moe':
             blocks = [Qwen2MoeBlock(s['hidden'], s['heads'], s['kv_heads'], s['moe_inter'], s['shared_inter'],
                                     s['experts'], s['top_k'], s['rms_eps']) for _ in range(n_layers)]
+            self.norm = RMSNorm(s['hidden'], s['rms_eps'])
+        elif s['kind'] == 'deepseek_v2':
+            blocks = [DeepseekV2Block(s, i) for i in range(n_layers)]
             self.norm = RMSNorm(s['hidden'], s['rms_eps'])
         else:
             blocks = [OPTBlock(s['hidden'], s['inter'], s['heads']) for _ in range(n_layers)]
@@ -710,7 +911,8 @@ class SynthModel:
         """The architecture part of the config.json `save_pretrained` would write for this shape."""
         s = self.shape
         arch = {'llama': ('LlamaForCausalLM', 'llama'), 'mixtral': ('MixtralForCausalLM', 'mixtral'),
-                'qwen2moe': ('Qwen2MoeForCausalLM', 'qwen2_moe'), 'opt': ('OPTForCausalLM', 'opt')}[self.kind]
+                'qwen2moe': ('Qwen2MoeForCausalLM', 'qwen2_moe'), 'opt': ('OPTForCausalLM', 'opt'),
+                'deepseek_v2': ('DeepseekV2ForCausalLM', 'deepseek_v2')}[self.kind]
         doc = {'architectures': [arch[0]], 'model_type': arch[1], 'hidden_size': s['hidden'],
                'num_hidden_layers': len(self.model.layers), 'num_attention_heads': s['heads'],
                'vocab_size': s['vocab'], 'torch_dtype': str(self.torch_dtype).replace('torch.', '')}
@@ -724,6 +926,14 @@ class SynthModel:
             doc.update({'num_experts': s['experts'], 'num_experts_per_tok': s['top_k'],
                         'moe_intermediate_size': s['moe_inter'], 'shared_expert_intermediate_size': s['shared_inter'],
                         'norm_topk_prob': False, 'qkv_bias': True, 'rms_norm_eps': s['rms_eps'],
+                        'rope_theta': s['rope_theta']})
+        if self.kind == 'deepseek_v2':
+            doc.update({'n_routed_experts': s['experts'], 'num_experts_per_tok': s['top_k'],
+                        'moe_intermediate_size': s['moe_inter'], 'n_shared_experts': s['shared_experts'],
+                        'first_k_dense_replace': s['first_k_dense'], 'kv_lora_rank': s['kv_lora'],
+                        'q_lora_rank': None, 'qk_rope_head_dim': s['rope_dim'], 'qk_nope_head_dim': s['nope_dim'],
+                        'v_head_dim': s['v_dim'], 'routed_scaling_factor': s['routed_scale'],
+                        'topk_method': 'greedy', 'norm_topk_prob': False, 'rms_norm_eps': s['rms_eps'],
                         'rope_theta': s['rope_theta']})
         return doc
 
@@ -739,7 +949,7 @@ class SynthModel:
     def get_extra_modules(self, block):
         if self.kind == 'mixtral':                         # models/mixtral.py:38-41
             return {'block_sparse_moe': block.block_sparse_moe}
-        if self.kind == 'qwen2moe':                        # models/qwen2moe.py:28-31
+        if self.kind in ('qwen2moe', 'deepseek_v2'):       # models/qwen2moe.py:28-31, deepseekv2.py:26-29
             return {'mlp': block.mlp}
         return {}
 
@@ -765,6 +975,8 @@ class SynthModel:
             ]
         if self.kind == 'qwen2moe':
             return self._qwen2moe_subsets(block)
+        if self.kind == 'deepseek_v2':
+            return self._deepseek_v2_subsets(block)
         if self.kind == 'llama':
             a, m = block.self_attn, block.mlp
             return [
@@ -821,7 +1033,50 @@ class SynthModel:
                  inspect=moe.shared_expert.down_proj, has_kwargs=False),
         ]
 
+    @staticmethod
+    def _deepseek_v2_subsets(block):
+        """models/deepseekv2.py:67-190: the q_proj branch (no q LoRA), then the MoE or the dense
+        branch by whether the mlp has a router."""
+        a, m = block.self_attn, block.mlp
+        subsets = [
+            dict(layers=OrderedDict([('self_attn.q_proj', a.q_proj),                                  # :69-81
+                                     ('self_attn.kv_a_proj_with_mqa', a.kv_a_proj_with_mqa)]),
+                 prev_op=[block.input_layernorm], input=['self_attn.q_proj'], inspect=a, has_kwargs=True),
+            dict(layers=OrderedDict([('self_attn.o_proj', a.o_proj)]), prev_op=[None],               # :106-114
+                 input=['self_attn.o_proj'], inspect=a.o_proj, has_kwargs=False),
+            dict(layers=OrderedDict([('self_attn.kv_b_proj', a.kv_b_proj)]), prev_op=[a.kv_a_layernorm],  # :115-124
+                 input=['self_attn.kv_b_proj'], inspect=a.kv_b_proj, has_kwargs=False, skip_rotate=True),
+        ]
+        if hasattr(m, 'gate'):
+            ne = len(m.experts)
+            first = OrderedDict([(f'mlp.experts.{i}.gate_proj', m.experts[i].gate_proj) for i in range(ne)])  # :130-131
+            first.update((f'mlp.experts.{i}.up_proj', m.experts[i].up_proj) for i in range(ne))              # :132-133
+            first['mlp.shared_experts.gate_proj'] = m.shared_experts.gate_proj                                # :134
+            first['mlp.shared_experts.up_proj'] = m.shared_experts.up_proj                                    # :135
+            first['mlp.gate'] = m.gate                                                                        # :136
+            subsets += [
+                dict(layers=first, prev_op=[block.post_attention_layernorm], input=['mlp'], inspect=m,   # :126-144
+                     has_kwargs=False, is_mlp=True),
+                *[dict(layers=OrderedDict([(f'mlp.experts.{i}.down_proj', m.experts[i].down_proj)]),      # :145-155
+                       prev_op=[m.experts[i].up_proj], input=[f'mlp.experts.{i}.down_proj'],
+                       inspect=m.experts[i].down_proj, has_kwargs=False, is_mlp=True) for i in range(ne)],
+                dict(layers=OrderedDict([('mlp.shared_experts.down_proj', m.shared_experts.down_proj)]),  # :157-165
+                     prev_op=[m.shared_experts.up_proj], input=['mlp.shared_experts.down_proj'],
+                     inspect=m.shared_experts.down_proj, has_kwargs=False),
+            ]
+        else:
+            subsets += [
+                dict(layers=OrderedDict([('mlp.gate_proj', m.gate_proj), ('mlp.up_proj', m.up_proj)]),   # :167-178
+                     prev_op=[block.post_attention_layernorm], input=['mlp.gate_proj'], inspect=m,
+                     has_kwargs=False),
+                dict(layers=OrderedDict([('mlp.down_proj', m.down_proj)]), prev_op=[m.up_proj],          # :180-188
+                     input=['mlp.down_proj'], inspect=m.down_proj, has_kwargs=False),
+            ]
+        return subsets
+
     def _rope(self, seq_len, device):
+        if self.kind == 'deepseek_v2':
+            return mla_rope_cos_sin(seq_len, self.shape['rope_dim'], device, self.shape['rope_theta'])
         hd = self.shape['hidden'] // self.shape['heads']
         return rope_cos_sin(seq_len, hd, device, self.torch_dtype, theta=self.shape.get('rope_theta', 500000.0))
 
@@ -837,7 +1092,7 @@ class SynthModel:
         data, kwargs = [], []
         step = n_samples if bs == -1 else bs
         kw = {}
-        if self.kind in ('llama', 'mixtral', 'qwen2moe'):
+        if self.kind in ('llama', 'mixtral', 'qwen2moe', 'deepseek_v2'):
             kw['position_embeddings'] = self._rope(seq_len, device)
         for i in range(0, n_samples, step):
             x = emb(ids[i:i + step].to(emb.weight.device)).to(device)
@@ -863,6 +1118,8 @@ class SynthModel:
         for name, m in list(subset['layers'].items()):
             if getattr(m, 'no_quant', False):
                 continue
+            if not isinstance(m, tuple(_LLMC_LINEAR_TYPES_ + _TRANSFORMERS_LINEAR_TYPES_)):
+                continue                                   # DeepseekV2Gate: a subset member, not a linear
             if isinstance(m, module_cls):
                 continue
             new = module_cls.new(m, **params_dict)
@@ -897,7 +1154,7 @@ class SynthModel:
         m = self.model
         x = m.embed_tokens(ids.to(m.embed_tokens.weight.device)).to(device)
         kw = {}
-        if self.kind in ('llama', 'mixtral', 'qwen2moe'):
+        if self.kind in ('llama', 'mixtral', 'qwen2moe', 'deepseek_v2'):
             kw['position_embeddings'] = self._rope(ids.shape[1], device)
         for b in m.layers:
             x = b(x, **kw)
